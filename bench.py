@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- Mchecks/sec of batched CheckPermission (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload cfg3] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--workload cfg3] [--impl reference] [--dump-outputs DIR]
 
 A "step" is one pass of the hot path (CheckBulkPermissions) over one batch of
 synthetic checks of the named workload (SURVEY.md 8d). Prints ONE JSON line.
@@ -20,6 +20,14 @@ synthetic checks of the named workload (SURVEY.md 8d). Prints ONE JSON line.
 Multi-GPU (--gpus N under torchrun): the store (<= 1.6 GB) is REPLICATED on every GPU
 and each rank answers its own batch: no data-path collective, "scaling": "weak".
 --impl reference: the oracle on all host threads, rank 0 only.
+--steps K: every timed loop runs exactly K steps (device-resident, e2e, the N > 1 sharded leg; --impl reference).
+The `sustained` leg is the exception by design: it runs the step back to back for --sustain-s seconds
+(0 = skip it) and reports how many steps that took.
+--dump-outputs DIR: after the timed steps, rank 0 writes the answers of the last timed step of every measured
+workload as DIR/answers_<workload>.npy (float32, one code per check: 1 = no permission, 2 = has permission,
+255 = error): the whole batch for cfg2/cfg3/cfg4, answers_cfg4_sharded.npy for the N > 1 sharded leg, and, with
+--impl reference, the oracle's answers on the sample it timed (the first n checks of the batch). The batches are
+seeded, so two builds can be compared answer for answer.
 """
 from __future__ import annotations
 
@@ -69,6 +77,9 @@ def parse_args():
     ap.add_argument("--sharded-timeout", type=float, default=300.0, help="hard limit of the sharded leg, seconds")
     ap.add_argument("--sustain-s", type=float, default=2.5,
                     help="length of the back-to-back 'sustained' leg of the primary workload (0 = skip)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the answers of the last timed step of each workload to DIR/answers_<workload>.npy "
+                         "(with --impl reference: the oracle's answers on its timed sample)")
     return ap.parse_args()
 
 
@@ -101,11 +112,11 @@ def measured_peak():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s)"
 
 
 def ncu_traffic(workload):
-    """dram bytes per launch of check_kernel from the committed ncu capture of the same build, if any:
+    """dram bytes per launch of check_kernel from an ncu capture of the same build, if one is committed:
     {"dram_bytes": ..., "kernel_ms": ..., "source": "profiles/..."} (older entries: a bare number)."""
     p = os.path.join(ROOT, "profiles", "ncu_traffic.json")
     if os.path.exists(p):
@@ -116,8 +127,8 @@ def ncu_traffic(workload):
 
 class ClockSampler:
     """Samples SM clock and throttle reasons DURING the timed region (NVML, every 5 ms, in a
-    thread). B200_PROFILING.md: a run that saw hw_slowdown / hw_thermal_slowdown /
-    sw_thermal_slowdown, or clocks stuck far below max with no reason, must be re-measured."""
+    thread). A run that saw hw_slowdown / hw_thermal_slowdown / sw_thermal_slowdown, or clocks
+    stuck far below max with no reason, must be re-measured."""
 
     def __init__(self, index):
         self.index = index
@@ -195,8 +206,11 @@ def cpu_reference_arm(args, rank, world):
         o.check_bulk(sample, nthreads=cores)
     t0 = time.perf_counter()
     for _ in range(args.steps):
-        o.check_bulk(sample, nthreads=cores)
+        got = o.check_bulk(sample, nthreads=cores)
     dt = time.perf_counter() - t0
+    if args.dump_outputs and args.steps > 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, f"answers_{w.name}.npy"), np.asarray(got).astype(np.float32))
     val = n * args.steps / dt / 1e6
     desc = f"first {n} checks of the {w.name} batch per step, {cores} threads"
     emit({
@@ -276,6 +290,9 @@ def measure_workload(name, args, rank, local_rank, world, dist, primary, sampler
     if dist:
         dist.barrier()
     dev_ms = sum(a.elapsed_time(b) for a, b in evs)
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, f"answers_{name}.npy"), d_out.cpu().numpy().astype(np.float32))
     launches = eng.stats()["launches"] - launches0
     t = torch.tensor([dev_ms], dtype=torch.float64, device="cuda")
     if dist:
@@ -320,7 +337,7 @@ def measure_workload(name, args, rank, local_rank, world, dist, primary, sampler
     pin_in.array[:] = items
     for _ in range(2):
         eng.check_bulk_ptr(pin_in.ptr, n, pin_out.ptr)
-    e2e_steps = max(3, min(steps, 50))
+    e2e_steps = steps
     if dist:
         dist.barrier()
     torch.cuda.synchronize()
@@ -437,7 +454,7 @@ def measure_sharded(args, rank, local_rank, world, dist):
     d_items = torch.from_numpy(mine.view(np.uint8).copy()).cuda()
     ck = zdist.DeviceShardedChecker(eng, zdist.TorchDeviceTransport())
     chunk = 1 << 18  # checks per rank per round: bounds the sub-queries a pass may raise (~20 per check, buffer 16 M)
-    steps = max(2, min(args.steps, 5))
+    steps = args.steps
 
     def one_step():
         outs = []
@@ -482,6 +499,9 @@ def measure_sharded(args, rank, local_rank, world, dist):
         want = rep.check_bulk(items)
         mism = int((full != want).sum())
         rep.close()
+        if args.dump_outputs:
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            np.save(os.path.join(args.dump_outputs, "answers_cfg4_sharded.npy"), full.astype(np.float32))
         rounds = steps * ((hi - lo + chunk - 1) // chunk)
         out = {"value": items.size * steps / dt / 1e6, "unit": UNIT, "ms_per_step": dt / steps * 1e3, "steps": steps,
                "mismatches_vs_replica": mism, "tuples_over_all_shards": int(n_tuples_owned.item()),
@@ -513,10 +533,11 @@ def run_sharded_leg(args, rank, world, dist):
     # under torchrun the workers use the AGENT's store; the children form their own group: rank 0's child hosts it
     env["TORCHELASTIC_USE_AGENT_STORE"] = "False"
     env["ZGPU_SHARDED_OUT"] = out_path
-    log_dir = os.path.join(ROOT, "gpurun_out")
-    os.makedirs(log_dir, exist_ok=True)
+    log_dir = tempfile.gettempdir()
     cmd = [sys.executable, os.path.abspath(__file__), "--sharded-child", "--gpus", str(world), "--steps", str(args.steps),
            "--warmup", str(args.warmup)]
+    if args.dump_outputs:
+        cmd += ["--dump-outputs", os.path.abspath(args.dump_outputs)]
     err = None
     log_path = os.path.join(log_dir, f"sharded_child_rank{rank}.log")
     try:

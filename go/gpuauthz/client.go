@@ -1,6 +1,6 @@
 // Package gpuauthz is the reference-side binding of libzgpu: an implementation of
 // v1.PermissionsServiceClient (authzed-go v1.6.0) that answers CheckPermission,
-// CheckBulkPermissions and LookupResources on a B200 through the C ABI in
+// CheckBulkPermissions and LookupResources on an H100 through the C ABI in
 // include/zgpu.h, and delegates everything else to the embedded SpiceDB it wraps.
 //
 // Injection point in the reference: pkg/proxy/options.go:371-377 only assigns

@@ -1,5 +1,5 @@
 /*
- * zgpu.h -- C ABI of libzgpu.so: a B200-native (sm_100a) batched Zanzibar
+ * zgpu.h -- C ABI of libzgpu.so: an H100-native (sm_90a) batched Zanzibar
  * permission-check engine that drops in behind the reference proxy's
  * v1.PermissionsServiceClient boundary (authzed/spicedb-kubeapi-proxy,
  * pkg/proxy/options.go:81-82,371-377).

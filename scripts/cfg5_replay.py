@@ -23,7 +23,7 @@ ap.add_argument("--clients", type=int, default=1000)
 ap.add_argument("--items", type=int, default=10000)
 ap.add_argument("--rounds", type=int, default=2)
 ap.add_argument("--devices", type=int, default=1)
-ap.add_argument("--cold", action="store_true", help="no untimed warm-up round (what the r2 artifacts in profiles/ measured)")
+ap.add_argument("--cold", action="store_true", help="no untimed warm-up round (first-use costs inside the timed phases)")
 a = ap.parse_args()
 
 w = workloads.cfg4(scale=a.scale)

@@ -1,4 +1,4 @@
-"""spicedb-kubeapi-proxy_b200 -- host side of libzgpu (B200-native batched Zanzibar
+"""spicedb-kubeapi-proxy_b200 -- host side of libzgpu (H100-native batched Zanzibar
 permission checks behind the reference proxy's v1.PermissionsServiceClient boundary).
 
 The directory name contains '-', so import it through the root-level shim:

@@ -95,10 +95,11 @@ def library_path() -> str:
 
 
 def build_library(force: bool = False) -> str:
-    """nvcc-compile csrc/ into libzgpu.so for sm_100a (cross-compiles without a GPU)."""
+    """nvcc-compile csrc/ into libzgpu.so for sm_90a (cross-compiles without a GPU)."""
     so = library_path()
     csrc = os.path.join(_HERE, "csrc")
-    srcs = [os.path.join(csrc, f) for f in os.listdir(csrc) if f.endswith((".cu", ".cc", ".h", ".cuh"))]
+    # the Makefile holds the architecture and compiler flags: a change there rebuilds too
+    srcs = [os.path.join(csrc, f) for f in os.listdir(csrc) if f.endswith((".cu", ".cc", ".h", ".cuh")) or f == "Makefile"]
     srcs.append(os.path.join(_ROOT, "include", "zgpu.h"))
     stale = not os.path.exists(so) or any(os.path.getmtime(s) > os.path.getmtime(so) for s in srcs)
     if os.environ.get("ZGPU_LIB"):

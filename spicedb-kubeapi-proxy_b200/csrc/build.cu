@@ -308,7 +308,8 @@ std::string gpu_build_snapshot(const Store& store, const Schema& sc, HostSnapsho
   s->delta_ok = true;
   if (nu >= (1u << 20)) {
     // The alternates of the incremental publish (merge_direction), with its headroom, come with the snapshot: the first
-    // write after a bulk load must not pay for three store-sized allocations (8 .. 560 ms, profiles/r2l_write_bench.json).
+    // write after a bulk load must not pay for three store-sized allocations (hundreds of ms where cudaMalloc is slow).
+    // That write still builds the host relationship index (Store::ensure_index), which a bulk load leaves stale.
     // Best effort: a failure here is met again, and reported, by the write that needs them.
     const size_t need = static_cast<size_t>(nu) * 4 + 64, roomy = need + need / 32 + (4u << 20);
     s->col_alt.ensure(roomy);
@@ -375,7 +376,7 @@ std::string merge_direction(const HostDelta& h, bool with_exp, DevBuf& row_ptr, 
                                                                                              edges.as<uint32_t>(), d, d_bad);
   if (ni || nd) {
     // headroom when the alternate has to grow (3 % + 4 MB): without it every write that adds edges re-allocates a
-    // store-sized buffer, and a cudaMalloc / cudaFree of 400 MB costs 100 ms on some boxes (profiles/r2k_write_bench.json)
+    // store-sized buffer, and a cudaMalloc / cudaFree of 400 MB can cost 100 ms
     const size_t need = std::max<uint64_t>(n_new, 1) * 4 + 64, roomy = need + need / 32 + (4u << 20);
     if (!edges_alt.ensure(edges_alt.cap < need ? roomy : need) || (with_exp && !exp_alt.ensure(exp_alt.cap < need ? roomy : need)))
       return "out of device memory (edge arrays)";

@@ -27,7 +27,7 @@ namespace zg {
 #define ZG_STR2(x) #x
 #define ZG_STR(x) ZG_STR2(x)
 const char* build_info() {
-  return "libzgpu sm_100a built " __DATE__ " " __TIME__ " L2_MODE=" ZG_STR(ZG_L2_MODE) " PRESENCE=" ZG_STR(ZG_PRESENCE) " POP_FAST=" ZG_STR(ZG_POP_FAST) " L2_MATCH=" ZG_STR(ZG_L2_MATCH) " L2_FILTER=" ZG_STR(ZG_L2_FILTER) " L2_SPLIT=" ZG_STR(ZG_L2_SPLIT)
+  return "libzgpu sm_90a built " __DATE__ " " __TIME__ " L2_MODE=" ZG_STR(ZG_L2_MODE) " PRESENCE=" ZG_STR(ZG_PRESENCE) " POP_FAST=" ZG_STR(ZG_POP_FAST) " L2_MATCH=" ZG_STR(ZG_L2_MATCH) " L2_FILTER=" ZG_STR(ZG_L2_FILTER) " L2_SPLIT=" ZG_STR(ZG_L2_SPLIT)
          " STACK_CAP=" ZG_STR(ZG_STACK_CAP) " RSET_CAP=" ZG_STR(ZG_RSET_CAP) " MIN_BLOCKS=" ZG_STR(ZG_MIN_BLOCKS);
 }
 

@@ -1,4 +1,4 @@
-// kernels.cuh -- sm_100a CUDA kernels of the permission-check hot path.
+// kernels.cuh -- sm_90a CUDA kernels of the permission-check hot path.
 //
 // What this replaces in the reference: the per-item graph evaluation that
 // CheckBulkPermissions / CheckPermission / LookupResources trigger inside the
@@ -6,7 +6,7 @@
 // watch.go:50, lookups.go:65; engine config pkg/spicedb/spicedb.go:25-56).
 //
 // Execution model (DESIGN.md "Kernels"):
-//   * persistent grid, 148 SMs x 4 CTAs x 8 warps; every WARP owns a private LIFO of edge
+//   * persistent grid, every SM (132 on an H100 SXM) x 4 CTAs x 8 warps; every WARP owns a private LIFO of edge
 //     RANGES in shared memory (spilling to a per-warp HBM area) and pulls batches of 32
 //     checks from a global counter;
 //   * admission loads each subject's reverse rows (its direct memberships) into a small
@@ -47,29 +47,31 @@ constexpr int kThreads = kWarpsPerBlock * 32;
 #ifndef ZG_RSET_CAP
 #define ZG_RSET_CAP 16
 #endif
+// The switches below were A/B-measured on the GPU this project targeted before the H100, not on the H100; only
+// ZG_MIN_BLOCKS was measured again there (4 beat 3 and 5 on cfg3 and cfg4, DESIGN.md §6).
 #ifndef ZG_PRESENCE
-#define ZG_PRESENCE 0  // presence word in front of the per-check set walk of a direct inverted probe (measured: -2 .. -3 %,
-                       // profiles/r2f: the walk is short and the extra shared-memory word costs more than it saves)
+#define ZG_PRESENCE 0  // presence word in front of the per-check set walk of a direct inverted probe (measured slower:
+                       // the walk is short and the extra shared-memory word costs more than it saves)
 #endif
 #ifndef ZG_POP_FAST
-#define ZG_POP_FAST 0  // pop: when every popped range holds <= 1 edge, skip the prefix scan / owner search (measured: no gain, r2g)
+#define ZG_POP_FAST 0  // pop: when every popped range holds <= 1 edge, skip the prefix scan / owner search (measured: no gain)
 #endif
 #ifndef ZG_L2_MATCH
 #define ZG_L2_MATCH 0  // cooperative two-level meet: match.any instead of a search for ranges of <= 16 children.
-                       // Measured 2x SLOWER (cfg3: 532 vs ~1 090 Mchecks/s, profiles/r2h): MATCH.ANY is a slow path on sm_100a
+                       // Measured much SLOWER on cfg3 (previous target GPU): MATCH.ANY was a slow path there
 #endif
 #ifndef ZG_L2_FILTER
 #define ZG_L2_FILTER 1  // cooperative two-level meet: a 2 048-bit blocked Bloom filter of the range's children in shared memory
                         // in front of the binary search (the search then runs only when the filter lets an element through).
-                        // Measured (profiles/r2j_ab_*): cfg3 1 056 -> 1 164 Mchecks/s, with ZG_L2_SPLIT 1 185; cfg4 unchanged
+                        // Measured faster on cfg3, more so together with ZG_L2_SPLIT; cfg4 unchanged
 #endif
 #ifndef ZG_L2_SPLIT
 #define ZG_L2_SPLIT 1  // cooperative two-level meet: 32 / ng lanes per membership row (any ng) instead of a power of two
-                       // (measured alone: cfg3 1 056 -> 1 079)
+                       // (measured alone: slightly faster on cfg3)
 #endif
 #ifndef ZG_L2_MODE
 #define ZG_L2_MODE 2  // two-level meet: 2 = warp-cooperative (default), 1 = per-lane Bloom word + 128-bit streaming
-                      // (measured slower: 919 vs 1 023 Mchecks/s on cfg3), 0 = per-lane sorted-segment intersection
+                      // (measured slower on cfg3), 0 = per-lane sorted-segment intersection
 #endif
 constexpr int kMinBlocks = ZG_MIN_BLOCKS;  // resident CTAs per SM the register budget is tuned for
 constexpr int kStackCap = ZG_STACK_CAP;    // range items per warp in shared memory
@@ -334,13 +336,13 @@ static_assert(kRsetCap <= 31, "class boundaries are 5-bit fields");
 
 // Two-level meet, warp-cooperative: ONE check's range against the reverse rows of its subject's memberships, all 32
 // lanes working on it. The per-lane form of this (every lane walking its own check's rows) ran with 9 of 32 lanes
-// active on average (profiles/r2d): row counts and early exits differ per check. Here the range's children F
+// active on average: row counts and early exits differ per check. Here the range's children F
 // (<= kFCap, ascending) go to shared memory with one coalesced load, every membership row gets a fixed group of lanes
 // (neighbouring lanes read neighbouring words of the row), and each lane tests its element against a Bloom filter of F;
 // F itself is binary-searched (warp-uniform trip count) only for what the filter lets through. Returns (warp-uniform) whether some element of some row is a child of the range.
 // Deliberately NOT inlined: inlined, its registers take part in the allocation of the whole traversal loop and cost
-// schemas that never use it 10 % (cfg4: 1 115 -> 944 Mchecks/s, profiles/r2e-r2g); a hash table of the range instead
-// of the binary search was slower still (864 vs 1 094 on cfg3, r2g).
+// schemas that never use it (measured on cfg4, previous target GPU); a hash table of the range instead of the binary search was slower
+// still (cfg3).
 // (all arguments by value: a reference to the warp context would force it into local memory)
 template <bool COUNT>
 __device__ __noinline__ bool coop_l2(const uint32_t* __restrict__ col, const uint32_t* __restrict__ rrow_ptr,
@@ -501,7 +503,7 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
     if (st.kind == ST_DIRECT && inverted && (st.flags & CF_INVERT)) {
       // direction-optimised probe: is obj among the subject's memberships of this class? Most probes miss: a
       // 32-bit presence word over (class, object) of the check's set (built at admission) rejects them
-      // without walking the set (the walk was 15 % of cfg4's instructions, profiles/r2d).
+      // without walking the set.
       const uint32_t present = c.rset[(kRsetCap + 5) * 32 + (jslot & 31)];
       if (!ZG_PRESENCE || ((present >> rset_bit(st.tinv, obj)) & 1u)) {
         const uint32_t kb = cst_at(cst, st.tinv), ke = cst_at(cst, st.tinv + 1u);

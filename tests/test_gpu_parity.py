@@ -843,7 +843,7 @@ def test_concurrent_lookups_share_launches_and_equal_the_oracle(zg, monkeypatch,
 
 def test_one_engine_owning_several_gpus_equals_a_single_gpu_engine(zg):
     """zg_config.n_devices: ONE handle, every device holds a replica and answers its slice of each bulk call
-    (the proxy keeps a single client: pkg/proxy/options.go:81-82). Needs >= 2 GPUs (gpurun --gpus 2)."""
+    (the proxy keeps a single client: pkg/proxy/options.go:81-82). Needs >= 2 GPUs."""
     import threading
 
     import torch

@@ -3,9 +3,9 @@
 
 What this is: a CPU-side check of the kernel's LOGIC -- admission, leaf loop with Kleene short circuit, meet in the
 middle (one and two levels), spills, path memo, sub-query passes and folds, batched LookupResources -- available without
-a GPU, so a kernel change is exercised before a gpurun call. What it is not: a product path (the emulator lives under
+a GPU, so a kernel change is exercised before it runs on a GPU. What it is not: a product path (the emulator lives under
 tests/, libzgpu.so has no CPU evaluation), a performance statement, or a substitute for the -m gpu parity tests, which
-run the same source on the B200 through the C ABI."""
+run the same source on the GPU through the C ABI."""
 import os
 import random
 import sys
