@@ -288,6 +288,94 @@ func (s *sliceStream) Context() context.Context     { return s.ctx }
 func (s *sliceStream) SendMsg(any) error            { return nil }
 func (s *sliceStream) RecvMsg(any) error            { return io.EOF }
 
+// LookupSubjects: "which subjects of a type have the permission on this resource" (who-can / audit). No proxy
+// call site issues it (it is in the client mock of pkg/authz/postfilter_test.go:71). A request with caveat
+// context, a concrete limit or a cursor goes to the wrapped SpiceDB: the library answers whole, uncaveated
+// lookups only. The concrete subjects come first, then -- when a wildcard grants the permission and the
+// request includes wildcards -- "*" with its excluded subjects. Like the rest of this file: never compiled.
+func (c *Client) LookupSubjects(ctx context.Context, req *v1.LookupSubjectsRequest, opts ...grpc.CallOption) (v1.PermissionsService_LookupSubjectsClient, error) {
+	if req.GetContext() != nil || req.GetOptionalConcreteLimit() != 0 || req.GetOptionalCursor() != nil {
+		return c.PermissionsServiceClient.LookupSubjects(ctx, req, opts...)
+	}
+	if c.broken.Load() {
+		return nil, errBroken
+	}
+	var s cstrs
+	defer s.free()
+	option := C.uint32_t(C.ZG_WILDCARDS_INCLUDE)
+	if req.GetWildcardOption() == v1.LookupSubjectsRequest_WILDCARD_OPTION_EXCLUDE_WILDCARDS {
+		option = C.ZG_WILDCARDS_EXCLUDE
+	}
+	capacity := C.size_t(1 << 16)
+	for {
+		buf := (*C.char)(C.malloc(capacity))
+		var need C.size_t
+		var n C.uint64_t
+		var rc C.int
+		err := call(func() C.int {
+			rc = C.zg_lookup_subjects_str(c.engine, s.add(req.GetResource().GetObjectType()),
+				s.add(req.GetResource().GetObjectId()), s.add(req.GetPermission()), s.add(req.GetSubjectObjectType()),
+				s.add(req.GetOptionalSubjectRelation()), option, buf, capacity, &need, &n)
+			if rc == C.ZG_E2BIG {
+				return 0
+			}
+			return rc
+		})
+		if rc == C.ZG_E2BIG {
+			C.free(unsafe.Pointer(buf))
+			capacity = need + 16
+			continue
+		}
+		if err != nil {
+			C.free(unsafe.Pointer(buf))
+			return nil, err
+		}
+		lines := strings.Split(strings.TrimSuffix(C.GoString(buf), "\n"), "\n")
+		C.free(unsafe.Pointer(buf))
+		if n == 0 {
+			lines = nil
+		}
+		var out []*v1.LookupSubjectsResponse
+		has := v1.LookupPermissionship_LOOKUP_PERMISSIONSHIP_HAS_PERMISSION
+		for i := 0; i < len(lines); i++ {
+			if lines[i] != "*" {
+				out = append(out, &v1.LookupSubjectsResponse{Subject: &v1.ResolvedSubject{SubjectObjectId: lines[i], Permissionship: has}})
+				continue
+			}
+			wild := &v1.LookupSubjectsResponse{Subject: &v1.ResolvedSubject{SubjectObjectId: "*", Permissionship: has}}
+			for _, x := range lines[i+1:] { // "!<id>": '!' is outside SpiceDB's object-id charset
+				wild.ExcludedSubjects = append(wild.ExcludedSubjects, &v1.ResolvedSubject{SubjectObjectId: strings.TrimPrefix(x, "!"), Permissionship: has})
+			}
+			out = append(out, wild)
+			break
+		}
+		return &subjectStream{ctx: ctx, items: out}, nil
+	}
+}
+
+type subjectStream struct {
+	ctx   context.Context
+	items []*v1.LookupSubjectsResponse
+	pos   int
+}
+
+func (s *subjectStream) Recv() (*v1.LookupSubjectsResponse, error) {
+	if err := s.ctx.Err(); err != nil {
+		return nil, status.FromContextError(err).Err()
+	}
+	if s.pos >= len(s.items) {
+		return nil, io.EOF
+	}
+	s.pos++
+	return s.items[s.pos-1], nil
+}
+func (s *subjectStream) Header() (metadata.MD, error) { return nil, nil }
+func (s *subjectStream) Trailer() metadata.MD         { return nil }
+func (s *subjectStream) CloseSend() error             { return nil }
+func (s *subjectStream) Context() context.Context     { return s.ctx }
+func (s *subjectStream) SendMsg(any) error            { return nil }
+func (s *subjectStream) RecvMsg(any) error            { return io.EOF }
+
 // WriteRelationships: SpiceDB stays the source of truth (preconditions, idempotency keys
 // with expiry: pkg/authz/distributedtx/activity.go:54-102); a successful write is mirrored
 // into the GPU store before returning so FullyConsistent checks observe it.

@@ -14,6 +14,7 @@
  *                                                      pkg/authz/postfilter.go:127-178
  *                               CheckPermission        pkg/authz/watch.go:50-67
  *   zg_lookup_resources*        LookupResources stream pkg/authz/lookups.go:49-88
+ *   zg_lookup_subjects*         LookupSubjects stream  (v1 API; pkg/authz/postfilter_test.go:71 mock)
  *   zg_write_relationships      WriteRelationships     pkg/authz/distributedtx/activity.go:54-76
  *   zg_delete_relationships     DeleteRelationships    (v1 API; filter semantics update.go:207-271)
  *   zg_read_relationships       ReadRelationships      pkg/authz/distributedtx/activity.go:128-171
@@ -41,7 +42,7 @@ extern "C" {
 #define ZG_ENOSNAPSHOT (-6) /* nothing published yet                             */
 #define ZG_E2BIG (-7)    /* output buffer too small; required size reported      */
 #define ZG_ENOMEM (-8)
-#define ZG_EDEPTH (-9)   /* LookupResources: a candidate hit the dispatch-depth cap / work budget */
+#define ZG_EDEPTH (-9)   /* LookupResources / LookupSubjects: a candidate hit the dispatch-depth cap / work budget */
 
 /* v1.CheckPermissionResponse.Permissionship (authzed-go v1.6.0); per-item codes */
 #define ZG_NO_PERMISSION 1
@@ -256,6 +257,31 @@ int zg_lookup_resources(zg_engine *e, uint16_t res_type, uint16_t perm, uint16_t
 int zg_lookup_resources_str(zg_engine *e, const char *res_type, const char *perm,
                             const char *subj_type, const char *subj_id, const char *subj_rel,
                             char *buf, size_t cap, size_t *need, uint64_t *n_out);
+
+/* LookupSubjects: which subjects of type stype[#srel] have `perm` on object `res` (of perm's type).
+ * Subjects granted through their own relationships are listed in ids (ascending). When a wildcard
+ * relationship (stype:*) grants perm and wildcard_option is ZG_WILDCARDS_INCLUDE, *wildcard = 1 and
+ * `excluded` lists (ascending) the subjects the wildcard does not cover (`user:* - banned`); every
+ * subject listed in neither has perm exactly when *wildcard is 1. With ZG_WILDCARDS_EXCLUDE the
+ * wildcard entry is left out. Candidates come from a forward walk of the resident snapshot from res
+ * (every object of stype when the walk overflows), verified by the check kernel. Returns 0; ZG_E2BIG
+ * with *n_out / *n_excluded = required sizes; ZG_EDEPTH when a subject cannot be decided (depth cap /
+ * work budget); ZG_EINVAL for unknown ids, or on a sharded engine; ZG_ECUDA on a host-only engine.
+ * A resource id that no relationship names gives an empty answer. No caveats, limits or cursors. */
+#define ZG_WILDCARDS_INCLUDE 0u /* v1.LookupSubjectsRequest WILDCARD_OPTION_UNSPECIFIED / INCLUDE_WILDCARDS */
+#define ZG_WILDCARDS_EXCLUDE 1u /* v1.LookupSubjectsRequest WILDCARD_OPTION_EXCLUDE_WILDCARDS               */
+int zg_lookup_subjects(zg_engine *e, uint16_t perm, uint32_t res, uint16_t stype, uint16_t srel,
+                       uint32_t wildcard_option, uint32_t *ids, uint64_t cap, uint64_t *n_out,
+                       uint32_t *excluded, uint64_t ex_cap, uint64_t *n_excluded, int32_t *wildcard);
+/* String form: '\n'-separated lines, one per concrete subject id; when the wildcard entry is present a
+ * "*" line follows, then one "!<id>" line per excluded subject. *n_out = lines, *need = bytes incl. NUL. */
+int zg_lookup_subjects_str(zg_engine *e, const char *res_type, const char *res_id, const char *perm,
+                           const char *subj_type, const char *subj_rel, uint32_t wildcard_option,
+                           char *buf, size_t cap, size_t *need, uint64_t *n_out);
+/* Cumulative LookupSubjects counters of the engine's device (zg_stats keeps its layout): out[0] lookups answered
+ * by the forward walk, out[1] lookups that verified every object of the subject type, out[2] check items of
+ * their first verification launches (the probe included). */
+int zg_lookup_subjects_counters(zg_engine *e, uint64_t *out);
 
 /* Pinned host memory for request/response buffers: zg_check_bulk copies straight
  * from/to such buffers (no staging memcpy). */

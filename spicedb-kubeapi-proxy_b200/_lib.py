@@ -16,6 +16,7 @@ NO_OBJECT = 0xFFFFFFFF
 OP_TOUCH, OP_CREATE, OP_DELETE = 0, 1, 2
 PRECOND_MUST_MATCH, PRECOND_MUST_NOT_MATCH = 1, 2
 E2BIG = -7
+WILDCARDS_INCLUDE, WILDCARDS_EXCLUDE = 0, 1  # zg_lookup_subjects wildcard_option
 
 CHECK_DTYPE = np.dtype(
     [("res", "<u4"), ("subj", "<u4"), ("perm", "<u2"), ("stype", "<u2"), ("srel", "<u2"), ("flags", "<u2")]
@@ -168,6 +169,12 @@ _SIGS = {
                                       C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),
     "zg_lookup_resources_str": (C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p,
                                           C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint64)]),
+    "zg_lookup_subjects": (C.c_int, [C.c_void_p, C.c_uint16, C.c_uint32, C.c_uint16, C.c_uint16, C.c_uint32, C.c_void_p,
+                                     C.c_uint64, C.POINTER(C.c_uint64), C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64),
+                                     C.POINTER(C.c_int32)]),
+    "zg_lookup_subjects_str": (C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint32,
+                                         C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint64)]),
+    "zg_lookup_subjects_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
     "zg_shard_pass": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.POINTER(C.c_uint64)]),
     "zg_shard_subqueries": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_uint64]),
     "zg_shard_fold": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_uint64, C.c_void_p]),
@@ -579,6 +586,45 @@ class Engine:
                 continue
             self._ck(rc)
             return [l for l in buf.value.decode().split("\n") if l]
+
+    def lookup_subjects_ids(self, res_type, res, perm, subj_type, srel=None, wildcards=WILDCARDS_INCLUDE, cap=1 << 14):
+        """LookupSubjects by ids -> (ids ascending, wildcard: bool, excluded ids ascending)."""
+        sr = SREL_NONE if srel is None else self.slot_id(subj_type, srel)
+        p = self.slot_id(res_type, perm)
+        ex_cap = cap
+        while True:  # ZG_E2BIG reports both required sizes
+            out, ex = np.empty(cap, dtype=np.uint32), np.empty(ex_cap, dtype=np.uint32)
+            n, nx, wild = C.c_uint64(0), C.c_uint64(0), C.c_int32(0)
+            rc = self._L.zg_lookup_subjects(self._h, p & 0xFFFF, int(res), self.type_id(subj_type) & 0xFFFF, sr & 0xFFFF,
+                                            int(wildcards), out.ctypes.data, cap, C.byref(n), ex.ctypes.data, ex_cap,
+                                            C.byref(nx), C.byref(wild))
+            if rc == E2BIG:
+                cap, ex_cap = max(cap, int(n.value)), max(ex_cap, int(nx.value))
+                continue
+            self._ck(rc)
+            return out[: n.value].copy(), bool(wild.value), ex[: nx.value].copy()
+
+    def lookup_subjects_str(self, res_type, res_id, perm, subj_type, subj_rel="", wildcards=WILDCARDS_INCLUDE, cap=1 << 16):
+        """LookupSubjects by names -> (subject ids, wildcard: bool, excluded subject ids) in internal-id order."""
+        while True:
+            buf = C.create_string_buffer(cap)
+            need, n = C.c_size_t(0), C.c_uint64(0)
+            rc = self._L.zg_lookup_subjects_str(self._h, _b(res_type), _b(res_id), _b(perm), _b(subj_type), _b(subj_rel or ""),
+                                                int(wildcards), buf, cap, C.byref(need), C.byref(n))
+            if rc == E2BIG:
+                cap = need.value + 16
+                continue
+            self._ck(rc)
+            lines = [l for l in buf.value.decode().split("\n") if l]
+            if "*" in lines:
+                at = lines.index("*")
+                return lines[:at], True, [l[1:] for l in lines[at + 1:]]
+            return lines, False, []
+
+    def lookup_subjects_counters(self) -> dict:
+        out = np.zeros(3, dtype=np.uint64)
+        self._ck(self._L.zg_lookup_subjects_counters(self._h, out.ctypes.data))
+        return {"walks": int(out[0]), "fallbacks": int(out[1]), "items_verified": int(out[2])}
 
     # -- sharded store (dist.ShardedStoreChecker drives these) --------------------
     def shard_pass(self, queries: np.ndarray, level: int) -> int:

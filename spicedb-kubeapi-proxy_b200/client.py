@@ -7,6 +7,7 @@ these methods on it:
     CheckBulkPermissions   pkg/authz/check.go:48, pkg/authz/postfilter.go:134
     CheckPermission        pkg/authz/watch.go:50
     LookupResources        pkg/authz/lookups.go:65  (server stream until io.EOF)
+    LookupSubjects         (v1 API; in the client mock of pkg/authz/postfilter_test.go:71, no call site)
     Watch                  pkg/authz/watch.go:29   (v1.WatchServiceClient, same connection)
     WriteRelationships     pkg/authz/distributedtx/activity.go:60
     ReadRelationships      pkg/authz/distributedtx/activity.go:107,154
@@ -33,6 +34,8 @@ PERMISSIONSHIP_HAS_PERMISSION = 2
 PERMISSIONSHIP_CONDITIONAL_PERMISSION = 3
 # v1.LookupPermissionship
 LOOKUP_PERMISSIONSHIP_HAS_PERMISSION = 1
+# v1.LookupSubjectsRequest_WildcardOption
+WILDCARD_OPTION_UNSPECIFIED, WILDCARD_OPTION_INCLUDE_WILDCARDS, WILDCARD_OPTION_EXCLUDE_WILDCARDS = 0, 1, 2
 # v1.RelationshipUpdate_Operation
 OPERATION_CREATE, OPERATION_TOUCH, OPERATION_DELETE = 1, 2, 3
 # v1.Precondition_Operation
@@ -133,6 +136,28 @@ class LookupResourcesRequest:
 class LookupResourcesResponse:
     resource_object_id: str
     permissionship: int = LOOKUP_PERMISSIONSHIP_HAS_PERMISSION
+
+
+@dataclass
+class LookupSubjectsRequest:
+    resource: ObjectReference
+    permission: str
+    subject_object_type: str
+    optional_subject_relation: str = ""
+    wildcard_option: int = WILDCARD_OPTION_UNSPECIFIED
+    fully_consistent: bool = True
+
+
+@dataclass
+class ResolvedSubject:
+    subject_object_id: str  # "*" for the wildcard
+    permissionship: int = LOOKUP_PERMISSIONSHIP_HAS_PERMISSION
+
+
+@dataclass
+class LookupSubjectsResponse:
+    subject: ResolvedSubject
+    excluded_subjects: List[ResolvedSubject] = field(default_factory=list)  # only on the wildcard
 
 
 @dataclass
@@ -266,6 +291,21 @@ class PermissionsClient:
         except ZgpuError as e:
             raise _rpc(e) from None
         return iter([LookupResourcesResponse(i) for i in ids])
+
+    def LookupSubjects(self, req: LookupSubjectsRequest) -> Iterator[LookupSubjectsResponse]:
+        """Slice-backed stand-in for the server stream: the concrete subjects, then (when a wildcard grants the
+        permission and the option includes wildcards) `*` with the subjects it excludes."""
+        opt = _lib.WILDCARDS_EXCLUDE if req.wildcard_option == WILDCARD_OPTION_EXCLUDE_WILDCARDS else _lib.WILDCARDS_INCLUDE
+        try:
+            ids, wild, excluded = self.engine.lookup_subjects_str(req.resource.object_type, req.resource.object_id,
+                                                                  req.permission, req.subject_object_type,
+                                                                  req.optional_subject_relation, opt)
+        except ZgpuError as e:
+            raise _rpc(e) from None
+        out = [LookupSubjectsResponse(ResolvedSubject(i)) for i in ids]
+        if wild:
+            out.append(LookupSubjectsResponse(ResolvedSubject("*"), [ResolvedSubject(x) for x in excluded]))
+        return iter(out)
 
     # -- relationships ------------------------------------------------------------
     def WriteRelationships(self, req: WriteRelationshipsRequest) -> WriteRelationshipsResponse:

@@ -1596,6 +1596,124 @@ extern "C" int zg_lookup_resources_str(zg_engine* e, const char* res_type, const
   return ZG_OK;
 }
 
+// ---- LookupSubjects --------------------------------------------------------------------------
+//
+// Arguments are checked before anything else (a host-only engine still reports ZG_EINVAL for them). The
+// device lock is FIFO, as for a single LookupResources; a multi-device engine answers on its first device.
+static int lookup_subjects_ids(zg_engine* e, uint16_t perm, uint32_t res, uint16_t stype, uint16_t srel, uint32_t option,
+                               Device::SubjectsAnswer* ans) {
+  const Schema& sc = e->schema;
+  if (perm >= sc.slots.size()) return fail(ZG_EINVAL, "unknown permission");
+  if (stype >= sc.types.size() || (srel != kNone && (srel >= sc.slots.size() || sc.slots[srel].type != stype)))
+    return fail(ZG_EINVAL, "unknown subject type or relation");
+  if (option != ZG_WILDCARDS_INCLUDE && option != ZG_WILDCARDS_EXCLUDE) return fail(ZG_EINVAL, "unknown wildcard option");
+  if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
+  if (e->dev.shard_count > 1) return fail(ZG_EINVAL, kShardedMsg);
+  LOCK_DEVICE(e);
+  if (e->dirty.load() || !e->dev.snap) {
+    LOCK_NAMES_UNIQUE(e);
+    int rc = publish_locked(e);
+    if (rc) return rc;
+  }
+  e->dev.now = now_of(e);
+  std::string err;
+  int rc = e->dev.lookup_subjects(sc.slots[perm].type, res, perm, stype, srel, option == ZG_WILDCARDS_INCLUDE, ans, &err);
+  return rc ? fail(rc, err) : ZG_OK;
+}
+
+extern "C" int zg_lookup_subjects(zg_engine* e, uint16_t perm, uint32_t res, uint16_t stype, uint16_t srel,
+                                  uint32_t wildcard_option, uint32_t* ids, uint64_t cap, uint64_t* n_out, uint32_t* excluded,
+                                  uint64_t ex_cap, uint64_t* n_excluded, int32_t* wildcard) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (!n_out || !n_excluded || !wildcard) return fail(ZG_EINVAL, "NULL n_out / n_excluded / wildcard");
+  Device::SubjectsAnswer ans;
+  int rc = lookup_subjects_ids(e, perm, res, stype, srel, wildcard_option, &ans);
+  if (rc) return rc;
+  *n_out = ans.ids.size();
+  *n_excluded = ans.excluded.size();
+  *wildcard = ans.wildcard ? 1 : 0;
+  if (ans.ids.size() > cap || ans.excluded.size() > ex_cap || (!ids && !ans.ids.empty()) ||
+      (!excluded && !ans.excluded.empty()))
+    return ZG_E2BIG;
+  if (!ans.ids.empty()) std::memcpy(ids, ans.ids.data(), ans.ids.size() * 4);
+  if (!ans.excluded.empty()) std::memcpy(excluded, ans.excluded.data(), ans.excluded.size() * 4);
+  return ZG_OK;
+}
+
+extern "C" int zg_lookup_subjects_str(zg_engine* e, const char* res_type, const char* res_id, const char* perm,
+                                      const char* subj_type, const char* subj_rel, uint32_t wildcard_option, char* buf,
+                                      size_t cap, size_t* need, uint64_t* n_out) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (!res_type || !res_id || !perm || !subj_type) return fail(ZG_EINVAL, "NULL argument");
+  int rt, p, st;
+  uint16_t sr = kNone;
+  uint32_t res;
+  {
+    LOCK_NAMES_SHARED(e);
+    const Schema& sc = e->schema;
+    rt = sc.type_id(res_type);
+    st = sc.type_id(subj_type);
+    if (rt < 0) return fail(ZG_EINVAL, std::string("object definition `") + res_type + "` not found");
+    if (st < 0) return fail(ZG_EINVAL, std::string("object definition `") + subj_type + "` not found");
+    p = sc.slot_id(rt, perm);
+    if (p < 0) return fail(ZG_EINVAL, std::string("relation/permission `") + perm + "` not found under definition `" + res_type + "`");
+    if (!none_rel(subj_rel)) {
+      int s = sc.slot_id(st, subj_rel);
+      if (s < 0) return fail(ZG_EINVAL, std::string("relation `") + subj_rel + "` not found under definition `" + subj_type + "`");
+      sr = static_cast<uint16_t>(s);
+    }
+    res = e->store.find(rt, res_id);
+  }
+  Device::SubjectsAnswer ans;
+  int rc = ZG_OK;
+  if (res == ZG_NO_OBJECT) {
+    // never written: no relationship names the resource. The engine state is still checked as for any lookup.
+    if (wildcard_option != ZG_WILDCARDS_INCLUDE && wildcard_option != ZG_WILDCARDS_EXCLUDE)
+      return fail(ZG_EINVAL, "unknown wildcard option");
+    if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
+    if (e->dev.shard_count > 1) return fail(ZG_EINVAL, kShardedMsg);
+  } else {
+    rc = lookup_subjects_ids(e, static_cast<uint16_t>(p), res, static_cast<uint16_t>(st), sr, wildcard_option, &ans);
+    if (rc) return rc;
+  }
+  // lines: concrete ids, then "*" and one "!<id>" per exclusion ('!' is outside SpiceDB's object-id charset)
+  std::vector<std::string> lines;
+  {
+    LOCK_NAMES_SHARED(e);
+    auto name = [&](uint32_t id) {
+      std::string_view n;
+      return e->store.name(st, id, &n) ? std::string(n) : std::to_string(id);
+    };
+    for (uint32_t id : ans.ids) lines.push_back(name(id));
+    if (ans.wildcard) {
+      lines.push_back("*");
+      for (uint32_t id : ans.excluded) lines.push_back("!" + name(id));
+    }
+  }
+  size_t total = 1;
+  for (const auto& l : lines) total += l.size() + 1;
+  if (need) *need = total;
+  if (n_out) *n_out = lines.size();
+  if (total > cap || !buf) return ZG_E2BIG;
+  size_t w = 0;
+  for (const auto& l : lines) {
+    std::memcpy(buf + w, l.data(), l.size());
+    w += l.size();
+    buf[w++] = '\n';
+  }
+  buf[w] = 0;
+  return ZG_OK;
+}
+
+extern "C" int zg_lookup_subjects_counters(zg_engine* e, uint64_t* out) {
+  if (!e || !out) return fail(ZG_EINVAL, "NULL argument");
+  LOCK_DEVICE(e);
+  out[0] = e->dev.subject_lookups_walk;
+  out[1] = e->dev.subject_lookups_exhaustive;
+  out[2] = e->dev.subject_items_verified;
+  return ZG_OK;
+}
+
 // ---- pre-filter: LookupResources ids -> kept list items --------------------------------------
 
 extern "C" int zg_list_keep_allowed(zg_engine* e, const char* body, size_t len, const zg_list_item* items, uint64_t n,

@@ -3,6 +3,7 @@
 // Call graph it replaces in the reference:
 //   CheckBulkPermissions (pkg/authz/check.go:48, postfilter.go:134) -> check_*()
 //   LookupResources      (pkg/authz/lookups.go:65)                    -> lookup()
+//   LookupSubjects       (v1 API, no proxy call site)                 -> lookup_subjects()
 #include "device.h"
 
 #include <algorithm>
@@ -62,6 +63,9 @@ Snapshot::~Snapshot() {
   type_bit_base.release();
   for (auto& r : resources) r.release();
   for (auto& f : flat_cls) f.release();
+  ls_fwd.release();
+  ls_type_off.release();
+  ls_mask.release();
 }
 
 Device::~Device() {
@@ -84,6 +88,7 @@ Device::~Device() {
   rb_front_[1].release();
   rb_cand_.release();
   for (auto* b : {&lb_params_, &lb_owner_, &lb_ctrl_, &lb_keys_[0], &lb_keys_[1]}) b->release();
+  for (auto* b : {&ls_jobs_, &ls_codes_, &ls_has_, &ls_ids_, &ls_ctrl_}) b->release();
   if (pin_in_) cudaFreeHost(pin_in_);
   if (pin_out_) cudaFreeHost(pin_out_);
   if (pin_ready_) cudaFreeHost(pin_ready_);
@@ -291,6 +296,14 @@ std::string Device::finish_publish(std::shared_ptr<Snapshot> s, const HostSnapsh
     s->n_objects = h.n_objects;
     if (ok) ok = up(s->type_bit_base, base.data(), base.size() * 8);
   }
+  {
+    std::vector<FwdClass> fwd;
+    std::vector<uint32_t> type_off;
+    sc.forward_tables(h.rels, &fwd, &type_off);
+    s->ls_mask_words = sc.fwd_mask_words;
+    if (ok) ok = up(s->ls_fwd, fwd.data(), fwd.size() * sizeof(FwdClass)) && up(s->ls_type_off, type_off.data(), type_off.size() * 4) &&
+                 up(s->ls_mask, sc.fwd_mask.data(), sc.fwd_mask.size() * 4);
+  }
   if (!ok || cudaStreamSynchronize(stream) != cudaSuccess)
     return std::string("snapshot upload failed: ") + cudaGetErrorString(cudaGetLastError());
   // flat-union slots: LookupResources is the union of the subject's reverse rows
@@ -398,6 +411,7 @@ int Device::run_pass(const Snapshot& s, const zg_check* queries, uint64_t nq, ui
   p.memo_after = memo_after_;
   p.shard_count = shard_count;
   p.shard_rank = shard_rank;
+  p.no_wildcards = no_wildcards_ ? 1 : 0;
   ZG_CUDA(cudaMemsetAsync(ctrl, 0, 16, st));  // next, subq_count
   const int per_sm = count ? blocks_per_sm_count_ : blocks_per_sm_;
   uint64_t want = (nq + kThreads - 1) / kThreads;
@@ -1296,6 +1310,181 @@ int Device::lookup_batch(const std::vector<LookupReq>& reqs, std::vector<std::ve
       (*ids)[i].clear();
     }
   return ZG_OK;
+}
+
+int Device::lookup_subjects(uint16_t res_type, uint32_t res, uint16_t perm, uint16_t stype, uint16_t srel,
+                            bool include_wildcard, SubjectsAnswer* ans, std::string* err) {
+  *ans = SubjectsAnswer{};
+  std::shared_ptr<Snapshot> s = snap;
+  if (!s) {
+    if (err) *err = "no snapshot published";
+    return ZG_ENOSNAPSHOT;
+  }
+  if (res_type >= s->n_objects.size() || stype >= s->n_objects.size()) {
+    if (err) *err = "unknown resource or subject type";
+    return ZG_EINVAL;
+  }
+  if (res >= s->n_objects[res_type]) return ZG_OK;  // never written: no relationship names it
+  ZG_CUDA(cudaSetDevice(device));
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  zg_check proto{};
+  proto.res = res;
+  proto.perm = perm;
+  proto.stype = stype;
+  proto.srel = srel;
+  const size_t n_ctrl = 8 + ZG_MAX_DEPTH + 4;  // [0] flags, [1] candidates, [2] HAS, [3] NO, [4] concrete, [5] scratch | level counts
+  if (!ls_ctrl_.ensure(n_ctrl * 8)) {
+    if (err) *err = "out of device memory (lookup)";
+    return ZG_ENOMEM;
+  }
+  unsigned long long* ctrl = ls_ctrl_.as<unsigned long long>();
+  unsigned long long* counts = ctrl + 8;
+  uint32_t* lflags = reinterpret_cast<uint32_t*>(ctrl);
+  ZG_CUDA(cudaMemsetAsync(ctrl, 0, n_ctrl * 8, stream));
+  uint64_t n = 0;  // items of the first verification, the probe included
+  bool walked = false;
+  const uint64_t cap = rb_cap_;
+  const unsigned long long words = (s->total_bits + 31) / 32 + 4;
+  if (use_rbfs && rb_visited_.ensure(words * 4) && rb_front_[0].ensure(cap * 8) && rb_front_[1].ensure(cap * 8) &&
+      ls_jobs_.ensure((cap + 2) * sizeof(zg_check))) {
+    ZG_CUDA(cudaMemsetAsync(rb_visited_.p, 0, words * 4, stream));
+    FwalkParams p{};
+    p.row_ptr = s->row_ptr.as<uint32_t>();
+    p.col = s->col.as<uint32_t>();
+    p.fwd = s->ls_fwd.as<FwdClass>();
+    p.type_off = s->ls_type_off.as<uint32_t>();
+    p.mask = s->ls_mask.as<uint32_t>() + static_cast<size_t>(perm) * s->ls_mask_words;
+    p.counts = counts;
+    p.cap = cap;
+    p.visited = rb_visited_.as<uint32_t>();
+    p.type_bit_base = s->type_bit_base.as<unsigned long long>();
+    p.proto = proto;
+    p.cand = ls_jobs_.as<zg_check>();
+    p.cand_count = ctrl + 1;
+    p.cand_cap = cap + 2;
+    p.flags = lflags;
+    p.in = rb_front_[0].as<unsigned long long>();
+    fwalk_seed_kernel<<<1, 32, 0, stream>>>(p, res_type);
+    ++launches;
+    constexpr int kLevelsPerRound = 10;
+    int level = 0, cur = 0;
+    for (;;) {
+      // a round of levels without a host round trip: a level whose input is empty costs one empty launch
+      for (int r = 0; r < kLevelsPerRound && level <= ZG_MAX_DEPTH + 1; ++r, ++level) {
+        p.in = rb_front_[cur].as<unsigned long long>();
+        p.out = rb_front_[cur ^ 1].as<unsigned long long>();
+        p.level = level;
+        fwalk_expand_kernel<<<sm_count_ * 8, 256, 0, stream>>>(p);
+        ++launches;
+        cur ^= 1;
+      }
+      unsigned long long host[2] = {0, 0}, last = 0;
+      ZG_CUDA(cudaMemcpyAsync(host, ctrl, sizeof host, cudaMemcpyDeviceToHost, stream));
+      ZG_CUDA(cudaMemcpyAsync(&last, counts + level, 8, cudaMemcpyDeviceToHost, stream));
+      ZG_CUDA(cudaStreamSynchronize(stream));
+      if (static_cast<uint32_t>(host[0]) & 16u) break;  // frontier / candidate buffers overflowed: verify every object
+      if (last == 0 || level > ZG_MAX_DEPTH + 1) {      // deeper objects cannot be within the dispatch cap anyway
+        walked = true;
+        n = host[1];
+        break;
+      }
+    }
+  }
+  if (walked) {
+    ++subject_lookups_walk;
+  } else {
+    const uint64_t no = s->n_objects[stype];
+    n = no + 1;
+    if (!ls_jobs_.ensure(n * sizeof(zg_check))) {
+      if (err) *err = "out of device memory (lookup)";
+      return ZG_ENOMEM;
+    }
+    ls_fill_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(proto, no, ls_jobs_.as<zg_check>());
+    ++launches;
+    ++subject_lookups_exhaustive;
+  }
+  ans->fell_back = !walked;
+  ans->n_verified = n;
+  subject_items_verified += n;
+  if (!ls_codes_.ensure(n) || !ls_has_.ensure(n * sizeof(zg_check)) || !ls_ids_.ensure(n * 16 + 64)) {
+    if (err) *err = "out of device memory (lookup)";
+    return ZG_ENOMEM;
+  }
+  uint32_t* has_ids = ls_ids_.as<uint32_t>();
+  uint32_t* no_ids = has_ids + n;
+  uint32_t* out_ids = no_ids + n;
+  uint32_t* tmp_ids = out_ids + n;
+  uint8_t* codes = ls_codes_.as<uint8_t>();
+  int rc = check_device(ls_jobs_.as<zg_check>(), n, codes, stream, true, nullptr, err);
+  if (rc) return rc;
+  if (n > 1) {
+    ls_split_kernel<<<static_cast<unsigned>((n - 1 + 255) / 256), 256, 0, stream>>>(
+        ls_jobs_.as<zg_check>(), codes, n, has_ids, ls_has_.as<zg_check>(), no_ids, ctrl + 2, lflags);
+    ++launches;
+  }
+  uint8_t probe = 0;
+  unsigned long long hc[4] = {0, 0, 0, 0};
+  uint32_t cflags = 0;
+  ZG_CUDA(cudaMemcpyAsync(&probe, codes, 1, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaMemcpyAsync(hc, ctrl, sizeof hc, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaMemcpyAsync(&cflags, ctrl_.as<unsigned long long>() + 3, 4, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  if (cflags & 1u) {
+    if (err) *err = "expansion stack overflow (per-warp spill area exhausted)";
+    return ZG_ENOMEM;
+  }
+  if (probe == ZG_ITEM_ERROR || (static_cast<uint32_t>(hc[0]) & 8u)) {
+    // as LookupResources: a silently shortened answer would read as "not allowed"
+    if (err) *err = "LookupSubjects: a subject could not be decided (max dispatch depth / work budget exceeded)";
+    return ZG_EDEPTH;
+  }
+  const uint64_t n_has = hc[2], n_no = hc[3];
+  const bool granted = srel == kNone && probe == ZG_HAS_PERMISSION;
+  const uint32_t* concrete = has_ids;
+  uint64_t n_concrete = n_has;
+  if (granted && n_has) {
+    // The wildcard is granted: list the subjects that also check HAS with every wildcard relationship
+    // invisible. An undecidable one is only "not listed": it checked HAS, the wildcard covers it.
+    no_wildcards_ = true;
+    rc = check_device(ls_has_.as<zg_check>(), n_has, codes, stream, true, nullptr, err);
+    no_wildcards_ = false;
+    if (rc) return rc;
+    lookup_compact_kernel<<<static_cast<unsigned>((n_has + 255) / 256), 256, 0, stream>>>(
+        has_ids, codes, n_has, out_ids, n_has, ctrl + 4, reinterpret_cast<uint32_t*>(ctrl + 5));
+    ++launches;
+    unsigned long long cnt = 0;
+    ZG_CUDA(cudaMemcpyAsync(&cnt, ctrl + 4, 8, cudaMemcpyDeviceToHost, stream));
+    ZG_CUDA(cudaMemcpyAsync(&cflags, ctrl_.as<unsigned long long>() + 3, 4, cudaMemcpyDeviceToHost, stream));
+    ZG_CUDA(cudaStreamSynchronize(stream));
+    if (cflags & 1u) {
+      if (err) *err = "expansion stack overflow (per-warp spill area exhausted)";
+      return ZG_ENOMEM;
+    }
+    concrete = out_ids;
+    n_concrete = cnt;
+  }
+  ans->wildcard = granted && include_wildcard;
+  // ascending ids: radix sort on the device when the list is large
+  auto fetch = [&](const uint32_t* d, uint64_t cnt, std::vector<uint32_t>* out) -> int {
+    out->resize(cnt);
+    if (!cnt) return ZG_OK;
+    const uint32_t* src = d;
+    if (cnt > 2048) {
+      std::string serr = sort_u32(d, tmp_ids, cnt, stream);
+      if (!serr.empty()) {
+        if (err) *err = serr;
+        return ZG_ECUDA;
+      }
+      src = tmp_ids;
+    }
+    ZG_CUDA(cudaMemcpyAsync(out->data(), src, cnt * 4, cudaMemcpyDeviceToHost, stream));
+    ZG_CUDA(cudaStreamSynchronize(stream));
+    if (cnt <= 2048) std::sort(out->begin(), out->end());
+    return ZG_OK;
+  };
+  rc = fetch(concrete, n_concrete, &ans->ids);
+  if (!rc && ans->wildcard) rc = fetch(no_ids, n_no, &ans->excluded);
+  return rc;
 }
 
 }  // namespace zg

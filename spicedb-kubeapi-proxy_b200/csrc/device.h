@@ -42,6 +42,9 @@ struct Snapshot {
   std::vector<DevBuf> flat_cls;
   std::vector<int> flat_n;
   std::vector<DevBuf> resources;  // per type
+  // LookupSubjects' forward walk: Schema::forward_tables / fwd_mask of this layout
+  DevBuf ls_fwd, ls_type_off, ls_mask;
+  uint32_t ls_mask_words = 1;
   std::vector<uint64_t> n_resources;
   uint32_t prog_bytes = 0;
   uint32_t max_leaves = 1;
@@ -88,6 +91,20 @@ class Device {
   int lookup_batch(const std::vector<LookupReq>& reqs, std::vector<std::vector<uint32_t>>* ids, std::vector<int>* rcs,
                    std::string* err);
   uint64_t lookup_batches = 0, lookups_batched = 0;
+  // LookupSubjects (T:res#perm, subjects of type stype[#srel]): forward walk from the resource (else every object of
+  // stype when the walk overflows or use_rbfs is off), the wildcard probe, one verification launch, a second
+  // one without wildcard relationships when the wildcard is granted, compaction, sort, one copy back. ids:
+  // subjects listed concretely, ascending; excluded: subjects the granted wildcard does not cover (only with
+  // include_wildcard). ZG_EDEPTH when the probe or a candidate cannot be decided.
+  struct SubjectsAnswer {
+    std::vector<uint32_t> ids, excluded;
+    bool wildcard = false;       // the wildcard entry is present
+    bool fell_back = false;      // every object of the subject type was verified
+    uint64_t n_verified = 0;     // items of the first verification launch (probe included)
+  };
+  int lookup_subjects(uint16_t res_type, uint32_t res, uint16_t perm, uint16_t stype, uint16_t srel, bool include_wildcard,
+                      SubjectsAnswer* ans, std::string* err);
+  uint64_t subject_lookups_walk = 0, subject_lookups_exhaustive = 0, subject_items_verified = 0;
 
   // ---- object-hash sharded store: one pass at a time, sub-queries routed by the host ----
   uint32_t shard_count = 1, shard_rank = 0;
@@ -146,6 +163,8 @@ class Device {
   DevBuf stage_in_, stage_out_, lk_jobs_, lk_codes_, lk_ids_;
   DevBuf rb_visited_, rb_front_[2], rb_cand_;
   DevBuf lb_params_, lb_owner_, lb_ctrl_, lb_keys_[2];  // batched lookups
+  DevBuf ls_jobs_, ls_codes_, ls_has_, ls_ids_, ls_ctrl_;   // LookupSubjects
+  bool no_wildcards_ = false;  // run_pass: KParams::no_wildcards (LookupSubjects' second verification)
   uint64_t lb_cap_ = 1ull << 24;  // frontier entries / candidates of one lookup batch (ZGPU_LOOKUP_BATCH_CAP)
   void* pin_lk_ = nullptr;
   size_t pin_lk_cap_ = 0;

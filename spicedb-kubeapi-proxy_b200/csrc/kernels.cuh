@@ -129,6 +129,9 @@ struct KParams {
   // number of leading queries that have landed (a 8-byte copy enqueued after each chunk on the copy stream);
   // a warp waits until its batch is there. nullptr: everything is resident.
   const unsigned long long* ready;
+  // LookupSubjects' second verification: every wildcard relationship is invisible (an ST_WILD step never matches),
+  // so a subject that checks HAS is granted through its own relationships. Never set by the public check calls.
+  int no_wildcards;
 };
 
 // View of the program blob. Only the base pointer is kept in registers; table addresses are
@@ -499,7 +502,7 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
     const DStep st = pr.steps()[sb + i];
     const bool expiry = (st.flags & CF_EXPIRY) != 0;
     const bool subject_fits = srel == kNone && stype == st.stype;
-    if (!subject_fits) continue;
+    if (!subject_fits || (st.kind == ST_WILD && p.no_wildcards)) continue;
     if (st.kind == ST_DIRECT && inverted && (st.flags & CF_INVERT)) {
       // direction-optimised probe: is obj among the subject's memberships of this class? Most probes miss: a
       // 32-bit presence word over (class, object) of the check's set (built at admission) rejects them
@@ -1389,6 +1392,143 @@ __global__ void lookup_compact_kernel(const uint32_t* cand, const uint8_t* codes
   if (has) {
     const unsigned long long at = base + __popc(m & ((1u << lane) - 1u));
     if (at < cap) out[at] = cand[i];
+  }
+}
+
+// ---- LookupSubjects: forward walk from the resource (the mirror of mrbfs_expand_kernel) -------------------
+//
+// Every subject s with Check(T:r#P @ ST:s[#SR]) = HAS is the subject of a relationship on some object the
+// evaluation of P visits, or is one of those objects itself (userset self-membership). Walking the forward CSR
+// from r over the edge classes P's evaluation can read (FwalkParams::mask, Schema::fwd_mask) therefore reaches a
+// SUPERSET of the answer (expiry and & / - are ignored), and one check launch verifies it. Wildcard classes
+// are not walked: they name no subject, the wildcard probe item covers them.
+struct FwalkParams {
+  const uint32_t* row_ptr;
+  const uint32_t* col;
+  const FwdClass* fwd;                 // fwd[type_off[t], type_off[t + 1]): edge classes of the relations of type t
+  const uint32_t* type_off;
+  const uint32_t* mask;                // bit gc: class gc is read by the permission's evaluation
+  unsigned long long* in;              // type << 32 | object
+  unsigned long long* out;
+  unsigned long long* counts;          // counts[level] = entries of `in`, counts[level + 1] = entries of `out`
+  int level;
+  unsigned long long cap;              // frontier capacity
+  uint32_t* visited;                   // bitmap over all objects, bit = type_bit_base[type] + object
+  const unsigned long long* type_bit_base;
+  zg_check proto;                      // res, perm, stype, srel of the lookup; subj is set per candidate
+  zg_check* cand;
+  unsigned long long* cand_count;
+  unsigned long long cand_cap;
+  uint32_t* flags;                     // bit 4: frontier / candidate overflow
+};
+
+// Level 0 of the walk and the two items every lookup verifies: [0] the wildcard probe (a never-written subject:
+// it stands for every subject outside the candidates), [1] the resource itself when it has the subject type.
+__global__ void fwalk_seed_kernel(const FwalkParams p, uint32_t res_type) {
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  const unsigned long long bit = p.type_bit_base[res_type] + p.proto.res;
+  p.visited[bit >> 5] |= 1u << (bit & 31);
+  p.in[0] = (static_cast<unsigned long long>(res_type) << 32) | p.proto.res;
+  p.counts[0] = 1;
+  zg_check q = p.proto;
+  q.subj = ZG_NO_OBJECT - 1;
+  p.cand[0] = q;
+  unsigned long long n = 1;
+  if (res_type == p.proto.stype) {
+    q.subj = p.proto.res;
+    p.cand[n++] = q;
+  }
+  *p.cand_count = n;
+}
+
+// One warp per frontier object: for every masked class of the object's type, read its forward row (coalesced)
+// and mark the subjects. Reads its input count from device memory: the level loop needs no host round trip.
+__global__ void __launch_bounds__(256) fwalk_expand_kernel(const FwalkParams p) {
+  const unsigned long long n_in = p.counts[p.level];
+  if (n_in == 0 || n_in > p.cap) return;
+  const unsigned lane = threadIdx.x & 31;
+  const unsigned long long n_warps = (static_cast<unsigned long long>(gridDim.x) * blockDim.x) >> 5;
+  for (unsigned long long w = (blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x) >> 5; w < n_in;
+       w += n_warps) {
+    const unsigned long long item = p.in[w];
+    const uint32_t type = static_cast<uint32_t>(item >> 32), obj = static_cast<uint32_t>(item);
+    for (uint32_t ci = p.type_off[type]; ci < p.type_off[type + 1]; ++ci) {
+      const FwdClass fc = p.fwd[ci];
+      if (!((p.mask[fc.gc >> 5] >> (fc.gc & 31)) & 1u) || obj >= fc.nres) continue;
+      const unsigned long long ri = fc.row_base + static_cast<unsigned long long>(obj) * fc.ncls;
+      const uint32_t b = __ldg(p.row_ptr + ri), e = __ldg(p.row_ptr + ri + 1);
+      const unsigned long long bit_base = p.type_bit_base[fc.stype];
+      for (uint32_t i0 = b; i0 < e; i0 += 32) {
+        const uint32_t i = i0 + lane;
+        bool fresh = false;
+        uint32_t s = 0;
+        if (i < e) {
+          s = __ldg(p.col + i);
+          const unsigned long long bit = bit_base + s;
+          const uint32_t m = 1u << (bit & 31);
+          fresh = !(atomicOr(p.visited + (bit >> 5), m) & m);
+        }
+        const unsigned fm = __ballot_sync(kFull, fresh);
+        if (fm) {
+          unsigned long long at = 0;
+          if (lane == 0) at = atomicAdd(p.counts + p.level + 1, static_cast<unsigned long long>(__popc(fm)));
+          at = __shfl_sync(kFull, at, 0) + __popc(fm & ((1u << lane) - 1u));
+          if (fresh) {
+            if (at < p.cap) p.out[at] = (static_cast<unsigned long long>(fc.stype) << 32) | s;
+            else atomicOr(p.flags, 16u);
+          }
+        }
+        const bool is_cand = fresh && fc.stype == p.proto.stype;
+        const unsigned cm = __ballot_sync(kFull, is_cand);
+        if (cm) {
+          unsigned long long at = 0;
+          if (lane == 0) at = atomicAdd(p.cand_count, static_cast<unsigned long long>(__popc(cm)));
+          at = __shfl_sync(kFull, at, 0) + __popc(cm & ((1u << lane) - 1u));
+          if (is_cand) {
+            if (at < p.cand_cap) {
+              zg_check q = p.proto;
+              q.subj = s;
+              p.cand[at] = q;
+            } else {
+              atomicOr(p.flags, 16u);
+            }
+          }
+        }
+      }
+    }
+  }
+}
+
+// Walk overflow (or ZGPU_NO_RBFS): every object of the subject type is a candidate, behind the probe item.
+__global__ void ls_fill_kernel(zg_check proto, unsigned long long n, zg_check* jobs) {
+  const unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x;
+  if (i > n) return;
+  proto.subj = i == 0 ? ZG_NO_OBJECT - 1 : static_cast<uint32_t>(i - 1);
+  jobs[i] = proto;
+}
+
+// Verified candidates [1, n) (item 0 is the probe): HAS subjects go to has_ids and has_items (the input of the
+// no-wildcards pass), NO subjects to no_ids; an undecidable candidate sets flags bit 3. counts: [0] HAS, [1] NO.
+__global__ void ls_split_kernel(const zg_check* items, const uint8_t* codes, unsigned long long n, uint32_t* has_ids,
+                                zg_check* has_items, uint32_t* no_ids, unsigned long long* counts, uint32_t* flags) {
+  const unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x + 1;
+  const uint8_t code = i < n ? codes[i] : 0;
+  const bool has = code == ZG_HAS_PERMISSION, no = code == ZG_NO_PERMISSION;
+  const unsigned lane = threadIdx.x & 31;
+  if (__any_sync(kFull, code == ZG_ITEM_ERROR) && lane == 0) atomicOr(flags, 8u);
+  const unsigned hm = __ballot_sync(kFull, has), nm = __ballot_sync(kFull, no);
+  unsigned long long hb = 0, nb = 0;
+  if (lane == 0 && hm) hb = atomicAdd(counts, static_cast<unsigned long long>(__popc(hm)));
+  if (lane == 0 && nm) nb = atomicAdd(counts + 1, static_cast<unsigned long long>(__popc(nm)));
+  hb = __shfl_sync(kFull, hb, 0);
+  nb = __shfl_sync(kFull, nb, 0);
+  const unsigned below = (1u << lane) - 1u;
+  if (has) {
+    const unsigned long long at = hb + __popc(hm & below);
+    has_ids[at] = items[i].subj;
+    has_items[at] = items[i];
+  } else if (no) {
+    no_ids[nb + __popc(nm & below)] = items[i].subj;
   }
 }
 

@@ -591,7 +591,70 @@ std::string Schema::compile() {
       if (d_cls[c].stype == t) d_rcls.push_back(static_cast<uint16_t>(c));
     d_type_rcls[t].end = static_cast<uint16_t>(d_rcls.size());
   }
+  compute_forward_masks();
   return "";
+}
+
+void Schema::compute_forward_masks() {
+  std::vector<uint32_t> cls_begin(rel_slots.size() + 1, 0);
+  for (size_t r = 0; r < rel_slots.size(); ++r)
+    cls_begin[r + 1] = cls_begin[r] + static_cast<uint32_t>(slots[rel_slots[r]].classes.size());
+  fwd_mask_words = std::max<uint32_t>(1, (cls_begin.back() + 31) / 32);
+  fwd_mask.assign(slots.size() * fwd_mask_words, 0);
+  for (size_t s = 0; s < slots.size(); ++s) {
+    uint32_t* m = fwd_mask.data() + s * fwd_mask_words;
+    std::vector<uint8_t> seen(slots.size(), 0);
+    std::vector<uint16_t> todo{static_cast<uint16_t>(s)};
+    while (!todo.empty()) {
+      const uint16_t x = todo.back();
+      todo.pop_back();
+      if (x >= slots.size() || seen[x]) continue;
+      seen[x] = 1;
+      std::vector<uint16_t> units;
+      if (d_slots[x].kind == SK_NONPURE) {
+        const DTree& t = d_trees[d_slots[x].unit];
+        for (uint16_t l = 0; l < t.n_leaves; ++l) units.push_back(d_leaf_units[t.leaf_begin + l]);
+      } else {
+        units.push_back(d_slots[x].unit);
+      }
+      for (uint16_t u : units)
+        for (int oi = d_units[u].op_begin; oi < d_units[u].op_end; ++oi) {
+          const DOp& op = d_ops[oi];
+          const auto& classes = slots[rel_slots[op.rel]].classes;
+          for (size_t k = 0; k < classes.size(); ++k) {
+            if (classes[k].sslot == kWildcard) continue;
+            const uint32_t gc = cls_begin[op.rel] + static_cast<uint32_t>(k);
+            m[gc >> 5] |= 1u << (gc & 31);
+            if (op.kind == OP_ARROW) todo.push_back(d_tgts[op.tgt_begin + k]);
+            else if (classes[k].sslot != kNone) todo.push_back(classes[k].sslot);
+          }
+        }
+    }
+  }
+}
+
+void Schema::forward_tables(const std::vector<DRel>& rels, std::vector<FwdClass>* fwd, std::vector<uint32_t>* type_off) const {
+  fwd->clear();
+  type_off->assign(types.size() + 1, 0);
+  for (size_t t = 0; t < types.size(); ++t) {
+    (*type_off)[t] = static_cast<uint32_t>(fwd->size());
+    for (size_t r = 0; r < rels.size() && r < rel_slots.size(); ++r) {
+      if (slots[rel_slots[r]].type != t) continue;
+      const DRel& d = rels[r];
+      for (uint16_t k = 0; k < d.ncls; ++k) {
+        const uint16_t gc = static_cast<uint16_t>(d.cls_begin + k);
+        if (d_cls[gc].sslot == kWildcard) continue;
+        FwdClass f{};
+        f.row_base = d.row_base + k;
+        f.nres = d.nres;
+        f.ncls = static_cast<uint16_t>(d.stride);
+        f.stype = d_cls[gc].stype;
+        f.gc = gc;
+        fwd->push_back(f);
+      }
+    }
+  }
+  (*type_off)[types.size()] = static_cast<uint32_t>(fwd->size());
 }
 
 std::vector<uint8_t> Schema::blob(const std::vector<DRel>& rels, const std::vector<DCls>& cls) const {

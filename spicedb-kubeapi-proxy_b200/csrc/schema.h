@@ -102,6 +102,14 @@ struct DCls {
   uint64_t rrow_base;  // reverse CSR: rrow_ptr index of (subject 0, this class); row of subject s =
                        // rrow_base + s * rstride
 };
+struct FwdClass {  // LookupSubjects' forward walk: one non-wildcard edge class, grouped by resource type
+  uint64_t row_base;  // row_ptr index of (object 0, this class)
+  uint32_t nres;      // objects covered by the relation's row table
+  uint16_t ncls;      // row stride per object
+  uint16_t stype;     // type of the subjects (the children)
+  uint16_t gc;        // global class id (bit of Schema::fwd_mask)
+  uint16_t pad[3];
+};
 struct DTypeInv {  // per subject type: the invertible direct classes (inv_cls[begin, end))
   uint16_t begin, end;
 };
@@ -191,8 +199,16 @@ class Schema {
   std::vector<uint8_t> blob(const std::vector<DRel>& rels, const std::vector<DCls>& cls) const;
   std::vector<DTypeInv> d_type_inv, d_type_rcls;
   std::vector<uint16_t> d_inv_cls, d_rcls;
+  // LookupSubjects: per slot, fwd_mask_words words whose bit gc says that class gc is read by the slot's
+  // evaluation (the closure over REL / ARROW ops and userset child slots, wildcard classes excluded).
+  std::vector<uint32_t> fwd_mask;
+  uint32_t fwd_mask_words = 1;
+  // Per resource type, its relations' non-wildcard classes with their rows in this snapshot's layout:
+  // fwd[type_off[t], type_off[t + 1]).
+  void forward_tables(const std::vector<DRel>& rels, std::vector<FwdClass>* fwd, std::vector<uint32_t>* type_off) const;
 
  private:
+  void compute_forward_masks();
   std::string compile();
   int name_id(const std::string& n);
 };
