@@ -431,6 +431,11 @@ int zg_stats_get(zg_engine *e, zg_stats *out);
  * ALGORITHMIC bytes it needed (DESIGN.md "Algorithmic bytes"); not for timing. */
 int zg_count_alg_bytes(zg_engine *e, const zg_check *items, uint64_t n, uint64_t *bytes);
 
+/* Cumulative clock64() cycles the check kernel's warps spent per phase since the engine was created:
+ * admission, root visit, two-level meet, one-level meet, pop loop (the visits exclude the meets inside them).
+ * Only a library built with -DZG_PHASE_CLOCKS=1 counts them; any other build returns ZG_EINVAL. */
+int zg_phase_clocks(zg_engine *e, uint64_t cycles[5]);
+
 #ifdef __cplusplus
 }
 #endif

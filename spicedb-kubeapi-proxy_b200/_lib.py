@@ -201,6 +201,7 @@ _SIGS = {
                                     C.c_size_t, C.POINTER(C.c_size_t)]),
     "zg_stats_get": (C.c_int, [C.c_void_p, C.POINTER(_Stats)]),
     "zg_count_alg_bytes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),
+    "zg_phase_clocks": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64)]),
 }
 
 
@@ -689,3 +690,11 @@ class Engine:
         b = C.c_uint64(0)
         self._ck(self._L.zg_count_alg_bytes(self._h, items.ctypes.data, items.size, C.byref(b)))
         return b.value
+
+    PHASES = ("admission", "root_visit", "l2_meet", "l1_meet", "pop_loop")
+
+    def phase_clocks(self) -> dict:
+        """Cumulative check-kernel cycles per phase (a library built with -DZG_PHASE_CLOCKS=1 only)."""
+        c = (C.c_uint64 * len(self.PHASES))()
+        self._ck(self._L.zg_phase_clocks(self._h, c))
+        return dict(zip(self.PHASES, (int(x) for x in c)))

@@ -937,6 +937,16 @@ extern "C" int zg_count_alg_bytes(zg_engine* e, const zg_check* items, uint64_t 
   return ZG_OK;
 }
 
+extern "C" int zg_phase_clocks(zg_engine* e, uint64_t cycles[5]) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (!cycles) return fail(ZG_EINVAL, "NULL argument");
+  std::lock_guard<FairMutex> g(e->mu);
+  if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
+  std::string err;
+  const int rc = e->dev.read_phase_clocks(cycles, &err);
+  return rc ? fail(rc, err) : ZG_OK;
+}
+
 // Resolve a CHECK item without interning anything (query strings must not grow the store).
 // The items of one bulk call mostly repeat their literal fields -- a post-filter sends one template
 // per list item, so type, permission and subject are constant and only the resource id varies

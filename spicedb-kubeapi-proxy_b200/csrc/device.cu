@@ -337,6 +337,11 @@ std::string Device::finish_publish(std::shared_ptr<Snapshot> s, const HostSnapsh
   s->prog_bytes = static_cast<uint32_t>(blob.size());
   s->max_leaves = sc.max_leaves;
   s->has_nonpure = sc.has_nonpure;
+  {
+    const DHeader* ph = reinterpret_cast<const DHeader*>(blob.data());
+    const DStep* steps = reinterpret_cast<const DStep*>(blob.data() + ph->off_steps);
+    for (uint32_t i = 0; i < ph->n_steps; ++i) s->has_l2 = s->has_l2 || (steps[i].flags & kStepTargetL2);
+  }
   s->revision = revision;
 
   // occupancy for this program size (dynamic shared memory = program + warp stacks)
@@ -353,6 +358,9 @@ std::string Device::finish_publish(std::shared_ptr<Snapshot> s, const HostSnapsh
       cudaFuncSetAttribute(check_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sm));
       cudaFuncSetAttribute(check_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sm));
       cudaFuncSetAttribute(check_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sm));
+      cudaFuncSetAttribute(check_kernel<false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sm));
+      cudaFuncSetAttribute(check_kernel<true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sm));
+      cudaFuncSetAttribute(check_kernel<false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sm));
       attr_bytes = sm;
     }
   }
@@ -418,9 +426,10 @@ int Device::run_pass(const Snapshot& s, const zg_check* queries, uint64_t nq, ui
   int grid = static_cast<int>(std::min<uint64_t>(want, static_cast<uint64_t>(sm_count_) * per_sm));
   if (grid < 1) grid = 1;
   size_t sm = smem_bytes(s.prog_bytes);
-  if (count) check_kernel<true><<<grid, kThreads, sm, st>>>(p);
-  else if (ready) check_kernel<false, true><<<grid, kThreads, sm, st>>>(p);
-  else check_kernel<false><<<grid, kThreads, sm, st>>>(p);
+  // a schema without a two-level step runs the kernel built without the two-level meet
+  if (count) (s.has_l2 ? check_kernel<true> : check_kernel<true, false, false>)<<<grid, kThreads, sm, st>>>(p);
+  else if (ready) (s.has_l2 ? check_kernel<false, true> : check_kernel<false, true, false>)<<<grid, kThreads, sm, st>>>(p);
+  else (s.has_l2 ? check_kernel<false> : check_kernel<false, false, false>)<<<grid, kThreads, sm, st>>>(p);
   ZG_CUDA(cudaGetLastError());
   ++launches;
   return ZG_OK;
@@ -433,6 +442,19 @@ void Device::read_events(uint64_t* spills, uint64_t* memo_batches) {
     cudaStreamSynchronize(stream);
   *spills = ev[0];
   *memo_batches = ev[1];
+}
+
+int Device::read_phase_clocks(uint64_t* cycles, std::string* err) {
+  if (!ZG_PHASE_CLOCKS) {
+    if (err) *err = "library built without phase clocks (scripts/build_variant.sh NAME -DZG_PHASE_CLOCKS=1)";
+    return ZG_EINVAL;
+  }
+  unsigned long long ph[kPhases] = {0};
+  ZG_CUDA(cudaSetDevice(device));
+  ZG_CUDA(cudaMemcpyAsync(ph, ctrl_.as<unsigned long long>() + 11, sizeof ph, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  for (int i = 0; i < kPhases; ++i) cycles[i] = ph[i];
+  return ZG_OK;
 }
 
 void Device::finish_timing() {

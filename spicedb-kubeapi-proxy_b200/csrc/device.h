@@ -49,6 +49,7 @@ struct Snapshot {
   uint32_t prog_bytes = 0;
   uint32_t max_leaves = 1;
   bool has_nonpure = false;
+  bool has_l2 = false;  // some step of the program meets two levels (kStepTargetL2)
   uint64_t n_tuples = 0, bytes = 0, revision = 0;
   ~Snapshot();
 };
@@ -138,6 +139,7 @@ class Device {
   uint64_t split_batches = 0;  // batches answered in halves because their sub-queries overflowed the pass buffer
   // cumulative device-side event counters: stack spills to HBM, batches that switched the path memo on
   void read_events(uint64_t* spills, uint64_t* memo_batches);
+  int read_phase_clocks(uint64_t* cycles, std::string* err);  // ZG_PHASE_CLOCKS builds: 5 cumulative phase totals
   uint64_t lookups_rbfs = 0, lookups_exhaustive = 0, lookups_flat = 0;
   bool use_rbfs = true;  // ZGPU_NO_RBFS=1: LookupResources checks every resource of the type  // batcher: launches that served > 1 caller
   double last_ms = 0;
@@ -156,7 +158,8 @@ class Device {
   uint32_t spill_cap_ = 4096, budget_ = 1u << 20;
   uint64_t subq_cap_ = 1ull << 22;
   DevBuf spill_, ctrl_, memo_;
-  uint32_t memo_entries_ = 8192, memo_after_ = 2048;  // ctrl: [0] next, [1] subq_count, [2] alg_bytes, then flags u32
+  uint32_t memo_entries_ = 8192, memo_after_ = 2048;  // ctrl: [0] next, [1] subq_count, [2] alg_bytes, then flags u32;
+                                                      // [8 .. 9] events, [10] items landed, [11 .. 15] phase clocks
   std::vector<DevBuf> q_, parent_, val_;  // per pass level: queries, raising (query, leaf), leaf values
   std::vector<uint64_t> shard_nq_, shard_nsub_;  // sharded mode: queries / raised sub-queries per level
   DevBuf shard_tmp_, route_ctrl_;

@@ -70,9 +70,15 @@ constexpr int kThreads = kWarpsPerBlock * 32;
                        // (measured alone: slightly faster on cfg3)
 #endif
 #ifndef ZG_L2_MODE
-#define ZG_L2_MODE 2  // two-level meet: 2 = warp-cooperative (default), 1 = per-lane Bloom word + 128-bit streaming
-                      // (measured slower on cfg3), 0 = per-lane sorted-segment intersection
+#define ZG_L2_MODE 2  // two-level meet: 2 = every requesting lane of a visit at once (batch_l2, default), 3 = one requesting
+                      // lane after the other with the whole warp on its range (coop_l2), 1 = per-lane Bloom word +
+                      // 128-bit streaming (measured slower on cfg3), 0 = per-lane sorted-segment intersection
 #endif
+#ifndef ZG_PHASE_CLOCKS
+#define ZG_PHASE_CLOCKS 0  // 1: every warp adds clock64() cycles per phase of a batch into KParams::events[3 .. 7]
+                           // (admission, root visit, two-level meet, one-level meet, pop loop; zg_phase_clocks)
+#endif
+constexpr int kPhases = 5;
 constexpr int kMinBlocks = ZG_MIN_BLOCKS;  // resident CTAs per SM the register budget is tuned for
 constexpr int kStackCap = ZG_STACK_CAP;    // range items per warp in shared memory
 constexpr int kRsetCap = ZG_RSET_CAP;      // reverse-row entries kept per check (subject's direct memberships), <= 31
@@ -80,6 +86,7 @@ constexpr int kStateWords = 6;             // per-lane query state parked in sha
 constexpr int kFCap = 64;                  // children of a range staged in shared memory by the two-level meet
 constexpr int kFBloom = ZG_L2_FILTER ? 64 : 0;  // words of the filter over those children
 constexpr size_t kWarpSmem = kStackCap * sizeof(uint4) + ((kRsetCap + kStateWords) * 32 + kFCap + kFBloom) * sizeof(uint32_t);
+static_assert(ZG_L2_MODE != 2 || kFCap + kFBloom >= 128, "batch_l2 keeps a 128-bit filter per lane in the meet's area");
 constexpr unsigned kFull = 0xFFFFFFFFu;
 constexpr uint16_t kJobDepthMask = 0x00FF;  // zg_check.flags of a raised sub-query: hop depth
 
@@ -124,7 +131,8 @@ struct KParams {
   uint32_t shard_count;   // 0 / 1 = not sharded
   uint32_t shard_rank;
   unsigned long long* alg_bytes;  // COUNT variant only
-  unsigned long long* events;     // [0] stack spills, [1] batches that switched the path memo on (cumulative)
+  unsigned long long* events;     // [0] stack spills, [1] batches that switched the path memo on (cumulative),
+                                  // [3 .. 7] phase cycles (ZG_PHASE_CLOCKS builds only)
   // Streamed admission: the queries are still being copied from the host while the kernel runs. *ready =
   // number of leading queries that have landed (a 8-byte copy enqueued after each chunk on the copy stream);
   // a warp waits until its batch is there. nullptr: everything is resident.
@@ -179,11 +187,14 @@ struct WarpCtx {
   // there are <= kRsetCap.
   uint32_t* rset;
   unsigned long long my_cst;  // class boundaries of this lane's own job (see cst_at)
-  unsigned inv_mask;  // jobs whose reverse rows fit
+  unsigned inv_mask;  // jobs that may meet in the middle: their reverse rows fit, or (cst bit kOverCap) only batch_l2 meets
   unsigned long long bytes;
   unsigned long long* events;
   bool fatal;
   unsigned lane;
+#if ZG_PHASE_CLOCKS
+  long long ph[kPhases];  // warp-uniform cycles: admission, root visit, two-level meet, one-level meet, pop loop
+#endif
 };
 
 template <bool COUNT>
@@ -326,7 +337,9 @@ __device__ __forceinline__ bool intersects(const uint32_t* __restrict__ a, uint3
 }
 
 // Boundaries of a job's reverse-row set per invertible class of its subject type:
-// 5 bits each (0..31), boundary i at bit 5*i; class i owns entries [b_i, b_{i+1}).
+// 5 bits each (0..31), boundary i at bit 5*i; class i owns entries [b_i, b_{i+1}). Bit kOverCap: the subject has more
+// memberships than the set holds (no boundary is valid; the two-level meet reads them from the subject's reverse rows).
+constexpr uint32_t kOverCap = 63;
 __device__ __forceinline__ uint32_t cst_at(unsigned long long cst, uint32_t i) {
   return static_cast<uint32_t>(cst >> (5u * i)) & 31u;
 }
@@ -472,11 +485,146 @@ __device__ __noinline__ bool coop_l2(const uint32_t* __restrict__ col, const uin
   return false;
 }
 
+// Filter of batch_l2: two bits per object id in 128 (two 64-bit words). False-positive rate (1 - e^(-2n/128))^2 over
+// a range of n children: 2 % at n = 10 (cfg3's mean), 12 % at n = 27 (its largest); only the search behind it answers.
+__device__ __forceinline__ void l2_bits(uint32_t v, uint32_t& b1, uint32_t& b2) {
+  const uint32_t hv = v * 0x9E3779B1u;
+  b1 = hv >> 25;
+  b2 = (hv >> 18) & 127u;
+}
+__device__ __forceinline__ bool l2_maybe(unsigned long long f0, unsigned long long f1, uint32_t v) {
+  uint32_t b1, b2;
+  l2_bits(v, b1, b2);
+  return ((((b1 & 64u) ? f1 : f0) >> (b1 & 63u)) & (((b2 & 64u) ? f1 : f0) >> (b2 & 63u)) & 1ull) != 0;
+}
+
+// Two-level meet, batched: every requesting lane of a visit round at once (coop_l2 serves them one after the other).
+// Lane j wants "does some membership g of its subject (class tinv) list a child of its range col[lo, hi) in class
+// tgc". Its memberships are rset entries [kb, ke) of its job, or -- for a subject with more memberships than the set
+// holds -- the subject's own reverse row of class tinv. The (lane, membership) pairs of the whole warp are numbered
+// with one scan and dealt out 32 at a time: every lane reads one pair's reverse row (all 32 rows in flight together)
+// and tests its elements against the owner's 128-bit filter of the range; a "maybe" is verified by a binary search of
+// the range, which lane j has just read. Pairs of a check that is already answered are skipped.
+// k packs ke << 8 | kb (set entries) or 0x8000 | tinv (reverse row), and tgc << 16. Requesting lanes are those of
+// checks not answered yet. Returns the job slots answered.
+// Ranges are <= kFCap children (the caller keeps larger ones). Inlined: out of line (as coop_l2 is) the call site
+// spilled more of the traversal loop's registers (ptxas) and ran no faster on cfg3 (H100, DESIGN.md §6).
+template <bool COUNT>
+__device__ __forceinline__ unsigned batch_l2(const uint32_t* __restrict__ col, const uint32_t* __restrict__ rrow_ptr,
+                                          const uint32_t* __restrict__ rcol, uint32_t* rset, uint32_t lane, bool want,
+                                          uint32_t lo, uint32_t hi, uint32_t k, uint32_t jslot, uint32_t sid, uint32_t stype,
+                                          unsigned long long* bytes) {
+  ZG_DYNAMIC_SMEM(smem);
+  const Prog pr = make_prog(smem);  // the program is staged at the start of shared memory
+  unsigned long long nb = 0;
+  unsigned long long f0 = 0, f1 = 0;
+  uint32_t mb = 0, me = 0;
+  if (want) {
+    for (uint32_t x = lo; x < hi; x += 4) {  // four independent loads in flight
+      uint32_t v[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) v[i] = x + i < hi ? __ldg(col + x + i) : 0u;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        if (x + i >= hi) break;
+        uint32_t b1, b2;
+        l2_bits(v[i], b1, b2);
+        if (b1 & 64u) f1 |= 1ull << (b1 & 63u); else f0 |= 1ull << (b1 & 63u);
+        if (b2 & 64u) f1 |= 1ull << (b2 & 63u); else f0 |= 1ull << (b2 & 63u);
+      }
+    }
+    if (COUNT) nb += 4ull * (hi - lo);
+    if (!(k & 0x8000u)) {
+      mb = k & 31u;
+      me = (k >> 8) & 31u;
+    } else {
+      const DCls scl = pr.cls()[pr.inv_cls()[pr.type_inv()[stype].begin + (k & 31u)]];
+      if (!(scl.flags & CF_EMPTY) && sid < scl.nsubj) {
+        const unsigned long long ri = scl.rrow_base + static_cast<unsigned long long>(sid) * scl.rstride;
+        mb = __ldg(rrow_ptr + ri);
+        me = __ldg(rrow_ptr + ri + 1);
+        if (COUNT) nb += 8;
+      }
+    }
+  }
+  unsigned long long* const fw = reinterpret_cast<unsigned long long*>(rset + (kRsetCap + kStateWords) * 32);
+  fw[lane] = f0;
+  fw[32 + lane] = f1;
+  const uint32_t cnt = me - mb;
+  uint32_t incl = cnt;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint32_t v = __shfl_up_sync(kFull, incl, d);
+    if (static_cast<int>(lane) >= d) incl += v;
+  }
+  const uint32_t total = __shfl_sync(kFull, incl, 31);
+  const uint32_t dm = mb - (incl - cnt);  // this lane's pair p is its membership p + dm
+  const uint32_t pk = (k & 0xFFFF8000u) | jslot;
+  __syncwarp();
+  unsigned hits = 0;
+  for (uint32_t base = 0; base < total; base += 32) {
+    const uint32_t p = base + lane;
+    int j = 0;  // owner lane of pair p: # lanes with incl <= p
+#pragma unroll
+    for (int step = 16; step >= 1; step >>= 1) {
+      const int probe_lane = j + step - 1;
+      const uint32_t v = __shfl_sync(kFull, incl, probe_lane & 31);
+      if (probe_lane < 32 && v <= p) j += step;
+    }
+    const uint32_t jdm = __shfl_sync(kFull, dm, j), jpk = __shfl_sync(kFull, pk, j);
+    const uint32_t jlo = __shfl_sync(kFull, lo, j), jhi = __shfl_sync(kFull, hi, j);
+    const uint32_t js = jpk & 31u;
+    bool hit = false;
+    if (p < total && !((hits >> js) & 1u)) {
+      const uint32_t r = p + jdm;
+      uint32_t g;
+      if (jpk & 0x8000u) {
+        g = __ldg(rcol + r);
+        if (COUNT) nb += 4;
+      } else {
+        g = rset[r * 32 + js];
+      }
+      const DCls cl = pr.cls()[jpk >> 16];
+      if (g < cl.nsubj) {
+        const unsigned long long ri = cl.rrow_base + static_cast<unsigned long long>(g) * cl.rstride;
+        const uint32_t h = __ldg(rrow_ptr + ri + 1);
+        uint32_t x = __ldg(rrow_ptr + ri);
+        const unsigned long long g0 = fw[j], g1 = fw[32 + j];
+        if (COUNT) nb += 8;
+        for (; x < h && !hit; x += 4) {
+          uint32_t v[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) v[i] = x + i < h ? __ldg(rcol + x + i) : 0u;
+          if (COUNT) nb += 4ull * (h - x < 4u ? h - x : 4u);
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            if (x + i >= h || hit || !l2_maybe(g0, g1, v[i])) continue;
+            uint32_t a = jlo, b = jhi;  // the filter said maybe: is v[i] a child of the range?
+            while (a < b) {
+              const uint32_t mid = a + ((b - a) >> 1), t = __ldg(col + mid);
+              if (COUNT) nb += 4;
+              if (t == v[i]) {
+                hit = true;
+                break;
+              }
+              if (t < v[i]) a = mid + 1; else b = mid;
+            }
+          }
+        }
+      }
+    }
+    hits |= __reduce_or_sync(kFull, hit ? (1u << js) : 0u);
+  }
+  if (COUNT) *bytes += nb;
+  return hits;
+}
+
 // Warp-collective node visit: every lane may carry one (job slot, object, unit).
 // Evaluates the unit's steps at the object: membership-of-itself test, direct and
 // wildcard probes (from the subject's reverse-row set when the job is inverted, else a
-// binary search of the row), and pushes the userset / arrow edge ranges.
-template <bool COUNT>
+// binary search of the row), and pushes the userset / arrow edge ranges. MEET2 = false: the schema has no two-level
+// step, and the two-level meet is left out (its code costs the traversal loop registers: cfg4, DESIGN.md §6).
+template <bool COUNT, bool MEET2>
 __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<COUNT>& c, bool active,
                                       uint32_t jslot, uint32_t obj, uint32_t unit, uint32_t depth) {
   const uint32_t sid = __shfl_sync(kFull, c.my_subj, jslot & 31);
@@ -485,6 +633,9 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
   const uint32_t stype = ss >> 16, srel = ss & 0xFFFFu;
   bool hit = false;
   int sb = 0, nprobe = 0, npush = 0;
+#if ZG_PHASE_CLOCKS
+  long long l1_cycles = 0;  // this lane's time in one-level meets (lanes of a warp run them side by side)
+#endif
   if (active) {
     const DUnit u = pr.units()[unit];
     if (srel != kNone && sid == obj)
@@ -495,7 +646,8 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
       npush = u.step_end - u.push_begin;
     }
   }
-  const bool inverted = (c.inv_mask >> (jslot & 31)) & 1u;
+  // meets: the job may meet in the middle; inverted: its memberships are in the per-check set as well
+  const bool meets = (c.inv_mask >> (jslot & 31)) & 1u, inverted = meets && !((cst >> kOverCap) & 1u);
   // ---- probes (DIRECT / WILD classes): every lane on its own, no warp collective involved. The steps of a unit
   // are ordered probes first (schema.cc); in round 1 every step, probe or not, went through the collective push.
   for (int i = 0; i < nprobe && !hit; ++i) {
@@ -558,6 +710,9 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
               // For each membership key ask ITS reverse row (short, and shared by every range
               // of this check, so it stays in L1): "does this object list the key as a subject
               // of class gc". Two searches are advanced together for memory-level parallelism.
+#if ZG_PHASE_CLOCKS
+              const long long t1 = clock64();
+#endif
               const DCls cl = pr.cls()[st.gc];
               for (uint32_t r = kb; r < ke && !hit; r += 2) {
                 uint32_t l0 = 0, h0 = 0, l1 = 0, h1 = 0;
@@ -579,21 +734,28 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
                 probe2(p.rcol, c, l0, h0, obj, l1, h1, obj, hit0, hit1);
                 hit = hit0 || hit1;
               }
+#if ZG_PHASE_CLOCKS
+              l1_cycles += clock64() - t1;
+#endif
             }
-          } else if ((st.flags & kStepTargetL2) && inverted && depth + 2 <= ZG_MAX_DEPTH) {
+          } else if (MEET2 && (st.flags & kStepTargetL2) && meets && depth + 2 <= ZG_MAX_DEPTH &&
+                     (inverted || (ZG_L2_MODE == 2 && hi - lo <= static_cast<uint32_t>(kFCap)))) {
             // Two levels at once (namespace -> team#member -> group#member -> user): a child t of this
             // range matches iff some membership g of the subject (class tinv) is a subject of t in the
             // children's single class tgc. The reverse row of g in that class lists exactly those t, in
             // ascending order like this range: the answer is "do the two sorted segments intersect",
-            // once per membership. The children are never visited, nothing is pushed.
+            // once per membership. The children are never visited, nothing is pushed. A subject with more
+            // memberships than the per-check set holds meets too (batch_l2 reads them from its reverse row);
+            // with more than kFCap children its range is walked.
             const uint32_t kb = cst_at(cst, st.tinv), ke = stype == st.tstype ? cst_at(cst, st.tinv + 1u) : kb;
             const DCls cl = pr.cls()[st.tgc];
-            if (ZG_L2_MODE == 2 && ke > kb && hi - lo <= static_cast<uint32_t>(kFCap)) {
-              // handed to the whole warp below (coop_l2), one requesting lane at a time
+            if ((ZG_L2_MODE == 2 || ZG_L2_MODE == 3) && hi - lo <= static_cast<uint32_t>(kFCap) &&
+                (inverted ? ke > kb : stype == st.tstype)) {
+              // handed to the whole warp below (batch_l2, or coop_l2 one requesting lane at a time)
               l2_want = true;
               l2_lo = lo;
               l2_hi = hi;
-              l2_k = kb | (ke << 8) | (static_cast<uint32_t>(st.tgc) << 16);
+              l2_k = (inverted ? kb | (ke << 8) : 0x8000u | st.tinv) | (static_cast<uint32_t>(st.tgc) << 16);
             } else
             if (ZG_L2_MODE == 1 && ke > kb && hi - lo <= 256u) {
               // Short range (the common case): a 64-bit Bloom word of its children stays in a register and the
@@ -640,8 +802,23 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
         }
       }
     }
-    if (ZG_L2_MODE == 2) {
+    if (MEET2 && ZG_L2_MODE == 2 && __ballot_sync(kFull, l2_want)) {
+#if ZG_PHASE_CLOCKS
+      const long long t2 = clock64();
+#endif
+      unsigned long long cb = 0;
+      c.found |= batch_l2<COUNT>(p.col, p.rrow_ptr, p.rcol, c.rset, c.lane, l2_want && !((c.found >> jslot) & 1u), l2_lo,
+                                 l2_hi, l2_k, jslot & 31u, sid, stype, COUNT ? &cb : nullptr);
+      if (COUNT) c.bytes += cb;
+#if ZG_PHASE_CLOCKS
+      c.ph[2] += clock64() - t2;
+#endif
+    }
+    if (MEET2 && ZG_L2_MODE == 3) {
       unsigned l2m = __ballot_sync(kFull, l2_want);
+#if ZG_PHASE_CLOCKS
+      const long long t2 = clock64();
+#endif
       while (l2m) {  // warp-uniform: one requesting lane after the other, the whole warp on its range
         const int r = __ffs(l2m) - 1;
         l2m &= l2m - 1;
@@ -656,10 +833,17 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
         if (h) c.found |= 1u << rj;
         __syncwarp();
       }
+#if ZG_PHASE_CLOCKS
+      c.ph[2] += clock64() - t2;
+#endif
     }
     push(c, want, item);
   }
   c.found |= __reduce_or_sync(kFull, hit ? (1u << jslot) : 0u);
+#if ZG_PHASE_CLOCKS
+  for (int d = 16; d >= 1; d >>= 1) l1_cycles = max(l1_cycles, __shfl_xor_sync(kFull, l1_cycles, d));
+  c.ph[3] += l1_cycles;
+#endif
 }
 
 __device__ __forceinline__ uint32_t kleene_or(uint32_t a, uint32_t b) {  // 0 F, 1 T, 2 E
@@ -719,7 +903,7 @@ __device__ __noinline__ void wait_ready(const unsigned long long* ready, unsigne
 // Per-lane query state parked in shared memory while the warp traverses (kStateWords words):
 //   0 resource object, 1 depth | leaves << 8 | is-tree << 15 | leaf_begin-or-unit << 16,
 //   2 tree id, 3 / 4 leaf values (2 bits each), 5 presence word of the reverse-row set
-template <bool COUNT, bool STREAMED = false>
+template <bool COUNT, bool STREAMED = false, bool MEET2 = true>
 __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KParams p) {
   ZG_DYNAMIC_SMEM(smem);
   for (uint32_t i = threadIdx.x; i < p.prog_bytes / 16; i += blockDim.x)
@@ -739,6 +923,9 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
   c.events = p.events;
   const uint32_t n_slots = pr.hdr()->n_slots, n_types = pr.hdr()->n_types;
   unsigned long long* const memo = p.memo + (static_cast<size_t>(blockIdx.x) * kWarpsPerBlock + warp) * p.memo_entries;
+#if ZG_PHASE_CLOCKS
+  for (int i = 0; i < kPhases; ++i) c.ph[i] = 0;
+#endif
 
   for (;;) {
     unsigned long long base = 0;
@@ -749,6 +936,9 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
     }
     base = __shfl_sync(kFull, base, 0);
     if (base >= p.nq) break;
+#if ZG_PHASE_CLOCKS
+    const long long t_adm = clock64();
+#endif
     const unsigned long long q = base + lane;
     const bool valid = q < p.nq;
     bool bad = false, expansive = false;
@@ -805,6 +995,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
           ncl = 0;
         }
       }
+      const bool meet = inv;  // stays when the memberships overflow the set: the two-level meet reads them itself
       const int maxcl = __reduce_max_sync(kFull, ncl);
       for (int i = 0; i < maxcl; ++i) {
         if (inv && i < ncl) {
@@ -830,11 +1021,15 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
           cst |= static_cast<unsigned long long>(rcnt) << (5u * (i + 1));
         }
       }
-      c.inv_mask = __ballot_sync(kFull, inv);
+      if (meet && !inv && ZG_L2_MODE == 2) cst |= 1ull << kOverCap;
+      c.inv_mask = __ballot_sync(kFull, ZG_L2_MODE == 2 ? meet : inv);
       c.my_cst = cst;
       state[160] = present;
       __syncwarp();
     }
+#if ZG_PHASE_CLOCKS
+    c.ph[0] += clock64() - t_adm;
+#endif
     c.fatal = false;
     bool undet = valid && !bad;
     uint32_t res = 2;  // invalid query -> error
@@ -856,7 +1051,18 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
       c.top = 0;
       c.spill_top = 0;
 
-      visit(p, pr, c, act, lane, obj, unit, depth);
+#if ZG_PHASE_CLOCKS
+      long long t_ph = clock64(), meets = c.ph[2] + c.ph[3];  // root visit and pop loop exclude the meets inside them
+#endif
+      visit<COUNT, MEET2>(p, pr, c, act, lane, obj, unit, depth);
+#if ZG_PHASE_CLOCKS
+      {
+        const long long now = clock64(), m = c.ph[2] + c.ph[3];
+        c.ph[1] += (now - t_ph) - (m - meets);
+        t_ph = now;
+        meets = m;
+      }
+#endif
 
       uint32_t iters = 0;
       bool use_memo = false;
@@ -985,8 +1191,11 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
           }
         }
         c.raised |= __reduce_or_sync(kFull, raise ? (1u << jslot) : 0u);
-        visit(p, pr, c, active, jslot, child, cunit, cdepth);
+        visit<COUNT, MEET2>(p, pr, c, active, jslot, child, cunit, cdepth);
       }
+#if ZG_PHASE_CLOCKS
+      c.ph[4] += (clock64() - t_ph) - (c.ph[2] + c.ph[3] - meets);
+#endif
 
       if (act) {
         const bool t = (c.found >> lane) & 1u, e = (c.err >> lane) & 1u, r = (c.raised >> lane) & 1u;
@@ -1020,6 +1229,10 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
     for (int d = 16; d >= 1; d >>= 1) b += __shfl_xor_sync(kFull, b, d);
     if (lane == 0 && b) atomicAdd(p.alg_bytes, b);
   }
+#if ZG_PHASE_CLOCKS
+  if (lane == 0)
+    for (int i = 0; i < kPhases; ++i) atomicAdd(p.events + 3 + i, static_cast<unsigned long long>(c.ph[i]));
+#endif
 }
 
 // ---- multi-pass runs: the boolean fold of a level whose queries raised sub-queries -------------
