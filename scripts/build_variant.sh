@@ -1,5 +1,5 @@
 #!/bin/bash
-# Builds an alternative libzgpu (tuning experiments): scripts/build_variant.sh NAME "-DZG_L2_BLOOM=0 ..."
+# Builds an alternative libzgpu (tuning experiments): scripts/build_variant.sh NAME "-DZG_PHASE_CLOCKS=1 ..."
 # -> spicedb-kubeapi-proxy_b200/variants/libzgpu_NAME.so ; select it with ZGPU_LIB=<path>.
 set -e
 name=$1; flags=$2

@@ -28,8 +28,7 @@ namespace zg {
 #define ZG_STR2(x) #x
 #define ZG_STR(x) ZG_STR2(x)
 const char* build_info() {
-  return "libzgpu sm_90a built " __DATE__ " " __TIME__ " L2_MODE=" ZG_STR(ZG_L2_MODE) " PRESENCE=" ZG_STR(ZG_PRESENCE) " POP_FAST=" ZG_STR(ZG_POP_FAST) " L2_MATCH=" ZG_STR(ZG_L2_MATCH) " L2_FILTER=" ZG_STR(ZG_L2_FILTER) " L2_SPLIT=" ZG_STR(ZG_L2_SPLIT)
-         " STACK_CAP=" ZG_STR(ZG_STACK_CAP) " RSET_CAP=" ZG_STR(ZG_RSET_CAP) " MIN_BLOCKS=" ZG_STR(ZG_MIN_BLOCKS);
+  return "libzgpu sm_90a built " __DATE__ " " __TIME__ " STACK_CAP=" ZG_STR(ZG_STACK_CAP) " RSET_CAP=" ZG_STR(ZG_RSET_CAP) " MIN_BLOCKS=" ZG_STR(ZG_MIN_BLOCKS);
 }
 
 bool DevBuf::ensure(size_t bytes) {
@@ -135,7 +134,6 @@ std::string Device::init(int dev, uint64_t subq_cap, uint32_t budget) {
   if ((e = cudaStreamCreateWithFlags(&cstream_, cudaStreamNonBlocking)) != cudaSuccess)
     return std::string("cudaStreamCreate: ") + cudaGetErrorString(e);
   cudaEventCreateWithFlags(&ev_reset_, cudaEventDisableTiming);
-  if (const char* v = std::getenv("ZGPU_NO_STREAM_H2D")) stream_h2d = !(*v && *v != '0');
   if (subq_cap) subq_cap_ = subq_cap;
   if (budget) budget_ = budget;
   if (!ctrl_.ensure(128)) return "out of device memory";
@@ -624,7 +622,7 @@ int Device::check_host_multi(const std::vector<HostReq>& reqs, std::string* err)
     pin_out_cap_ = total;
   }
   unsigned long long* d_ready = ctrl_.as<unsigned long long>() + 10;
-  const bool streamed = stream_h2d && total >= kStreamMinItems;
+  const bool streamed = total >= kStreamMinItems;
   const unsigned long long* ready_arg = nullptr;
   // A large group of many callers (1 000 lists of 10 000 items under BASELINE config 5): one thread gathering 16 B per
   // item into the staging area takes longer than the kernel that answers them. Helpers copy contiguous shares.

@@ -135,7 +135,6 @@ class Device {
   uint64_t launches = 0, passes = 0, checks = 0;
   uint64_t coalesced_launches = 0, coalesced_requests = 0;
   uint64_t streamed_calls = 0;  // host calls whose items were streamed in behind the running kernel
-  bool stream_h2d = true;       // ZGPU_NO_STREAM_H2D=1: one copy, then the kernel (A/B measurement)
   uint64_t split_batches = 0;  // batches answered in halves because their sub-queries overflowed the pass buffer
   // cumulative device-side event counters: stack spills to HBM, batches that switched the path memo on
   void read_events(uint64_t* spills, uint64_t* memo_batches);

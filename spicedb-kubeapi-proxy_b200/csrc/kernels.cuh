@@ -47,33 +47,8 @@ constexpr int kThreads = kWarpsPerBlock * 32;
 #ifndef ZG_RSET_CAP
 #define ZG_RSET_CAP 16
 #endif
-// The switches below were A/B-measured on the GPU this project targeted before the H100, not on the H100; only
-// ZG_MIN_BLOCKS was measured again there (4 beat 3 and 5 on cfg3 and cfg4, DESIGN.md §6).
-#ifndef ZG_PRESENCE
-#define ZG_PRESENCE 0  // presence word in front of the per-check set walk of a direct inverted probe (measured slower:
-                       // the walk is short and the extra shared-memory word costs more than it saves)
-#endif
-#ifndef ZG_POP_FAST
-#define ZG_POP_FAST 0  // pop: when every popped range holds <= 1 edge, skip the prefix scan / owner search (measured: no gain)
-#endif
-#ifndef ZG_L2_MATCH
-#define ZG_L2_MATCH 0  // cooperative two-level meet: match.any instead of a search for ranges of <= 16 children.
-                       // Measured much SLOWER on cfg3 (previous target GPU): MATCH.ANY was a slow path there
-#endif
-#ifndef ZG_L2_FILTER
-#define ZG_L2_FILTER 1  // cooperative two-level meet: a 2 048-bit blocked Bloom filter of the range's children in shared memory
-                        // in front of the binary search (the search then runs only when the filter lets an element through).
-                        // Measured faster on cfg3, more so together with ZG_L2_SPLIT; cfg4 unchanged
-#endif
-#ifndef ZG_L2_SPLIT
-#define ZG_L2_SPLIT 1  // cooperative two-level meet: 32 / ng lanes per membership row (any ng) instead of a power of two
-                       // (measured alone: slightly faster on cfg3)
-#endif
-#ifndef ZG_L2_MODE
-#define ZG_L2_MODE 2  // two-level meet: 2 = every requesting lane of a visit at once (batch_l2, default), 3 = one requesting
-                      // lane after the other with the whole warp on its range (coop_l2), 1 = per-lane Bloom word +
-                      // 128-bit streaming (measured slower on cfg3), 0 = per-lane sorted-segment intersection
-#endif
+// Build-time tuning knobs (scripts/build_variant.sh). ZG_MIN_BLOCKS was A/B-measured on the H100: 4 beat 3 and 5 on
+// cfg3 and cfg4 (DESIGN.md §6). ZG_PHASE_CLOCKS is an instrument, off in the library.
 #ifndef ZG_PHASE_CLOCKS
 #define ZG_PHASE_CLOCKS 0  // 1: every warp adds clock64() cycles per phase of a batch into KParams::events[3 .. 7]
                            // (admission, root visit, two-level meet, one-level meet, pop loop; zg_phase_clocks)
@@ -82,11 +57,10 @@ constexpr int kPhases = 5;
 constexpr int kMinBlocks = ZG_MIN_BLOCKS;  // resident CTAs per SM the register budget is tuned for
 constexpr int kStackCap = ZG_STACK_CAP;    // range items per warp in shared memory
 constexpr int kRsetCap = ZG_RSET_CAP;      // reverse-row entries kept per check (subject's direct memberships), <= 31
-constexpr int kStateWords = 6;             // per-lane query state parked in shared memory between leaf passes
-constexpr int kFCap = 64;                  // children of a range staged in shared memory by the two-level meet
-constexpr int kFBloom = ZG_L2_FILTER ? 64 : 0;  // words of the filter over those children
-constexpr size_t kWarpSmem = kStackCap * sizeof(uint4) + ((kRsetCap + kStateWords) * 32 + kFCap + kFBloom) * sizeof(uint32_t);
-static_assert(ZG_L2_MODE != 2 || kFCap + kFBloom >= 128, "batch_l2 keeps a 128-bit filter per lane in the meet's area");
+constexpr int kStateWords = 5;             // per-lane query state parked in shared memory between leaf passes
+constexpr int kMeetWords = 128;            // batch_l2's 128-bit filter of each lane's range (two 64-bit words per lane)
+constexpr int kFCap = 64;                  // the largest range (children) the two-level meet answers
+constexpr size_t kWarpSmem = kStackCap * sizeof(uint4) + ((kRsetCap + kStateWords) * 32 + kMeetWords) * sizeof(uint32_t);
 constexpr unsigned kFull = 0xFFFFFFFFu;
 constexpr uint16_t kJobDepthMask = 0x00FF;  // zg_check.flags of a raised sub-query: hop depth
 
@@ -344,146 +318,7 @@ __device__ __forceinline__ uint32_t cst_at(unsigned long long cst, uint32_t i) {
   return static_cast<uint32_t>(cst >> (5u * i)) & 31u;
 }
 constexpr int kMaxInvClasses = 11;
-// bit of (invertible class index, object) in a check's 32-bit presence word
-__device__ __forceinline__ uint32_t rset_bit(uint32_t tinv, uint32_t obj) {
-  return ((obj + tinv * 0x632BE5ABu) * 0x9E3779B1u) >> 27;
-}
 static_assert(kRsetCap <= 31, "class boundaries are 5-bit fields");
-
-// Two-level meet, warp-cooperative: ONE check's range against the reverse rows of its subject's memberships, all 32
-// lanes working on it. The per-lane form of this (every lane walking its own check's rows) ran with 9 of 32 lanes
-// active on average: row counts and early exits differ per check. Here the range's children F
-// (<= kFCap, ascending) go to shared memory with one coalesced load, every membership row gets a fixed group of lanes
-// (neighbouring lanes read neighbouring words of the row), and each lane tests its element against a Bloom filter of F;
-// F itself is binary-searched (warp-uniform trip count) only for what the filter lets through. Returns (warp-uniform) whether some element of some row is a child of the range.
-// Deliberately NOT inlined: inlined, its registers take part in the allocation of the whole traversal loop and cost
-// schemas that never use it (measured on cfg4, previous target GPU); a hash table of the range instead of the binary search was slower
-// still (cfg3).
-// (all arguments by value: a reference to the warp context would force it into local memory)
-template <bool COUNT>
-__device__ __noinline__ bool coop_l2(const uint32_t* __restrict__ col, const uint32_t* __restrict__ rrow_ptr,
-                                     const uint32_t* __restrict__ rcol, uint32_t* rset, uint32_t lane, uint32_t lo, uint32_t hi,
-                                     uint32_t kb, uint32_t ke, uint32_t jslot, unsigned long long rrow_base, uint32_t rstride,
-                                     uint32_t nsubj, unsigned long long* bytes) {
-  uint32_t* const fs = rset + (kRsetCap + kStateWords) * 32;
-  const uint32_t nf = hi - lo, ng = ke - kb;  // nf <= kFCap (64), 1 <= ng <= kRsetCap (16)
-#if ZG_L2_MATCH
-  if (nf <= 16u) {
-    // Short range (the common case): its children sit in lanes 0-15, sixteen row elements at a time in lanes 16-31,
-    // and ONE match.any tells every element lane whether an F lane holds the same value: no search at all.
-    // Unused lanes hold values no object id can take (ids stay below 0xFFFFFFF0), all different.
-    const uint32_t pad = 0xFFFFFFE0u + lane;
-    const uint32_t fval = lane < nf ? __ldg(col + lo + lane) : pad;
-    const uint32_t el = lane - 16u;  // element lane index (lanes 16-31)
-    const uint32_t sh = ng <= 1 ? 4u : (ng <= 2 ? 3u : (ng <= 4 ? 2u : (ng <= 8 ? 1u : 0u)));  // log2(lanes per row)
-    const uint32_t w = 1u << sh, row = el >> sh, k = el & (w - 1u);
-    uint32_t x = 0, h = 0;
-    if (lane >= 16u && row < ng) {
-      const uint32_t g = rset[(kb + row) * 32 + jslot];
-      if (g < nsubj) {
-        const unsigned long long ri = rrow_base + static_cast<unsigned long long>(g) * rstride;
-        x = __ldg(rrow_ptr + ri) + k;
-        h = __ldg(rrow_ptr + ri + 1);
-        if (COUNT && k == 0) *bytes += 8ull + 4ull * (h - (x - k));
-      }
-    }
-    if (COUNT && lane == 0) *bytes += 4ull * nf;
-    while (__any_sync(kFull, x < h)) {
-      uint32_t v = fval;
-      if (lane >= 16u) {
-        v = pad;
-        if (x < h) {
-          v = __ldg(rcol + x);
-          x += w;
-        }
-      }
-      const unsigned same = __match_any_sync(kFull, v);
-      if (__any_sync(kFull, lane >= 16u && (same & 0xFFFFu))) return true;
-    }
-    return false;
-  }
-#endif
-#if ZG_L2_FILTER
-  // filter word = top 6 bits of the hash, two bits inside it from the next 2 x 5 bits
-  uint32_t* const fb = fs + kFCap;
-  fb[lane] = 0;
-  fb[lane + 32] = 0;
-  __syncwarp();
-  if (lane < nf) {
-    const uint32_t v = __ldg(col + lo + lane), hv = v * 0x9E3779B1u;
-    fs[lane] = v;
-    atomicOr(&fb[hv >> 26], (1u << ((hv >> 21) & 31u)) | (1u << ((hv >> 16) & 31u)));
-  }
-  if (lane + 32 < nf) {
-    const uint32_t v = __ldg(col + lo + lane + 32), hv = v * 0x9E3779B1u;
-    fs[lane + 32] = v;
-    atomicOr(&fb[hv >> 26], (1u << ((hv >> 21) & 31u)) | (1u << ((hv >> 16) & 31u)));
-  }
-#else
-  if (lane < nf) fs[lane] = __ldg(col + lo + lane);
-  if (lane + 32 < nf) fs[lane + 32] = __ldg(col + lo + lane + 32);
-#endif
-  // W lanes per membership row: lane = row * W + k walks elements k, k + W, ... of its row. No prefix sums, no owner
-  // search: the lanes of a row read the same two offsets (one broadcast load).
-#if ZG_L2_SPLIT
-  uint32_t w, magic;  // W = 32 / ng; row = lane / W as (lane * ceil(256 / W)) >> 8, exact for lane < 32
-  if (ng <= 2) { w = 16; magic = 16; }
-  else if (ng == 3) { w = 10; magic = 26; }
-  else if (ng == 4) { w = 8; magic = 32; }
-  else if (ng == 5) { w = 6; magic = 43; }
-  else if (ng == 6) { w = 5; magic = 52; }
-  else if (ng <= 8) { w = 4; magic = 64; }
-  else if (ng <= 10) { w = 3; magic = 86; }
-  else { w = 2; magic = 128; }
-  const uint32_t row = (lane * magic) >> 8, k = lane - row * w;
-#else
-  const uint32_t sh = ng <= 2 ? 4u : (ng <= 4 ? 3u : (ng <= 8 ? 2u : 1u));  // log2(W): 32 / next power of two of ng
-  const uint32_t w = 1u << sh, row = lane >> sh, k = lane & (w - 1u);
-#endif
-  uint32_t x = 0, h = 0;
-  if (row < ng) {
-    const uint32_t g = rset[(kb + row) * 32 + jslot];
-    if (g < nsubj) {
-      const unsigned long long ri = rrow_base + static_cast<unsigned long long>(g) * rstride;
-      x = __ldg(rrow_ptr + ri) + k;
-      h = __ldg(rrow_ptr + ri + 1);
-      if (COUNT && k == 0) *bytes += 8ull + 4ull * (h - (x - k));
-    }
-  }
-  if (COUNT && lane == 0) *bytes += 4ull * nf;
-  __syncwarp();
-  const uint32_t span = nf > 1 ? 1u << (32 - __clz(nf - 1)) : 1u;  // smallest power of two >= nf
-  while (__any_sync(kFull, x < h)) {
-    bool found = false;
-#if ZG_L2_FILTER
-    uint32_t t = 0;
-    if (x < h) {
-      t = __ldg(rcol + x);
-      const uint32_t ht = t * 0x9E3779B1u, m = (1u << ((ht >> 21) & 31u)) | (1u << ((ht >> 16) & 31u));
-      found = (fb[ht >> 26] & m) == m;  // "maybe": verified below
-      x += w;
-    }
-    if (__any_sync(kFull, found)) {
-      uint32_t pos = 0;  // lower bound of t in fs[0, nf): warp-uniform trip count
-      for (uint32_t s = span; s >= 1; s >>= 1)
-        if (pos + s <= nf && fs[pos + s - 1] < t) pos += s;
-      found = found && pos < nf && fs[pos] == t;
-      if (__any_sync(kFull, found)) return true;
-    }
-#else
-    if (x < h) {
-      const uint32_t t = __ldg(rcol + x);
-      uint32_t pos = 0;  // lower bound of t in fs[0, nf): warp-uniform trip count
-      for (uint32_t s = span; s >= 1; s >>= 1)
-        if (pos + s <= nf && fs[pos + s - 1] < t) pos += s;
-      found = pos < nf && fs[pos] == t;
-      x += w;
-    }
-    if (__any_sync(kFull, found)) return true;
-#endif
-  }
-  return false;
-}
 
 // Filter of batch_l2: two bits per object id in 128 (two 64-bit words). False-positive rate (1 - e^(-2n/128))^2 over
 // a range of n children: 2 % at n = 10 (cfg3's mean), 12 % at n = 27 (its largest); only the search behind it answers.
@@ -498,17 +333,17 @@ __device__ __forceinline__ bool l2_maybe(unsigned long long f0, unsigned long lo
   return ((((b1 & 64u) ? f1 : f0) >> (b1 & 63u)) & (((b2 & 64u) ? f1 : f0) >> (b2 & 63u)) & 1ull) != 0;
 }
 
-// Two-level meet, batched: every requesting lane of a visit round at once (coop_l2 serves them one after the other).
-// Lane j wants "does some membership g of its subject (class tinv) list a child of its range col[lo, hi) in class
-// tgc". Its memberships are rset entries [kb, ke) of its job, or -- for a subject with more memberships than the set
+// Two-level meet, batched: every requesting lane of a visit round is served at once (per-lane meets ran with few of
+// the 32 lanes active: row counts and early exits differ per check). Lane j wants "does some membership g of its
+// subject (class tinv) list a child of its range col[lo, hi) in class tgc". Its memberships are rset entries [kb, ke) of its job, or -- for a subject with more memberships than the set
 // holds -- the subject's own reverse row of class tinv. The (lane, membership) pairs of the whole warp are numbered
 // with one scan and dealt out 32 at a time: every lane reads one pair's reverse row (all 32 rows in flight together)
 // and tests its elements against the owner's 128-bit filter of the range; a "maybe" is verified by a binary search of
 // the range, which lane j has just read. Pairs of a check that is already answered are skipped.
 // k packs ke << 8 | kb (set entries) or 0x8000 | tinv (reverse row), and tgc << 16. Requesting lanes are those of
 // checks not answered yet. Returns the job slots answered.
-// Ranges are <= kFCap children (the caller keeps larger ones). Inlined: out of line (as coop_l2 is) the call site
-// spilled more of the traversal loop's registers (ptxas) and ran no faster on cfg3 (H100, DESIGN.md §6).
+// Ranges are <= kFCap children (the caller keeps larger ones). Inlined: out of line, the call site spilled more of
+// the traversal loop's registers (ptxas) and ran no faster on cfg3 (H100, DESIGN.md §6).
 template <bool COUNT>
 __device__ __forceinline__ unsigned batch_l2(const uint32_t* __restrict__ col, const uint32_t* __restrict__ rrow_ptr,
                                           const uint32_t* __restrict__ rcol, uint32_t* rset, uint32_t lane, bool want,
@@ -547,7 +382,7 @@ __device__ __forceinline__ unsigned batch_l2(const uint32_t* __restrict__ col, c
       }
     }
   }
-  unsigned long long* const fw = reinterpret_cast<unsigned long long*>(rset + (kRsetCap + kStateWords) * 32);
+  unsigned long long* const fw = reinterpret_cast<unsigned long long*>(rset + (kRsetCap + kStateWords) * 32);  // kMeetWords
   fw[lane] = f0;
   fw[32 + lane] = f1;
   const uint32_t cnt = me - mb;
@@ -656,15 +491,10 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
     const bool subject_fits = srel == kNone && stype == st.stype;
     if (!subject_fits || (st.kind == ST_WILD && p.no_wildcards)) continue;
     if (st.kind == ST_DIRECT && inverted && (st.flags & CF_INVERT)) {
-      // direction-optimised probe: is obj among the subject's memberships of this class? Most probes miss: a
-      // 32-bit presence word over (class, object) of the check's set (built at admission) rejects them
-      // without walking the set.
-      const uint32_t present = c.rset[(kRsetCap + 5) * 32 + (jslot & 31)];
-      if (!ZG_PRESENCE || ((present >> rset_bit(st.tinv, obj)) & 1u)) {
-        const uint32_t kb = cst_at(cst, st.tinv), ke = cst_at(cst, st.tinv + 1u);
-        for (uint32_t r = kb; r < ke; ++r)
-          hit = hit || c.rset[r * 32 + (jslot & 31)] == obj;
-      }
+      // direction-optimised probe: is obj among the subject's memberships of this class?
+      const uint32_t kb = cst_at(cst, st.tinv), ke = cst_at(cst, st.tinv + 1u);
+      for (uint32_t r = kb; r < ke; ++r)
+        hit = hit || c.rset[r * 32 + (jslot & 31)] == obj;
     } else if (obj < st.nres) {
       const unsigned long long ridx = st.row_base + static_cast<unsigned long long>(obj) * st.ncls;
       const uint32_t lo = __ldg(p.row_ptr + ridx), hi = __ldg(p.row_ptr + ridx + 1);
@@ -739,7 +569,7 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
 #endif
             }
           } else if (MEET2 && (st.flags & kStepTargetL2) && meets && depth + 2 <= ZG_MAX_DEPTH &&
-                     (inverted || (ZG_L2_MODE == 2 && hi - lo <= static_cast<uint32_t>(kFCap)))) {
+                     (inverted || hi - lo <= static_cast<uint32_t>(kFCap))) {
             // Two levels at once (namespace -> team#member -> group#member -> user): a child t of this
             // range matches iff some membership g of the subject (class tinv) is a subject of t in the
             // children's single class tgc. The reverse row of g in that class lists exactly those t, in
@@ -748,44 +578,16 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
             // memberships than the per-check set holds meets too (batch_l2 reads them from its reverse row);
             // with more than kFCap children its range is walked.
             const uint32_t kb = cst_at(cst, st.tinv), ke = stype == st.tstype ? cst_at(cst, st.tinv + 1u) : kb;
-            const DCls cl = pr.cls()[st.tgc];
-            if ((ZG_L2_MODE == 2 || ZG_L2_MODE == 3) && hi - lo <= static_cast<uint32_t>(kFCap) &&
-                (inverted ? ke > kb : stype == st.tstype)) {
-              // handed to the whole warp below (batch_l2, or coop_l2 one requesting lane at a time)
+            if (hi - lo <= static_cast<uint32_t>(kFCap) && (inverted ? ke > kb : stype == st.tstype)) {
+              // handed to the whole warp below (batch_l2)
               l2_want = true;
               l2_lo = lo;
               l2_hi = hi;
               l2_k = (inverted ? kb | (ke << 8) : 0x8000u | st.tinv) | (static_cast<uint32_t>(st.tgc) << 16);
-            } else
-            if (ZG_L2_MODE == 1 && ke > kb && hi - lo <= 256u) {
-              // Short range (the common case): a 64-bit Bloom word of its children stays in a register and the
-              // reverse rows are STREAMED against it with 128-bit loads -- independent loads, no dependent
-              // chain per element; only a Bloom hit is verified by a binary search of the range.
-              unsigned long long bloom = 0;
-              for (uint32_t x = lo & ~3u; x < hi; x += 4) {
-                const uint4 v = __ldg(reinterpret_cast<const uint4*>(p.col + x));
-                if (x >= lo) bloom |= 1ull << ((v.x * 0x9E3779B1u) >> 26);
-                if (x + 1 >= lo && x + 1 < hi) bloom |= 1ull << ((v.y * 0x9E3779B1u) >> 26);
-                if (x + 2 >= lo && x + 2 < hi) bloom |= 1ull << ((v.z * 0x9E3779B1u) >> 26);
-                if (x + 3 >= lo && x + 3 < hi) bloom |= 1ull << ((v.w * 0x9E3779B1u) >> 26);
-              }
-              if (COUNT) c.bytes += 4ull * (hi - lo);  // the words of the range (the padding of a 128-bit load is not work)
-              for (uint32_t r = kb; r < ke && !hit; ++r) {
-                const uint32_t g = c.rset[r * 32 + (jslot & 31)];
-                if (g >= cl.nsubj) continue;
-                const unsigned long long ri = cl.rrow_base + static_cast<unsigned long long>(g) * cl.rstride;
-                const uint32_t l = __ldg(p.rrow_ptr + ri), h = __ldg(p.rrow_ptr + ri + 1);
-                if (COUNT) c.bytes += 8 + 4ull * (h - l);
-                for (uint32_t x = l & ~3u; x < h && !hit; x += 4) {
-                  const uint4 v = __ldg(reinterpret_cast<const uint4*>(p.rcol + x));
-                  const uint32_t e4[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-                  for (int k = 0; k < 4; ++k)
-                    if (x + k >= l && x + k < h && ((bloom >> ((e4[k] * 0x9E3779B1u) >> 26)) & 1ull))
-                      hit = hit || find_in(p.col, c, lo, hi, e4[k]);
-                }
-              }
             } else {
+              // An inverted check whose range has more than kFCap children: this lane intersects the range with
+              // each membership's reverse row on its own.
+              const DCls cl = pr.cls()[st.tgc];
               for (uint32_t r = kb; r < ke && !hit; ++r) {
                 const uint32_t g = c.rset[r * 32 + (jslot & 31)];
                 if (g >= cl.nsubj) continue;
@@ -802,7 +604,7 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
         }
       }
     }
-    if (MEET2 && ZG_L2_MODE == 2 && __ballot_sync(kFull, l2_want)) {
+    if (MEET2 && __ballot_sync(kFull, l2_want)) {
 #if ZG_PHASE_CLOCKS
       const long long t2 = clock64();
 #endif
@@ -810,29 +612,6 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
       c.found |= batch_l2<COUNT>(p.col, p.rrow_ptr, p.rcol, c.rset, c.lane, l2_want && !((c.found >> jslot) & 1u), l2_lo,
                                  l2_hi, l2_k, jslot & 31u, sid, stype, COUNT ? &cb : nullptr);
       if (COUNT) c.bytes += cb;
-#if ZG_PHASE_CLOCKS
-      c.ph[2] += clock64() - t2;
-#endif
-    }
-    if (MEET2 && ZG_L2_MODE == 3) {
-      unsigned l2m = __ballot_sync(kFull, l2_want);
-#if ZG_PHASE_CLOCKS
-      const long long t2 = clock64();
-#endif
-      while (l2m) {  // warp-uniform: one requesting lane after the other, the whole warp on its range
-        const int r = __ffs(l2m) - 1;
-        l2m &= l2m - 1;
-        const uint32_t rlo = __shfl_sync(kFull, l2_lo, r), rhi = __shfl_sync(kFull, l2_hi, r), rk = __shfl_sync(kFull, l2_k, r);
-        const uint32_t rj = __shfl_sync(kFull, jslot, r) & 31u;
-        if ((c.found >> rj) & 1u) continue;  // another node of the same check already answered it
-        const DCls rcl = pr.cls()[rk >> 16];
-        unsigned long long cb = 0;
-        const bool h = coop_l2<COUNT>(p.col, p.rrow_ptr, p.rcol, c.rset, c.lane, rlo, rhi, rk & 0xFFu, (rk >> 8) & 0xFFu, rj,
-                                      rcl.rrow_base, rcl.rstride, rcl.nsubj, &cb);
-        if (COUNT) c.bytes += cb;
-        if (h) c.found |= 1u << rj;
-        __syncwarp();
-      }
 #if ZG_PHASE_CLOCKS
       c.ph[2] += clock64() - t2;
 #endif
@@ -902,7 +681,7 @@ __device__ __noinline__ void wait_ready(const unsigned long long* ready, unsigne
 
 // Per-lane query state parked in shared memory while the warp traverses (kStateWords words):
 //   0 resource object, 1 depth | leaves << 8 | is-tree << 15 | leaf_begin-or-unit << 16,
-//   2 tree id, 3 / 4 leaf values (2 bits each), 5 presence word of the reverse-row set
+//   2 tree id, 3 / 4 leaf values (2 bits each)
 template <bool COUNT, bool STREAMED = false, bool MEET2 = true>
 __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KParams p) {
   ZG_DYNAMIC_SMEM(smem);
@@ -983,7 +762,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
     // query: every leaf of a non-pure permission shares them.
     {
       bool inv = p.invert && valid && !bad && (c.my_ss & 0xFFFFu) == kNone && expansive;
-      uint32_t rcnt = 0, present = 0;
+      uint32_t rcnt = 0;
       unsigned long long cst = 0;
       int ib = 0, ncl = 0;
       if (inv) {
@@ -1010,9 +789,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
               inv = false;  // too many memberships: this check probes forward
             } else {
               for (uint32_t x = b; x < e; ++x) {
-                const uint32_t m = __ldg(p.rcol + x);
-                c.rset[rcnt * 32 + lane] = m;
-                present |= 1u << rset_bit(static_cast<uint32_t>(i), m);
+                c.rset[rcnt * 32 + lane] = __ldg(p.rcol + x);
                 ++rcnt;
               }
               if (COUNT) c.bytes += 4ull * (e - b);
@@ -1021,10 +798,9 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
           cst |= static_cast<unsigned long long>(rcnt) << (5u * (i + 1));
         }
       }
-      if (meet && !inv && ZG_L2_MODE == 2) cst |= 1ull << kOverCap;
-      c.inv_mask = __ballot_sync(kFull, ZG_L2_MODE == 2 ? meet : inv);
+      if (meet && !inv) cst |= 1ull << kOverCap;
+      c.inv_mask = __ballot_sync(kFull, meet);
       c.my_cst = cst;
-      state[160] = present;
       __syncwarp();
     }
 #if ZG_PHASE_CLOCKS
@@ -1091,48 +867,33 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
         if (static_cast<int>(lane) < n) it = c.stack[c.top - 1 - lane];
         const bool dead = (c.found >> (it.z & 31)) & 1u;
         const uint32_t len = (static_cast<int>(lane) < n && !dead) ? it.y - it.x : 0u;
-        uint32_t total, jb, jmeta, jexcl;
-        if (ZG_POP_FAST && !__ballot_sync(kFull, len > 1u)) {
-          // Every popped range holds at most one edge (arrows to a single parent, singleton usersets: the common
-          // case on document / folder hierarchies): no prefix scan and no owner search -- lane k takes the k-th
-          // live item, found with one ballot and one find-nth-set.
-          const unsigned ones = __ballot_sync(kFull, len == 1u);
-          total = static_cast<uint32_t>(__popc(ones));
-          c.top -= n;
-          const int j = lane < total ? static_cast<int>(__fns(ones, 0, static_cast<int>(lane) + 1)) : 0;
-          jb = __shfl_sync(kFull, it.x, j & 31);
-          jmeta = __shfl_sync(kFull, it.z, j & 31);
-          jexcl = lane;
-          __syncwarp();
-        } else {
-          uint32_t incl = len;
+        uint32_t incl = len;
 #pragma unroll
-          for (int d = 1; d < 32; d <<= 1) {
-            uint32_t v = __shfl_up_sync(kFull, incl, d);
-            if (static_cast<int>(lane) >= d) incl += v;
-          }
-          const uint32_t excl = incl - len;
-          const unsigned fullm = __ballot_sync(kFull, static_cast<int>(lane) < n && incl <= 32u);
-          const int nfull = __popc(fullm);  // prefix of fully consumed items
-          total = __shfl_sync(kFull, incl, 31);
-          if (total > 32u) total = 32u;
-          __syncwarp();
-          if (static_cast<int>(lane) == nfull && static_cast<int>(lane) < n)  // partially consumed item stays on top
-            c.stack[c.top - 1 - lane].x = it.x + (32u - excl);
-          c.top -= nfull;
-          __syncwarp();
-          // ---- lane k takes edge k: owner item j = #items with incl <= k
-          int j = 0;
-#pragma unroll
-          for (int step = 16; step >= 1; step >>= 1) {
-            const int probe_lane = j + step - 1;
-            const uint32_t v = __shfl_sync(kFull, incl, probe_lane & 31);
-            if (probe_lane < 32 && v <= lane) j += step;
-          }
-          jb = __shfl_sync(kFull, it.x, j & 31);
-          jmeta = __shfl_sync(kFull, it.z, j & 31);
-          jexcl = __shfl_sync(kFull, excl, j & 31);
+        for (int d = 1; d < 32; d <<= 1) {
+          uint32_t v = __shfl_up_sync(kFull, incl, d);
+          if (static_cast<int>(lane) >= d) incl += v;
         }
+        const uint32_t excl = incl - len;
+        const unsigned fullm = __ballot_sync(kFull, static_cast<int>(lane) < n && incl <= 32u);
+        const int nfull = __popc(fullm);  // prefix of fully consumed items
+        uint32_t total = __shfl_sync(kFull, incl, 31);
+        if (total > 32u) total = 32u;
+        __syncwarp();
+        if (static_cast<int>(lane) == nfull && static_cast<int>(lane) < n)  // partially consumed item stays on top
+          c.stack[c.top - 1 - lane].x = it.x + (32u - excl);
+        c.top -= nfull;
+        __syncwarp();
+        // ---- lane k takes edge k: owner item j = #items with incl <= k
+        int j = 0;
+#pragma unroll
+        for (int step = 16; step >= 1; step >>= 1) {
+          const int probe_lane = j + step - 1;
+          const uint32_t v = __shfl_sync(kFull, incl, probe_lane & 31);
+          if (probe_lane < 32 && v <= lane) j += step;
+        }
+        const uint32_t jb = __shfl_sync(kFull, it.x, j & 31);
+        const uint32_t jmeta = __shfl_sync(kFull, it.z, j & 31);
+        const uint32_t jexcl = __shfl_sync(kFull, excl, j & 31);
         bool active = lane < total;
         const uint32_t jslot = jmeta & 31u, cdepth = (jmeta >> 5) & 63u, tslot = jmeta >> 16;
         uint32_t child = 0;

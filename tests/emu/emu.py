@@ -32,7 +32,7 @@ def default_opts(**kw):
 
 
 def build() -> str:
-    extra = os.environ.get("ZGPU_EMU_CFLAGS", "").split()  # tuning macros of kernels.cuh (-DZG_L2_FILTER=1 ...)
+    extra = os.environ.get("ZGPU_EMU_CFLAGS", "").split()  # tuning macros of kernels.cuh (-DZG_PHASE_CLOCKS=1 ...)
     so = os.path.join(_HERE, "libzgemu" + ("_" + "".join(c if c.isalnum() else "_" for c in "".join(extra)) if extra else "") + ".so")
     srcs = [os.path.join(_HERE, f) for f in ("emu_main.cc", "cuda_emu.h")] + \
            [os.path.join(_CSRC, f) for f in ("kernels.cuh", "delta.cuh", "schema.cc", "schema.h", "store.cc", "store.h")]

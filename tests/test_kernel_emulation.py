@@ -123,10 +123,10 @@ definition doc {
 
 
 def test_two_level_meet_over_every_range_size_and_membership_count_under_the_emulator(emu):
-    """The cooperative two-level meet stages <= 64 children of a range (plus their filter) in shared memory and gives
-    every membership row 32 / ng lanes: ranges of 1 .. 70 children (beyond 64: the walk takes over), subjects with
-    1 .. 17 memberships (beyond 16: the per-check set overflows into forward probes), hits on the first / last child,
-    near misses (ids that differ in one bit from a child: filter false positives must die in the search)."""
+    """The two-level meet (batch_l2) answers ranges of <= 64 children against a 128-bit filter of each: ranges of
+    1 .. 70 children (beyond 64: the walk takes over), subjects with 1 .. 17 memberships (beyond 16: the per-check set
+    overflows and the meet reads them from the subject's reverse row), hits on the first / last child, near misses
+    (filter false positives must die in the search)."""
     schema = """definition user {}
 definition group { relation member: user }
 definition team { relation member: group#member }
@@ -150,23 +150,6 @@ definition namespace { relation viewer: team#member  permission view = viewer }"
     e, o = _compare_strings(emu, schema, rels, checks)
     got = e.check_bulk(e.items_from_strings(checks, split_rel))
     assert 0.1 < (got == 2).mean() < 0.9  # both answers occur
-
-
-def test_two_level_meet_filter_false_positives_die_in_the_search_under_the_emulator(emu):
-    """Ids that collide in the filter of the range's children (tests/l2_cases.py): the subject reaches a team that the
-    filter cannot tell from a child of the range; only the search behind the filter may answer."""
-    import l2_cases as L
-
-    e = emu.EmuEngine(L.L2_SCHEMA)
-    e.write_rels(L.padding_rels(), split_rel)
-    rels, cases = L.collision_cases(lambda name: e._id("team", name, False))
-    e.write_rels(rels, split_rel)
-    e.publish()
-    got = e.check_bulk(e.items_from_strings([q for q, _ in cases], split_rel))
-    assert [int(x) for x in got] == [w for _, w in cases]
-    e2 = emu.EmuEngine(L.L2_SCHEMA)  # forward-only probes agree
-    e2.write_rels(L.padding_rels() + rels, split_rel), e2.publish()
-    assert np.array_equal(e2.check_bulk(e2.items_from_strings([q for q, _ in cases], split_rel), emu.default_opts(invert=0)), got)
 
 
 @pytest.mark.parametrize("wl,scale,n", [("cfg2", 0.01, 2000), ("cfg3", 0.003, 3000), ("cfg4", 0.001, 3000)])

@@ -192,27 +192,6 @@ definition namespace { relation viewer: team#member  permission view = viewer }"
     assert 0.1 < (got == 2).mean() < 0.9
 
 
-def test_two_level_meet_filter_false_positives_die_in_the_search():
-    """Ids that collide in the filter over a range's children (tests/l2_cases.py): the filter lets the subject's team
-    through, the search behind it must say no. Same cases as under the emulator."""
-    import l2_cases as L
-    import zgpu
-
-    C = zgpu.client
-    c = C.PermissionsClient(L.L2_SCHEMA)
-
-    def write(rels):
-        for i in range(0, len(rels), 1000):
-            c.WriteRelationships(C.WriteRelationshipsRequest(
-                [C.RelationshipUpdate(C.OPERATION_TOUCH, C.Relationship.parse(r)) for r in rels[i:i + 1000]]))
-
-    write(L.padding_rels())
-    rels, cases = L.collision_cases(lambda name: int(c.engine.find("team", name)))
-    write(rels)
-    got = c.engine.check_bulk_str([q for q, _ in cases])
-    assert [int(x) for x in got] == [w for _, w in cases]
-
-
 def test_prefilter_of_a_protobuf_encoded_list():
     """zg_list_prefilter with ZG_LIST_PROTOBUF: LookupResources on the GPU, then the items of a protobuf-encoded PodList
     (what kube clients receive for built-in types) whose namespace/name it returned are kept, byte for byte
