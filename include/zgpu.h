@@ -299,7 +299,8 @@ int zg_debug_row(zg_engine *e, uint16_t rel_slot, uint32_t res, uint32_t cls, ui
  * into a non-pure permission) is raised as a sub-query. The host runs the ranks pass by pass
  * and exchanges the raised sub-queries (all-to-all) until none are left, then folds the values
  * back level by level (spicedb-kubeapi-proxy_b200/dist.py ShardedStoreChecker). On sharded
- * engines zg_check_bulk / zg_lookup_resources are refused: use these three calls. */
+ * engines zg_check_bulk / zg_lookup_resources are refused: use these three calls (checks) or the
+ * zg_shard_lookup_*_dev calls below (LookupResources). */
 int zg_shard_pass(zg_engine *e, const zg_check *queries, uint64_t n, int level, uint64_t *n_sub);
 /* The sub-queries pass `level` raised, in emission order (same layout; flags = hop depth). */
 int zg_shard_subqueries(zg_engine *e, int level, zg_check *out, uint64_t n);
@@ -324,6 +325,37 @@ int zg_shard_pass_dev(zg_engine *e, const zg_check *d_queries, uint64_t n, int l
 int zg_shard_fold_dev(zg_engine *e, int level, const uint8_t *d_child_vals, const uint32_t *d_src,
                       uint64_t n_sub, uint8_t *d_out, int final_codes);
 int zg_shard_unroute_dev(zg_engine *e, const uint32_t *d_src, const uint8_t *d_val, uint64_t n, uint8_t *d_out);
+
+/* LookupResources on a sharded engine (dist.DeviceShardedLookup), in rounds of k <= 64 lookups that every rank
+ * runs with the same list. Shard r discovers, in its own reverse rows, only objects it owns, so the walk needs no
+ * cross-shard dedup: each level every rank expands the whole replicated frontier and the next frontier is every
+ * rank's new entries, all-gathered. Candidates are verified by the sharded check protocol above, and the answers are
+ * sent to the rank that asked the lookup. Same conventions as the zg_shard_*_dev calls; ZG_EINVAL on an engine
+ * that is not sharded, ZG_ECUDA on a host-only one. zg_lookup_resources* stays refused on sharded engines.
+ *   zg_shard_lookup_begin_dev      starts a round: res_types / protos (subj, perm, stype, srel) / home (rank that
+ *                                  asked) are HOST arrays of k; d_seeds (device, k entries) receives the level-0
+ *                                  frontier; walk_cap bounds every frontier and the walk's candidates
+ *   zg_shard_lookup_expand_dev     expands the n_in frontier entries of d_front against this shard's reverse rows
+ *                                  into d_next (walk_cap entries): *n_next new entries; *overflow = 1 when a frontier
+ *                                  or the candidates did not fit (redo the round in halves; a single lookup verifies
+ *                                  every resource of its type instead)
+ *   zg_shard_lookup_candidates_dev this shard's candidates as check items (the walk's, or with exhaustive every owned
+ *                                  resource of the type, plus owned userset subjects naming their own object); with
+ *                                  d_items NULL, *n = the capacity needed; ZG_E2BIG when cap is smaller
+ *   zg_shard_lookup_route_dev      d_codes (one per candidate) -> answer keys (lookup << 32 | id; bit 38: a walk candidate
+ *                                  could not be decided; an undecidable self-membership is left out, as in
+ *                                  zg_lookup_resources) in d_routed, bucketed by home rank; counts[d] (HOST, n_dest)
+ *   zg_shard_lookup_finish_dev     the keys that arrived home -> d_ids: ascending ids of lookup 0, then lookup 1, ...;
+ *                                  per_lookup[i] (HOST, k) = ids of lookup i; *err_mask bit i: lookup i is ZG_EDEPTH */
+int zg_shard_lookup_begin_dev(zg_engine *e, const uint16_t *res_types, const zg_check *protos, const uint8_t *home,
+                              uint32_t k, uint64_t walk_cap, uint64_t *d_seeds);
+int zg_shard_lookup_expand_dev(zg_engine *e, const uint64_t *d_front, uint64_t n_in, int level, uint64_t *d_next,
+                               uint64_t *n_next, int *overflow);
+int zg_shard_lookup_candidates_dev(zg_engine *e, int exhaustive, zg_check *d_items, uint64_t cap, uint64_t *n);
+int zg_shard_lookup_route_dev(zg_engine *e, const uint8_t *d_codes, uint64_t n, uint32_t n_dest, uint64_t *d_routed,
+                              uint64_t *counts);
+int zg_shard_lookup_finish_dev(zg_engine *e, const uint64_t *d_keys, uint64_t n, uint32_t *d_ids, uint64_t *per_lookup,
+                               uint64_t *err_mask);
 
 /* Watch feed (v1.WatchServiceClient.Watch, pkg/authz/watch.go:27-48): the relationship changes made
  * visible by revisions > since_revision, oldest first, as '\n'-separated lines

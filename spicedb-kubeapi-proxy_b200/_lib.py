@@ -183,6 +183,14 @@ _SIGS = {
     "zg_shard_pass_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.POINTER(C.c_uint64)]),
     "zg_shard_fold_dev": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_int]),
     "zg_shard_unroute_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
+    "zg_shard_lookup_begin_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64,
+                                            C.c_void_p]),
+    "zg_shard_lookup_expand_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_void_p,
+                                             C.POINTER(C.c_uint64), C.POINTER(C.c_int)]),
+    "zg_shard_lookup_candidates_dev": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),
+    "zg_shard_lookup_route_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p]),
+    "zg_shard_lookup_finish_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
+                                             C.POINTER(C.c_uint64)]),
     "zg_debug_row": (C.c_int, [C.c_void_p, C.c_uint16, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64,
                                C.POINTER(C.c_uint64)]),
     "zg_host_alloc": (C.c_void_p, [C.c_size_t]),
@@ -662,6 +670,40 @@ class Engine:
 
     def shard_unroute_dev(self, d_src: int, d_val: int, n: int, d_out: int):
         self._ck(self._L.zg_shard_unroute_dev(self._h, d_src or None, d_val or None, n, d_out or None))
+
+    # sharded LookupResources (dist.DeviceShardedLookup drives these): one round of <= 64 lookups at a time
+    def shard_lookup_begin_dev(self, res_types, protos, home, walk_cap: int, d_seeds: int):
+        """res_types (uint16), protos (CHECK_DTYPE: subj, perm, stype, srel), home (uint8): host arrays of k."""
+        rt = np.ascontiguousarray(res_types, dtype=np.uint16)
+        pr = np.ascontiguousarray(protos, dtype=CHECK_DTYPE)
+        hm = np.ascontiguousarray(home, dtype=np.uint8)
+        self._ck(self._L.zg_shard_lookup_begin_dev(self._h, rt.ctypes.data, pr.ctypes.data, hm.ctypes.data, rt.size, walk_cap,
+                                                   d_seeds or None))
+
+    def shard_lookup_expand_dev(self, d_front: int, n_in: int, level: int, d_next: int):
+        """-> (new frontier entries, overflow)"""
+        n, ovf = C.c_uint64(0), C.c_int(0)
+        self._ck(self._L.zg_shard_lookup_expand_dev(self._h, d_front or None, n_in, level, d_next or None, C.byref(n),
+                                                    C.byref(ovf)))
+        return n.value, bool(ovf.value)
+
+    def shard_lookup_candidates_dev(self, exhaustive: bool, d_items: int, cap: int) -> int:
+        """d_items == 0: the capacity needed; else the candidates written."""
+        n = C.c_uint64(0)
+        self._ck(self._L.zg_shard_lookup_candidates_dev(self._h, 1 if exhaustive else 0, d_items or None, cap, C.byref(n)))
+        return n.value
+
+    def shard_lookup_route_dev(self, d_codes: int, n: int, n_dest: int, d_routed: int) -> list:
+        counts = (C.c_uint64 * n_dest)()
+        self._ck(self._L.zg_shard_lookup_route_dev(self._h, d_codes or None, n, n_dest, d_routed or None, counts))
+        return [int(c) for c in counts]
+
+    def shard_lookup_finish_dev(self, d_keys: int, n: int, d_ids: int, k: int):
+        """-> (answers per lookup of the round, error mask)"""
+        per = (C.c_uint64 * max(k, 1))()
+        mask = C.c_uint64(0)
+        self._ck(self._L.zg_shard_lookup_finish_dev(self._h, d_keys or None, n, d_ids or None, per, C.byref(mask)))
+        return [int(per[i]) for i in range(k)], mask.value
 
     def debug_row(self, type_name, rel, res, cls=0, reverse=False) -> np.ndarray:
         """Forward row (resource `res`, class) or, reverse=True, the reverse row of subject `res`."""

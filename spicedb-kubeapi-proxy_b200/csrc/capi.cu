@@ -1942,6 +1942,59 @@ extern "C" int zg_shard_unroute_dev(zg_engine* e, const uint32_t* d_src, const u
   return rc ? fail(rc, err) : ZG_OK;
 }
 
+// LookupResources on the sharded store: the same prologue, and only on a sharded engine
+#define SHARD_LOOKUP_PROLOGUE()                                                                                       \
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);                                                                                       \
+  std::lock_guard<FairMutex> g(e->mu);                                                                               \
+  if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");      \
+  if (e->dev.shard_count < 2) return fail(ZG_EINVAL, "not a sharded engine: use zg_lookup_resources");               \
+  if (!e->dev.snap) return fail(ZG_ENOSNAPSHOT, "no snapshot published (call zg_publish)");
+
+extern "C" int zg_shard_lookup_begin_dev(zg_engine* e, const uint16_t* res_types, const zg_check* protos, const uint8_t* home,
+                                         uint32_t k, uint64_t walk_cap, uint64_t* d_seeds) {
+  if (!res_types || !protos || !home || !d_seeds) return fail(ZG_EINVAL, "NULL argument");
+  SHARD_LOOKUP_PROLOGUE();
+  std::vector<Device::LookupReq> reqs(k);
+  for (uint32_t i = 0; i < k; ++i) reqs[i] = Device::LookupReq{res_types[i], protos[i]};
+  std::string err;
+  int rc = e->dev.shard_lookup_begin(reqs, home, walk_cap, reinterpret_cast<unsigned long long*>(d_seeds), &err);
+  return rc ? fail(rc, err) : ZG_OK;
+}
+extern "C" int zg_shard_lookup_expand_dev(zg_engine* e, const uint64_t* d_front, uint64_t n_in, int level, uint64_t* d_next,
+                                          uint64_t* n_next, int* overflow) {
+  if ((!d_front && n_in) || !d_next || !n_next || !overflow) return fail(ZG_EINVAL, "NULL argument");
+  SHARD_LOOKUP_PROLOGUE();
+  std::string err;
+  bool ovf = false;
+  int rc = e->dev.shard_lookup_expand(reinterpret_cast<const unsigned long long*>(d_front), n_in, level,
+                                      reinterpret_cast<unsigned long long*>(d_next), n_next, &ovf, &err);
+  *overflow = ovf ? 1 : 0;
+  return rc ? fail(rc, err) : ZG_OK;
+}
+extern "C" int zg_shard_lookup_candidates_dev(zg_engine* e, int exhaustive, zg_check* d_items, uint64_t cap, uint64_t* n) {
+  if (!n) return fail(ZG_EINVAL, "NULL argument");
+  SHARD_LOOKUP_PROLOGUE();
+  std::string err;
+  int rc = e->dev.shard_lookup_candidates(exhaustive != 0, d_items, cap, n, &err);
+  return rc ? fail(rc, err) : ZG_OK;
+}
+extern "C" int zg_shard_lookup_route_dev(zg_engine* e, const uint8_t* d_codes, uint64_t n, uint32_t n_dest, uint64_t* d_routed,
+                                         uint64_t* counts) {
+  if (!counts || ((!d_codes || !d_routed) && n)) return fail(ZG_EINVAL, "NULL argument");
+  SHARD_LOOKUP_PROLOGUE();
+  std::string err;
+  int rc = e->dev.shard_lookup_route(d_codes, n, n_dest, reinterpret_cast<unsigned long long*>(d_routed), counts, &err);
+  return rc ? fail(rc, err) : ZG_OK;
+}
+extern "C" int zg_shard_lookup_finish_dev(zg_engine* e, const uint64_t* d_keys, uint64_t n, uint32_t* d_ids, uint64_t* per_lookup,
+                                          uint64_t* err_mask) {
+  if (!per_lookup || !err_mask || ((!d_keys || !d_ids) && n)) return fail(ZG_EINVAL, "NULL argument");
+  SHARD_LOOKUP_PROLOGUE();
+  std::string err;
+  int rc = e->dev.shard_lookup_finish(reinterpret_cast<const unsigned long long*>(d_keys), n, d_ids, per_lookup, err_mask, &err);
+  return rc ? fail(rc, err) : ZG_OK;
+}
+
 extern "C" int zg_debug_row(zg_engine* e, uint16_t rel_slot, uint32_t res, uint32_t cls, uint32_t* out, uint64_t cap,
                             uint64_t* n_out) {
   NEED_SCHEMA(e, ZG_ENOSCHEMA);

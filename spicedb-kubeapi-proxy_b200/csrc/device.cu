@@ -859,6 +859,19 @@ int Device::route_by_owner(const zg_check* d_items, uint64_t n, int level, uint3
     }
     d_items = q_[lv + 1].as<zg_check>();
   }
+  return route_<true>(d_items, n, n_dest, ResOwner{}, d_routed, d_src, counts, err);
+}
+
+// Counting sort of n items by owner(item, n_dest) into d_routed (destination-major), with their source indices in
+// d_src when kSrc; counts[d] (host) = items for destination d.
+template <bool kSrc, class Item, class Owner>
+int Device::route_(const Item* d_items, uint64_t n, uint32_t n_dest, Owner owner, Item* d_routed, uint32_t* d_src, uint64_t* counts,
+                   std::string* err) {
+  if (n_dest == 0 || n_dest > kMaxRouteDest) {  // the histogram and the cursors hold kMaxRouteDest destinations
+    if (err) *err = "routing: destination count out of range (1 .. 64)";
+    return ZG_EINVAL;
+  }
+  for (uint32_t d = 0; d < n_dest; ++d) counts[d] = 0;
   if (n == 0) return ZG_OK;
   if (!route_ctrl_.ensure(2 * kMaxRouteDest * 8)) return ZG_ENOMEM;
   unsigned long long* d_counts = route_ctrl_.as<unsigned long long>();
@@ -866,7 +879,7 @@ int Device::route_by_owner(const zg_check* d_items, uint64_t n, int level, uint3
   if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
   ZG_CUDA(cudaMemsetAsync(d_counts, 0, kMaxRouteDest * 8, stream));
   const unsigned grid = static_cast<unsigned>(std::min<uint64_t>((n + 255) / 256, static_cast<uint64_t>(sm_count_) * 8));
-  route_count_kernel<<<grid, 256, 0, stream>>>(d_items, n, n_dest, d_counts);
+  route_count_kernel<<<grid, 256, 0, stream>>>(d_items, n, n_dest, d_counts, owner);
   unsigned long long h[kMaxRouteDest];
   ZG_CUDA(cudaMemcpyAsync(h, d_counts, n_dest * 8, cudaMemcpyDeviceToHost, stream));
   ZG_CUDA(cudaStreamSynchronize(stream));
@@ -877,7 +890,7 @@ int Device::route_by_owner(const zg_check* d_items, uint64_t n, int level, uint3
     acc += h[d];
   }
   ZG_CUDA(cudaMemcpyAsync(d_cursor, off, n_dest * 8, cudaMemcpyHostToDevice, stream));
-  route_scatter_kernel<<<grid, 256, 0, stream>>>(d_items, n, n_dest, d_cursor, d_routed, d_src);
+  route_scatter_kernel<Item, Owner, kSrc><<<grid, 256, 0, stream>>>(d_items, n, n_dest, d_cursor, d_routed, d_src, owner);
   launches += 2;
   ZG_CUDA(cudaGetLastError());
   ZG_CUDA(cudaEventRecord(last_done_, stream));
@@ -989,6 +1002,288 @@ int Device::unroute(const uint32_t* d_src, const uint8_t* d_val, uint64_t n, uin
   ZG_CUDA(cudaEventRecord(last_done_, stream));
   have_last_ = true;
   ZG_CUDA(cudaStreamSynchronize(stream));
+  return ZG_OK;
+}
+
+// ---- LookupResources on the object-hash sharded store (DESIGN.md 4, dist.DeviceShardedLookup) ------------------
+// sl_ctrl_ words: [0] flags, [1] candidates, [2] keys, [3] error mask, then the level counts, then first[] / end[] of
+// every lookup's answers after the final sort.
+namespace {
+constexpr size_t kSlCounts = 8, kSlFirst = kSlCounts + ZG_MAX_DEPTH + 4, kSlEnd = kSlFirst + kMaxLookupBatch,
+                 kSlCtrlWords = kSlEnd + kMaxLookupBatch;
+}
+
+int Device::shard_lookup_begin(const std::vector<LookupReq>& reqs, const uint8_t* home, uint64_t walk_cap,
+                               unsigned long long* d_seeds, std::string* err) {
+  std::shared_ptr<Snapshot> s = snap;
+  const size_t K = reqs.size();
+  sl_snap_.reset();
+  sl_n_cand_ = sl_n_walk_ = 0;
+  if (!s) {
+    if (err) *err = "no snapshot published";
+    return ZG_ENOSNAPSHOT;
+  }
+  if (K == 0 || K > kMaxLookupBatch || walk_cap == 0 || shard_count > kMaxRouteDest) {
+    if (err) *err = "shard_lookup_begin: 1..64 lookups, a non-zero walk capacity and at most 64 shards";
+    return ZG_EINVAL;
+  }
+  for (size_t k = 0; k < K; ++k)
+    if (reqs[k].res_type >= s->n_objects.size() || reqs[k].proto.stype >= s->n_objects.size() || home[k] >= shard_count) {
+      if (err) *err = "shard_lookup_begin: unknown type or home rank";
+      return ZG_EINVAL;
+    }
+  ZG_CUDA(cudaSetDevice(device));
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  const unsigned long long words = (s->total_bits + 31) / 32 + 4;
+  if (!rb_visited_.ensure(words * 4 * K) || !lk_jobs_.ensure((walk_cap + K) * sizeof(zg_check)) || !lb_owner_.ensure(walk_cap + K) ||
+      !lb_params_.ensure(K * sizeof(LookupParam)) || !sl_home_.ensure(K) || !sl_ctrl_.ensure(kSlCtrlWords * 8)) {
+    if (err) *err = "out of device memory (sharded lookup buffers)";
+    return ZG_ENOMEM;
+  }
+  std::vector<LookupParam> lp(K);
+  std::vector<unsigned long long> seeds(K);
+  for (size_t i = 0; i < K; ++i) {
+    const zg_check& q = reqs[i].proto;
+    lp[i] = LookupParam{q.subj, reqs[i].res_type, q.perm, q.stype, q.srel};
+    seeds[i] = (static_cast<unsigned long long>(i) << 48) | (static_cast<unsigned long long>(q.stype) << 32) | q.subj;
+  }
+  ZG_CUDA(cudaMemsetAsync(sl_ctrl_.p, 0, kSlCtrlWords * 8, stream));
+  ZG_CUDA(cudaMemsetAsync(rb_visited_.p, 0, words * 4 * K, stream));
+  ZG_CUDA(cudaMemcpyAsync(lb_params_.p, lp.data(), K * sizeof(LookupParam), cudaMemcpyHostToDevice, stream));
+  ZG_CUDA(cudaMemcpyAsync(sl_home_.p, home, K, cudaMemcpyHostToDevice, stream));
+  ZG_CUDA(cudaMemcpyAsync(d_seeds, seeds.data(), K * 8, cudaMemcpyHostToDevice, stream));
+  ZG_CUDA(cudaEventRecord(last_done_, stream));
+  have_last_ = true;
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  sl_snap_ = s;
+  sl_reqs_ = reqs;
+  sl_cap_ = walk_cap;
+  return ZG_OK;
+}
+
+int Device::shard_lookup_expand(const unsigned long long* d_front, uint64_t n_in, int level, unsigned long long* d_next,
+                                uint64_t* n_next, bool* overflow, std::string* err) {
+  *n_next = 0;
+  *overflow = false;
+  if (!sl_snap_ || level < 0 || level > ZG_MAX_DEPTH + 1) {
+    if (err) *err = "shard_lookup_expand: no round begun, or level out of range";
+    return ZG_EINVAL;
+  }
+  // the gathered frontier is the same on every rank, so every rank reports this overflow in the same level
+  if (n_in > sl_cap_) {
+    *overflow = true;
+    return ZG_OK;
+  }
+  if (n_in == 0) return ZG_OK;
+  const Snapshot& s = *sl_snap_;
+  ZG_CUDA(cudaSetDevice(device));
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  unsigned long long* ctrl = sl_ctrl_.as<unsigned long long>();
+  unsigned long long* counts = ctrl + kSlCounts;
+  const unsigned long long c[2] = {n_in, 0};
+  ZG_CUDA(cudaMemcpyAsync(counts + level, c, sizeof c, cudaMemcpyHostToDevice, stream));
+  MrbfsParams p{};
+  p.rrow_ptr = s.rrow_ptr.as<uint32_t>();
+  p.rcol = s.rcol.as<uint32_t>();
+  p.prog = s.prog.as<uint8_t>();
+  p.lk = lb_params_.as<LookupParam>();
+  p.in = d_front;
+  p.out = d_next;
+  p.counts = counts;
+  p.level = level;
+  p.cap = sl_cap_;
+  p.visited = rb_visited_.as<uint32_t>();
+  p.words = (s.total_bits + 31) / 32 + 4;
+  p.type_bit_base = s.type_bit_base.as<unsigned long long>();
+  p.cand = lk_jobs_.as<zg_check>();
+  p.cand_owner = lb_owner_.as<uint8_t>();
+  p.cand_count = ctrl + 1;
+  p.cand_cap = sl_cap_;
+  p.flags = reinterpret_cast<uint32_t*>(ctrl);
+  mrbfs_expand_kernel<<<sm_count_ * 8, 256, 0, stream>>>(p);
+  ++launches;
+  ZG_CUDA(cudaGetLastError());
+  unsigned long long flags = 0, cnt = 0;
+  ZG_CUDA(cudaMemcpyAsync(&flags, ctrl, 8, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaMemcpyAsync(&cnt, counts + level + 1, 8, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaEventRecord(last_done_, stream));
+  have_last_ = true;
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  *overflow = (static_cast<uint32_t>(flags) & 16u) != 0;
+  *n_next = std::min<uint64_t>(cnt, sl_cap_);
+  return ZG_OK;
+}
+
+int Device::shard_lookup_candidates(bool exhaustive, zg_check* d_items, uint64_t cap, uint64_t* n, std::string* err) {
+  *n = 0;
+  if (!sl_snap_) {
+    if (err) *err = "shard_lookup_candidates: no round begun";
+    return ZG_EINVAL;
+  }
+  Snapshot& s = *sl_snap_;
+  const size_t K = sl_reqs_.size();
+  ZG_CUDA(cudaSetDevice(device));
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  unsigned long long* ctrl = sl_ctrl_.as<unsigned long long>();
+  const unsigned long long words = (s.total_bits + 31) / 32 + 4;
+  // userset subjects T:x#r of lookups of type T whose x this shard owns: x is a member of T:x#P for every relation r
+  // inlined into P, and the walk only reaches x through stored edges (run_lookup_group asks the check kernel the same)
+  std::vector<SelfCand> self;
+  uint64_t bit_base = 0;
+  for (size_t k = 0; k < K; ++k) {
+    const LookupReq& r = sl_reqs_[k];
+    const zg_check& q = r.proto;
+    if (q.srel == kNone || q.stype != r.res_type || q.subj >= ZG_NO_OBJECT - 1 || q.subj % shard_count != shard_rank) continue;
+    bit_base = 0;
+    for (uint16_t t = 0; t < r.res_type; ++t) bit_base += (uint64_t(s.n_objects[t]) + 31) & ~31ull;
+    self.push_back(SelfCand{static_cast<uint32_t>(k), 0, q.subj < s.n_objects[r.res_type] ? bit_base + q.subj : ~0ull});
+  }
+  uint64_t need = self.size();
+  unsigned long long walked = 0;
+  if (exhaustive) {
+    if (s.resources_stale) {
+      std::string rerr = gpu_resource_lists(&s, stream);
+      if (!rerr.empty()) {
+        if (err) *err = rerr;
+        return ZG_ECUDA;
+      }
+    }
+    for (const LookupReq& r : sl_reqs_) need += s.n_resources[r.res_type];
+  } else {
+    ZG_CUDA(cudaMemcpyAsync(&walked, ctrl + 1, 8, cudaMemcpyDeviceToHost, stream));
+    ZG_CUDA(cudaStreamSynchronize(stream));
+    if (walked > sl_cap_) {
+      if (err) *err = "shard_lookup_candidates: the walk overflowed (redo the round in halves, or exhaustive)";
+      return ZG_EINVAL;
+    }
+    need += walked;
+  }
+  if (!d_items) {
+    *n = need;
+    return ZG_OK;
+  }
+  if (cap < need) {
+    if (err) *err = "shard_lookup_candidates: item buffer too small";
+    return ZG_E2BIG;
+  }
+  if (exhaustive) {
+    if (!lk_jobs_.ensure(std::max<uint64_t>(need, 1) * sizeof(zg_check)) || !lb_owner_.ensure(std::max<uint64_t>(need, 1))) {
+      if (err) *err = "out of device memory (sharded lookup candidates)";
+      return ZG_ENOMEM;
+    }
+    ZG_CUDA(cudaMemsetAsync(rb_visited_.p, 0, words * 4 * K, stream));
+    uint64_t at = 0;
+    for (size_t k = 0; k < K; ++k) {
+      const LookupReq& r = sl_reqs_[k];
+      const uint64_t nr = s.n_resources[r.res_type];
+      if (!nr) continue;
+      uint64_t base = 0;
+      for (uint16_t t = 0; t < r.res_type; ++t) base += (uint64_t(s.n_objects[t]) + 31) & ~31ull;
+      const LookupParam l{r.proto.subj, r.res_type, r.proto.perm, r.proto.stype, r.proto.srel};
+      lookup_fill_owned_kernel<<<static_cast<unsigned>((nr + 255) / 256), 256, 0, stream>>>(
+          s.resources[r.res_type].as<uint32_t>(), nr, l, static_cast<uint32_t>(k), rb_visited_.as<uint32_t>() + k * words, base,
+          lk_jobs_.as<zg_check>() + at, lb_owner_.as<uint8_t>() + at);
+      ++launches;
+      at += nr;
+    }
+    const unsigned long long filled = at;
+    ZG_CUDA(cudaMemcpyAsync(ctrl + 1, &filled, 8, cudaMemcpyHostToDevice, stream));
+    ZG_CUDA(cudaStreamSynchronize(stream));  // `filled` lives on this stack frame
+  }
+  // the self-membership candidates come after these: only the walk's / the fill's can fail the lookup
+  sl_n_walk_ = exhaustive ? need - self.size() : walked;
+  if (!self.empty()) {
+    if (!sl_self_.ensure(self.size() * sizeof(SelfCand))) return ZG_ENOMEM;
+    ZG_CUDA(cudaMemcpyAsync(sl_self_.p, self.data(), self.size() * sizeof(SelfCand), cudaMemcpyHostToDevice, stream));
+    lookup_self_kernel<<<1, kMaxLookupBatch, 0, stream>>>(lb_params_.as<LookupParam>(), sl_self_.as<SelfCand>(),
+                                                          static_cast<uint32_t>(self.size()), rb_visited_.as<uint32_t>(), words,
+                                                          lk_jobs_.as<zg_check>(), lb_owner_.as<uint8_t>(), ctrl + 1);
+    ++launches;
+  }
+  unsigned long long total = 0;
+  ZG_CUDA(cudaMemcpyAsync(&total, ctrl + 1, 8, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  if (total) ZG_CUDA(cudaMemcpyAsync(d_items, lk_jobs_.p, total * sizeof(zg_check), cudaMemcpyDeviceToDevice, stream));
+  ZG_CUDA(cudaGetLastError());
+  ZG_CUDA(cudaEventRecord(last_done_, stream));
+  have_last_ = true;
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  sl_n_cand_ = total;
+  *n = total;
+  return ZG_OK;
+}
+
+int Device::shard_lookup_route(const uint8_t* d_codes, uint64_t n, uint32_t n_dest, unsigned long long* d_routed,
+                               uint64_t* counts, std::string* err) {
+  for (uint32_t d = 0; d < n_dest && d < kMaxRouteDest; ++d) counts[d] = 0;
+  if (!sl_snap_ || n != sl_n_cand_ || n_dest != shard_count) {
+    if (err) *err = "shard_lookup_route: no candidates of this round, or a count / shard count mismatch";
+    return ZG_EINVAL;
+  }
+  if (n == 0) return ZG_OK;
+  ZG_CUDA(cudaSetDevice(device));
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  if (!lb_keys_[0].ensure(n * 8)) {
+    if (err) *err = "out of device memory (sharded lookup keys)";
+    return ZG_ENOMEM;
+  }
+  unsigned long long* ctrl = sl_ctrl_.as<unsigned long long>();
+  ZG_CUDA(cudaMemsetAsync(ctrl + 2, 0, 16, stream));
+  // per-lookup counts of this shard's answers are not needed: the home rank counts after the final sort
+  lookup_keys_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(
+      lk_jobs_.as<zg_check>(), lb_owner_.as<uint8_t>(), d_codes, n, lb_keys_[0].as<unsigned long long>(), ctrl + 2,
+      ctrl + kSlFirst, ctrl + 3, sl_n_walk_);
+  ++launches;
+  unsigned long long n_keys = 0;
+  ZG_CUDA(cudaMemcpyAsync(&n_keys, ctrl + 2, 8, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaEventRecord(last_done_, stream));
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  have_last_ = true;
+  return route_<false>(static_cast<const unsigned long long*>(lb_keys_[0].as<unsigned long long>()), n_keys, n_dest,
+                       KeyHomeOwner{sl_home_.as<uint8_t>()}, d_routed, static_cast<uint32_t*>(nullptr), counts, err);
+}
+
+int Device::shard_lookup_finish(const unsigned long long* d_keys, uint64_t n, uint32_t* d_ids, uint64_t* per_lookup,
+                                uint64_t* err_mask, std::string* err) {
+  *err_mask = 0;
+  if (!sl_snap_) {
+    if (err) *err = "shard_lookup_finish: no round begun";
+    return ZG_EINVAL;
+  }
+  const size_t K = sl_reqs_.size();
+  // the round ends here, whatever follows: the snapshot it read is not kept resident past it
+  sl_snap_.reset();
+  sl_reqs_.clear();
+  sl_n_cand_ = sl_n_walk_ = 0;
+  for (size_t k = 0; k < K; ++k) per_lookup[k] = 0;
+  if (n == 0) return ZG_OK;
+  ZG_CUDA(cudaSetDevice(device));
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  if (!lb_keys_[1].ensure(n * 8)) {
+    if (err) *err = "out of device memory (sharded lookup keys)";
+    return ZG_ENOMEM;
+  }
+  unsigned long long* ctrl = sl_ctrl_.as<unsigned long long>();
+  ZG_CUDA(cudaMemsetAsync(ctrl + 3, 0, 8, stream));
+  ZG_CUDA(cudaMemsetAsync(ctrl + kSlFirst, 0, 2 * kMaxLookupBatch * 8, stream));
+  // ascending (error bit, lookup, id): answers per lookup in lookup order, the error keys last
+  std::string serr = sort_u64(d_keys, lb_keys_[1].as<unsigned long long>(), n, kErrKeyBit + 1, stream);
+  if (!serr.empty()) {
+    if (err) *err = serr;
+    return ZG_ECUDA;
+  }
+  lookup_split_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(
+      lb_keys_[1].as<unsigned long long>(), n, d_ids, ctrl + kSlFirst, ctrl + kSlEnd, ctrl + 3);
+  ++launches;
+  unsigned long long host[1 + 2 * kMaxLookupBatch];
+  ZG_CUDA(cudaMemcpyAsync(host, ctrl + 3, 8, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaMemcpyAsync(host + 1, ctrl + kSlFirst, 2 * kMaxLookupBatch * 8, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaGetLastError());
+  ZG_CUDA(cudaEventRecord(last_done_, stream));
+  have_last_ = true;
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  *err_mask = host[0];
+  for (size_t k = 0; k < K; ++k) per_lookup[k] = host[1 + kMaxLookupBatch + k] - host[1 + k];
   return ZG_OK;
 }
 

@@ -128,6 +128,26 @@ class Device {
   int shard_fold_dev(int level, const uint8_t* d_child_vals, const uint32_t* d_src, uint64_t n_sub, uint8_t* d_out,
                      bool final_codes, std::string* err);
   int unroute(const uint32_t* d_src, const uint8_t* d_val, uint64_t n, uint8_t* d_out, std::string* err);
+  // ---- LookupResources on the sharded store (dist.DeviceShardedLookup): one round of K <= 64 lookups at a time ----
+  // Starts a round (the same lookups on every rank; home[k] = rank that asked lookup k) and clears its visited slices.
+  // d_seeds receives the K level-0 frontier entries; walk_cap bounds every frontier and the walk's candidates.
+  int shard_lookup_begin(const std::vector<LookupReq>& reqs, const uint8_t* home, uint64_t walk_cap,
+                         unsigned long long* d_seeds, std::string* err);
+  // Expands the n_in entries of d_front (level `level` of the replicated frontier) against this shard's reverse rows
+  // into d_next (walk_cap entries). *overflow: the frontier or the candidates did not fit.
+  int shard_lookup_expand(const unsigned long long* d_front, uint64_t n_in, int level, unsigned long long* d_next,
+                          uint64_t* n_next, bool* overflow, std::string* err);
+  // The round's candidates on this shard as check items: the walk's (exhaustive: every owned resource of the type)
+  // plus the self-membership of owned userset subjects. d_items == nullptr: *n = the capacity d_items needs.
+  int shard_lookup_candidates(bool exhaustive, zg_check* d_items, uint64_t cap, uint64_t* n, std::string* err);
+  // Codes of the candidates -> answer keys (lookup << 32 | id; undecidable ones flagged) in d_routed, bucketed by home
+  // rank; counts[d] (host) = keys for rank d.
+  int shard_lookup_route(const uint8_t* d_codes, uint64_t n, uint32_t n_dest, unsigned long long* d_routed, uint64_t* counts,
+                         std::string* err);
+  // Keys that arrived home -> d_ids, ascending per lookup in lookup order; per_lookup[k] (host, K) = answers of
+  // lookup k; *err_mask bit k: lookup k had an undecidable candidate.
+  int shard_lookup_finish(const unsigned long long* d_keys, uint64_t n, uint32_t* d_ids, uint64_t* per_lookup,
+                          uint64_t* err_mask, std::string* err);
 
   std::shared_ptr<Snapshot> snap;
   cudaStream_t stream = nullptr;
@@ -166,6 +186,16 @@ class Device {
   DevBuf rb_visited_, rb_front_[2], rb_cand_;
   DevBuf lb_params_, lb_owner_, lb_ctrl_, lb_keys_[2];  // batched lookups
   DevBuf ls_jobs_, ls_codes_, ls_has_, ls_ids_, ls_ctrl_;   // LookupSubjects
+  // sharded LookupResources round: walk state in rb_visited_ / lk_jobs_ / lb_owner_ / lb_params_ / lb_keys_ (a sharded
+  // engine never runs lookup_batch), the round's home ranks, self-membership list and control words here
+  DevBuf sl_home_, sl_self_, sl_ctrl_;
+  std::shared_ptr<Snapshot> sl_snap_;  // the round reads one snapshot from begin to finish (released there)
+  std::vector<LookupReq> sl_reqs_;
+  uint64_t sl_cap_ = 0, sl_n_cand_ = 0;
+  uint64_t sl_n_walk_ = 0;  // candidates before the self-membership ones: only these can fail a lookup
+  template <bool kSrc, class Item, class Owner>
+  int route_(const Item* d_items, uint64_t n, uint32_t n_dest, Owner owner, Item* d_routed, uint32_t* d_src, uint64_t* counts,
+             std::string* err);
   bool no_wildcards_ = false;  // run_pass: KParams::no_wildcards (LookupSubjects' second verification)
   uint64_t lb_cap_ = 1ull << 24;  // frontier entries / candidates of one lookup batch (ZGPU_LOOKUP_BATCH_CAP)
   void* pin_lk_ = nullptr;

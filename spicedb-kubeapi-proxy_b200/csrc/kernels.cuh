@@ -1053,28 +1053,36 @@ __global__ void or_children_kernel(const uint32_t* parent, const uint8_t* child_
 // owner(item) = item.res % n_dest. Two passes of a counting sort: per-destination counts (shared-memory
 // histogram, one atomic per block and destination), then a scatter that writes every item behind its
 // destination's cursor together with its source index, so that the values coming back in ROUTED order can be
-// folded into the (query, leaf) that raised them without un-permuting anything.
+// folded into the (query, leaf) that raised them without un-permuting anything. The owner is a functor: the
+// sharded LookupResources routes its answer keys home with the same two kernels (KeyHomeOwner below).
 constexpr int kMaxRouteDest = 64;
-__global__ void __launch_bounds__(256) route_count_kernel(const zg_check* items, unsigned long long n, uint32_t n_dest,
-                                                          unsigned long long* counts) {
+struct ResOwner {
+  __device__ __forceinline__ uint32_t operator()(const zg_check& it, uint32_t n_dest) const { return it.res % n_dest; }
+};
+template <class Item = zg_check, class Owner = ResOwner>
+__global__ void __launch_bounds__(256) route_count_kernel(const Item* items, unsigned long long n, uint32_t n_dest,
+                                                          unsigned long long* counts, Owner owner = Owner{}) {
   ZG_BLOCK_SHARED_U32(hist, kMaxRouteDest);
   for (uint32_t i = threadIdx.x; i < n_dest; i += blockDim.x) hist[i] = 0;
   __syncthreads();
   const unsigned long long stride = static_cast<unsigned long long>(gridDim.x) * blockDim.x;
   for (unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x; i < n; i += stride)
-    atomicAdd(&hist[items[i].res % n_dest], 1u);
+    atomicAdd(&hist[owner(items[i], n_dest)], 1u);
   __syncthreads();
   for (uint32_t i = threadIdx.x; i < n_dest; i += blockDim.x)
     if (hist[i]) atomicAdd(counts + i, static_cast<unsigned long long>(hist[i]));
 }
-__global__ void __launch_bounds__(256) route_scatter_kernel(const zg_check* items, unsigned long long n, uint32_t n_dest,
-                                                            unsigned long long* cursor, zg_check* routed, uint32_t* src) {
+// kSrc = false: nothing is folded back in routed order, src is not written (and may be null)
+template <class Item = zg_check, class Owner = ResOwner, bool kSrc = true>
+__global__ void __launch_bounds__(256) route_scatter_kernel(const Item* items, unsigned long long n, uint32_t n_dest,
+                                                            unsigned long long* cursor, Item* routed, uint32_t* src,
+                                                            Owner owner = Owner{}) {
   const unsigned long long stride = static_cast<unsigned long long>(gridDim.x) * blockDim.x;
   for (unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x; i < n; i += stride) {
-    const zg_check it = items[i];
-    const unsigned long long at = atomicAdd(cursor + (it.res % n_dest), 1ull);
+    const Item it = items[i];
+    const unsigned long long at = atomicAdd(cursor + owner(it, n_dest), 1ull);
     routed[at] = it;
-    src[at] = static_cast<uint32_t>(i);
+    if constexpr (kSrc) src[at] = static_cast<uint32_t>(i);
   }
 }
 // values of routed sub-queries (routed order) OR-ed into the (query, leaf) that raised sub-query src[i]
@@ -1286,24 +1294,30 @@ __global__ void __launch_bounds__(256) mrbfs_expand_kernel(const MrbfsParams p) 
 }
 
 // HAS candidates -> keys (owner << 32 | resource id), compacted; per-lookup result counts; lookups with an
-// undecidable candidate (ITEM_ERROR) are flagged in err_mask.
+// undecidable candidate (ITEM_ERROR) are flagged in err_mask. err_below: ITEM_ERROR candidates i < err_below become
+// keys too, with bit kErrKeyBit set, so that the flag travels with the answers (sharded LookupResources sends them
+// home; its self-membership candidates come after the walk's and, as on a replica, are left out when undecidable).
+constexpr int kErrKeyBit = 38;  // just above the lookup index (< kMaxLookupBatch = 2^6) in the high word
 __global__ void lookup_keys_kernel(const zg_check* cand, const uint8_t* owner, const uint8_t* codes, unsigned long long n,
                                    unsigned long long* keys, unsigned long long* n_keys, unsigned long long* per_lookup,
-                                   unsigned long long* err_mask) {
+                                   unsigned long long* err_mask, unsigned long long err_below = 0) {
   unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x;
   const bool in = i < n;
   const uint8_t code = in ? codes[i] : 0;
   const bool has = code == ZG_HAS_PERMISSION;
-  if (in && code == ZG_ITEM_ERROR) atomicOr(err_mask, 1ull << owner[i]);
-  const unsigned m = __ballot_sync(kFull, has);
+  const bool bad = in && code == ZG_ITEM_ERROR;
+  if (bad) atomicOr(err_mask, 1ull << owner[i]);
+  const bool emit = has || (bad && i < err_below);
+  const unsigned m = __ballot_sync(kFull, emit);
   if (!m) return;
   const unsigned lane = threadIdx.x & 31;
   unsigned long long base = 0;
   if (lane == 0) base = atomicAdd(n_keys, static_cast<unsigned long long>(__popc(m)));
   base = __shfl_sync(kFull, base, 0);
-  if (has) {
-    keys[base + __popc(m & ((1u << lane) - 1u))] = (static_cast<unsigned long long>(owner[i]) << 32) | cand[i].res;
-    atomicAdd(per_lookup + owner[i], 1ull);
+  if (emit) {
+    keys[base + __popc(m & ((1u << lane) - 1u))] = (static_cast<unsigned long long>(bad) << kErrKeyBit) |
+                                                   (static_cast<unsigned long long>(owner[i]) << 32) | cand[i].res;
+    if (has) atomicAdd(per_lookup + owner[i], 1ull);
   }
 }
 __global__ void low_words_kernel(const unsigned long long* keys, unsigned long long n, uint32_t* out) {
@@ -1367,6 +1381,86 @@ __global__ void lookup_compact_kernel(const uint32_t* cand, const uint8_t* codes
     const unsigned long long at = base + __popc(m & ((1u << lane) - 1u));
     if (at < cap) out[at] = cand[i];
   }
+}
+
+// ---- LookupResources on the object-hash sharded store (dist.DeviceShardedLookup) ------------------------------
+//
+// Shard k holds the reverse rows of the relationships whose resource it owns, so every object it discovers with
+// mrbfs_expand_kernel is its own: each rank keeps its own visited slices, each object enters the replicated frontier
+// once, and candidates start on their owner. The kernels below complete the candidates, send the verified ones
+// home and split them per lookup there.
+
+// Answer keys (lookup << 32 | id, kErrKeyBit for an undecidable candidate) go to the rank that asked the lookup.
+struct KeyHomeOwner {
+  const uint8_t* home;  // per lookup of the round
+  __device__ __forceinline__ uint32_t operator()(unsigned long long key, uint32_t) const {
+    return home[(key >> 32) & (kMaxLookupBatch - 1)];
+  }
+};
+
+// A userset subject T:x#r of a lookup of type T whose object x this shard owns; bit: x's bit in the lookup's visited
+// slice, ~0 when x is no object of this shard (the walk cannot have reached it).
+struct SelfCand {
+  uint32_t k, pad;
+  unsigned long long bit;
+};
+// x becomes a candidate of its own lookup unless the walk (or the exhaustive fill) already made it one
+__global__ void lookup_self_kernel(const LookupParam* lk, const SelfCand* self, uint32_t n_self, const uint32_t* visited,
+                                   unsigned long long words, zg_check* cand, uint8_t* cand_owner, unsigned long long* cand_count) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n_self) return;
+  const SelfCand s = self[i];
+  if (s.bit != ~0ull && ((visited[s.k * words + (s.bit >> 5)] >> (s.bit & 31)) & 1u)) return;
+  const LookupParam l = lk[s.k];
+  zg_check q;
+  q.res = l.subj;
+  q.subj = l.subj;
+  q.perm = l.perm;
+  q.stype = l.stype;
+  q.srel = l.srel;
+  q.flags = 0;
+  const unsigned long long at = atomicAdd(cand_count, 1ull);
+  cand[at] = q;
+  cand_owner[at] = static_cast<uint8_t>(s.k);
+}
+
+// Exhaustive candidates of lookup k (its walk overflowed): every resource of its type this shard owns, marked in
+// the lookup's visited slice (cleared by the caller) so that lookup_self_kernel does not add one of them twice.
+__global__ void lookup_fill_owned_kernel(const uint32_t* res, unsigned long long n, LookupParam l, uint32_t k, uint32_t* vis,
+                                         unsigned long long bit_base, zg_check* cand, uint8_t* cand_owner) {
+  const unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t r = res[i];
+  zg_check q;
+  q.res = r;
+  q.subj = l.subj;
+  q.perm = l.perm;
+  q.stype = l.stype;
+  q.srel = l.srel;
+  q.flags = 0;
+  cand[i] = q;
+  cand_owner[i] = static_cast<uint8_t>(k);
+  const unsigned long long bit = bit_base + r;
+  atomicOr(vis + (bit >> 5), 1u << (bit & 31));
+}
+
+// Keys that arrived home, sorted: the answers in (lookup, id) order, then the error keys. ids[i] = id of answer i;
+// lookup k's answers are ids[first[k] .. end[k]) (both left 0 for a lookup without answers); err_mask: lookups with
+// an undecidable candidate.
+__global__ void lookup_split_kernel(const unsigned long long* keys, unsigned long long n, uint32_t* ids,
+                                    unsigned long long* first, unsigned long long* end, unsigned long long* err_mask) {
+  const unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x;
+  if (i >= n) return;
+  const unsigned long long key = keys[i];
+  const uint32_t k = static_cast<uint32_t>(key >> 32) & (kMaxLookupBatch - 1);
+  if ((key >> kErrKeyBit) & 1ull) {
+    atomicOr(err_mask, 1ull << k);
+    return;
+  }
+  ids[i] = static_cast<uint32_t>(key);
+  const unsigned long long run = key >> 32;  // lookup and error bit: a run of answers ends at either change
+  if (i == 0 || (keys[i - 1] >> 32) != run) first[k] = i;
+  if (i + 1 == n || (keys[i + 1] >> 32) != run) end[k] = i + 1;
 }
 
 // ---- LookupSubjects: forward walk from the resource (the mirror of mrbfs_expand_kernel) -------------------

@@ -15,6 +15,8 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
+from ._lib import CHECK_DTYPE
+
 
 def shard_bounds(n: int, rank: int, world: int):
     """Contiguous, balanced slice of n items for this rank."""
@@ -348,3 +350,118 @@ class DeviceShardedChecker:
         answers = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
         self.e.shard_unroute_dev(levels[0]["src"].data_ptr() if n else 0, home.data_ptr() if n else 0, n, answers.data_ptr())
         return answers[:n]
+
+
+# ---------------------------------------------------------------------------------------------
+# LookupResources over the object-hash sharded store (DESIGN.md 4 and 7).
+#
+# Shard k holds the relationships whose resource it owns, so every object it discovers in its own reverse rows is
+# an object it owns: each rank dedups what it discovers with its own visited slices, and each object enters the
+# frontier once. A level is a local expand of the WHOLE replicated frontier on every rank, then an all-gather of
+# the new entries (one count exchange that also carries the overflow flag, one all-to-all). Candidates start on
+# their owner, are verified by the sharded check protocol, and the answers go home with one more all-to-all.
+
+MAX_DEPTH = 50  # ZG_MAX_DEPTH (include/zgpu.h): the walk expands levels 0 .. MAX_DEPTH + 1, as a replica's does
+LOOKUP_ROUND = 64  # lookups per round (visited slices; the lookup index in an answer key has 6 bits)
+
+
+class DeviceShardedLookup:
+    """LookupResources over an object-hash sharded store, device resident. `lookup_resources` is collective: every
+    rank brings its own list of requests (possibly empty) and gets one answer per request of its own."""
+
+    REQ = np.dtype([("subj", "<u4"), ("res_type", "<u2"), ("perm", "<u2"), ("stype", "<u2"), ("srel", "<u2")])
+
+    def __init__(self, engine, transport, walk_cap: int = 1 << 22, checker: DeviceShardedChecker | None = None,
+                 verify_chunk: int = 1 << 16):
+        """walk_cap: entries of a frontier and of the walk's candidates on one rank; a round that overflows it is
+        redone in halves, and a single lookup then verifies every resource of its type the rank owns. verify_chunk:
+        candidates per check_bulk call, so that their raised sub-queries fit the engine's sub-query buffer."""
+        self.e, self.t, self.walk_cap, self.verify_chunk = engine, transport, int(walk_cap), int(verify_chunk)
+        self.checker = checker or DeviceShardedChecker(engine, transport)
+        self.stats = {"rounds": 0, "levels": 0, "frontier_entries": 0, "frontier_bytes": 0, "bytes_sent": 0,
+                      "candidates": 0, "fallbacks": 0, "halvings": 0}
+
+    def lookup_resources(self, reqs) -> list:
+        """reqs: [(res_type_id, perm_slot, subj_type_id, subj_id, subj_rel_slot)] of this rank (subj_rel_slot = SREL_NONE
+        for a plain subject). -> per request an ascending uint32 array of resource ids, or None where
+        zg_lookup_resources would return ZG_EDEPTH (a candidate could not be decided)."""
+        t, w = self.t, self.t.world
+        mine = np.zeros(len(reqs), self.REQ)
+        for i, (rt, perm, st, subj, srel) in enumerate(reqs):
+            mine[i] = (subj, rt, perm, st, srel)
+        counts = t.exchange_counts([mine.size] * w)  # requests of every rank, in rank order
+        send = torch.from_numpy(np.tile(mine.view(np.uint8), w)).to(t.device)
+        got = t.alltoall(send, [mine.size] * w, counts, self.REQ.itemsize)
+        self.stats["bytes_sent"] += mine.size * self.REQ.itemsize * (w - 1)
+        every = got.cpu().numpy().view(self.REQ)
+        home = np.repeat(np.arange(w, dtype=np.uint8), counts)
+        out = [None] * mine.size
+        first = sum(counts[: t.rank])
+        for lo in range(0, every.size, LOOKUP_ROUND):
+            self._round(every[lo:lo + LOOKUP_ROUND], home[lo:lo + LOOKUP_ROUND], lo - first, out)
+        return out
+
+    def _round(self, reqs, home, base, out):
+        """One round of <= 64 lookups on every rank; answers of this rank's lookups go to out[base + k]."""
+        t, w, dev = self.t, self.t.world, self.t.device
+        K = reqs.size
+        self.stats["rounds"] += 1
+        protos = np.zeros(K, CHECK_DTYPE)
+        protos["subj"], protos["perm"], protos["stype"], protos["srel"] = reqs["subj"], reqs["perm"], reqs["stype"], reqs["srel"]
+        front = torch.empty(K * 8, dtype=torch.uint8, device=dev)
+        nxt = torch.empty(self.walk_cap * 8, dtype=torch.uint8, device=dev)
+        self.e.shard_lookup_begin_dev(reqs["res_type"], protos, home, self.walk_cap, front.data_ptr())
+        n_in, level, overflow = K, 0, False
+        while True:
+            n_out, ovf = self.e.shard_lookup_expand_dev(front.data_ptr(), n_in, level, nxt.data_ptr())
+            got = t.exchange_counts([2 * n_out + int(ovf)] * w)  # new entries, overflow flag in bit 0
+            self.stats["levels"] += 1
+            if any(g & 1 for g in got):
+                overflow = True
+                break
+            rc = [g >> 1 for g in got]
+            n_in = sum(rc)
+            if n_in == 0 or level == MAX_DEPTH + 1:
+                break
+            # all-gather: this rank's new entries to every rank (itself included), the gathered frontier back
+            front = t.alltoall(nxt[: n_out * 8].repeat(w), [n_out] * w, rc, 8)
+            self.stats["frontier_entries"] += n_out
+            self.stats["frontier_bytes"] += n_out * 8 * (w - 1)
+            level += 1
+        if overflow and K > 1:
+            self.stats["halvings"] += 1
+            h = K // 2
+            self._round(reqs[:h], home[:h], base, out)
+            self._round(reqs[h:], home[h:], base + h, out)
+            return
+        if overflow:
+            self.stats["fallbacks"] += 1
+        need = self.e.shard_lookup_candidates_dev(overflow, 0, 0)
+        items = torch.empty(max(need, 1) * DeviceShardedChecker.ITEM, dtype=torch.uint8, device=dev)
+        n = self.e.shard_lookup_candidates_dev(overflow, items.data_ptr(), need)
+        self.stats["candidates"] += n
+        # verified in chunks that bound the check protocol's sub-query buffers; every rank runs as many chunks as
+        # the rank with the most candidates (check_bulk is collective)
+        codes = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
+        item = DeviceShardedChecker.ITEM
+        for lo in range(0, max(t.exchange_counts([n] * w)), self.verify_chunk):
+            m = max(0, min(self.verify_chunk, n - lo))
+            codes[lo:lo + m] = self.checker.check_bulk(items[lo * item:(lo + m) * item] if m else items, m)
+        # the copies into `codes` run on torch's stream, the engine reads `codes` on its own: they must have landed
+        # (and the chunks' answer tensors they read must not be handed out again) before the engine's next call
+        if dev.type == "cuda":
+            torch.cuda.current_stream().synchronize()
+        routed = torch.empty(max(n, 1) * 8, dtype=torch.uint8, device=dev)
+        sc = self.e.shard_lookup_route_dev(codes.data_ptr() if n else 0, n, w, routed.data_ptr())
+        rc = t.exchange_counts(sc)
+        keys = t.alltoall(routed[: sum(sc) * 8], sc, rc, 8)
+        self.stats["bytes_sent"] += (sum(sc) - sc[t.rank]) * 8
+        nk = sum(rc)
+        ids = torch.empty(max(nk, 1) * 4, dtype=torch.uint8, device=dev)
+        per, err = self.e.shard_lookup_finish_dev(keys.data_ptr() if nk else 0, nk, ids.data_ptr(), K)
+        host = ids[: sum(per) * 4].cpu().numpy().view(np.uint32)
+        off = 0
+        for k in range(K):
+            if home[k] == t.rank:
+                out[base + k] = None if (err >> k) & 1 else host[off:off + per[k]].copy()
+            off += per[k]
