@@ -266,7 +266,8 @@ int zg_lookup_resources_str(zg_engine *e, const char *res_type, const char *perm
  * wildcard entry is left out. Candidates come from a forward walk of the resident snapshot from res
  * (every object of stype when the walk overflows), verified by the check kernel. Returns 0; ZG_E2BIG
  * with *n_out / *n_excluded = required sizes; ZG_EDEPTH when a subject cannot be decided (depth cap /
- * work budget); ZG_EINVAL for unknown ids, or on a sharded engine; ZG_ECUDA on a host-only engine.
+ * work budget); ZG_EINVAL for unknown ids; ZG_ECUDA on a host-only engine. A sharded engine refuses this
+ * call and the string form (ZG_EINVAL): use the zg_shard_subjects_*_dev calls (dist.DeviceShardedLookup).
  * A resource id that no relationship names gives an empty answer. No caveats, limits or cursors. */
 #define ZG_WILDCARDS_INCLUDE 0u /* v1.LookupSubjectsRequest WILDCARD_OPTION_UNSPECIFIED / INCLUDE_WILDCARDS */
 #define ZG_WILDCARDS_EXCLUDE 1u /* v1.LookupSubjectsRequest WILDCARD_OPTION_EXCLUDE_WILDCARDS               */
@@ -299,8 +300,8 @@ int zg_debug_row(zg_engine *e, uint16_t rel_slot, uint32_t res, uint32_t cls, ui
  * into a non-pure permission) is raised as a sub-query. The host runs the ranks pass by pass
  * and exchanges the raised sub-queries (all-to-all) until none are left, then folds the values
  * back level by level (spicedb-kubeapi-proxy_b200/dist.py ShardedStoreChecker). On sharded
- * engines zg_check_bulk / zg_lookup_resources are refused: use these three calls (checks) or the
- * zg_shard_lookup_*_dev calls below (LookupResources). */
+ * engines zg_check_bulk / zg_lookup_resources / zg_lookup_subjects are refused: use these three calls (checks),
+ * the zg_shard_lookup_*_dev calls below (LookupResources) or the zg_shard_subjects_*_dev calls (LookupSubjects). */
 int zg_shard_pass(zg_engine *e, const zg_check *queries, uint64_t n, int level, uint64_t *n_sub);
 /* The sub-queries pass `level` raised, in emission order (same layout; flags = hop depth). */
 int zg_shard_subqueries(zg_engine *e, int level, zg_check *out, uint64_t n);
@@ -356,6 +357,54 @@ int zg_shard_lookup_route_dev(zg_engine *e, const uint8_t *d_codes, uint64_t n, 
                               uint64_t *counts);
 int zg_shard_lookup_finish_dev(zg_engine *e, const uint64_t *d_keys, uint64_t n, uint32_t *d_ids, uint64_t *per_lookup,
                                uint64_t *err_mask);
+
+/* LookupSubjects on a sharded engine (dist.DeviceShardedLookup.lookup_subjects), in rounds of k <= 64 lookups that
+ * every rank runs with the same list; the answers are zg_lookup_subjects' on a replica. Shard r holds the forward rows
+ * of the objects it owns, but their subjects can be owned by any shard: each level, every rank expands its own
+ * frontier, routes the subjects it finds to their owners (one all-to-all), and the owner admits each object once per
+ * lookup. Candidates are verified by the sharded check protocol, a second time with zg_shard_pass_nowild_dev when
+ * the wildcard is granted, and the answers are sent to the rank that asked the lookup. A round ends a LookupResources
+ * round begun on the same engine, and the other way round. Same conventions as the zg_shard_lookup_*_dev calls.
+ *   zg_shard_pass_nowild_dev         zg_shard_pass_dev with every wildcard relationship invisible
+ *   zg_shard_subjects_begin_dev      starts a round: res_types, reqs (res, perm of that type, stype, srel), options
+ *                                    (ZG_WILDCARDS_*) and home (rank that asked) are HOST arrays of k; the
+ *                                    owner of each resource puts it in d_front (device, walk_cap entries, *n_front)
+ *   zg_shard_subjects_expand_dev     expands the n_in entries of this rank's frontier d_front over its forward rows;
+ *                                    the subjects found go to d_routed (walk_cap entries) bucketed by owner (id % n_dest),
+ *                                    counts[d] (HOST, n_dest); *overflow = 1 when an outbox, a frontier or the
+ *                                    candidates did not fit in this round so far (redo it in halves; a single lookup
+ *                                    verifies every object of the subject type instead), and nothing is routed
+ *   zg_shard_subjects_admit_dev      the n_in entries that arrived from every rank -> the fresh ones in d_next
+ *                                    (walk_cap entries), *n_next; fresh objects of the subject type become candidates
+ *   zg_shard_subjects_candidates_dev this rank's check items: the probe of each owned resource (subject
+ *                                    ZG_NO_OBJECT - 1), then the walk's candidates, or with exhaustive every owned id
+ *                                    of the subject type; with d_items NULL, *n = the capacity needed; ZG_E2BIG when
+ *                                    cap is smaller
+ *   zg_shard_subjects_verdicts_dev   d_codes (one per item) -> *granted bit i: lookup i's probe checks HAS without a
+ *                                    subject relation; *failed bit i: an item of lookup i is undecidable (ZG_EDEPTH)
+ *   zg_shard_subjects_nowild_dev     with every rank's masks OR-ed: the HAS candidates of granted lookups -> d_items
+ *                                    (cap >= the candidates), *n_nw, for the no-wildcards verification
+ *   zg_shard_subjects_route_dev      d_codes of that verification (one per item) -> answer keys (excluded << 38 |
+ *                                    lookup << 32 | id) in d_routed (the candidates' count), bucketed by home rank;
+ *                                    counts[d] (HOST, n_dest)
+ *   zg_shard_subjects_finish_dev     the keys that arrived home -> d_ids: the listed ids of lookup 0, 1, ... then the
+ *                                    excluded ids of lookup 0, 1, ..., ascending each; listed[i] / excluded[i] (HOST,
+ *                                    k) = their counts. The wildcard entry of lookup i is present when it is granted,
+ *                                    not failed, and asked for with ZG_WILDCARDS_INCLUDE. */
+int zg_shard_pass_nowild_dev(zg_engine *e, const zg_check *d_queries, uint64_t n, int level, uint64_t *n_sub);
+int zg_shard_subjects_begin_dev(zg_engine *e, const uint16_t *res_types, const zg_check *reqs, const uint32_t *options,
+                                const uint8_t *home, uint32_t k, uint64_t walk_cap, uint64_t *d_front, uint64_t *n_front);
+int zg_shard_subjects_expand_dev(zg_engine *e, const uint64_t *d_front, uint64_t n_in, uint32_t n_dest, uint64_t *d_routed,
+                                 uint64_t *counts, int *overflow);
+int zg_shard_subjects_admit_dev(zg_engine *e, const uint64_t *d_in, uint64_t n_in, uint64_t *d_next, uint64_t *n_next);
+int zg_shard_subjects_candidates_dev(zg_engine *e, int exhaustive, zg_check *d_items, uint64_t cap, uint64_t *n);
+int zg_shard_subjects_verdicts_dev(zg_engine *e, const uint8_t *d_codes, uint64_t n, uint64_t *granted, uint64_t *failed);
+int zg_shard_subjects_nowild_dev(zg_engine *e, const uint8_t *d_codes, uint64_t n, uint64_t granted, uint64_t failed,
+                                 zg_check *d_items, uint64_t cap, uint64_t *n_nw);
+int zg_shard_subjects_route_dev(zg_engine *e, const uint8_t *d_codes, uint64_t n, uint32_t n_dest, uint64_t *d_routed,
+                                uint64_t *counts);
+int zg_shard_subjects_finish_dev(zg_engine *e, const uint64_t *d_keys, uint64_t n, uint32_t *d_ids, uint64_t *listed,
+                                 uint64_t *excluded);
 
 /* Watch feed (v1.WatchServiceClient.Watch, pkg/authz/watch.go:27-48): the relationship changes made
  * visible by revisions > since_revision, oldest first, as '\n'-separated lines

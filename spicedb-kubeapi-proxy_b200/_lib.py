@@ -191,6 +191,19 @@ _SIGS = {
     "zg_shard_lookup_route_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p]),
     "zg_shard_lookup_finish_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
                                              C.POINTER(C.c_uint64)]),
+    "zg_shard_pass_nowild_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.POINTER(C.c_uint64)]),
+    "zg_shard_subjects_begin_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
+                                              C.c_uint64, C.c_void_p, C.POINTER(C.c_uint64)]),
+    "zg_shard_subjects_expand_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p,
+                                               C.POINTER(C.c_int)]),
+    "zg_shard_subjects_admit_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.POINTER(C.c_uint64)]),
+    "zg_shard_subjects_candidates_dev": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),
+    "zg_shard_subjects_verdicts_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64),
+                                                 C.POINTER(C.c_uint64)]),
+    "zg_shard_subjects_nowild_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint64, C.c_void_p,
+                                               C.c_uint64, C.POINTER(C.c_uint64)]),
+    "zg_shard_subjects_route_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p]),
+    "zg_shard_subjects_finish_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "zg_debug_row": (C.c_int, [C.c_void_p, C.c_uint16, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64,
                                C.POINTER(C.c_uint64)]),
     "zg_host_alloc": (C.c_void_p, [C.c_size_t]),
@@ -704,6 +717,67 @@ class Engine:
         mask = C.c_uint64(0)
         self._ck(self._L.zg_shard_lookup_finish_dev(self._h, d_keys or None, n, d_ids or None, per, C.byref(mask)))
         return [int(per[i]) for i in range(k)], mask.value
+
+    def shard_pass_nowild_dev(self, d_queries: int, n: int, level: int) -> int:
+        """shard_pass_dev with every wildcard relationship invisible (LookupSubjects' second verification)."""
+        ns = C.c_uint64(0)
+        self._ck(self._L.zg_shard_pass_nowild_dev(self._h, d_queries or None, n, level, C.byref(ns)))
+        return ns.value
+
+    # sharded LookupSubjects (dist.DeviceShardedLookup.lookup_subjects drives these): one round of <= 64 lookups at a time
+    def shard_subjects_begin_dev(self, res_types, reqs, options, home, walk_cap: int, d_front: int) -> int:
+        """res_types (uint16), reqs (CHECK_DTYPE: res, perm, stype, srel), options (uint32 ZG_WILDCARDS_*), home (uint8):
+        host arrays of k. -> entries of this rank's level-0 frontier."""
+        rt = np.ascontiguousarray(res_types, dtype=np.uint16)
+        rq = np.ascontiguousarray(reqs, dtype=CHECK_DTYPE)
+        op = np.ascontiguousarray(options, dtype=np.uint32)
+        hm = np.ascontiguousarray(home, dtype=np.uint8)
+        n = C.c_uint64(0)
+        self._ck(self._L.zg_shard_subjects_begin_dev(self._h, rt.ctypes.data, rq.ctypes.data, op.ctypes.data, hm.ctypes.data,
+                                                     rq.size, walk_cap, d_front or None, C.byref(n)))
+        return n.value
+
+    def shard_subjects_expand_dev(self, d_front: int, n_in: int, n_dest: int, d_routed: int):
+        """-> (entries per destination rank, overflow)"""
+        counts = (C.c_uint64 * n_dest)()
+        ovf = C.c_int(0)
+        self._ck(self._L.zg_shard_subjects_expand_dev(self._h, d_front or None, n_in, n_dest, d_routed or None, counts,
+                                                      C.byref(ovf)))
+        return [int(c) for c in counts], bool(ovf.value)
+
+    def shard_subjects_admit_dev(self, d_in: int, n_in: int, d_next: int) -> int:
+        n = C.c_uint64(0)
+        self._ck(self._L.zg_shard_subjects_admit_dev(self._h, d_in or None, n_in, d_next or None, C.byref(n)))
+        return n.value
+
+    def shard_subjects_candidates_dev(self, exhaustive: bool, d_items: int, cap: int) -> int:
+        """d_items == 0: the capacity needed; else the candidates written."""
+        n = C.c_uint64(0)
+        self._ck(self._L.zg_shard_subjects_candidates_dev(self._h, 1 if exhaustive else 0, d_items or None, cap, C.byref(n)))
+        return n.value
+
+    def shard_subjects_verdicts_dev(self, d_codes: int, n: int):
+        """-> (granted mask, failed mask) of this rank's items"""
+        g, f = C.c_uint64(0), C.c_uint64(0)
+        self._ck(self._L.zg_shard_subjects_verdicts_dev(self._h, d_codes or None, n, C.byref(g), C.byref(f)))
+        return g.value, f.value
+
+    def shard_subjects_nowild_dev(self, d_codes: int, n: int, granted: int, failed: int, d_items: int, cap: int) -> int:
+        m = C.c_uint64(0)
+        self._ck(self._L.zg_shard_subjects_nowild_dev(self._h, d_codes or None, n, granted, failed, d_items or None, cap,
+                                                      C.byref(m)))
+        return m.value
+
+    def shard_subjects_route_dev(self, d_codes: int, n: int, n_dest: int, d_routed: int) -> list:
+        counts = (C.c_uint64 * n_dest)()
+        self._ck(self._L.zg_shard_subjects_route_dev(self._h, d_codes or None, n, n_dest, d_routed or None, counts))
+        return [int(c) for c in counts]
+
+    def shard_subjects_finish_dev(self, d_keys: int, n: int, d_ids: int, k: int):
+        """-> (listed ids per lookup, excluded ids per lookup) of the round"""
+        listed, excluded = (C.c_uint64 * max(k, 1))(), (C.c_uint64 * max(k, 1))()
+        self._ck(self._L.zg_shard_subjects_finish_dev(self._h, d_keys or None, n, d_ids or None, listed, excluded))
+        return [int(listed[i]) for i in range(k)], [int(excluded[i]) for i in range(k)]
 
     def debug_row(self, type_name, rel, res, cls=0, reverse=False) -> np.ndarray:
         """Forward row (resource `res`, class) or, reverse=True, the reverse row of subject `res`."""

@@ -1942,13 +1942,16 @@ extern "C" int zg_shard_unroute_dev(zg_engine* e, const uint32_t* d_src, const u
   return rc ? fail(rc, err) : ZG_OK;
 }
 
-// LookupResources on the sharded store: the same prologue, and only on a sharded engine
-#define SHARD_LOOKUP_PROLOGUE()                                                                                       \
+// LookupResources / LookupSubjects on the sharded store: the same prologue, and only on a sharded engine (the
+// message names the unsharded call)
+#define SHARD_ONLY_PROLOGUE(unsharded_msg)                                                                            \
   NEED_SCHEMA(e, ZG_ENOSCHEMA);                                                                                       \
   std::lock_guard<FairMutex> g(e->mu);                                                                               \
   if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");      \
-  if (e->dev.shard_count < 2) return fail(ZG_EINVAL, "not a sharded engine: use zg_lookup_resources");               \
+  if (e->dev.shard_count < 2) return fail(ZG_EINVAL, unsharded_msg);                                                 \
   if (!e->dev.snap) return fail(ZG_ENOSNAPSHOT, "no snapshot published (call zg_publish)");
+#define SHARD_LOOKUP_PROLOGUE() SHARD_ONLY_PROLOGUE("not a sharded engine: use zg_lookup_resources")
+#define SHARD_SUBJECTS_PROLOGUE() SHARD_ONLY_PROLOGUE("not a sharded engine: use zg_lookup_subjects")
 
 extern "C" int zg_shard_lookup_begin_dev(zg_engine* e, const uint16_t* res_types, const zg_check* protos, const uint8_t* home,
                                          uint32_t k, uint64_t walk_cap, uint64_t* d_seeds) {
@@ -1992,6 +1995,94 @@ extern "C" int zg_shard_lookup_finish_dev(zg_engine* e, const uint64_t* d_keys, 
   SHARD_LOOKUP_PROLOGUE();
   std::string err;
   int rc = e->dev.shard_lookup_finish(reinterpret_cast<const unsigned long long*>(d_keys), n, d_ids, per_lookup, err_mask, &err);
+  return rc ? fail(rc, err) : ZG_OK;
+}
+
+// LookupSubjects on the sharded store
+extern "C" int zg_shard_pass_nowild_dev(zg_engine* e, const zg_check* d_queries, uint64_t n, int level, uint64_t* n_sub) {
+  if ((!d_queries && n) || !n_sub || level < 0 || level > ZG_MAX_DEPTH + 2) return fail(ZG_EINVAL, "bad argument");
+  SHARD_SUBJECTS_PROLOGUE();
+  e->dev.now = now_of(e);
+  std::string err;
+  int rc = e->dev.shard_pass_nowild_dev(d_queries, n, level, n_sub, &err);
+  return rc ? fail(rc, err) : ZG_OK;
+}
+extern "C" int zg_shard_subjects_begin_dev(zg_engine* e, const uint16_t* res_types, const zg_check* reqs, const uint32_t* options,
+                                           const uint8_t* home, uint32_t k, uint64_t walk_cap, uint64_t* d_front, uint64_t* n_front) {
+  if (!res_types || !reqs || !options || !home || !d_front || !n_front) return fail(ZG_EINVAL, "NULL argument");
+  SHARD_SUBJECTS_PROLOGUE();
+  const Schema& sc = e->schema;
+  std::vector<Device::SubjectsReq> rs(k);
+  uint64_t include = 0;
+  for (uint32_t i = 0; i < k; ++i) {
+    const zg_check& q = reqs[i];
+    // as zg_lookup_subjects (the permission's slot also bounds the walk's mask read)
+    if (q.perm >= sc.slots.size() || sc.slots[q.perm].type != res_types[i]) return fail(ZG_EINVAL, "unknown permission of the resource type");
+    if (q.stype >= sc.types.size() || (q.srel != kNone && (q.srel >= sc.slots.size() || sc.slots[q.srel].type != q.stype)))
+      return fail(ZG_EINVAL, "unknown subject type or relation");
+    if (options[i] != ZG_WILDCARDS_INCLUDE && options[i] != ZG_WILDCARDS_EXCLUDE) return fail(ZG_EINVAL, "unknown wildcard option");
+    rs[i] = Device::SubjectsReq{q.res, res_types[i], q.perm, q.stype, q.srel};
+    if (options[i] == ZG_WILDCARDS_INCLUDE && i < 64) include |= 1ull << i;
+  }
+  std::string err;
+  int rc = e->dev.shard_subjects_begin(rs, home, include, walk_cap, reinterpret_cast<unsigned long long*>(d_front), n_front, &err);
+  return rc ? fail(rc, err) : ZG_OK;
+}
+extern "C" int zg_shard_subjects_expand_dev(zg_engine* e, const uint64_t* d_front, uint64_t n_in, uint32_t n_dest, uint64_t* d_routed,
+                                            uint64_t* counts, int* overflow) {
+  if ((!d_front && n_in) || !d_routed || !counts || !overflow) return fail(ZG_EINVAL, "NULL argument");
+  SHARD_SUBJECTS_PROLOGUE();
+  std::string err;
+  bool ovf = false;
+  int rc = e->dev.shard_subjects_expand(reinterpret_cast<const unsigned long long*>(d_front), n_in, n_dest,
+                                        reinterpret_cast<unsigned long long*>(d_routed), counts, &ovf, &err);
+  *overflow = ovf ? 1 : 0;
+  return rc ? fail(rc, err) : ZG_OK;
+}
+extern "C" int zg_shard_subjects_admit_dev(zg_engine* e, const uint64_t* d_in, uint64_t n_in, uint64_t* d_next, uint64_t* n_next) {
+  if ((!d_in && n_in) || !d_next || !n_next) return fail(ZG_EINVAL, "NULL argument");
+  SHARD_SUBJECTS_PROLOGUE();
+  std::string err;
+  int rc = e->dev.shard_subjects_admit(reinterpret_cast<const unsigned long long*>(d_in), n_in, reinterpret_cast<unsigned long long*>(d_next),
+                                       n_next, &err);
+  return rc ? fail(rc, err) : ZG_OK;
+}
+extern "C" int zg_shard_subjects_candidates_dev(zg_engine* e, int exhaustive, zg_check* d_items, uint64_t cap, uint64_t* n) {
+  if (!n) return fail(ZG_EINVAL, "NULL argument");
+  SHARD_SUBJECTS_PROLOGUE();
+  std::string err;
+  int rc = e->dev.shard_subjects_candidates(exhaustive != 0, d_items, cap, n, &err);
+  return rc ? fail(rc, err) : ZG_OK;
+}
+extern "C" int zg_shard_subjects_verdicts_dev(zg_engine* e, const uint8_t* d_codes, uint64_t n, uint64_t* granted, uint64_t* failed) {
+  if ((!d_codes && n) || !granted || !failed) return fail(ZG_EINVAL, "NULL argument");
+  SHARD_SUBJECTS_PROLOGUE();
+  std::string err;
+  int rc = e->dev.shard_subjects_verdicts(d_codes, n, granted, failed, &err);
+  return rc ? fail(rc, err) : ZG_OK;
+}
+extern "C" int zg_shard_subjects_nowild_dev(zg_engine* e, const uint8_t* d_codes, uint64_t n, uint64_t granted, uint64_t failed,
+                                            zg_check* d_items, uint64_t cap, uint64_t* n_nw) {
+  if (((!d_codes || !d_items) && n) || !n_nw) return fail(ZG_EINVAL, "NULL argument");
+  SHARD_SUBJECTS_PROLOGUE();
+  std::string err;
+  int rc = e->dev.shard_subjects_nowild(d_codes, n, granted, failed, d_items, cap, n_nw, &err);
+  return rc ? fail(rc, err) : ZG_OK;
+}
+extern "C" int zg_shard_subjects_route_dev(zg_engine* e, const uint8_t* d_codes, uint64_t n, uint32_t n_dest, uint64_t* d_routed,
+                                           uint64_t* counts) {
+  if (!counts || !d_routed || (!d_codes && n)) return fail(ZG_EINVAL, "NULL argument");
+  SHARD_SUBJECTS_PROLOGUE();
+  std::string err;
+  int rc = e->dev.shard_subjects_route(d_codes, n, n_dest, reinterpret_cast<unsigned long long*>(d_routed), counts, &err);
+  return rc ? fail(rc, err) : ZG_OK;
+}
+extern "C" int zg_shard_subjects_finish_dev(zg_engine* e, const uint64_t* d_keys, uint64_t n, uint32_t* d_ids, uint64_t* listed,
+                                            uint64_t* excluded) {
+  if (!listed || !excluded || ((!d_keys || !d_ids) && n)) return fail(ZG_EINVAL, "NULL argument");
+  SHARD_SUBJECTS_PROLOGUE();
+  std::string err;
+  int rc = e->dev.shard_subjects_finish(reinterpret_cast<const unsigned long long*>(d_keys), n, d_ids, listed, excluded, &err);
   return rc ? fail(rc, err) : ZG_OK;
 }
 

@@ -1018,6 +1018,7 @@ int Device::shard_lookup_begin(const std::vector<LookupReq>& reqs, const uint8_t
   std::shared_ptr<Snapshot> s = snap;
   const size_t K = reqs.size();
   sl_snap_.reset();
+  ss_snap_.reset();  // a sharded LookupSubjects round shares the walk buffers
   sl_n_cand_ = sl_n_walk_ = 0;
   if (!s) {
     if (err) *err = "no snapshot published";
@@ -1284,6 +1285,384 @@ int Device::shard_lookup_finish(const unsigned long long* d_keys, uint64_t n, ui
   ZG_CUDA(cudaStreamSynchronize(stream));
   *err_mask = host[0];
   for (size_t k = 0; k < K; ++k) per_lookup[k] = host[1 + kMaxLookupBatch + k] - host[1 + k];
+  return ZG_OK;
+}
+
+int Device::shard_pass_nowild_dev(const zg_check* d_queries, uint64_t n, int level, uint64_t* n_sub, std::string* err) {
+  no_wildcards_ = true;
+  const int rc = shard_pass_dev(d_queries, n, level, n_sub, err);
+  no_wildcards_ = false;
+  return rc;
+}
+
+// ---- LookupSubjects on the object-hash sharded store (DESIGN.md 4, dist.DeviceShardedLookup.lookup_subjects) -------
+// ss_ctrl_ words: [0] flags, [1] outbox entries, [2] admitted entries, [3] candidates, [4] keys, [5] no-wildcards
+// items, [6] granted mask, [7] failed mask, then first[] / end[] of the 128 answer runs after the final sort.
+namespace {
+constexpr size_t kSsFirst = 8, kSsEnd = kSsFirst + 2 * kMaxLookupBatch, kSsCtrlWords = kSsEnd + 2 * kMaxLookupBatch;
+
+SsWalkParams ss_walk_params(const Snapshot& s, const SubjectsParam* lk, uint32_t* visited, unsigned long long* ctrl, uint32_t rank,
+                            uint32_t count) {
+  SsWalkParams p{};
+  p.row_ptr = s.row_ptr.as<uint32_t>();
+  p.col = s.col.as<uint32_t>();
+  p.fwd = s.ls_fwd.as<FwdClass>();
+  p.type_off = s.ls_type_off.as<uint32_t>();
+  p.mask = s.ls_mask.as<uint32_t>();
+  p.mask_words = s.ls_mask_words;
+  p.shard_rank = rank;
+  p.shard_count = count;
+  p.lk = lk;
+  p.visited = visited;
+  p.words = (s.total_bits + 31) / 32 + 4;
+  p.type_bit_base = s.type_bit_base.as<unsigned long long>();
+  p.flags = reinterpret_cast<uint32_t*>(ctrl);
+  return p;
+}
+}  // namespace
+
+int Device::shard_subjects_begin(const std::vector<SubjectsReq>& reqs, const uint8_t* home, uint64_t include, uint64_t walk_cap,
+                                 unsigned long long* d_front, uint64_t* n_front, std::string* err) {
+  std::shared_ptr<Snapshot> s = snap;
+  const size_t K = reqs.size();
+  *n_front = 0;
+  ss_snap_.reset();
+  sl_snap_.reset();  // a sharded LookupResources round shares the walk buffers
+  ss_n_cand_ = ss_n_nw_ = 0;
+  if (!s) {
+    if (err) *err = "no snapshot published";
+    return ZG_ENOSNAPSHOT;
+  }
+  if (K == 0 || K > kMaxLookupBatch || walk_cap == 0 || shard_count > kMaxRouteDest) {
+    if (err) *err = "shard_subjects_begin: 1..64 lookups, a non-zero walk capacity and at most 64 shards";
+    return ZG_EINVAL;
+  }
+  for (size_t k = 0; k < K; ++k)
+    if (reqs[k].res_type >= s->n_objects.size() || reqs[k].stype >= s->n_objects.size() || home[k] >= shard_count) {
+      if (err) *err = "shard_subjects_begin: unknown type or home rank";
+      return ZG_EINVAL;
+    }
+  ZG_CUDA(cudaSetDevice(device));
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  const unsigned long long words = (s->total_bits + 31) / 32 + 4;
+  if (!rb_visited_.ensure(words * 4 * K) || !lk_jobs_.ensure((walk_cap + K) * sizeof(zg_check)) || !lb_owner_.ensure(walk_cap + K) ||
+      !lb_params_.ensure(K * sizeof(SubjectsParam)) || !ss_out_.ensure(std::max<uint64_t>(walk_cap, K) * 8) || !ss_home_.ensure(K) ||
+      !ss_ctrl_.ensure(kSsCtrlWords * 8)) {
+    if (err) *err = "out of device memory (sharded lookup buffers)";
+    return ZG_ENOMEM;
+  }
+  std::vector<SubjectsParam> lp(K);
+  std::vector<unsigned long long> seeds;
+  ss_probes_.clear();
+  ss_probe_owner_.clear();
+  for (size_t k = 0; k < K; ++k) {
+    const SubjectsReq& r = reqs[k];
+    lp[k] = SubjectsParam{r.res, r.res_type, r.perm, r.stype, r.srel};
+    // a resource no relationship names has an empty answer (n_objects is the same on every shard)
+    if (r.res >= s->n_objects[r.res_type] || r.res % shard_count != shard_rank) continue;
+    zg_check q{};
+    q.res = r.res;
+    q.subj = ZG_NO_OBJECT - 1;
+    q.perm = r.perm;
+    q.stype = r.stype;
+    q.srel = r.srel;
+    ss_probes_.push_back(q);
+    ss_probe_owner_.push_back(static_cast<uint8_t>(k));
+    seeds.push_back((static_cast<unsigned long long>(k) << 48) | (static_cast<unsigned long long>(r.res_type) << 32) | r.res);
+  }
+  const unsigned long long n_probe = ss_probes_.size();
+  unsigned long long* ctrl = ss_ctrl_.as<unsigned long long>();
+  ZG_CUDA(cudaMemsetAsync(ctrl, 0, kSsCtrlWords * 8, stream));
+  ZG_CUDA(cudaMemsetAsync(rb_visited_.p, 0, words * 4 * K, stream));
+  ZG_CUDA(cudaMemcpyAsync(lb_params_.p, lp.data(), K * sizeof(SubjectsParam), cudaMemcpyHostToDevice, stream));
+  ZG_CUDA(cudaMemcpyAsync(ss_home_.p, home, K, cudaMemcpyHostToDevice, stream));
+  if (n_probe) {
+    ZG_CUDA(cudaMemcpyAsync(lk_jobs_.p, ss_probes_.data(), n_probe * sizeof(zg_check), cudaMemcpyHostToDevice, stream));
+    ZG_CUDA(cudaMemcpyAsync(lb_owner_.p, ss_probe_owner_.data(), n_probe, cudaMemcpyHostToDevice, stream));
+    ZG_CUDA(cudaMemcpyAsync(ctrl + 3, &n_probe, 8, cudaMemcpyHostToDevice, stream));
+    ZG_CUDA(cudaMemcpyAsync(ss_out_.p, seeds.data(), seeds.size() * 8, cudaMemcpyHostToDevice, stream));
+  }
+  ZG_CUDA(cudaEventRecord(last_done_, stream));
+  have_last_ = true;
+  ZG_CUDA(cudaStreamSynchronize(stream));  // the host arrays above live on this frame
+  ss_snap_ = s;
+  ss_reqs_ = reqs;
+  ss_cap_ = walk_cap;
+  ss_include_ = include;
+  // the seeds are admitted like any arrived entry: a resource of the subject type becomes its own candidate
+  return shard_subjects_admit(ss_out_.as<unsigned long long>(), seeds.size(), d_front, n_front, err);
+}
+
+int Device::shard_subjects_expand(const unsigned long long* d_front, uint64_t n_in, uint32_t n_dest, unsigned long long* d_routed,
+                                  uint64_t* counts, bool* overflow, std::string* err) {
+  *overflow = false;
+  for (uint32_t d = 0; d < n_dest && d < kMaxRouteDest; ++d) counts[d] = 0;
+  if (!ss_snap_ || n_dest != shard_count || n_in > ss_cap_) {
+    if (err) *err = "shard_subjects_expand: no round begun, a shard count mismatch, or a frontier over the walk capacity";
+    return ZG_EINVAL;
+  }
+  ZG_CUDA(cudaSetDevice(device));
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  unsigned long long* ctrl = ss_ctrl_.as<unsigned long long>();
+  ZG_CUDA(cudaMemsetAsync(ctrl + 1, 0, 8, stream));
+  if (n_in) {
+    SsWalkParams p = ss_walk_params(*ss_snap_, lb_params_.as<SubjectsParam>(), rb_visited_.as<uint32_t>(), ctrl, shard_rank, shard_count);
+    p.in = d_front;
+    p.n_in = n_in;
+    p.out = ss_out_.as<unsigned long long>();
+    p.out_count = ctrl + 1;
+    p.cap = ss_cap_;
+    ss_expand_kernel<<<sm_count_ * 8, 256, 0, stream>>>(p);
+    ++launches;
+    ZG_CUDA(cudaGetLastError());
+  }
+  unsigned long long host[2] = {0, 0};
+  ZG_CUDA(cudaMemcpyAsync(host, ctrl, sizeof host, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaEventRecord(last_done_, stream));
+  have_last_ = true;
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  // flags are sticky: an admission (or the begin's) that did not fit is reported here
+  *overflow = (static_cast<uint32_t>(host[0]) & 16u) != 0;
+  if (*overflow) return ZG_OK;
+  return route_<false>(static_cast<const unsigned long long*>(ss_out_.as<unsigned long long>()), host[1], n_dest, EntryOwner{},
+                       d_routed, static_cast<uint32_t*>(nullptr), counts, err);
+}
+
+int Device::shard_subjects_admit(const unsigned long long* d_in, uint64_t n_in, unsigned long long* d_next, uint64_t* n_next,
+                                 std::string* err) {
+  *n_next = 0;
+  if (!ss_snap_) {
+    if (err) *err = "shard_subjects_admit: no round begun";
+    return ZG_EINVAL;
+  }
+  if (n_in == 0) return ZG_OK;
+  ZG_CUDA(cudaSetDevice(device));
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  unsigned long long* ctrl = ss_ctrl_.as<unsigned long long>();
+  ZG_CUDA(cudaMemsetAsync(ctrl + 2, 0, 8, stream));
+  SsWalkParams p = ss_walk_params(*ss_snap_, lb_params_.as<SubjectsParam>(), rb_visited_.as<uint32_t>(), ctrl, shard_rank, shard_count);
+  p.in = d_in;
+  p.n_in = n_in;
+  p.out = d_next;
+  p.out_count = ctrl + 2;
+  p.cap = ss_cap_;
+  p.cand = lk_jobs_.as<zg_check>();
+  p.cand_owner = lb_owner_.as<uint8_t>();
+  p.cand_count = ctrl + 3;
+  p.cand_cap = ss_cap_ + ss_probes_.size();
+  ss_admit_kernel<<<static_cast<unsigned>((n_in + 255) / 256), 256, 0, stream>>>(p);
+  ++launches;
+  ZG_CUDA(cudaGetLastError());
+  unsigned long long cnt = 0;
+  ZG_CUDA(cudaMemcpyAsync(&cnt, ctrl + 2, 8, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaEventRecord(last_done_, stream));
+  have_last_ = true;
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  *n_next = std::min<uint64_t>(cnt, ss_cap_);
+  return ZG_OK;
+}
+
+int Device::shard_subjects_candidates(bool exhaustive, zg_check* d_items, uint64_t cap, uint64_t* n, std::string* err) {
+  *n = 0;
+  if (!ss_snap_) {
+    if (err) *err = "shard_subjects_candidates: no round begun";
+    return ZG_EINVAL;
+  }
+  const Snapshot& s = *ss_snap_;
+  const size_t K = ss_reqs_.size();
+  const uint64_t n_probe = ss_probes_.size();
+  ZG_CUDA(cudaSetDevice(device));
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  unsigned long long* ctrl = ss_ctrl_.as<unsigned long long>();
+  std::vector<uint64_t> owned(K, 0);  // exhaustive: ids rank, rank + shard_count, ... below n_objects of the subject type
+  unsigned long long need = n_probe;
+  if (exhaustive) {
+    for (size_t k = 0; k < K; ++k) {
+      const uint64_t no = s.n_objects[ss_reqs_[k].stype];
+      owned[k] = no > shard_rank ? (no - shard_rank - 1) / shard_count + 1 : 0;
+      need += owned[k];
+    }
+  } else {
+    ZG_CUDA(cudaMemcpyAsync(&need, ctrl + 3, 8, cudaMemcpyDeviceToHost, stream));
+    ZG_CUDA(cudaStreamSynchronize(stream));
+    if (need > ss_cap_ + n_probe) {
+      if (err) *err = "shard_subjects_candidates: the walk overflowed (redo the round in halves, or exhaustive)";
+      return ZG_EINVAL;
+    }
+  }
+  if (!d_items) {
+    *n = need;
+    return ZG_OK;
+  }
+  if (cap < need) {
+    if (err) *err = "shard_subjects_candidates: item buffer too small";
+    return ZG_E2BIG;
+  }
+  if (exhaustive) {
+    if (!lk_jobs_.ensure(std::max<uint64_t>(need, 1) * sizeof(zg_check)) || !lb_owner_.ensure(std::max<uint64_t>(need, 1))) {
+      if (err) *err = "out of device memory (sharded lookup candidates)";
+      return ZG_ENOMEM;
+    }
+    // the probes first (a grown buffer does not keep them), then every owned id of each lookup's subject type
+    if (n_probe) {
+      ZG_CUDA(cudaMemcpyAsync(lk_jobs_.p, ss_probes_.data(), n_probe * sizeof(zg_check), cudaMemcpyHostToDevice, stream));
+      ZG_CUDA(cudaMemcpyAsync(lb_owner_.p, ss_probe_owner_.data(), n_probe, cudaMemcpyHostToDevice, stream));
+    }
+    uint64_t at = n_probe;
+    for (size_t k = 0; k < K; ++k) {
+      if (!owned[k]) continue;
+      const SubjectsReq& r = ss_reqs_[k];
+      ss_fill_owned_kernel<<<static_cast<unsigned>((owned[k] + 255) / 256), 256, 0, stream>>>(
+          SubjectsParam{r.res, r.res_type, r.perm, r.stype, r.srel}, static_cast<uint32_t>(k), owned[k], shard_rank, shard_count,
+          lk_jobs_.as<zg_check>() + at, lb_owner_.as<uint8_t>() + at);
+      ++launches;
+      at += owned[k];
+    }
+    ZG_CUDA(cudaGetLastError());
+  }
+  if (need) ZG_CUDA(cudaMemcpyAsync(d_items, lk_jobs_.p, need * sizeof(zg_check), cudaMemcpyDeviceToDevice, stream));
+  ZG_CUDA(cudaEventRecord(last_done_, stream));
+  have_last_ = true;
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  ss_n_cand_ = need;
+  *n = need;
+  return ZG_OK;
+}
+
+int Device::shard_subjects_verdicts(const uint8_t* d_codes, uint64_t n, uint64_t* granted, uint64_t* failed, std::string* err) {
+  *granted = *failed = 0;
+  if (!ss_snap_ || n != ss_n_cand_) {
+    if (err) *err = "shard_subjects_verdicts: no candidates of this round, or a count mismatch";
+    return ZG_EINVAL;
+  }
+  if (n == 0) return ZG_OK;
+  ZG_CUDA(cudaSetDevice(device));
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  unsigned long long* ctrl = ss_ctrl_.as<unsigned long long>();
+  ZG_CUDA(cudaMemsetAsync(ctrl + 6, 0, 16, stream));
+  ss_verdict_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(lk_jobs_.as<zg_check>(), lb_owner_.as<uint8_t>(), d_codes,
+                                                                                n, ctrl + 6, ctrl + 7);
+  ++launches;
+  ZG_CUDA(cudaGetLastError());
+  unsigned long long host[2] = {0, 0};
+  ZG_CUDA(cudaMemcpyAsync(host, ctrl + 6, sizeof host, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaEventRecord(last_done_, stream));
+  have_last_ = true;
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  *granted = host[0];
+  *failed = host[1];
+  return ZG_OK;
+}
+
+int Device::shard_subjects_nowild(const uint8_t* d_codes, uint64_t n, uint64_t granted, uint64_t failed, zg_check* d_items,
+                                  uint64_t cap, uint64_t* n_nw, std::string* err) {
+  *n_nw = 0;
+  if (!ss_snap_ || n != ss_n_cand_) {
+    if (err) *err = "shard_subjects_nowild: no candidates of this round, or a count mismatch";
+    return ZG_EINVAL;
+  }
+  if (cap < n) {
+    if (err) *err = "shard_subjects_nowild: item buffer smaller than the candidates";
+    return ZG_E2BIG;
+  }
+  ZG_CUDA(cudaSetDevice(device));
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  // every candidate gives at most one key, or one no-wildcards item that gives at most one key
+  const uint64_t m = std::max<uint64_t>(n, 1);
+  if (!lb_keys_[0].ensure(m * 8) || !ss_nw_.ensure(m * sizeof(zg_check)) || !ss_nw_owner_.ensure(m)) {
+    if (err) *err = "out of device memory (sharded lookup keys)";
+    return ZG_ENOMEM;
+  }
+  unsigned long long* ctrl = ss_ctrl_.as<unsigned long long>();
+  ZG_CUDA(cudaMemsetAsync(ctrl + 4, 0, 16, stream));
+  unsigned long long nw = 0;
+  if (n) {
+    ss_keys_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(
+        lk_jobs_.as<zg_check>(), lb_owner_.as<uint8_t>(), d_codes, n, granted, failed, ss_include_, lb_keys_[0].as<unsigned long long>(),
+        ctrl + 4, ss_nw_.as<zg_check>(), ss_nw_owner_.as<uint8_t>(), ctrl + 5);
+    ++launches;
+    ZG_CUDA(cudaGetLastError());
+    ZG_CUDA(cudaMemcpyAsync(&nw, ctrl + 5, 8, cudaMemcpyDeviceToHost, stream));
+    ZG_CUDA(cudaStreamSynchronize(stream));
+    if (nw) ZG_CUDA(cudaMemcpyAsync(d_items, ss_nw_.p, nw * sizeof(zg_check), cudaMemcpyDeviceToDevice, stream));
+  }
+  ZG_CUDA(cudaEventRecord(last_done_, stream));
+  have_last_ = true;
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  ss_n_nw_ = nw;
+  *n_nw = nw;
+  return ZG_OK;
+}
+
+int Device::shard_subjects_route(const uint8_t* d_codes, uint64_t n, uint32_t n_dest, unsigned long long* d_routed, uint64_t* counts,
+                                 std::string* err) {
+  for (uint32_t d = 0; d < n_dest && d < kMaxRouteDest; ++d) counts[d] = 0;
+  if (!ss_snap_ || n != ss_n_nw_ || n_dest != shard_count) {
+    if (err) *err = "shard_subjects_route: no no-wildcards items of this round, or a count / shard count mismatch";
+    return ZG_EINVAL;
+  }
+  ZG_CUDA(cudaSetDevice(device));
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  unsigned long long* ctrl = ss_ctrl_.as<unsigned long long>();
+  if (n) {
+    // granted = failed = 0: each item that checks HAS without the wildcard relationships is listed
+    ss_keys_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(
+        ss_nw_.as<zg_check>(), ss_nw_owner_.as<uint8_t>(), d_codes, n, 0, 0, 0, lb_keys_[0].as<unsigned long long>(), ctrl + 4,
+        nullptr, nullptr, ctrl + 5);
+    ++launches;
+    ZG_CUDA(cudaGetLastError());
+  }
+  unsigned long long n_keys = 0;
+  ZG_CUDA(cudaMemcpyAsync(&n_keys, ctrl + 4, 8, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaEventRecord(last_done_, stream));
+  have_last_ = true;
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  return route_<false>(static_cast<const unsigned long long*>(lb_keys_[0].as<unsigned long long>()), n_keys, n_dest,
+                       KeyHomeOwner{ss_home_.as<uint8_t>()}, d_routed, static_cast<uint32_t*>(nullptr), counts, err);
+}
+
+int Device::shard_subjects_finish(const unsigned long long* d_keys, uint64_t n, uint32_t* d_ids, uint64_t* listed, uint64_t* excluded,
+                                  std::string* err) {
+  if (!ss_snap_) {
+    if (err) *err = "shard_subjects_finish: no round begun";
+    return ZG_EINVAL;
+  }
+  const size_t K = ss_reqs_.size();
+  // the round ends here, whatever follows: the snapshot it read is not kept resident past it
+  ss_snap_.reset();
+  ss_reqs_.clear();
+  ss_n_cand_ = ss_n_nw_ = 0;
+  for (size_t k = 0; k < K; ++k) listed[k] = excluded[k] = 0;
+  if (n == 0) return ZG_OK;
+  ZG_CUDA(cudaSetDevice(device));
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  if (!lb_keys_[1].ensure(n * 8)) {
+    if (err) *err = "out of device memory (sharded lookup keys)";
+    return ZG_ENOMEM;
+  }
+  unsigned long long* ctrl = ss_ctrl_.as<unsigned long long>();
+  ZG_CUDA(cudaMemsetAsync(ctrl + kSsFirst, 0, 4 * kMaxLookupBatch * 8, stream));
+  // ascending (excluded bit, lookup, id): the listed runs in lookup order, then the excluded runs
+  std::string serr = sort_u64(d_keys, lb_keys_[1].as<unsigned long long>(), n, kExclKeyBit + 1, stream);
+  if (!serr.empty()) {
+    if (err) *err = serr;
+    return ZG_ECUDA;
+  }
+  ss_split_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(lb_keys_[1].as<unsigned long long>(), n, d_ids,
+                                                                              ctrl + kSsFirst, ctrl + kSsEnd);
+  ++launches;
+  unsigned long long host[4 * kMaxLookupBatch];
+  ZG_CUDA(cudaMemcpyAsync(host, ctrl + kSsFirst, sizeof host, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaGetLastError());
+  ZG_CUDA(cudaEventRecord(last_done_, stream));
+  have_last_ = true;
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  const unsigned long long* first = host;
+  const unsigned long long* end = host + 2 * kMaxLookupBatch;
+  for (size_t k = 0; k < K; ++k) {
+    listed[k] = end[k] - first[k];
+    excluded[k] = end[kMaxLookupBatch + k] - first[kMaxLookupBatch + k];
+  }
   return ZG_OK;
 }
 

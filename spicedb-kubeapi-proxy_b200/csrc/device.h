@@ -148,6 +148,45 @@ class Device {
   // lookup k; *err_mask bit k: lookup k had an undecidable candidate.
   int shard_lookup_finish(const unsigned long long* d_keys, uint64_t n, uint32_t* d_ids, uint64_t* per_lookup,
                           uint64_t* err_mask, std::string* err);
+  // shard_pass_dev with KParams::no_wildcards (LookupSubjects' second verification, on every pass of every rank)
+  int shard_pass_nowild_dev(const zg_check* d_queries, uint64_t n, int level, uint64_t* n_sub, std::string* err);
+  // ---- LookupSubjects on the sharded store (dist.DeviceShardedLookup.lookup_subjects): one round of K <= 64 ----
+  struct SubjectsReq {  // T:res#perm, subjects of type stype[#srel]
+    uint32_t res;
+    uint16_t res_type, perm, stype, srel;
+  };
+  // A round ends a LookupResources round begun on the same engine, and the other way round: they share buffers.
+  // Starts a round (the same lookups on every rank; home[k] = rank that asked lookup k; include bit k: lookup k
+  // asks for the wildcard entry). The owner of each written resource admits it as the level-0 frontier (d_front,
+  // walk_cap entries; *n_front) and holds the lookup's probe item (and, with the walk, the resource as a candidate
+  // when it has the subject type).
+  int shard_subjects_begin(const std::vector<SubjectsReq>& reqs, const uint8_t* home, uint64_t include, uint64_t walk_cap,
+                           unsigned long long* d_front, uint64_t* n_front, std::string* err);
+  // Expands this rank's frontier (n_in entries of one level) over its forward rows; the discoveries, bucketed by
+  // owner, go to d_routed (walk_cap entries); counts[d] (host) = entries for rank d. *overflow: an outbox, a frontier
+  // or the candidates of the round did not fit (sticky for the round); nothing is routed then.
+  int shard_subjects_expand(const unsigned long long* d_front, uint64_t n_in, uint32_t n_dest, unsigned long long* d_routed,
+                            uint64_t* counts, bool* overflow, std::string* err);
+  // Admits the n_in entries that arrived from every rank: the fresh ones are the next frontier (d_next, walk_cap).
+  int shard_subjects_admit(const unsigned long long* d_in, uint64_t n_in, unsigned long long* d_next, uint64_t* n_next,
+                           std::string* err);
+  // This rank's candidates as check items: the probes, then the walk's candidates (exhaustive: every owned id of the
+  // subject type). d_items == nullptr: *n = the capacity d_items needs.
+  int shard_subjects_candidates(bool exhaustive, zg_check* d_items, uint64_t cap, uint64_t* n, std::string* err);
+  // Codes of the first verification -> this rank's part of the round's granted / failed masks (host).
+  int shard_subjects_verdicts(const uint8_t* d_codes, uint64_t n, uint64_t* granted, uint64_t* failed, std::string* err);
+  // With the masks of every rank OR-ed: the answer keys of the first verification are kept, and the HAS candidates
+  // of granted lookups go to d_items (cap >= the candidates) for the no-wildcards verification; *n_nw of them.
+  int shard_subjects_nowild(const uint8_t* d_codes, uint64_t n, uint64_t granted, uint64_t failed, zg_check* d_items, uint64_t cap,
+                            uint64_t* n_nw, std::string* err);
+  // Codes of the no-wildcards verification: its HAS subjects are listed; every key goes to d_routed, bucketed by home
+  // rank; counts[d] (host) = keys for rank d.
+  int shard_subjects_route(const uint8_t* d_codes, uint64_t n, uint32_t n_dest, unsigned long long* d_routed, uint64_t* counts,
+                           std::string* err);
+  // Keys that arrived home -> d_ids: the listed ids of lookup 0, 1, ... then the excluded ids of lookup 0, 1, ...,
+  // ascending each; listed[k] / excluded[k] (host, K) = their counts. Ends the round.
+  int shard_subjects_finish(const unsigned long long* d_keys, uint64_t n, uint32_t* d_ids, uint64_t* listed, uint64_t* excluded,
+                            std::string* err);
 
   std::shared_ptr<Snapshot> snap;
   cudaStream_t stream = nullptr;
@@ -193,6 +232,14 @@ class Device {
   std::vector<LookupReq> sl_reqs_;
   uint64_t sl_cap_ = 0, sl_n_cand_ = 0;
   uint64_t sl_n_walk_ = 0;  // candidates before the self-membership ones: only these can fail a lookup
+  // sharded LookupSubjects round: visited slices, candidates, params and keys in the buffers above; the outbox,
+  // the no-wildcards items, home ranks and control words here
+  DevBuf ss_out_, ss_nw_, ss_nw_owner_, ss_home_, ss_ctrl_;
+  std::shared_ptr<Snapshot> ss_snap_;  // read from begin to finish (released there)
+  std::vector<SubjectsReq> ss_reqs_;
+  std::vector<zg_check> ss_probes_;  // this rank's probe items (the lookups whose resource it owns) and their lookups
+  std::vector<uint8_t> ss_probe_owner_;
+  uint64_t ss_cap_ = 0, ss_include_ = 0, ss_n_cand_ = 0, ss_n_nw_ = 0;
   template <bool kSrc, class Item, class Owner>
   int route_(const Item* d_items, uint64_t n, uint32_t n_dest, Owner owner, Item* d_routed, uint32_t* d_src, uint64_t* counts,
              std::string* err);

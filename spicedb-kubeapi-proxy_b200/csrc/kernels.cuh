@@ -1600,4 +1600,219 @@ __global__ void ls_split_kernel(const zg_check* items, const uint8_t* codes, uns
   }
 }
 
+// ---- LookupSubjects on the object-hash sharded store (dist.DeviceShardedLookup.lookup_subjects) ---------------
+//
+// Shard k holds the forward rows of the objects it owns, but the subjects in those rows can be owned by any shard.
+// So the walk routes what it discovers to the owner, and the owner deduplicates: every rank keeps a visited slice
+// per lookup, in which the bit of an object it owns means "admitted" (it entered this rank's frontier once), and
+// the bit of an object it does not own means "already sent for this lookup". An object enters the frontier of its
+// owner at the first level any rank discovers it, which is the level a replica's fwalk_expand_kernel reaches it:
+// the admitted objects, and so the candidates, are the replica's.
+struct SubjectsParam {  // one per lookup of the round
+  uint32_t res;
+  uint16_t res_type, perm, stype, srel;
+};
+struct SsWalkParams {
+  const uint32_t* row_ptr;
+  const uint32_t* col;
+  const FwdClass* fwd;                 // as FwalkParams
+  const uint32_t* type_off;
+  const uint32_t* mask;                // Schema::fwd_mask: mask_words words per permission slot
+  uint32_t mask_words;
+  uint32_t shard_rank, shard_count;
+  const SubjectsParam* lk;
+  const unsigned long long* in;        // lookup << 48 | type << 32 | object
+  unsigned long long n_in;
+  unsigned long long* out;             // expand: the outbox; admit: the next frontier
+  unsigned long long* out_count;
+  unsigned long long cap;              // entries of `out`
+  uint32_t* visited;                   // K slices of `words` u32, bit = type_bit_base[type] + object
+  unsigned long long words;
+  const unsigned long long* type_bit_base;
+  zg_check* cand;                      // admit: candidate checks of this rank
+  uint8_t* cand_owner;
+  unsigned long long* cand_count;
+  unsigned long long cand_cap;
+  uint32_t* flags;                     // bit 4: outbox / frontier / candidate overflow
+};
+
+// One warp per frontier object (all owned by this rank), the classes of its type that the lookup's permission
+// reads, as fwalk_expand_kernel. A subject is put in the outbox unless this rank already admitted it (owned) or
+// already sent it (not owned) for this lookup; the owner's admission decides whether it is new.
+__global__ void __launch_bounds__(256) ss_expand_kernel(const SsWalkParams p) {
+  const unsigned lane = threadIdx.x & 31;
+  const unsigned long long n_warps = (static_cast<unsigned long long>(gridDim.x) * blockDim.x) >> 5;
+  for (unsigned long long w = (blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x) >> 5; w < p.n_in;
+       w += n_warps) {
+    const unsigned long long item = p.in[w];
+    const uint32_t k = static_cast<uint32_t>(item >> 48), type = static_cast<uint32_t>(item >> 32) & 0xFFFFu,
+                   obj = static_cast<uint32_t>(item);
+    const uint32_t* const mask = p.mask + static_cast<size_t>(p.lk[k].perm) * p.mask_words;
+    uint32_t* const vis = p.visited + k * p.words;
+    for (uint32_t ci = p.type_off[type]; ci < p.type_off[type + 1]; ++ci) {
+      const FwdClass fc = p.fwd[ci];
+      if (!((mask[fc.gc >> 5] >> (fc.gc & 31)) & 1u) || obj >= fc.nres) continue;
+      const unsigned long long ri = fc.row_base + static_cast<unsigned long long>(obj) * fc.ncls;
+      const uint32_t b = __ldg(p.row_ptr + ri), e = __ldg(p.row_ptr + ri + 1);
+      const unsigned long long bit_base = p.type_bit_base[fc.stype];
+      for (uint32_t i0 = b; i0 < e; i0 += 32) {
+        const uint32_t i = i0 + lane;
+        bool fresh = false;
+        uint32_t s = 0;
+        if (i < e) {
+          s = __ldg(p.col + i);
+          const unsigned long long bit = bit_base + s;
+          const uint32_t m = 1u << (bit & 31);
+          // owned bits are only set by ss_admit_kernel, never while this kernel runs
+          fresh = s % p.shard_count == p.shard_rank ? !(vis[bit >> 5] & m) : !(atomicOr(vis + (bit >> 5), m) & m);
+        }
+        const unsigned fm = __ballot_sync(kFull, fresh);
+        if (fm) {
+          unsigned long long at = 0;
+          if (lane == 0) at = atomicAdd(p.out_count, static_cast<unsigned long long>(__popc(fm)));
+          at = __shfl_sync(kFull, at, 0) + __popc(fm & ((1u << lane) - 1u));
+          if (fresh) {
+            if (at < p.cap) p.out[at] = (item & (0xFFFFull << 48)) | (static_cast<unsigned long long>(fc.stype) << 32) | s;
+            else atomicOr(p.flags, 16u);
+          }
+        }
+      }
+    }
+  }
+}
+
+// Outbox entries are routed to the owner of their object
+struct EntryOwner {
+  __device__ __forceinline__ uint32_t operator()(unsigned long long entry, uint32_t n_dest) const {
+    return static_cast<uint32_t>(entry) % n_dest;
+  }
+};
+
+// Admission at the owner, one thread per arrived entry: a test-and-set of the object's bit in the lookup's slice.
+// A fresh entry joins the next frontier; a fresh object of the lookup's subject type is also a candidate
+// {res, object, perm, stype, srel}. The round's level-0 seeds (each resource, on its owner) are admitted the same way.
+__global__ void ss_admit_kernel(const SsWalkParams p) {
+  const unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x;
+  const unsigned lane = threadIdx.x & 31;
+  bool fresh = false, is_cand = false;
+  unsigned long long item = 0;
+  SubjectsParam l{};
+  if (i < p.n_in) {
+    item = p.in[i];
+    const uint32_t k = static_cast<uint32_t>(item >> 48), type = static_cast<uint32_t>(item >> 32) & 0xFFFFu;
+    const unsigned long long bit = p.type_bit_base[type] + static_cast<uint32_t>(item);
+    const uint32_t m = 1u << (bit & 31);
+    fresh = !(atomicOr(p.visited + k * p.words + (bit >> 5), m) & m);
+    l = p.lk[k];
+    is_cand = fresh && type == l.stype;
+  }
+  const unsigned fm = __ballot_sync(kFull, fresh), cm = __ballot_sync(kFull, is_cand);
+  const unsigned below = (1u << lane) - 1u;
+  unsigned long long fb = 0, cb = 0;
+  if (lane == 0 && fm) fb = atomicAdd(p.out_count, static_cast<unsigned long long>(__popc(fm)));
+  if (lane == 0 && cm) cb = atomicAdd(p.cand_count, static_cast<unsigned long long>(__popc(cm)));
+  fb = __shfl_sync(kFull, fb, 0) + __popc(fm & below);
+  cb = __shfl_sync(kFull, cb, 0) + __popc(cm & below);
+  if (fresh) {
+    if (fb < p.cap) p.out[fb] = item;
+    else atomicOr(p.flags, 16u);
+  }
+  if (is_cand) {
+    if (cb < p.cand_cap) {
+      zg_check q;
+      q.res = l.res;
+      q.subj = static_cast<uint32_t>(item);
+      q.perm = l.perm;
+      q.stype = l.stype;
+      q.srel = l.srel;
+      q.flags = 0;
+      p.cand[cb] = q;
+      p.cand_owner[cb] = static_cast<uint8_t>(item >> 48);
+    } else {
+      atomicOr(p.flags, 16u);
+    }
+  }
+}
+
+// Exhaustive candidates of lookup k (its walk overflowed): the n ids of the subject type this rank owns,
+// rank, rank + shard_count, ...
+__global__ void ss_fill_owned_kernel(SubjectsParam l, uint32_t k, unsigned long long n, uint32_t shard_rank, uint32_t shard_count,
+                                     zg_check* cand, uint8_t* cand_owner) {
+  const unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x;
+  if (i >= n) return;
+  zg_check q;
+  q.res = l.res;
+  q.subj = static_cast<uint32_t>(shard_rank + i * shard_count);
+  q.perm = l.perm;
+  q.stype = l.stype;
+  q.srel = l.srel;
+  q.flags = 0;
+  cand[i] = q;
+  cand_owner[i] = static_cast<uint8_t>(k);
+}
+
+// First verification of this rank's candidates: failed bit k: the probe or a candidate of lookup k is undecidable
+// (the lookup is ZG_EDEPTH); granted bit k: lookup k's probe checks HAS without a subject relation (the wildcard
+// grants the permission). Only the owner of the resource holds the probe (subject ZG_NO_OBJECT - 1).
+__global__ void ss_verdict_kernel(const zg_check* cand, const uint8_t* owner, const uint8_t* codes, unsigned long long n,
+                                  unsigned long long* granted, unsigned long long* failed) {
+  const unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x;
+  if (i >= n) return;
+  const uint8_t code = codes[i];
+  if (code == ZG_ITEM_ERROR) atomicOr(failed, 1ull << owner[i]);
+  else if (code == ZG_HAS_PERMISSION && cand[i].subj == ZG_NO_OBJECT - 1 && cand[i].srel == kNone)
+    atomicOr(granted, 1ull << owner[i]);
+}
+
+// Answer keys (excluded << kExclKeyBit | lookup << 32 | id; KeyHomeOwner sends them home) of the verified candidates
+// other than the probes, for the lookups that did not fail: a HAS candidate is listed, unless its lookup is granted,
+// in which case it goes to the no-wildcards verification (nw, nw_owner); a NO candidate of a granted lookup whose
+// wildcard entry is asked for is excluded. After that verification the same kernel runs over its items with
+// granted = failed = 0: its HAS subjects are listed.
+constexpr int kExclKeyBit = 38;  // just above the lookup index: a lookup's listed ids sort before every excluded one
+__global__ void ss_keys_kernel(const zg_check* cand, const uint8_t* owner, const uint8_t* codes, unsigned long long n,
+                               unsigned long long granted, unsigned long long failed, unsigned long long include,
+                               unsigned long long* keys, unsigned long long* n_keys, zg_check* nw, uint8_t* nw_owner,
+                               unsigned long long* n_nw) {
+  const unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x;
+  const unsigned lane = threadIdx.x & 31;
+  bool listed = false, excl = false, again = false;
+  uint32_t k = 0, subj = 0;
+  if (i < n) {
+    k = owner[i];
+    subj = cand[i].subj;
+    const uint8_t code = codes[i];
+    const bool live = subj != ZG_NO_OBJECT - 1 && !((failed >> k) & 1ull), g = (granted >> k) & 1ull;
+    listed = live && code == ZG_HAS_PERMISSION && !g;
+    again = live && code == ZG_HAS_PERMISSION && g;
+    excl = live && code == ZG_NO_PERMISSION && g && ((include >> k) & 1ull);
+  }
+  const bool key = listed || excl;
+  const unsigned km = __ballot_sync(kFull, key), am = __ballot_sync(kFull, again);
+  const unsigned below = (1u << lane) - 1u;
+  unsigned long long kb = 0, ab = 0;
+  if (lane == 0 && km) kb = atomicAdd(n_keys, static_cast<unsigned long long>(__popc(km)));
+  if (lane == 0 && am) ab = atomicAdd(n_nw, static_cast<unsigned long long>(__popc(am)));
+  kb = __shfl_sync(kFull, kb, 0) + __popc(km & below);
+  ab = __shfl_sync(kFull, ab, 0) + __popc(am & below);
+  if (key)
+    keys[kb] = (static_cast<unsigned long long>(excl) << kExclKeyBit) | (static_cast<unsigned long long>(k) << 32) | subj;
+  if (again) {
+    nw[ab] = cand[i];
+    nw_owner[ab] = static_cast<uint8_t>(k);
+  }
+}
+
+// Keys that arrived home, sorted: run r = key >> 32 (lookup k's listed ids: r = k; its excluded ids:
+// r = 64 + k) is ids[first[r] .. end[r]), both left 0 for an empty run.
+__global__ void ss_split_kernel(const unsigned long long* keys, unsigned long long n, uint32_t* ids, unsigned long long* first,
+                                unsigned long long* end) {
+  const unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x;
+  if (i >= n) return;
+  const unsigned long long key = keys[i], run = key >> 32;
+  ids[i] = static_cast<uint32_t>(key);
+  if (i == 0 || (keys[i - 1] >> 32) != run) first[run] = i;
+  if (i + 1 == n || (keys[i + 1] >> 32) != run) end[run] = i + 1;
+}
+
 }  // namespace zg

@@ -310,8 +310,11 @@ class DeviceShardedChecker:
         counts = self.e.shard_route_dev(d_items, n, level, w, routed.data_ptr(), src.data_ptr())
         return routed[: n * self.ITEM], src[:n], counts, self.t.exchange_counts(counts)
 
-    def check_bulk(self, d_items: torch.Tensor, n: int) -> torch.Tensor:
+    def check_bulk(self, d_items: torch.Tensor, n: int, no_wildcards: bool = False) -> torch.Tensor:
+        """no_wildcards: every pass of every rank evaluates with the wildcard relationships invisible (LookupSubjects'
+        second verification; the sub-queries raised to other shards are evaluated the same way)."""
         dev, t = self.t.device, self.t
+        shard_pass = self.e.shard_pass_nowild_dev if no_wildcards else self.e.shard_pass_dev
         # level "-1": this rank's own batch goes to the owners of its resources
         routed, src0, sc, rc = self._route(d_items.data_ptr(), n, -1)
         queries = t.alltoall(routed, sc, rc, self.ITEM)
@@ -320,7 +323,7 @@ class DeviceShardedChecker:
         lv = 0
         while True:
             nq = queries.numel() // self.ITEM
-            nsub = self.e.shard_pass_dev(queries.data_ptr() if nq else 0, nq, lv)
+            nsub = shard_pass(queries.data_ptr() if nq else 0, nq, lv)
             routed, src, sc, rc = self._route(0, nsub, lv)
             nxt = t.alltoall(routed, sc, rc, self.ITEM)
             self.stats["exchanges"] += 1
@@ -363,6 +366,7 @@ class DeviceShardedChecker:
 
 MAX_DEPTH = 50  # ZG_MAX_DEPTH (include/zgpu.h): the walk expands levels 0 .. MAX_DEPTH + 1, as a replica's does
 LOOKUP_ROUND = 64  # lookups per round (visited slices; the lookup index in an answer key has 6 bits)
+WILDCARDS_INCLUDE = 0  # ZG_WILDCARDS_INCLUDE (include/zgpu.h)
 
 
 class DeviceShardedLookup:
@@ -378,25 +382,46 @@ class DeviceShardedLookup:
         candidates per check_bulk call, so that their raised sub-queries fit the engine's sub-query buffer."""
         self.e, self.t, self.walk_cap, self.verify_chunk = engine, transport, int(walk_cap), int(verify_chunk)
         self.checker = checker or DeviceShardedChecker(engine, transport)
+        # entries_sent / admitted / nowild_verified: LookupSubjects' walk entries sent to other ranks, objects admitted
+        # into a frontier by their owner, and items of the no-wildcards verification
         self.stats = {"rounds": 0, "levels": 0, "frontier_entries": 0, "frontier_bytes": 0, "bytes_sent": 0,
-                      "candidates": 0, "fallbacks": 0, "halvings": 0}
+                      "candidates": 0, "fallbacks": 0, "halvings": 0, "entries_sent": 0, "admitted": 0, "nowild_verified": 0}
+
+    def _gather_requests(self, mine):
+        """Every rank's requests (structured array `mine` of this rank's) -> (all of them in rank order, on every rank;
+        the home rank of each; the index of this rank's first)."""
+        t, w = self.t, self.t.world
+        counts = t.exchange_counts([mine.size] * w)  # requests of every rank, in rank order
+        send = torch.from_numpy(np.tile(mine.view(np.uint8), w)).to(t.device)
+        got = t.alltoall(send, [mine.size] * w, counts, mine.dtype.itemsize)
+        self.stats["bytes_sent"] += mine.size * mine.dtype.itemsize * (w - 1)
+        every = got.cpu().numpy().view(mine.dtype)
+        return every, np.repeat(np.arange(w, dtype=np.uint8), counts), sum(counts[: t.rank])
+
+    def _verify(self, items, n, no_wildcards=False):
+        """Codes of this rank's n check items, in chunks that bound the check protocol's sub-query buffers; every rank
+        runs as many chunks as the rank with the most items (check_bulk is collective)."""
+        t, w, dev = self.t, self.t.world, self.t.device
+        item = DeviceShardedChecker.ITEM
+        codes = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
+        for lo in range(0, max(t.exchange_counts([n] * w)), self.verify_chunk):
+            m = max(0, min(self.verify_chunk, n - lo))
+            codes[lo:lo + m] = self.checker.check_bulk(items[lo * item:(lo + m) * item] if m else items, m, no_wildcards)
+        # the copies into `codes` run on torch's stream, the engine reads `codes` on its own: they must have landed
+        # (and the chunks' answer tensors they read must not be handed out again) before the engine's next call
+        if dev.type == "cuda":
+            torch.cuda.current_stream().synchronize()
+        return codes
 
     def lookup_resources(self, reqs) -> list:
         """reqs: [(res_type_id, perm_slot, subj_type_id, subj_id, subj_rel_slot)] of this rank (subj_rel_slot = SREL_NONE
         for a plain subject). -> per request an ascending uint32 array of resource ids, or None where
         zg_lookup_resources would return ZG_EDEPTH (a candidate could not be decided)."""
-        t, w = self.t, self.t.world
         mine = np.zeros(len(reqs), self.REQ)
         for i, (rt, perm, st, subj, srel) in enumerate(reqs):
             mine[i] = (subj, rt, perm, st, srel)
-        counts = t.exchange_counts([mine.size] * w)  # requests of every rank, in rank order
-        send = torch.from_numpy(np.tile(mine.view(np.uint8), w)).to(t.device)
-        got = t.alltoall(send, [mine.size] * w, counts, self.REQ.itemsize)
-        self.stats["bytes_sent"] += mine.size * self.REQ.itemsize * (w - 1)
-        every = got.cpu().numpy().view(self.REQ)
-        home = np.repeat(np.arange(w, dtype=np.uint8), counts)
+        every, home, first = self._gather_requests(mine)
         out = [None] * mine.size
-        first = sum(counts[: t.rank])
         for lo in range(0, every.size, LOOKUP_ROUND):
             self._round(every[lo:lo + LOOKUP_ROUND], home[lo:lo + LOOKUP_ROUND], lo - first, out)
         return out
@@ -440,17 +465,7 @@ class DeviceShardedLookup:
         items = torch.empty(max(need, 1) * DeviceShardedChecker.ITEM, dtype=torch.uint8, device=dev)
         n = self.e.shard_lookup_candidates_dev(overflow, items.data_ptr(), need)
         self.stats["candidates"] += n
-        # verified in chunks that bound the check protocol's sub-query buffers; every rank runs as many chunks as
-        # the rank with the most candidates (check_bulk is collective)
-        codes = torch.empty(max(n, 1), dtype=torch.uint8, device=dev)
-        item = DeviceShardedChecker.ITEM
-        for lo in range(0, max(t.exchange_counts([n] * w)), self.verify_chunk):
-            m = max(0, min(self.verify_chunk, n - lo))
-            codes[lo:lo + m] = self.checker.check_bulk(items[lo * item:(lo + m) * item] if m else items, m)
-        # the copies into `codes` run on torch's stream, the engine reads `codes` on its own: they must have landed
-        # (and the chunks' answer tensors they read must not be handed out again) before the engine's next call
-        if dev.type == "cuda":
-            torch.cuda.current_stream().synchronize()
+        codes = self._verify(items, n)
         routed = torch.empty(max(n, 1) * 8, dtype=torch.uint8, device=dev)
         sc = self.e.shard_lookup_route_dev(codes.data_ptr() if n else 0, n, w, routed.data_ptr())
         rc = t.exchange_counts(sc)
@@ -465,3 +480,103 @@ class DeviceShardedLookup:
             if home[k] == t.rank:
                 out[base + k] = None if (err >> k) & 1 else host[off:off + per[k]].copy()
             off += per[k]
+
+    # -----------------------------------------------------------------------------------------
+    # LookupSubjects (DESIGN.md 4 and 7). Shard k holds the forward rows of the objects it owns, but the subjects in
+    # those rows can be owned by any shard: each level, every rank expands its own frontier, sends what it finds to
+    # the owners (a count exchange that also carries the overflow flag and whether the rank had a frontier, then one
+    # all-to-all of 8-byte entries), and each owner admits an object once per lookup. Each rank's candidates are then
+    # its batch of check_bulk; the probe verdicts travel to every rank once per round, the HAS candidates of granted
+    # lookups are verified again without wildcards, and the answers go home with one more all-to-all.
+
+    SUBJ_REQ = np.dtype([("res", "<u4"), ("res_type", "<u2"), ("perm", "<u2"), ("stype", "<u2"), ("srel", "<u2"),
+                         ("option", "<u4")])
+
+    def lookup_subjects(self, reqs) -> list:
+        """reqs: [(res_type_id, res_id, perm_slot, subj_type_id, subj_rel_slot, wildcard_option)] of this rank (subj_rel_slot
+        = SREL_NONE for a plain subject type; wildcard_option ZG_WILDCARDS_INCLUDE = 0 or EXCLUDE = 1). -> per request
+        (ids, wildcard, excluded): the ascending uint32 ids listed, whether the wildcard entry is present, and the
+        ascending uint32 ids it excludes; None where zg_lookup_subjects on a replica returns ZG_EDEPTH."""
+        mine = np.zeros(len(reqs), self.SUBJ_REQ)
+        for i, (rt, res, perm, st, srel, opt) in enumerate(reqs):
+            mine[i] = (res, rt, perm, st, srel, opt)
+        every, home, first = self._gather_requests(mine)
+        out = [None] * mine.size
+        for lo in range(0, every.size, LOOKUP_ROUND):
+            self._subjects_round(every[lo:lo + LOOKUP_ROUND], home[lo:lo + LOOKUP_ROUND], lo - first, out)
+        return out
+
+    def _subjects_round(self, reqs, home, base, out):
+        """One round of <= 64 lookups on every rank; answers of this rank's lookups go to out[base + k]."""
+        t, w, dev, e = self.t, self.t.world, self.t.device, self.e
+        K = reqs.size
+        self.stats["rounds"] += 1
+        protos = np.zeros(K, CHECK_DTYPE)
+        protos["res"], protos["perm"], protos["stype"], protos["srel"] = reqs["res"], reqs["perm"], reqs["stype"], reqs["srel"]
+        front = torch.empty(self.walk_cap * 8, dtype=torch.uint8, device=dev)
+        routed = torch.empty(self.walk_cap * 8, dtype=torch.uint8, device=dev)
+        n_front = e.shard_subjects_begin_dev(reqs["res_type"], protos, reqs["option"], home, self.walk_cap, front.data_ptr())
+        self.stats["admitted"] += n_front
+        level, overflow = 0, False
+        while True:
+            # levels 0 .. MAX_DEPTH + 1 are expanded, as on a replica; one more exchange reports the last admissions'
+            # overflow and ends the walk
+            live = n_front if level <= MAX_DEPTH + 1 else 0
+            sc, ovf = e.shard_subjects_expand_dev(front.data_ptr(), live, w, routed.data_ptr())
+            got = t.exchange_counts([c << 2 | (live > 0) << 1 | int(ovf) for c in sc])
+            if any(g & 1 for g in got):
+                overflow = True
+                break
+            if not any(g & 2 for g in got):  # no rank had a frontier at this level: the walk is over
+                break
+            self.stats["levels"] += 1
+            rc = [g >> 2 for g in got]
+            arrived = t.alltoall(routed[: sum(sc) * 8], sc, rc, 8)
+            self.stats["entries_sent"] += sum(sc) - sc[t.rank]
+            self.stats["bytes_sent"] += (sum(sc) - sc[t.rank]) * 8
+            n_front = e.shard_subjects_admit_dev(arrived.data_ptr() if sum(rc) else 0, sum(rc), front.data_ptr())
+            self.stats["admitted"] += n_front
+            level += 1
+        if overflow and K > 1:
+            self.stats["halvings"] += 1
+            h = K // 2
+            self._subjects_round(reqs[:h], home[:h], base, out)
+            self._subjects_round(reqs[h:], home[h:], base + h, out)
+            return
+        if overflow:
+            self.stats["fallbacks"] += 1
+        need = e.shard_subjects_candidates_dev(overflow, 0, 0)
+        item = DeviceShardedChecker.ITEM
+        items = torch.empty(max(need, 1) * item, dtype=torch.uint8, device=dev)
+        n = e.shard_subjects_candidates_dev(overflow, items.data_ptr(), need)
+        self.stats["candidates"] += n
+        codes = self._verify(items, n)
+        granted, failed = e.shard_subjects_verdicts_dev(codes.data_ptr() if n else 0, n)
+        # the probe verdicts are known on the resources' owners only: every rank ORs every rank's masks
+        masks = np.array([granted, failed], dtype=np.uint64).view(np.uint8)
+        got = t.alltoall(torch.from_numpy(np.tile(masks, w)).to(dev), [1] * w, [1] * w, 16)
+        got = np.bitwise_or.reduce(got.cpu().numpy().view(np.uint64).reshape(w, 2), axis=0)
+        granted, failed = int(got[0]), int(got[1])
+        self.stats["bytes_sent"] += 16 * (w - 1)
+        nw_items = torch.empty(max(n, 1) * item, dtype=torch.uint8, device=dev)
+        n_nw = e.shard_subjects_nowild_dev(codes.data_ptr() if n else 0, n, granted, failed, nw_items.data_ptr(), max(n, 1))
+        self.stats["nowild_verified"] += n_nw
+        # every rank takes part in the no-wildcards verification when any lookup of the round is granted
+        nw_codes = self._verify(nw_items, n_nw, no_wildcards=True) if granted & ~failed else nw_items[:1]
+        keys = torch.empty(max(n, 1) * 8, dtype=torch.uint8, device=dev)
+        sc = e.shard_subjects_route_dev(nw_codes.data_ptr() if n_nw else 0, n_nw, w, keys.data_ptr())
+        rc = t.exchange_counts(sc)
+        arrived = t.alltoall(keys[: sum(sc) * 8], sc, rc, 8)
+        self.stats["bytes_sent"] += (sum(sc) - sc[t.rank]) * 8
+        nk = sum(rc)
+        ids = torch.empty(max(nk, 1) * 4, dtype=torch.uint8, device=dev)
+        listed, excluded = e.shard_subjects_finish_dev(arrived.data_ptr() if nk else 0, nk, ids.data_ptr(), K)
+        host = ids[: nk * 4].cpu().numpy().view(np.uint32)
+        at_l, at_x = 0, sum(listed)
+        for k in range(K):
+            if home[k] == t.rank:
+                wild = bool((granted >> k) & 1) and reqs["option"][k] == WILDCARDS_INCLUDE
+                out[base + k] = None if (failed >> k) & 1 else (
+                    host[at_l:at_l + listed[k]].copy(), wild, host[at_x:at_x + excluded[k]].copy())
+            at_l += listed[k]
+            at_x += excluded[k]
