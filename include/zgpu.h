@@ -191,6 +191,11 @@ uint32_t zg_intern_object(zg_engine *e, int type_id, const char *object_id);
 uint32_t zg_find_object(const zg_engine *e, int type_id, const char *object_id); /* ZG_NO_OBJECT */
 /* Copies the name into buf (NUL terminated); returns its length or ZG_E2BIG/ZG_EINVAL. */
 int zg_object_name(const zg_engine *e, int type_id, uint32_t id, char *buf, size_t cap);
+/* Bulk zg_intern_object over the packed layout: the n ids are [off[i], off[i+1]) of ids. out_ids[i] = the id of
+ * name i (an existing name keeps its id; the empty id gives ZG_NO_OBJECT, as zg_intern_object refuses it).
+ * ZG_EINVAL for an unknown type or a decreasing offset (nothing is interned then). Host only. */
+int zg_intern_objects_packed(zg_engine *e, int type_id, const char *ids, const uint32_t *off, uint64_t n,
+                             uint32_t *out_ids);
 
 /* ---- relationship store -------------------------------------------------- */
 /* Bulk TOUCH of interned relationships (expires may be NULL). Not visible to
@@ -247,6 +252,30 @@ int zg_resolve_checks_packed(zg_engine *e, const char *res_type, const char *rel
 int zg_check_bulk_packed(zg_engine *e, const char *res_type, const char *relation, const char *subj_type,
                          const char *subj_rel, const char *res_ids, const uint32_t *res_off,
                          const char *subj_ids, const uint32_t *subj_off, uint64_t n, uint8_t *out);
+/* Device ingress: the same resolution on the GPU, against a device mirror of the interned names that the first such
+ * call on an engine creates and every later one brings up to date (only names interned since are uploaded; a schema
+ * load discards it). The items are bit-identical to zg_resolve_checks_packed's. Both calls take the device lock and
+ * return after their GPU work has completed; they use the engine's first device.
+ *   zg_resolve_checks_packed_device  DEVICE blobs, offsets and d_out, on cuda_stream (NULL = default stream). With
+ *                                    d_subj_off NULL, d_subj_ids is the one subject as a HOST NUL-terminated string.
+ *                                    ZG_EINVAL when an offset decreases. Allowed on sharded engines (it reads only
+ *                                    names); composes with zg_check_bulk_device.
+ *   zg_check_bulk_packed_ingress     zg_check_bulk_packed's arguments (HOST buffers): publishes pending writes, then
+ *                                    stages the ids in pinned memory, resolves and checks them on the GPU and copies
+ *                                    the answers back in one launch sequence. It does not join the coalescing batcher:
+ *                                    small calls should keep using zg_check_bulk_packed. Refused on sharded engines.
+ * ZG_ECUDA on host-only engines. */
+int zg_resolve_checks_packed_device(zg_engine *e, const char *res_type, const char *relation, const char *subj_type,
+                                    const char *subj_rel, const char *d_res_ids, const uint32_t *d_res_off,
+                                    const char *d_subj_ids, const uint32_t *d_subj_off, uint64_t n, zg_check *d_out,
+                                    void *cuda_stream);
+int zg_check_bulk_packed_ingress(zg_engine *e, const char *res_type, const char *relation, const char *subj_type,
+                                 const char *subj_rel, const char *res_ids, const uint32_t *res_off,
+                                 const char *subj_ids, const uint32_t *subj_off, uint64_t n, uint8_t *out);
+/* Cumulative device-ingress counters (zg_stats keeps its layout): out[0] names mirrored, out[1] device bytes of the
+ * mirror, out[2] calls that uploaded names, out[3] table rebuilds (a full table re-inserted at twice the size),
+ * out[4] items resolved on the device. All 0 before the first device-ingress call. */
+int zg_ingress_counters(zg_engine *e, uint64_t *out);
 
 /* LookupResources: ids (ascending) of every object of res_type with HAS_PERMISSION.
  * Returns 0, or ZG_E2BIG with *n_out = required capacity. */

@@ -175,6 +175,10 @@ _SIGS = {
     "zg_lookup_subjects_str": (C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint32,
                                          C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint64)]),
     "zg_lookup_subjects_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "zg_resolve_checks_packed_device": (C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]),
+    "zg_check_bulk_packed_ingress": (C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_void_p, C.c_char_p, C.c_void_p, C.c_uint64, C.c_void_p]),
+    "zg_intern_objects_packed": (C.c_int, [C.c_void_p, C.c_int, C.c_char_p, C.c_void_p, C.c_uint64, C.c_void_p]),
+    "zg_ingress_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
     "zg_shard_pass": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.POINTER(C.c_uint64)]),
     "zg_shard_subqueries": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_uint64]),
     "zg_shard_fold": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_uint64, C.c_void_p]),
@@ -573,6 +577,34 @@ class Engine:
     def check_bulk_packed(self, res_type, relation, subj_type, res_ids, subjects, subj_rel="") -> np.ndarray:
         return self._packed_call(self._L.zg_check_bulk_packed, res_type, relation, subj_type, subj_rel, res_ids, subjects,
                                  np.empty(len(res_ids), dtype=np.uint8))
+
+    def check_bulk_packed_ingress(self, res_type, relation, subj_type, res_ids, subjects, subj_rel="") -> np.ndarray:
+        """check_bulk_packed with the ids resolved on the GPU (one launch sequence, outside the batcher)."""
+        return self._packed_call(self._L.zg_check_bulk_packed_ingress, res_type, relation, subj_type, subj_rel, res_ids,
+                                 subjects, np.empty(len(res_ids), dtype=np.uint8))
+
+    def resolve_checks_packed_device(self, res_type, relation, subj_type, d_res_ids: int, d_res_off: int, n: int,
+                                     d_out: int, subjects=None, d_subj_off: int = 0, subj_rel="", stream: int = 0):
+        """zg_resolve_checks_packed_device: DEVICE pointers as ints (blob, n + 1 u32 offsets, n zg_check out). `subjects`:
+        the one subject (str) for every item, or the device pointer of the per-item subject blob with d_subj_off."""
+        one = isinstance(subjects, (str, bytes))
+        self._ck(self._L.zg_resolve_checks_packed_device(
+            self._h, _b(res_type), _b(relation), _b(subj_type), _b(subj_rel or ""), d_res_ids, d_res_off,
+            _b(subjects) if one else subjects, None if one else d_subj_off, n, d_out, stream))
+
+    def intern_packed(self, type_name, ids) -> np.ndarray:
+        """zg_intern_objects_packed: the ids of the names (str or bytes), interning the new ones."""
+        blob, off = self.pack_ids(ids)
+        out = np.empty(len(ids), dtype=np.uint32)
+        self._ck(self._L.zg_intern_objects_packed(self._h, self.type_id(type_name), blob or b"\0", off.ctypes.data, len(ids),
+                                                  out.ctypes.data))
+        return out
+
+    def ingress_counters(self) -> dict:
+        out = np.zeros(5, dtype=np.uint64)
+        self._ck(self._L.zg_ingress_counters(self._h, out.ctypes.data))
+        return {"names": int(out[0]), "device_bytes": int(out[1]), "sync_uploads": int(out[2]), "rebuilds": int(out[3]),
+                "items_resolved": int(out[4])}
 
     def resolve_checks(self, rels) -> np.ndarray:
         """Strings -> interned zg_check items (no GPU work); feed them to check_bulk."""

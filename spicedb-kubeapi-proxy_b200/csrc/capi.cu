@@ -320,6 +320,7 @@ extern "C" int zg_load_schema(zg_engine* e, const char* dsl, size_t len) {
   e->store.shard_count = e->dev.shard_count;
   e->store.shard_rank = e->dev.shard_rank;
   e->dev.snap.reset();
+  e->dev.ingress_reset();  // the device mirror of the names
   for (auto& r : e->replicas) r->dev.snap.reset();
   e->dirty = true;
   return ZG_OK;
@@ -1148,6 +1149,105 @@ extern "C" int zg_check_bulk_str(zg_engine* e, const zg_rel_str* items, uint64_t
   // through the batcher like any zg_check_bulk call: concurrent string callers -- one goroutine per
   // rule check in the proxy, pkg/authz/check.go:77-93 -- share launches too.
   return zg_check_bulk(e, c.data(), n, out);
+}
+
+// ---- device ingress: packed ids resolved on the GPU against a mirror of the interned names ----------
+//
+// Each call takes the device lock, then the names lock shared: the mirror's sync (Device::ingress_sync) and the
+// resolve kernel never race a writer or each other, and the call returns after its GPU work has completed.
+
+// The literal fields, resolved once exactly as resolve_packed_locked resolves them.
+static Device::IngressLiterals ingress_literals(zg_engine* e, const char* res_type, const char* relation,
+                                               const char* subj_type, const char* subj_rel, const char* one_subj) {
+  Device::IngressLiterals lit;
+  ResolveMemo memo;
+  const zg_rel_str proto{res_type, "", relation, subj_type, one_subj ? one_subj : "", subj_rel};
+  resolve_check(e, proto, &lit.base, &memo);
+  lit.ok = lit.base.perm != kNone;
+  if (lit.ok) {
+    lit.rt = memo.parts[memo.last].rt;
+    lit.st = memo.parts[memo.last].st;
+  }
+  if (one_subj) {
+    lit.one_subj = one_subj;
+    lit.one_len = std::strlen(one_subj);
+    lit.one_su = memo.su;
+  }
+  return lit;
+}
+
+static const char* kHostOnlyMsg = "host-only engine: no CUDA device, and libzgpu has no CPU fallback";
+
+extern "C" int zg_resolve_checks_packed_device(zg_engine* e, const char* res_type, const char* relation,
+                                               const char* subj_type, const char* subj_rel, const char* d_res_ids,
+                                               const uint32_t* d_res_off, const char* d_subj_ids,
+                                               const uint32_t* d_subj_off, uint64_t n, zg_check* d_out, void* stream) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (!(res_type && relation && subj_type && (n == 0 || (d_res_ids && d_res_off && d_subj_ids && d_out))))
+    return fail(ZG_EINVAL, "NULL argument");
+  if (e->host_only) return fail(ZG_ECUDA, kHostOnlyMsg);
+  if (n == 0) return ZG_OK;
+  LOCK_DEVICE(e);
+  LOCK_NAMES_SHARED(e);
+  const Device::IngressLiterals lit =
+      ingress_literals(e, res_type, relation, subj_type, subj_rel, d_subj_off ? nullptr : d_subj_ids);
+  std::string err;
+  const int rc = e->dev.ingress_resolve(e->store, lit, d_res_ids, d_res_off, d_subj_ids, d_subj_off, n, d_out,
+                                        static_cast<cudaStream_t>(stream), &err);
+  return rc ? fail(rc, err) : ZG_OK;
+}
+
+extern "C" int zg_check_bulk_packed_ingress(zg_engine* e, const char* res_type, const char* relation,
+                                            const char* subj_type, const char* subj_rel, const char* res_ids,
+                                            const uint32_t* res_off, const char* subj_ids, const uint32_t* subj_off,
+                                            uint64_t n, uint8_t* out) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (!PACKED_ARGS_OK()) return fail(ZG_EINVAL, "NULL argument");
+  if (e->host_only) return fail(ZG_ECUDA, kHostOnlyMsg);
+  if (e->dev.shard_count > 1) return fail(ZG_EINVAL, kShardedMsg);
+  if (n == 0) return ZG_OK;
+  int rc = publish_if_needed(e);
+  if (rc) return rc;
+  LOCK_DEVICE(e);
+  LOCK_NAMES_SHARED(e);
+  const Device::IngressLiterals lit =
+      ingress_literals(e, res_type, relation, subj_type, subj_rel, subj_off ? nullptr : subj_ids);
+  e->dev.now = now_of(e);
+  std::string err;
+  rc = e->dev.ingress_check_host(e->store, lit, res_ids, res_off, subj_ids, subj_off, n, out, &err);
+  return rc ? fail(rc, err) : ZG_OK;
+}
+
+extern "C" int zg_intern_objects_packed(zg_engine* e, int type_id, const char* ids, const uint32_t* off, uint64_t n,
+                                        uint32_t* out_ids) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (type_id < 0 || type_id >= static_cast<int>(e->schema.types.size())) return fail(ZG_EINVAL, "unknown type");
+  if (n && (!ids || !off || !out_ids)) return fail(ZG_EINVAL, "NULL argument");
+  for (uint64_t i = 0; i < n; ++i)
+    if (off[i] > off[i + 1]) return fail(ZG_EINVAL, "offsets must not decrease");
+  LOCK_NAMES_UNIQUE(e);
+  std::string s;
+  for (uint64_t i = 0; i < n; ++i) {
+    if (off[i] == off[i + 1]) {  // the empty id names no object, as in zg_intern_object
+      out_ids[i] = ZG_NO_OBJECT;
+      continue;
+    }
+    s.assign(ids + off[i], off[i + 1] - off[i]);
+    out_ids[i] = e->store.intern(type_id, s);
+  }
+  return ZG_OK;
+}
+
+extern "C" int zg_ingress_counters(zg_engine* e, uint64_t* out) {
+  if (!e || !out) return fail(ZG_EINVAL, "NULL argument");
+  LOCK_DEVICE(e);
+  const IngressMirror* m = e->dev.ingress_.get();
+  out[0] = m ? m->names : 0;
+  out[1] = m ? m->device_bytes() : 0;
+  out[2] = m ? m->sync_uploads : 0;
+  out[3] = m ? m->rebuilds : 0;
+  out[4] = m ? m->items_resolved : 0;
+  return ZG_OK;
 }
 
 // ---- list templates: scanned items -> interned checks without per-item strings --------------

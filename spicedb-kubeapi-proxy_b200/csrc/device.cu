@@ -12,6 +12,7 @@
 #include <mutex>
 #include <thread>
 
+#include "ingress.cuh"
 #include "kernels.cuh"
 
 namespace zg {
@@ -2179,6 +2180,216 @@ int Device::lookup_subjects(uint16_t res_type, uint32_t res, uint16_t perm, uint
   rc = fetch(concrete, n_concrete, &ans->ids);
   if (!rc && ans->wildcard) rc = fetch(no_ids, n_no, &ans->excluded);
   return rc;
+}
+
+// ---- device ingress ----------------------------------------------------------------------------
+
+IngressMirror::~IngressMirror() {
+  for (auto& t : types)
+    for (auto* b : {&t.arena, &t.offs, &t.slots}) b->release();
+  for (auto* b : {&stage, &items, &out, &one, &bad}) b->release();
+  if (pin) cudaFreeHost(pin);
+  if (pin_out) cudaFreeHost(pin_out);
+}
+
+uint64_t IngressMirror::device_bytes() const {
+  uint64_t b = 0;
+  for (const auto& t : types) b += t.arena.cap + t.offs.cap + t.slots.cap;
+  return b;
+}
+
+static unsigned ingress_grid(uint64_t n, int sm_count) {
+  const uint64_t want = (n + kIngressThreads - 1) / kIngressThreads;
+  return static_cast<unsigned>(std::max<uint64_t>(1, std::min<uint64_t>(want, uint64_t(std::max(sm_count, 1)) * 16)));
+}
+
+// Names are append-only between schema loads, so the mirror only ever uploads the arena bytes it has not seen.
+int Device::ingress_sync(const Store& store, cudaStream_t st, std::string* err) {
+  constexpr uint64_t kMinTable = 1024;
+  if (!ingress_) ingress_.reset(new IngressMirror());
+  IngressMirror& m = *ingress_;
+  if (m.types.size() != store.n_types()) m.types.resize(store.n_types());
+  bool uploaded = false;
+  for (size_t t = 0; t < m.types.size(); ++t) {
+    const std::vector<char>& ar = store.name_arena(static_cast<int>(t));
+    IngressMirror::Type& y = m.types[t];
+    if (ar.size() < y.bytes) {  // not the arena this mirror was built from: start the type over
+      m.names -= y.host_offs.size();
+      for (auto* b : {&y.arena, &y.offs, &y.slots}) b->release();
+      y = IngressMirror::Type{};
+    }
+    if (ar.size() == y.bytes) continue;
+    if (ar.size() >= kIngressOffMask) {
+      if (err) *err = "interned names of one type exceed 2^40 bytes";
+      return ZG_ENOMEM;
+    }
+    uploaded = true;
+    const uint64_t n_old = y.host_offs.size();
+    for (uint64_t off = y.bytes; off < ar.size();) {
+      uint32_t len;
+      std::memcpy(&len, ar.data() + off + 4, 4);
+      y.host_offs.push_back(off);
+      off += 8 + uint64_t(len);
+    }
+    const uint64_t n_all = y.host_offs.size();
+    // arena: the new bytes, or all of them into a buffer twice the size
+    if (ar.size() > y.arena.cap) {
+      if (!y.arena.ensure(std::max<size_t>(ar.size(), y.arena.cap * 2))) {
+        if (err) *err = "out of device memory (name mirror)";
+        return ZG_ENOMEM;
+      }
+      ZG_CUDA(cudaMemcpyAsync(y.arena.p, ar.data(), ar.size(), cudaMemcpyHostToDevice, st));
+    } else {
+      ZG_CUDA(cudaMemcpyAsync(y.arena.as<char>() + y.bytes, ar.data() + y.bytes, ar.size() - y.bytes,
+                              cudaMemcpyHostToDevice, st));
+    }
+    // record offsets, likewise
+    if (n_all * 8 > y.offs.cap) {
+      if (!y.offs.ensure(std::max<size_t>(n_all * 8, y.offs.cap * 2))) {
+        if (err) *err = "out of device memory (name mirror)";
+        return ZG_ENOMEM;
+      }
+      ZG_CUDA(cudaMemcpyAsync(y.offs.p, y.host_offs.data(), n_all * 8, cudaMemcpyHostToDevice, st));
+    } else {
+      ZG_CUDA(cudaMemcpyAsync(y.offs.as<uint64_t>() + n_old, y.host_offs.data() + n_old, (n_all - n_old) * 8,
+                              cudaMemcpyHostToDevice, st));
+    }
+    // table: insert the new records, or every record into a table twice the size when the load would pass 1/2
+    uint64_t cap = y.cap ? y.cap : kMinTable;
+    while (n_all * 2 > cap) cap *= 2;
+    uint64_t from = n_old;
+    if (cap != y.cap) {
+      if (!y.slots.ensure(cap * 8)) {
+        if (err) *err = "out of device memory (name mirror)";
+        return ZG_ENOMEM;
+      }
+      ZG_CUDA(cudaMemsetAsync(y.slots.p, 0, cap * 8, st));
+      if (y.cap) ++m.rebuilds;
+      y.cap = cap;
+      from = 0;
+    }
+    IngressInsertParams p{};
+    p.arena = y.arena.as<uint8_t>();
+    p.offs = y.offs.as<unsigned long long>();
+    p.from = from;
+    p.to = n_all;
+    p.slots = y.slots.as<unsigned long long>();
+    p.mask = cap - 1;
+    ingress_insert_kernel<<<ingress_grid(n_all - from, sm_count_), kIngressThreads, 0, st>>>(p);
+    ZG_CUDA(cudaGetLastError());
+    ++launches;
+    y.bytes = ar.size();
+    m.names += n_all - n_old;
+  }
+  if (uploaded) ++m.sync_uploads;
+  return ZG_OK;
+}
+
+int Device::ingress_resolve(const Store& store, const IngressLiterals& lit, const char* d_res_ids, const uint32_t* d_res_off,
+                            const char* d_subj_ids, const uint32_t* d_subj_off, uint64_t n, zg_check* d_out, cudaStream_t st,
+                            std::string* err) {
+  if (n == 0) return ZG_OK;
+  ZG_CUDA(cudaSetDevice(device));
+  int rc = ingress_sync(store, st, err);
+  if (rc) return rc;
+  IngressMirror& m = *ingress_;
+  if (!m.bad.ensure(4) || (lit.one_subj && !m.one.ensure(lit.one_len + 1))) {
+    if (err) *err = "out of device memory (ingress scratch)";
+    return ZG_ENOMEM;
+  }
+  ZG_CUDA(cudaMemsetAsync(m.bad.p, 0, 4, st));
+  if (lit.one_subj && lit.one_len)
+    ZG_CUDA(cudaMemcpyAsync(m.one.p, lit.one_subj, lit.one_len, cudaMemcpyHostToDevice, st));
+  auto table = [&](int t) {
+    IngressTable x{nullptr, nullptr, 0};
+    if (t >= 0 && t < static_cast<int>(m.types.size()) && m.types[t].cap) {
+      x.arena = m.types[t].arena.as<uint8_t>();
+      x.slots = m.types[t].slots.as<unsigned long long>();
+      x.mask = m.types[t].cap - 1;
+    }
+    return x;
+  };
+  IngressResolveParams p{};
+  p.rt = table(lit.rt);
+  p.st = table(lit.st);
+  p.res_ids = reinterpret_cast<const uint8_t*>(d_res_ids);
+  p.res_off = d_res_off;
+  p.subj_ids = lit.one_subj ? m.one.as<uint8_t>() : reinterpret_cast<const uint8_t*>(d_subj_ids);
+  p.subj_off = lit.one_subj ? nullptr : d_subj_off;
+  p.one_len = lit.one_len;
+  p.one_su = lit.one_su;
+  p.ok = lit.ok ? 1 : 0;
+  p.same_type = lit.rt == lit.st ? 1 : 0;
+  p.base = lit.base;
+  p.n = n;
+  p.tag_mask = kIngressTagMask;
+  p.out = d_out;
+  p.bad = m.bad.as<unsigned>();
+  ingress_resolve_kernel<<<ingress_grid(n, sm_count_), kIngressThreads, 0, st>>>(p);
+  ZG_CUDA(cudaGetLastError());
+  ++launches;
+  unsigned bad = 0;
+  ZG_CUDA(cudaMemcpyAsync(&bad, m.bad.p, 4, cudaMemcpyDeviceToHost, st));
+  ZG_CUDA(cudaStreamSynchronize(st));
+  m.items_resolved += n;
+  if (bad) {
+    if (err) *err = "offsets must not decrease";
+    return ZG_EINVAL;
+  }
+  return ZG_OK;
+}
+
+int Device::ingress_check_host(const Store& store, const IngressLiterals& lit, const char* res_ids, const uint32_t* res_off,
+                               const char* subj_ids, const uint32_t* subj_off, uint64_t n, uint8_t* out, std::string* err) {
+  if (n == 0) return ZG_OK;
+  ZG_CUDA(cudaSetDevice(device));
+  for (uint64_t i = 0; i < n; ++i)
+    if (res_off[i] > res_off[i + 1] || (subj_off && subj_off[i] > subj_off[i + 1])) {
+      if (err) *err = "offsets must not decrease";
+      return ZG_EINVAL;
+    }
+  // one staging area, one copy: [res_off][subj_off][res blob][subj blob], each part 16-byte aligned
+  auto al = [](uint64_t b) { return (b + 15) & ~uint64_t(15); };
+  const uint64_t off_bytes = (n + 1) * 4, rblob = res_off[n], sblob = subj_off ? subj_off[n] : 0;
+  const uint64_t o_soff = al(off_bytes), o_rids = o_soff + (subj_off ? al(off_bytes) : 0), o_sids = o_rids + al(rblob);
+  const uint64_t total = o_sids + al(sblob);
+  if (!ingress_) ingress_.reset(new IngressMirror());
+  IngressMirror& m = *ingress_;
+  if (total > m.pin_cap) {
+    if (m.pin) cudaFreeHost(m.pin);
+    m.pin = nullptr;
+    m.pin_cap = 0;
+    ZG_CUDA(cudaHostAlloc(&m.pin, total + total / 4, cudaHostAllocDefault));
+    m.pin_cap = total + total / 4;
+  }
+  if (n > m.pin_out_cap) {
+    if (m.pin_out) cudaFreeHost(m.pin_out);
+    m.pin_out = nullptr;
+    m.pin_out_cap = 0;
+    ZG_CUDA(cudaHostAlloc(&m.pin_out, n + n / 4, cudaHostAllocDefault));
+    m.pin_out_cap = n + n / 4;
+  }
+  if (!m.stage.ensure(total) || !m.items.ensure(n * sizeof(zg_check)) || !m.out.ensure(n)) {
+    if (err) *err = "out of device memory (ingress staging)";
+    return ZG_ENOMEM;
+  }
+  char* pin = static_cast<char*>(m.pin);
+  std::memcpy(pin, res_off, off_bytes);
+  if (subj_off) std::memcpy(pin + o_soff, subj_off, off_bytes);
+  std::memcpy(pin + o_rids, res_ids, rblob);
+  if (subj_off) std::memcpy(pin + o_sids, subj_ids, sblob);
+  ZG_CUDA(cudaMemcpyAsync(m.stage.p, pin, total, cudaMemcpyHostToDevice, stream));
+  char* d = m.stage.as<char>();
+  int rc = ingress_resolve(store, lit, d + o_rids, reinterpret_cast<const uint32_t*>(d),
+                           subj_off ? d + o_sids : nullptr, subj_off ? reinterpret_cast<const uint32_t*>(d + o_soff) : nullptr,
+                           n, m.items.as<zg_check>(), stream, err);
+  if (rc) return rc;
+  rc = check_device(m.items.as<zg_check>(), n, m.out.as<uint8_t>(), stream, true, nullptr, err);
+  if (rc) return rc;
+  ZG_CUDA(cudaMemcpyAsync(m.pin_out, m.out.p, n, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  std::memcpy(out, m.pin_out, n);
+  return ZG_OK;
 }
 
 }  // namespace zg

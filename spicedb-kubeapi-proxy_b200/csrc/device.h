@@ -54,6 +54,27 @@ struct Snapshot {
   ~Snapshot();
 };
 
+// Device mirror of the interned names (ingress.cuh), built on the first device-ingress call and synced at the start
+// of every one: the arena bytes past `bytes` are uploaded, their records inserted into the table, and the table is
+// rebuilt at twice the size when its load would pass 1/2.
+struct IngressMirror {
+  struct Type {
+    DevBuf arena, offs, slots;
+    std::vector<uint64_t> host_offs;  // record offsets, as uploaded to offs
+    uint64_t bytes = 0;               // arena bytes mirrored
+    uint64_t cap = 0;                 // table slots (power of two), 0 = no table yet
+  };
+  std::vector<Type> types;
+  // staging of zg_check_bulk_packed_ingress (offsets and blobs, pinned host -> device; items; answers) and the
+  // resolve's scratch (the one subject's bytes, the decreasing-offset flag)
+  DevBuf stage, items, out, one, bad;
+  void *pin = nullptr, *pin_out = nullptr;
+  size_t pin_cap = 0, pin_out_cap = 0;
+  uint64_t names = 0, sync_uploads = 0, rebuilds = 0, items_resolved = 0;
+  ~IngressMirror();
+  uint64_t device_bytes() const;
+};
+
 class Device {
  public:
   ~Device();
@@ -188,6 +209,29 @@ class Device {
   int shard_subjects_finish(const unsigned long long* d_keys, uint64_t n, uint32_t* d_ids, uint64_t* listed, uint64_t* excluded,
                             std::string* err);
 
+  // ---- device ingress (ingress.cuh): packed string ids -> interned checks against the mirror of the store's names ----
+  // The literal fields of a packed call, resolved once on the host exactly as zg_resolve_checks_packed resolves them.
+  struct IngressLiterals {
+    zg_check base;       // every item starts as this (ok == false: answers ZG_ITEM_ERROR)
+    bool ok = false;
+    int rt = -1, st = -1;  // resource / subject type
+    uint32_t one_su = ZG_NO_OBJECT;  // the one subject's id (one_subj != nullptr)
+    const char* one_subj = nullptr;  // HOST bytes of the one subject, or nullptr: per-item subjects
+    size_t one_len = 0;
+  };
+  // Brings the mirror in step with the store's names (creating it on first use), then resolves the n packed items
+  // (DEVICE blobs and n + 1 offsets) into d_out on `st` and waits for it. The caller holds the names lock, shared or
+  // exclusive. ZG_EINVAL when an offset decreases.
+  int ingress_resolve(const Store& store, const IngressLiterals& lit, const char* d_res_ids, const uint32_t* d_res_off,
+                      const char* d_subj_ids, const uint32_t* d_subj_off, uint64_t n, zg_check* d_out, cudaStream_t st,
+                      std::string* err);
+  // HOST blobs and offsets -> v1 codes in out: staged through pinned memory, resolved and checked on the engine's
+  // stream in one launch sequence. The offsets are checked on the host while they are staged.
+  int ingress_check_host(const Store& store, const IngressLiterals& lit, const char* res_ids, const uint32_t* res_off,
+                         const char* subj_ids, const uint32_t* subj_off, uint64_t n, uint8_t* out, std::string* err);
+  void ingress_reset() { ingress_.reset(); }  // a schema (re)load: the names are gone
+  std::unique_ptr<IngressMirror> ingress_;     // nullptr until the first device-ingress call
+
   std::shared_ptr<Snapshot> snap;
   cudaStream_t stream = nullptr;
   int device = 0;
@@ -206,6 +250,7 @@ class Device {
   uint64_t last_alg_bytes = 0;
 
  private:
+  int ingress_sync(const Store& store, cudaStream_t st, std::string* err);
   std::string finish_publish(std::shared_ptr<Snapshot> s, const HostSnapshot& lay, const Schema& sc, uint64_t revision);
   // One check_kernel launch over `nq` queries: val (may be null) receives the per-(query, leaf) value
   // bits, out (may be null) the per-query v1 codes / value bits.

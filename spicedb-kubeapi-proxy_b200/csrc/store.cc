@@ -5,6 +5,8 @@
 #include <cstring>
 #include <numeric>
 
+#include "hash_bytes.h"
+
 namespace zg {
 
 void Store::reset(const Schema* s) {
@@ -28,26 +30,6 @@ void Store::clear_relationships() {
   index_.clear();
   indexed_ = true;
   live_ = 0;
-}
-
-static inline uint64_t hash_bytes(const char* s, size_t n) {
-  uint64_t h = 0x9E3779B97F4A7C15ull ^ (n * 0xD6E8FEB86659FD93ull);
-  while (n >= 8) {
-    uint64_t w;
-    std::memcpy(&w, s, 8);
-    h = (h ^ w) * 0xD6E8FEB86659FD93ull;
-    h ^= h >> 32;
-    s += 8;
-    n -= 8;
-  }
-  if (n) {
-    uint64_t w = 0;
-    std::memcpy(&w, s, n);
-    h = (h ^ w) * 0xD6E8FEB86659FD93ull;
-    h ^= h >> 32;
-  }
-  h *= 0x9E3779B97F4A7C15ull;
-  return h ^ (h >> 29);
 }
 
 static inline void rec_read(const std::vector<char>& arena, uint64_t off, uint32_t* id, uint32_t* len) {

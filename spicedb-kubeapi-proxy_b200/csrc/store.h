@@ -61,6 +61,11 @@ class Store {
   uint32_t find(int type, const char* id, size_t len) const;  // no temporary string: the check-ingress path
   // false for a numeric-only object (bulk loads) or an id out of range
   bool name(int type, uint32_t id, std::string_view* out) const;
+  // Read-only view of a type's interned names, for the device mirror (ingress.cuh): the records
+  // [u32 id][u32 len][bytes] back to back (append-only until reset) and how many there are.
+  size_t n_types() const { return objs_.size(); }
+  const std::vector<char>& name_arena(int type) const { return objs_[type].arena; }
+  uint32_t n_interned(int type) const { return objs_[type].n_interned; }
 
   // Returns "" or an error message; `code` receives the ZG_* code.
   std::string validate(const zg_tuple& t, bool has_expiry) const;

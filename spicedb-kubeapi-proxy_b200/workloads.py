@@ -352,6 +352,45 @@ def cfg4(seed=4, scale=1.0, batch=1 << 20, nonpure_folders=False) -> Workload:
     return w
 
 
+def object_name(type_name: str, i: int) -> str:
+    """String id of dense object i in the named stores: users u%07d, pods ns%05d/p%07d (1 000 pods per namespace),
+    every other type <type>%07d."""
+    if type_name == "user":
+        return "u%07d" % i
+    if type_name == "pod":
+        return "ns%05d/p%07d" % (i // 1000, i)
+    return "%s%07d" % (type_name, i)
+
+
+def object_counts(w: Workload) -> dict:
+    """Per type: 1 + the largest object id the workload's relationships and checks name."""
+    n = {}
+
+    def see(t, ids):
+        if ids.size:
+            n[t] = max(n.get(t, 0), int(ids.max()) + 1)
+
+    for g in w.groups:
+        see(g.res_type, g.res)
+        if not g.wildcard:
+            see(g.subj_type, g.subj)
+    for c in w.checks:
+        see(c.res_type, c.res)
+        see(c.subj_type, c.subj)
+    return n
+
+
+def intern_names(w: Workload, engine) -> int:
+    """Gives every object of the workload its name (object_name), interned in id order BEFORE the relationships are
+    loaded, so that each name's interned id is the dense id the workload uses. Returns the names interned."""
+    total = 0
+    for t, n in sorted(object_counts(w).items()):
+        ids = engine.intern_packed(t, [object_name(t, i) for i in range(n)])
+        assert ids.size == n and int(ids[0]) == 0 and int(ids[-1]) == n - 1, f"{t}: names did not intern in id order"
+        total += n
+    return total
+
+
 def by_name(name: str, scale: float = 1.0, **kw) -> Workload:
     if name == "cfg1":
         return cfg1()
