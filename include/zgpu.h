@@ -326,26 +326,21 @@ int zg_debug_row(zg_engine *e, uint16_t rel_slot, uint32_t res, uint32_t cls, ui
 
 /* ---- object-hash sharded store (one engine per GPU, shard_count > 1) --------
  * A check starts on the owner of its resource; an edge to an object owned by another shard (or
- * into a non-pure permission) is raised as a sub-query. The host runs the ranks pass by pass
- * and exchanges the raised sub-queries (all-to-all) until none are left, then folds the values
- * back level by level (spicedb-kubeapi-proxy_b200/dist.py ShardedStoreChecker). On sharded
- * engines zg_check_bulk / zg_lookup_resources / zg_lookup_subjects are refused: use these three calls (checks),
- * the zg_shard_lookup_*_dev calls below (LookupResources) or the zg_shard_subjects_*_dev calls (LookupSubjects). */
-int zg_shard_pass(zg_engine *e, const zg_check *queries, uint64_t n, int level, uint64_t *n_sub);
-/* The sub-queries pass `level` raised, in emission order (same layout; flags = hop depth). */
-int zg_shard_subqueries(zg_engine *e, int level, zg_check *out, uint64_t n);
-/* child_vals[i]: value of raised sub-query i (bit0 HAS, bit1 ERROR). out[q]: level 0: v1 code of
- * query q; deeper levels: its value bits, to be sent back to the rank that raised it. */
-int zg_shard_fold(zg_engine *e, int level, const uint8_t *child_vals, uint64_t n_sub, uint8_t *out);
-
-/* The same protocol with every buffer resident on the device (dist.DeviceShardedChecker): checks and raised
- * sub-queries are bucketised by owner in a kernel, exchanged device to device (NCCL all-to-all over NVLink, or
- * peer copies), and the values coming back are folded without a host copy. All pointers are DEVICE pointers of
- * the engine's GPU; every call returns after its work completed (the exchange runs on the caller's stream).
+ * into a non-pure permission) is raised as a sub-query. The ranks run pass by pass and exchange
+ * the raised sub-queries (all-to-all) until none are left, then fold the values back level by
+ * level (spicedb-kubeapi-proxy_b200/dist.py DeviceShardedChecker). Every buffer stays resident on
+ * the device: checks and raised sub-queries are bucketised by owner in a kernel, exchanged device to
+ * device (NCCL all-to-all over NVLink, or peer copies), and the values coming back are folded without
+ * a host copy. All pointers are DEVICE pointers of the engine's GPU; every call returns after its work
+ * completed (the exchange runs on the caller's stream). On sharded engines zg_check_bulk /
+ * zg_lookup_resources / zg_lookup_subjects are refused: use these zg_shard_*_dev calls (checks), the
+ * zg_shard_lookup_*_dev calls below (LookupResources) or the zg_shard_subjects_*_dev calls (LookupSubjects).
  *   zg_shard_route_dev   items (d_items, or the sub-queries raised by pass `level` when d_items is NULL) ->
  *                        d_routed in destination-major order + d_src[i] = source index of d_routed[i];
  *                        counts[d] (HOST array of n_dest) = items for destination d = res % n_dest
- *   zg_shard_pass_dev    zg_shard_pass with the level's queries already on the device
+ *   zg_shard_pass_dev    evaluates the level's n queries (d_queries) in one pass: level 0 takes the callers'
+ *                        items routed to this shard, deeper levels the routed sub-queries with the hop depth in
+ *                        flags; *n_sub = the sub-queries the pass raised
  *   zg_shard_fold_dev    d_child_vals in ROUTED order + the d_src of that routing -> d_out[q] per query of the
  *                        level (v1 codes when final_codes, else value bits for the rank that raised it)
  *   zg_shard_unroute_dev d_out[d_src[i]] = d_val[i]: answers restored to the caller's order */

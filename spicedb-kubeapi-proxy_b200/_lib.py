@@ -179,9 +179,6 @@ _SIGS = {
     "zg_check_bulk_packed_ingress": (C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_void_p, C.c_char_p, C.c_void_p, C.c_uint64, C.c_void_p]),
     "zg_intern_objects_packed": (C.c_int, [C.c_void_p, C.c_int, C.c_char_p, C.c_void_p, C.c_uint64, C.c_void_p]),
     "zg_ingress_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
-    "zg_shard_pass": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.POINTER(C.c_uint64)]),
-    "zg_shard_subqueries": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_uint64]),
-    "zg_shard_fold": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_uint64, C.c_void_p]),
     "zg_shard_route_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_uint32, C.c_void_p, C.c_void_p,
                                      C.c_void_p]),
     "zg_shard_pass_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.POINTER(C.c_uint64)]),
@@ -680,25 +677,8 @@ class Engine:
         self._ck(self._L.zg_lookup_subjects_counters(self._h, out.ctypes.data))
         return {"walks": int(out[0]), "fallbacks": int(out[1]), "items_verified": int(out[2])}
 
-    # -- sharded store (dist.ShardedStoreChecker drives these) --------------------
-    def shard_pass(self, queries: np.ndarray, level: int) -> int:
-        q = np.ascontiguousarray(queries, dtype=CHECK_DTYPE)
-        n = C.c_uint64(0)
-        self._ck(self._L.zg_shard_pass(self._h, q.ctypes.data, q.size, level, C.byref(n)))
-        return n.value
-
-    def shard_subqueries(self, level: int, n: int) -> np.ndarray:
-        out = np.empty(n, dtype=CHECK_DTYPE)
-        self._ck(self._L.zg_shard_subqueries(self._h, level, out.ctypes.data, n))
-        return out
-
-    def shard_fold(self, level: int, child_vals: np.ndarray, n_queries: int) -> np.ndarray:
-        cv = np.ascontiguousarray(child_vals, dtype=np.uint8)
-        out = np.empty(n_queries, dtype=np.uint8)
-        self._ck(self._L.zg_shard_fold(self._h, level, cv.ctypes.data, cv.size, out.ctypes.data))
-        return out
-
-    # device-resident variants: every pointer is a device address on this engine's GPU (ints, e.g. tensor.data_ptr())
+    # -- sharded store (dist.DeviceShardedChecker drives these) --------------------
+    # every pointer is a device address on this engine's GPU (ints, e.g. tensor.data_ptr())
     def shard_route_dev(self, d_items: int, n: int, level: int, n_dest: int, d_routed: int, d_src: int) -> list:
         counts = (C.c_uint64 * n_dest)()
         self._ck(self._L.zg_shard_route_dev(self._h, d_items or None, n, level, n_dest, d_routed or None, d_src or None, counts))

@@ -219,7 +219,8 @@ static void on_all_devices(zg_engine* e, const std::function<void(Device&, size_
 static thread_local std::string g_err;
 static constexpr size_t kMaxLookupGroup = 64;  // = kMaxLookupBatch (kernels.cuh)
 static const char* kShardedMsg =
-    "sharded engine: use zg_shard_pass / zg_shard_subqueries / zg_shard_fold (dist.ShardedStoreChecker)";
+    "sharded engine: use zg_shard_route_dev / zg_shard_pass_dev / zg_shard_fold_dev / zg_shard_unroute_dev "
+    "(dist.DeviceShardedChecker)";
 
 static int fail(int code, const std::string& msg) {
   g_err = msg;
@@ -1971,36 +1972,6 @@ extern "C" int zg_stats_get(zg_engine* e, zg_stats* out) {
     out->snapshot_bytes = e->dev.snap->bytes;
   }
   return ZG_OK;
-}
-
-extern "C" int zg_shard_pass(zg_engine* e, const zg_check* queries, uint64_t n, int level, uint64_t* n_sub) {
-  NEED_SCHEMA(e, ZG_ENOSCHEMA);
-  if ((!queries && n) || !n_sub || level < 0 || level > ZG_MAX_DEPTH + 2) return fail(ZG_EINVAL, "bad argument");
-  std::lock_guard<FairMutex> g(e->mu);
-  if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
-  if (!e->dev.snap) return fail(ZG_ENOSNAPSHOT, "no snapshot published (call zg_publish)");
-  e->dev.now = now_of(e);
-  std::string err;
-  int rc = e->dev.shard_pass(queries, n, level, n_sub, &err);
-  return rc ? fail(rc, err) : ZG_OK;
-}
-extern "C" int zg_shard_subqueries(zg_engine* e, int level, zg_check* out, uint64_t n) {
-  NEED_SCHEMA(e, ZG_ENOSCHEMA);
-  if ((!out && n) || level < 0) return fail(ZG_EINVAL, "bad argument");
-  std::lock_guard<FairMutex> g(e->mu);
-  if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
-  std::string err;
-  int rc = e->dev.shard_subqueries(level, out, n, &err);
-  return rc ? fail(rc, err) : ZG_OK;
-}
-extern "C" int zg_shard_fold(zg_engine* e, int level, const uint8_t* child_vals, uint64_t n_sub, uint8_t* out) {
-  NEED_SCHEMA(e, ZG_ENOSCHEMA);
-  if ((!child_vals && n_sub) || level < 0) return fail(ZG_EINVAL, "bad argument");
-  std::lock_guard<FairMutex> g(e->mu);
-  if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
-  std::string err;
-  int rc = e->dev.shard_fold(level, child_vals, n_sub, out, &err);
-  return rc ? fail(rc, err) : ZG_OK;
 }
 
 // ---- sharded store, device-resident protocol (no host staging between passes) ----

@@ -78,7 +78,6 @@ Device::~Device() {
     for (auto& b : *v) b.release();
   stage_in_.release();
   stage_out_.release();
-  shard_tmp_.release();
   route_ctrl_.release();
   lk_jobs_.release();
   lk_codes_.release();
@@ -734,115 +733,7 @@ int Device::check_host_multi(const std::vector<HostReq>& reqs, std::string* err)
   return ZG_OK;
 }
 
-// ---- sharded store: one pass per call; the host exchanges the raised sub-queries -----------
-//
-// Buffers per level lv: q_[lv] = this level's queries, val_[lv] = their leaf values,
-// q_[lv+1] / parent_[lv+1] = the sub-queries the pass raised (the same buffers the single-GPU
-// multi-pass loop uses; here their consumers live on other ranks).
-int Device::shard_pass(const zg_check* queries, uint64_t n, int level, uint64_t* n_sub, std::string* err) {
-  std::shared_ptr<Snapshot> s = snap;
-  if (!s) {
-    if (err) *err = "no snapshot published";
-    return ZG_ENOSNAPSHOT;
-  }
-  ZG_CUDA(cudaSetDevice(device));
-  const size_t lv = static_cast<size_t>(level);
-  if (q_.size() <= lv + 1) {
-    q_.resize(lv + 2);
-    parent_.resize(lv + 2);
-    val_.resize(lv + 2);
-  }
-  if (shard_nq_.size() <= lv) {
-    shard_nq_.resize(lv + 1);
-    shard_nsub_.resize(lv + 1);
-  }
-  shard_nq_[lv] = n;
-  shard_nsub_[lv] = 0;
-  *n_sub = 0;
-  if (n == 0) return ZG_OK;
-  const uint32_t L = s->max_leaves;
-  if (n * L >= (1ull << 32)) {
-    if (err) *err = "pass too large (n * leaves >= 2^32)";
-    return ZG_EINVAL;
-  }
-  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
-  // level > 0 queries arrive in a host buffer too; level 0 is staged apart from the raised-sub-query buffer q_[1]
-  DevBuf& qbuf = lv == 0 ? stage_in_ : q_[lv];  // q_[lv] (lv > 0) was the producer-side buffer of level lv-1 on
-                                              // THIS rank; its content was already read back by shard_subqueries
-  if (!qbuf.ensure(std::max<size_t>(n * sizeof(zg_check), subq_cap_ * sizeof(zg_check))) || !val_[lv].ensure(n * L + 4) ||
-      !q_[lv + 1].ensure(subq_cap_ * sizeof(zg_check)) || !parent_[lv + 1].ensure(subq_cap_ * 4)) {
-    if (err) *err = "out of device memory (shard pass buffers)";
-    return ZG_ENOMEM;
-  }
-  ZG_CUDA(cudaMemcpyAsync(qbuf.p, queries, n * sizeof(zg_check), cudaMemcpyHostToDevice, stream));
-  unsigned long long* ctrl = ctrl_.as<unsigned long long>();
-  ZG_CUDA(cudaMemsetAsync(ctrl + 2, 0, 16, stream));
-  ZG_CUDA(cudaMemsetAsync(val_[lv].p, 0, n * L + 4, stream));
-  int rc = run_pass(*s, qbuf.as<zg_check>(), n, val_[lv].as<uint8_t>(), nullptr, false, level == 0, q_[lv + 1].as<zg_check>(),
-                    parent_[lv + 1].as<uint32_t>(), stream, false, err);
-  if (rc) return rc;
-  unsigned long long host_ctrl[4];
-  ZG_CUDA(cudaMemcpyAsync(host_ctrl, ctrl, sizeof host_ctrl, cudaMemcpyDeviceToHost, stream));
-  ZG_CUDA(cudaEventRecord(last_done_, stream));
-  have_last_ = true;
-  ZG_CUDA(cudaStreamSynchronize(stream));
-  const uint32_t flags = static_cast<uint32_t>(host_ctrl[3] & 0xFFFFFFFFu);
-  if (host_ctrl[1] > subq_cap_) {
-    if (err) *err = "sub-query buffer overflow: raise zg_config.subquery_capacity or shrink the batch";
-    return ZG_ENOMEM;
-  }
-  if (flags & 1u) {
-    if (err) *err = "expansion stack overflow";
-    return ZG_ENOMEM;
-  }
-  shard_nsub_[lv] = host_ctrl[1];
-  *n_sub = host_ctrl[1];
-  checks += level == 0 ? n : 0;
-  ++passes;
-  return ZG_OK;
-}
-
-int Device::shard_subqueries(int level, zg_check* out, uint64_t n, std::string* err) {
-  const size_t lv = static_cast<size_t>(level);
-  if (lv >= shard_nsub_.size() || n != shard_nsub_[lv]) {
-    if (err) *err = "shard_subqueries: level / count mismatch";
-    return ZG_EINVAL;
-  }
-  if (n == 0) return ZG_OK;
-  ZG_CUDA(cudaSetDevice(device));
-  ZG_CUDA(cudaMemcpyAsync(out, q_[lv + 1].p, n * sizeof(zg_check), cudaMemcpyDeviceToHost, stream));
-  ZG_CUDA(cudaStreamSynchronize(stream));
-  return ZG_OK;
-}
-
-int Device::shard_fold(int level, const uint8_t* child_vals, uint64_t n_sub, uint8_t* out, std::string* err) {
-  std::shared_ptr<Snapshot> s = snap;
-  const size_t lv = static_cast<size_t>(level);
-  if (!s || lv >= shard_nq_.size() || n_sub != shard_nsub_[lv]) {
-    if (err) *err = "shard_fold: level / count mismatch";
-    return ZG_EINVAL;
-  }
-  const uint64_t n = shard_nq_[lv];
-  if (n == 0) return ZG_OK;
-  ZG_CUDA(cudaSetDevice(device));
-  const unsigned blk = 256;
-  if (n_sub) {
-    if (!shard_tmp_.ensure(n_sub)) return ZG_ENOMEM;
-    ZG_CUDA(cudaMemcpyAsync(shard_tmp_.p, child_vals, n_sub, cudaMemcpyHostToDevice, stream));
-    or_children_kernel<<<static_cast<unsigned>((n_sub + blk - 1) / blk), blk, 0, stream>>>(
-        parent_[lv + 1].as<uint32_t>(), shard_tmp_.as<uint8_t>(), n_sub, val_[lv].as<uint8_t>());
-    ++launches;
-  }
-  if (!stage_out_.ensure(n)) return ZG_ENOMEM;
-  const DevBuf& qbuf = lv == 0 ? stage_in_ : q_[lv];
-  fold_kernel<<<static_cast<unsigned>((n + blk - 1) / blk), blk, 0, stream>>>(
-      s->prog.as<uint8_t>(), qbuf.as<zg_check>(), n, s->max_leaves, val_[lv].as<uint8_t>(), stage_out_.as<uint8_t>(),
-      nullptr, nullptr, level == 0 ? 0 : 1);
-  ++launches;
-  ZG_CUDA(cudaMemcpyAsync(out, stage_out_.p, n, cudaMemcpyDeviceToHost, stream));
-  ZG_CUDA(cudaStreamSynchronize(stream));
-  return ZG_OK;
-}
+// ---- sharded store: one pass per call; the raised sub-queries are exchanged device to device -------------------
 
 int Device::route_by_owner(const zg_check* d_items, uint64_t n, int level, uint32_t n_dest, zg_check* d_routed, uint32_t* d_src,
                            uint64_t* counts, std::string* err) {
@@ -900,6 +791,9 @@ int Device::route_(const Item* d_items, uint64_t n, uint32_t n_dest, Owner owner
   return ZG_OK;
 }
 
+// Buffers per level lv: q_[lv] = this level's queries (stage_in_ at level 0), val_[lv] = their leaf values,
+// q_[lv+1] / parent_[lv+1] = the sub-queries the pass raised (the same buffers the single-GPU multi-pass loop
+// uses; here their consumers live on other ranks).
 int Device::shard_pass_dev(const zg_check* d_queries, uint64_t n, int level, uint64_t* n_sub, std::string* err) {
   std::shared_ptr<Snapshot> s = snap;
   if (!s) {

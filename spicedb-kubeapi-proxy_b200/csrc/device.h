@@ -128,21 +128,15 @@ class Device {
                       SubjectsAnswer* ans, std::string* err);
   uint64_t subject_lookups_walk = 0, subject_lookups_exhaustive = 0, subject_items_verified = 0;
 
-  // ---- object-hash sharded store: one pass at a time, sub-queries routed by the host ----
+  // ---- object-hash sharded store: one pass at a time, everything resident on the device (dist.DeviceShardedChecker) ----
   uint32_t shard_count = 1, shard_rank = 0;
-  // Evaluates `n` host queries as pass `level` (level 0: caller items; deeper: routed
-  // sub-queries, depth in flags). *n_sub = sub-queries this pass raised.
-  int shard_pass(const zg_check* queries, uint64_t n, int level, uint64_t* n_sub, std::string* err);
-  int shard_subqueries(int level, zg_check* out, uint64_t n, std::string* err);
-  // child_vals: one byte per raised sub-query (kValT|kValE bits) in emission order. out: one byte
-  // per query of the level: v1 codes at level 0, value bits deeper.
-  int shard_fold(int level, const uint8_t* child_vals, uint64_t n_sub, uint8_t* out, std::string* err);
-  // ---- the same protocol with everything resident on the device (dist.DeviceShardedChecker) ----
   // Bucketises n check items by owner = res % n_dest into d_routed (destination-major) with their source
   // indices in d_src; counts[d] (host) = items for destination d. d_items == nullptr: the sub-queries raised by
-  // pass `level` (shard_pass / shard_pass_dev).
+  // pass `level` (shard_pass_dev).
   int route_by_owner(const zg_check* d_items, uint64_t n, int level, uint32_t n_dest, zg_check* d_routed, uint32_t* d_src,
                      uint64_t* counts, std::string* err);
+  // Evaluates `n` device queries as pass `level` (level 0: caller items routed to this shard; deeper: routed
+  // sub-queries, depth in flags). *n_sub = sub-queries this pass raised.
   int shard_pass_dev(const zg_check* d_queries, uint64_t n, int level, uint64_t* n_sub, std::string* err);
   // d_child_vals: one byte per raised sub-query in ROUTED order, d_src = the source indices route_by_owner wrote.
   // d_out: one byte per query of the level (v1 codes when final_codes, else value bits).
@@ -265,7 +259,7 @@ class Device {
                                                       // [8 .. 9] events, [10] items landed, [11 .. 15] phase clocks
   std::vector<DevBuf> q_, parent_, val_;  // per pass level: queries, raising (query, leaf), leaf values
   std::vector<uint64_t> shard_nq_, shard_nsub_;  // sharded mode: queries / raised sub-queries per level
-  DevBuf shard_tmp_, route_ctrl_;
+  DevBuf route_ctrl_;
   DevBuf stage_in_, stage_out_, lk_jobs_, lk_codes_, lk_ids_;
   DevBuf rb_visited_, rb_front_[2], rb_cand_;
   DevBuf lb_params_, lb_owner_, lb_ctrl_, lb_keys_[2];  // batched lookups

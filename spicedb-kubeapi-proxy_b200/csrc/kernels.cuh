@@ -1036,18 +1036,6 @@ __global__ void fold_kernel(const uint8_t* prog, const zg_check* queries, unsign
   }
 }
 
-// Sharded store: values of routed sub-queries come back from their owners and are OR-ed into
-// the jobs that raised them.
-__global__ void or_children_kernel(const uint32_t* parent, const uint8_t* child_val, unsigned long long n,
-                                   uint8_t* parent_val) {
-  unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x;
-  if (i >= n) return;
-  const uint32_t bits = child_val[i] & (kValT | kValE);
-  if (!bits) return;
-  const uint32_t pj = parent[i];
-  atomicOr(reinterpret_cast<unsigned int*>(parent_val + (pj & ~3u)), bits << (8 * (pj & 3u)));
-}
-
 // ---- sharded store: device-side routing of checks / raised sub-queries to their owners ---------------
 //
 // owner(item) = item.res % n_dest. Two passes of a counting sort: per-destination counts (shared-memory

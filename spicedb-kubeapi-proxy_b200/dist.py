@@ -64,146 +64,12 @@ def max_over_ranks(value: float, group=None, device: str = "cpu") -> float:
 
 
 # ---------------------------------------------------------------------------------------------
-# Object-hash sharded STORE (north-star's other multi-GPU mode; DESIGN.md 7).
+# Object-hash sharded STORE (north-star's other multi-GPU mode; SURVEY.md 8e, DESIGN.md 7), device resident.
 #
-# Every rank owns the relationships whose resource id % world == rank. A check starts on the
-# owner of its resource; an edge to an object of another shard (or into a non-pure permission)
-# is raised as a sub-query. Ranks run pass by pass; between passes the raised sub-queries are
-# exchanged with one all-to-all (NCCL over NVLink on GPUs), until no rank raises any; values
-# then travel back level by level with the reverse all-to-all and are folded into the jobs that
-# raised them. Cross-shard traffic is 16 B per sub-query out, 1 B back.
-
-
-class TorchTransport:
-    """all-to-all of ragged byte arrays over torch.distributed (nccl: CUDA tensors, gloo: CPU)."""
-
-    def __init__(self, group=None, device: str | None = None):
-        self.group = group
-        self.rank = dist.get_rank(group)
-        self.world = dist.get_world_size(group)
-        self.device = device or ("cuda" if dist.get_backend(group) == "nccl" else "cpu")
-
-    def alltoall(self, send):
-        """send[d]: 1-D uint8 array for rank d -> list recv[s] of uint8 arrays from every rank s."""
-        counts = torch.tensor([int(a.size) for a in send], dtype=torch.int64, device=self.device)
-        rcounts = torch.empty_like(counts)
-        dist.all_to_all_single(rcounts, counts, group=self.group)
-        rc = [int(x) for x in rcounts.cpu()]
-        flat = np.concatenate([np.ascontiguousarray(a, dtype=np.uint8).ravel() for a in send]) if send else np.empty(0, np.uint8)
-        tin = torch.from_numpy(flat.copy() if flat.size else np.zeros(0, np.uint8)).to(self.device)
-        tout = torch.empty(sum(rc), dtype=torch.uint8, device=self.device)
-        dist.all_to_all_single(tout, tin, output_split_sizes=rc, input_split_sizes=[int(a.size) for a in send],
-                               group=self.group)
-        out, host, off = [], tout.cpu().numpy(), 0
-        for c in rc:
-            out.append(host[off:off + c].copy())
-            off += c
-        return out
-
-    def allreduce_sum(self, x: int) -> int:
-        t = torch.tensor([int(x)], dtype=torch.int64, device=self.device)
-        dist.all_reduce(t, op=dist.ReduceOp.SUM, group=self.group)
-        return int(t.item())
-
-
-class LocalTransport:
-    """The same interface for `world` virtual ranks living in ONE process (threads): used to
-    test the sharded protocol on a single GPU. Build with LocalTransport.cluster(world)."""
-
-    def __init__(self, rank, world, shared):
-        self.rank, self.world, self._s = rank, world, shared
-
-    @staticmethod
-    def cluster(world):
-        import threading
-
-        shared = {"box": [None] * world, "bar": threading.Barrier(world), "sum": [0] * world}
-        return [LocalTransport(r, world, shared) for r in range(world)]
-
-    def alltoall(self, send):
-        s = self._s
-        s["box"][self.rank] = [np.ascontiguousarray(a, dtype=np.uint8).ravel().copy() for a in send]
-        s["bar"].wait()
-        out = [s["box"][src][self.rank] for src in range(self.world)]
-        s["bar"].wait()
-        return out
-
-    def allreduce_sum(self, x):
-        s = self._s
-        s["sum"][self.rank] = int(x)
-        s["bar"].wait()
-        tot = sum(s["sum"])
-        s["bar"].wait()
-        return tot
-
-
-class ShardedStoreChecker:
-    """CheckBulkPermissions over an object-hash sharded store. Every rank calls check_bulk with the
-    SAME items; every rank gets the full answer vector. `engine` must have been created with
-    shard_rank=transport.rank, shard_count=transport.world and loaded with the full relationship
-    stream (it keeps only what it owns)."""
-
-    def __init__(self, engine, transport, check_dtype):
-        self.e, self.t, self.dtype = engine, transport, np.dtype(check_dtype)
-        self.stats = {"levels": 0, "subqueries_sent": 0, "bytes_sent": 0}
-
-    def _route(self, subs):
-        w = self.t.world
-        dest = subs["res"] % np.uint32(w)
-        groups = [np.flatnonzero(dest == d) for d in range(w)]  # stable partition, O(n * w), no sort
-        order = np.concatenate(groups) if groups else np.empty(0, np.int64)
-        return order, [subs[g].view(np.uint8) for g in groups]
-
-    def check_bulk(self, items: np.ndarray) -> np.ndarray:
-        items = np.ascontiguousarray(items, dtype=self.dtype)
-        w, r = self.t.world, self.t.rank
-        mine = np.nonzero(items["res"] % w == r)[0]
-        queries = items[mine]
-        levels = []
-        while True:
-            lv = len(levels)
-            nsub = self.e.shard_pass(queries, lv)
-            subs = self.e.shard_subqueries(lv, nsub)
-            order, parts = self._route(subs)
-            recv = self.t.alltoall(parts)
-            levels.append({"nq": int(queries.size), "nsub": int(nsub), "order": order,
-                           "recv_counts": [a.size // self.dtype.itemsize for a in recv]})
-            self.stats["subqueries_sent"] += int(nsub)
-            self.stats["bytes_sent"] += int(nsub) * self.dtype.itemsize
-            queries = np.concatenate(recv).view(self.dtype) if recv else np.empty(0, self.dtype)
-            if self.t.allreduce_sum(queries.size) == 0:
-                break
-            if lv > 60:
-                raise RuntimeError("sharded check did not converge within the dispatch depth")
-        self.stats["levels"] = max(self.stats["levels"], len(levels))
-        out_next = None
-        for lv in reversed(range(len(levels))):
-            L = levels[lv]
-            if lv == len(levels) - 1:
-                child = np.empty(0, np.uint8)  # the deepest level raised nothing
-            else:
-                # values of the level lv+1 queries go back to the ranks that raised them
-                rc = levels[lv]["recv_counts"]
-                offs = np.concatenate([[0], np.cumsum(rc)])
-                back = [out_next[offs[s]:offs[s + 1]] for s in range(w)]
-                got = self.t.alltoall(back)
-                flat = np.concatenate(got) if got else np.empty(0, np.uint8)
-                child = np.empty(L["nsub"], np.uint8)
-                child[L["order"]] = flat
-                self.stats["bytes_sent"] += int(flat.size)
-            out_next = self.e.shard_fold(lv, child, L["nq"])
-        # everyone learns every answer: 4-byte index + 1-byte code per owned check
-        payload = np.concatenate([mine.astype(np.uint32).view(np.uint8), out_next.astype(np.uint8)])
-        got = self.t.alltoall([payload] * w)
-        out = np.empty(items.size, np.uint8)
-        for g in got:
-            k = g.size // 5
-            out[g[: 4 * k].view(np.uint32)] = g[4 * k:]
-        return out
-
-
-# ---------------------------------------------------------------------------------------------
-# The same protocol with every buffer resident on the device (SURVEY.md 8e, north-star's mode).
+# Every rank owns the relationships whose resource id % world == rank. A check starts on the owner of its
+# resource; an edge to an object of another shard (or into a non-pure permission) is raised as a sub-query. Ranks
+# run pass by pass until no rank raises any; values then travel back level by level and are folded into the jobs
+# that raised them. Cross-shard traffic is 16 B per sub-query out, 1 B back.
 #
 # Per level: ONE kernel pass over the level's queries (zg_shard_pass_dev), a counting-sort kernel that bucketises
 # the raised sub-queries by owner (zg_shard_route_dev), an N-int count exchange and one all-to-all of the 16-byte
@@ -213,7 +79,8 @@ class ShardedStoreChecker:
 
 
 class TorchDeviceTransport:
-    """Ragged all-to-all of CUDA tensors over torch.distributed (backend nccl)."""
+    """Ragged all-to-all of tensors over torch.distributed: CUDA tensors over nccl, or CPU tensors over gloo
+    (device=torch.device("cpu"))."""
 
     def __init__(self, group=None, device=None):
         self.group = group
@@ -232,7 +99,8 @@ class TorchDeviceTransport:
         out = torch.empty(sum(recv_counts) * width, dtype=torch.uint8, device=self.device)
         dist.all_to_all_single(out, send, output_split_sizes=[c * width for c in recv_counts],
                                input_split_sizes=[c * width for c in send_counts], group=self.group)
-        torch.cuda.current_stream().synchronize()  # the engine's calls run on its own stream
+        if self.device.type == "cuda":
+            torch.cuda.current_stream().synchronize()  # the engine's calls run on its own stream
         return out
 
     def allreduce_sum(self, x: int) -> int:

@@ -1,6 +1,7 @@
 """world_size-2 gloo test of the N>1 host logic (spicedb-kubeapi-proxy_b200/dist.py):
 slicing, all-gather back to caller order, max-over-ranks timing. The evaluator is the
-CPU oracle here (there is no GPU); on the GPU box the same class wraps engine.check_bulk."""
+CPU oracle here (there is no GPU); on the GPU box the same class wraps engine.check_bulk.
+A world_size-3 test runs the sharded store's TorchDeviceTransport on CPU tensors."""
 import os
 import sys
 
@@ -78,8 +79,15 @@ def test_shard_bounds_cover_exactly():
             assert max(hi - lo for lo, hi in b) - min(hi - lo for lo, hi in b) <= 1
 
 
+def _a2a_part(src, dst):
+    """The items rank src sends rank dst: (src + dst) % 3 * 5 of them (ragged, some empty), 3 bytes each."""
+    n = (src + dst) % 3 * 5
+    return np.stack([np.full(n, 10 * src + dst), np.arange(n), np.full(n, 7)], axis=1).astype(np.uint8)
+
+
 def _a2a_worker(rank, world, port, q):
     sys.path.insert(0, ROOT)
+    import torch
     import torch.distributed as dist
 
     import zgpu  # noqa: F401
@@ -89,17 +97,20 @@ def _a2a_worker(rank, world, port, q):
     os.environ["MASTER_PORT"] = str(port)
     dist.init_process_group("gloo", rank=rank, world_size=world)
     try:
-        t = zdist.TorchTransport()
-        # rank r sends (r + d + 1) bytes of value 10*r + d to rank d (ragged, some empty)
-        send = [np.full((rank + d) % 3 * 5, 10 * rank + d, dtype=np.uint8) for d in range(world)]
-        recv = t.alltoall(send)
-        ok = all(np.array_equal(recv[s], np.full((s + rank) % 3 * 5, 10 * s + rank, dtype=np.uint8)) for s in range(world))
+        t = zdist.TorchDeviceTransport(device=torch.device("cpu"))
+        send_counts = [_a2a_part(rank, d).shape[0] for d in range(world)]
+        recv_counts = t.exchange_counts(send_counts)
+        send = torch.from_numpy(np.concatenate([_a2a_part(rank, d).ravel() for d in range(world)]))
+        got = t.alltoall(send, send_counts, recv_counts, 3)
+        want = np.concatenate([_a2a_part(s, rank).ravel() for s in range(world)])
+        ok = recv_counts == [_a2a_part(s, rank).shape[0] for s in range(world)] and np.array_equal(got.numpy(), want)
         q.put((rank, ok, t.allreduce_sum(rank + 1)))
     finally:
         dist.destroy_process_group()
 
 
-def test_torch_transport_ragged_alltoall_world3():
+def test_torch_device_transport_ragged_alltoall_world3():
+    """The transport of the device-resident sharded store (nccl in bench.py), here on CPU tensors over gloo."""
     import socket
 
     s = socket.socket()
@@ -114,25 +125,3 @@ def test_torch_transport_ragged_alltoall_world3():
     [p.join(timeout=60) for p in procs]
     assert [r[1] for r in res] == [True, True, True], res
     assert [r[2] for r in res] == [6, 6, 6]
-
-
-def test_local_transport_matches_semantics():
-    import threading
-
-    sys.path.insert(0, ROOT)
-    import zgpu  # noqa: F401
-    from spicedb_kubeapi_proxy_b200.dist import LocalTransport
-
-    ts = LocalTransport.cluster(3)
-    out = [None] * 3
-
-    def run(t):
-        send = [np.full(t.rank + d, 10 * t.rank + d, dtype=np.uint8) for d in range(3)]
-        recv = t.alltoall(send)
-        out[t.rank] = (all(np.array_equal(recv[s], np.full(s + t.rank, 10 * s + t.rank, dtype=np.uint8)) for s in range(3)),
-                       t.allreduce_sum(t.rank))
-
-    th = [threading.Thread(target=run, args=(t,)) for t in ts]
-    [x.start() for x in th]
-    [x.join() for x in th]
-    assert out == [(True, 3)] * 3

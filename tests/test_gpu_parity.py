@@ -555,114 +555,6 @@ def _items_from_strings(e, zg, checks):
     return items
 
 
-def _run_sharded(zg, schema, load, items, world=3):
-    """`world` virtual shards on this one GPU (threads + LocalTransport); returns rank 0's answers
-    after checking that every rank got the same vector."""
-    import threading
-
-    from spicedb_kubeapi_proxy_b200 import dist as zdist
-
-    ts = zdist.LocalTransport.cluster(world)
-    engines = [zg.Engine(schema, shard_rank=r, shard_count=world) for r in range(world)]
-    for e in engines:
-        load(e)
-        e.publish()
-    out, errs, checkers = [None] * world, [], []
-
-    def run(r):
-        try:
-            ck = zdist.ShardedStoreChecker(engines[r], ts[r], zg.CHECK_DTYPE)
-            checkers.append(ck)
-            out[r] = ck.check_bulk(items)
-        except Exception as ex:  # noqa: BLE001
-            errs.append(repr(ex))
-            ts[r]._s["bar"].abort()
-
-    th = [threading.Thread(target=run, args=(r,)) for r in range(world)]
-    [x.start() for x in th]
-    [x.join() for x in th]
-    assert not errs, errs
-    for r in range(1, world):
-        assert np.array_equal(out[r], out[0])
-    total = sum(e.num_tuples() for e in engines)
-    return out[0], total, checkers[0].stats
-
-
-@pytest.mark.parametrize("name,scale", [("cfg3", 0.005), ("cfg4", 0.001)])
-def test_sharded_store_equals_oracle_on_workloads(zg, name, scale):
-    """Object-hash sharded store (north-star's multi-GPU mode): relationships are split by
-    resource id % 3 over three engines, sub-queries cross shards between passes, and the answers
-    equal the oracle's on the whole store."""
-    from oracle.pyoracle import Oracle
-    from spicedb_kubeapi_proxy_b200 import workloads
-
-    w = workloads.by_name(name, scale)
-    o = Oracle(w.schema)
-    w.load_into(o)
-    items = w.check_items(o, zg.CHECK_DTYPE)[:6000]
-    got, total, stats = _run_sharded(zg, w.schema, w.load_into, items)
-    assert np.array_equal(got, o.check_bulk(items))
-    assert total == o_num_unique(w), "every relationship lives on exactly one shard"
-    assert stats["subqueries_sent"] > 0 and stats["levels"] >= 2
-
-
-@pytest.mark.parametrize("seed", range(6))
-def test_sharded_store_random_schemas(zg, seed):
-    """& / - / arrows / usersets / wildcards across shards, incl. the depth cap and cycles."""
-    from oracle.pyoracle import Oracle
-
-    rng = random.Random(900 + seed)
-    if seed < 3:
-        schema = randgen.FIXED_SCHEMAS[sorted(randgen.FIXED_SCHEMAS)[seed]]
-        model = randgen.model_from_schema(schema)
-    else:
-        schema, model = randgen.random_schema(rng)
-    rels = randgen.random_relationships(rng, model, n_obj=7, n_user=6, density=0.3)
-    checks = randgen.random_checks(rng, model, 500, n_obj=7, n_user=6)
-    o = Oracle(schema)
-    for r in rels:
-        o.touch(r)
-
-    def load(e):
-        ups = [(zg._lib.OP_TOUCH, r, 0) for r in rels]
-        for i in range(0, len(ups), 1000):
-            e.write_relationships(ups[i:i + 1000])
-
-    probe = zg.Engine(schema, host_only=True)  # same interning order as the shards: ids agree
-    load(probe)
-    items = _items_from_strings(probe, zg, checks)
-    got, _, _ = _run_sharded(zg, schema, load, items)
-    want = np.array([o.check(*split_rel(q)) for q in checks], dtype=np.uint8)
-    bad = [(q, int(g), int(x)) for q, g, x in zip(checks, got, want) if g != x]
-    assert not bad, bad[:5]
-
-
-def test_sharded_store_depth_cap_across_shards(zg):
-    from oracle.pyoracle import Oracle
-    from test_oracle_random import CHAIN
-
-    rels = [f"group:g{i}#member@group:g{i+1}#member" for i in range(51)] + ["group:g51#member@user:deep"]
-    rels += ["group:a#member@group:b#member", "group:b#member@group:a#member", "group:b#member@user:x"]
-    rels += [f"folder:f{i}#parent@folder:f{i+1}" for i in range(51)] + ["folder:f0#viewer@user:v"]
-    checks = ["group:g0#member@user:deep", "group:g1#member@user:deep", "group:g2#member@user:nobody",
-              "group:a#member@user:x", "group:a#member@user:y", "folder:f0#view@user:v", "folder:f0#view@user:w",
-              "folder:f0#not_view@user:v", "folder:f0#not_view@user:w", "folder:f40#view@user:v"]
-    o = Oracle(CHAIN)
-    for r in rels:
-        o.touch(r)
-
-    def load(e):
-        e.write_relationships([(zg._lib.OP_TOUCH, r, 0) for r in rels])
-
-    probe = zg.Engine(CHAIN, host_only=True)
-    load(probe)
-    items = _items_from_strings(probe, zg, checks)
-    got, _, stats = _run_sharded(zg, CHAIN, load, items)
-    assert list(got) == [o.check(*split_rel(q)) for q in checks]
-    assert list(got[:5]) == [255, 2, 1, 2, 255]
-    assert stats["levels"] > 20, "the 51-hop chain must cross shards level by level"
-
-
 def test_interleaved_writes_and_checks_stay_consistent(zg):
     """FullyConsistent (every call site in the reference sets it: pkg/authz/check.go:42-44):
     after each WriteRelationships / DeleteRelationships returns, checks and lookups observe it.
@@ -894,7 +786,8 @@ def test_one_engine_owning_several_gpus_equals_a_single_gpu_engine(zg):
 
 def _run_sharded_device(zg, schema, load, items, world=3):
     """The device-resident protocol (dist.DeviceShardedChecker) on `world` virtual shards of this one GPU: every
-    rank brings a slice of the batch as a CUDA tensor and gets that slice's answers back."""
+    rank brings a slice of the batch as a CUDA tensor and gets that slice's answers back. Returns the answers, the
+    relationships held over all shards and rank 0's checker stats."""
     import threading
 
     import torch
@@ -925,11 +818,14 @@ def _run_sharded_device(zg, schema, load, items, world=3):
     [x.start() for x in th]
     [x.join() for x in th]
     assert not errs, errs
-    return np.concatenate(out), checkers[0].stats
+    return np.concatenate(out), sum(e.num_tuples() for e in engines), checkers[0].stats
 
 
 @pytest.mark.parametrize("name,scale", [("cfg3", 0.005), ("cfg4", 0.001)])
 def test_device_resident_sharded_store_equals_oracle_on_workloads(zg, name, scale):
+    """Object-hash sharded store (north-star's multi-GPU mode): relationships are split by
+    resource id % 3 over three engines, sub-queries cross shards between passes, and the answers
+    equal the oracle's on the whole store."""
     from oracle.pyoracle import Oracle
     from spicedb_kubeapi_proxy_b200 import workloads
 
@@ -937,13 +833,15 @@ def test_device_resident_sharded_store_equals_oracle_on_workloads(zg, name, scal
     o = Oracle(w.schema)
     w.load_into(o)
     items = w.check_items(o, zg.CHECK_DTYPE)[:6000]
-    got, stats = _run_sharded_device(zg, w.schema, w.load_into, items)
+    got, total, stats = _run_sharded_device(zg, w.schema, w.load_into, items)
     assert np.array_equal(got, o.check_bulk(items))
+    assert total == o_num_unique(w), "every relationship lives on exactly one shard"
     assert stats["subqueries_sent"] > 0 and stats["levels"] >= 2
 
 
 @pytest.mark.parametrize("seed", range(6))
 def test_device_resident_sharded_store_random_schemas(zg, seed):
+    """& / - / arrows / usersets / wildcards across shards, incl. the depth cap and cycles."""
     from oracle.pyoracle import Oracle
 
     rng = random.Random(900 + seed)
@@ -966,7 +864,7 @@ def test_device_resident_sharded_store_random_schemas(zg, seed):
     probe = zg.Engine(schema, host_only=True)
     load(probe)
     items = _items_from_strings(probe, zg, checks)
-    got, _ = _run_sharded_device(zg, schema, load, items)
+    got, _, _ = _run_sharded_device(zg, schema, load, items)
     want = np.array([o.check(*split_rel(q)) for q in checks], dtype=np.uint8)
     bad = [(q, int(g), int(x)) for q, g, x in zip(checks, got, want) if g != x]
     assert not bad, bad[:5]
@@ -992,6 +890,7 @@ def test_device_resident_sharded_store_depth_cap_across_shards(zg):
     probe = zg.Engine(CHAIN, host_only=True)
     load(probe)
     items = _items_from_strings(probe, zg, checks)
-    got, stats = _run_sharded_device(zg, CHAIN, load, items)
+    got, _, stats = _run_sharded_device(zg, CHAIN, load, items)
     assert list(got) == [o.check(*split_rel(q)) for q in checks]
-    assert stats["levels"] > 20
+    assert list(got[:5]) == [255, 2, 1, 2, 255]
+    assert stats["levels"] > 20, "the 51-hop chain must cross shards level by level"
