@@ -58,10 +58,24 @@ type Client struct {
 	// then fails (pkg/authz/authz.go:93-97 turns an error into a denial) instead of answering from a
 	// store that may still hold revoked grants.
 	broken atomic.Bool
+	// sharded: the engine is a sharded handle (Shards), which answers checks and writes but refuses
+	// LookupResources / LookupSubjects; those go to the embedded SpiceDB
+	sharded bool
 }
 
 // AllDevices: every visible GPU from `device` on (zg_config.n_devices).
 const AllDevices = uint32(C.ZG_ALL_DEVICES)
+
+// Option adjusts the engine's configuration before it is created.
+type Option func(*C.zg_config)
+
+// Shards makes the one engine hold the n shards of an object-hash sharded store (zg_config.n_shards): shard k keeps
+// the relationships whose resource id % n == k and lives on device `device + k % nDevices` (with nDevices = 1, the n
+// shards share one GPU). For stores larger than one GPU. Checks and writes are answered by the engine;
+// LookupResources and LookupSubjects are delegated to the embedded SpiceDB.
+func Shards(n uint32) Option {
+	return func(cfg *C.zg_config) { cfg.n_shards = C.uint32_t(n) }
+}
 
 var errBroken = status.Error(codes.Unavailable, "gpu mirror is out of sync with SpiceDB and could not be rebuilt")
 
@@ -71,13 +85,16 @@ var errBroken = status.Error(codes.Unavailable, "gpu mirror is out of sync with 
 // nDevices > 1 (or AllDevices) makes the one engine own that many GPUs of the box, each holding a replica of the
 // snapshot and answering its slice of every bulk call: the proxy keeps a single client (pkg/proxy/options.go:81-82),
 // so this is how it uses more than one GPU.
-func New(ctx context.Context, inner v1.PermissionsServiceClient, schema string, device int, nDevices uint32) (*Client, error) {
+func New(ctx context.Context, inner v1.PermissionsServiceClient, schema string, device int, nDevices uint32, opts ...Option) (*Client, error) {
 	cfg := C.zg_config{device: C.int32_t(device), n_devices: C.uint32_t(nDevices)}
+	for _, o := range opts {
+		o(&cfg)
+	}
 	var eng *C.zg_engine
 	if err := call(func() C.int { return C.zg_engine_create(&cfg, &eng) }); err != nil {
 		return nil, err // fail closed: no CPU fallback inside the library
 	}
-	c := &Client{PermissionsServiceClient: inner, engine: eng}
+	c := &Client{PermissionsServiceClient: inner, engine: eng, sharded: cfg.n_shards > 1}
 	cs := C.CString(schema)
 	defer C.free(unsafe.Pointer(cs))
 	if err := call(func() C.int { return C.zg_load_schema(eng, cs, C.size_t(len(schema))) }); err != nil {
@@ -223,7 +240,10 @@ func (c *Client) CheckPermission(ctx context.Context, req *v1.CheckPermissionReq
 
 // LookupResources: pkg/authz/lookups.go:65-88 reads the stream until io.EOF and keeps
 // LOOKUP_PERMISSIONSHIP_HAS_PERMISSION entries; order is irrelevant (a set).
-func (c *Client) LookupResources(ctx context.Context, req *v1.LookupResourcesRequest, _ ...grpc.CallOption) (v1.PermissionsService_LookupResourcesClient, error) {
+func (c *Client) LookupResources(ctx context.Context, req *v1.LookupResourcesRequest, opts ...grpc.CallOption) (v1.PermissionsService_LookupResourcesClient, error) {
+	if c.sharded {
+		return c.PermissionsServiceClient.LookupResources(ctx, req, opts...)
+	}
 	if c.broken.Load() {
 		return nil, errBroken
 	}
@@ -294,7 +314,7 @@ func (s *sliceStream) RecvMsg(any) error            { return io.EOF }
 // lookups only. The concrete subjects come first, then -- when a wildcard grants the permission and the
 // request includes wildcards -- "*" with its excluded subjects. Like the rest of this file: never compiled.
 func (c *Client) LookupSubjects(ctx context.Context, req *v1.LookupSubjectsRequest, opts ...grpc.CallOption) (v1.PermissionsService_LookupSubjectsClient, error) {
-	if req.GetContext() != nil || req.GetOptionalConcreteLimit() != 0 || req.GetOptionalCursor() != nil {
+	if c.sharded || req.GetContext() != nil || req.GetOptionalConcreteLimit() != 0 || req.GetOptionalCursor() != nil {
 		return c.PermissionsServiceClient.LookupSubjects(ctx, req, opts...)
 	}
 	if c.broken.Load() {

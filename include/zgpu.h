@@ -87,7 +87,13 @@ typedef struct {
                                 holding a replica of the snapshot and answering its slice of every bulk call
                                 (SURVEY.md 8e mode 1: no data-path collective); ZG_ALL_DEVICES = every
                                 visible device from `device` on                                            */
-  uint32_t reserved;
+  uint32_t n_shards;         /* 0 / 1 = one store per device (above); S > 1 = this ONE handle holds the S shards of an
+                                object-hash sharded store: shard k keeps the relationships whose resource id % S == k
+                                and lives on device `device + k % D` (D = n_devices, 1 by default; with one GPU the
+                                S shards share it). Checks cross the shards in-process, sub-queries delivered through
+                                peer memory; every device pair must have peer access. Not with shard_count > 1;
+                                S <= 64. LookupResources / LookupSubjects / the list pre-filter, zg_check_bulk_device,
+                                the device-ingress calls and the zg_shard_*_dev calls are refused (ZG_EINVAL).    */
 } zg_config;
 #define ZG_ALL_DEVICES 0xFFFFFFFFu
 
@@ -161,6 +167,10 @@ typedef struct {
   uint64_t lookup_batches;     /* launch sequences that answered more than one LookupResources           */
   uint64_t lookups_batched;    /* LookupResources calls answered by those                                */
   uint64_t devices;            /* GPUs this engine owns (counters above are summed over them)            */
+  uint64_t shards;             /* zg_config.n_shards of a sharded handle, else 1                         */
+  uint64_t last_levels;        /* sharded handle, last coalesced group: pass levels run over the shards  */
+  uint64_t last_subqueries;    /*   sub-queries the shards raised to each other                          */
+  uint64_t last_round_trips;   /*   times the host waited for the devices                                */
 } zg_stats;
 
 /* ---- lifecycle --------------------------------------------------------- */
@@ -323,6 +333,10 @@ void zg_host_free(void *p);
  * class for subject id `res`. Returns 0 / ZG_E2BIG (*n_out = size). */
 int zg_debug_row(zg_engine *e, uint16_t rel_slot, uint32_t res, uint32_t cls, uint32_t *out,
                  uint64_t cap, uint64_t *n_out);
+/* The same row of shard `shard` of a sharded handle (zg_config.n_shards > 1): the host builder's arrays of the
+ * relationships that shard owns. ZG_EINVAL on any other engine or shard index. */
+int zg_debug_shard_row(zg_engine *e, uint32_t shard, uint16_t rel_slot, uint32_t res, uint32_t cls, uint32_t *out,
+                       uint64_t cap, uint64_t *n_out);
 
 /* ---- object-hash sharded store (one engine per GPU, shard_count > 1) --------
  * A check starts on the owner of its resource; an edge to an object owned by another shard (or

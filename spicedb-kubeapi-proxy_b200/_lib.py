@@ -35,7 +35,7 @@ class ZgpuError(RuntimeError):
 class _Config(C.Structure):
     _fields_ = [("device", C.c_int32), ("flags", C.c_uint32), ("subquery_capacity", C.c_uint64),
                 ("work_budget", C.c_uint32), ("shard_rank", C.c_uint16), ("shard_count", C.c_uint16),
-                ("n_devices", C.c_uint32), ("reserved", C.c_uint32)]
+                ("n_devices", C.c_uint32), ("n_shards", C.c_uint32)]
 
 
 class _RelStr(C.Structure):
@@ -66,7 +66,8 @@ class _Stats(C.Structure):
                 ("stack_spills", C.c_uint64), ("memo_batches", C.c_uint64), ("split_batches", C.c_uint64),
                 ("delta_publishes", C.c_uint64), ("full_publishes", C.c_uint64), ("last_publish_ms", C.c_double),
                 ("streamed_calls", C.c_uint64), ("lookup_batches", C.c_uint64), ("lookups_batched", C.c_uint64),
-                ("devices", C.c_uint64)]
+                ("devices", C.c_uint64), ("shards", C.c_uint64), ("last_levels", C.c_uint64),
+                ("last_subqueries", C.c_uint64), ("last_round_trips", C.c_uint64)]
 
 
 class _Update(C.Structure):
@@ -207,6 +208,8 @@ _SIGS = {
     "zg_shard_subjects_finish_dev": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]),
     "zg_debug_row": (C.c_int, [C.c_void_p, C.c_uint16, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64,
                                C.POINTER(C.c_uint64)]),
+    "zg_debug_shard_row": (C.c_int, [C.c_void_p, C.c_uint32, C.c_uint16, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64,
+                                     C.POINTER(C.c_uint64)]),
     "zg_host_alloc": (C.c_void_p, [C.c_size_t]),
     "zg_host_free": (None, [C.c_void_p]),
     "zg_list_scan": (C.c_int64, [C.c_char_p, C.c_size_t, C.c_uint32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64),
@@ -327,12 +330,13 @@ class Engine:
 
     def __init__(self, schema: str | None = None, device: int = -1, subquery_capacity: int = 0, work_budget: int = 0,
                  host_only: bool = False, forward_only: bool = False, shard_rank: int = 0, shard_count: int = 0,
-                 n_devices: int = 0):
+                 n_devices: int = 0, n_shards: int = 0):
         """host_only=True builds schema/store/snapshot without a GPU (CPU unit tests of
-        the host logic); every check/lookup on such an engine raises ZgpuError."""
+        the host logic); every check/lookup on such an engine raises ZgpuError. n_shards=S > 1: this one handle
+        holds the S shards of an object-hash sharded store (zg_config.n_shards)."""
         self._L = lib()
         cfg = _Config(device, (1 if host_only else 0) | (2 if forward_only else 0), subquery_capacity, work_budget,
-                      shard_rank, shard_count, n_devices & 0xFFFFFFFF, 0)
+                      shard_rank, shard_count, n_devices & 0xFFFFFFFF, n_shards)
         h = C.c_void_p()
         rc = self._L.zg_engine_create(C.byref(cfg), C.byref(h))
         if rc:
@@ -791,16 +795,21 @@ class Engine:
         self._ck(self._L.zg_shard_subjects_finish_dev(self._h, d_keys or None, n, d_ids or None, listed, excluded))
         return [int(listed[i]) for i in range(k)], [int(excluded[i]) for i in range(k)]
 
-    def debug_row(self, type_name, rel, res, cls=0, reverse=False) -> np.ndarray:
-        """Forward row (resource `res`, class) or, reverse=True, the reverse row of subject `res`."""
+    def debug_row(self, type_name, rel, res, cls=0, reverse=False, shard=None) -> np.ndarray:
+        """Forward row (resource `res`, class) or, reverse=True, the reverse row of subject `res`; shard=k: that row in
+        shard k of a sharded handle."""
         if reverse:
             cls |= 0x80000000
         cap = 1 << 10
         while True:
             out = np.empty(cap, dtype=np.uint32)
             n = C.c_uint64(0)
-            rc = self._L.zg_debug_row(self._h, self.slot_id(type_name, rel), int(res), int(cls), out.ctypes.data, cap,
-                                      C.byref(n))
+            slot = self.slot_id(type_name, rel)
+            if shard is None:
+                rc = self._L.zg_debug_row(self._h, slot, int(res), int(cls), out.ctypes.data, cap, C.byref(n))
+            else:
+                rc = self._L.zg_debug_shard_row(self._h, int(shard), slot, int(res), int(cls), out.ctypes.data, cap,
+                                                C.byref(n))
             if rc == E2BIG:
                 cap = int(n.value)
                 continue

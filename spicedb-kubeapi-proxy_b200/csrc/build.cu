@@ -43,16 +43,18 @@ struct BSlot {  // per relation slot
   } while (0)
 
 
-// dead_key = pool: tombstoned relationships sort after every real row
+// dead_key = pool: tombstoned relationships, and those another shard owns (res % own_count != own_rank), sort after
+// every real row
 __global__ void key_kernel(const zg_tuple* t, unsigned long long n, const BSlot* slots, const DCls* cls,
-                           unsigned long long dead_key, unsigned long long* rowkey, uint32_t* subj, uint32_t* idx) {
+                           unsigned long long dead_key, uint32_t own_rank, uint32_t own_count, unsigned long long* rowkey,
+                           uint32_t* subj, uint32_t* idx) {
   unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x;
   if (i >= n) return;
   const zg_tuple x = t[i];
   idx[i] = static_cast<uint32_t>(i);
   subj[i] = x.srel == kWildcard ? 0u : x.subj;
   unsigned long long key = dead_key;
-  if (!(x.flags & 1)) {
+  if (!(x.flags & 1) && (own_count < 2 || x.res % own_count == own_rank)) {
     const BSlot s = slots[x.rel];
     for (uint32_t k = 0; k < s.ncls; ++k) {
       const DCls c = cls[s.cls_begin + k];
@@ -183,7 +185,8 @@ std::string gpu_resource_lists(Snapshot* s, cudaStream_t st) {
 
 // Fills `s` (row_ptr, col, exp, rrow_ptr, rcol, resources) from the store's relationship list.
 // `lay` comes from Store::layout(); on return lay->cls has CF_EMPTY cleared for non-empty classes.
-std::string gpu_build_snapshot(const Store& store, const Schema& sc, HostSnapshot* lay, cudaStream_t st, Snapshot* s) {
+std::string gpu_build_snapshot(const Store& store, const Schema& sc, HostSnapshot* lay, cudaStream_t st, Snapshot* s,
+                               uint32_t owner_rank, uint32_t owner_count) {
   const uint64_t n = store.tuples.size();
   if (n >= 0xFFFFFFF0ull) return "more than 2^32 relationships in one snapshot";
   const uint64_t pool = lay->pool, rpool = lay->rpool;
@@ -226,8 +229,8 @@ std::string gpu_build_snapshot(const Store& store, const Schema& sc, HostSnapsho
   uint64_t n_unique = 0;
   if (n) {
     const int kbits = bits_for(pool);  // keys are < pool, tombstones == pool
-    key_kernel<<<grid, blk, 0, st>>>(d_t.as<zg_tuple>(), n, d_slots.as<BSlot>(), d_cls.as<DCls>(), pool,
-                                     d_key[0].as<unsigned long long>(), d_subj[0].as<uint32_t>(), d_idx[0].as<uint32_t>());
+    key_kernel<<<grid, blk, 0, st>>>(d_t.as<zg_tuple>(), n, d_slots.as<BSlot>(), d_cls.as<DCls>(), pool, owner_rank,
+                                     owner_count, d_key[0].as<unsigned long long>(), d_subj[0].as<uint32_t>(), d_idx[0].as<uint32_t>());
     // pass A: stable sort of tuple indices by subject
     size_t tmp_bytes = 0;
     cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, d_subj[0].as<uint32_t>(), d_subj[1].as<uint32_t>(),
@@ -410,11 +413,11 @@ std::string merge_direction(const HostDelta& h, bool with_exp, DevBuf& row_ptr, 
 }  // namespace
 
 std::string gpu_apply_delta(const Store& store, const Schema& sc, const HostSnapshot& lay, cudaStream_t st, Snapshot* s,
-                            std::vector<uint32_t>* cls_delta) {
+                            std::vector<uint32_t>* cls_delta, uint32_t owner_rank, uint32_t owner_count) {
   const bool with_exp = sc.has_expiry;
   HostDelta f, r;
   {
-    std::string perr = prepare_delta(store, sc, lay, &f, &r, cls_delta);
+    std::string perr = prepare_delta(store, sc, lay, &f, &r, cls_delta, owner_rank, owner_count);
     if (!perr.empty()) return perr;
   }
   if (f.ins_key.empty() && f.del_key.empty() && f.tch_key.empty()) return "";

@@ -179,6 +179,16 @@ struct zg_engine {
   static constexpr size_t kLookupCache = 128;
   HostSnapshot last_built;  // kept only for zg_debug_row / host-only engines
   bool keep_built = false;
+  // Sharded handle (zg_config.n_shards = S > 1): ONE store, S shards of its snapshot. Shard 0 is `dev`, shard k the
+  // device of replicas[k - 1] (own_rank k, own_count S); run_sharded drives a check group across them.
+  uint32_t n_shards = 1, shard_devices = 1;
+  void* group_pin = nullptr;  // a group's items, then its answers (pinned: the shards copy their slices from / to it)
+  size_t group_pin_cap = 0;
+  uint64_t last_levels = 0, last_subqueries = 0, last_round_trips = 0;
+  std::vector<HostSnapshot> shard_built;  // zg_debug_shard_row: the host builder's arrays per shard
+  ~zg_engine() {
+    if (group_pin) cudaFreeHost(group_pin);
+  }
   // Watch feed (pkg/authz/watch.go:29-31): what WriteRelationships / DeleteRelationships changed,
   // stamped with the revision that made it visible. Bounded: the oldest entries are dropped and
   // a reader that asks for them is told so (as SpiceDB does past its GC window).
@@ -221,6 +231,18 @@ static constexpr size_t kMaxLookupGroup = 64;  // = kMaxLookupBatch (kernels.cuh
 static const char* kShardedMsg =
     "sharded engine: use zg_shard_route_dev / zg_shard_pass_dev / zg_shard_fold_dev / zg_shard_unroute_dev "
     "(dist.DeviceShardedChecker)";
+static const char* kHandleLookupMsg =
+    "sharded handle (zg_config.n_shards > 1): LookupResources, LookupSubjects and the list pre-filter are not served "
+    "by it; run them on one engine per shard (dist.DeviceShardedLookup) or on a replica";
+static const char* kHandleDeviceMsg =
+    "sharded handle (zg_config.n_shards > 1): calls on device buffers and the device-ingress calls are not served by "
+    "it; use zg_check_bulk, zg_check_bulk_str or zg_check_bulk_packed";
+static const char* kHandleShardCallMsg =
+    "sharded handle (zg_config.n_shards > 1): the zg_shard_*_dev calls drive one shard per engine; this handle runs "
+    "the sharded protocol itself (zg_check_bulk)";
+static bool is_handle(const zg_engine* e) { return e->n_shards > 1; }
+// shard k of a sharded handle
+static Device& shard(zg_engine* e, uint32_t k) { return k == 0 ? e->dev : e->replicas[k - 1]->dev; }
 
 static int fail(int code, const std::string& msg) {
   g_err = msg;
@@ -245,8 +267,14 @@ static bool none_rel(const char* s) { return !s || !*s || std::strcmp(s, "...") 
 extern "C" int zg_engine_create(const zg_config* cfg, zg_engine** out) {
   if (!out) return fail(ZG_EINVAL, "out is NULL");
   *out = nullptr;
+  const uint32_t S = cfg && cfg->n_shards > 1 ? cfg->n_shards : 1;
+  if (S > 1 && cfg->shard_count > 1)
+    return fail(ZG_EINVAL, "n_shards > 1 holds every shard in this one handle, shard_count > 1 makes this engine one "
+                           "shard of several: set only one of them");
+  if (S > static_cast<uint32_t>(kMaxShards)) return fail(ZG_EINVAL, "n_shards exceeds 64 (the routing kernels' destinations)");
   zg_engine* e = new (std::nothrow) zg_engine();
   if (!e) return fail(ZG_ENOMEM, "out of memory");
+  e->n_shards = S;
   if (cfg && (cfg->flags & ZG_FLAG_HOST_ONLY)) {
     e->host_only = true;
     e->keep_built = true;
@@ -267,7 +295,54 @@ extern "C" int zg_engine_create(const zg_config* cfg, zg_engine** out) {
     e->dev.shard_count = cfg->shard_count;
     e->dev.shard_rank = cfg->shard_rank;
   }
-  if (cfg && cfg->n_devices > 1) {
+  if (S > 1) {
+    // shard k on device first + k % D; every pair of distinct devices reads and writes the other's memory
+    int visible = 0;
+    cudaGetDeviceCount(&visible);
+    const int first = e->dev.device;
+    const int D = cfg->n_devices == ZG_ALL_DEVICES ? visible - first : std::max<int>(1, static_cast<int>(cfg->n_devices));
+    if (D < 1 || first + D > visible) {
+      delete e;
+      return fail(ZG_EINVAL, "n_devices exceeds the visible CUDA devices");
+    }
+    const int used = std::min<int>(D, static_cast<int>(S));
+    for (int a = first; a < first + used; ++a)
+      for (int b = first; b < first + used; ++b) {
+        if (a == b) continue;
+        int can = 0;
+        if (cudaDeviceCanAccessPeer(&can, a, b) != cudaSuccess || !can) {
+          delete e;
+          return fail(ZG_EINVAL, "n_shards over several devices: device " + std::to_string(a) + " cannot access the memory of device " +
+                                     std::to_string(b) + " (peer access), which the sharded handle's exchange needs");
+        }
+        cudaSetDevice(a);
+        const cudaError_t pe = cudaDeviceEnablePeerAccess(b, 0);  // this process's context only
+        if (pe != cudaSuccess && pe != cudaErrorPeerAccessAlreadyEnabled) {
+          delete e;
+          return fail(ZG_ECUDA, std::string("cudaDeviceEnablePeerAccess: ") + cudaGetErrorString(pe));
+        }
+        cudaGetLastError();
+      }
+    cudaSetDevice(first);
+    e->shard_devices = static_cast<uint32_t>(used);
+    for (uint32_t k = 1; k < S; ++k) {
+      e->replicas.emplace_back(new Replica());
+      e->replicas.back()->worker.start();
+    }
+    std::vector<std::string> errs(S);
+    const zg_config c = *cfg;
+    on_all_devices(e, [&](Device& dev, size_t k) {
+      if (k) errs[k] = dev.init(first + static_cast<int>(k % static_cast<size_t>(D)), c.subquery_capacity, c.work_budget);
+      if (c.flags & ZG_FLAG_FORWARD_ONLY) dev.invert = false;
+      dev.shard_rank = dev.own_rank = static_cast<uint32_t>(k);
+      dev.shard_count = dev.own_count = S;
+    });
+    for (const auto& m : errs)
+      if (!m.empty()) {
+        delete e;
+        return fail(ZG_ECUDA, m);
+      }
+  } else if (cfg && cfg->n_devices > 1) {
     if (cfg->shard_count > 1) {
       delete e;
       return fail(ZG_EINVAL, "n_devices > 1 makes replicas; a sharded engine owns one device");
@@ -318,11 +393,14 @@ extern "C" int zg_load_schema(zg_engine* e, const char* dsl, size_t len) {
   e->schema = std::move(s);
   e->has_schema = true;
   e->store.reset(&e->schema);
-  e->store.shard_count = e->dev.shard_count;
-  e->store.shard_rank = e->dev.shard_rank;
+  if (!is_handle(e)) {  // a sharded handle's store holds every shard's relationships
+    e->store.shard_count = e->dev.shard_count;
+    e->store.shard_rank = e->dev.shard_rank;
+  }
   e->dev.snap.reset();
   e->dev.ingress_reset();  // the device mirror of the names
   for (auto& r : e->replicas) r->dev.snap.reset();
+  e->shard_built.clear();
   e->dirty = true;
   return ZG_OK;
 }
@@ -411,6 +489,14 @@ extern "C" int zg_apply_updates(zg_engine* e, const zg_update* u, uint64_t n) {
   return ZG_OK;
 }
 
+// A sharded handle answers from every shard's snapshot of one revision or from none: after a failed publish no
+// shard answers until a publish succeeds.
+static int publish_failed(zg_engine* e, const std::string& err) {
+  if (is_handle(e))
+    for (uint32_t k = 0; k < e->n_shards; ++k) shard(e, k).snap.reset();
+  return fail(ZG_ECUDA, err);
+}
+
 // Caller holds e->mu AND e->names exclusively.
 static int publish_locked(zg_engine* e) {
   (void)e->store.layout();  // settles the object capacities once: the replicas' publishes below only read the store
@@ -433,14 +519,30 @@ static int publish_locked(zg_engine* e) {
         errs[i] = err;
       });
       for (const auto& err : errs)
-        if (!err.empty()) return fail(ZG_ECUDA, err);
+        if (!err.empty()) return publish_failed(e, err);
       ++e->revision;
       e->store.journal_clear();
       e->last_built = HostSnapshot();
+      e->shard_built.clear();
+      e->dirty = false;
+      return ZG_OK;
+    }
+    if (is_handle(e)) {  // host-built shards: each holds the relationships it owns
+      std::vector<std::string> errs(e->n_shards);
+      on_all_devices(e, [&](Device& dev, size_t i) {
+        HostSnapshot h = e->store.build(dev.own_rank, dev.own_count);
+        errs[i] = h.err.empty() ? dev.publish(h, e->schema, e->revision + 1) : h.err;
+      });
+      for (const auto& err : errs)
+        if (!err.empty()) return publish_failed(e, err);
+      ++e->revision;
+      e->store.journal_clear();
+      e->shard_built.clear();
       e->dirty = false;
       return ZG_OK;
     }
   }
+  e->shard_built.clear();
   HostSnapshot h = e->store.build();
   if (!h.err.empty()) return fail(ZG_EINVAL, h.err);
   if (e->host_only) {
@@ -782,7 +884,7 @@ extern "C" int zg_watch_read(zg_engine* e, uint64_t since_revision, const char* 
 // there is something to publish; call it with NO lock held.
 static int publish_if_needed(zg_engine* e) {
   if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
-  if (e->dev.shard_count > 1) return fail(ZG_EINVAL, kShardedMsg);
+  if (e->dev.shard_count > 1 && !is_handle(e)) return fail(ZG_EINVAL, kShardedMsg);
   if (!e->dirty.load() && e->dev.snap) return ZG_OK;
   LOCK_DEVICE(e);
   LOCK_NAMES_UNIQUE(e);
@@ -790,19 +892,151 @@ static int publish_if_needed(zg_engine* e) {
   return ZG_OK;
 }
 
+// One coalesced group on a sharded handle: the levels of dist.DeviceShardedChecker.check_bulk, driven in this process.
+// items / out: n pinned host entries. Shard k brings the slice dist.shard_bounds gives it and routes it to the owners.
+// Per level, every shard writes its queries straight into the owners' inboxes (where, the host computes from every
+// shard's counts: the level's one round trip), each owner's pass starts when the shards delivering to it are done
+// (events, not host waits), and the values are folded back level by level where their owners left them.
+static int run_sharded(zg_engine* e, const zg_check* items, uint64_t n, uint8_t* out, std::string* err) {
+  const uint32_t S = e->n_shards;
+  auto lo = [&](uint32_t k) { return k * (n / S) + std::min<uint64_t>(k, n % S); };
+  std::vector<uint64_t> counts(size_t(S) * S, 0);  // [k * S + d]: queries shard k sends to shard d this level
+  std::vector<int> rcs(S, ZG_OK);
+  std::vector<std::string> errs(S);
+  auto first_error = [&]() {
+    for (uint32_t k = 0; k < S; ++k)
+      if (rcs[k]) {
+        *err = errs[k];
+        return rcs[k];
+      }
+    return static_cast<int>(ZG_OK);
+  };
+  const uint32_t now = now_of(e);
+  on_all_devices(e, [&](Device& dev, size_t k) {
+    dev.now = now;
+    rcs[k] = dev.peer_begin(items + lo(k), lo(k + 1) - lo(k), &counts[k * S], &errs[k]);
+  });
+  ++e->last_round_trips;
+  if (int rc = first_error()) return rc;
+  std::vector<PeerTable> tab(S);
+  std::vector<cudaEvent_t> wait(S);
+  auto events = [&](int level) {
+    for (uint32_t k = 0; k < S; ++k) wait[k] = shard(e, k).peer_event(level);
+  };
+  std::vector<uint64_t> nsub(S);
+  std::vector<char> overflow(S);
+  int level = 0;
+  for (;; ++level) {
+    uint64_t total = 0;
+    for (uint32_t d = 0; d < S; ++d) {
+      uint64_t at = 0;
+      for (uint32_t k = 0; k < S; ++k) {
+        tab[k].base[d] = at;
+        at += counts[size_t(k) * S + d];
+      }
+      zg_check* inbox = shard(e, d).peer_inbox(level, at, err);
+      if (!inbox) return ZG_ENOMEM;
+      for (uint32_t k = 0; k < S; ++k) tab[k].p[d] = inbox;
+      total += at;
+    }
+    if (total == 0) break;
+    if (level > ZG_MAX_DEPTH + 1) {
+      *err = "sub-query passes exceeded the depth cap";
+      return ZG_ECUDA;
+    }
+    on_all_devices(e, [&](Device& dev, size_t k) { rcs[k] = dev.peer_scatter(level, tab[k], &errs[k]); });
+    if (int rc = first_error()) return rc;
+    events(level);
+    on_all_devices(e, [&](Device& dev, size_t k) {
+      bool o = false;
+      rcs[k] = dev.peer_pass(level, wait, &nsub[k], &counts[k * S], &o, &errs[k]);
+      overflow[k] = o;
+    });
+    ++e->last_round_trips;
+    e->last_levels = std::max<uint64_t>(e->last_levels, static_cast<uint64_t>(level) + 1);
+    if (int rc = first_error()) return rc;
+    if (std::find(overflow.begin(), overflow.end(), 1) != overflow.end()) {
+      // a pass raised more sub-queries than its buffer holds: checks are independent, answer the group in halves
+      if (n < 2) {
+        *err = "sub-query buffer overflow on a single check: raise zg_config.subquery_capacity";
+        return ZG_ENOMEM;
+      }
+      ++e->dev.split_batches;
+      const uint64_t h = n / 2;
+      if (int rc = run_sharded(e, items, h, out, err)) return rc;
+      return run_sharded(e, items + h, n - h, out + h, err);
+    }
+    for (uint32_t k = 0; k < S; ++k) e->last_subqueries += nsub[k];
+  }
+  // values back: the deepest pass raised nothing; every shallower level folds in its children's values
+  for (int lv = level - 2; lv >= 0; --lv) {
+    for (uint32_t d = 0; d < S; ++d) {
+      tab[0].p[d] = const_cast<uint8_t*>(shard(e, d).peer_values(lv + 1));
+      tab[0].base[d] = 0;
+    }
+    events(lv + 1);
+    on_all_devices(e, [&](Device& dev, size_t k) { rcs[k] = dev.peer_fold(lv, tab[0], wait, &errs[k]); });
+    if (int rc = first_error()) return rc;
+  }
+  for (uint32_t d = 0; d < S; ++d) {
+    tab[0].p[d] = const_cast<uint8_t*>(shard(e, d).peer_values(0));
+    tab[0].base[d] = 0;
+  }
+  events(0);
+  on_all_devices(e, [&](Device& dev, size_t k) { rcs[k] = dev.peer_finish(tab[0], wait, out + lo(k), &errs[k]); });
+  ++e->last_round_trips;
+  return first_error();
+}
+
 // Runs one group of queued requests; the caller holds the device lock.
 static void run_group(zg_engine* e, std::vector<BatchReq*>& group) {
   int rc = ZG_OK;
   std::string err;
-  if (e->dev.shard_count > 1) {
+  bool published = e->dev.snap != nullptr;
+  for (uint32_t k = 1; k < e->n_shards && !e->host_only; ++k) published = published && shard(e, k).snap;
+  if (e->dev.shard_count > 1 && !is_handle(e)) {
     rc = ZG_EINVAL;
     err = kShardedMsg;
   } else if (e->host_only) {
     rc = ZG_ECUDA;
     err = "host-only engine: no CUDA device, and libzgpu has no CPU fallback";
-  } else if (!e->dev.snap) {
+  } else if (!published) {
     rc = ZG_ENOSNAPSHOT;
     err = "no snapshot published (call zg_publish)";
+  } else if (is_handle(e)) {
+    uint64_t total = 0;
+    for (BatchReq* r : group) total += r->n;
+    const size_t bytes = total * (sizeof(zg_check) + 1);  // the items, then their answers
+    if (e->group_pin_cap < bytes) {
+      if (e->group_pin) cudaFreeHost(e->group_pin);
+      e->group_pin = nullptr;
+      e->group_pin_cap = 0;
+      if (cudaMallocHost(&e->group_pin, bytes) == cudaSuccess) e->group_pin_cap = bytes;
+      else cudaGetLastError();
+    }
+    if (!e->group_pin) {
+      rc = ZG_ENOMEM;
+      err = "out of pinned host memory (sharded handle staging)";
+    } else {
+      zg_check* items = static_cast<zg_check*>(e->group_pin);
+      uint64_t off = 0;
+      for (BatchReq* r : group) {
+        std::memcpy(items + off, r->items, r->n * sizeof(zg_check));
+        off += r->n;
+      }
+      uint8_t* answers = reinterpret_cast<uint8_t*>(items + total);
+      e->last_levels = e->last_subqueries = e->last_round_trips = 0;
+      rc = run_sharded(e, items, total, answers, &err);
+      off = 0;
+      for (BatchReq* r : group) {
+        if (!rc) std::memcpy(r->out, answers + off, r->n);
+        off += r->n;
+      }
+      if (group.size() > 1) {
+        ++e->dev.coalesced_launches;
+        e->dev.coalesced_requests += group.size();
+      }
+    }
   } else {
     std::vector<Device::HostReq> reqs;
     reqs.reserve(group.size());
@@ -910,6 +1144,7 @@ extern "C" int zg_check_bulk_device(zg_engine* e, const zg_check* d_items, uint6
   if ((!d_items || !d_out) && n) return fail(ZG_EINVAL, "NULL argument");
   std::lock_guard<FairMutex> g(e->mu);
   if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
+  if (is_handle(e)) return fail(ZG_EINVAL, kHandleDeviceMsg);
   if (e->dev.shard_count > 1) return fail(ZG_EINVAL, kShardedMsg);
   e->dev.now = now_of(e);
   std::string err;
@@ -922,6 +1157,7 @@ extern "C" int zg_count_alg_bytes(zg_engine* e, const zg_check* items, uint64_t 
   if (!items || !bytes) return fail(ZG_EINVAL, "NULL argument");
   std::lock_guard<FairMutex> g(e->mu);
   if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
+  if (is_handle(e)) return fail(ZG_EINVAL, kHandleDeviceMsg);
   e->dev.now = now_of(e);
   std::string err;
   void *d_in = nullptr, *d_out = nullptr;
@@ -1187,6 +1423,7 @@ extern "C" int zg_resolve_checks_packed_device(zg_engine* e, const char* res_typ
   if (!(res_type && relation && subj_type && (n == 0 || (d_res_ids && d_res_off && d_subj_ids && d_out))))
     return fail(ZG_EINVAL, "NULL argument");
   if (e->host_only) return fail(ZG_ECUDA, kHostOnlyMsg);
+  if (is_handle(e)) return fail(ZG_EINVAL, kHandleDeviceMsg);
   if (n == 0) return ZG_OK;
   LOCK_DEVICE(e);
   LOCK_NAMES_SHARED(e);
@@ -1205,6 +1442,7 @@ extern "C" int zg_check_bulk_packed_ingress(zg_engine* e, const char* res_type, 
   NEED_SCHEMA(e, ZG_ENOSCHEMA);
   if (!PACKED_ARGS_OK()) return fail(ZG_EINVAL, "NULL argument");
   if (e->host_only) return fail(ZG_ECUDA, kHostOnlyMsg);
+  if (is_handle(e)) return fail(ZG_EINVAL, kHandleDeviceMsg);
   if (e->dev.shard_count > 1) return fail(ZG_EINVAL, kShardedMsg);
   if (n == 0) return ZG_OK;
   int rc = publish_if_needed(e);
@@ -1447,7 +1685,7 @@ static void run_lookup_group(zg_engine* e, std::vector<zg_engine::LookupJob*>& g
     }
   };
   if (e->host_only) return fail_all(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
-  if (e->dev.shard_count > 1) return fail_all(ZG_EINVAL, kShardedMsg);
+  if (e->dev.shard_count > 1) return fail_all(ZG_EINVAL, is_handle(e) ? kHandleLookupMsg : kShardedMsg);
   if (e->dirty.load() || !e->dev.snap) {
     LOCK_NAMES_UNIQUE(e);
     int rc = publish_locked(e);
@@ -1719,7 +1957,7 @@ static int lookup_subjects_ids(zg_engine* e, uint16_t perm, uint32_t res, uint16
     return fail(ZG_EINVAL, "unknown subject type or relation");
   if (option != ZG_WILDCARDS_INCLUDE && option != ZG_WILDCARDS_EXCLUDE) return fail(ZG_EINVAL, "unknown wildcard option");
   if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
-  if (e->dev.shard_count > 1) return fail(ZG_EINVAL, kShardedMsg);
+  if (e->dev.shard_count > 1) return fail(ZG_EINVAL, is_handle(e) ? kHandleLookupMsg : kShardedMsg);
   LOCK_DEVICE(e);
   if (e->dirty.load() || !e->dev.snap) {
     LOCK_NAMES_UNIQUE(e);
@@ -1782,7 +2020,7 @@ extern "C" int zg_lookup_subjects_str(zg_engine* e, const char* res_type, const 
     if (wildcard_option != ZG_WILDCARDS_INCLUDE && wildcard_option != ZG_WILDCARDS_EXCLUDE)
       return fail(ZG_EINVAL, "unknown wildcard option");
     if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
-    if (e->dev.shard_count > 1) return fail(ZG_EINVAL, kShardedMsg);
+    if (e->dev.shard_count > 1) return fail(ZG_EINVAL, is_handle(e) ? kHandleLookupMsg : kShardedMsg);
   } else {
     rc = lookup_subjects_ids(e, static_cast<uint16_t>(p), res, static_cast<uint16_t>(st), sr, wildcard_option, &ans);
     if (rc) return rc;
@@ -1878,6 +2116,7 @@ extern "C" int zg_list_prefilter(zg_engine* e, const char* body, size_t len, uin
   if (!body || !out_len || !tpl) return fail(ZG_EINVAL, "NULL argument");
   if (!tpl->res_type || !tpl->permission || !tpl->subj_type || !tpl->subj_id) return fail(ZG_EINVAL, "NULL template field");
   if (mode > ZG_LIST_PROTOBUF) return fail(ZG_EINVAL, "unknown mode");
+  if (is_handle(e) && !e->host_only) return fail(ZG_EINVAL, kHandleLookupMsg);
   // 1. the allowed ids (one LookupResources on the GPU; concurrent list requests share launches)
   std::vector<uint32_t> ids;
   std::string self;
@@ -1954,7 +2193,11 @@ extern "C" int zg_stats_get(zg_engine* e, zg_stats* out) {
   out->lookup_batches = e->dev.lookup_batches;
   out->lookups_batched = e->dev.lookups_batched;
   if (!e->host_only) e->dev.read_events(&out->stack_spills, &out->memo_batches);
-  out->devices = 1 + e->replicas.size();
+  out->devices = is_handle(e) ? e->shard_devices : 1 + e->replicas.size();
+  out->shards = e->n_shards;
+  out->last_levels = e->last_levels;
+  out->last_subqueries = e->last_subqueries;
+  out->last_round_trips = e->last_round_trips;
   for (auto& r : e->replicas) {
     const Device& d = r->dev;
     out->checks += d.checks;
@@ -1971,6 +2214,11 @@ extern "C" int zg_stats_get(zg_engine* e, zg_stats* out) {
     out->tuples = e->dev.snap->n_tuples;
     out->snapshot_bytes = e->dev.snap->bytes;
   }
+  for (uint32_t k = 1; k < e->n_shards && !e->host_only; ++k)  // a sharded handle: every shard's part
+    if (const auto s = shard(e, k).snap) {
+      out->tuples += s->n_tuples;
+      out->snapshot_bytes += s->bytes;
+    }
   return ZG_OK;
 }
 
@@ -1979,6 +2227,7 @@ extern "C" int zg_stats_get(zg_engine* e, zg_stats* out) {
   NEED_SCHEMA(e, ZG_ENOSCHEMA);                                                                                       \
   std::lock_guard<FairMutex> g(e->mu);                                                                               \
   if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");      \
+  if (is_handle(e)) return fail(ZG_EINVAL, kHandleShardCallMsg);                                                     \
   if (!e->dev.snap) return fail(ZG_ENOSNAPSHOT, "no snapshot published (call zg_publish)");
 
 extern "C" int zg_shard_route_dev(zg_engine* e, const zg_check* d_items, uint64_t n, int level, uint32_t n_dest,
@@ -2019,6 +2268,7 @@ extern "C" int zg_shard_unroute_dev(zg_engine* e, const uint32_t* d_src, const u
   NEED_SCHEMA(e, ZG_ENOSCHEMA);                                                                                       \
   std::lock_guard<FairMutex> g(e->mu);                                                                               \
   if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");      \
+  if (is_handle(e)) return fail(ZG_EINVAL, kHandleShardCallMsg);                                                     \
   if (e->dev.shard_count < 2) return fail(ZG_EINVAL, unsharded_msg);                                                 \
   if (!e->dev.snap) return fail(ZG_ENOSNAPSHOT, "no snapshot published (call zg_publish)");
 #define SHARD_LOOKUP_PROLOGUE() SHARD_ONLY_PROLOGUE("not a sharded engine: use zg_lookup_resources")
@@ -2157,6 +2407,34 @@ extern "C" int zg_shard_subjects_finish_dev(zg_engine* e, const uint64_t* d_keys
   return rc ? fail(rc, err) : ZG_OK;
 }
 
+static int debug_row_of(const zg_engine* e, const HostSnapshot& h, uint16_t rel_slot, uint32_t res, uint32_t cls, uint32_t* out,
+                        uint64_t cap, uint64_t* n_out) {
+  const Schema& sc = e->schema;
+  if (rel_slot >= sc.slots.size() || sc.slots[rel_slot].is_perm) return fail(ZG_EINVAL, "not a relation");
+  const DRel& r = h.rels[sc.slots[rel_slot].rel_index];
+  *n_out = 0;
+  if (cls & 0x80000000u) {  // reverse row: `res` is the SUBJECT id, result = resources listing it
+    cls &= 0x7FFFFFFFu;
+    if (cls >= r.ncls) return fail(ZG_EINVAL, "class out of range");
+    const DCls& c = h.cls[r.cls_begin + cls];
+    const uint32_t row = c.sslot == kWildcard ? 0u : res;
+    if (row >= c.nsubj) return ZG_OK;
+    const uint64_t ri = c.rrow_base + uint64_t(row) * c.rstride;
+    uint32_t b = h.rrow_ptr[ri], en = h.rrow_ptr[ri + 1];
+    *n_out = en - b;
+    if (en - b > cap) return ZG_E2BIG;
+    for (uint32_t i = b; i < en; ++i) out[i - b] = h.rcol[i];
+    return ZG_OK;
+  }
+  if (cls >= r.ncls) return fail(ZG_EINVAL, "class out of range");
+  if (res >= r.nres) return ZG_OK;
+  uint64_t idx = r.row_base + uint64_t(res) * r.stride + cls;
+  uint32_t b = h.row_ptr[idx], en = h.row_ptr[idx + 1];
+  *n_out = en - b;
+  if (en - b > cap) return ZG_E2BIG;
+  for (uint32_t i = b; i < en; ++i) out[i - b] = h.col[i];
+  return ZG_OK;
+}
 extern "C" int zg_debug_row(zg_engine* e, uint16_t rel_slot, uint32_t res, uint32_t cls, uint32_t* out, uint64_t cap,
                             uint64_t* n_out) {
   NEED_SCHEMA(e, ZG_ENOSCHEMA);
@@ -2168,31 +2446,22 @@ extern "C" int zg_debug_row(zg_engine* e, uint16_t rel_slot, uint32_t res, uint3
     e->last_built = e->store.build();
     if (!e->last_built.err.empty()) return fail(ZG_EINVAL, e->last_built.err);
   }
-  const Schema& sc = e->schema;
-  if (rel_slot >= sc.slots.size() || sc.slots[rel_slot].is_perm) return fail(ZG_EINVAL, "not a relation");
-  const DRel& r = e->last_built.rels[sc.slots[rel_slot].rel_index];
-  *n_out = 0;
-  if (cls & 0x80000000u) {  // reverse row: `res` is the SUBJECT id, result = resources listing it
-    cls &= 0x7FFFFFFFu;
-    if (cls >= r.ncls) return fail(ZG_EINVAL, "class out of range");
-    const DCls& c = e->last_built.cls[r.cls_begin + cls];
-    const uint32_t row = c.sslot == kWildcard ? 0u : res;
-    if (row >= c.nsubj) return ZG_OK;
-    const uint64_t ri = c.rrow_base + uint64_t(row) * c.rstride;
-    uint32_t b = e->last_built.rrow_ptr[ri], en = e->last_built.rrow_ptr[ri + 1];
-    *n_out = en - b;
-    if (en - b > cap) return ZG_E2BIG;
-    for (uint32_t i = b; i < en; ++i) out[i - b] = e->last_built.rcol[i];
-    return ZG_OK;
+  return debug_row_of(e, e->last_built, rel_slot, res, cls, out, cap, n_out);
+}
+extern "C" int zg_debug_shard_row(zg_engine* e, uint32_t shard, uint16_t rel_slot, uint32_t res, uint32_t cls, uint32_t* out,
+                                  uint64_t cap, uint64_t* n_out) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (!n_out) return fail(ZG_EINVAL, "NULL n_out");
+  if (!is_handle(e) || shard >= e->n_shards) return fail(ZG_EINVAL, "not a shard of a sharded handle (zg_config.n_shards)");
+  LOCK_DEVICE(e);
+  LOCK_NAMES_UNIQUE(e);
+  if (e->shard_built.size() != e->n_shards) e->shard_built.assign(e->n_shards, HostSnapshot());
+  HostSnapshot& h = e->shard_built[shard];
+  if (h.rels.empty() && !e->schema.rel_slots.empty()) {
+    h = e->store.build(shard, e->n_shards);
+    if (!h.err.empty()) return fail(ZG_EINVAL, h.err);
   }
-  if (cls >= r.ncls) return fail(ZG_EINVAL, "class out of range");
-  if (res >= r.nres) return ZG_OK;
-  uint64_t idx = r.row_base + uint64_t(res) * r.stride + cls;
-  uint32_t b = e->last_built.row_ptr[idx], en = e->last_built.row_ptr[idx + 1];
-  *n_out = en - b;
-  if (en - b > cap) return ZG_E2BIG;
-  for (uint32_t i = b; i < en; ++i) out[i - b] = e->last_built.col[i];
-  return ZG_OK;
+  return debug_row_of(e, h, rel_slot, res, cls, out, cap, n_out);
 }
 
 extern "C" const char* zg_build_info(void) { return zg::build_info(); }

@@ -180,9 +180,10 @@ struct HostDelta {
 
 // Net effect of the store's journal as sorted forward / reverse deltas (several applies may precede one publish).
 // cls_delta: per-class change of the relationship count. Returns "", "relayout" (an object beyond the capacities
-// of the resident layout) or an error.
+// of the resident layout) or an error. Owner filter (rank, count): only the entries whose resource id % count == rank
+// (one shard of a sharded handle, Store::build).
 inline std::string prepare_delta(const Store& store, const Schema& sc, const HostSnapshot& lay, HostDelta* f, HostDelta* r,
-                                 std::vector<uint32_t>* cls_delta) {
+                                 std::vector<uint32_t>* cls_delta, uint32_t owner_rank = 0, uint32_t owner_count = 1) {
   struct Net {
     zg_tuple t;
     bool was, is;
@@ -191,6 +192,7 @@ inline std::string prepare_delta(const Store& store, const Schema& sc, const Hos
   std::unordered_map<Key, Net, KeyHash> net;
   net.reserve(store.journal.size() * 2);
   for (const auto& j : store.journal) {
+    if (owner_count > 1 && j.t.res % owner_count != owner_rank) continue;
     const Key k = key_of(j.t);
     auto it = net.find(k);
     const bool now_is = j.kind != Store::kDeleted;

@@ -88,6 +88,12 @@ Device::~Device() {
   rb_cand_.release();
   for (auto* b : {&lb_params_, &lb_owner_, &lb_ctrl_, &lb_keys_[0], &lb_keys_[1]}) b->release();
   for (auto* b : {&ls_jobs_, &ls_codes_, &ls_has_, &ls_ids_, &ls_ctrl_}) b->release();
+  for (auto& l : pl_)
+    for (auto* b : {&l.in, &l.val, &l.out, &l.raised, &l.parent, &l.pos}) b->release();
+  for (auto* b : {&home_, &home_pos_, &home_out_, &peer_ctrl_}) b->release();
+  if (pin_peer_) cudaFreeHost(pin_peer_);
+  for (cudaEvent_t ev : ev_peer_)
+    if (ev) cudaEventDestroy(ev);
   if (pin_in_) cudaFreeHost(pin_in_);
   if (pin_out_) cudaFreeHost(pin_out_);
   if (pin_ready_) cudaFreeHost(pin_ready_);
@@ -173,7 +179,7 @@ std::string Device::publish_gpu(const Store& store, const Schema& sc, uint64_t r
   cudaEventCreate(&e0);
   cudaEventCreate(&e1);
   cudaEventRecord(e0, stream);
-  std::string err = gpu_build_snapshot(store, sc, &lay, stream, s.get());
+  std::string err = gpu_build_snapshot(store, sc, &lay, stream, s.get(), own_rank, own_count);
   cudaEventRecord(e1, stream);
   cudaEventSynchronize(e1);
   float ms = 0;
@@ -198,7 +204,7 @@ std::string Device::verify_snapshot(Snapshot& sn, const Store& store, const Sche
     if (!rerr.empty()) return rerr;
   }
   cudaStreamSynchronize(stream);
-  HostSnapshot h = store.build();
+  HostSnapshot h = store.build(own_rank, own_count);
   if (!h.err.empty()) return h.err;
   auto same = [&](const DevBuf& d, const std::vector<uint32_t>& v, const char* what) -> std::string {
     std::vector<uint32_t> got(v.size());
@@ -235,7 +241,9 @@ std::string Device::verify_against_host(const Store& store, const Schema& sc) {
 std::string Device::publish_delta(const Store& store, const Schema& sc, uint64_t revision) {
   constexpr size_t kMaxDelta = 1u << 16;
   std::shared_ptr<Snapshot> s = snap;
-  if (!s || !s->delta_ok || !store.journal_ok || shard_count > 1 || store.journal.size() > kMaxDelta || !store.layout_stable())
+  // an engine that is one shard of a store per process (shard_count > 1 over a store of its own) always rebuilds
+  const bool own_store_shard = shard_count > 1 && own_count < 2;
+  if (!s || !s->delta_ok || !store.journal_ok || own_store_shard || store.journal.size() > kMaxDelta || !store.layout_stable())
     return "full";
   cudaSetDevice(device);
   HostSnapshot lay = store.layout();  // same capacities as the resident snapshot: same bases
@@ -247,7 +255,7 @@ std::string Device::publish_delta(const Store& store, const Schema& sc, uint64_t
   cudaEventCreate(&e1);
   cudaEventRecord(e0, stream);
   std::vector<uint32_t> cls_delta;
-  std::string err = gpu_apply_delta(store, sc, lay, stream, s.get(), &cls_delta);
+  std::string err = gpu_apply_delta(store, sc, lay, stream, s.get(), &cls_delta, own_rank, own_count);
   cudaEventRecord(e1, stream);
   cudaEventRecord(last_done_, stream);
   have_last_ = true;
@@ -894,6 +902,164 @@ int Device::unroute(const uint32_t* d_src, const uint8_t* d_val, uint64_t n, uin
   unroute_kernel<<<static_cast<unsigned>((n + 255) / 256), 256, 0, stream>>>(d_src, d_val, n, d_out);
   ++launches;
   ZG_CUDA(cudaGetLastError());
+  ZG_CUDA(cudaEventRecord(last_done_, stream));
+  have_last_ = true;
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  return ZG_OK;
+}
+
+// ---- sharded handle (capi.cu run_sharded): the levels of DeviceShardedChecker, exchanged through peer memory --------
+static_assert(kMaxShards == kMaxRouteDest, "a PeerTable holds every routing destination");
+
+int Device::peer_begin(const zg_check* h_items, uint64_t n, uint64_t* counts, std::string* err) {
+  for (uint32_t d = 0; d < own_count; ++d) counts[d] = 0;
+  home_n_ = n;
+  ZG_CUDA(cudaSetDevice(device));
+  if (!ev_peer_[0])
+    for (cudaEvent_t& ev : ev_peer_) ZG_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  if (!pin_peer_) ZG_CUDA(cudaMallocHost(&pin_peer_, (4 + kMaxShards) * sizeof(unsigned long long)));
+  if (!peer_ctrl_.ensure(2 * kMaxShards * sizeof(unsigned long long)) || !home_.ensure(n * sizeof(zg_check)) ||
+      !home_pos_.ensure(n * 4) || !home_out_.ensure(n)) {
+    if (err) *err = "out of device memory (sharded handle buffers)";
+    return ZG_ENOMEM;
+  }
+  if (n == 0) return ZG_OK;
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  unsigned long long* d_counts = peer_ctrl_.as<unsigned long long>();
+  ZG_CUDA(cudaMemcpyAsync(home_.p, h_items, n * sizeof(zg_check), cudaMemcpyHostToDevice, stream));
+  ZG_CUDA(cudaMemsetAsync(d_counts, 0, kMaxShards * sizeof(unsigned long long), stream));
+  const unsigned grid = static_cast<unsigned>(std::min<uint64_t>((n + 255) / 256, static_cast<uint64_t>(sm_count_) * 8));
+  route_count_kernel<<<grid, 256, 0, stream>>>(home_.as<zg_check>(), n, own_count, d_counts);
+  ZG_CUDA(cudaGetLastError());
+  ++launches;
+  ZG_CUDA(cudaMemcpyAsync(pin_peer_, d_counts, own_count * sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaEventRecord(last_done_, stream));
+  have_last_ = true;
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  for (uint32_t d = 0; d < own_count; ++d) counts[d] = pin_peer_[d];
+  return ZG_OK;
+}
+
+zg_check* Device::peer_inbox(int level, uint64_t n, std::string* err) {
+  const size_t lv = static_cast<size_t>(level);
+  if (pl_.size() <= lv) pl_.resize(lv + 1);
+  PeerLevel& L = pl_[lv];
+  L.nq = n;
+  L.nsub = 0;
+  if (cudaSetDevice(device) != cudaSuccess || !L.in.ensure(std::max<uint64_t>(n, 1) * sizeof(zg_check))) {
+    if (err) *err = "out of device memory (sharded handle inbox)";
+    return nullptr;
+  }
+  return L.in.as<zg_check>();
+}
+
+int Device::peer_scatter(int level, const PeerTable& t, std::string* err) {
+  const bool callers = level == 0;
+  const PeerLevel* from = callers ? nullptr : &pl_[static_cast<size_t>(level) - 1];
+  const uint64_t n = callers ? home_n_ : from->nsub;
+  ZG_CUDA(cudaSetDevice(device));
+  if (n) {
+    unsigned long long* d_cursor = peer_ctrl_.as<unsigned long long>() + kMaxShards;
+    ZG_CUDA(cudaMemsetAsync(d_cursor, 0, kMaxShards * sizeof(unsigned long long), stream));
+    const unsigned grid = static_cast<unsigned>(std::min<uint64_t>((n + 255) / 256, static_cast<uint64_t>(sm_count_) * 8));
+    peer_scatter_kernel<<<grid, 256, 0, stream>>>(callers ? home_.as<zg_check>() : from->raised.as<zg_check>(), n, own_count,
+                                                  d_cursor, t, callers ? home_pos_.as<uint32_t>() : from->pos.as<uint32_t>());
+    ZG_CUDA(cudaGetLastError());
+    ++launches;
+  }
+  ZG_CUDA(cudaEventRecord(peer_event(level), stream));
+  return ZG_OK;
+}
+
+int Device::peer_pass(int level, const std::vector<cudaEvent_t>& wait, uint64_t* n_sub, uint64_t* counts, bool* overflow,
+                      std::string* err) {
+  for (uint32_t d = 0; d < own_count; ++d) counts[d] = 0;
+  *n_sub = 0;
+  *overflow = false;
+  std::shared_ptr<Snapshot> s = snap;
+  if (!s) {
+    if (err) *err = "no snapshot published";
+    return ZG_ENOSNAPSHOT;
+  }
+  PeerLevel& L = pl_[static_cast<size_t>(level)];
+  if (L.nq == 0) return ZG_OK;
+  const uint64_t nq = L.nq, Lv = s->max_leaves;
+  if (nq * Lv >= (1ull << 32)) {
+    if (err) *err = "pass too large (queries * leaves >= 2^32)";
+    return ZG_EINVAL;
+  }
+  ZG_CUDA(cudaSetDevice(device));
+  for (cudaEvent_t ev : wait) ZG_CUDA(cudaStreamWaitEvent(stream, ev, 0));
+  if (!L.val.ensure(nq * Lv + 4) || !L.out.ensure(nq) || !L.raised.ensure(subq_cap_ * sizeof(zg_check)) ||
+      !L.parent.ensure(subq_cap_ * 4) || !L.pos.ensure(subq_cap_ * 4)) {
+    if (err) *err = "out of device memory (sharded handle pass buffers)";
+    return ZG_ENOMEM;
+  }
+  unsigned long long* ctrl = ctrl_.as<unsigned long long>();
+  unsigned long long* d_counts = peer_ctrl_.as<unsigned long long>();
+  ZG_CUDA(cudaMemsetAsync(ctrl + 2, 0, 16, stream));
+  ZG_CUDA(cudaMemsetAsync(L.val.p, 0, nq * Lv + 4, stream));
+  // level 0: the callers' items (flags ignored), v1 codes written straight out (final unless the level raised
+  // sub-queries: then peer_fold rewrites them); deeper: routed sub-queries (flags = hop depth), value bits
+  int rc = run_pass(*s, L.in.as<zg_check>(), nq, L.val.as<uint8_t>(), L.out.as<uint8_t>(), level == 0, level == 0,
+                    L.raised.as<zg_check>(), L.parent.as<uint32_t>(), stream, false, err);
+  if (rc) return rc;
+  ZG_CUDA(cudaMemsetAsync(d_counts, 0, kMaxShards * sizeof(unsigned long long), stream));
+  const unsigned grid = static_cast<unsigned>(std::min<uint64_t>(subq_cap_ / 256 + 1, static_cast<uint64_t>(sm_count_) * 8));
+  peer_count_kernel<<<grid, 256, 0, stream>>>(L.raised.as<zg_check>(), ctrl + 1, subq_cap_, own_count, d_counts);
+  ZG_CUDA(cudaGetLastError());
+  ++launches;
+  ZG_CUDA(cudaMemcpyAsync(pin_peer_, ctrl, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaMemcpyAsync(pin_peer_ + 4, d_counts, own_count * sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaEventRecord(last_done_, stream));
+  have_last_ = true;
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  const uint64_t raised = pin_peer_[1];
+  const uint32_t flags = static_cast<uint32_t>(pin_peer_[3] & 0xFFFFFFFFu);
+  *n_sub = raised;
+  if (raised > subq_cap_) {
+    *overflow = true;
+    return ZG_OK;
+  }
+  if (flags & 1u) {
+    if (err) *err = "expansion stack overflow (per-warp spill area exhausted)";
+    return ZG_ENOMEM;
+  }
+  L.nsub = raised;
+  for (uint32_t d = 0; d < own_count; ++d) counts[d] = pin_peer_[4 + d];
+  if (level == 0) checks += nq;
+  else ++passes;
+  return ZG_OK;
+}
+
+int Device::peer_fold(int level, const PeerTable& t, const std::vector<cudaEvent_t>& wait, std::string* err) {
+  const PeerLevel& L = pl_[static_cast<size_t>(level)];
+  if (L.nsub == 0) return ZG_OK;  // the pass's own values are final
+  std::shared_ptr<Snapshot> s = snap;
+  ZG_CUDA(cudaSetDevice(device));
+  for (cudaEvent_t ev : wait) ZG_CUDA(cudaStreamWaitEvent(stream, ev, 0));
+  const unsigned blk = 256;
+  peer_or_children_kernel<<<static_cast<unsigned>((L.nsub + blk - 1) / blk), blk, 0, stream>>>(
+      L.raised.as<zg_check>(), L.parent.as<uint32_t>(), L.pos.as<uint32_t>(), L.nsub, own_count, t, L.val.as<uint8_t>());
+  fold_kernel<<<static_cast<unsigned>((L.nq + blk - 1) / blk), blk, 0, stream>>>(
+      s->prog.as<uint8_t>(), L.in.as<zg_check>(), L.nq, s->max_leaves, L.val.as<uint8_t>(), L.out.as<uint8_t>(), nullptr,
+      nullptr, level == 0 ? 0 : 1);
+  ZG_CUDA(cudaGetLastError());
+  launches += 2;
+  ZG_CUDA(cudaEventRecord(peer_event(level), stream));
+  return ZG_OK;
+}
+
+int Device::peer_finish(const PeerTable& t, const std::vector<cudaEvent_t>& wait, uint8_t* h_out, std::string* err) {
+  ZG_CUDA(cudaSetDevice(device));
+  if (home_n_) {
+    for (cudaEvent_t ev : wait) ZG_CUDA(cudaStreamWaitEvent(stream, ev, 0));
+    peer_gather_kernel<<<static_cast<unsigned>((home_n_ + 255) / 256), 256, 0, stream>>>(
+        home_.as<zg_check>(), home_pos_.as<uint32_t>(), home_n_, own_count, t, home_out_.as<uint8_t>());
+    ZG_CUDA(cudaGetLastError());
+    ++launches;
+    ZG_CUDA(cudaMemcpyAsync(h_out, home_out_.p, home_n_, cudaMemcpyDeviceToHost, stream));
+  }
   ZG_CUDA(cudaEventRecord(last_done_, stream));
   have_last_ = true;
   ZG_CUDA(cudaStreamSynchronize(stream));

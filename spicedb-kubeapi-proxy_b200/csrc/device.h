@@ -75,6 +75,15 @@ struct IngressMirror {
   uint64_t device_bytes() const;
 };
 
+// Sharded handle: where a level's queries go. Queries are written straight into their owners' inboxes (peer memory),
+// and values are read back where their owners left them. p[d] = shard d's buffer, base[d] = where this shard's part of
+// it starts. Passed to the kernels by value.
+constexpr int kMaxShards = 64;  // = kMaxRouteDest (kernels.cuh)
+struct PeerTable {
+  void* p[kMaxShards];
+  unsigned long long base[kMaxShards];
+};
+
 class Device {
  public:
   ~Device();
@@ -163,6 +172,31 @@ class Device {
   // lookup k; *err_mask bit k: lookup k had an undecidable candidate.
   int shard_lookup_finish(const unsigned long long* d_keys, uint64_t n, uint32_t* d_ids, uint64_t* per_lookup,
                           uint64_t* err_mask, std::string* err);
+  // ---- one shard of a sharded handle (zg_config.n_shards, capi.cu run_sharded): the handle drives every shard --------
+  // The handle's ONE store holds every shard's relationships; this device's snapshot keeps those whose resource id %
+  // own_count == own_rank (shard_rank / shard_count equal them). own_count = 1: the store is this device's alone.
+  uint32_t own_rank = 0, own_count = 1;
+  // Level 0: uploads this shard's n callers' items (pinned host) and counts them by owner: counts[d] (host, own_count).
+  // Waits for the counts (a round trip).
+  int peer_begin(const zg_check* h_items, uint64_t n, uint64_t* counts, std::string* err);
+  // The inbox of `level` on this shard, grown to n queries; the level then holds n queries.
+  zg_check* peer_inbox(int level, uint64_t n, std::string* err);
+  // Writes the queries of `level` this shard sends (level 0: its callers' items; deeper: what pass level - 1 raised)
+  // into the owners' inboxes at t.p[d] + t.base[d] + ..., and where each went; then records peer_event(level).
+  int peer_scatter(int level, const PeerTable& t, std::string* err);
+  // After every shard's peer_event(level) (`wait`, one per shard): evaluates the level's queries in one pass and counts
+  // the sub-queries it raised by owner: *n_sub, counts[d] (host). Waits for them (a round trip). ZG_ENOMEM with
+  // *overflow: the pass raised more than the sub-query capacity; the batch must be answered in halves.
+  int peer_pass(int level, const std::vector<cudaEvent_t>& wait, uint64_t* n_sub, uint64_t* counts, bool* overflow,
+                std::string* err);
+  // When pass `level` raised sub-queries: after every shard's peer_event(level + 1), ORs their values (t.p[d] = shard
+  // d's values of level + 1) into the raising leaves and folds the level; records peer_event(level).
+  int peer_fold(int level, const PeerTable& t, const std::vector<cudaEvent_t>& wait, std::string* err);
+  const uint8_t* peer_values(int level) const { return pl_[static_cast<size_t>(level)].out.as<uint8_t>(); }
+  // After every shard's peer_event(0): the answers of this shard's callers' items (t as in peer_fold, level 0) -> h_out
+  // (pinned host). Waits for them (a round trip).
+  int peer_finish(const PeerTable& t, const std::vector<cudaEvent_t>& wait, uint8_t* h_out, std::string* err);
+  cudaEvent_t peer_event(int level) const { return ev_peer_[level & 1]; }  // alternates: a fold waits on one, records the other
   // shard_pass_dev with KParams::no_wildcards (LookupSubjects' second verification, on every pass of every rank)
   int shard_pass_nowild_dev(const zg_check* d_queries, uint64_t n, int level, uint64_t* n_sub, std::string* err);
   // ---- LookupSubjects on the sharded store (dist.DeviceShardedLookup.lookup_subjects): one round of K <= 64 ----
@@ -282,6 +316,17 @@ class Device {
   template <bool kSrc, class Item, class Owner>
   int route_(const Item* d_items, uint64_t n, uint32_t n_dest, Owner owner, Item* d_routed, uint32_t* d_src, uint64_t* counts,
              std::string* err);
+  // sharded handle: per level, the queries the shards delivered here, their leaf values and values, and the sub-queries
+  // the pass raised (their raising (query, leaf), where their owners put them); the callers' items of level 0 in home_
+  struct PeerLevel {
+    DevBuf in, val, out, raised, parent, pos;
+    uint64_t nq = 0, nsub = 0;
+  };
+  std::vector<PeerLevel> pl_;
+  DevBuf home_, home_pos_, home_out_, peer_ctrl_;  // peer_ctrl_: counts[64], cursors[64]
+  uint64_t home_n_ = 0;
+  unsigned long long* pin_peer_ = nullptr;  // pinned: the control words and counts a round trip reads
+  cudaEvent_t ev_peer_[2] = {nullptr, nullptr};
   bool no_wildcards_ = false;  // run_pass: KParams::no_wildcards (LookupSubjects' second verification)
   uint64_t lb_cap_ = 1ull << 24;  // frontier entries / candidates of one lookup batch (ZGPU_LOOKUP_BATCH_CAP)
   void* pin_lk_ = nullptr;
@@ -316,11 +361,13 @@ const char* build_info();
 // Device radix sort of n u32 keys (build.cu keeps the cub instantiations in one translation unit).
 std::string sort_u32(const uint32_t* d_in, uint32_t* d_out, uint64_t n, cudaStream_t st);
 std::string sort_u64(const unsigned long long* d_in, unsigned long long* d_out, uint64_t n, int end_bit, cudaStream_t st);
-std::string gpu_build_snapshot(const Store& store, const Schema& sc, HostSnapshot* lay, cudaStream_t st, Snapshot* s);
+// Owner filter (rank, count) of both: only the relationships whose resource id % count == rank (Store::build).
+std::string gpu_build_snapshot(const Store& store, const Schema& sc, HostSnapshot* lay, cudaStream_t st, Snapshot* s,
+                               uint32_t owner_rank = 0, uint32_t owner_count = 1);
 // Applies store.journal to the arrays of `s` (same layout). cls_delta: per-class change of the relationship count.
 // "relayout" / "corrupt": the caller must rebuild.
 std::string gpu_apply_delta(const Store& store, const Schema& sc, const HostSnapshot& lay, cudaStream_t st, Snapshot* s,
-                            std::vector<uint32_t>* cls_delta);
+                            std::vector<uint32_t>* cls_delta, uint32_t owner_rank = 0, uint32_t owner_count = 1);
 // (Re)builds s->resources[] / n_resources[] from the forward row table.
 std::string gpu_resource_lists(Snapshot* s, cudaStream_t st);
 

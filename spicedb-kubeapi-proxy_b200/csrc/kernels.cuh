@@ -1089,6 +1089,61 @@ __global__ void unroute_kernel(const uint32_t* src, const uint8_t* val, unsigned
   if (i < n) out[src[i]] = val[i];
 }
 
+// ---- sharded handle: the exchange through peer memory (device.h PeerTable, capi.cu run_sharded) ---------------
+//
+// One process holds every shard, so a routed query is written straight into its owner's inbox, behind the part of
+// every lower shard (t.base[d], from all shards' counts), and a value is read where its owner left it: no copy
+// call, no staging, no reverse exchange. The table of the destinations' buffers (t.p[d]) is a kernel argument.
+
+// route_count_kernel over the sub-queries a pass raised, their number read on the device (*n_dev, at most cap): the
+// counts come back with the pass's control words in the level's one round trip
+__global__ void __launch_bounds__(256) peer_count_kernel(const zg_check* items, const unsigned long long* n_dev,
+                                                         unsigned long long cap, uint32_t n_dest, unsigned long long* counts) {
+  ZG_BLOCK_SHARED_U32(hist, kMaxRouteDest);
+  for (uint32_t i = threadIdx.x; i < n_dest; i += blockDim.x) hist[i] = 0;
+  __syncthreads();
+  const unsigned long long n = min(*n_dev, cap);
+  const unsigned long long stride = static_cast<unsigned long long>(gridDim.x) * blockDim.x;
+  for (unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x; i < n; i += stride)
+    atomicAdd(&hist[ResOwner{}(items[i], n_dest)], 1u);
+  __syncthreads();
+  for (uint32_t i = threadIdx.x; i < n_dest; i += blockDim.x)
+    if (hist[i]) atomicAdd(counts + i, static_cast<unsigned long long>(hist[i]));
+}
+// route_scatter_kernel into the owners' inboxes: item i goes to t.p[d][t.base[d] + cursor[d]++] (d = its owner), and
+// pos[i] = its index there, where the owner leaves its value
+template <class Table>
+__global__ void __launch_bounds__(256) peer_scatter_kernel(const zg_check* items, unsigned long long n, uint32_t n_dest,
+                                                           unsigned long long* cursor, const Table t, uint32_t* pos) {
+  const unsigned long long stride = static_cast<unsigned long long>(gridDim.x) * blockDim.x;
+  for (unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x; i < n; i += stride) {
+    const zg_check it = items[i];
+    const uint32_t d = ResOwner{}(it, n_dest);
+    const unsigned long long at = t.base[d] + atomicAdd(cursor + d, 1ull);
+    static_cast<zg_check*>(t.p[d])[at] = it;
+    pos[i] = static_cast<uint32_t>(at);
+  }
+}
+// or_children_src_kernel reading each child's value from its owner (t.p[d] = shard d's values of the next level)
+template <class Table>
+__global__ void peer_or_children_kernel(const zg_check* raised, const uint32_t* parent, const uint32_t* pos, unsigned long long n,
+                                        uint32_t n_dest, const Table t, uint8_t* parent_val) {
+  unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t d = raised[i].res % n_dest;
+  const uint32_t bits = static_cast<const uint8_t*>(t.p[d])[pos[i]] & (kValT | kValE);
+  if (!bits) return;
+  const uint32_t pj = parent[i];
+  atomicOr(reinterpret_cast<unsigned int*>(parent_val + (pj & ~3u)), bits << (8 * (pj & 3u)));
+}
+// the callers' answers in their own order: out[i] = the level-0 code its owner computed (t.p[d] = shard d's codes)
+template <class Table>
+__global__ void peer_gather_kernel(const zg_check* items, const uint32_t* pos, unsigned long long n, uint32_t n_dest,
+                                   const Table t, uint8_t* out) {
+  unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x;
+  if (i < n) out[i] = static_cast<const uint8_t*>(t.p[items[i].res % n_dest])[pos[i]];
+}
+
 // ---- LookupResources: candidate generation by reverse BFS ----------------------------
 //
 // Every true result r of LookupResources(T, P, S) has a forward path r -> o1 -> ... -> ok

@@ -351,7 +351,7 @@ bool Store::layout_stable() const {
   return true;
 }
 
-HostSnapshot Store::build() const {
+HostSnapshot Store::build(uint32_t owner_rank, uint32_t owner_count) const {
   const Schema& sc = *schema;
   HostSnapshot h = layout();
   const size_t nt = sc.types.size();
@@ -368,10 +368,11 @@ HostSnapshot Store::build() const {
 
   std::vector<std::vector<uint8_t>> seen(nt);
   for (size_t t = 0; t < nt; ++t) seen[t].assign(h.n_objects[t], 0);
+  auto skip = [&](const zg_tuple& t) { return (t.flags & 1) || (owner_count > 1 && t.res % owner_count != owner_rank); };
   uint64_t n_live = 0;
   for (size_t i = 0; i < tuples.size(); ++i) {
     const zg_tuple& t = tuples[i];
-    if (t.flags & 1) continue;
+    if (skip(t)) continue;
     ++h.row_ptr[row_index(t) + 1];
     seen[sc.slots[t.rel].type][t.res] = 1;
     ++n_live;
@@ -387,7 +388,7 @@ HostSnapshot Store::build() const {
     std::vector<uint32_t> cur(h.row_ptr.begin(), h.row_ptr.end() - 1);
     for (size_t i = 0; i < tuples.size(); ++i) {
       const zg_tuple& t = tuples[i];
-      if (t.flags & 1) continue;
+      if (skip(t)) continue;
       uint32_t pos = cur[row_index(t)]++;
       h.col[pos] = t.srel == kWildcard ? 0u : t.subj;
       if (with_exp) h.exp[pos] = expires[i];

@@ -114,7 +114,9 @@ class Store {
   HostSnapshot layout() const;
   // true when layout() would still return the capacities it returned last time
   bool layout_stable() const;
-  HostSnapshot build() const;
+  // owner filter (rank, count): only the relationships whose resource id % count == rank, with the capacities of the
+  // whole store -- one shard of a sharded handle, whose store holds every shard's relationships. count = 1: all.
+  HostSnapshot build(uint32_t owner_rank = 0, uint32_t owner_count = 1) const;
   uint64_t size() const { return live_; }
 
   const Schema* schema = nullptr;
