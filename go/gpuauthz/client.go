@@ -59,8 +59,8 @@ type Client struct {
 	// store that may still hold revoked grants.
 	broken atomic.Bool
 	// sharded: the engine is a sharded handle (Shards), which answers checks and writes but refuses
-	// LookupResources / LookupSubjects; those go to the embedded SpiceDB
-	sharded bool
+	// LookupSubjects, and LookupResources unless HandleLookups is set; what it refuses goes to the embedded SpiceDB
+	sharded, handleLookups bool
 }
 
 // AllDevices: every visible GPU from `device` on (zg_config.n_devices).
@@ -75,6 +75,13 @@ type Option func(*C.zg_config)
 // LookupResources and LookupSubjects are delegated to the embedded SpiceDB.
 func Shards(n uint32) Option {
 	return func(cfg *C.zg_config) { cfg.n_shards = C.uint32_t(n) }
+}
+
+// HandleLookups, with Shards, makes the sharded engine answer LookupResources and PrefilterListResponse itself
+// (ZG_FLAG_HANDLE_LOOKUPS): the reverse walk runs on every shard and the answers equal a replica's, so a store larger
+// than one GPU serves pre-filtered lists without a second engine. LookupSubjects stays delegated.
+func HandleLookups() Option {
+	return func(cfg *C.zg_config) { cfg.flags |= C.ZG_FLAG_HANDLE_LOOKUPS }
 }
 
 var errBroken = status.Error(codes.Unavailable, "gpu mirror is out of sync with SpiceDB and could not be rebuilt")
@@ -94,7 +101,8 @@ func New(ctx context.Context, inner v1.PermissionsServiceClient, schema string, 
 	if err := call(func() C.int { return C.zg_engine_create(&cfg, &eng) }); err != nil {
 		return nil, err // fail closed: no CPU fallback inside the library
 	}
-	c := &Client{PermissionsServiceClient: inner, engine: eng, sharded: cfg.n_shards > 1}
+	c := &Client{PermissionsServiceClient: inner, engine: eng, sharded: cfg.n_shards > 1,
+		handleLookups: cfg.flags&C.ZG_FLAG_HANDLE_LOOKUPS != 0}
 	cs := C.CString(schema)
 	defer C.free(unsafe.Pointer(cs))
 	if err := call(func() C.int { return C.zg_load_schema(eng, cs, C.size_t(len(schema))) }); err != nil {
@@ -241,7 +249,7 @@ func (c *Client) CheckPermission(ctx context.Context, req *v1.CheckPermissionReq
 // LookupResources: pkg/authz/lookups.go:65-88 reads the stream until io.EOF and keeps
 // LOOKUP_PERMISSIONSHIP_HAS_PERMISSION entries; order is irrelevant (a set).
 func (c *Client) LookupResources(ctx context.Context, req *v1.LookupResourcesRequest, opts ...grpc.CallOption) (v1.PermissionsService_LookupResourcesClient, error) {
-	if c.sharded {
+	if c.sharded && !c.handleLookups {
 		return c.PermissionsServiceClient.LookupResources(ctx, req, opts...)
 	}
 	if c.broken.Load() {

@@ -72,6 +72,11 @@ typedef struct zg_engine zg_engine;
 /* Forward expansion only: every direct probe is a binary search of the resource's row
  * (no direction-optimised probes from the subject's reverse rows). For A/B measurement. */
 #define ZG_FLAG_FORWARD_ONLY 2u
+/* Sharded handle (n_shards > 1) only: the handle answers zg_lookup_resources, zg_lookup_resources_str and
+ * zg_list_prefilter itself. Each round's reverse walk runs on every shard, its frontier and answer keys exchanged
+ * through peer memory, and its candidates are verified by the handle's check protocol (zg_handle_lookup_counters).
+ * The answers equal a replica's. On any other engine, zg_engine_create returns ZG_EINVAL. */
+#define ZG_FLAG_HANDLE_LOOKUPS 4u
 
 typedef struct {
   int32_t device;            /* CUDA device ordinal; -1 = current device          */
@@ -93,7 +98,8 @@ typedef struct {
                                 S shards share it). Checks cross the shards in-process, sub-queries delivered through
                                 peer memory; every device pair must have peer access. Not with shard_count > 1;
                                 S <= 64. LookupResources / LookupSubjects / the list pre-filter, zg_check_bulk_device,
-                                the device-ingress calls and the zg_shard_*_dev calls are refused (ZG_EINVAL).    */
+                                the device-ingress calls and the zg_shard_*_dev calls are refused (ZG_EINVAL);
+                                with ZG_FLAG_HANDLE_LOOKUPS, LookupResources and the list pre-filter are answered. */
 } zg_config;
 #define ZG_ALL_DEVICES 0xFFFFFFFFu
 
@@ -322,6 +328,13 @@ int zg_lookup_subjects_str(zg_engine *e, const char *res_type, const char *res_i
  * by the forward walk, out[1] lookups that verified every object of the subject type, out[2] check items of
  * their first verification launches (the probe included). */
 int zg_lookup_subjects_counters(zg_engine *e, uint64_t *out);
+/* Cumulative LookupResources counters of a sharded handle with ZG_FLAG_HANDLE_LOOKUPS (zeros on any other engine):
+ * out[0] rounds begun on the shards (a round answers up to 64 lookups; a halved round counts its halves too), out[1]
+ * walk levels expanded, out[2] times the host waited for the shards (the verification's included), out[3] frontier
+ * entries all-gathered, out[4] candidates verified, out[5] rounds redone in halves (a frontier or the candidates
+ * overflowed ZGPU_LOOKUP_BATCH_CAP), out[6] rounds that verified every resource of the type (a single lookup that
+ * overflowed, or ZGPU_NO_RBFS=1). */
+int zg_handle_lookup_counters(zg_engine *e, uint64_t *out);
 
 /* Pinned host memory for request/response buffers: zg_check_bulk copies straight
  * from/to such buffers (no staging memcpy). */

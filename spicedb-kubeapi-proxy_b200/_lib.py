@@ -176,6 +176,7 @@ _SIGS = {
     "zg_lookup_subjects_str": (C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint32,
                                          C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint64)]),
     "zg_lookup_subjects_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "zg_handle_lookup_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
     "zg_resolve_checks_packed_device": (C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]),
     "zg_check_bulk_packed_ingress": (C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_void_p, C.c_char_p, C.c_void_p, C.c_uint64, C.c_void_p]),
     "zg_intern_objects_packed": (C.c_int, [C.c_void_p, C.c_int, C.c_char_p, C.c_void_p, C.c_uint64, C.c_void_p]),
@@ -330,13 +331,15 @@ class Engine:
 
     def __init__(self, schema: str | None = None, device: int = -1, subquery_capacity: int = 0, work_budget: int = 0,
                  host_only: bool = False, forward_only: bool = False, shard_rank: int = 0, shard_count: int = 0,
-                 n_devices: int = 0, n_shards: int = 0):
+                 n_devices: int = 0, n_shards: int = 0, handle_lookups: bool = False):
         """host_only=True builds schema/store/snapshot without a GPU (CPU unit tests of
         the host logic); every check/lookup on such an engine raises ZgpuError. n_shards=S > 1: this one handle
-        holds the S shards of an object-hash sharded store (zg_config.n_shards)."""
+        holds the S shards of an object-hash sharded store (zg_config.n_shards); handle_lookups=True
+        (ZG_FLAG_HANDLE_LOOKUPS) makes it answer LookupResources and the list pre-filter too."""
         self._L = lib()
-        cfg = _Config(device, (1 if host_only else 0) | (2 if forward_only else 0), subquery_capacity, work_budget,
-                      shard_rank, shard_count, n_devices & 0xFFFFFFFF, n_shards)
+        flags = (1 if host_only else 0) | (2 if forward_only else 0) | (4 if handle_lookups else 0)
+        cfg = _Config(device, flags, subquery_capacity, work_budget, shard_rank, shard_count, n_devices & 0xFFFFFFFF,
+                      n_shards)
         h = C.c_void_p()
         rc = self._L.zg_engine_create(C.byref(cfg), C.byref(h))
         if rc:
@@ -680,6 +683,14 @@ class Engine:
         out = np.zeros(3, dtype=np.uint64)
         self._ck(self._L.zg_lookup_subjects_counters(self._h, out.ctypes.data))
         return {"walks": int(out[0]), "fallbacks": int(out[1]), "items_verified": int(out[2])}
+
+    HANDLE_LOOKUP_COUNTERS = ("rounds", "levels", "round_trips", "frontier_entries", "candidates", "halvings", "fallbacks")
+
+    def handle_lookup_counters(self) -> dict:
+        """Cumulative LookupResources counters of a sharded handle with handle_lookups (zg_handle_lookup_counters)."""
+        out = np.zeros(len(self.HANDLE_LOOKUP_COUNTERS), dtype=np.uint64)
+        self._ck(self._L.zg_handle_lookup_counters(self._h, out.ctypes.data))
+        return {k: int(v) for k, v in zip(self.HANDLE_LOOKUP_COUNTERS, out)}
 
     # -- sharded store (dist.DeviceShardedChecker drives these) --------------------
     # every pointer is a device address on this engine's GPU (ints, e.g. tensor.data_ptr())

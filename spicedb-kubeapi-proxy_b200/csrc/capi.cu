@@ -126,6 +126,11 @@ struct Replica {
   Device dev;
   DeviceWorker worker;
 };
+// what one run of the sharded check protocol cost: pass levels, sub-queries the shards raised to each other, and the
+// times the host waited for the devices
+struct PeerCounts {
+  uint64_t levels = 0, subqueries = 0, round_trips = 0;
+};
 
 struct zg_engine {
   // Two locks, always taken in this order:
@@ -184,7 +189,11 @@ struct zg_engine {
   uint32_t n_shards = 1, shard_devices = 1;
   void* group_pin = nullptr;  // a group's items, then its answers (pinned: the shards copy their slices from / to it)
   size_t group_pin_cap = 0;
-  uint64_t last_levels = 0, last_subqueries = 0, last_round_trips = 0;
+  PeerCounts last_group;  // zg_stats last_levels / last_subqueries / last_round_trips
+  // ZG_FLAG_HANDLE_LOOKUPS: run_sharded_lookup answers LookupResources; zg_handle_lookup_counters
+  bool handle_lookups = false;
+  uint64_t hl_rounds = 0, hl_levels = 0, hl_round_trips = 0, hl_frontier = 0, hl_candidates = 0, hl_halvings = 0,
+           hl_fallbacks = 0;
   std::vector<HostSnapshot> shard_built;  // zg_debug_shard_row: the host builder's arrays per shard
   ~zg_engine() {
     if (group_pin) cudaFreeHost(group_pin);
@@ -240,7 +249,14 @@ static const char* kHandleDeviceMsg =
 static const char* kHandleShardCallMsg =
     "sharded handle (zg_config.n_shards > 1): the zg_shard_*_dev calls drive one shard per engine; this handle runs "
     "the sharded protocol itself (zg_check_bulk)";
+static const char* kHandleSubjectsMsg =
+    "sharded handle (zg_config.n_shards > 1): LookupSubjects is not served by it, with or without "
+    "ZG_FLAG_HANDLE_LOOKUPS; run it on one engine per shard (dist.DeviceShardedLookup) or on a replica";
 static bool is_handle(const zg_engine* e) { return e->n_shards > 1; }
+// why a sharded engine refuses LookupSubjects
+static const char* subjects_refusal(const zg_engine* e) {
+  return !is_handle(e) ? kShardedMsg : e->handle_lookups ? kHandleSubjectsMsg : kHandleLookupMsg;
+}
 // shard k of a sharded handle
 static Device& shard(zg_engine* e, uint32_t k) { return k == 0 ? e->dev : e->replicas[k - 1]->dev; }
 
@@ -272,9 +288,12 @@ extern "C" int zg_engine_create(const zg_config* cfg, zg_engine** out) {
     return fail(ZG_EINVAL, "n_shards > 1 holds every shard in this one handle, shard_count > 1 makes this engine one "
                            "shard of several: set only one of them");
   if (S > static_cast<uint32_t>(kMaxShards)) return fail(ZG_EINVAL, "n_shards exceeds 64 (the routing kernels' destinations)");
+  const bool handle_lookups = cfg && (cfg->flags & ZG_FLAG_HANDLE_LOOKUPS);
+  if (handle_lookups && S < 2) return fail(ZG_EINVAL, "ZG_FLAG_HANDLE_LOOKUPS needs n_shards > 1");
   zg_engine* e = new (std::nothrow) zg_engine();
   if (!e) return fail(ZG_ENOMEM, "out of memory");
   e->n_shards = S;
+  e->handle_lookups = handle_lookups;
   if (cfg && (cfg->flags & ZG_FLAG_HOST_ONLY)) {
     e->host_only = true;
     e->keep_built = true;
@@ -892,31 +911,42 @@ static int publish_if_needed(zg_engine* e) {
   return ZG_OK;
 }
 
-// One coalesced group on a sharded handle: the levels of dist.DeviceShardedChecker.check_bulk, driven in this process.
-// items / out: n pinned host entries. Shard k brings the slice dist.shard_bounds gives it and routes it to the owners.
-// Per level, every shard writes its queries straight into the owners' inboxes (where, the host computes from every
-// shard's counts: the level's one round trip), each owner's pass starts when the shards delivering to it are done
-// (events, not host waits), and the values are folded back level by level where their owners left them.
-static int run_sharded(zg_engine* e, const zg_check* items, uint64_t n, uint8_t* out, std::string* err) {
+// The first failing shard's code and message (per-shard steps run concurrently).
+static int first_error(const std::vector<int>& rcs, const std::vector<std::string>& errs, std::string* err) {
+  for (size_t k = 0; k < rcs.size(); ++k)
+    if (rcs[k]) {
+      *err = errs[k];
+      return rcs[k];
+    }
+  return ZG_OK;
+}
+
+// The checks of one run of the handle's check protocol: shard k brings n[k] items at items[k] and gets their codes at
+// out[k], in the same order. Host (pinned) or that shard's device memory, both.
+struct ShardLists {
+  std::vector<const zg_check*> items;
+  std::vector<uint64_t> n;
+  std::vector<uint8_t*> out;
+};
+
+// The levels of dist.DeviceShardedChecker.check_bulk, driven in this process. Every shard routes its list to the
+// owners. Per level, every shard writes its queries straight into the owners' inboxes (where, the host computes from
+// every shard's counts: the level's one round trip), each owner's pass starts when the shards delivering to it are
+// done (events, not host waits), and the values are folded back level by level where their owners left them.
+// *overflow: a pass raised more sub-queries than its buffer holds; nothing is answered.
+static int sharded_levels(zg_engine* e, const ShardLists& L, PeerCounts* pc, bool* overflow_out, std::string* err) {
   const uint32_t S = e->n_shards;
-  auto lo = [&](uint32_t k) { return k * (n / S) + std::min<uint64_t>(k, n % S); };
+  *overflow_out = false;
   std::vector<uint64_t> counts(size_t(S) * S, 0);  // [k * S + d]: queries shard k sends to shard d this level
   std::vector<int> rcs(S, ZG_OK);
   std::vector<std::string> errs(S);
-  auto first_error = [&]() {
-    for (uint32_t k = 0; k < S; ++k)
-      if (rcs[k]) {
-        *err = errs[k];
-        return rcs[k];
-      }
-    return static_cast<int>(ZG_OK);
-  };
+  auto first_error = [&]() { return ::first_error(rcs, errs, err); };
   const uint32_t now = now_of(e);
   on_all_devices(e, [&](Device& dev, size_t k) {
     dev.now = now;
-    rcs[k] = dev.peer_begin(items + lo(k), lo(k + 1) - lo(k), &counts[k * S], &errs[k]);
+    rcs[k] = dev.peer_begin(L.items[k], L.n[k], &counts[k * S], &errs[k]);
   });
-  ++e->last_round_trips;
+  ++pc->round_trips;
   if (int rc = first_error()) return rc;
   std::vector<PeerTable> tab(S);
   std::vector<cudaEvent_t> wait(S);
@@ -952,21 +982,14 @@ static int run_sharded(zg_engine* e, const zg_check* items, uint64_t n, uint8_t*
       rcs[k] = dev.peer_pass(level, wait, &nsub[k], &counts[k * S], &o, &errs[k]);
       overflow[k] = o;
     });
-    ++e->last_round_trips;
-    e->last_levels = std::max<uint64_t>(e->last_levels, static_cast<uint64_t>(level) + 1);
+    ++pc->round_trips;
+    pc->levels = std::max<uint64_t>(pc->levels, static_cast<uint64_t>(level) + 1);
     if (int rc = first_error()) return rc;
     if (std::find(overflow.begin(), overflow.end(), 1) != overflow.end()) {
-      // a pass raised more sub-queries than its buffer holds: checks are independent, answer the group in halves
-      if (n < 2) {
-        *err = "sub-query buffer overflow on a single check: raise zg_config.subquery_capacity";
-        return ZG_ENOMEM;
-      }
-      ++e->dev.split_batches;
-      const uint64_t h = n / 2;
-      if (int rc = run_sharded(e, items, h, out, err)) return rc;
-      return run_sharded(e, items + h, n - h, out + h, err);
+      *overflow_out = true;
+      return ZG_OK;
     }
-    for (uint32_t k = 0; k < S; ++k) e->last_subqueries += nsub[k];
+    for (uint32_t k = 0; k < S; ++k) pc->subqueries += nsub[k];
   }
   // values back: the deepest pass raised nothing; every shallower level folds in its children's values
   for (int lv = level - 2; lv >= 0; --lv) {
@@ -983,9 +1006,48 @@ static int run_sharded(zg_engine* e, const zg_check* items, uint64_t n, uint8_t*
     tab[0].base[d] = 0;
   }
   events(0);
-  on_all_devices(e, [&](Device& dev, size_t k) { rcs[k] = dev.peer_finish(tab[0], wait, out + lo(k), &errs[k]); });
-  ++e->last_round_trips;
+  on_all_devices(e, [&](Device& dev, size_t k) { rcs[k] = dev.peer_finish(tab[0], wait, L.out[k], &errs[k]); });
+  ++pc->round_trips;
   return first_error();
+}
+
+// sharded_levels, and on overflow the same in halves (checks are independent): the first half of the items taken in
+// shard order, then the rest. Where an item starts does not change where it is evaluated (at its owner).
+static int run_sharded_lists(zg_engine* e, const ShardLists& L, PeerCounts* pc, std::string* err) {
+  bool overflow = false;
+  if (int rc = sharded_levels(e, L, pc, &overflow, err)) return rc;
+  if (!overflow) return ZG_OK;
+  uint64_t n = 0;
+  for (uint64_t m : L.n) n += m;
+  if (n < 2) {
+    *err = "sub-query buffer overflow on a single check: raise zg_config.subquery_capacity";
+    return ZG_ENOMEM;
+  }
+  ++e->dev.split_batches;
+  ShardLists a = L, b = L;
+  uint64_t h = n / 2;
+  for (size_t k = 0; k < L.n.size(); ++k) {
+    a.n[k] = std::min(h, L.n[k]);
+    h -= a.n[k];
+    b.n[k] = L.n[k] - a.n[k];
+    b.items[k] += a.n[k];
+    b.out[k] += a.n[k];
+  }
+  if (int rc = run_sharded_lists(e, a, pc, err)) return rc;
+  return run_sharded_lists(e, b, pc, err);
+}
+
+// n checks in host memory (out: their codes): shard k brings the slice dist.shard_bounds gives it.
+static int run_sharded(zg_engine* e, const zg_check* items, uint64_t n, uint8_t* out, PeerCounts* pc, std::string* err) {
+  const uint32_t S = e->n_shards;
+  auto lo = [&](uint32_t k) { return k * (n / S) + std::min<uint64_t>(k, n % S); };
+  ShardLists L;
+  for (uint32_t k = 0; k < S; ++k) {
+    L.items.push_back(items + lo(k));
+    L.n.push_back(lo(k + 1) - lo(k));
+    L.out.push_back(out + lo(k));
+  }
+  return run_sharded_lists(e, L, pc, err);
 }
 
 // Runs one group of queued requests; the caller holds the device lock.
@@ -1025,8 +1087,8 @@ static void run_group(zg_engine* e, std::vector<BatchReq*>& group) {
         off += r->n;
       }
       uint8_t* answers = reinterpret_cast<uint8_t*>(items + total);
-      e->last_levels = e->last_subqueries = e->last_round_trips = 0;
-      rc = run_sharded(e, items, total, answers, &err);
+      e->last_group = PeerCounts();
+      rc = run_sharded(e, items, total, answers, &e->last_group, &err);
       off = 0;
       for (BatchReq* r : group) {
         if (!rc) std::memcpy(r->out, answers + off, r->n);
@@ -1675,6 +1737,187 @@ extern "C" int zg_list_postfilter(zg_engine* e, const char* body, size_t len, co
   return rc == ZG_EINVAL ? fail(rc, "zg_list_filter: inconsistent item ranges") : rc;
 }
 
+// LookupResources on a sharded handle (ZG_FLAG_HANDLE_LOOKUPS): one round of dist.DeviceShardedLookup._round over
+// reqs[lo, lo + K) (K <= 64), driven in this process; ids[i] / rcs[i] answer reqs[i]. The handle is every rank, so
+// every answer goes to shard 0. Shard k owns the objects whose id % S == k and discovers only those in its reverse
+// rows, so each object enters the frontier once. Per level, every shard expands the whole replicated frontier (its
+// counts and overflow flag: the level's one round trip), then writes its new entries into every shard's next frontier
+// behind those of the lower shards (peer_put: the all-gather). The candidates, each on its owner, are verified by the
+// handle's check protocol where they lie, and their answer keys gathered on shard 0, sorted and split there.
+//
+// Why no frontier is overwritten early. (1) A source's new entries (hl.next) are read only by its own peer_put, on
+// its own stream, and only its next expand, later on that stream, overwrites them. (2) The put of level L writes
+// hl.front[(L + 1) & 1]; the expand of level L reads hl.front[L & 1], and the expand of level L - 1, the last reader of
+// hl.front[(L + 1) & 1], has completed on every shard: the host read its counts before it issued any put of level L.
+// (3) Every shard's expand of level L + 1 waits on every shard's put event of level L (peer_wait), so it reads the
+// whole frontier. The answer keys follow (1) and (3) with shard 0 as the one destination.
+static int run_sharded_lookup(zg_engine* e, const std::vector<Device::LookupReq>& reqs, size_t lo, size_t K,
+                              std::vector<std::vector<uint32_t>>* ids, std::vector<int>* rcs, std::string* err) {
+  const uint32_t S = e->n_shards;
+  const std::vector<Device::LookupReq> round(reqs.begin() + static_cast<long>(lo), reqs.begin() + static_cast<long>(lo + K));
+  const std::vector<uint8_t> home(K, 0);
+  const uint64_t cap = e->dev.lookup_walk_cap();
+  std::vector<int> src(S, ZG_OK);
+  std::vector<std::string> errs(S);
+  std::vector<uint64_t> per(K);
+  auto first_error = [&]() { return ::first_error(src, errs, err); };
+  // a failed round is ended on every shard, so that no shard keeps its snapshot resident
+  auto fail_round = [&](int rc) {
+    on_all_devices(e, [&](Device& dev, size_t) {
+      uint64_t mask = 0;
+      std::vector<uint64_t> none(K);
+      dev.shard_lookup_finish(nullptr, 0, nullptr, none.data(), &mask, nullptr);
+    });
+    return rc;
+  };
+  ++e->hl_rounds;
+  on_all_devices(e, [&](Device& dev, size_t k) {
+    src[k] = !dev.hl_ensure(dev.hl.front[0], K * 8) || !dev.hl_ensure(dev.hl.next, cap * 8)
+                 ? ZG_ENOMEM
+                 : dev.shard_lookup_begin(round, home.data(), cap, dev.hl.front[0].as<unsigned long long>(), &errs[k]);
+    if (src[k] == ZG_ENOMEM && errs[k].empty()) errs[k] = "out of device memory (sharded handle lookup buffers)";
+  });
+  ++e->hl_round_trips;
+  if (int rc = first_error()) return fail_round(rc);
+  // ---- the walk
+  const bool exhaustive = !e->dev.use_rbfs;  // ZGPU_NO_RBFS=1: every owned resource of the type is a candidate
+  bool overflow = false;
+  std::vector<uint64_t> n_out(S);
+  std::vector<char> ovf(S);
+  std::vector<PeerTable> tab(S);
+  std::vector<cudaEvent_t> wait;
+  uint64_t n_in = K;
+  for (int level = 0; !exhaustive; ++level) {
+    on_all_devices(e, [&](Device& dev, size_t k) {
+      bool o = false;
+      src[k] = level ? dev.peer_wait(wait, &errs[k]) : ZG_OK;
+      if (!src[k])
+        src[k] = dev.shard_lookup_expand(dev.hl.front[level & 1].as<unsigned long long>(), n_in, level,
+                                         dev.hl.next.as<unsigned long long>(), &n_out[k], &o, &errs[k]);
+      ovf[k] = o;
+    });
+    ++e->hl_levels;
+    ++e->hl_round_trips;
+    if (int rc = first_error()) return fail_round(rc);
+    uint64_t total = 0;
+    for (uint32_t k = 0; k < S; ++k) total += n_out[k];
+    overflow = std::find(ovf.begin(), ovf.end(), 1) != ovf.end();
+    if (overflow || total == 0 || level == ZG_MAX_DEPTH + 1) break;
+    // a gathered frontier past the walk capacity is the overflow the next expand would report on every shard
+    if ((overflow = total > cap)) break;
+    uint64_t at = 0;
+    for (uint32_t k = 0; k < S; ++k) {
+      for (uint32_t d = 0; d < S; ++d) tab[k].base[d] = at;
+      at += n_out[k];
+    }
+    for (uint32_t d = 0; d < S; ++d) {
+      Device& dev = shard(e, d);
+      if (!dev.hl_ensure(dev.hl.front[(level + 1) & 1], total * 8)) {
+        *err = "out of device memory (sharded handle lookup frontier)";
+        return fail_round(ZG_ENOMEM);
+      }
+      for (uint32_t k = 0; k < S; ++k) tab[k].p[d] = dev.hl.front[(level + 1) & 1].p;
+    }
+    on_all_devices(e, [&](Device& dev, size_t k) {
+      src[k] = dev.peer_put(dev.hl.next.as<unsigned long long>(), n_out[k], S, tab[k], level, &errs[k]);
+    });
+    if (int rc = first_error()) return fail_round(rc);
+    wait.clear();
+    for (uint32_t k = 0; k < S; ++k) wait.push_back(shard(e, k).peer_event(level));
+    e->hl_frontier += total;
+    n_in = total;
+  }
+  if (overflow && K > 1) {  // checks of the two halves' candidates fit where the whole round's did not
+    ++e->hl_halvings;
+    const size_t h = K / 2;
+    if (int rc = run_sharded_lookup(e, reqs, lo, h, ids, rcs, err)) return rc;
+    return run_sharded_lookup(e, reqs, lo + h, K - h, ids, rcs, err);
+  }
+  if (overflow || exhaustive) ++e->hl_fallbacks;
+  // ---- the candidates, verified where they lie
+  std::vector<uint64_t> nc(S);
+  on_all_devices(e, [&](Device& dev, size_t k) {
+    uint64_t need = 0;
+    src[k] = dev.shard_lookup_candidates(overflow || exhaustive, nullptr, 0, &need, &errs[k]);
+    if (!src[k] && (!dev.hl_ensure(dev.hl.items, need * sizeof(zg_check)) || !dev.hl_ensure(dev.hl.codes, need) ||
+                    !dev.hl_ensure(dev.hl.routed, need * 8))) {
+      src[k] = ZG_ENOMEM;
+      errs[k] = "out of device memory (sharded handle lookup candidates)";
+    }
+    if (!src[k]) src[k] = dev.shard_lookup_candidates(overflow || exhaustive, dev.hl.items.as<zg_check>(), need, &nc[k], &errs[k]);
+  });
+  ++e->hl_round_trips;
+  if (int rc = first_error()) return fail_round(rc);
+  ShardLists V;
+  for (uint32_t k = 0; k < S; ++k) {
+    V.items.push_back(shard(e, k).hl.items.as<zg_check>());
+    V.n.push_back(nc[k]);
+    V.out.push_back(shard(e, k).hl.codes.as<uint8_t>());
+    e->hl_candidates += nc[k];
+  }
+  PeerCounts pc;
+  int vrc = run_sharded_lists(e, V, &pc, err);
+  e->hl_round_trips += pc.round_trips;
+  if (vrc) return fail_round(vrc);
+  // ---- the answer keys, gathered, sorted and split on shard 0
+  std::vector<uint64_t> counts(size_t(S) * S, 0);
+  on_all_devices(e, [&](Device& dev, size_t k) {
+    src[k] = dev.shard_lookup_route(dev.hl.codes.as<uint8_t>(), nc[k], S, dev.hl.routed.as<unsigned long long>(), &counts[k * S],
+                                    &errs[k]);
+  });
+  ++e->hl_round_trips;
+  if (int rc = first_error()) return fail_round(rc);
+  uint64_t n_keys = 0;
+  for (uint32_t k = 0; k < S; ++k) {
+    tab[k].base[0] = n_keys;
+    n_keys += counts[size_t(k) * S];
+  }
+  Device& d0 = e->dev;
+  if (!d0.hl_ensure(d0.hl.keys, n_keys * 8) || !d0.hl_ensure(d0.hl.ids, n_keys * 4)) {
+    *err = "out of device memory (sharded handle lookup keys)";
+    return fail_round(ZG_ENOMEM);
+  }
+  for (uint32_t k = 0; k < S; ++k) tab[k].p[0] = d0.hl.keys.p;
+  on_all_devices(e, [&](Device& dev, size_t k) {
+    src[k] = dev.peer_put(dev.hl.routed.as<unsigned long long>(), counts[k * S], 1, tab[k], 0, &errs[k]);
+  });
+  if (int rc = first_error()) return fail_round(rc);
+  wait.clear();
+  for (uint32_t k = 0; k < S; ++k) wait.push_back(shard(e, k).peer_event(0));
+  uint64_t err_mask = 0;
+  on_all_devices(e, [&](Device& dev, size_t k) {
+    uint64_t mask = 0;
+    std::vector<uint64_t> none(K);
+    src[k] = k ? dev.shard_lookup_finish(nullptr, 0, nullptr, none.data(), &mask, &errs[k])  // ends the round
+               : dev.peer_wait(wait, &errs[k]);
+    if (!k && !src[k])
+      src[k] = dev.shard_lookup_finish(dev.hl.keys.as<unsigned long long>(), n_keys, dev.hl.ids.as<uint32_t>(), per.data(),
+                                       &err_mask, &errs[k]);
+  });
+  ++e->hl_round_trips;
+  if (int rc = first_error()) return fail_round(rc);
+  uint64_t n_ids = 0;
+  for (uint64_t m : per) n_ids += m;
+  std::vector<uint32_t> host(n_ids);
+  if (n_ids) {
+    const cudaError_t ce = cudaSetDevice(d0.device) == cudaSuccess
+                               ? cudaMemcpy(host.data(), d0.hl.ids.p, n_ids * 4, cudaMemcpyDeviceToHost)
+                               : cudaGetLastError();
+    ++e->hl_round_trips;
+    if (ce != cudaSuccess) {
+      *err = std::string("cudaMemcpy (lookup answers): ") + cudaGetErrorString(ce);
+      return ZG_ECUDA;
+    }
+  }
+  uint64_t off = 0;
+  for (size_t k = 0; k < K; ++k) {
+    if ((err_mask >> k) & 1) (*rcs)[lo + k] = ZG_EDEPTH;
+    else (*ids)[lo + k].assign(host.begin() + static_cast<long>(off), host.begin() + static_cast<long>(off + per[k]));
+    off += per[k];
+  }
+  return ZG_OK;
+}
+
 // Answers a group of queued lookups under the engine lock: cache hits first, the rest in one batched launch
 // sequence, then the self-membership of userset subjects (Check is the arbiter of LookupResources).
 static void run_lookup_group(zg_engine* e, std::vector<zg_engine::LookupJob*>& group) {  // device lock held
@@ -1685,8 +1928,9 @@ static void run_lookup_group(zg_engine* e, std::vector<zg_engine::LookupJob*>& g
     }
   };
   if (e->host_only) return fail_all(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
-  if (e->dev.shard_count > 1) return fail_all(ZG_EINVAL, is_handle(e) ? kHandleLookupMsg : kShardedMsg);
-  if (e->dirty.load() || !e->dev.snap) {
+  const bool handle = is_handle(e) && e->handle_lookups;
+  if (e->dev.shard_count > 1 && !handle) return fail_all(ZG_EINVAL, is_handle(e) ? kHandleLookupMsg : kShardedMsg);
+  if (e->dirty.load() || !e->dev.snap) {  // a handle's failed publish clears every shard's snapshot
     LOCK_NAMES_UNIQUE(e);
     int rc = publish_locked(e);
     if (rc) return fail_all(rc, g_err);
@@ -1724,7 +1968,15 @@ static void run_lookup_group(zg_engine* e, std::vector<zg_engine::LookupJob*>& g
     std::string err;
     int rc = ZG_OK;
     const size_t nd = 1 + e->replicas.size();
-    if (nd == 1 || reqs.size() < 2) {
+    if (handle) {
+      ids.resize(reqs.size());
+      rcs.assign(reqs.size(), ZG_OK);
+      rc = run_sharded_lookup(e, reqs, 0, reqs.size(), &ids, &rcs, &err);
+      if (reqs.size() > 1) {
+        ++e->dev.lookup_batches;
+        e->dev.lookups_batched += reqs.size();
+      }
+    } else if (nd == 1 || reqs.size() < 2) {
       rc = e->dev.lookup_batch(reqs, &ids, &rcs, &err);
     } else {
       // replicas: the lookups of the group are dealt out to the devices
@@ -1767,9 +2019,9 @@ static void run_lookup_group(zg_engine* e, std::vector<zg_engine::LookupJob*>& g
       j->ids = std::move(ids[r]);
       // A userset subject T:x#r is a member of T:x#P for every relation r inlined into P's union, with or
       // without relationships, and the reverse walk only reaches x through stored edges: ask the check
-      // kernel about the one candidate res = subj.
+      // kernel about the one candidate res = subj. (A handle's round made it a candidate on x's owner.)
       const zg_engine::LookupKey& k = j->key;
-      if (k.srel != kNone && k.stype == k.res_type && k.subj < ZG_NO_OBJECT - 1 &&
+      if (!handle && k.srel != kNone && k.stype == k.res_type && k.subj < ZG_NO_OBJECT - 1 &&
           !std::binary_search(j->ids.begin(), j->ids.end(), k.subj)) {
         zg_check self = reqs[r].proto;
         self.res = k.subj;
@@ -1804,7 +2056,9 @@ static void run_lookup_group(zg_engine* e, std::vector<zg_engine::LookupJob*>& g
       self.srel = j->key.srel;
       uint8_t code = 0;
       std::string cerr;
-      int crc = e->dev.check_host(&self, 1, &code, &cerr);
+      PeerCounts pc;  // a handle checks the one item through its check protocol
+      int crc = handle ? run_sharded(e, &self, 1, &code, &pc, &cerr) : e->dev.check_host(&self, 1, &code, &cerr);
+      e->hl_round_trips += pc.round_trips;
       if (crc) {
         j->rc = crc;
         j->err = cerr;
@@ -1957,7 +2211,7 @@ static int lookup_subjects_ids(zg_engine* e, uint16_t perm, uint32_t res, uint16
     return fail(ZG_EINVAL, "unknown subject type or relation");
   if (option != ZG_WILDCARDS_INCLUDE && option != ZG_WILDCARDS_EXCLUDE) return fail(ZG_EINVAL, "unknown wildcard option");
   if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
-  if (e->dev.shard_count > 1) return fail(ZG_EINVAL, is_handle(e) ? kHandleLookupMsg : kShardedMsg);
+  if (e->dev.shard_count > 1) return fail(ZG_EINVAL, subjects_refusal(e));
   LOCK_DEVICE(e);
   if (e->dirty.load() || !e->dev.snap) {
     LOCK_NAMES_UNIQUE(e);
@@ -2020,7 +2274,7 @@ extern "C" int zg_lookup_subjects_str(zg_engine* e, const char* res_type, const 
     if (wildcard_option != ZG_WILDCARDS_INCLUDE && wildcard_option != ZG_WILDCARDS_EXCLUDE)
       return fail(ZG_EINVAL, "unknown wildcard option");
     if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
-    if (e->dev.shard_count > 1) return fail(ZG_EINVAL, is_handle(e) ? kHandleLookupMsg : kShardedMsg);
+    if (e->dev.shard_count > 1) return fail(ZG_EINVAL, subjects_refusal(e));
   } else {
     rc = lookup_subjects_ids(e, static_cast<uint16_t>(p), res, static_cast<uint16_t>(st), sr, wildcard_option, &ans);
     if (rc) return rc;
@@ -2060,6 +2314,15 @@ extern "C" int zg_lookup_subjects_counters(zg_engine* e, uint64_t* out) {
   out[0] = e->dev.subject_lookups_walk;
   out[1] = e->dev.subject_lookups_exhaustive;
   out[2] = e->dev.subject_items_verified;
+  return ZG_OK;
+}
+
+extern "C" int zg_handle_lookup_counters(zg_engine* e, uint64_t* out) {
+  if (!e || !out) return fail(ZG_EINVAL, "NULL argument");
+  LOCK_DEVICE(e);
+  const uint64_t c[7] = {e->hl_rounds, e->hl_levels, e->hl_round_trips, e->hl_frontier, e->hl_candidates, e->hl_halvings,
+                         e->hl_fallbacks};
+  std::memcpy(out, c, sizeof c);
   return ZG_OK;
 }
 
@@ -2116,7 +2379,7 @@ extern "C" int zg_list_prefilter(zg_engine* e, const char* body, size_t len, uin
   if (!body || !out_len || !tpl) return fail(ZG_EINVAL, "NULL argument");
   if (!tpl->res_type || !tpl->permission || !tpl->subj_type || !tpl->subj_id) return fail(ZG_EINVAL, "NULL template field");
   if (mode > ZG_LIST_PROTOBUF) return fail(ZG_EINVAL, "unknown mode");
-  if (is_handle(e) && !e->host_only) return fail(ZG_EINVAL, kHandleLookupMsg);
+  if (is_handle(e) && !e->host_only && !e->handle_lookups) return fail(ZG_EINVAL, kHandleLookupMsg);
   // 1. the allowed ids (one LookupResources on the GPU; concurrent list requests share launches)
   std::vector<uint32_t> ids;
   std::string self;
@@ -2195,9 +2458,9 @@ extern "C" int zg_stats_get(zg_engine* e, zg_stats* out) {
   if (!e->host_only) e->dev.read_events(&out->stack_spills, &out->memo_batches);
   out->devices = is_handle(e) ? e->shard_devices : 1 + e->replicas.size();
   out->shards = e->n_shards;
-  out->last_levels = e->last_levels;
-  out->last_subqueries = e->last_subqueries;
-  out->last_round_trips = e->last_round_trips;
+  out->last_levels = e->last_group.levels;
+  out->last_subqueries = e->last_group.subqueries;
+  out->last_round_trips = e->last_group.round_trips;
   for (auto& r : e->replicas) {
     const Device& d = r->dev;
     out->checks += d.checks;

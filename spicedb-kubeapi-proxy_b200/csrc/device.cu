@@ -91,6 +91,7 @@ Device::~Device() {
   for (auto& l : pl_)
     for (auto* b : {&l.in, &l.val, &l.out, &l.raised, &l.parent, &l.pos}) b->release();
   for (auto* b : {&home_, &home_pos_, &home_out_, &peer_ctrl_}) b->release();
+  for (auto* b : {&hl.front[0], &hl.front[1], &hl.next, &hl.items, &hl.codes, &hl.routed, &hl.keys, &hl.ids}) b->release();
   if (pin_peer_) cudaFreeHost(pin_peer_);
   for (cudaEvent_t ev : ev_peer_)
     if (ev) cudaEventDestroy(ev);
@@ -911,12 +912,17 @@ int Device::unroute(const uint32_t* d_src, const uint8_t* d_val, uint64_t n, uin
 // ---- sharded handle (capi.cu run_sharded): the levels of DeviceShardedChecker, exchanged through peer memory --------
 static_assert(kMaxShards == kMaxRouteDest, "a PeerTable holds every routing destination");
 
-int Device::peer_begin(const zg_check* h_items, uint64_t n, uint64_t* counts, std::string* err) {
+int Device::peer_events_(std::string* err) {
+  if (!ev_peer_[0])
+    for (cudaEvent_t& ev : ev_peer_) ZG_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  return ZG_OK;
+}
+
+int Device::peer_begin(const zg_check* items, uint64_t n, uint64_t* counts, std::string* err) {
   for (uint32_t d = 0; d < own_count; ++d) counts[d] = 0;
   home_n_ = n;
   ZG_CUDA(cudaSetDevice(device));
-  if (!ev_peer_[0])
-    for (cudaEvent_t& ev : ev_peer_) ZG_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  if (int rc = peer_events_(err)) return rc;
   if (!pin_peer_) ZG_CUDA(cudaMallocHost(&pin_peer_, (4 + kMaxShards) * sizeof(unsigned long long)));
   if (!peer_ctrl_.ensure(2 * kMaxShards * sizeof(unsigned long long)) || !home_.ensure(n * sizeof(zg_check)) ||
       !home_pos_.ensure(n * 4) || !home_out_.ensure(n)) {
@@ -926,7 +932,7 @@ int Device::peer_begin(const zg_check* h_items, uint64_t n, uint64_t* counts, st
   if (n == 0) return ZG_OK;
   if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
   unsigned long long* d_counts = peer_ctrl_.as<unsigned long long>();
-  ZG_CUDA(cudaMemcpyAsync(home_.p, h_items, n * sizeof(zg_check), cudaMemcpyHostToDevice, stream));
+  ZG_CUDA(cudaMemcpyAsync(home_.p, items, n * sizeof(zg_check), cudaMemcpyDefault, stream));
   ZG_CUDA(cudaMemsetAsync(d_counts, 0, kMaxShards * sizeof(unsigned long long), stream));
   const unsigned grid = static_cast<unsigned>(std::min<uint64_t>((n + 255) / 256, static_cast<uint64_t>(sm_count_) * 8));
   route_count_kernel<<<grid, 256, 0, stream>>>(home_.as<zg_check>(), n, own_count, d_counts);
@@ -1050,7 +1056,7 @@ int Device::peer_fold(int level, const PeerTable& t, const std::vector<cudaEvent
   return ZG_OK;
 }
 
-int Device::peer_finish(const PeerTable& t, const std::vector<cudaEvent_t>& wait, uint8_t* h_out, std::string* err) {
+int Device::peer_finish(const PeerTable& t, const std::vector<cudaEvent_t>& wait, uint8_t* out, std::string* err) {
   ZG_CUDA(cudaSetDevice(device));
   if (home_n_) {
     for (cudaEvent_t ev : wait) ZG_CUDA(cudaStreamWaitEvent(stream, ev, 0));
@@ -1058,11 +1064,33 @@ int Device::peer_finish(const PeerTable& t, const std::vector<cudaEvent_t>& wait
         home_.as<zg_check>(), home_pos_.as<uint32_t>(), home_n_, own_count, t, home_out_.as<uint8_t>());
     ZG_CUDA(cudaGetLastError());
     ++launches;
-    ZG_CUDA(cudaMemcpyAsync(h_out, home_out_.p, home_n_, cudaMemcpyDeviceToHost, stream));
+    ZG_CUDA(cudaMemcpyAsync(out, home_out_.p, home_n_, cudaMemcpyDefault, stream));
   }
   ZG_CUDA(cudaEventRecord(last_done_, stream));
   have_last_ = true;
   ZG_CUDA(cudaStreamSynchronize(stream));
+  return ZG_OK;
+}
+
+bool Device::hl_ensure(DevBuf& b, uint64_t bytes) { return cudaSetDevice(device) == cudaSuccess && b.ensure(std::max<uint64_t>(bytes, 8)); }
+
+int Device::peer_put(const unsigned long long* src, uint64_t n, uint32_t n_dest, const PeerTable& t, int level, std::string* err) {
+  ZG_CUDA(cudaSetDevice(device));
+  if (int rc = peer_events_(err)) return rc;
+  if (n) {
+    if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+    const unsigned grid = static_cast<unsigned>(std::min<uint64_t>((n + 255) / 256, static_cast<uint64_t>(sm_count_) * 8));
+    peer_put_kernel<<<grid, 256, 0, stream>>>(src, n, n_dest, t);
+    ZG_CUDA(cudaGetLastError());
+    ++launches;
+  }
+  ZG_CUDA(cudaEventRecord(peer_event(level), stream));
+  return ZG_OK;
+}
+
+int Device::peer_wait(const std::vector<cudaEvent_t>& wait, std::string* err) {
+  ZG_CUDA(cudaSetDevice(device));
+  for (cudaEvent_t ev : wait) ZG_CUDA(cudaStreamWaitEvent(stream, ev, 0));
   return ZG_OK;
 }
 

@@ -176,9 +176,9 @@ class Device {
   // The handle's ONE store holds every shard's relationships; this device's snapshot keeps those whose resource id %
   // own_count == own_rank (shard_rank / shard_count equal them). own_count = 1: the store is this device's alone.
   uint32_t own_rank = 0, own_count = 1;
-  // Level 0: uploads this shard's n callers' items (pinned host) and counts them by owner: counts[d] (host, own_count).
-  // Waits for the counts (a round trip).
-  int peer_begin(const zg_check* h_items, uint64_t n, uint64_t* counts, std::string* err);
+  // Level 0: copies in this shard's n callers' items (pinned host or this device's memory) and counts them by owner:
+  // counts[d] (host, own_count). Waits for the counts (a round trip).
+  int peer_begin(const zg_check* items, uint64_t n, uint64_t* counts, std::string* err);
   // The inbox of `level` on this shard, grown to n queries; the level then holds n queries.
   zg_check* peer_inbox(int level, uint64_t n, std::string* err);
   // Writes the queries of `level` this shard sends (level 0: its callers' items; deeper: what pass level - 1 raised)
@@ -193,10 +193,24 @@ class Device {
   // d's values of level + 1) into the raising leaves and folds the level; records peer_event(level).
   int peer_fold(int level, const PeerTable& t, const std::vector<cudaEvent_t>& wait, std::string* err);
   const uint8_t* peer_values(int level) const { return pl_[static_cast<size_t>(level)].out.as<uint8_t>(); }
-  // After every shard's peer_event(0): the answers of this shard's callers' items (t as in peer_fold, level 0) -> h_out
-  // (pinned host). Waits for them (a round trip).
-  int peer_finish(const PeerTable& t, const std::vector<cudaEvent_t>& wait, uint8_t* h_out, std::string* err);
+  // After every shard's peer_event(0): the answers of this shard's callers' items (t as in peer_fold, level 0) -> out
+  // (pinned host or this device's memory). Waits for them (a round trip).
+  int peer_finish(const PeerTable& t, const std::vector<cudaEvent_t>& wait, uint8_t* out, std::string* err);
   cudaEvent_t peer_event(int level) const { return ev_peer_[level & 1]; }  // alternates: a fold waits on one, records the other
+  // LookupResources on a sharded handle (capi.cu run_sharded_lookup drives the shard_lookup_* round above on every
+  // shard): the walk's buffers of this shard. front[level & 1] = the replicated frontier `level` expands, next = what
+  // this shard's expand found (walk capacity), items / codes = its candidates and their codes, routed = its answer
+  // keys, keys / ids = every shard's keys and the answers (shard 0).
+  struct HandleLookupBufs {
+    DevBuf front[2], next, items, codes, routed, keys, ids;
+  } hl;
+  bool hl_ensure(DevBuf& b, uint64_t bytes);  // b (one of hl) grown to bytes on this device
+  uint64_t lookup_walk_cap() const { return lb_cap_; }
+  // Writes n 8-byte entries of src (this device) to t.p[d] + t.base[d] for every d < n_dest, then records
+  // peer_event(level). Runs on this shard's stream: its next work cannot overwrite src before they are written.
+  int peer_put(const unsigned long long* src, uint64_t n, uint32_t n_dest, const PeerTable& t, int level, std::string* err);
+  // This shard's next work starts after `wait` (other shards' peer_event of a level), with no host wait.
+  int peer_wait(const std::vector<cudaEvent_t>& wait, std::string* err);
   // shard_pass_dev with KParams::no_wildcards (LookupSubjects' second verification, on every pass of every rank)
   int shard_pass_nowild_dev(const zg_check* d_queries, uint64_t n, int level, uint64_t* n_sub, std::string* err);
   // ---- LookupSubjects on the sharded store (dist.DeviceShardedLookup.lookup_subjects): one round of K <= 64 ----
@@ -327,6 +341,7 @@ class Device {
   uint64_t home_n_ = 0;
   unsigned long long* pin_peer_ = nullptr;  // pinned: the control words and counts a round trip reads
   cudaEvent_t ev_peer_[2] = {nullptr, nullptr};
+  int peer_events_(std::string* err);  // creates ev_peer_ on first use
   bool no_wildcards_ = false;  // run_pass: KParams::no_wildcards (LookupSubjects' second verification)
   uint64_t lb_cap_ = 1ull << 24;  // frontier entries / candidates of one lookup batch (ZGPU_LOOKUP_BATCH_CAP)
   void* pin_lk_ = nullptr;

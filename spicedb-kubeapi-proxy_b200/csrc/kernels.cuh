@@ -1089,7 +1089,7 @@ __global__ void unroute_kernel(const uint32_t* src, const uint8_t* val, unsigned
   if (i < n) out[src[i]] = val[i];
 }
 
-// ---- sharded handle: the exchange through peer memory (device.h PeerTable, capi.cu run_sharded) ---------------
+// ---- sharded handle: the exchange through peer memory (device.h PeerTable, capi.cu run_sharded / run_sharded_lookup) --
 //
 // One process holds every shard, so a routed query is written straight into its owner's inbox, behind the part of
 // every lower shard (t.base[d], from all shards' counts), and a value is read where its owner left it: no copy
@@ -1142,6 +1142,18 @@ __global__ void peer_gather_kernel(const zg_check* items, const uint32_t* pos, u
                                    const Table t, uint8_t* out) {
   unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x;
   if (i < n) out[i] = static_cast<const uint8_t*>(t.p[items[i].res % n_dest])[pos[i]];
+}
+// LookupResources on the handle: a source shard's n 8-byte entries written to t.p[d] + t.base[d] for every d < n_dest,
+// behind the parts of the lower shards. Every shard's new frontier entries to every shard (n_dest = S, the all-gather
+// of a level), and every shard's answer keys to shard 0 (n_dest = 1).
+template <class Table>
+__global__ void __launch_bounds__(256) peer_put_kernel(const unsigned long long* src, unsigned long long n, uint32_t n_dest,
+                                                       const Table t) {
+  const unsigned long long stride = static_cast<unsigned long long>(gridDim.x) * blockDim.x;
+  for (unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x; i < n; i += stride) {
+    const unsigned long long v = src[i];
+    for (uint32_t d = 0; d < n_dest; ++d) static_cast<unsigned long long*>(t.p[d])[t.base[d] + i] = v;
+  }
 }
 
 // ---- LookupResources: candidate generation by reverse BFS ----------------------------
