@@ -335,6 +335,17 @@ int zg_lookup_subjects_counters(zg_engine *e, uint64_t *out);
  * overflowed ZGPU_LOOKUP_BATCH_CAP), out[6] rounds that verified every resource of the type (a single lookup that
  * overflowed, or ZGPU_NO_RBFS=1). */
 int zg_handle_lookup_counters(zg_engine *e, uint64_t *out);
+/* Closure indexes of the two-level steps in the engine's published snapshot (zg_stats keeps its layout): out[0] pairs
+ * indexed, out[1] pairs over the size budget (their steps meet through the memberships' reverse rows instead), out[2]
+ * index entries, out[3] index device bytes; out[4] index builds since creation (the rebuilds after writes included),
+ * out[5] device microseconds of the last publish's index builds, out[6] builds that failed (that pair then meets
+ * without an index until its next build). */
+int zg_closure_index_counters(zg_engine *e, uint64_t *out);
+/* Copies closure index `pair` (0-based, in the order of the program's two-level steps) of the published snapshot:
+ * *n_rows + 1 row offsets to row_ptr, *n_entries entries to col. ZG_E2BIG (sizes filled) when a buffer is too small,
+ * ZG_EINVAL when the pair has no index. For inspection and tests. */
+int zg_closure_index_copy(zg_engine *e, uint32_t pair, uint32_t *row_ptr, uint64_t row_cap, uint32_t *col,
+                          uint64_t col_cap, uint64_t *n_rows, uint64_t *n_entries);
 
 /* Pinned host memory for request/response buffers: zg_check_bulk copies straight
  * from/to such buffers (no staging memcpy). */

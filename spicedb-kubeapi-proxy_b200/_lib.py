@@ -177,6 +177,9 @@ _SIGS = {
                                          C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint64)]),
     "zg_lookup_subjects_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
     "zg_handle_lookup_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "zg_closure_index_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "zg_closure_index_copy": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
+                                        C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "zg_resolve_checks_packed_device": (C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]),
     "zg_check_bulk_packed_ingress": (C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_void_p, C.c_char_p, C.c_void_p, C.c_uint64, C.c_void_p]),
     "zg_intern_objects_packed": (C.c_int, [C.c_void_p, C.c_int, C.c_char_p, C.c_void_p, C.c_uint64, C.c_void_p]),
@@ -683,6 +686,25 @@ class Engine:
         out = np.zeros(3, dtype=np.uint64)
         self._ck(self._L.zg_lookup_subjects_counters(self._h, out.ctypes.data))
         return {"walks": int(out[0]), "fallbacks": int(out[1]), "items_verified": int(out[2])}
+
+    CLOSURE_INDEX_COUNTERS = ("indexed", "over_budget", "entries", "device_bytes", "builds", "last_build_us", "failures")
+
+    def closure_index_counters(self) -> dict:
+        """Closure indexes of the two-level steps in the published snapshot (zg_closure_index_counters)."""
+        out = np.zeros(len(self.CLOSURE_INDEX_COUNTERS), dtype=np.uint64)
+        self._ck(self._L.zg_closure_index_counters(self._h, out.ctypes.data))
+        return {k: int(v) for k, v in zip(self.CLOSURE_INDEX_COUNTERS, out)}
+
+    def closure_index(self, pair: int = 0):
+        """(row_ptr, col) of closure index `pair` of the published snapshot (zg_closure_index_copy)."""
+        nr, ne = C.c_uint64(0), C.c_uint64(0)
+        rc = self._L.zg_closure_index_copy(self._h, pair, None, 0, None, 0, C.byref(nr), C.byref(ne))
+        if rc != E2BIG:
+            self._ck(rc)
+        row_ptr, col = np.empty(nr.value + 1, dtype=np.uint32), np.empty(max(ne.value, 1), dtype=np.uint32)
+        self._ck(self._L.zg_closure_index_copy(self._h, pair, row_ptr.ctypes.data, row_ptr.size, col.ctypes.data, col.size,
+                                               C.byref(nr), C.byref(ne)))
+        return row_ptr, col[: ne.value]
 
     HANDLE_LOOKUP_COUNTERS = ("rounds", "levels", "round_trips", "frontier_entries", "candidates", "halvings", "fallbacks")
 

@@ -124,7 +124,153 @@ int bits_for(unsigned long long max_value) {
   return b;
 }
 
+// ---- closure index of a two-level pair (a = innermost direct class, b = userset class tgc) ----
+// row u = the union of rrow(g, b) over g in rrow(u, a); the reverse rows are read from the resident snapshot
+
+__device__ __forceinline__ void rrow_of(const uint32_t* rrow_ptr, const DCls& c, uint32_t s, uint32_t* lo, uint32_t* hi) {
+  const unsigned long long ri = c.rrow_base + static_cast<unsigned long long>(s) * c.rstride;
+  *lo = rrow_ptr[ri];
+  *hi = rrow_ptr[ri + 1];
+}
+
+// cnt[u + 1] = sum of |rrow(g, b)| over the memberships g of u; *rels += relationships of class a (and of class b for
+// the subjects g < b.nsubj, counted by the threads u < b.nsubj)
+__global__ void closure_count_kernel(const uint32_t* rrow_ptr, const uint32_t* rcol, DCls a, DCls b, uint32_t n,
+                                     unsigned long long* cnt, unsigned long long* rels) {
+  const uint32_t u = blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned long long sum = 0, own = 0;
+  if (u < n) {
+    uint32_t lo = 0, hi = 0;
+    if (u < a.nsubj) rrow_of(rrow_ptr, a, u, &lo, &hi);
+    own = hi - lo;
+    for (uint32_t x = lo; x < hi; ++x) {
+      const uint32_t g = rcol[x];
+      if (g >= b.nsubj) continue;
+      uint32_t l = 0, h = 0;
+      rrow_of(rrow_ptr, b, g, &l, &h);
+      sum += h - l;
+    }
+    cnt[u + 1] = sum;
+    if (u < b.nsubj) {
+      uint32_t l = 0, h = 0;
+      rrow_of(rrow_ptr, b, u, &l, &h);
+      own += h - l;
+    }
+  }
+  for (int d = 16; d >= 1; d >>= 1) own += __shfl_xor_sync(0xFFFFFFFFu, own, d);
+  if ((threadIdx.x & 31) == 0 && own) atomicAdd(rels, own);
+}
+
+__global__ void closure_fill_kernel(const uint32_t* rrow_ptr, const uint32_t* rcol, DCls a, DCls b, uint32_t n,
+                                    const unsigned long long* off, uint32_t* out) {
+  const uint32_t u = blockIdx.x * blockDim.x + threadIdx.x;
+  if (u >= n || u >= a.nsubj) return;
+  unsigned long long at = off[u];
+  uint32_t lo, hi;
+  rrow_of(rrow_ptr, a, u, &lo, &hi);
+  for (uint32_t x = lo; x < hi; ++x) {
+    const uint32_t g = rcol[x];
+    if (g >= b.nsubj) continue;
+    uint32_t l, h;
+    rrow_of(rrow_ptr, b, g, &l, &h);
+    for (uint32_t y = l; y < h; ++y) out[at++] = rcol[y];
+  }
+}
+
+// distinct entries of each sorted row: counted into ucnt[u + 1] (out == nullptr), or written to out[row_ptr[u] ..]
+__global__ void closure_unique_kernel(const uint32_t* sorted, const unsigned long long* off, uint32_t n, uint32_t* ucnt,
+                                      const uint32_t* row_ptr, uint32_t* out) {
+  const uint32_t u = blockIdx.x * blockDim.x + threadIdx.x;
+  if (u >= n) return;
+  const unsigned long long lo = off[u], hi = off[u + 1];
+  uint32_t k = 0, at = out ? row_ptr[u] : 0u;
+  for (unsigned long long x = lo; x < hi; ++x) {
+    if (x > lo && sorted[x] == sorted[x - 1]) continue;
+    if (out) out[at + k] = sorted[x];
+    ++k;
+  }
+  if (!out) ucnt[u + 1] = k;
+}
+
 }  // namespace
+
+std::string gpu_build_closure(const Snapshot& s, const DCls& a, const DCls& b, uint64_t cap, Snapshot::Closure* c,
+                              cudaStream_t st) {
+  c->built = false;
+  c->entries = 0;
+  c->nsubj = a.nsubj;
+  const uint32_t n = std::max(a.nsubj, b.nsubj);  // threads of the count pass (it also sums class b's relationships)
+  if (a.nsubj == 0) return "";
+  DevBuf d_off, d_keys[2], d_tmp, d_rels;
+  struct Release {
+    std::vector<DevBuf*> v;
+    ~Release() {
+      for (DevBuf* x : v) x->release();
+    }
+  } rel{{&d_off, &d_keys[0], &d_keys[1], &d_tmp, &d_rels}};
+  if (!d_off.ensure((size_t(n) + 1) * 8) || !d_rels.ensure(16)) return "out of device memory (closure index)";
+  BCUDA(cudaMemsetAsync(d_off.p, 0, (size_t(n) + 1) * 8, st));
+  BCUDA(cudaMemsetAsync(d_rels.p, 0, 8, st));
+  const unsigned blk = 256, grid = (n + blk - 1) / blk;
+  const uint32_t* rp = s.rrow_ptr.as<uint32_t>();
+  const uint32_t* rc = s.rcol.as<uint32_t>();
+  closure_count_kernel<<<grid, blk, 0, st>>>(rp, rc, a, b, n, d_off.as<unsigned long long>(), d_rels.as<unsigned long long>());
+  unsigned long long* off = d_off.as<unsigned long long>();
+  size_t tb = 0;
+  cub::DeviceScan::InclusiveSum(nullptr, tb, off, off, a.nsubj + 1, st);
+  if (!d_tmp.ensure(tb + 256)) return "out of device memory (closure index)";
+  tb = d_tmp.cap;
+  BCUDA(cub::DeviceScan::InclusiveSum(d_tmp.p, tb, off, off, a.nsubj + 1, st));
+  unsigned long long hb[2] = {0, 0};
+  BCUDA(cudaMemcpyAsync(&hb[0], off + a.nsubj, 8, cudaMemcpyDeviceToHost, st));
+  BCUDA(cudaMemcpyAsync(&hb[1], d_rels.p, 8, cudaMemcpyDeviceToHost, st));
+  BCUDA(cudaStreamSynchronize(st));
+  const uint64_t total = hb[0], rels = hb[1];
+  // Size budget, checked on the exact count before anything is allocated: the entries before duplicates are removed
+  // (sorted twice) must stay within kClosureRatio x the relationships of the two classes, a quarter of the free device
+  // memory, and what one cub sort takes (2^31 keys). `cap` (ZGPU_CLOSURE_CAP) replaces the ratio.
+  size_t free_b = 0, total_b = 0;
+  BCUDA(cudaMemGetInfo(&free_b, &total_b));
+  const uint64_t limit = std::min<uint64_t>({cap != ~0ull ? cap : kClosureRatio * rels, free_b / 4 / 12, (1ull << 31) - 1});
+  if (total > limit) {  // no index: the pair's steps keep batch_l2
+    c->row_ptr.release();
+    c->col.release();
+    return "";
+  }
+  if (total) {
+    if (!d_keys[0].ensure(total * 4) || !d_keys[1].ensure(total * 4)) return "out of device memory (closure index)";
+    closure_fill_kernel<<<(a.nsubj + blk - 1) / blk, blk, 0, st>>>(rp, rc, a, b, a.nsubj, off, d_keys[0].as<uint32_t>());
+    size_t sb = 0;
+    cub::DeviceSegmentedSort::SortKeys(nullptr, sb, d_keys[0].as<uint32_t>(), d_keys[1].as<uint32_t>(), static_cast<int>(total),
+                                       static_cast<int>(a.nsubj), off, off + 1, st);
+    if (!d_tmp.ensure(sb + 256)) return "out of device memory (closure sort scratch)";
+    sb = d_tmp.cap;
+    BCUDA(cub::DeviceSegmentedSort::SortKeys(d_tmp.p, sb, d_keys[0].as<uint32_t>(), d_keys[1].as<uint32_t>(),
+                                             static_cast<int>(total), static_cast<int>(a.nsubj), off, off + 1, st));
+  }
+  if (!c->row_ptr.ensure((size_t(a.nsubj) + 1) * 4)) return "out of device memory (closure index)";
+  uint32_t* crow = c->row_ptr.as<uint32_t>();
+  BCUDA(cudaMemsetAsync(crow, 0, (size_t(a.nsubj) + 1) * 4, st));
+  const unsigned ug = (a.nsubj + blk - 1) / blk;
+  if (total) closure_unique_kernel<<<ug, blk, 0, st>>>(d_keys[1].as<uint32_t>(), off, a.nsubj, crow, nullptr, nullptr);
+  tb = 0;
+  cub::DeviceScan::InclusiveSum(nullptr, tb, crow, crow, a.nsubj + 1, st);
+  if (!d_tmp.ensure(tb + 256)) return "out of device memory (closure index)";
+  tb = d_tmp.cap;
+  BCUDA(cub::DeviceScan::InclusiveSum(d_tmp.p, tb, crow, crow, a.nsubj + 1, st));
+  uint32_t nu = 0;
+  BCUDA(cudaMemcpyAsync(&nu, crow + a.nsubj, 4, cudaMemcpyDeviceToHost, st));
+  BCUDA(cudaStreamSynchronize(st));
+  // + 4 words: the aligned 16-byte block that holds a row's last entry ends inside the allocation
+  if (!c->col.ensure((size_t(nu) + 4) * 4)) return "out of device memory (closure index)";
+  BCUDA(cudaMemsetAsync(c->col.p, 0, (size_t(nu) + 4) * 4, st));
+  if (total) closure_unique_kernel<<<ug, blk, 0, st>>>(d_keys[1].as<uint32_t>(), off, a.nsubj, nullptr, crow, c->col.as<uint32_t>());
+  BCUDA(cudaStreamSynchronize(st));
+  BCUDA(cudaGetLastError());
+  c->entries = nu;
+  c->built = true;
+  return "";
+}
 
 std::string sort_u32(const uint32_t* d_in, uint32_t* d_out, uint64_t n, cudaStream_t st) {
   static thread_local DevBuf tmp;  // grow-only scratch per calling thread

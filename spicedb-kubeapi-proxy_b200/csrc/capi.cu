@@ -2317,6 +2317,40 @@ extern "C" int zg_lookup_subjects_counters(zg_engine* e, uint64_t* out) {
   return ZG_OK;
 }
 
+extern "C" int zg_closure_index_counters(zg_engine* e, uint64_t* out) {
+  if (!e || !out) return fail(ZG_EINVAL, "NULL argument");
+  LOCK_DEVICE(e);
+  uint64_t c[7] = {0, 0, 0, 0, e->dev.closure_builds, static_cast<uint64_t>(e->dev.closure_ms * 1000.0),
+                   e->dev.closure_failures};
+  if (const auto s = e->dev.snap)
+    for (const auto& x : s->closure) {
+      ++c[x.built ? 0 : 1];
+      c[2] += x.entries;
+      c[3] += x.row_ptr.cap + x.col.cap;
+    }
+  std::memcpy(out, c, sizeof c);
+  return ZG_OK;
+}
+
+extern "C" int zg_closure_index_copy(zg_engine* e, uint32_t pair, uint32_t* row_ptr, uint64_t row_cap, uint32_t* col,
+                                     uint64_t col_cap, uint64_t* n_rows, uint64_t* n_entries) {
+  if (!e || !n_rows || !n_entries) return fail(ZG_EINVAL, "NULL argument");
+  LOCK_DEVICE(e);
+  const auto s = e->dev.snap;
+  if (!s) return fail(ZG_ENOSNAPSHOT, "no snapshot published (call zg_publish)");
+  if (pair >= s->closure.size() || !s->closure[pair].built) return fail(ZG_EINVAL, "no closure index for this pair");
+  const auto& x = s->closure[pair];
+  *n_rows = x.nsubj;
+  *n_entries = x.entries;
+  if (row_cap < uint64_t(x.nsubj) + 1 || col_cap < x.entries || !row_ptr || (!col && x.entries))
+    return fail(ZG_E2BIG, "buffers too small for the closure index");
+  cudaError_t ce = cudaSetDevice(e->dev.device);
+  if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->dev.stream);
+  if (ce == cudaSuccess) ce = cudaMemcpy(row_ptr, x.row_ptr.p, (uint64_t(x.nsubj) + 1) * 4, cudaMemcpyDeviceToHost);
+  if (ce == cudaSuccess && x.entries) ce = cudaMemcpy(col, x.col.p, x.entries * 4, cudaMemcpyDeviceToHost);
+  return ce == cudaSuccess ? ZG_OK : fail(ZG_ECUDA, std::string("zg_closure_index_copy: ") + cudaGetErrorString(ce));
+}
+
 extern "C" int zg_handle_lookup_counters(zg_engine* e, uint64_t* out) {
   if (!e || !out) return fail(ZG_EINVAL, "NULL argument");
   LOCK_DEVICE(e);

@@ -66,6 +66,10 @@ Snapshot::~Snapshot() {
   ls_fwd.release();
   ls_type_off.release();
   ls_mask.release();
+  for (auto& c : closure) {
+    c.row_ptr.release();
+    c.col.release();
+  }
 }
 
 Device::~Device() {
@@ -118,6 +122,7 @@ std::string Device::init(int dev, uint64_t subq_cap, uint32_t budget) {
   if (const char* v = std::getenv("ZGPU_NO_INVERT")) invert = !(*v && *v != '0');
   if (const char* v = std::getenv("ZGPU_NO_RBFS")) use_rbfs = !(*v && *v != '0');
   if (const char* v = std::getenv("ZGPU_LOOKUP_BATCH_CAP")) lb_cap_ = std::max<uint64_t>(1024, std::strtoull(v, nullptr, 10));
+  if (const char* v = std::getenv("ZGPU_CLOSURE_CAP")) closure_cap_ = std::strtoull(v, nullptr, 10);  // tests: 0 = no index
   int count = 0;
   cudaError_t e = cudaGetDeviceCount(&count);
   if (e != cudaSuccess || count == 0)
@@ -150,6 +155,7 @@ std::string Device::init(int dev, uint64_t subq_cap, uint32_t budget) {
 
 std::string Device::publish(const HostSnapshot& h, const Schema& sc, uint64_t revision) {
   cudaSetDevice(device);
+  closure_ms = 0;
   auto s = std::make_shared<Snapshot>();
   auto up = [&](DevBuf& b, const void* src, size_t bytes) -> bool {
     if (!b.ensure(bytes + 64)) return false;  // + 64: rows are streamed with aligned 128-bit loads (build.cu)
@@ -174,6 +180,7 @@ std::string Device::publish(const HostSnapshot& h, const Schema& sc, uint64_t re
 
 std::string Device::publish_gpu(const Store& store, const Schema& sc, uint64_t revision, bool verify) {
   cudaSetDevice(device);
+  closure_ms = 0;
   HostSnapshot lay = store.layout();
   auto s = std::make_shared<Snapshot>();
   cudaEvent_t e0, e1;
@@ -247,6 +254,7 @@ std::string Device::publish_delta(const Store& store, const Schema& sc, uint64_t
   if (!s || !s->delta_ok || !store.journal_ok || own_store_shard || store.journal.size() > kMaxDelta || !store.layout_stable())
     return "full";
   cudaSetDevice(device);
+  closure_ms = 0;
   HostSnapshot lay = store.layout();  // same capacities as the resident snapshot: same bases
   if (lay.n_objects != s->n_objects) return "full";
   // readers on other streams (zg_check_bulk_device) are ordered through last_done_
@@ -257,6 +265,16 @@ std::string Device::publish_delta(const Store& store, const Schema& sc, uint64_t
   cudaEventRecord(e0, stream);
   std::vector<uint32_t> cls_delta;
   std::string err = gpu_apply_delta(store, sc, lay, stream, s.get(), &cls_delta, own_rank, own_count);
+  if (err.empty() && !s->closure.empty()) {
+    // a closure index whose classes this write changed is rebuilt from the merged reverse rows before anybody reads
+    // the snapshot again: a stale index is never read
+    std::vector<uint8_t> touched(lay.cls.size(), 0);
+    for (const auto& j : store.journal) {
+      const int k = sc.class_of(j.t.rel, j.t.stype, j.t.srel);
+      if (k >= 0) touched[lay.rels[sc.slots[j.t.rel].rel_index].cls_begin + k] = 1;
+    }
+    build_closures(s.get(), lay.cls, &touched);
+  }
   cudaEventRecord(e1, stream);
   cudaEventRecord(last_done_, stream);
   have_last_ = true;
@@ -285,6 +303,41 @@ std::string Device::publish_delta(const Store& store, const Schema& sc, uint64_t
     if (s->cls_count[c]) lay.cls[c].flags &= static_cast<uint16_t>(~CF_EMPTY);
   lay.n_tuples = s->n_tuples;
   return finish_publish(s, lay, sc, revision);
+}
+
+void Device::build_closures(Snapshot* s, const std::vector<DCls>& cls, const std::vector<uint8_t>* rebuild) {
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  for (auto& c : s->closure) {
+    if (rebuild ? !((*rebuild)[c.inner] || (*rebuild)[c.tgc]) : c.done) continue;
+    if (!e0) {
+      cudaEventCreate(&e0);
+      cudaEventCreate(&e1);
+    }
+    cudaEventRecord(e0, stream);
+    std::string err = gpu_build_closure(*s, cls[c.inner], cls[c.tgc], closure_cap_, &c, stream);
+    cudaEventRecord(e1, stream);
+    cudaEventSynchronize(e1);
+    float ms = 0;
+    cudaEventElapsedTime(&ms, e0, e1);
+    closure_ms += ms;
+    c.done = true;
+    if (!err.empty()) {
+      // The index is optional: a build that fails (an allocation the budget did not foresee) leaves the pair without
+      // one, and its steps meet through batch_l2. Nothing half built is ever handed to the kernel.
+      c.built = false;
+      c.entries = 0;
+      c.row_ptr.release();
+      c.col.release();
+      cudaGetLastError();
+      ++closure_failures;
+      continue;
+    }
+    ++closure_builds;
+  }
+  if (e0) {
+    cudaEventDestroy(e0);
+    cudaEventDestroy(e1);
+  }
 }
 
 std::string Device::finish_publish(std::shared_ptr<Snapshot> s, const HostSnapshot& h, const Schema& sc, uint64_t revision) {
@@ -347,7 +400,38 @@ std::string Device::finish_publish(std::shared_ptr<Snapshot> s, const HostSnapsh
   {
     const DHeader* ph = reinterpret_cast<const DHeader*>(blob.data());
     const DStep* steps = reinterpret_cast<const DStep*>(blob.data() + ph->off_steps);
-    for (uint32_t i = 0; i < ph->n_steps; ++i) s->has_l2 = s->has_l2 || (steps[i].flags & kStepTargetL2);
+    // the pairs of the two-level steps: a pair indexed by an earlier publish of this snapshot keeps its index (a write
+    // that changed one of its classes has rebuilt it already, publish_delta). Only an unsharded engine with the
+    // direction-optimised probes has any: a shard does not hold the subjects' reverse rows, and without the probes
+    // nothing meets. An engine without pairs builds nothing, at publish or after a write.
+    const bool indexable = invert && shard_count <= 1 && own_count <= 1;
+    std::vector<Snapshot::Closure> pairs;
+    for (uint32_t i = 0; i < ph->n_steps; ++i) {
+      if (!(steps[i].flags & kStepTargetL2)) continue;
+      s->has_l2 = true;
+      if (!indexable) continue;
+      const uint16_t inner = sc.d_inv_cls[sc.d_type_inv[steps[i].tstype].begin + steps[i].tinv], tgc = steps[i].tgc;
+      bool seen = false;
+      for (const auto& c : pairs) seen = seen || c.tgc == tgc;
+      if (seen || pairs.size() == static_cast<size_t>(kMaxClosure)) continue;
+      auto old = std::find_if(s->closure.begin(), s->closure.end(),
+                              [&](const Snapshot::Closure& c) { return c.tgc == tgc && c.inner == inner; });
+      if (old != s->closure.end()) {
+        pairs.push_back(*old);
+        old->row_ptr = DevBuf{};  // moved
+        old->col = DevBuf{};
+      } else {
+        pairs.emplace_back();
+        pairs.back().inner = inner;
+        pairs.back().tgc = tgc;
+      }
+    }
+    for (auto& c : s->closure) {
+      c.row_ptr.release();
+      c.col.release();
+    }
+    s->closure = std::move(pairs);
+    build_closures(s.get(), h.cls, nullptr);
   }
   s->revision = revision;
 
@@ -427,6 +511,8 @@ int Device::run_pass(const Snapshot& s, const zg_check* queries, uint64_t nq, ui
   p.shard_count = shard_count;
   p.shard_rank = shard_rank;
   p.no_wildcards = no_wildcards_ ? 1 : 0;
+  for (const auto& c : s.closure)
+    if (c.built) p.closure[p.n_closure++] = ClosureRef{c.row_ptr.as<uint32_t>(), c.col.as<uint32_t>(), c.nsubj, c.tgc};
   ZG_CUDA(cudaMemsetAsync(ctrl, 0, 16, st));  // next, subq_count
   const int per_sm = count ? blocks_per_sm_count_ : blocks_per_sm_;
   uint64_t want = (nq + kThreads - 1) / kThreads;

@@ -50,6 +50,17 @@ struct Snapshot {
   uint32_t max_leaves = 1;
   bool has_nonpure = false;
   bool has_l2 = false;  // some step of the program meets two levels (kStepTargetL2)
+  // Closure index of every (innermost direct class, userset class tgc) pair of the two-level steps (kernels.cuh
+  // ClosureRef; built by gpu_build_closure, unsharded engines only). A pair over the size budget has none.
+  struct Closure {
+    uint16_t inner = 0, tgc = 0;
+    DevBuf row_ptr, col;
+    uint32_t nsubj = 0;
+    uint64_t entries = 0;
+    bool done = false;   // the budget was checked against this snapshot's relationships
+    bool built = false;  // ... and the index built
+  };
+  std::vector<Closure> closure;
   uint64_t n_tuples = 0, bytes = 0, revision = 0;
   ~Snapshot();
 };
@@ -95,6 +106,9 @@ class Device {
   // can publish this state (no snapshot, re-layout, bulk load, huge delta), else an error message.
   std::string publish_delta(const Store& store, const Schema& sc, uint64_t revision);
   uint64_t delta_publishes = 0, full_publishes = 0;
+  uint64_t closure_builds = 0;    // closure indexes built (the rebuilds after writes included)
+  uint64_t closure_failures = 0;  // builds that failed (the pair met through batch_l2 until its next build)
+  double closure_ms = 0;          // device time of the closure index builds of the last publish
   // ZGPU_VERIFY_BUILD=1: every array of the resident snapshot against the host builder's
   std::string verify_against_host(const Store& store, const Schema& sc);
   std::string verify_snapshot(Snapshot& s, const Store& store, const Schema& sc, const HostSnapshot* lay);
@@ -292,6 +306,11 @@ class Device {
   uint64_t last_alg_bytes = 0;
 
  private:
+  uint64_t closure_cap_ = ~0ull;  // ZGPU_CLOSURE_CAP: entries a closure index may hold (tests; ~0 = the size budget)
+  // (Re)builds the closure index of every pair of s->closure that is not built yet (`rebuild` false) or whose inner or
+  // tgc class is marked in `rebuild` (a write changed it), from the classes' reverse rows described by cls. A pair whose
+  // build fails is left without an index (closure_failures).
+  void build_closures(Snapshot* s, const std::vector<DCls>& cls, const std::vector<uint8_t>* rebuild);
   int ingress_sync(const Store& store, cudaStream_t st, std::string* err);
   std::string finish_publish(std::shared_ptr<Snapshot> s, const HostSnapshot& lay, const Schema& sc, uint64_t revision);
   // One check_kernel launch over `nq` queries: val (may be null) receives the per-(query, leaf) value
@@ -385,5 +404,12 @@ std::string gpu_apply_delta(const Store& store, const Schema& sc, const HostSnap
                             std::vector<uint32_t>* cls_delta, uint32_t owner_rank = 0, uint32_t owner_count = 1);
 // (Re)builds s->resources[] / n_resources[] from the forward row table.
 std::string gpu_resource_lists(Snapshot* s, cudaStream_t st);
+// Size budget of a closure index: entries (before duplicates are removed) per relationship of its two classes. cfg3's
+// shape (8 memberships per user, 10 teams per group) needs about 9.
+constexpr uint64_t kClosureRatio = 16;
+// Builds the closure index of the pair (a, b) from the resident reverse CSR of s into *c, unless it would hold more
+// than cap entries (~0: the budget above) or more than a quarter of the free device memory; c->built tells which.
+std::string gpu_build_closure(const Snapshot& s, const DCls& a, const DCls& b, uint64_t cap, Snapshot::Closure* c,
+                              cudaStream_t st);
 
 }  // namespace zg

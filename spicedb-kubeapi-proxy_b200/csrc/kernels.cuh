@@ -67,6 +67,26 @@ constexpr uint16_t kJobDepthMask = 0x00FF;  // zg_check.flags of a raised sub-qu
 // value bits of a (query, leaf) pair and of a sub-query
 constexpr uint8_t kValT = 1, kValE = 2;
 
+// Closure index of one two-level pair (DESIGN.md §4), built at publish (build.cu gpu_build_closure): for the
+// kStepTargetL2 steps of class tgc, row u = col[row_ptr[u], row_ptr[u + 1]) lists, ascending and distinct, every object
+// the subject u reaches through one of its memberships g: the union of g's reverse rows in class tgc. col is padded so
+// that the aligned 16-byte block holding a row's last word lies inside the allocation.
+constexpr int kMaxClosure = 4;
+#ifndef ZG_CLOSURE_BLOCKS
+#define ZG_CLOSURE_BLOCKS 2
+#endif
+#ifndef ZG_CLOSURE_VERIFY
+#define ZG_CLOSURE_VERIFY 8
+#endif
+constexpr int kClosureBlocks = ZG_CLOSURE_BLOCKS;  // 16-byte blocks in flight per lane per round of closure_meet
+constexpr int kClosureVerify = ZG_CLOSURE_VERIFY;  // pending "maybe"s of a warp that trigger their searches
+struct ClosureRef {
+  const uint32_t* row_ptr;
+  const uint32_t* col;
+  uint32_t nsubj;  // rows (subjects of the innermost direct class)
+  uint32_t tgc;
+};
+
 struct KParams {
   const uint32_t* row_ptr;
   const uint32_t* col;
@@ -114,6 +134,9 @@ struct KParams {
   // LookupSubjects' second verification: every wildcard relationship is invisible (an ST_WILD step never matches),
   // so a subject that checks HAS is granted through its own relationships. Never set by the public check calls.
   int no_wildcards;
+  // two-level steps whose pair has a closure index meet over it; the others keep batch_l2
+  ClosureRef closure[kMaxClosure];
+  uint32_t n_closure;
 };
 
 // View of the program blob. Only the base pointer is kept in registers; table addresses are
@@ -332,6 +355,35 @@ __device__ __forceinline__ bool l2_maybe(unsigned long long f0, unsigned long lo
   l2_bits(v, b1, b2);
   return ((((b1 & 64u) ? f1 : f0) >> (b1 & 63u)) & (((b2 & 64u) ? f1 : f0) >> (b2 & 63u)) & 1ull) != 0;
 }
+// The filter of the range col[lo, hi), four independent loads in flight.
+__device__ __forceinline__ void l2_filter(const uint32_t* __restrict__ col, uint32_t lo, uint32_t hi, unsigned long long& f0,
+                                          unsigned long long& f1) {
+  for (uint32_t x = lo; x < hi; x += 4) {
+    uint32_t v[4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) v[i] = x + i < hi ? __ldg(col + x + i) : 0u;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      if (x + i >= hi) break;
+      uint32_t b1, b2;
+      l2_bits(v[i], b1, b2);
+      if (b1 & 64u) f1 |= 1ull << (b1 & 63u); else f0 |= 1ull << (b1 & 63u);
+      if (b2 & 64u) f1 |= 1ull << (b2 & 63u); else f0 |= 1ull << (b2 & 63u);
+    }
+  }
+}
+// Is v an element of the sorted range col[a, b)? (the filter said maybe)
+template <bool COUNT>
+__device__ __forceinline__ bool l2_verify(const uint32_t* __restrict__ col, uint32_t a, uint32_t b, uint32_t v,
+                                          unsigned long long& nb) {
+  while (a < b) {
+    const uint32_t mid = a + ((b - a) >> 1), t = __ldg(col + mid);
+    if (COUNT) nb += 4;
+    if (t == v) return true;
+    if (t < v) a = mid + 1; else b = mid;
+  }
+  return false;
+}
 
 // Two-level meet, batched: every requesting lane of a visit round is served at once (per-lane meets ran with few of
 // the 32 lanes active: row counts and early exits differ per check). Lane j wants "does some membership g of its
@@ -355,19 +407,7 @@ __device__ __forceinline__ unsigned batch_l2(const uint32_t* __restrict__ col, c
   unsigned long long f0 = 0, f1 = 0;
   uint32_t mb = 0, me = 0;
   if (want) {
-    for (uint32_t x = lo; x < hi; x += 4) {  // four independent loads in flight
-      uint32_t v[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) v[i] = x + i < hi ? __ldg(col + x + i) : 0u;
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        if (x + i >= hi) break;
-        uint32_t b1, b2;
-        l2_bits(v[i], b1, b2);
-        if (b1 & 64u) f1 |= 1ull << (b1 & 63u); else f0 |= 1ull << (b1 & 63u);
-        if (b2 & 64u) f1 |= 1ull << (b2 & 63u); else f0 |= 1ull << (b2 & 63u);
-      }
-    }
+    l2_filter(col, lo, hi, f0, f1);
     if (COUNT) nb += 4ull * (hi - lo);
     if (!(k & 0x8000u)) {
       mb = k & 31u;
@@ -434,21 +474,109 @@ __device__ __forceinline__ unsigned batch_l2(const uint32_t* __restrict__ col, c
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
             if (x + i >= h || hit || !l2_maybe(g0, g1, v[i])) continue;
-            uint32_t a = jlo, b = jhi;  // the filter said maybe: is v[i] a child of the range?
-            while (a < b) {
-              const uint32_t mid = a + ((b - a) >> 1), t = __ldg(col + mid);
-              if (COUNT) nb += 4;
-              if (t == v[i]) {
-                hit = true;
-                break;
-              }
-              if (t < v[i]) a = mid + 1; else b = mid;
-            }
+            hit = l2_verify<COUNT>(col, jlo, jhi, v[i], nb);
           }
         }
       }
     }
     hits |= __reduce_or_sync(kFull, hit ? (1u << js) : 0u);
+  }
+  if (COUNT) *bytes += nb;
+  return hits;
+}
+
+// Two-level meet over a closure index, batched like batch_l2: lane j wants "does its range col[lo, hi) list an element
+// of its subject's closure row ccol[rb, re)" (rb < re). The rows of the requesting lanes are cut into aligned 16-byte
+// blocks, numbered with one scan and dealt out 32 at a time, so neighbouring lanes read neighbouring blocks of a row and
+// no load waits for another. Each word of a block that lies inside its row is tested against the owner's 128-bit filter
+// of the range; a "maybe" is verified by a binary search of the range. Blocks of a check already answered are skipped.
+// fw: kMeetWords words of shared memory per warp. Returns the job slots answered.
+template <bool COUNT>
+__device__ __forceinline__ unsigned closure_meet(const uint32_t* __restrict__ col, const uint32_t* ccol, unsigned long long* fw,
+                                                 uint32_t lane, bool want, uint32_t lo, uint32_t hi, uint32_t rb, uint32_t re,
+                                                 uint32_t jslot, unsigned long long* bytes) {
+  unsigned long long nb = 0;
+  unsigned long long f0 = 0, f1 = 0;
+  uint32_t b0 = 0, cnt = 0;
+  if (want) {
+    l2_filter(col, lo, hi, f0, f1);
+    if (COUNT) nb += 4ull * (hi - lo);
+    b0 = rb >> 2;
+    cnt = ((re - 1) >> 2) + 1 - b0;
+  }
+  fw[lane] = f0;
+  fw[32 + lane] = f1;
+  uint32_t incl = cnt;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) {
+    const uint32_t v = __shfl_up_sync(kFull, incl, d);
+    if (static_cast<int>(lane) >= d) incl += v;
+  }
+  const uint32_t total = __shfl_sync(kFull, incl, 31);
+  const uint32_t db = b0 - (incl - cnt);  // this lane's block p is block p + db of ccol
+  const unsigned long long cp = reinterpret_cast<unsigned long long>(ccol);
+  __syncwarp();
+  unsigned hits = 0;
+  // This lane's pending "maybe": a word the filter of owner pj let through, not verified yet (pj < 0: none). The
+  // searches are deferred and run for the whole warp at once: verified one by one, nearly every round had a lane whose
+  // search the warp waited for.
+  int pj = -1;
+  uint32_t pv = 0;
+  for (uint32_t base = 0; base < total; base += 32u * kClosureBlocks) {
+    uint4 q[kClosureBlocks];
+    int jj[kClosureBlocks];  // owner lane of each block loaded, -1: none
+#pragma unroll
+    for (int k = 0; k < kClosureBlocks; ++k) {
+      const uint32_t p = base + 32u * k + lane;
+      int j = 0;  // owner lane of block p: # lanes with incl <= p
+#pragma unroll
+      for (int step = 16; step >= 1; step >>= 1) {
+        const int probe_lane = j + step - 1;
+        const uint32_t v = __shfl_sync(kFull, incl, probe_lane & 31);
+        if (probe_lane < 32 && v <= p) j += step;
+      }
+      const uint32_t jdb = __shfl_sync(kFull, db, j & 31), js = __shfl_sync(kFull, jslot, j & 31);
+      const uint4* const jcol = reinterpret_cast<const uint4*>(__shfl_sync(kFull, cp, j & 31));
+      jj[k] = -1;
+      q[k] = make_uint4(0, 0, 0, 0);
+      if (p < total && !((hits >> js) & 1u)) {
+        jj[k] = j;
+        q[k] = __ldg(jcol + (p + jdb));  // all blocks of the round in flight together (p + jdb wraps in 32 bits)
+      }
+    }
+    unsigned mine = 0;  // job slots this lane answered in this round
+#pragma unroll
+    for (int k = 0; k < kClosureBlocks; ++k) {
+      const int j = jj[k];
+      const uint32_t src = j < 0 ? 0u : static_cast<uint32_t>(j);
+      const uint32_t jdb = __shfl_sync(kFull, db, src), js = __shfl_sync(kFull, jslot, src);
+      const uint32_t jrb = __shfl_sync(kFull, rb, src), jre = __shfl_sync(kFull, re, src);
+      const uint32_t jlo = __shfl_sync(kFull, lo, src), jhi = __shfl_sync(kFull, hi, src);
+      if (j < 0) continue;
+      const uint32_t w0 = (base + 32u * k + lane + jdb) * 4u;
+      const uint32_t v[4] = {q[k].x, q[k].y, q[k].z, q[k].w};
+      if (COUNT) nb += 4ull * (min(jre, w0 + 4u) - max(jrb, w0));
+      const unsigned long long g0 = fw[j], g1 = fw[32 + j];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        if (w0 + i < jrb || w0 + i >= jre || ((mine >> js) & 1u) || !l2_maybe(g0, g1, v[i])) continue;
+        if (pj < 0) {
+          pj = j;
+          pv = v[i];
+        } else if (l2_verify<COUNT>(col, jlo, jhi, v[i], nb)) {  // the slot is taken: verify this one now
+          mine |= 1u << js;
+        }
+      }
+    }
+    const unsigned pend = __ballot_sync(kFull, pj >= 0);
+    if (__popc(pend) >= kClosureVerify || (pend && base + 32u * kClosureBlocks >= total)) {
+      const uint32_t src = pj < 0 ? 0u : static_cast<uint32_t>(pj);
+      const uint32_t plo = __shfl_sync(kFull, lo, src), phi = __shfl_sync(kFull, hi, src);
+      const uint32_t ps = __shfl_sync(kFull, jslot, src);
+      if (pj >= 0 && !(((hits | mine) >> ps) & 1u) && l2_verify<COUNT>(col, plo, phi, pv, nb)) mine |= 1u << ps;
+      pj = -1;
+    }
+    hits |= __reduce_or_sync(kFull, mine);
   }
   if (COUNT) *bytes += nb;
   return hits;
@@ -517,8 +645,9 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
   // ---- edge classes that may push a range (userset subjects, arrows): warp-collective
   const int maxsteps = __reduce_max_sync(kFull, npush);
   for (int i = 0; i < maxsteps; ++i) {
-    bool want = false, l2_want = false;
-    uint32_t l2_lo = 0, l2_hi = 0, l2_k = 0;
+    bool want = false, l2_want = false, cl_want = false;
+    uint32_t l2_lo = 0, l2_hi = 0, l2_k = 0, cl_rb = 0, cl_re = 0;
+    const uint32_t* cl_col = nullptr;
     uint4 item = make_uint4(0, 0, 0, 0);
     if (i < npush && !hit) {
       const DStep st = pr.steps()[sb + i];
@@ -578,7 +707,37 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
             // memberships than the per-check set holds meets too (batch_l2 reads them from its reverse row);
             // with more than kFCap children its range is walked.
             const uint32_t kb = cst_at(cst, st.tinv), ke = stype == st.tstype ? cst_at(cst, st.tinv + 1u) : kb;
-            if (hi - lo <= static_cast<uint32_t>(kFCap) && (inverted ? ke > kb : stype == st.tstype)) {
+            const uint32_t* crow = nullptr;
+            const uint32_t* ccol = nullptr;
+            uint32_t cn = 0;
+#pragma unroll
+            for (int k = 0; k < kMaxClosure; ++k)  // (by value: the address of a kernel parameter costs a local copy)
+              if (k < static_cast<int>(p.n_closure) && p.closure[k].tgc == st.tgc) {
+                crow = p.closure[k].row_ptr;
+                ccol = p.closure[k].col;
+                cn = p.closure[k].nsubj;
+              }
+            if (crow) {
+              // The pair has a closure index: the union of the memberships' reverse rows is the subject's row of it.
+              // Ranges of up to kFCap children are handed to the whole warp below (closure_meet); a larger one is
+              // intersected with the row by this lane.
+              uint32_t rb = 0, re = 0;
+              if (stype == st.tstype && sid < cn) {
+                rb = __ldg(crow + sid);
+                re = __ldg(crow + sid + 1);
+                if (COUNT) c.bytes += 8;
+              }
+              if (hi - lo <= static_cast<uint32_t>(kFCap)) {
+                cl_want = re > rb;
+                l2_lo = lo;
+                l2_hi = hi;
+                cl_rb = rb;
+                cl_re = re;
+                cl_col = ccol;
+              } else {
+                hit = intersects(p.col, lo, hi, ccol, rb, re, c);
+              }
+            } else if (hi - lo <= static_cast<uint32_t>(kFCap) && (inverted ? ke > kb : stype == st.tstype)) {
               // handed to the whole warp below (batch_l2)
               l2_want = true;
               l2_lo = lo;
@@ -611,6 +770,19 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
       unsigned long long cb = 0;
       c.found |= batch_l2<COUNT>(p.col, p.rrow_ptr, p.rcol, c.rset, c.lane, l2_want && !((c.found >> jslot) & 1u), l2_lo,
                                  l2_hi, l2_k, jslot & 31u, sid, stype, COUNT ? &cb : nullptr);
+      if (COUNT) c.bytes += cb;
+#if ZG_PHASE_CLOCKS
+      c.ph[2] += clock64() - t2;
+#endif
+    }
+    if (MEET2 && __ballot_sync(kFull, cl_want)) {
+#if ZG_PHASE_CLOCKS
+      const long long t2 = clock64();
+#endif
+      unsigned long long cb = 0;
+      c.found |= closure_meet<COUNT>(p.col, cl_col, reinterpret_cast<unsigned long long*>(c.rset + (kRsetCap + kStateWords) * 32),
+                                     c.lane, cl_want && !((c.found >> jslot) & 1u), l2_lo, l2_hi, cl_rb, cl_re, jslot & 31u,
+                                     COUNT ? &cb : nullptr);
       if (COUNT) c.bytes += cb;
 #if ZG_PHASE_CLOCKS
       c.ph[2] += clock64() - t2;
