@@ -341,9 +341,13 @@ int zg_handle_lookup_counters(zg_engine *e, uint64_t *out);
  * out[5] device microseconds of the last publish's index builds, out[6] builds that failed (that pair then meets
  * without an index until its next build). */
 int zg_closure_index_counters(zg_engine *e, uint64_t *out);
+/* Closure index `pair` (0-based, in the order of the program's two-level steps) of the published snapshot: out[0] 1 when
+ * it is built, out[1] its entry width in bytes (2 when every id of its target type fits 16 bits, else 4; the same for
+ * every pair of a snapshot), out[2] entries, out[3] device bytes. ZG_EINVAL when there is no such pair. */
+int zg_closure_index_info(zg_engine *e, uint32_t pair, uint64_t *out);
 /* Copies closure index `pair` (0-based, in the order of the program's two-level steps) of the published snapshot:
- * *n_rows + 1 row offsets to row_ptr, *n_entries entries to col. ZG_E2BIG (sizes filled) when a buffer is too small,
- * ZG_EINVAL when the pair has no index. For inspection and tests. */
+ * *n_rows + 1 row offsets to row_ptr, *n_entries entries to col (32-bit whatever the index's width). ZG_E2BIG (sizes
+ * filled) when a buffer is too small, ZG_EINVAL when the pair has no index. For inspection and tests. */
 int zg_closure_index_copy(zg_engine *e, uint32_t pair, uint32_t *row_ptr, uint64_t row_cap, uint32_t *col,
                           uint64_t col_cap, uint64_t *n_rows, uint64_t *n_entries);
 

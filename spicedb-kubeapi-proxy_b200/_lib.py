@@ -178,6 +178,7 @@ _SIGS = {
     "zg_lookup_subjects_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
     "zg_handle_lookup_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
     "zg_closure_index_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "zg_closure_index_info": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p]),
     "zg_closure_index_copy": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
                                         C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "zg_resolve_checks_packed_device": (C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]),
@@ -694,6 +695,12 @@ class Engine:
         out = np.zeros(len(self.CLOSURE_INDEX_COUNTERS), dtype=np.uint64)
         self._ck(self._L.zg_closure_index_counters(self._h, out.ctypes.data))
         return {k: int(v) for k, v in zip(self.CLOSURE_INDEX_COUNTERS, out)}
+
+    def closure_index_info(self, pair: int = 0) -> dict:
+        """Built flag, entry width in bytes, entries and device bytes of closure index `pair` (zg_closure_index_info)."""
+        out = np.zeros(4, dtype=np.uint64)
+        self._ck(self._L.zg_closure_index_info(self._h, pair, out.ctypes.data))
+        return {k: int(v) for k, v in zip(("built", "width", "entries", "device_bytes"), out)}
 
     def closure_index(self, pair: int = 0):
         """(row_ptr, col) of closure index `pair` of the published snapshot (zg_closure_index_copy)."""

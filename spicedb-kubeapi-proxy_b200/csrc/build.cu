@@ -177,16 +177,18 @@ __global__ void closure_fill_kernel(const uint32_t* rrow_ptr, const uint32_t* rc
   }
 }
 
-// distinct entries of each sorted row: counted into ucnt[u + 1] (out == nullptr), or written to out[row_ptr[u] ..]
+// distinct entries of each sorted row: counted into ucnt[u + 1] (out == nullptr), or written to out[row_ptr[u] ..] at
+// the index's width (T = uint16_t: every entry is below 65 536)
+template <class T>
 __global__ void closure_unique_kernel(const uint32_t* sorted, const unsigned long long* off, uint32_t n, uint32_t* ucnt,
-                                      const uint32_t* row_ptr, uint32_t* out) {
+                                      const uint32_t* row_ptr, T* out) {
   const uint32_t u = blockIdx.x * blockDim.x + threadIdx.x;
   if (u >= n) return;
   const unsigned long long lo = off[u], hi = off[u + 1];
   uint32_t k = 0, at = out ? row_ptr[u] : 0u;
   for (unsigned long long x = lo; x < hi; ++x) {
     if (x > lo && sorted[x] == sorted[x - 1]) continue;
-    if (out) out[at + k] = sorted[x];
+    if (out) out[at + k] = static_cast<T>(sorted[x]);
     ++k;
   }
   if (!out) ucnt[u + 1] = k;
@@ -228,10 +230,12 @@ std::string gpu_build_closure(const Snapshot& s, const DCls& a, const DCls& b, u
   const uint64_t total = hb[0], rels = hb[1];
   // Size budget, checked on the exact count before anything is allocated: the entries before duplicates are removed
   // (sorted twice) must stay within kClosureRatio x the relationships of the two classes, a quarter of the free device
-  // memory, and what one cub sort takes (2^31 keys). `cap` (ZGPU_CLOSURE_CAP) replaces the ratio.
+  // memory (two 32-bit sort buffers and the index at its width per entry), and what one cub sort takes (2^31 keys).
+  // `cap` (ZGPU_CLOSURE_CAP) replaces the ratio.
   size_t free_b = 0, total_b = 0;
   BCUDA(cudaMemGetInfo(&free_b, &total_b));
-  const uint64_t limit = std::min<uint64_t>({cap != ~0ull ? cap : kClosureRatio * rels, free_b / 4 / 12, (1ull << 31) - 1});
+  const uint64_t limit =
+      std::min<uint64_t>({cap != ~0ull ? cap : kClosureRatio * rels, free_b / 4 / (8 + c->width), (1ull << 31) - 1});
   if (total > limit) {  // no index: the pair's steps keep batch_l2
     c->row_ptr.release();
     c->col.release();
@@ -252,7 +256,7 @@ std::string gpu_build_closure(const Snapshot& s, const DCls& a, const DCls& b, u
   uint32_t* crow = c->row_ptr.as<uint32_t>();
   BCUDA(cudaMemsetAsync(crow, 0, (size_t(a.nsubj) + 1) * 4, st));
   const unsigned ug = (a.nsubj + blk - 1) / blk;
-  if (total) closure_unique_kernel<<<ug, blk, 0, st>>>(d_keys[1].as<uint32_t>(), off, a.nsubj, crow, nullptr, nullptr);
+  if (total) closure_unique_kernel<uint32_t><<<ug, blk, 0, st>>>(d_keys[1].as<uint32_t>(), off, a.nsubj, crow, nullptr, nullptr);
   tb = 0;
   cub::DeviceScan::InclusiveSum(nullptr, tb, crow, crow, a.nsubj + 1, st);
   if (!d_tmp.ensure(tb + 256)) return "out of device memory (closure index)";
@@ -261,10 +265,15 @@ std::string gpu_build_closure(const Snapshot& s, const DCls& a, const DCls& b, u
   uint32_t nu = 0;
   BCUDA(cudaMemcpyAsync(&nu, crow + a.nsubj, 4, cudaMemcpyDeviceToHost, st));
   BCUDA(cudaStreamSynchronize(st));
-  // + 4 words: the aligned 16-byte block that holds a row's last entry ends inside the allocation
-  if (!c->col.ensure((size_t(nu) + 4) * 4)) return "out of device memory (closure index)";
-  BCUDA(cudaMemsetAsync(c->col.p, 0, (size_t(nu) + 4) * 4, st));
-  if (total) closure_unique_kernel<<<ug, blk, 0, st>>>(d_keys[1].as<uint32_t>(), off, a.nsubj, nullptr, crow, c->col.as<uint32_t>());
+  // + 4 words, or + 16 16-bit entries: the aligned 16-byte block (32-byte sector) that holds a row's last entry ends
+  // inside the allocation
+  const size_t col_bytes = (size_t(nu) + (c->width == 2 ? 16 : 4)) * c->width;
+  if (!c->col.ensure(col_bytes)) return "out of device memory (closure index)";
+  BCUDA(cudaMemsetAsync(c->col.p, 0, col_bytes, st));
+  if (total && c->width == 2)
+    closure_unique_kernel<<<ug, blk, 0, st>>>(d_keys[1].as<uint32_t>(), off, a.nsubj, nullptr, crow, c->col.as<uint16_t>());
+  else if (total)
+    closure_unique_kernel<<<ug, blk, 0, st>>>(d_keys[1].as<uint32_t>(), off, a.nsubj, nullptr, crow, c->col.as<uint32_t>());
   BCUDA(cudaStreamSynchronize(st));
   BCUDA(cudaGetLastError());
   c->entries = nu;

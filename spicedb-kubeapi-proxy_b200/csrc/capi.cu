@@ -2347,8 +2347,25 @@ extern "C" int zg_closure_index_copy(zg_engine* e, uint32_t pair, uint32_t* row_
   cudaError_t ce = cudaSetDevice(e->dev.device);
   if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->dev.stream);
   if (ce == cudaSuccess) ce = cudaMemcpy(row_ptr, x.row_ptr.p, (uint64_t(x.nsubj) + 1) * 4, cudaMemcpyDeviceToHost);
-  if (ce == cudaSuccess && x.entries) ce = cudaMemcpy(col, x.col.p, x.entries * 4, cudaMemcpyDeviceToHost);
+  if (ce == cudaSuccess && x.entries) ce = cudaMemcpy(col, x.col.p, x.entries * x.width, cudaMemcpyDeviceToHost);
+  if (ce == cudaSuccess && x.width == 2) {
+    // widened in place from the back: entry i (bytes 2i ..) is read before word i (bytes 4i ..) is written
+    const uint16_t* narrow = reinterpret_cast<const uint16_t*>(col);
+    for (uint64_t i = x.entries; i-- > 0;) col[i] = narrow[i];
+  }
   return ce == cudaSuccess ? ZG_OK : fail(ZG_ECUDA, std::string("zg_closure_index_copy: ") + cudaGetErrorString(ce));
+}
+
+extern "C" int zg_closure_index_info(zg_engine* e, uint32_t pair, uint64_t* out) {
+  if (!e || !out) return fail(ZG_EINVAL, "NULL argument");
+  LOCK_DEVICE(e);
+  const auto s = e->dev.snap;
+  if (!s) return fail(ZG_ENOSNAPSHOT, "no snapshot published (call zg_publish)");
+  if (pair >= s->closure.size()) return fail(ZG_EINVAL, "no two-level pair with this number");
+  const auto& x = s->closure[pair];
+  const uint64_t c[4] = {x.built ? 1u : 0u, x.built ? x.width : 0u, x.entries, x.built ? x.row_ptr.cap + x.col.cap : 0u};
+  std::memcpy(out, c, sizeof c);
+  return ZG_OK;
 }
 
 extern "C" int zg_handle_lookup_counters(zg_engine* e, uint64_t* out) {

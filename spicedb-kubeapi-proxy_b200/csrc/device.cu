@@ -273,7 +273,7 @@ std::string Device::publish_delta(const Store& store, const Schema& sc, uint64_t
       const int k = sc.class_of(j.t.rel, j.t.stype, j.t.srel);
       if (k >= 0) touched[lay.rels[sc.slots[j.t.rel].rel_index].cls_begin + k] = 1;
     }
-    build_closures(s.get(), lay.cls, &touched);
+    build_closures(s.get(), lay, &touched);
   }
   cudaEventRecord(e1, stream);
   cudaEventRecord(last_done_, stream);
@@ -305,10 +305,17 @@ std::string Device::publish_delta(const Store& store, const Schema& sc, uint64_t
   return finish_publish(s, lay, sc, revision);
 }
 
-void Device::build_closures(Snapshot* s, const std::vector<DCls>& cls, const std::vector<uint8_t>* rebuild) {
+void Device::build_closures(Snapshot* s, const HostSnapshot& h, const std::vector<uint8_t>* rebuild) {
+  const std::vector<DCls>& cls = h.cls;
+  // One width for the whole snapshot, so that a kernel instantiation inlines one meet. Object ids of a type stay below
+  // its capacity, and a write that grows a capacity lays the snapshot out again (a full publish).
+  uint8_t width = 2;
+  for (const auto& c : s->closure)
+    if (h.n_objects[cls[c.tgc].rtype] > 65536u) width = 4;
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   for (auto& c : s->closure) {
-    if (rebuild ? !((*rebuild)[c.inner] || (*rebuild)[c.tgc]) : c.done) continue;
+    if (c.width == width && (rebuild ? !((*rebuild)[c.inner] || (*rebuild)[c.tgc]) : c.done)) continue;
+    c.width = width;
     if (!e0) {
       cudaEventCreate(&e0);
       cudaEventCreate(&e1);
@@ -431,7 +438,7 @@ std::string Device::finish_publish(std::shared_ptr<Snapshot> s, const HostSnapsh
       c.col.release();
     }
     s->closure = std::move(pairs);
-    build_closures(s.get(), h.cls, nullptr);
+    build_closures(s.get(), h, nullptr);
   }
   s->revision = revision;
 
@@ -446,12 +453,10 @@ std::string Device::finish_publish(std::shared_ptr<Snapshot> s, const HostSnapsh
     size_t& attr_bytes = attr_by_device[device & 63];
     std::lock_guard<std::mutex> g(attr_mu);
     if (sm > attr_bytes) {
-      cudaFuncSetAttribute(check_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sm));
-      cudaFuncSetAttribute(check_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sm));
-      cudaFuncSetAttribute(check_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sm));
-      cudaFuncSetAttribute(check_kernel<false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sm));
-      cudaFuncSetAttribute(check_kernel<true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sm));
-      cudaFuncSetAttribute(check_kernel<false, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sm));
+      for (auto k : {check_kernel<false>, check_kernel<true>, check_kernel<false, true>, check_kernel<false, false, kMeetNone>,
+                     check_kernel<true, false, kMeetNone>, check_kernel<false, true, kMeetNone>, check_kernel<false, false, kMeet16>,
+                     check_kernel<true, false, kMeet16>, check_kernel<false, true, kMeet16>})
+        cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sm));
       attr_bytes = sm;
     }
   }
@@ -511,18 +516,27 @@ int Device::run_pass(const Snapshot& s, const zg_check* queries, uint64_t nq, ui
   p.shard_count = shard_count;
   p.shard_rank = shard_rank;
   p.no_wildcards = no_wildcards_ ? 1 : 0;
+  int meet = s.has_l2 ? kMeet32 : kMeetNone;
   for (const auto& c : s.closure)
-    if (c.built) p.closure[p.n_closure++] = ClosureRef{c.row_ptr.as<uint32_t>(), c.col.as<uint32_t>(), c.nsubj, c.tgc};
+    if (c.built) {
+      p.closure[p.n_closure++] = ClosureRef{c.row_ptr.as<uint32_t>(), c.col.p, c.nsubj, c.tgc, c.width};
+      if (c.width == 2) meet = kMeet16;  // every built index of a snapshot has the same width
+    }
   ZG_CUDA(cudaMemsetAsync(ctrl, 0, 16, st));  // next, subq_count
   const int per_sm = count ? blocks_per_sm_count_ : blocks_per_sm_;
   uint64_t want = (nq + kThreads - 1) / kThreads;
   int grid = static_cast<int>(std::min<uint64_t>(want, static_cast<uint64_t>(sm_count_) * per_sm));
   if (grid < 1) grid = 1;
   size_t sm = smem_bytes(s.prog_bytes);
-  // a schema without a two-level step runs the kernel built without the two-level meet
-  if (count) (s.has_l2 ? check_kernel<true> : check_kernel<true, false, false>)<<<grid, kThreads, sm, st>>>(p);
-  else if (ready) (s.has_l2 ? check_kernel<false, true> : check_kernel<false, true, false>)<<<grid, kThreads, sm, st>>>(p);
-  else (s.has_l2 ? check_kernel<false> : check_kernel<false, false, false>)<<<grid, kThreads, sm, st>>>(p);
+  // a schema without a two-level step runs the kernel built without the two-level meet; one with 16-bit closure
+  // indexes the kernel whose meet reads them
+  auto pick = [meet](auto none, auto m32, auto m16) { return meet == kMeetNone ? none : meet == kMeet16 ? m16 : m32; };
+  if (count)
+    pick(check_kernel<true, false, kMeetNone>, check_kernel<true>, check_kernel<true, false, kMeet16>)<<<grid, kThreads, sm, st>>>(p);
+  else if (ready)
+    pick(check_kernel<false, true, kMeetNone>, check_kernel<false, true>, check_kernel<false, true, kMeet16>)<<<grid, kThreads, sm, st>>>(p);
+  else
+    pick(check_kernel<false, false, kMeetNone>, check_kernel<false>, check_kernel<false, false, kMeet16>)<<<grid, kThreads, sm, st>>>(p);
   ZG_CUDA(cudaGetLastError());
   ++launches;
   return ZG_OK;

@@ -57,6 +57,7 @@ struct Snapshot {
     DevBuf row_ptr, col;
     uint32_t nsubj = 0;
     uint64_t entries = 0;
+    uint8_t width = 0;   // bytes per entry, 2 or 4: one width for every pair of the snapshot (build_closures)
     bool done = false;   // the budget was checked against this snapshot's relationships
     bool built = false;  // ... and the index built
   };
@@ -308,9 +309,11 @@ class Device {
  private:
   uint64_t closure_cap_ = ~0ull;  // ZGPU_CLOSURE_CAP: entries a closure index may hold (tests; ~0 = the size budget)
   // (Re)builds the closure index of every pair of s->closure that is not built yet (`rebuild` false) or whose inner or
-  // tgc class is marked in `rebuild` (a write changed it), from the classes' reverse rows described by cls. A pair whose
-  // build fails is left without an index (closure_failures).
-  void build_closures(Snapshot* s, const std::vector<DCls>& cls, const std::vector<uint8_t>* rebuild);
+  // tgc class is marked in `rebuild` (a write changed it), from the classes' reverse rows described by h.cls. Decides
+  // the entry width from h's object capacities first: 16-bit when every pair's tgc resource type holds at most 65 536
+  // objects, else 32-bit, and rebuilds every pair built at another width. A pair whose build fails is left without an
+  // index (closure_failures).
+  void build_closures(Snapshot* s, const HostSnapshot& h, const std::vector<uint8_t>* rebuild);
   int ingress_sync(const Store& store, cudaStream_t st, std::string* err);
   std::string finish_publish(std::shared_ptr<Snapshot> s, const HostSnapshot& lay, const Schema& sc, uint64_t revision);
   // One check_kernel launch over `nq` queries: val (may be null) receives the per-(query, leaf) value
@@ -407,8 +410,9 @@ std::string gpu_resource_lists(Snapshot* s, cudaStream_t st);
 // Size budget of a closure index: entries (before duplicates are removed) per relationship of its two classes. cfg3's
 // shape (8 memberships per user, 10 teams per group) needs about 9.
 constexpr uint64_t kClosureRatio = 16;
-// Builds the closure index of the pair (a, b) from the resident reverse CSR of s into *c, unless it would hold more
-// than cap entries (~0: the budget above) or more than a quarter of the free device memory; c->built tells which.
+// Builds the closure index of the pair (a, b) from the resident reverse CSR of s into *c with entries of c->width bytes
+// (2 only when every resource id of class b is below 65 536), unless it would hold more than cap entries (~0: the
+// budget above) or more than a quarter of the free device memory; c->built tells which.
 std::string gpu_build_closure(const Snapshot& s, const DCls& a, const DCls& b, uint64_t cap, Snapshot::Closure* c,
                               cudaStream_t st);
 

@@ -70,7 +70,9 @@ constexpr uint8_t kValT = 1, kValE = 2;
 // Closure index of one two-level pair (DESIGN.md §4), built at publish (build.cu gpu_build_closure): for the
 // kStepTargetL2 steps of class tgc, row u = col[row_ptr[u], row_ptr[u + 1]) lists, ascending and distinct, every object
 // the subject u reaches through one of its memberships g: the union of g's reverse rows in class tgc. col is padded so
-// that the aligned 16-byte block holding a row's last word lies inside the allocation.
+// that the aligned 16-byte block holding a row's last word lies inside the allocation. The entries are 16-bit when
+// every object id of class tgc's resource type is below 65 536 in every pair of the snapshot, else 32-bit (width, in
+// bytes); 16-bit rows are padded so that the aligned 32-byte sector holding a row's last entry lies inside it.
 constexpr int kMaxClosure = 4;
 #ifndef ZG_CLOSURE_BLOCKS
 #define ZG_CLOSURE_BLOCKS 2
@@ -82,10 +84,15 @@ constexpr int kClosureBlocks = ZG_CLOSURE_BLOCKS;  // 16-byte blocks in flight p
 constexpr int kClosureVerify = ZG_CLOSURE_VERIFY;  // pending "maybe"s of a warp that trigger their searches
 struct ClosureRef {
   const uint32_t* row_ptr;
-  const uint32_t* col;
-  uint32_t nsubj;  // rows (subjects of the innermost direct class)
-  uint32_t tgc;
+  const void* col;  // entries of `width` bytes
+  uint32_t nsubj;   // rows (subjects of the innermost direct class)
+  uint16_t tgc;
+  uint16_t width;   // 2 or 4; a kernel instantiated for one width reads only the indexes of that width
 };
+// check_kernel's MEET argument: no two-level step in the schema, or the width of the closure entries it reads
+constexpr int kMeetNone = 0, kMeet16 = 2, kMeet32 = 4;
+template <int MEET> struct ClosureEntry { using type = uint32_t; };
+template <> struct ClosureEntry<kMeet16> { using type = uint16_t; };
 
 struct KParams {
   const uint32_t* row_ptr;
@@ -242,13 +249,13 @@ __device__ __forceinline__ void push(WarpCtx<COUNT>& c, bool want, const uint4& 
 }
 
 // Binary search of the sorted segment arr[lo, hi) for key.
-template <bool COUNT>
-__device__ __forceinline__ bool find_in(const uint32_t* __restrict__ arr, WarpCtx<COUNT>& c, uint32_t lo, uint32_t hi,
+template <bool COUNT, class T>
+__device__ __forceinline__ bool find_in(const T* __restrict__ arr, WarpCtx<COUNT>& c, uint32_t lo, uint32_t hi,
                                         uint32_t key, uint32_t* at = nullptr) {
   while (lo < hi) {
     const uint32_t mid = lo + ((hi - lo) >> 1);
     const uint32_t v = __ldg(arr + mid);
-    if (COUNT) c.bytes += 4;
+    if (COUNT) c.bytes += sizeof(T);
     if (v == key) {
       if (at) *at = mid;
       return true;
@@ -297,15 +304,15 @@ __device__ __forceinline__ void probe2(const uint32_t* __restrict__ arr, WarpCtx
 // Do the sorted segments a[a0, a1) and b[b0, b1) share an element? Sizes within 4x of each other:
 // two-pointer merge (one load per step); otherwise every element of the short one is searched in
 // the long one.
-template <bool COUNT>
+template <bool COUNT, class B>
 __device__ __forceinline__ bool intersects(const uint32_t* __restrict__ a, uint32_t a0, uint32_t a1,
-                                           const uint32_t* __restrict__ b, uint32_t b0, uint32_t b1, WarpCtx<COUNT>& c) {
+                                           const B* __restrict__ b, uint32_t b0, uint32_t b1, WarpCtx<COUNT>& c) {
   const uint32_t na = a1 - a0, nb = b1 - b0;
   if (na == 0 || nb == 0) return false;
   if (na > 4u * nb) {
     for (uint32_t x = b0; x < b1; ++x) {
       const uint32_t k = __ldg(b + x);
-      if (COUNT) c.bytes += 4;
+      if (COUNT) c.bytes += sizeof(B);
       if (find_in(a, c, a0, a1, k)) return true;
     }
     return false;
@@ -319,17 +326,18 @@ __device__ __forceinline__ bool intersects(const uint32_t* __restrict__ a, uint3
     return false;
   }
   uint32_t va = __ldg(a + a0), vb = __ldg(b + b0);
-  if (COUNT) c.bytes += 8;
+  if (COUNT) c.bytes += 4 + sizeof(B);
   for (;;) {
     if (va == vb) return true;
     if (va < vb) {
       if (++a0 == a1) return false;
       va = __ldg(a + a0);
+      if (COUNT) c.bytes += 4;
     } else {
       if (++b0 == b1) return false;
       vb = __ldg(b + b0);
+      if (COUNT) c.bytes += sizeof(B);
     }
-    if (COUNT) c.bytes += 4;
   }
 }
 
@@ -486,23 +494,30 @@ __device__ __forceinline__ unsigned batch_l2(const uint32_t* __restrict__ col, c
 }
 
 // Two-level meet over a closure index, batched like batch_l2: lane j wants "does its range col[lo, hi) list an element
-// of its subject's closure row ccol[rb, re)" (rb < re). The rows of the requesting lanes are cut into aligned 16-byte
-// blocks, numbered with one scan and dealt out 32 at a time, so neighbouring lanes read neighbouring blocks of a row and
-// no load waits for another. Each word of a block that lies inside its row is tested against the owner's 128-bit filter
-// of the range; a "maybe" is verified by a binary search of the range. Blocks of a check already answered are skipped.
-// fw: kMeetWords words of shared memory per warp. Returns the job slots answered.
-template <bool COUNT>
-__device__ __forceinline__ unsigned closure_meet(const uint32_t* __restrict__ col, const uint32_t* ccol, unsigned long long* fw,
+// of its subject's closure row ccol[rb, re)" (rb < re). The rows of the requesting lanes are cut into aligned units --
+// 16-byte blocks of 32-bit entries, kClosureBlocks per lane per round, or 32-byte sectors of 16-bit entries, one per
+// lane per round (two 16-byte loads: the same registers in flight, four times the entries) -- numbered with one scan
+// and dealt out 32 at a time, so neighbouring lanes read neighbouring units of a row and no load waits for another. Each
+// entry of a unit that lies inside its row is tested against the owner's 128-bit filter of the range; a "maybe" is
+// verified by a binary search of the range. Units of a check already answered are skipped. The COUNT variant counts
+// sizeof(E) bytes per entry of a row streamed. fw: kMeetWords words of shared memory per warp. Returns the job slots
+// answered.
+template <bool COUNT, class E>
+__device__ __forceinline__ unsigned closure_meet(const uint32_t* __restrict__ col, const E* ccol, unsigned long long* fw,
                                                  uint32_t lane, bool want, uint32_t lo, uint32_t hi, uint32_t rb, uint32_t re,
                                                  uint32_t jslot, unsigned long long* bytes) {
+  constexpr bool kNarrow = sizeof(E) == 2;
+  constexpr uint32_t kPer = kNarrow ? 16u : 4u;        // entries per unit
+  constexpr int kVec = kNarrow ? 2 : 1;                // 16-byte loads per unit
+  constexpr int kUnits = kNarrow ? 1 : kClosureBlocks;  // units per lane per round
   unsigned long long nb = 0;
   unsigned long long f0 = 0, f1 = 0;
   uint32_t b0 = 0, cnt = 0;
   if (want) {
     l2_filter(col, lo, hi, f0, f1);
     if (COUNT) nb += 4ull * (hi - lo);
-    b0 = rb >> 2;
-    cnt = ((re - 1) >> 2) + 1 - b0;
+    b0 = rb / kPer;
+    cnt = (re - 1) / kPer + 1 - b0;
   }
   fw[lane] = f0;
   fw[32 + lane] = f1;
@@ -513,22 +528,22 @@ __device__ __forceinline__ unsigned closure_meet(const uint32_t* __restrict__ co
     if (static_cast<int>(lane) >= d) incl += v;
   }
   const uint32_t total = __shfl_sync(kFull, incl, 31);
-  const uint32_t db = b0 - (incl - cnt);  // this lane's block p is block p + db of ccol
+  const uint32_t db = b0 - (incl - cnt);  // this lane's unit p is unit p + db of ccol
   const unsigned long long cp = reinterpret_cast<unsigned long long>(ccol);
   __syncwarp();
   unsigned hits = 0;
-  // This lane's pending "maybe": a word the filter of owner pj let through, not verified yet (pj < 0: none). The
+  // This lane's pending "maybe": an entry the filter of owner pj let through, not verified yet (pj < 0: none). The
   // searches are deferred and run for the whole warp at once: verified one by one, nearly every round had a lane whose
   // search the warp waited for.
   int pj = -1;
   uint32_t pv = 0;
-  for (uint32_t base = 0; base < total; base += 32u * kClosureBlocks) {
-    uint4 q[kClosureBlocks];
-    int jj[kClosureBlocks];  // owner lane of each block loaded, -1: none
+  for (uint32_t base = 0; base < total; base += 32u * kUnits) {
+    uint4 q[kUnits][kVec];
+    int jj[kUnits];  // owner lane of each unit loaded, -1: none
 #pragma unroll
-    for (int k = 0; k < kClosureBlocks; ++k) {
+    for (int k = 0; k < kUnits; ++k) {
       const uint32_t p = base + 32u * k + lane;
-      int j = 0;  // owner lane of block p: # lanes with incl <= p
+      int j = 0;  // owner lane of unit p: # lanes with incl <= p
 #pragma unroll
       for (int step = 16; step >= 1; step >>= 1) {
         const int probe_lane = j + step - 1;
@@ -538,38 +553,66 @@ __device__ __forceinline__ unsigned closure_meet(const uint32_t* __restrict__ co
       const uint32_t jdb = __shfl_sync(kFull, db, j & 31), js = __shfl_sync(kFull, jslot, j & 31);
       const uint4* const jcol = reinterpret_cast<const uint4*>(__shfl_sync(kFull, cp, j & 31));
       jj[k] = -1;
-      q[k] = make_uint4(0, 0, 0, 0);
+#pragma unroll
+      for (int h = 0; h < kVec; ++h) q[k][h] = make_uint4(0, 0, 0, 0);
       if (p < total && !((hits >> js) & 1u)) {
         jj[k] = j;
-        q[k] = __ldg(jcol + (p + jdb));  // all blocks of the round in flight together (p + jdb wraps in 32 bits)
+        // all loads of the round in flight together (p + jdb wraps in 32 bits)
+#pragma unroll
+        for (int h = 0; h < kVec; ++h) q[k][h] = __ldg(jcol + (p + jdb) * kVec + h);
       }
     }
     unsigned mine = 0;  // job slots this lane answered in this round
 #pragma unroll
-    for (int k = 0; k < kClosureBlocks; ++k) {
+    for (int k = 0; k < kUnits; ++k) {
       const int j = jj[k];
       const uint32_t src = j < 0 ? 0u : static_cast<uint32_t>(j);
       const uint32_t jdb = __shfl_sync(kFull, db, src), js = __shfl_sync(kFull, jslot, src);
       const uint32_t jrb = __shfl_sync(kFull, rb, src), jre = __shfl_sync(kFull, re, src);
       const uint32_t jlo = __shfl_sync(kFull, lo, src), jhi = __shfl_sync(kFull, hi, src);
       if (j < 0) continue;
-      const uint32_t w0 = (base + 32u * k + lane + jdb) * 4u;
-      const uint32_t v[4] = {q[k].x, q[k].y, q[k].z, q[k].w};
-      if (COUNT) nb += 4ull * (min(jre, w0 + 4u) - max(jrb, w0));
+      const uint32_t w0 = (base + 32u * k + lane + jdb) * kPer;
+      if (COUNT) nb += sizeof(E) * static_cast<unsigned long long>(min(jre, w0 + kPer) - max(jrb, w0));
       const unsigned long long g0 = fw[j], g1 = fw[32 + j];
+      if constexpr (!kNarrow) {
+        const uint32_t v[4] = {q[k][0].x, q[k][0].y, q[k][0].z, q[k][0].w};
 #pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        if (w0 + i < jrb || w0 + i >= jre || ((mine >> js) & 1u) || !l2_maybe(g0, g1, v[i])) continue;
-        if (pj < 0) {
-          pj = j;
-          pv = v[i];
-        } else if (l2_verify<COUNT>(col, jlo, jhi, v[i], nb)) {  // the slot is taken: verify this one now
-          mine |= 1u << js;
+        for (int i = 0; i < 4; ++i) {
+          if (w0 + i < jrb || w0 + i >= jre || ((mine >> js) & 1u) || !l2_maybe(g0, g1, v[i])) continue;
+          if (pj < 0) {
+            pj = j;
+            pv = v[i];
+          } else if (l2_verify<COUNT>(col, jlo, jhi, v[i], nb)) {  // the slot is taken: verify this one now
+            mine |= 1u << js;
+          }
+        }
+      } else {
+        // 16 entries, two per word (entry 2t in the low half of word t): the filter is tested on all of them first,
+        // and only the "maybe"s inside the row reach the one search below (rare: ~2 % of the entries on cfg3)
+        const uint32_t w[8] = {q[k][0].x, q[k][0].y, q[k][0].z, q[k][0].w, q[k][1].x, q[k][1].y, q[k][1].z, q[k][1].w};
+        uint32_t m = 0;
+#pragma unroll
+        for (int i = 0; i < 16; ++i) m |= l2_maybe(g0, g1, (w[i >> 1] >> (16 * (i & 1))) & 0xFFFFu) ? 1u << i : 0u;
+        const uint32_t first = jrb > w0 ? jrb - w0 : 0u, end = min(jre - w0, kPer);  // the row's entries of the sector
+        m &= ((1u << end) - 1u) & ~((1u << first) - 1u);
+        while (m && !((mine >> js) & 1u)) {
+          const int i = __ffs(m) - 1;
+          m &= m - 1;
+          uint32_t wi = w[0];
+#pragma unroll
+          for (int t = 1; t < 8; ++t) wi = (i >> 1) == t ? w[t] : wi;
+          const uint32_t v = (wi >> (16 * (i & 1))) & 0xFFFFu;
+          if (pj < 0) {
+            pj = j;
+            pv = v;
+          } else if (l2_verify<COUNT>(col, jlo, jhi, v, nb)) {  // the slot is taken: verify this one now
+            mine |= 1u << js;
+          }
         }
       }
     }
     const unsigned pend = __ballot_sync(kFull, pj >= 0);
-    if (__popc(pend) >= kClosureVerify || (pend && base + 32u * kClosureBlocks >= total)) {
+    if (__popc(pend) >= kClosureVerify || (pend && base + 32u * kUnits >= total)) {
       const uint32_t src = pj < 0 ? 0u : static_cast<uint32_t>(pj);
       const uint32_t plo = __shfl_sync(kFull, lo, src), phi = __shfl_sync(kFull, hi, src);
       const uint32_t ps = __shfl_sync(kFull, jslot, src);
@@ -585,9 +628,10 @@ __device__ __forceinline__ unsigned closure_meet(const uint32_t* __restrict__ co
 // Warp-collective node visit: every lane may carry one (job slot, object, unit).
 // Evaluates the unit's steps at the object: membership-of-itself test, direct and
 // wildcard probes (from the subject's reverse-row set when the job is inverted, else a
-// binary search of the row), and pushes the userset / arrow edge ranges. MEET2 = false: the schema has no two-level
-// step, and the two-level meet is left out (its code costs the traversal loop registers: cfg4, DESIGN.md §6).
-template <bool COUNT, bool MEET2>
+// binary search of the row), and pushes the userset / arrow edge ranges. MEET = kMeetNone: the schema has no two-level
+// step, and the two-level meet is left out (its code costs the traversal loop registers: cfg4, DESIGN.md §6); else the
+// width of the closure entries the meet reads (kMeet16 / kMeet32: one closure_meet is inlined per instantiation).
+template <bool COUNT, int MEET>
 __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<COUNT>& c, bool active,
                                       uint32_t jslot, uint32_t obj, uint32_t unit, uint32_t depth) {
   const uint32_t sid = __shfl_sync(kFull, c.my_subj, jslot & 31);
@@ -645,9 +689,10 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
   // ---- edge classes that may push a range (userset subjects, arrows): warp-collective
   const int maxsteps = __reduce_max_sync(kFull, npush);
   for (int i = 0; i < maxsteps; ++i) {
+    using CE = typename ClosureEntry<MEET>::type;
     bool want = false, l2_want = false, cl_want = false;
     uint32_t l2_lo = 0, l2_hi = 0, l2_k = 0, cl_rb = 0, cl_re = 0;
-    const uint32_t* cl_col = nullptr;
+    const CE* cl_col = nullptr;
     uint4 item = make_uint4(0, 0, 0, 0);
     if (i < npush && !hit) {
       const DStep st = pr.steps()[sb + i];
@@ -656,6 +701,27 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
         const unsigned long long ridx = st.row_base + static_cast<unsigned long long>(obj) * st.ncls;
         const uint32_t lo = __ldg(p.row_ptr + ridx), hi = __ldg(p.row_ptr + ridx + 1);
         if (COUNT) c.bytes += 8;
+        // A two-level step whose pair has a closure index reads the subject's row of it: its offsets depend on the
+        // subject alone, so they are loaded together with the range's instead of after them.
+        const CE* ccol = nullptr;
+        uint32_t rb = 0, re = 0;
+        bool crow_read = false;  // (counted where the offsets are used)
+        if (MEET != kMeetNone && (st.flags & kStepTargetL2) && meets && depth + 2 <= ZG_MAX_DEPTH) {
+          const uint32_t* crow = nullptr;
+          uint32_t cn = 0;
+#pragma unroll
+          for (int k = 0; k < kMaxClosure; ++k)  // (by value: the address of a kernel parameter costs a local copy)
+            if (k < static_cast<int>(p.n_closure) && p.closure[k].tgc == st.tgc && p.closure[k].width == sizeof(CE)) {
+              crow = p.closure[k].row_ptr;
+              ccol = static_cast<const CE*>(p.closure[k].col);
+              cn = p.closure[k].nsubj;
+            }
+          if (crow && stype == st.tstype && sid < cn) {
+            rb = __ldg(crow + sid);
+            re = __ldg(crow + sid + 1);
+            crow_read = true;
+          }
+        }
         if (hi > lo) {
           if ((st.flags & kStepTargetLeaf) && inverted && !expiry && depth + 1 <= ZG_MAX_DEPTH) {
             // Children of this range can only be answered by "is the child one of the
@@ -697,7 +763,7 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
               l1_cycles += clock64() - t1;
 #endif
             }
-          } else if (MEET2 && (st.flags & kStepTargetL2) && meets && depth + 2 <= ZG_MAX_DEPTH &&
+          } else if (MEET != kMeetNone && (st.flags & kStepTargetL2) && meets && depth + 2 <= ZG_MAX_DEPTH &&
                      (inverted || hi - lo <= static_cast<uint32_t>(kFCap))) {
             // Two levels at once (namespace -> team#member -> group#member -> user): a child t of this
             // range matches iff some membership g of the subject (class tinv) is a subject of t in the
@@ -707,26 +773,11 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
             // memberships than the per-check set holds meets too (batch_l2 reads them from its reverse row);
             // with more than kFCap children its range is walked.
             const uint32_t kb = cst_at(cst, st.tinv), ke = stype == st.tstype ? cst_at(cst, st.tinv + 1u) : kb;
-            const uint32_t* crow = nullptr;
-            const uint32_t* ccol = nullptr;
-            uint32_t cn = 0;
-#pragma unroll
-            for (int k = 0; k < kMaxClosure; ++k)  // (by value: the address of a kernel parameter costs a local copy)
-              if (k < static_cast<int>(p.n_closure) && p.closure[k].tgc == st.tgc) {
-                crow = p.closure[k].row_ptr;
-                ccol = p.closure[k].col;
-                cn = p.closure[k].nsubj;
-              }
-            if (crow) {
+            if (ccol) {
               // The pair has a closure index: the union of the memberships' reverse rows is the subject's row of it.
               // Ranges of up to kFCap children are handed to the whole warp below (closure_meet); a larger one is
               // intersected with the row by this lane.
-              uint32_t rb = 0, re = 0;
-              if (stype == st.tstype && sid < cn) {
-                rb = __ldg(crow + sid);
-                re = __ldg(crow + sid + 1);
-                if (COUNT) c.bytes += 8;
-              }
+              if (COUNT && crow_read) c.bytes += 8;
               if (hi - lo <= static_cast<uint32_t>(kFCap)) {
                 cl_want = re > rb;
                 l2_lo = lo;
@@ -763,7 +814,7 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
         }
       }
     }
-    if (MEET2 && __ballot_sync(kFull, l2_want)) {
+    if (MEET != kMeetNone && __ballot_sync(kFull, l2_want)) {
 #if ZG_PHASE_CLOCKS
       const long long t2 = clock64();
 #endif
@@ -775,7 +826,7 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
       c.ph[2] += clock64() - t2;
 #endif
     }
-    if (MEET2 && __ballot_sync(kFull, cl_want)) {
+    if (MEET != kMeetNone && __ballot_sync(kFull, cl_want)) {
 #if ZG_PHASE_CLOCKS
       const long long t2 = clock64();
 #endif
@@ -854,7 +905,7 @@ __device__ __noinline__ void wait_ready(const unsigned long long* ready, unsigne
 // Per-lane query state parked in shared memory while the warp traverses (kStateWords words):
 //   0 resource object, 1 depth | leaves << 8 | is-tree << 15 | leaf_begin-or-unit << 16,
 //   2 tree id, 3 / 4 leaf values (2 bits each)
-template <bool COUNT, bool STREAMED = false, bool MEET2 = true>
+template <bool COUNT, bool STREAMED = false, int MEET = kMeet32>
 __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KParams p) {
   ZG_DYNAMIC_SMEM(smem);
   for (uint32_t i = threadIdx.x; i < p.prog_bytes / 16; i += blockDim.x)
@@ -1002,7 +1053,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
 #if ZG_PHASE_CLOCKS
       long long t_ph = clock64(), meets = c.ph[2] + c.ph[3];  // root visit and pop loop exclude the meets inside them
 #endif
-      visit<COUNT, MEET2>(p, pr, c, act, lane, obj, unit, depth);
+      visit<COUNT, MEET>(p, pr, c, act, lane, obj, unit, depth);
 #if ZG_PHASE_CLOCKS
       {
         const long long now = clock64(), m = c.ph[2] + c.ph[3];
@@ -1124,7 +1175,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
           }
         }
         c.raised |= __reduce_or_sync(kFull, raise ? (1u << jslot) : 0u);
-        visit<COUNT, MEET2>(p, pr, c, active, jslot, child, cunit, cdepth);
+        visit<COUNT, MEET>(p, pr, c, active, jslot, child, cunit, cdepth);
       }
 #if ZG_PHASE_CLOCKS
       c.ph[4] += (clock64() - t_ph) - (c.ph[2] + c.ph[3] - meets);
