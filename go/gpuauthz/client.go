@@ -58,9 +58,10 @@ type Client struct {
 	// then fails (pkg/authz/authz.go:93-97 turns an error into a denial) instead of answering from a
 	// store that may still hold revoked grants.
 	broken atomic.Bool
-	// sharded: the engine is a sharded handle (Shards), which answers checks and writes but refuses
-	// LookupSubjects, and LookupResources unless HandleLookups is set; what it refuses goes to the embedded SpiceDB
-	sharded, handleLookups bool
+	// sharded: the engine is a sharded handle (Shards), which answers checks and writes but refuses LookupResources
+	// unless HandleLookups is set, and LookupSubjects unless HandleSubjects is set; what it refuses goes to the
+	// embedded SpiceDB
+	sharded, handleLookups, handleSubjects bool
 }
 
 // AllDevices: every visible GPU from `device` on (zg_config.n_devices).
@@ -72,16 +73,25 @@ type Option func(*C.zg_config)
 // Shards makes the one engine hold the n shards of an object-hash sharded store (zg_config.n_shards): shard k keeps
 // the relationships whose resource id % n == k and lives on device `device + k % nDevices` (with nDevices = 1, the n
 // shards share one GPU). For stores larger than one GPU. Checks and writes are answered by the engine;
-// LookupResources and LookupSubjects are delegated to the embedded SpiceDB.
+// LookupResources and LookupSubjects are delegated to the embedded SpiceDB unless HandleLookups / HandleSubjects
+// is set.
 func Shards(n uint32) Option {
 	return func(cfg *C.zg_config) { cfg.n_shards = C.uint32_t(n) }
 }
 
 // HandleLookups, with Shards, makes the sharded engine answer LookupResources and PrefilterListResponse itself
 // (ZG_FLAG_HANDLE_LOOKUPS): the reverse walk runs on every shard and the answers equal a replica's, so a store larger
-// than one GPU serves pre-filtered lists without a second engine. LookupSubjects stays delegated.
+// than one GPU serves pre-filtered lists without a second engine. LookupSubjects stays delegated unless
+// HandleSubjects is set too.
 func HandleLookups() Option {
 	return func(cfg *C.zg_config) { cfg.flags |= C.ZG_FLAG_HANDLE_LOOKUPS }
+}
+
+// HandleSubjects, with Shards, makes the sharded engine answer LookupSubjects itself (ZG_FLAG_HANDLE_SUBJECTS): the
+// forward walk runs on every shard, each discovery sent to its owner, and the answers equal a replica's. Independent
+// of HandleLookups.
+func HandleSubjects() Option {
+	return func(cfg *C.zg_config) { cfg.flags |= C.ZG_FLAG_HANDLE_SUBJECTS }
 }
 
 var errBroken = status.Error(codes.Unavailable, "gpu mirror is out of sync with SpiceDB and could not be rebuilt")
@@ -102,7 +112,7 @@ func New(ctx context.Context, inner v1.PermissionsServiceClient, schema string, 
 		return nil, err // fail closed: no CPU fallback inside the library
 	}
 	c := &Client{PermissionsServiceClient: inner, engine: eng, sharded: cfg.n_shards > 1,
-		handleLookups: cfg.flags&C.ZG_FLAG_HANDLE_LOOKUPS != 0}
+		handleLookups: cfg.flags&C.ZG_FLAG_HANDLE_LOOKUPS != 0, handleSubjects: cfg.flags&C.ZG_FLAG_HANDLE_SUBJECTS != 0}
 	cs := C.CString(schema)
 	defer C.free(unsafe.Pointer(cs))
 	if err := call(func() C.int { return C.zg_load_schema(eng, cs, C.size_t(len(schema))) }); err != nil {
@@ -319,10 +329,11 @@ func (s *sliceStream) RecvMsg(any) error            { return io.EOF }
 // LookupSubjects: "which subjects of a type have the permission on this resource" (who-can / audit). No proxy
 // call site issues it (it is in the client mock of pkg/authz/postfilter_test.go:71). A request with caveat
 // context, a concrete limit or a cursor goes to the wrapped SpiceDB: the library answers whole, uncaveated
-// lookups only. The concrete subjects come first, then -- when a wildcard grants the permission and the
-// request includes wildcards -- "*" with its excluded subjects. Like the rest of this file: never compiled.
+// lookups only, and a sharded engine only with HandleSubjects. The concrete subjects come first, then -- when a
+// wildcard grants the permission and the request includes wildcards -- "*" with its excluded subjects. Like the
+// rest of this file: never compiled.
 func (c *Client) LookupSubjects(ctx context.Context, req *v1.LookupSubjectsRequest, opts ...grpc.CallOption) (v1.PermissionsService_LookupSubjectsClient, error) {
-	if c.sharded || req.GetContext() != nil || req.GetOptionalConcreteLimit() != 0 || req.GetOptionalCursor() != nil {
+	if (c.sharded && !c.handleSubjects) || req.GetContext() != nil || req.GetOptionalConcreteLimit() != 0 || req.GetOptionalCursor() != nil {
 		return c.PermissionsServiceClient.LookupSubjects(ctx, req, opts...)
 	}
 	if c.broken.Load() {

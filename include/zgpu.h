@@ -77,6 +77,12 @@ typedef struct zg_engine zg_engine;
  * through peer memory, and its candidates are verified by the handle's check protocol (zg_handle_lookup_counters).
  * The answers equal a replica's. On any other engine, zg_engine_create returns ZG_EINVAL. */
 #define ZG_FLAG_HANDLE_LOOKUPS 4u
+/* Sharded handle (n_shards > 1) only, independent of ZG_FLAG_HANDLE_LOOKUPS: the handle answers zg_lookup_subjects and
+ * zg_lookup_subjects_str itself, one lookup per call. Its forward walk runs on every shard, each discovery written into
+ * its owner's inbox through peer memory; the candidates are verified by the handle's check protocol, the second
+ * (no-wildcards) verification too (zg_handle_subjects_counters). The answers equal a replica's. On any other engine,
+ * zg_engine_create returns ZG_EINVAL. */
+#define ZG_FLAG_HANDLE_SUBJECTS 8u
 
 typedef struct {
   int32_t device;            /* CUDA device ordinal; -1 = current device          */
@@ -99,7 +105,8 @@ typedef struct {
                                 peer memory; every device pair must have peer access. Not with shard_count > 1;
                                 S <= 64. LookupResources / LookupSubjects / the list pre-filter, zg_check_bulk_device,
                                 the device-ingress calls and the zg_shard_*_dev calls are refused (ZG_EINVAL);
-                                with ZG_FLAG_HANDLE_LOOKUPS, LookupResources and the list pre-filter are answered. */
+                                with ZG_FLAG_HANDLE_LOOKUPS, LookupResources and the list pre-filter are answered,
+                                with ZG_FLAG_HANDLE_SUBJECTS, LookupSubjects. */
 } zg_config;
 #define ZG_ALL_DEVICES 0xFFFFFFFFu
 
@@ -312,8 +319,11 @@ int zg_lookup_resources_str(zg_engine *e, const char *res_type, const char *perm
  * (every object of stype when the walk overflows), verified by the check kernel. Returns 0; ZG_E2BIG
  * with *n_out / *n_excluded = required sizes; ZG_EDEPTH when a subject cannot be decided (depth cap /
  * work budget); ZG_EINVAL for unknown ids; ZG_ECUDA on a host-only engine. A sharded engine refuses this
- * call and the string form (ZG_EINVAL): use the zg_shard_subjects_*_dev calls (dist.DeviceShardedLookup).
- * A resource id that no relationship names gives an empty answer. No caveats, limits or cursors. */
+ * call and the string form (ZG_EINVAL): use the zg_shard_subjects_*_dev calls (dist.DeviceShardedLookup). So does a
+ * sharded handle (zg_config.n_shards > 1), unless it was created with ZG_FLAG_HANDLE_SUBJECTS: it then answers both
+ * forms as a replica holding the same relationships does, the walk overflowing ZGPU_LOOKUP_BATCH_CAP straight into
+ * verifying every object of the subject type. A resource id that no relationship names gives an empty answer. No
+ * caveats, limits or cursors. */
 #define ZG_WILDCARDS_INCLUDE 0u /* v1.LookupSubjectsRequest WILDCARD_OPTION_UNSPECIFIED / INCLUDE_WILDCARDS */
 #define ZG_WILDCARDS_EXCLUDE 1u /* v1.LookupSubjectsRequest WILDCARD_OPTION_EXCLUDE_WILDCARDS               */
 int zg_lookup_subjects(zg_engine *e, uint16_t perm, uint32_t res, uint16_t stype, uint16_t srel,
@@ -335,6 +345,12 @@ int zg_lookup_subjects_counters(zg_engine *e, uint64_t *out);
  * overflowed ZGPU_LOOKUP_BATCH_CAP), out[6] rounds that verified every resource of the type (a single lookup that
  * overflowed, or ZGPU_NO_RBFS=1). */
 int zg_handle_lookup_counters(zg_engine *e, uint64_t *out);
+/* Cumulative LookupSubjects counters of a sharded handle with ZG_FLAG_HANDLE_SUBJECTS (zeros on any other engine):
+ * out[0] lookups, out[1] walk levels expanded, out[2] times the host waited for the shards (both verifications'
+ * included), out[3] walk entries written to another shard's inbox, out[4] candidates verified, out[5] items of the
+ * no-wildcards verification, out[6] lookups that verified every object of the subject type (the walk overflowed
+ * ZGPU_LOOKUP_BATCH_CAP, or ZGPU_NO_RBFS=1). */
+int zg_handle_subjects_counters(zg_engine *e, uint64_t *out);
 /* Closure indexes of the two-level steps in the engine's published snapshot (zg_stats keeps its layout): out[0] pairs
  * indexed, out[1] pairs over the size budget (their steps meet through the memberships' reverse rows instead), out[2]
  * index entries, out[3] index device bytes; out[4] index builds since creation (the rebuilds after writes included),

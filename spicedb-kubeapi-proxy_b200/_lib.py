@@ -177,6 +177,7 @@ _SIGS = {
                                          C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint64)]),
     "zg_lookup_subjects_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
     "zg_handle_lookup_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "zg_handle_subjects_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
     "zg_closure_index_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
     "zg_closure_index_info": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p]),
     "zg_closure_index_copy": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
@@ -335,13 +336,15 @@ class Engine:
 
     def __init__(self, schema: str | None = None, device: int = -1, subquery_capacity: int = 0, work_budget: int = 0,
                  host_only: bool = False, forward_only: bool = False, shard_rank: int = 0, shard_count: int = 0,
-                 n_devices: int = 0, n_shards: int = 0, handle_lookups: bool = False):
+                 n_devices: int = 0, n_shards: int = 0, handle_lookups: bool = False, handle_subjects: bool = False):
         """host_only=True builds schema/store/snapshot without a GPU (CPU unit tests of
         the host logic); every check/lookup on such an engine raises ZgpuError. n_shards=S > 1: this one handle
         holds the S shards of an object-hash sharded store (zg_config.n_shards); handle_lookups=True
-        (ZG_FLAG_HANDLE_LOOKUPS) makes it answer LookupResources and the list pre-filter too."""
+        (ZG_FLAG_HANDLE_LOOKUPS) makes it answer LookupResources and the list pre-filter too, handle_subjects=True
+        (ZG_FLAG_HANDLE_SUBJECTS) LookupSubjects."""
         self._L = lib()
-        flags = (1 if host_only else 0) | (2 if forward_only else 0) | (4 if handle_lookups else 0)
+        flags = ((1 if host_only else 0) | (2 if forward_only else 0) | (4 if handle_lookups else 0)
+                 | (8 if handle_subjects else 0))
         cfg = _Config(device, flags, subquery_capacity, work_budget, shard_rank, shard_count, n_devices & 0xFFFFFFFF,
                       n_shards)
         h = C.c_void_p()
@@ -720,6 +723,15 @@ class Engine:
         out = np.zeros(len(self.HANDLE_LOOKUP_COUNTERS), dtype=np.uint64)
         self._ck(self._L.zg_handle_lookup_counters(self._h, out.ctypes.data))
         return {k: int(v) for k, v in zip(self.HANDLE_LOOKUP_COUNTERS, out)}
+
+    HANDLE_SUBJECTS_COUNTERS = ("lookups", "levels", "host_waits", "inbox_entries", "candidates", "nowild_items",
+                                "fallbacks")
+
+    def handle_subjects_counters(self) -> dict:
+        """Cumulative LookupSubjects counters of a sharded handle with handle_subjects (zg_handle_subjects_counters)."""
+        out = np.zeros(len(self.HANDLE_SUBJECTS_COUNTERS), dtype=np.uint64)
+        self._ck(self._L.zg_handle_subjects_counters(self._h, out.ctypes.data))
+        return {k: int(v) for k, v in zip(self.HANDLE_SUBJECTS_COUNTERS, out)}
 
     # -- sharded store (dist.DeviceShardedChecker drives these) --------------------
     # every pointer is a device address on this engine's GPU (ints, e.g. tensor.data_ptr())

@@ -194,6 +194,9 @@ struct zg_engine {
   bool handle_lookups = false;
   uint64_t hl_rounds = 0, hl_levels = 0, hl_round_trips = 0, hl_frontier = 0, hl_candidates = 0, hl_halvings = 0,
            hl_fallbacks = 0;
+  // ZG_FLAG_HANDLE_SUBJECTS: run_sharded_subjects answers LookupSubjects; zg_handle_subjects_counters
+  bool handle_subjects = false;
+  uint64_t hs_lookups = 0, hs_levels = 0, hs_waits = 0, hs_entries = 0, hs_candidates = 0, hs_nowild = 0, hs_fallbacks = 0;
   std::vector<HostSnapshot> shard_built;  // zg_debug_shard_row: the host builder's arrays per shard
   ~zg_engine() {
     if (group_pin) cudaFreeHost(group_pin);
@@ -253,6 +256,8 @@ static const char* kHandleSubjectsMsg =
     "sharded handle (zg_config.n_shards > 1): LookupSubjects is not served by it, with or without "
     "ZG_FLAG_HANDLE_LOOKUPS; run it on one engine per shard (dist.DeviceShardedLookup) or on a replica";
 static bool is_handle(const zg_engine* e) { return e->n_shards > 1; }
+// a sharded handle that answers LookupSubjects itself (run_sharded_subjects)
+static bool serves_subjects(const zg_engine* e) { return is_handle(e) && e->handle_subjects; }
 // why a sharded engine refuses LookupSubjects
 static const char* subjects_refusal(const zg_engine* e) {
   return !is_handle(e) ? kShardedMsg : e->handle_lookups ? kHandleSubjectsMsg : kHandleLookupMsg;
@@ -290,10 +295,13 @@ extern "C" int zg_engine_create(const zg_config* cfg, zg_engine** out) {
   if (S > static_cast<uint32_t>(kMaxShards)) return fail(ZG_EINVAL, "n_shards exceeds 64 (the routing kernels' destinations)");
   const bool handle_lookups = cfg && (cfg->flags & ZG_FLAG_HANDLE_LOOKUPS);
   if (handle_lookups && S < 2) return fail(ZG_EINVAL, "ZG_FLAG_HANDLE_LOOKUPS needs n_shards > 1");
+  const bool handle_subjects = cfg && (cfg->flags & ZG_FLAG_HANDLE_SUBJECTS);
+  if (handle_subjects && S < 2) return fail(ZG_EINVAL, "ZG_FLAG_HANDLE_SUBJECTS needs n_shards > 1");
   zg_engine* e = new (std::nothrow) zg_engine();
   if (!e) return fail(ZG_ENOMEM, "out of memory");
   e->n_shards = S;
   e->handle_lookups = handle_lookups;
+  e->handle_subjects = handle_subjects;
   if (cfg && (cfg->flags & ZG_FLAG_HOST_ONLY)) {
     e->host_only = true;
     e->keep_built = true;
@@ -933,8 +941,10 @@ struct ShardLists {
 // owners. Per level, every shard writes its queries straight into the owners' inboxes (where, the host computes from
 // every shard's counts: the level's one round trip), each owner's pass starts when the shards delivering to it are
 // done (events, not host waits), and the values are folded back level by level where their owners left them.
-// *overflow: a pass raised more sub-queries than its buffer holds; nothing is answered.
-static int sharded_levels(zg_engine* e, const ShardLists& L, PeerCounts* pc, bool* overflow_out, std::string* err) {
+// *overflow: a pass raised more sub-queries than its buffer holds; nothing is answered. no_wildcards: every pass of
+// every shard, the sub-queries' included, sees no wildcard relationship (LookupSubjects' second verification).
+static int sharded_levels(zg_engine* e, const ShardLists& L, PeerCounts* pc, bool no_wildcards, bool* overflow_out,
+                          std::string* err) {
   const uint32_t S = e->n_shards;
   *overflow_out = false;
   std::vector<uint64_t> counts(size_t(S) * S, 0);  // [k * S + d]: queries shard k sends to shard d this level
@@ -979,7 +989,7 @@ static int sharded_levels(zg_engine* e, const ShardLists& L, PeerCounts* pc, boo
     events(level);
     on_all_devices(e, [&](Device& dev, size_t k) {
       bool o = false;
-      rcs[k] = dev.peer_pass(level, wait, &nsub[k], &counts[k * S], &o, &errs[k]);
+      rcs[k] = dev.peer_pass(level, wait, &nsub[k], &counts[k * S], &o, no_wildcards, &errs[k]);
       overflow[k] = o;
     });
     ++pc->round_trips;
@@ -1013,9 +1023,9 @@ static int sharded_levels(zg_engine* e, const ShardLists& L, PeerCounts* pc, boo
 
 // sharded_levels, and on overflow the same in halves (checks are independent): the first half of the items taken in
 // shard order, then the rest. Where an item starts does not change where it is evaluated (at its owner).
-static int run_sharded_lists(zg_engine* e, const ShardLists& L, PeerCounts* pc, std::string* err) {
+static int run_sharded_lists(zg_engine* e, const ShardLists& L, PeerCounts* pc, bool no_wildcards, std::string* err) {
   bool overflow = false;
-  if (int rc = sharded_levels(e, L, pc, &overflow, err)) return rc;
+  if (int rc = sharded_levels(e, L, pc, no_wildcards, &overflow, err)) return rc;
   if (!overflow) return ZG_OK;
   uint64_t n = 0;
   for (uint64_t m : L.n) n += m;
@@ -1033,8 +1043,8 @@ static int run_sharded_lists(zg_engine* e, const ShardLists& L, PeerCounts* pc, 
     b.items[k] += a.n[k];
     b.out[k] += a.n[k];
   }
-  if (int rc = run_sharded_lists(e, a, pc, err)) return rc;
-  return run_sharded_lists(e, b, pc, err);
+  if (int rc = run_sharded_lists(e, a, pc, no_wildcards, err)) return rc;
+  return run_sharded_lists(e, b, pc, no_wildcards, err);
 }
 
 // n checks in host memory (out: their codes): shard k brings the slice dist.shard_bounds gives it.
@@ -1047,7 +1057,7 @@ static int run_sharded(zg_engine* e, const zg_check* items, uint64_t n, uint8_t*
     L.n.push_back(lo(k + 1) - lo(k));
     L.out.push_back(out + lo(k));
   }
-  return run_sharded_lists(e, L, pc, err);
+  return run_sharded_lists(e, L, pc, false, err);
 }
 
 // Runs one group of queued requests; the caller holds the device lock.
@@ -1856,7 +1866,7 @@ static int run_sharded_lookup(zg_engine* e, const std::vector<Device::LookupReq>
     e->hl_candidates += nc[k];
   }
   PeerCounts pc;
-  int vrc = run_sharded_lists(e, V, &pc, err);
+  int vrc = run_sharded_lists(e, V, &pc, false, err);
   e->hl_round_trips += pc.round_trips;
   if (vrc) return fail_round(vrc);
   // ---- the answer keys, gathered, sorted and split on shard 0
@@ -2200,9 +2210,228 @@ extern "C" int zg_lookup_resources_str(zg_engine* e, const char* res_type, const
 }
 
 // ---- LookupSubjects --------------------------------------------------------------------------
+
+// LookupSubjects on a sharded handle (ZG_FLAG_HANDLE_SUBJECTS): one round of dist.DeviceShardedLookup's
+// _subjects_round with one lookup (home 0), driven in this process; every call runs its own round on every shard.
+// Shard k holds the forward rows of the objects it owns, but the subjects in them can be owned by any shard, so each
+// discovery goes to its owner, which admits it once per lookup (the owner of req.res seeds the walk and holds the
+// probe). Per level, every shard expands its own frontier into its outbox and counts the outbox by owner on the device;
+// the host reads every shard's overflow flag and counts (the level's first wait), lays out every owner's inbox from
+// them, and every shard writes its outbox straight into the owners' inboxes (peer memory). Each owner admits what
+// arrived once every shard's scatter of the level is done (events); its admitted count sizes its next expand (the
+// second wait). Levels 0 .. ZG_MAX_DEPTH + 1 are expanded, as on a replica, and one more count reports the last
+// admissions' overflow. An overflow goes straight to the exhaustive candidates: a single lookup is not halved. The
+// candidates are verified where they lie by the handle's check protocol; the probe verdicts of the shards are OR-ed
+// on the host (the handle is every rank); when the wildcard is granted, the HAS candidates are verified again with
+// no wildcard relationship visible on any pass of any shard; the answer keys are gathered, sorted and split on shard 0.
 //
+// Why no buffer is overwritten before it is read. (1) A shard's outbox is read only by its own scatter, on its own
+// stream, and only its next expand, later on that stream, overwrites it. (2) Shard d's inbox (hl.inbox) is written by
+// every shard's scatter of level L and read by d's admit of level L, which waits on every shard's scatter event of
+// level L (peer_wait). No scatter of level L + 1 is issued before the host has waited for every admit of level L (the
+// admitted counts), so one inbox per shard is enough; the inbox is grown only while every shard is idle. (3) A shard's
+// frontier (hl.front[0]) is read by its expand and rewritten by its admit, in that order on its stream. The answer
+// keys follow (1) and (2) with shard 0 as the one destination. The walk buffers and hl are shared with the handle's
+// LookupResources round (run_sharded_lookup); both run under the device lock, so they never interleave.
+static int run_sharded_subjects(zg_engine* e, const Device::SubjectsReq& req, bool include, Device::SubjectsAnswer* ans,
+                                std::string* err) {
+  *ans = Device::SubjectsAnswer{};
+  const uint32_t S = e->n_shards;
+  const std::vector<Device::SubjectsReq> round{req};
+  const uint8_t home = 0;
+  const uint64_t cap = e->dev.lookup_walk_cap();
+  std::vector<int> src(S, ZG_OK);
+  std::vector<std::string> errs(S);
+  auto first_error = [&]() { return ::first_error(src, errs, err); };
+  auto end_round = [](Device& dev, std::string* e2) {
+    uint64_t listed = 0, excluded = 0;
+    return dev.shard_subjects_finish(nullptr, 0, nullptr, &listed, &excluded, e2);
+  };
+  // a failed round is ended on every shard, so that no shard keeps its snapshot resident
+  auto fail_round = [&](int rc) {
+    on_all_devices(e, [&](Device& dev, size_t) { end_round(dev, nullptr); });
+    return rc;
+  };
+  ++e->hs_lookups;
+  std::vector<uint64_t> n_front(S, 0);
+  on_all_devices(e, [&](Device& dev, size_t k) {
+    src[k] = !dev.hl_ensure(dev.hl.front[0], cap * 8)
+                 ? ZG_ENOMEM
+                 : dev.shard_subjects_begin(round, &home, include ? 1 : 0, cap, dev.hl.front[0].as<unsigned long long>(),
+                                            &n_front[k], &errs[k]);
+    if (src[k] == ZG_ENOMEM && errs[k].empty()) errs[k] = "out of device memory (sharded handle subjects frontier)";
+  });
+  ++e->hs_waits;
+  if (int rc = first_error()) return fail_round(rc);
+  // ---- the walk
+  const bool exhaustive = !e->dev.use_rbfs;  // ZGPU_NO_RBFS=1: every owned object of the subject type is a candidate
+  bool overflow = false;
+  std::vector<uint64_t> counts(size_t(S) * S, 0), arrived(S, 0);
+  std::vector<char> ovf(S);
+  std::vector<PeerTable> tab(S);
+  std::vector<cudaEvent_t> wait(S);
+  for (int level = 0; !exhaustive; ++level) {
+    const bool expand = level <= ZG_MAX_DEPTH + 1;
+    on_all_devices(e, [&](Device& dev, size_t k) {
+      bool o = false;
+      src[k] = dev.shard_subjects_expand_count(dev.hl.front[0].as<unsigned long long>(), expand ? n_front[k] : 0,
+                                               &counts[k * S], &o, &errs[k]);
+      ovf[k] = o;
+    });
+    ++e->hs_waits;
+    if (int rc = first_error()) return fail_round(rc);
+    if ((overflow = std::find(ovf.begin(), ovf.end(), 1) != ovf.end())) break;
+    if (!expand || std::all_of(n_front.begin(), n_front.end(), [](uint64_t n) { return n == 0; })) break;
+    ++e->hs_levels;
+    for (uint32_t d = 0; d < S; ++d) {
+      uint64_t at = 0;
+      for (uint32_t k = 0; k < S; ++k) {
+        tab[k].base[d] = at;
+        at += counts[size_t(k) * S + d];
+        if (k != d) e->hs_entries += counts[size_t(k) * S + d];
+      }
+      arrived[d] = at;
+      Device& dev = shard(e, d);
+      if (!dev.hl_ensure(dev.hl.inbox, at * 8)) {
+        *err = "out of device memory (sharded handle subjects inbox)";
+        return fail_round(ZG_ENOMEM);
+      }
+      for (uint32_t k = 0; k < S; ++k) tab[k].p[d] = dev.hl.inbox.p;
+    }
+    on_all_devices(e, [&](Device& dev, size_t k) {
+      uint64_t n = 0;
+      for (uint32_t d = 0; d < S; ++d) n += counts[k * S + d];
+      src[k] = dev.shard_subjects_scatter(n, tab[k], level, &errs[k]);
+    });
+    if (int rc = first_error()) return fail_round(rc);
+    for (uint32_t k = 0; k < S; ++k) wait[k] = shard(e, k).peer_event(level);
+    on_all_devices(e, [&](Device& dev, size_t k) {
+      src[k] = dev.peer_wait(wait, &errs[k]);
+      if (!src[k])
+        src[k] = dev.shard_subjects_admit(dev.hl.inbox.as<unsigned long long>(), arrived[k],
+                                          dev.hl.front[0].as<unsigned long long>(), &n_front[k], &errs[k]);
+    });
+    ++e->hs_waits;
+    if (int rc = first_error()) return fail_round(rc);
+  }
+  const bool every = overflow || exhaustive;
+  if (every) ++e->hs_fallbacks;
+  // ---- the first verification, where the candidates lie
+  std::vector<uint64_t> nc(S, 0);
+  on_all_devices(e, [&](Device& dev, size_t k) {
+    uint64_t need = 0;
+    src[k] = dev.shard_subjects_candidates(every, nullptr, 0, &need, &errs[k]);
+    if (!src[k] && (!dev.hl_ensure(dev.hl.items, need * sizeof(zg_check)) || !dev.hl_ensure(dev.hl.codes, need) ||
+                    !dev.hl_ensure(dev.hl.routed, need * 8))) {
+      src[k] = ZG_ENOMEM;
+      errs[k] = "out of device memory (sharded handle subjects candidates)";
+    }
+    if (!src[k]) src[k] = dev.shard_subjects_candidates(every, dev.hl.items.as<zg_check>(), need, &nc[k], &errs[k]);
+  });
+  ++e->hs_waits;
+  if (int rc = first_error()) return fail_round(rc);
+  ShardLists V;
+  for (uint32_t k = 0; k < S; ++k) {
+    V.items.push_back(shard(e, k).hl.items.as<zg_check>());
+    V.n.push_back(nc[k]);
+    V.out.push_back(shard(e, k).hl.codes.as<uint8_t>());
+    e->hs_candidates += nc[k];
+    ans->n_verified += nc[k];
+  }
+  PeerCounts pc;
+  int vrc = run_sharded_lists(e, V, &pc, false, err);
+  e->hs_waits += pc.round_trips;
+  if (vrc) return fail_round(vrc);
+  std::vector<uint64_t> granted(S, 0), failed(S, 0);
+  on_all_devices(e, [&](Device& dev, size_t k) {
+    src[k] = dev.shard_subjects_verdicts(dev.hl.codes.as<uint8_t>(), nc[k], &granted[k], &failed[k], &errs[k]);
+  });
+  ++e->hs_waits;
+  if (int rc = first_error()) return fail_round(rc);
+  uint64_t g = 0, f = 0;  // the probe's verdict is on the resource's owner, a failed candidate anywhere
+  for (uint32_t k = 0; k < S; ++k) {
+    g |= granted[k];
+    f |= failed[k];
+  }
+  if (f & 1) {
+    *err = "LookupSubjects: a subject could not be decided (max dispatch depth / work budget exceeded)";
+    return fail_round(ZG_EDEPTH);
+  }
+  // ---- the keys of the first verification, and the no-wildcards verification of the HAS candidates when granted.
+  // Its items and codes take the place of the first verification's, which shard_subjects_nowild has read (it waits).
+  std::vector<uint64_t> nnw(S, 0);
+  on_all_devices(e, [&](Device& dev, size_t k) {
+    src[k] = dev.shard_subjects_nowild(dev.hl.codes.as<uint8_t>(), nc[k], g, f, dev.hl.items.as<zg_check>(), nc[k], &nnw[k],
+                                       &errs[k]);
+  });
+  ++e->hs_waits;
+  if (int rc = first_error()) return fail_round(rc);
+  if (g & 1) {
+    ShardLists W;
+    for (uint32_t k = 0; k < S; ++k) {
+      W.items.push_back(shard(e, k).hl.items.as<zg_check>());
+      W.n.push_back(nnw[k]);
+      W.out.push_back(shard(e, k).hl.codes.as<uint8_t>());
+      e->hs_nowild += nnw[k];
+    }
+    PeerCounts pw;
+    vrc = run_sharded_lists(e, W, &pw, true, err);
+    e->hs_waits += pw.round_trips;
+    if (vrc) return fail_round(vrc);
+  }
+  // ---- the answer keys, gathered, sorted and split on shard 0 (home 0: every key is routed to destination 0)
+  on_all_devices(e, [&](Device& dev, size_t k) {
+    src[k] = dev.shard_subjects_route(dev.hl.codes.as<uint8_t>(), nnw[k], S, dev.hl.routed.as<unsigned long long>(),
+                                      &counts[k * S], &errs[k]);
+  });
+  ++e->hs_waits;
+  if (int rc = first_error()) return fail_round(rc);
+  uint64_t n_keys = 0;
+  for (uint32_t k = 0; k < S; ++k) {
+    tab[k].base[0] = n_keys;
+    n_keys += counts[size_t(k) * S];
+  }
+  Device& d0 = e->dev;
+  if (!d0.hl_ensure(d0.hl.keys, n_keys * 8) || !d0.hl_ensure(d0.hl.ids, n_keys * 4)) {
+    *err = "out of device memory (sharded handle subjects keys)";
+    return fail_round(ZG_ENOMEM);
+  }
+  for (uint32_t k = 0; k < S; ++k) tab[k].p[0] = d0.hl.keys.p;
+  on_all_devices(e, [&](Device& dev, size_t k) {
+    src[k] = dev.peer_put(dev.hl.routed.as<unsigned long long>(), counts[k * S], 1, tab[k], 0, &errs[k]);
+  });
+  if (int rc = first_error()) return fail_round(rc);
+  for (uint32_t k = 0; k < S; ++k) wait[k] = shard(e, k).peer_event(0);
+  uint64_t listed = 0, excluded = 0;
+  on_all_devices(e, [&](Device& dev, size_t k) {
+    src[k] = k ? end_round(dev, &errs[k]) : dev.peer_wait(wait, &errs[k]);
+    if (!k && !src[k])
+      src[k] = dev.shard_subjects_finish(dev.hl.keys.as<unsigned long long>(), n_keys, dev.hl.ids.as<uint32_t>(), &listed,
+                                         &excluded, &errs[k]);
+  });
+  ++e->hs_waits;
+  if (int rc = first_error()) return fail_round(rc);
+  std::vector<uint32_t> host(listed + excluded);
+  if (!host.empty()) {
+    const cudaError_t ce = cudaSetDevice(d0.device) == cudaSuccess
+                               ? cudaMemcpy(host.data(), d0.hl.ids.p, host.size() * 4, cudaMemcpyDeviceToHost)
+                               : cudaGetLastError();
+    ++e->hs_waits;
+    if (ce != cudaSuccess) {
+      *err = std::string("cudaMemcpy (lookup answers): ") + cudaGetErrorString(ce);
+      return ZG_ECUDA;
+    }
+  }
+  ans->ids.assign(host.begin(), host.begin() + static_cast<long>(listed));
+  ans->wildcard = (g & 1) && include;
+  if (ans->wildcard) ans->excluded.assign(host.begin() + static_cast<long>(listed), host.end());
+  ans->fell_back = every;
+  return ZG_OK;
+}
+
 // Arguments are checked before anything else (a host-only engine still reports ZG_EINVAL for them). The
-// device lock is FIFO, as for a single LookupResources; a multi-device engine answers on its first device.
+// device lock is FIFO, as for a single LookupResources; a multi-device engine answers on its first device, a sharded
+// handle with ZG_FLAG_HANDLE_SUBJECTS on every shard (run_sharded_subjects).
 static int lookup_subjects_ids(zg_engine* e, uint16_t perm, uint32_t res, uint16_t stype, uint16_t srel, uint32_t option,
                                Device::SubjectsAnswer* ans) {
   const Schema& sc = e->schema;
@@ -2211,16 +2440,24 @@ static int lookup_subjects_ids(zg_engine* e, uint16_t perm, uint32_t res, uint16
     return fail(ZG_EINVAL, "unknown subject type or relation");
   if (option != ZG_WILDCARDS_INCLUDE && option != ZG_WILDCARDS_EXCLUDE) return fail(ZG_EINVAL, "unknown wildcard option");
   if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
-  if (e->dev.shard_count > 1) return fail(ZG_EINVAL, subjects_refusal(e));
+  if (e->dev.shard_count > 1 && !serves_subjects(e)) return fail(ZG_EINVAL, subjects_refusal(e));
   LOCK_DEVICE(e);
-  if (e->dirty.load() || !e->dev.snap) {
+  if (e->dirty.load() || !e->dev.snap) {  // a handle's failed publish clears every shard's snapshot
     LOCK_NAMES_UNIQUE(e);
     int rc = publish_locked(e);
     if (rc) return rc;
   }
-  e->dev.now = now_of(e);
+  const uint32_t now = now_of(e);
   std::string err;
-  int rc = e->dev.lookup_subjects(sc.slots[perm].type, res, perm, stype, srel, option == ZG_WILDCARDS_INCLUDE, ans, &err);
+  int rc = ZG_OK;
+  if (serves_subjects(e)) {
+    for (uint32_t k = 0; k < e->n_shards; ++k) shard(e, k).now = now;
+    const Device::SubjectsReq req{res, static_cast<uint16_t>(sc.slots[perm].type), perm, stype, srel};
+    rc = run_sharded_subjects(e, req, option == ZG_WILDCARDS_INCLUDE, ans, &err);
+  } else {
+    e->dev.now = now;
+    rc = e->dev.lookup_subjects(sc.slots[perm].type, res, perm, stype, srel, option == ZG_WILDCARDS_INCLUDE, ans, &err);
+  }
   return rc ? fail(rc, err) : ZG_OK;
 }
 
@@ -2274,7 +2511,7 @@ extern "C" int zg_lookup_subjects_str(zg_engine* e, const char* res_type, const 
     if (wildcard_option != ZG_WILDCARDS_INCLUDE && wildcard_option != ZG_WILDCARDS_EXCLUDE)
       return fail(ZG_EINVAL, "unknown wildcard option");
     if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
-    if (e->dev.shard_count > 1) return fail(ZG_EINVAL, subjects_refusal(e));
+    if (e->dev.shard_count > 1 && !serves_subjects(e)) return fail(ZG_EINVAL, subjects_refusal(e));
   } else {
     rc = lookup_subjects_ids(e, static_cast<uint16_t>(p), res, static_cast<uint16_t>(st), sr, wildcard_option, &ans);
     if (rc) return rc;
@@ -2373,6 +2610,15 @@ extern "C" int zg_handle_lookup_counters(zg_engine* e, uint64_t* out) {
   LOCK_DEVICE(e);
   const uint64_t c[7] = {e->hl_rounds, e->hl_levels, e->hl_round_trips, e->hl_frontier, e->hl_candidates, e->hl_halvings,
                          e->hl_fallbacks};
+  std::memcpy(out, c, sizeof c);
+  return ZG_OK;
+}
+
+extern "C" int zg_handle_subjects_counters(zg_engine* e, uint64_t* out) {
+  if (!e || !out) return fail(ZG_EINVAL, "NULL argument");
+  LOCK_DEVICE(e);
+  const uint64_t c[7] = {e->hs_lookups, e->hs_levels, e->hs_waits, e->hs_entries, e->hs_candidates, e->hs_nowild,
+                         e->hs_fallbacks};
   std::memcpy(out, c, sizeof c);
   return ZG_OK;
 }

@@ -1078,7 +1078,7 @@ int Device::peer_scatter(int level, const PeerTable& t, std::string* err) {
 }
 
 int Device::peer_pass(int level, const std::vector<cudaEvent_t>& wait, uint64_t* n_sub, uint64_t* counts, bool* overflow,
-                      std::string* err) {
+                      bool no_wildcards, std::string* err) {
   for (uint32_t d = 0; d < own_count; ++d) counts[d] = 0;
   *n_sub = 0;
   *overflow = false;
@@ -1107,8 +1107,10 @@ int Device::peer_pass(int level, const std::vector<cudaEvent_t>& wait, uint64_t*
   ZG_CUDA(cudaMemsetAsync(L.val.p, 0, nq * Lv + 4, stream));
   // level 0: the callers' items (flags ignored), v1 codes written straight out (final unless the level raised
   // sub-queries: then peer_fold rewrites them); deeper: routed sub-queries (flags = hop depth), value bits
+  no_wildcards_ = no_wildcards;
   int rc = run_pass(*s, L.in.as<zg_check>(), nq, L.val.as<uint8_t>(), L.out.as<uint8_t>(), level == 0, level == 0,
                     L.raised.as<zg_check>(), L.parent.as<uint32_t>(), stream, false, err);
+  no_wildcards_ = false;
   if (rc) return rc;
   ZG_CUDA(cudaMemsetAsync(d_counts, 0, kMaxShards * sizeof(unsigned long long), stream));
   const unsigned grid = static_cast<unsigned>(std::min<uint64_t>(subq_cap_ / 256 + 1, static_cast<uint64_t>(sm_count_) * 8));
@@ -1615,6 +1617,69 @@ int Device::shard_subjects_expand(const unsigned long long* d_front, uint64_t n_
   if (*overflow) return ZG_OK;
   return route_<false>(static_cast<const unsigned long long*>(ss_out_.as<unsigned long long>()), host[1], n_dest, EntryOwner{},
                        d_routed, static_cast<uint32_t*>(nullptr), counts, err);
+}
+
+int Device::shard_subjects_expand_count(const unsigned long long* d_front, uint64_t n_in, uint64_t* counts, bool* overflow,
+                                        std::string* err) {
+  *overflow = false;
+  for (uint32_t d = 0; d < shard_count && d < kMaxRouteDest; ++d) counts[d] = 0;
+  if (!ss_snap_ || shard_count > kMaxRouteDest || n_in > ss_cap_) {
+    if (err) *err = "shard_subjects_expand_count: no round begun, or a frontier over the walk capacity";
+    return ZG_EINVAL;
+  }
+  ZG_CUDA(cudaSetDevice(device));
+  if (int rc = peer_events_(err)) return rc;
+  if (!pin_peer_) ZG_CUDA(cudaMallocHost(&pin_peer_, (4 + kMaxShards) * sizeof(unsigned long long)));
+  if (!peer_ctrl_.ensure(2 * kMaxShards * sizeof(unsigned long long))) {
+    if (err) *err = "out of device memory (sharded handle buffers)";
+    return ZG_ENOMEM;
+  }
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  unsigned long long* ctrl = ss_ctrl_.as<unsigned long long>();
+  unsigned long long* d_counts = peer_ctrl_.as<unsigned long long>();
+  ZG_CUDA(cudaMemsetAsync(ctrl + 1, 0, 8, stream));
+  ZG_CUDA(cudaMemsetAsync(d_counts, 0, kMaxShards * sizeof(unsigned long long), stream));
+  if (n_in) {
+    SsWalkParams p = ss_walk_params(*ss_snap_, lb_params_.as<SubjectsParam>(), rb_visited_.as<uint32_t>(), ctrl, shard_rank, shard_count);
+    p.in = d_front;
+    p.n_in = n_in;
+    p.out = ss_out_.as<unsigned long long>();
+    p.out_count = ctrl + 1;
+    p.cap = ss_cap_;
+    ss_expand_kernel<<<sm_count_ * 8, 256, 0, stream>>>(p);
+    const unsigned grid = static_cast<unsigned>(std::min<uint64_t>(ss_cap_ / 256 + 1, static_cast<uint64_t>(sm_count_) * 8));
+    peer_entry_count_kernel<<<grid, 256, 0, stream>>>(ss_out_.as<unsigned long long>(), ctrl + 1, ss_cap_, shard_count, d_counts);
+    launches += 2;
+    ZG_CUDA(cudaGetLastError());
+  }
+  ZG_CUDA(cudaMemcpyAsync(pin_peer_, ctrl, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaMemcpyAsync(pin_peer_ + 4, d_counts, shard_count * sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaEventRecord(last_done_, stream));
+  have_last_ = true;
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  // flags are sticky: an admission (or the begin's) that did not fit is reported here
+  *overflow = (static_cast<uint32_t>(pin_peer_[0]) & 16u) != 0;
+  if (*overflow) return ZG_OK;
+  for (uint32_t d = 0; d < shard_count; ++d) counts[d] = pin_peer_[4 + d];
+  return ZG_OK;
+}
+
+int Device::shard_subjects_scatter(uint64_t n, const PeerTable& t, int level, std::string* err) {
+  if (!ss_snap_ || n > ss_cap_) {
+    if (err) *err = "shard_subjects_scatter: no round begun, or an outbox over the walk capacity";
+    return ZG_EINVAL;
+  }
+  ZG_CUDA(cudaSetDevice(device));
+  if (n) {
+    unsigned long long* d_cursor = peer_ctrl_.as<unsigned long long>() + kMaxShards;
+    ZG_CUDA(cudaMemsetAsync(d_cursor, 0, kMaxShards * sizeof(unsigned long long), stream));
+    const unsigned grid = static_cast<unsigned>(std::min<uint64_t>((n + 255) / 256, static_cast<uint64_t>(sm_count_) * 8));
+    peer_entry_scatter_kernel<<<grid, 256, 0, stream>>>(ss_out_.as<unsigned long long>(), n, shard_count, d_cursor, t);
+    ZG_CUDA(cudaGetLastError());
+    ++launches;
+  }
+  ZG_CUDA(cudaEventRecord(peer_event(level), stream));
+  return ZG_OK;
 }
 
 int Device::shard_subjects_admit(const unsigned long long* d_in, uint64_t n_in, unsigned long long* d_next, uint64_t* n_next,

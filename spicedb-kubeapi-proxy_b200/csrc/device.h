@@ -201,9 +201,10 @@ class Device {
   int peer_scatter(int level, const PeerTable& t, std::string* err);
   // After every shard's peer_event(level) (`wait`, one per shard): evaluates the level's queries in one pass and counts
   // the sub-queries it raised by owner: *n_sub, counts[d] (host). Waits for them (a round trip). ZG_ENOMEM with
-  // *overflow: the pass raised more than the sub-query capacity; the batch must be answered in halves.
+  // *overflow: the pass raised more than the sub-query capacity; the batch must be answered in halves. no_wildcards:
+  // the pass runs with KParams::no_wildcards (LookupSubjects' second verification, on every pass of every shard).
   int peer_pass(int level, const std::vector<cudaEvent_t>& wait, uint64_t* n_sub, uint64_t* counts, bool* overflow,
-                std::string* err);
+                bool no_wildcards, std::string* err);
   // When pass `level` raised sub-queries: after every shard's peer_event(level + 1), ORs their values (t.p[d] = shard
   // d's values of level + 1) into the raising leaves and folds the level; records peer_event(level).
   int peer_fold(int level, const PeerTable& t, const std::vector<cudaEvent_t>& wait, std::string* err);
@@ -215,9 +216,11 @@ class Device {
   // LookupResources on a sharded handle (capi.cu run_sharded_lookup drives the shard_lookup_* round above on every
   // shard): the walk's buffers of this shard. front[level & 1] = the replicated frontier `level` expands, next = what
   // this shard's expand found (walk capacity), items / codes = its candidates and their codes, routed = its answer
-  // keys, keys / ids = every shard's keys and the answers (shard 0).
+  // keys, keys / ids = every shard's keys and the answers (shard 0). LookupSubjects on the handle (run_sharded_subjects)
+  // uses front[0] as this shard's frontier, inbox for the walk entries the shards deliver to it, and items / codes /
+  // routed / keys / ids as above. Both rounds run under the handle's device lock, so they never interleave.
   struct HandleLookupBufs {
-    DevBuf front[2], next, items, codes, routed, keys, ids;
+    DevBuf front[2], next, items, codes, routed, keys, ids, inbox;
   } hl;
   bool hl_ensure(DevBuf& b, uint64_t bytes);  // b (one of hl) grown to bytes on this device
   uint64_t lookup_walk_cap() const { return lb_cap_; }
@@ -245,6 +248,15 @@ class Device {
   // or the candidates of the round did not fit (sticky for the round); nothing is routed then.
   int shard_subjects_expand(const unsigned long long* d_front, uint64_t n_in, uint32_t n_dest, unsigned long long* d_routed,
                             uint64_t* counts, bool* overflow, std::string* err);
+  // The sharded handle's expand (capi.cu run_sharded_subjects): expands this shard's frontier into its outbox and counts
+  // the outbox by owner on the device (the outbox size read there), with one wait for the flags and counts[d] (host,
+  // shard_count), where shard_subjects_expand waits and then routes into a local buffer. *overflow as there; the
+  // counts are then zero. The outbox stays put for shard_subjects_scatter.
+  int shard_subjects_expand_count(const unsigned long long* d_front, uint64_t n_in, uint64_t* counts, bool* overflow,
+                                  std::string* err);
+  // Writes the n entries of the outbox into their owners' inboxes at t.p[d] + t.base[d] + ... (peer memory), then
+  // records peer_event(level). No wait.
+  int shard_subjects_scatter(uint64_t n, const PeerTable& t, int level, std::string* err);
   // Admits the n_in entries that arrived from every rank: the fresh ones are the next frontier (d_next, walk_cap).
   int shard_subjects_admit(const unsigned long long* d_in, uint64_t n_in, unsigned long long* d_next, uint64_t* n_next,
                            std::string* err);

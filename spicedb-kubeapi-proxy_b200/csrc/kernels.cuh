@@ -1318,34 +1318,48 @@ __global__ void unroute_kernel(const uint32_t* src, const uint8_t* val, unsigned
 // every lower shard (t.base[d], from all shards' counts), and a value is read where its owner left it: no copy
 // call, no staging, no reverse exchange. The table of the destinations' buffers (t.p[d]) is a kernel argument.
 
-// route_count_kernel over the sub-queries a pass raised, their number read on the device (*n_dev, at most cap): the
-// counts come back with the pass's control words in the level's one round trip
-__global__ void __launch_bounds__(256) peer_count_kernel(const zg_check* items, const unsigned long long* n_dev,
-                                                         unsigned long long cap, uint32_t n_dest, unsigned long long* counts) {
+// The count and the scatter are written once over the item type and its owner: the check protocol's sub-queries
+// (zg_check, ResOwner) here, LookupSubjects' walk entries (8 bytes, EntryOwner) in peer_entry_*_kernel below.
+// route_count_kernel over the items a step wrote, their number read on the device (*n_dev, at most cap): the counts
+// come back with the step's control words in the level's one round trip
+template <class Item, class Owner>
+__device__ __forceinline__ void peer_count_items(const Item* items, const unsigned long long* n_dev, unsigned long long cap,
+                                                 uint32_t n_dest, unsigned long long* counts, Owner owner) {
   ZG_BLOCK_SHARED_U32(hist, kMaxRouteDest);
   for (uint32_t i = threadIdx.x; i < n_dest; i += blockDim.x) hist[i] = 0;
   __syncthreads();
   const unsigned long long n = min(*n_dev, cap);
   const unsigned long long stride = static_cast<unsigned long long>(gridDim.x) * blockDim.x;
   for (unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x; i < n; i += stride)
-    atomicAdd(&hist[ResOwner{}(items[i], n_dest)], 1u);
+    atomicAdd(&hist[owner(items[i], n_dest)], 1u);
   __syncthreads();
   for (uint32_t i = threadIdx.x; i < n_dest; i += blockDim.x)
     if (hist[i]) atomicAdd(counts + i, static_cast<unsigned long long>(hist[i]));
 }
-// route_scatter_kernel into the owners' inboxes: item i goes to t.p[d][t.base[d] + cursor[d]++] (d = its owner), and
-// pos[i] = its index there, where the owner leaves its value
+// route_scatter_kernel into the owners' inboxes: item i goes to t.p[d][t.base[d] + cursor[d]++] (d = its owner), and,
+// with kPos, pos[i] = its index there, where the owner leaves its value
+template <class Item, class Owner, bool kPos, class Table>
+__device__ __forceinline__ void peer_scatter_items(const Item* items, unsigned long long n, uint32_t n_dest,
+                                                   unsigned long long* cursor, const Table& t, uint32_t* pos, Owner owner) {
+  const unsigned long long stride = static_cast<unsigned long long>(gridDim.x) * blockDim.x;
+  for (unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x; i < n; i += stride) {
+    const Item it = items[i];
+    const uint32_t d = owner(it, n_dest);
+    const unsigned long long at = t.base[d] + atomicAdd(cursor + d, 1ull);
+    static_cast<Item*>(t.p[d])[at] = it;
+    if constexpr (kPos) pos[i] = static_cast<uint32_t>(at);
+  }
+}
+// the sub-queries a pass raised, counted by owner
+__global__ void __launch_bounds__(256) peer_count_kernel(const zg_check* items, const unsigned long long* n_dev,
+                                                         unsigned long long cap, uint32_t n_dest, unsigned long long* counts) {
+  peer_count_items(items, n_dev, cap, n_dest, counts, ResOwner{});
+}
+// ... and written into their owners' inboxes, with where each went (pos)
 template <class Table>
 __global__ void __launch_bounds__(256) peer_scatter_kernel(const zg_check* items, unsigned long long n, uint32_t n_dest,
                                                            unsigned long long* cursor, const Table t, uint32_t* pos) {
-  const unsigned long long stride = static_cast<unsigned long long>(gridDim.x) * blockDim.x;
-  for (unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x; i < n; i += stride) {
-    const zg_check it = items[i];
-    const uint32_t d = ResOwner{}(it, n_dest);
-    const unsigned long long at = t.base[d] + atomicAdd(cursor + d, 1ull);
-    static_cast<zg_check*>(t.p[d])[at] = it;
-    pos[i] = static_cast<uint32_t>(at);
-  }
+  peer_scatter_items<zg_check, ResOwner, true>(items, n, n_dest, cursor, t, pos, ResOwner{});
 }
 // or_children_src_kernel reading each child's value from its owner (t.p[d] = shard d's values of the next level)
 template <class Table>
@@ -1965,6 +1979,19 @@ struct EntryOwner {
     return static_cast<uint32_t>(entry) % n_dest;
   }
 };
+
+// LookupSubjects on the sharded handle (capi.cu run_sharded_subjects): a level's outbox (ss_expand_kernel's entries,
+// their number read on the device) counted by owner, then written straight into the owners' inboxes behind the parts
+// of the lower shards. Nothing comes back per entry, so no position is kept.
+__global__ void __launch_bounds__(256) peer_entry_count_kernel(const unsigned long long* entries, const unsigned long long* n_dev,
+                                                               unsigned long long cap, uint32_t n_dest, unsigned long long* counts) {
+  peer_count_items(entries, n_dev, cap, n_dest, counts, EntryOwner{});
+}
+template <class Table>
+__global__ void __launch_bounds__(256) peer_entry_scatter_kernel(const unsigned long long* entries, unsigned long long n,
+                                                                 uint32_t n_dest, unsigned long long* cursor, const Table t) {
+  peer_scatter_items<unsigned long long, EntryOwner, false>(entries, n, n_dest, cursor, t, nullptr, EntryOwner{});
+}
 
 // Admission at the owner, one thread per arrived entry: a test-and-set of the object's bit in the lookup's slice.
 // A fresh entry joins the next frontier; a fresh object of the lookup's subject type is also a candidate
