@@ -351,6 +351,13 @@ int zg_handle_lookup_counters(zg_engine *e, uint64_t *out);
  * no-wildcards verification, out[6] lookups that verified every object of the subject type (the walk overflowed
  * ZGPU_LOOKUP_BATCH_CAP, or ZGPU_NO_RBFS=1). */
 int zg_handle_subjects_counters(zg_engine *e, uint64_t *out);
+/* Cumulative counters of the relationship filters of zg_read_relationships, zg_delete_relationships and the
+ * preconditions of both write calls (zg_stats keeps its layout). A filter is answered from the published snapshot on
+ * the device when the engine has one and nothing was loaded or applied since; otherwise (host-only engines,
+ * unpublished changes) by a scan of the host store. out[0] filters answered on the device, out[1] filters answered by
+ * the host scan, out[2] relationships the device returned (a precondition only counts, and returns none), out[3..5]
+ * device filters by shape: resource given, subject given without a resource, neither. */
+int zg_filter_counters(zg_engine *e, uint64_t *out);
 /* Closure indexes of the two-level steps in the engine's published snapshot (zg_stats keeps its layout): out[0] pairs
  * indexed, out[1] pairs over the size budget (their steps meet through the memberships' reverse rows instead), out[2]
  * index entries, out[3] index device bytes; out[4] index builds since creation (the rebuilds after writes included),

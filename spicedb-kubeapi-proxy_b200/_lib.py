@@ -178,6 +178,7 @@ _SIGS = {
     "zg_lookup_subjects_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
     "zg_handle_lookup_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
     "zg_handle_subjects_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "zg_filter_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
     "zg_closure_index_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
     "zg_closure_index_info": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p]),
     "zg_closure_index_copy": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
@@ -732,6 +733,15 @@ class Engine:
         out = np.zeros(len(self.HANDLE_SUBJECTS_COUNTERS), dtype=np.uint64)
         self._ck(self._L.zg_handle_subjects_counters(self._h, out.ctypes.data))
         return {k: int(v) for k, v in zip(self.HANDLE_SUBJECTS_COUNTERS, out)}
+
+    FILTER_COUNTERS = ("device_filters", "host_filters", "device_relationships", "by_resource", "by_subject", "by_scan")
+
+    def filter_counters(self) -> dict:
+        """Cumulative counters of the relationship filters of reads, deletes by filter and preconditions: answered from
+        the snapshot on the device or by the host scan (zg_filter_counters)."""
+        out = np.zeros(len(self.FILTER_COUNTERS), dtype=np.uint64)
+        self._ck(self._L.zg_filter_counters(self._h, out.ctypes.data))
+        return {k: int(v) for k, v in zip(self.FILTER_COUNTERS, out)}
 
     # -- sharded store (dist.DeviceShardedChecker drives these) --------------------
     # every pointer is a device address on this engine's GPU (ints, e.g. tensor.data_ptr())

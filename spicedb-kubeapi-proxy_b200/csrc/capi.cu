@@ -198,6 +198,9 @@ struct zg_engine {
   bool handle_subjects = false;
   uint64_t hs_lookups = 0, hs_levels = 0, hs_waits = 0, hs_entries = 0, hs_candidates = 0, hs_nowild = 0, hs_fallbacks = 0;
   std::vector<HostSnapshot> shard_built;  // zg_debug_shard_row: the host builder's arrays per shard
+  // zg_filter_counters: relationship filters (reads, deletes by filter, preconditions) answered from the snapshot on
+  // the device and by Store::match, relationships the device returned, device filters by Device::FilterShape
+  std::atomic<uint64_t> flt_device{0}, flt_host{0}, flt_returned{0}, flt_shape[3] = {};
   ~zg_engine() {
     if (group_pin) cudaFreeHost(group_pin);
   }
@@ -667,6 +670,8 @@ static std::string resolve_write(zg_engine* e, const zg_rel_str& r, zg_tuple* t)
   return "";
 }
 
+static int first_error(const std::vector<int>& rcs, const std::vector<std::string>& errs, std::string* err);
+
 static Store::Filter resolve_filter(const zg_engine* e, const zg_filter_str& f, std::string* err) {
   const Schema& sc = e->schema;
   Store::Filter o;
@@ -735,14 +740,78 @@ static Store::Filter resolve_filter(const zg_engine* e, const zg_filter_str& f, 
   return o;
 }
 
+// A relationship filter is answered from the snapshot on the device when that snapshot is the store: the engine has a
+// device, every shard holds the snapshot of the current revision, and nothing was loaded or applied since it was
+// published. Otherwise Store::match answers: host-only engines, and stores with unpublished changes (a read never
+// publishes: relationships loaded and not yet published stay invisible to checks). Caller holds e->mu.
+static bool filters_on_device(const zg_engine* e) {
+  if (e->host_only || e->dirty.load()) return false;
+  const uint32_t n = is_handle(e) ? e->n_shards : 1;
+  for (uint32_t k = 0; k < n; ++k) {
+    const auto& s = shard(const_cast<zg_engine*>(e), k).snap;
+    if (!s || s->revision != e->revision) return false;
+  }
+  return true;
+}
+
+// The device path of a filter. Caller holds e->mu and e->names (shared is enough) and has seen filters_on_device.
+// *count = the matching relationships; with `tuples`, the records in no particular order. A sharded handle asks every
+// shard (they own disjoint relationships), or the owner alone when the resource is given; replicas hold the same
+// snapshot, so the first device answers. *too_big: the records would not fit the device's output budget and the
+// caller runs Store::match instead (holding e->names exclusively).
+static int match_on_device(zg_engine* e, const Store::Filter& f, uint32_t now, uint64_t* count, std::vector<zg_tuple>* tuples,
+                           bool* too_big) {
+  *count = 0;
+  *too_big = false;
+  if (tuples) tuples->clear();
+  const uint32_t S = is_handle(e) ? e->n_shards : 1;
+  std::vector<uint64_t> n(S, 0);
+  std::vector<std::vector<zg_tuple>> got(tuples ? S : 0);
+  std::vector<int> rcs(S, ZG_OK);
+  std::vector<std::string> errs(S);
+  std::vector<char> big(S, 0);
+  auto one = [&](Device& dev, size_t k) {
+    bool b = false;
+    rcs[k] = dev.match_filter(e->schema, f, now, &n[k], tuples ? &got[k] : nullptr, nullptr, &b, &errs[k]);
+    big[k] = b;
+  };
+  if (S == 1) one(e->dev, 0);
+  else if (f.has_res) one(shard(e, f.res % S), f.res % S);
+  else on_all_devices(e, one);
+  std::string err;
+  if (int rc = first_error(rcs, errs, &err)) return fail(rc == ZG_ENOMEM ? ZG_ECUDA : rc, err);
+  for (uint32_t k = 0; k < S; ++k) {
+    *count += n[k];
+    *too_big = *too_big || big[k];
+  }
+  if (*too_big) return ZG_OK;
+  ++e->flt_device;
+  ++e->flt_shape[Device::filter_shape(f)];
+  if (tuples) {
+    for (auto& g : got) tuples->insert(tuples->end(), g.begin(), g.end());
+    e->flt_returned += tuples->size();
+  }
+  return ZG_OK;
+}
+
+// Caller holds e->mu AND e->names exclusively (every writer does).
 static int check_preconditions(zg_engine* e, const zg_precondition_str* pre, uint64_t n_pre) {
   std::vector<uint64_t> idx;
+  const bool on_device = n_pre && filters_on_device(e);
   for (uint64_t i = 0; i < n_pre; ++i) {
     std::string err;
     Store::Filter f = resolve_filter(e, pre[i].filter, &err);
     if (!err.empty()) return fail(ZG_EINVAL, "precondition " + std::to_string(i) + ": " + err);
-    e->store.match(f, now_of(e), &idx);
-    const bool any = !idx.empty();
+    uint64_t count = 0;
+    bool too_big = false;  // never: a count needs no output
+    if (on_device) {
+      if (int rc = match_on_device(e, f, now_of(e), &count, nullptr, &too_big)) return rc;
+    } else {
+      e->store.match(f, now_of(e), &idx);
+      ++e->flt_host;
+      count = idx.size();
+    }
+    const bool any = count != 0;
     if (pre[i].op == ZG_PRECOND_MUST_MATCH && !any)
       return fail(ZG_EPRECOND, "precondition " + std::to_string(i) + " (MUST_MATCH) failed");
     if (pre[i].op == ZG_PRECOND_MUST_NOT_MATCH && any)
@@ -789,6 +858,7 @@ extern "C" int zg_write_relationships(zg_engine* e, const zg_update_str* ups, ui
   std::vector<uint8_t> changed;
   std::string err = e->store.apply(u.data(), n, &code, &changed);
   if (!err.empty()) return fail(code, err);
+  e->dirty = true;  // until the publish succeeds the snapshot is not the store: filters_on_device
   rc = publish_locked(e);
   if (rc == ZG_OK) e->log_changes(u, changed);
   return rc;
@@ -805,8 +875,24 @@ extern "C" int zg_delete_relationships(zg_engine* e, const zg_filter_str* filter
   if (!err.empty()) return fail(ZG_EINVAL, err);
   int rc = check_preconditions(e, pre, n_pre);
   if (rc) return rc;
-  std::vector<uint64_t> idx;
-  e->store.match(f, 0, &idx);  // expired relationships are deleted too
+  std::vector<uint64_t> idx;  // expired relationships are deleted too: clock 0
+  bool on_device = filters_on_device(e);
+  if (on_device) {
+    std::vector<zg_tuple> found;
+    uint64_t count = 0;
+    bool too_big = false;
+    rc = match_on_device(e, f, 0, &count, &found, &too_big);
+    if (rc) return rc;
+    on_device = !too_big;
+    // apply() needs the store's index anyway; through it the device's records become store positions, and in
+    // ascending order the updates and the watch feed are those of the host scan
+    if (on_device && !e->store.locate(found.data(), found.size(), &idx))
+      return fail(ZG_ECUDA, "delete by filter: the snapshot holds a relationship the store does not");
+  }
+  if (!on_device) {
+    e->store.match(f, 0, &idx);
+    ++e->flt_host;
+  }
   std::vector<zg_update> u(idx.size());
   for (size_t i = 0; i < idx.size(); ++i) {
     u[i].t = e->store.tuples[idx[i]];
@@ -817,6 +903,7 @@ extern "C" int zg_delete_relationships(zg_engine* e, const zg_filter_str* filter
   std::vector<uint8_t> changed;
   err = e->store.apply(u.data(), u.size(), &code, &changed);
   if (!err.empty()) return fail(code, err);
+  e->dirty = true;
   if (n_deleted) *n_deleted = idx.size();
   rc = publish_locked(e);
   if (rc == ZG_OK) e->log_changes(u, changed);
@@ -841,15 +928,40 @@ extern "C" int zg_read_relationships(zg_engine* e, const zg_filter_str* filter, 
                                      uint64_t* n_out) {
   NEED_SCHEMA(e, ZG_ENOSCHEMA);
   if (!filter) return fail(ZG_EINVAL, "NULL filter");
-  LOCK_NAMES_UNIQUE(e);  // match() may (re)build the relationship index
+  // Device path: the device lock, then the names lock SHARED, the order every other call uses; checks keep resolving
+  // their strings beside the read, and the store's relationship index is never built. Host scan: the names lock
+  // exclusively, since match() may (re)build that index.
+  std::unique_lock<FairMutex> dl(e->mu, std::defer_lock);
+  if (!e->host_only) dl.lock();
+  std::shared_lock<std::shared_mutex> shared(e->names, std::defer_lock);
+  std::unique_lock<std::shared_mutex> exclusive(e->names, std::defer_lock);
+  bool on_device = filters_on_device(e);
+  if (on_device) shared.lock();
+  else exclusive.lock();
   std::string err;
   Store::Filter f = resolve_filter(e, *filter, &err);
   if (!err.empty()) return fail(ZG_EINVAL, err);
-  std::vector<uint64_t> idx;
-  e->store.match(f, now_of(e), &idx);
+  std::vector<zg_tuple> found;
+  if (on_device) {
+    uint64_t count = 0;
+    bool too_big = false;
+    if (int rc = match_on_device(e, f, now_of(e), &count, &found, &too_big)) return rc;
+    if (too_big) {  // writers wait for the device lock held here, and object ids never change: f stays resolved
+      on_device = false;
+      shared.unlock();
+      exclusive.lock();
+    }
+  }
+  if (!on_device) {
+    std::vector<uint64_t> idx;
+    e->store.match(f, now_of(e), &idx);
+    ++e->flt_host;
+    found.reserve(idx.size());
+    for (uint64_t i : idx) found.push_back(e->store.tuples[i]);
+  }
   std::vector<std::string> lines;
-  lines.reserve(idx.size());
-  for (uint64_t i : idx) lines.push_back(tuple_text(e, e->store.tuples[i]));
+  lines.reserve(found.size());
+  for (const zg_tuple& t : found) lines.push_back(tuple_text(e, t));
   std::sort(lines.begin(), lines.end());
   size_t total = 1;
   for (const auto& l : lines) total += l.size() + 1;
@@ -2619,6 +2731,15 @@ extern "C" int zg_handle_subjects_counters(zg_engine* e, uint64_t* out) {
   LOCK_DEVICE(e);
   const uint64_t c[7] = {e->hs_lookups, e->hs_levels, e->hs_waits, e->hs_entries, e->hs_candidates, e->hs_nowild,
                          e->hs_fallbacks};
+  std::memcpy(out, c, sizeof c);
+  return ZG_OK;
+}
+
+extern "C" int zg_filter_counters(zg_engine* e, uint64_t* out) {
+  if (!e || !out) return fail(ZG_EINVAL, "NULL argument");
+  const uint64_t c[6] = {e->flt_device.load(), e->flt_host.load(), e->flt_returned.load(),
+                         e->flt_shape[Device::kByResource].load(), e->flt_shape[Device::kBySubject].load(),
+                         e->flt_shape[Device::kByScan].load()};
   std::memcpy(out, c, sizeof c);
   return ZG_OK;
 }

@@ -12,6 +12,7 @@
 #include <mutex>
 #include <thread>
 
+#include "filter.cuh"
 #include "ingress.cuh"
 #include "kernels.cuh"
 
@@ -92,6 +93,7 @@ Device::~Device() {
   rb_cand_.release();
   for (auto* b : {&lb_params_, &lb_owner_, &lb_ctrl_, &lb_keys_[0], &lb_keys_[1]}) b->release();
   for (auto* b : {&ls_jobs_, &ls_codes_, &ls_has_, &ls_ids_, &ls_ctrl_}) b->release();
+  for (auto* b : {&flt_out_, &flt_exp_, &flt_ctrl_}) b->release();
   for (auto& l : pl_)
     for (auto* b : {&l.in, &l.val, &l.out, &l.raised, &l.parent, &l.pos}) b->release();
   for (auto* b : {&home_, &home_pos_, &home_out_, &peer_ctrl_}) b->release();
@@ -361,6 +363,8 @@ std::string Device::finish_publish(std::shared_ptr<Snapshot> s, const HostSnapsh
     for (size_t t = 0; t < h.n_objects.size(); ++t) base[t + 1] = base[t] + ((uint64_t(h.n_objects[t]) + 31) & ~31ull);
     s->total_bits = base.back();
     s->n_objects = h.n_objects;
+    s->rels = h.rels;
+    s->cls = h.cls;
     if (ok) ok = up(s->type_bit_base, base.data(), base.size() * 8);
   }
   {
@@ -2433,6 +2437,121 @@ int Device::lookup_subjects(uint16_t res_type, uint32_t res, uint16_t perm, uint
   rc = fetch(concrete, n_concrete, &ans->ids);
   if (!rc && ans->wildcard) rc = fetch(no_ids, n_no, &ans->excluded);
   return rc;
+}
+
+// ---- relationship filters (filter.cuh) --------------------------------------------------------
+
+int Device::match_filter(const Schema& sc, const Store::Filter& f, uint32_t now, uint64_t* count, std::vector<zg_tuple>* tuples,
+                         std::vector<uint32_t>* expires, bool* too_big, std::string* err) {
+  *count = 0;
+  *too_big = false;
+  if (tuples) tuples->clear();
+  if (expires) expires->clear();
+  std::shared_ptr<Snapshot> s = snap;
+  if (!s) {
+    if (err) *err = "no snapshot published";
+    return ZG_ENOSNAPSHOT;
+  }
+  if (f.impossible) return ZG_OK;
+  // the classes whose relation, subject type and subject relation agree with the filter
+  std::vector<FilterSel> sel;
+  for (size_t ri = 0; ri < sc.rel_slots.size() && ri < s->rels.size(); ++ri) {
+    const int slot = sc.rel_slots[ri];
+    if ((f.res_type >= 0 && sc.slots[slot].type != f.res_type) || (f.rel >= 0 && slot != f.rel)) continue;
+    const DRel& r = s->rels[ri];
+    for (uint16_t k = 0; k < r.ncls; ++k) {
+      const DCls& c = s->cls[r.cls_begin + k];
+      if (f.subj_type >= 0 && c.stype != f.subj_type) continue;
+      if (f.subj_wildcard && c.sslot != kWildcard) continue;
+      if (f.has_subj && c.sslot == kWildcard) continue;  // a concrete id never matches a wildcard relationship
+      if (f.has_srel && c.sslot != f.srel) continue;
+      FilterSel x{};
+      x.row_base = r.row_base + k;
+      x.rrow_base = c.rrow_base;
+      x.nres = r.nres;
+      x.nsubj = c.nsubj;
+      x.stride = r.stride;
+      x.rstride = c.rstride;
+      x.rel = static_cast<uint16_t>(slot);
+      x.stype = c.stype;
+      x.srel = c.sslot;
+      sel.push_back(x);
+    }
+  }
+  if (sel.empty() || s->n_tuples == 0) return ZG_OK;
+  ZG_CUDA(cudaSetDevice(device));
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  if (!flt_ctrl_.ensure(8)) {
+    if (err) *err = "out of device memory (filter)";
+    return ZG_ENOMEM;
+  }
+  FilterPlan p{};
+  p.row_ptr = s->row_ptr.as<uint32_t>();
+  p.col = s->col.as<uint32_t>();
+  p.exp = sc.has_expiry ? s->exp.as<uint32_t>() : nullptr;
+  p.rrow_ptr = s->rrow_ptr.as<uint32_t>();
+  p.rcol = s->rcol.as<uint32_t>();
+  p.has_subj = f.has_subj;
+  p.res = f.res;
+  p.subj = f.has_subj ? f.subj : 0;
+  p.now = now;
+  p.count = flt_ctrl_.as<unsigned long long>();
+  const FilterShape shape = filter_shape(f);
+  // every selected class, kMaxFilterSel per launch; the launches append behind one count
+  auto run = [&](bool emit) -> int {
+    ZG_CUDA(cudaMemsetAsync(p.count, 0, 8, stream));
+    const unsigned grid = static_cast<unsigned>(sm_count_) * 8;
+    for (size_t at = 0; at < sel.size(); at += kMaxFilterSel) {
+      p.n_sel = static_cast<uint32_t>(std::min<size_t>(kMaxFilterSel, sel.size() - at));
+      std::copy(sel.begin() + at, sel.begin() + at + p.n_sel, p.sel);
+      if (shape == kByResource) {
+        if (emit) filter_resource_kernel<true><<<grid, kFilterThreads, 0, stream>>>(p);
+        else filter_resource_kernel<false><<<grid, kFilterThreads, 0, stream>>>(p);
+      } else if (shape == kBySubject) {
+        if (emit) filter_subject_kernel<true><<<grid, kFilterThreads, 0, stream>>>(p);
+        else filter_subject_kernel<false><<<grid, kFilterThreads, 0, stream>>>(p);
+      } else {
+        if (emit) filter_scan_kernel<true><<<grid, kFilterThreads, 0, stream>>>(p);
+        else filter_scan_kernel<false><<<grid, kFilterThreads, 0, stream>>>(p);
+      }
+      ++launches;
+    }
+    ZG_CUDA(cudaGetLastError());
+    return ZG_OK;
+  };
+  if (int rc = run(false)) return rc;
+  unsigned long long n = 0;
+  ZG_CUDA(cudaMemcpyAsync(&n, p.count, 8, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  *count = n;
+  if (!tuples || n == 0) return ZG_OK;
+  size_t free_b = 0, total_b = 0;
+  ZG_CUDA(cudaMemGetInfo(&free_b, &total_b));
+  const size_t bytes = n * (sizeof(zg_tuple) + 4);
+  if (bytes > flt_out_.cap + flt_exp_.cap && bytes > free_b / 4) {
+    *too_big = true;
+    return ZG_OK;
+  }
+  if (!flt_out_.ensure(n * sizeof(zg_tuple)) || !flt_exp_.ensure(n * 4)) {
+    if (err) *err = "out of device memory (filter output)";
+    return ZG_ENOMEM;
+  }
+  p.out = flt_out_.as<zg_tuple>();
+  p.out_exp = flt_exp_.as<uint32_t>();
+  p.cap = n;
+  if (int rc = run(true)) return rc;
+  unsigned long long n2 = 0;
+  tuples->resize(n);
+  if (expires) expires->resize(n);
+  ZG_CUDA(cudaMemcpyAsync(&n2, p.count, 8, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaMemcpyAsync(tuples->data(), p.out, n * sizeof(zg_tuple), cudaMemcpyDeviceToHost, stream));
+  if (expires) ZG_CUDA(cudaMemcpyAsync(expires->data(), p.out_exp, n * 4, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  if (n2 != n) {  // the snapshot cannot change under the device lock
+    if (err) *err = "filter: the emit launch found " + std::to_string(n2) + " relationships, the count launch " + std::to_string(n);
+    return ZG_ECUDA;
+  }
+  return ZG_OK;
 }
 
 // ---- device ingress ----------------------------------------------------------------------------

@@ -36,6 +36,8 @@ struct Snapshot {
   bool delta_ok = false;             // built by the GPU builder: counts are known
   bool resources_stale = false;      // resources[] predate an incremental publish: rebuilt on first use
   std::vector<uint32_t> n_objects;  // per type
+  std::vector<DRel> rels;           // the layout's row tables, for the host to plan from (Device::match_filter);
+  std::vector<DCls> cls;            // the classes' CF_EMPTY flags are those of the last structural publish
   uint64_t total_bits = 0;          // visited bitmap size for the reverse BFS
   // Per slot: device array of FlatLookupClass when the slot is a flat union of direct
   // (non-expiring) relations; flat_n[slot] = -1 otherwise.
@@ -278,6 +280,18 @@ class Device {
   int shard_subjects_finish(const unsigned long long* d_keys, uint64_t n, uint32_t* d_ids, uint64_t* listed, uint64_t* excluded,
                             std::string* err);
 
+  // ---- relationship filters (filter.cuh): ReadRelationships, DeleteRelationships, write preconditions ----
+  enum FilterShape { kByResource = 0, kBySubject = 1, kByScan = 2 };
+  static FilterShape filter_shape(const Store::Filter& f) {
+    return f.has_res ? kByResource : (f.has_subj || f.subj_wildcard) ? kBySubject : kByScan;
+  }
+  // The relationships of the resident snapshot that match f at clock `now` (0: expired ones too), what Store::match
+  // returns for the store the snapshot was published from: *count of them, and with `tuples` the records, in no
+  // particular order (expires, optional, parallel to them). A count launch sizes the output, then an emit launch fills
+  // it. *too_big: the records would take more than a quarter of the free device memory; only *count is valid.
+  int match_filter(const Schema& sc, const Store::Filter& f, uint32_t now, uint64_t* count, std::vector<zg_tuple>* tuples,
+                   std::vector<uint32_t>* expires, bool* too_big, std::string* err);
+
   // ---- device ingress (ingress.cuh): packed string ids -> interned checks against the mirror of the store's names ----
   // The literal fields of a packed call, resolved once on the host exactly as zg_resolve_checks_packed resolves them.
   struct IngressLiterals {
@@ -346,6 +360,7 @@ class Device {
   DevBuf rb_visited_, rb_front_[2], rb_cand_;
   DevBuf lb_params_, lb_owner_, lb_ctrl_, lb_keys_[2];  // batched lookups
   DevBuf ls_jobs_, ls_codes_, ls_has_, ls_ids_, ls_ctrl_;   // LookupSubjects
+  DevBuf flt_out_, flt_exp_, flt_ctrl_;                     // match_filter: records, expirations, the count
   // sharded LookupResources round: walk state in rb_visited_ / lk_jobs_ / lb_owner_ / lb_params_ / lb_keys_ (a sharded
   // engine never runs lookup_batch), the round's home ranks, self-membership list and control words here
   DevBuf sl_home_, sl_self_, sl_ctrl_;

@@ -276,6 +276,18 @@ void Store::match(const Filter& f, uint32_t now, std::vector<uint64_t>* idx) con
   }
 }
 
+bool Store::locate(const zg_tuple* t, uint64_t n, std::vector<uint64_t>* idx) {
+  ensure_index();
+  idx->resize(n);
+  for (uint64_t i = 0; i < n; ++i) {
+    auto it = index_.find(key_of(t[i]));
+    if (it == index_.end()) return false;
+    (*idx)[i] = it->second;
+  }
+  std::sort(idx->begin(), idx->end());
+  return true;
+}
+
 HostSnapshot Store::layout() const {
   const Schema& sc = *schema;
   HostSnapshot h;

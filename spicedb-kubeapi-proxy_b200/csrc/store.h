@@ -106,6 +106,9 @@ class Store {
     bool impossible = false;  // names an object/relation that does not exist
   };
   void match(const Filter& f, uint32_t now, std::vector<uint64_t>* idx) const;
+  // Where the n live relationships t[] sit in `tuples`, ascending: the order match() lists them in. Builds the
+  // relationship index when a bulk load left it behind. false when one of them is not in the store.
+  bool locate(const zg_tuple* t, uint64_t n, std::vector<uint64_t>* idx);
 
   // Sizes and bases only (n_objects, rels, cls with rrow_base / nsubj and CF_EMPTY set on every
   // class): what both the host builder and the GPU builder (build.cu) start from.
