@@ -39,6 +39,7 @@ import (
 	"strings"
 	"sync"
 	"sync/atomic"
+	"time"
 	"unsafe"
 
 	v1 "github.com/authzed/authzed-go/proto/authzed/api/v1"
@@ -481,6 +482,20 @@ func (c *Client) DeleteRelationships(ctx context.Context, req *v1.DeleteRelation
 		}
 	}
 	return resp, nil
+}
+
+// CollectExpired removes from the mirror every relationship whose expiration is at or before `before`, which must
+// not be later than the engine's clock, and returns how many it removed. Answers at any later time do not change and
+// the watch feed records nothing; SpiceDB collects its own copy on its GC window. Nothing calls it automatically: run
+// it periodically, e.g. every hour with time.Now().Add(-24 * time.Hour).
+func (c *Client) CollectExpired(before time.Time) (uint64, error) {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	var n C.uint64_t
+	if err := call(func() C.int { return C.zg_collect_expired(c.engine, C.int64_t(before.Unix()), &n) }); err != nil {
+		return 0, err
+	}
+	return uint64(n), nil
 }
 
 // resync rebuilds the mirror from a full ReadRelationships per resource type. The mirror is EMPTIED

@@ -17,6 +17,7 @@
  *   zg_lookup_subjects*         LookupSubjects stream  (v1 API; pkg/authz/postfilter_test.go:71 mock)
  *   zg_write_relationships      WriteRelationships     pkg/authz/distributedtx/activity.go:54-76
  *   zg_delete_relationships     DeleteRelationships    (v1 API; filter semantics update.go:207-271)
+ *   zg_collect_expired          the datastore's garbage collection of expired relationships (pkg/spicedb/spicedb.go:53)
  *   zg_read_relationships       ReadRelationships      pkg/authz/distributedtx/activity.go:128-171
  *   zg_watch_read               WatchService.Watch     pkg/authz/watch.go:27-48
  *   zg_engine_create/load_schema embedded SpiceDB ctor pkg/spicedb/spicedb.go:18-57
@@ -243,6 +244,21 @@ int zg_write_relationships(zg_engine *e, const zg_update_str *updates, uint64_t 
 /* v1 DeleteRelationships by filter; *n_deleted may be NULL. */
 int zg_delete_relationships(zg_engine *e, const zg_filter_str *filter,
                             const zg_precondition_str *pre, uint64_t n_pre, uint64_t *n_deleted);
+/* Removes every relationship whose expiration is set and <= before_unix from the store and from the resident
+ * snapshot(s). before_unix must not be later than the engine's clock (zg_set_clock, else wall clock): ZG_EINVAL.
+ * Every check, lookup and read at a clock >= before_unix answers as before the call. *n_removed may be NULL.
+ *   - Relationships without an expiration (expires == 0) are never removed; a schema without expiration removes
+ *     nothing. Nothing calls this automatically: a deployment runs it on its own schedule (INTEGRATION.md).
+ *   - Takes the device lock, then the names lock exclusively, as zg_delete_relationships does.
+ *   - When nothing qualifies it returns 0 removed: nothing is applied or published, the revision does not move. On a
+ *     current snapshot that costs one count launch. Otherwise the DELETEs are applied and published once (pending
+ *     changes included, as every write call does), and the revision advances.
+ *   - It writes nothing to the watch feed: an expiration is not a write, and no answer at a clock >= before_unix
+ *     changes. Interned names are kept, as after every delete.
+ *   - Found on the device (a scan of the classes that may carry an expiration; every shard of a sharded handle scans
+ *     its own rows) when the snapshot is current, else by a scan of the host store; zg_filter_counters counts it as
+ *     it counts a delete by filter. */
+int zg_collect_expired(zg_engine *e, int64_t before_unix, uint64_t *n_removed);
 /* v1 ReadRelationships: matching live relationships as "type:id#rel@stype:sid[#srel]\n"
  * lines, sorted. Returns 0 or ZG_E2BIG (*need = bytes required incl. NUL). */
 int zg_read_relationships(zg_engine *e, const zg_filter_str *filter, char *buf, size_t cap,

@@ -156,6 +156,7 @@ _SIGS = {
     "zg_write_relationships": (C.c_int, [C.c_void_p, C.POINTER(_UpdateStr), C.c_uint64, C.POINTER(_Precond), C.c_uint64]),
     "zg_delete_relationships": (C.c_int, [C.c_void_p, C.POINTER(_RelStr), C.POINTER(_Precond), C.c_uint64,
                                           C.POINTER(C.c_uint64)]),
+    "zg_collect_expired": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(C.c_uint64)]),
     "zg_read_relationships": (C.c_int, [C.c_void_p, C.POINTER(_RelStr), C.c_char_p, C.c_size_t,
                                         C.POINTER(C.c_size_t), C.POINTER(C.c_uint64)]),
     "zg_watch_read": (C.c_int, [C.c_void_p, C.c_uint64, C.c_char_p, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t),
@@ -450,6 +451,13 @@ class Engine:
         n = C.c_uint64(0)
         f = self._filter(flt)
         self._ck(self._L.zg_delete_relationships(self._h, C.byref(f), pre, len(preconditions), C.byref(n)))
+        return n.value
+
+    def collect_expired(self, before: int) -> int:
+        """zg_collect_expired: removes every relationship whose expiration is set and <= before (unix seconds, not
+        later than the engine's clock); returns how many. Answers at clocks >= before do not change."""
+        n = C.c_uint64(0)
+        self._ck(self._L.zg_collect_expired(self._h, int(before), C.byref(n)))
         return n.value
 
     def read_relationships(self, **flt):

@@ -754,13 +754,13 @@ static bool filters_on_device(const zg_engine* e) {
   return true;
 }
 
-// The device path of a filter. Caller holds e->mu and e->names (shared is enough) and has seen filters_on_device.
-// *count = the matching relationships; with `tuples`, the records in no particular order. A sharded handle asks every
-// shard (they own disjoint relationships), or the owner alone when the resource is given; replicas hold the same
-// snapshot, so the first device answers. *too_big: the records would not fit the device's output budget and the
-// caller runs Store::match instead (holding e->names exclusively).
-static int match_on_device(zg_engine* e, const Store::Filter& f, uint32_t now, uint64_t* count, std::vector<zg_tuple>* tuples,
-                           bool* too_big) {
+// A device's part of a filter or a collection: Device::match_filter or Device::match_expired.
+using DeviceMatch = std::function<int(Device&, uint64_t* count, std::vector<zg_tuple>* tuples, bool* too_big, std::string* err)>;
+
+// Runs `ask` on the first device, or on every shard of a sharded handle, or on shard `owner` alone (>= 0), adds up
+// the counts and concatenates the records, and counts a device filter of `shape`.
+static int ask_devices(zg_engine* e, int owner, Device::FilterShape shape, const DeviceMatch& ask, uint64_t* count,
+                       std::vector<zg_tuple>* tuples, bool* too_big) {
   *count = 0;
   *too_big = false;
   if (tuples) tuples->clear();
@@ -772,11 +772,11 @@ static int match_on_device(zg_engine* e, const Store::Filter& f, uint32_t now, u
   std::vector<char> big(S, 0);
   auto one = [&](Device& dev, size_t k) {
     bool b = false;
-    rcs[k] = dev.match_filter(e->schema, f, now, &n[k], tuples ? &got[k] : nullptr, nullptr, &b, &errs[k]);
+    rcs[k] = ask(dev, &n[k], tuples ? &got[k] : nullptr, &b, &errs[k]);
     big[k] = b;
   };
   if (S == 1) one(e->dev, 0);
-  else if (f.has_res) one(shard(e, f.res % S), f.res % S);
+  else if (owner >= 0) one(shard(e, static_cast<uint32_t>(owner)), static_cast<size_t>(owner));
   else on_all_devices(e, one);
   std::string err;
   if (int rc = first_error(rcs, errs, &err)) return fail(rc == ZG_ENOMEM ? ZG_ECUDA : rc, err);
@@ -786,12 +786,48 @@ static int match_on_device(zg_engine* e, const Store::Filter& f, uint32_t now, u
   }
   if (*too_big) return ZG_OK;
   ++e->flt_device;
-  ++e->flt_shape[Device::filter_shape(f)];
+  ++e->flt_shape[shape];
   if (tuples) {
     for (auto& g : got) tuples->insert(tuples->end(), g.begin(), g.end());
     e->flt_returned += tuples->size();
   }
   return ZG_OK;
+}
+
+// The device path of a filter. Caller holds e->mu and e->names (shared is enough) and has seen filters_on_device.
+// *count = the matching relationships; with `tuples`, the records in no particular order. A sharded handle asks every
+// shard (they own disjoint relationships), or the owner alone when the resource is given; replicas hold the same
+// snapshot, so the first device answers. *too_big: the records would not fit the device's output budget and the
+// caller runs Store::match instead (holding e->names exclusively).
+static int match_on_device(zg_engine* e, const Store::Filter& f, uint32_t now, uint64_t* count, std::vector<zg_tuple>* tuples,
+                           bool* too_big) {
+  const int owner = is_handle(e) && f.has_res ? static_cast<int>(f.res % e->n_shards) : -1;
+  return ask_devices(e, owner, Device::filter_shape(f), [&](Device& dev, uint64_t* n, std::vector<zg_tuple>* got, bool* big,
+                                                            std::string* err) {
+    return dev.match_filter(e->schema, f, now, n, got, nullptr, big, err);
+  }, count, tuples, too_big);
+}
+
+// Removes the relationships a delete by filter or a collection found. On the device path the records `found` (any
+// order) become store positions through the index apply() needs anyway, and in ascending order the updates and the
+// watch feed are those of the host scan, which leaves its positions in *idx (found == nullptr). Applies the DELETEs
+// (*u, and *changed for the feed), sets *n_done, and publishes once. Caller holds e->mu AND e->names exclusively.
+static int delete_found(zg_engine* e, const char* what, const std::vector<zg_tuple>* found, std::vector<uint64_t>* idx,
+                        std::vector<zg_update>* u, std::vector<uint8_t>* changed, uint64_t* n_done) {
+  if (found && !e->store.locate(found->data(), found->size(), idx))
+    return fail(ZG_ECUDA, std::string(what) + ": the snapshot holds a relationship the store does not");
+  u->resize(idx->size());
+  for (size_t i = 0; i < idx->size(); ++i) {
+    (*u)[i].t = e->store.tuples[(*idx)[i]];
+    (*u)[i].expires_at = 0;
+    (*u)[i].op = ZG_OP_DELETE;
+  }
+  int code = ZG_OK;
+  std::string err = e->store.apply(u->data(), u->size(), &code, changed);
+  if (!err.empty()) return fail(code, err);
+  e->dirty = true;
+  if (n_done) *n_done = idx->size();
+  return publish_locked(e);
 }
 
 // Caller holds e->mu AND e->names exclusively (every writer does).
@@ -876,38 +912,61 @@ extern "C" int zg_delete_relationships(zg_engine* e, const zg_filter_str* filter
   int rc = check_preconditions(e, pre, n_pre);
   if (rc) return rc;
   std::vector<uint64_t> idx;  // expired relationships are deleted too: clock 0
+  std::vector<zg_tuple> found;
   bool on_device = filters_on_device(e);
   if (on_device) {
-    std::vector<zg_tuple> found;
     uint64_t count = 0;
     bool too_big = false;
     rc = match_on_device(e, f, 0, &count, &found, &too_big);
     if (rc) return rc;
     on_device = !too_big;
-    // apply() needs the store's index anyway; through it the device's records become store positions, and in
-    // ascending order the updates and the watch feed are those of the host scan
-    if (on_device && !e->store.locate(found.data(), found.size(), &idx))
-      return fail(ZG_ECUDA, "delete by filter: the snapshot holds a relationship the store does not");
   }
   if (!on_device) {
     e->store.match(f, 0, &idx);
     ++e->flt_host;
   }
-  std::vector<zg_update> u(idx.size());
-  for (size_t i = 0; i < idx.size(); ++i) {
-    u[i].t = e->store.tuples[idx[i]];
-    u[i].expires_at = 0;
-    u[i].op = ZG_OP_DELETE;
-  }
-  int code = ZG_OK;
+  std::vector<zg_update> u;
   std::vector<uint8_t> changed;
-  err = e->store.apply(u.data(), u.size(), &code, &changed);
-  if (!err.empty()) return fail(code, err);
-  e->dirty = true;
-  if (n_deleted) *n_deleted = idx.size();
-  rc = publish_locked(e);
+  rc = delete_found(e, "delete by filter", on_device ? &found : nullptr, &idx, &u, &changed, n_deleted);
   if (rc == ZG_OK) e->log_changes(u, changed);
   return rc;
+}
+
+extern "C" int zg_collect_expired(zg_engine* e, int64_t before_unix, uint64_t* n_removed) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (n_removed) *n_removed = 0;
+  LOCK_DEVICE(e);
+  LOCK_NAMES_UNIQUE(e);
+  const int64_t clock = e->clock ? e->clock : static_cast<int64_t>(time(nullptr));
+  if (before_unix > clock)
+    return fail(ZG_EINVAL, "collect expired: before (" + std::to_string(before_unix) + ") is later than the engine's clock (" +
+                               std::to_string(clock) + ")");
+  // expirations are stored as unsigned 32-bit seconds, and 0 means "never"
+  if (!e->schema.has_expiry || before_unix <= 0) return ZG_OK;
+  const uint32_t before = static_cast<uint32_t>(std::min<int64_t>(before_unix, 0xFFFFFFFFll));
+  std::vector<uint64_t> idx;
+  std::vector<zg_tuple> found;
+  bool on_device = filters_on_device(e);
+  if (on_device) {
+    uint64_t count = 0;
+    bool too_big = false;
+    int rc = ask_devices(e, -1, Device::kByScan, [&](Device& dev, uint64_t* n, std::vector<zg_tuple>* got, bool* big,
+                                                     std::string* err) {
+      return dev.match_expired(e->schema, before, n, got, big, err);
+    }, &count, &found, &too_big);
+    if (rc) return rc;
+    on_device = !too_big;
+    if (on_device && count == 0) return ZG_OK;
+  }
+  if (!on_device) {
+    e->store.expired(before, &idx);
+    ++e->flt_host;
+    if (idx.empty()) return ZG_OK;
+  }
+  // an expiration is not a write: the watch feed records none of these DELETEs
+  std::vector<zg_update> u;
+  std::vector<uint8_t> changed;
+  return delete_found(e, "collect expired", on_device ? &found : nullptr, &idx, &u, &changed, n_removed);
 }
 
 static std::string tuple_text(const zg_engine* e, const zg_tuple& t) {

@@ -2479,24 +2479,62 @@ int Device::match_filter(const Schema& sc, const Store::Filter& f, uint32_t now,
     }
   }
   if (sel.empty() || s->n_tuples == 0) return ZG_OK;
+  FilterPlan p{};
+  p.has_subj = f.has_subj;
+  p.res = f.res;
+  p.subj = f.has_subj ? f.subj : 0;
+  p.now = now;
+  return run_filter(sc, *s, sel, p, filter_shape(f), false, count, tuples, expires, too_big, err);
+}
+
+int Device::match_expired(const Schema& sc, uint32_t before, uint64_t* count, std::vector<zg_tuple>* tuples, bool* too_big,
+                          std::string* err) {
+  *count = 0;
+  *too_big = false;
+  if (tuples) tuples->clear();
+  std::shared_ptr<Snapshot> s = snap;
+  if (!s) {
+    if (err) *err = "no snapshot published";
+    return ZG_ENOSNAPSHOT;
+  }
+  // every class whose relationships may carry an expiration; the rows of any other class hold none
+  std::vector<FilterSel> sel;
+  for (size_t ri = 0; ri < sc.rel_slots.size() && ri < s->rels.size(); ++ri) {
+    const DRel& r = s->rels[ri];
+    for (uint16_t k = 0; k < r.ncls; ++k) {
+      const DCls& c = s->cls[r.cls_begin + k];
+      if (!(c.flags & CF_EXPIRY)) continue;
+      FilterSel x{};
+      x.row_base = r.row_base + k;
+      x.nres = r.nres;
+      x.stride = r.stride;
+      x.rel = static_cast<uint16_t>(sc.rel_slots[ri]);
+      x.stype = c.stype;
+      x.srel = c.sslot;
+      sel.push_back(x);
+    }
+  }
+  if (sel.empty() || s->n_tuples == 0) return ZG_OK;
+  FilterPlan p{};
+  p.now = before;
+  return run_filter(sc, *s, sel, p, kByScan, true, count, tuples, nullptr, too_big, err);
+}
+
+int Device::run_filter(const Schema& sc, const Snapshot& s, const std::vector<FilterSel>& sel, FilterPlan& p, FilterShape shape,
+                       bool expired, uint64_t* count, std::vector<zg_tuple>* tuples, std::vector<uint32_t>* expires,
+                       bool* too_big, std::string* err) {
   ZG_CUDA(cudaSetDevice(device));
   if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
   if (!flt_ctrl_.ensure(8)) {
     if (err) *err = "out of device memory (filter)";
     return ZG_ENOMEM;
   }
-  FilterPlan p{};
-  p.row_ptr = s->row_ptr.as<uint32_t>();
-  p.col = s->col.as<uint32_t>();
-  p.exp = sc.has_expiry ? s->exp.as<uint32_t>() : nullptr;
-  p.rrow_ptr = s->rrow_ptr.as<uint32_t>();
-  p.rcol = s->rcol.as<uint32_t>();
-  p.has_subj = f.has_subj;
-  p.res = f.res;
-  p.subj = f.has_subj ? f.subj : 0;
-  p.now = now;
+  p.row_ptr = s.row_ptr.as<uint32_t>();
+  p.col = s.col.as<uint32_t>();
+  p.exp = sc.has_expiry ? s.exp.as<uint32_t>() : nullptr;
+  p.rrow_ptr = s.rrow_ptr.as<uint32_t>();
+  p.rcol = s.rcol.as<uint32_t>();
   p.count = flt_ctrl_.as<unsigned long long>();
-  const FilterShape shape = filter_shape(f);
   // every selected class, kMaxFilterSel per launch; the launches append behind one count
   auto run = [&](bool emit) -> int {
     ZG_CUDA(cudaMemsetAsync(p.count, 0, 8, stream));
@@ -2504,7 +2542,10 @@ int Device::match_filter(const Schema& sc, const Store::Filter& f, uint32_t now,
     for (size_t at = 0; at < sel.size(); at += kMaxFilterSel) {
       p.n_sel = static_cast<uint32_t>(std::min<size_t>(kMaxFilterSel, sel.size() - at));
       std::copy(sel.begin() + at, sel.begin() + at + p.n_sel, p.sel);
-      if (shape == kByResource) {
+      if (expired) {
+        if (emit) filter_expired_kernel<true><<<grid, kFilterThreads, 0, stream>>>(p);
+        else filter_expired_kernel<false><<<grid, kFilterThreads, 0, stream>>>(p);
+      } else if (shape == kByResource) {
         if (emit) filter_resource_kernel<true><<<grid, kFilterThreads, 0, stream>>>(p);
         else filter_resource_kernel<false><<<grid, kFilterThreads, 0, stream>>>(p);
       } else if (shape == kBySubject) {

@@ -14,6 +14,9 @@
 
 namespace zg {
 
+struct FilterSel;   // filter.cuh
+struct FilterPlan;
+
 struct DevBuf {
   void* p = nullptr;
   size_t cap = 0;
@@ -291,6 +294,11 @@ class Device {
   // it. *too_big: the records would take more than a quarter of the free device memory; only *count is valid.
   int match_filter(const Schema& sc, const Store::Filter& f, uint32_t now, uint64_t* count, std::vector<zg_tuple>* tuples,
                    std::vector<uint32_t>* expires, bool* too_big, std::string* err);
+  // The relationships of the resident snapshot whose expiration is set and <= before (zg_collect_expired), what
+  // Store::expired returns for the store the snapshot was published from; otherwise as match_filter. Only the classes
+  // with CF_EXPIRY are read. A count launch that finds nothing is the whole call.
+  int match_expired(const Schema& sc, uint32_t before, uint64_t* count, std::vector<zg_tuple>* tuples, bool* too_big,
+                    std::string* err);
 
   // ---- device ingress (ingress.cuh): packed string ids -> interned checks against the mirror of the store's names ----
   // The literal fields of a packed call, resolved once on the host exactly as zg_resolve_checks_packed resolves them.
@@ -340,6 +348,11 @@ class Device {
   // objects, else 32-bit, and rebuilds every pair built at another width. A pair whose build fails is left without an
   // index (closure_failures).
   void build_closures(Snapshot* s, const HostSnapshot& h, const std::vector<uint8_t>* rebuild);
+  // match_filter / match_expired: the count launch over the classes `sel` (p holds the rest of the plan), then with
+  // `tuples` the emit launch sized by it, of filter_expired_kernel (`expired`) or the kernel of `shape`.
+  int run_filter(const Schema& sc, const Snapshot& s, const std::vector<FilterSel>& sel, FilterPlan& p, FilterShape shape,
+                 bool expired, uint64_t* count, std::vector<zg_tuple>* tuples, std::vector<uint32_t>* expires, bool* too_big,
+                 std::string* err);
   int ingress_sync(const Store& store, cudaStream_t st, std::string* err);
   std::string finish_publish(std::shared_ptr<Snapshot> s, const HostSnapshot& lay, const Schema& sc, uint64_t revision);
   // One check_kernel launch over `nq` queries: val (may be null) receives the per-(query, leaf) value

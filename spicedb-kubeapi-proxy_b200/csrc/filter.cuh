@@ -10,6 +10,10 @@
 // Every kernel counts its matches; the emitting instantiation also appends them as zg_tuple records (+ expirations).
 // The host sizes the output from a count launch, so `cap` only guards: a record that does not fit is not written.
 // No kernel reads past a row: an id at or beyond a table's object count matches nothing.
+//
+// filter_expired_kernel (zg_collect_expired) is the "neither" scan with another predicate: an entry matches when its
+// expiration is set and at or before `now`, which it reads as the collection's `before`. Device::match_expired selects
+// the classes that may carry an expiration (CF_EXPIRY) and no other.
 #pragma once
 #ifndef ZG_EMULATE  // tests/emu/: the same source under a CPU SIMT emulator (test infrastructure, never in libzgpu.so)
 #include <cuda_runtime.h>
@@ -55,6 +59,7 @@ __device__ __forceinline__ uint32_t filter_lower_bound(const uint32_t* a, uint32
   return lo;
 }
 __device__ __forceinline__ bool filter_live(uint32_t expires, uint32_t now) { return now == 0 || expires == 0 || expires > now; }
+__device__ __forceinline__ bool filter_expired(uint32_t expires, uint32_t before) { return expires != 0 && expires <= before; }
 
 // Warp-collective: counts the lanes with `hit`, and (kEmit) appends their records behind one reservation.
 template <bool kEmit>
@@ -79,8 +84,9 @@ __device__ __forceinline__ void filter_append(const FilterPlan& p, const FilterS
   }
 }
 
-// The entries [b, e) of the forward row of `res`, dealt out to the grid's warps 32 at a time.
-template <bool kEmit>
+// The entries [b, e) of the forward row of `res`, dealt out to the grid's warps 32 at a time. kExpired: the entries
+// filter_expired selects instead of the live ones.
+template <bool kEmit, bool kExpired = false>
 __device__ __forceinline__ void filter_forward_row(const FilterPlan& p, const FilterSel& s, uint32_t res, uint32_t b, uint32_t e,
                                                    unsigned long long first, unsigned long long step, unsigned lane) {
   for (unsigned long long i0 = b + first; i0 < e; i0 += step) {
@@ -90,7 +96,7 @@ __device__ __forceinline__ void filter_forward_row(const FilterPlan& p, const Fi
     if (hit) {
       subj = __ldg(p.col + i);
       if (p.exp) ex = __ldg(p.exp + i);
-      hit = filter_live(ex, p.now);
+      hit = kExpired ? filter_expired(ex, p.now) : filter_live(ex, p.now);
     }
     filter_append<kEmit>(p, s, hit, res, subj, ex, lane);
   }
@@ -149,13 +155,15 @@ __global__ void __launch_bounds__(kFilterThreads) filter_subject_kernel(const Fi
 }
 
 // Neither: every row of the selected classes. A warp reads the offsets of 32 consecutive objects, one per lane, then
-// works each non-empty row together. A count that does not depend on expirations needs the offsets only.
-template <bool kEmit>
-__global__ void __launch_bounds__(kFilterThreads) filter_scan_kernel(const FilterPlan p) {
+// works each non-empty row together. A count that does not depend on expirations needs the offsets only. kExpired:
+// the entries filter_expired selects, which always depends on them. The plan is taken by value: inlined into the
+// kernels it stays the kernel parameter, and filter_scan_kernel compiles to the SASS it had as a kernel of its own.
+template <bool kEmit, bool kExpired>
+__device__ __forceinline__ void filter_scan(const FilterPlan p) {
   const unsigned lane = threadIdx.x & 31;
   const unsigned long long w = (blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x) >> 5;
   const unsigned long long n_warps = (static_cast<unsigned long long>(gridDim.x) * blockDim.x) >> 5;
-  const bool offsets_only = !kEmit && !(p.exp && p.now);
+  const bool offsets_only = !kEmit && !kExpired && !(p.exp && p.now);
   for (uint32_t k = 0; k < p.n_sel; ++k) {
     const FilterSel& s = p.sel[k];
     for (unsigned long long obj0 = w * 32; obj0 < s.nres; obj0 += n_warps * 32) {
@@ -177,10 +185,21 @@ __global__ void __launch_bounds__(kFilterThreads) filter_scan_kernel(const Filte
         const int src = __ffs(rows) - 1;
         rows &= rows - 1;
         const uint32_t rb = __shfl_sync(kFilterFull, b, src), re = __shfl_sync(kFilterFull, e, src);
-        filter_forward_row<kEmit>(p, s, static_cast<uint32_t>(obj0 + src), rb, re, 0, 32, lane);
+        filter_forward_row<kEmit, kExpired>(p, s, static_cast<uint32_t>(obj0 + src), rb, re, 0, 32, lane);
       }
     }
   }
+}
+
+template <bool kEmit>
+__global__ void __launch_bounds__(kFilterThreads) filter_scan_kernel(const FilterPlan p) {
+  filter_scan<kEmit, false>(p);
+}
+
+// Expired relationships of the selected classes: p.now is the collection's `before` (never 0).
+template <bool kEmit>
+__global__ void __launch_bounds__(kFilterThreads) filter_expired_kernel(const FilterPlan p) {
+  filter_scan<kEmit, true>(p);
 }
 
 }  // namespace zg

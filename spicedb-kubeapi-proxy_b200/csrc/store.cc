@@ -288,6 +288,13 @@ bool Store::locate(const zg_tuple* t, uint64_t n, std::vector<uint64_t>* idx) {
   return true;
 }
 
+void Store::expired(uint32_t before, std::vector<uint64_t>* idx) {
+  idx->clear();
+  ensure_index();
+  for (uint64_t i = 0; i < tuples.size(); ++i)
+    if (!(tuples[i].flags & 1) && expires[i] != 0 && expires[i] <= before) idx->push_back(i);
+}
+
 HostSnapshot Store::layout() const {
   const Schema& sc = *schema;
   HostSnapshot h;

@@ -109,6 +109,9 @@ class Store {
   // Where the n live relationships t[] sit in `tuples`, ascending: the order match() lists them in. Builds the
   // relationship index when a bulk load left it behind. false when one of them is not in the store.
   bool locate(const zg_tuple* t, uint64_t n, std::vector<uint64_t>* idx);
+  // Where the live relationships whose expiration is set and <= before sit in `tuples`, ascending: what
+  // zg_collect_expired removes. Folds the duplicates of bulk loads first, as match() does.
+  void expired(uint32_t before, std::vector<uint64_t>* idx);
 
   // Sizes and bases only (n_objects, rels, cls with rrow_base / nsubj and CF_EMPTY set on every
   // class): what both the host builder and the GPU builder (build.cu) start from.
