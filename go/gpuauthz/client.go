@@ -498,6 +498,19 @@ func (c *Client) CollectExpired(before time.Time) (uint64, error) {
 	return uint64(n), nil
 }
 
+// RetireUnusedNames frees the interned names that no relationship of the mirror and no retained watch change mentions
+// any more, and returns how many; later names reuse their ids, so the id space stays flat under the proxy's churn.
+// The shim passes only strings and holds no ids, so nothing it caches goes stale. Run it right after CollectExpired.
+func (c *Client) RetireUnusedNames() (uint64, error) {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	var n C.uint64_t
+	if err := call(func() C.int { return C.zg_retire_unused_names(c.engine, &n) }); err != nil {
+		return 0, err
+	}
+	return uint64(n), nil
+}
+
 // resync rebuilds the mirror from a full ReadRelationships per resource type. The mirror is EMPTIED
 // first: it runs when a mirrored write failed after SpiceDB committed, and a batch that was rejected as a
 // whole may have carried DELETEs -- re-TOUCHing what SpiceDB holds now would leave those revoked grants

@@ -18,6 +18,7 @@
  *   zg_write_relationships      WriteRelationships     pkg/authz/distributedtx/activity.go:54-76
  *   zg_delete_relationships     DeleteRelationships    (v1 API; filter semantics update.go:207-271)
  *   zg_collect_expired          the datastore's garbage collection of expired relationships (pkg/spicedb/spicedb.go:53)
+ *   zg_retire_unused_names      frees the interned names no relationship mentions any more, for reuse
  *   zg_read_relationships       ReadRelationships      pkg/authz/distributedtx/activity.go:128-171
  *   zg_watch_read               WatchService.Watch     pkg/authz/watch.go:27-48
  *   zg_engine_create/load_schema embedded SpiceDB ctor pkg/spicedb/spicedb.go:18-57
@@ -259,6 +260,41 @@ int zg_delete_relationships(zg_engine *e, const zg_filter_str *filter,
  *     its own rows) when the snapshot is current, else by a scan of the host store; zg_filter_counters counts it as
  *     it counts a delete by filter. */
 int zg_collect_expired(zg_engine *e, int64_t before_unix, uint64_t *n_removed);
+/* Retires every interned name (type, id) that no relationship in the store names as its resource or its subject (live,
+ * expired and not yet collected, or loaded / applied and not yet published) and no change retained in the watch feed
+ * names; *n_retired (may be NULL) = how many. Ids that bulk loads use without a name are never touched.
+ *   - After the call a retired name is as if it had never been written: zg_find_object gives ZG_NO_OBJECT,
+ *     zg_object_name of its old id ZG_EINVAL, and every string-form call answers as before, since nothing mentioned it.
+ *     Names that are not retired keep their ids.
+ *   - Nothing is published, the revision does not move, the watch feed records nothing, the snapshot is not touched.
+ *   - Id reuse: later interning (zg_intern_object, zg_intern_objects_packed, the write calls) hands out the freed ids
+ *     lowest first before it extends the type's id space, so object capacities stay flat under churn. A freed id that
+ *     zg_load_tuples / zg_apply_updates names directly is no longer free.
+ *   - A caller must not use an id of a retired name obtained earlier: until it is reused it answers as a never-written
+ *     object, after reuse it denotes the new name. An engine on which this is never called behaves as before.
+ *   - The lookup answers kept for the ZG_E2BIG protocol stay valid: every id in an answer is mentioned at its revision.
+ *   - The string calls that resolve names and answer after releasing the names lock (zg_check_bulk_str,
+ *     zg_check_bulk_packed, zg_lookup_resources_str, zg_lookup_subjects_str, zg_list_postfilter, zg_list_prefilter)
+ *     resolve and answer again when a retirement ran in between, so they never answer for, or print, a name that
+ *     took over a retired name's id. Each retirement that retires a name makes such calls in flight start over.
+ *   - Takes the device lock, then the names lock exclusively, as zg_collect_expired does. ZG_EINVAL on a standalone
+ *     shard (zg_config.shard_count > 1: its store does not hold the other shards' relationships); sharded handles and
+ *     replicas are served. The device mirror of the names (device ingress) is dropped when a name is retired and
+ *     rebuilt by the next device-ingress call.
+ *   - The mentioned ids are read from the resident snapshot (every shard of a sharded handle scans its own, OR-ed)
+ *     when it is the store, else by a scan of the host store (host-only engines, unpublished changes). */
+int zg_retire_unused_names(zg_engine *e, uint64_t *n_retired);
+/* Name counters (zg_stats keeps its layout): out[0] named objects, out[1] names retired since the schema was loaded,
+ * out[2] free ids (retired, not reused yet), out[3] the id extent summed over types (the larger of the named and the
+ * numeric ids: what object capacities follow), out[4] bytes of the host name arenas, out[5] / out[6] names retired by
+ * calls that read the mentions on the device / by the host scan. */
+int zg_name_counters(zg_engine *e, uint64_t *out);
+/* The object capacity of type_id in the last layout (what the snapshot's row tables cover; 0 before the first
+ * publish). Capacities grow in steps and never shrink; a capacity step makes the next publish a full rebuild. */
+uint64_t zg_object_capacity(const zg_engine *e, int type_id);
+/* Tests only: hook(arg) runs inside the string checks and lookups listed under zg_retire_unused_names, after they
+ * resolved their names and before they answer, with no lock held (NULL removes it). */
+int zg_debug_set_resolve_hook(zg_engine *e, void (*hook)(void *), void *arg);
 /* v1 ReadRelationships: matching live relationships as "type:id#rel@stype:sid[#srel]\n"
  * lines, sorted. Returns 0 or ZG_E2BIG (*need = bytes required incl. NUL). */
 int zg_read_relationships(zg_engine *e, const zg_filter_str *filter, char *buf, size_t cap,
@@ -277,8 +313,8 @@ int zg_check_bulk_device(zg_engine *e, const zg_check *d_items, uint64_t n, uint
 int zg_check_bulk_str(zg_engine *e, const zg_rel_str *items, uint64_t n, uint8_t *out);
 /* Only the resolution step of zg_check_bulk_str (strings -> interned checks; no GPU work, nothing is
  * interned: never-written names get the ZG_NO_OBJECT sentinels, unknown types / permissions give an
- * item that answers ZG_ITEM_ERROR). Lets a caller intern once and reuse the ids; they stay valid for
- * the life of the engine. */
+ * item that answers ZG_ITEM_ERROR). Lets a caller intern once and reuse the ids; they stay valid
+ * until zg_retire_unused_names retires their name. */
 int zg_resolve_checks(zg_engine *e, const zg_rel_str *items, uint64_t n, zg_check *out);
 /* Packed form for a bulk request whose items share their literal fields (one rule template evaluated per
  * item: pkg/authz/postfilter.go:88-110): the n resource ids are the byte ranges

@@ -157,6 +157,10 @@ _SIGS = {
     "zg_delete_relationships": (C.c_int, [C.c_void_p, C.POINTER(_RelStr), C.POINTER(_Precond), C.c_uint64,
                                           C.POINTER(C.c_uint64)]),
     "zg_collect_expired": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(C.c_uint64)]),
+    "zg_retire_unused_names": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint64)]),
+    "zg_name_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "zg_object_capacity": (C.c_uint64, [C.c_void_p, C.c_int]),
+    "zg_debug_set_resolve_hook": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "zg_read_relationships": (C.c_int, [C.c_void_p, C.POINTER(_RelStr), C.c_char_p, C.c_size_t,
                                         C.POINTER(C.c_size_t), C.POINTER(C.c_uint64)]),
     "zg_watch_read": (C.c_int, [C.c_void_p, C.c_uint64, C.c_char_p, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t),
@@ -392,6 +396,14 @@ class Engine:
 
     def find(self, type_name, object_id):
         return self._L.zg_find_object(self._h, self.type_id(type_name), _b(object_id))
+
+    def object_name(self, type_name, oid: int) -> str:
+        """zg_object_name: the name of id `oid`; ZgpuError(ZG_EINVAL) when it has none."""
+        buf = C.create_string_buffer(1 << 12)
+        rc = self._L.zg_object_name(self._h, self.type_id(type_name), oid, buf, len(buf))
+        if rc < 0:
+            self._ck(rc)
+        return buf.value.decode()
 
     # -- store ----------------------------------------------------------------
     def load_tuples(self, tuples: np.ndarray, expires: np.ndarray | None = None):
@@ -750,6 +762,33 @@ class Engine:
         out = np.zeros(len(self.FILTER_COUNTERS), dtype=np.uint64)
         self._ck(self._L.zg_filter_counters(self._h, out.ctypes.data))
         return {k: int(v) for k, v in zip(self.FILTER_COUNTERS, out)}
+
+    def retire_unused_names(self) -> int:
+        """zg_retire_unused_names: retires every interned name no relationship in the store and no retained watch
+        change mentions; returns how many. Their ids are handed to new names, lowest first."""
+        n = C.c_uint64(0)
+        self._ck(self._L.zg_retire_unused_names(self._h, C.byref(n)))
+        return n.value
+
+    NAME_COUNTERS = ("named", "retired", "free_ids", "id_extent", "arena_bytes", "retired_device", "retired_host")
+
+    def name_counters(self) -> dict:
+        """Interned names, retirements, free ids, the id extent and the host arena bytes (zg_name_counters)."""
+        out = np.zeros(len(self.NAME_COUNTERS), dtype=np.uint64)
+        self._ck(self._L.zg_name_counters(self._h, out.ctypes.data))
+        return {k: int(v) for k, v in zip(self.NAME_COUNTERS, out)}
+
+    _HOOK = C.CFUNCTYPE(None, C.c_void_p)
+
+    def set_resolve_hook(self, fn):
+        """Tests only (zg_debug_set_resolve_hook): fn() runs inside the string checks and lookups between resolving their
+        names and answering; None removes it."""
+        self._resolve_hook = None if fn is None else self._HOOK(lambda _arg: fn())
+        self._ck(self._L.zg_debug_set_resolve_hook(self._h, self._resolve_hook, None))
+
+    def object_capacity(self, type_name) -> int:
+        """The object capacity of a type in the last layout (zg_object_capacity)."""
+        return int(self._L.zg_object_capacity(self._h, self.type_id(type_name)))
 
     # -- sharded store (dist.DeviceShardedChecker drives these) --------------------
     # every pointer is a device address on this engine's GPU (ints, e.g. tensor.data_ptr())

@@ -179,7 +179,8 @@ struct zg_engine {
     bool leader_active = false;
   } lookups;
   // ZG_E2BIG protocol: recent answers are kept so that a caller's retry with a larger buffer (same arguments,
-  // same snapshot revision) does not recompute them
+  // same snapshot revision) does not recompute them. zg_retire_unused_names leaves them valid: every id in an answer is
+  // mentioned by a relationship at that revision, and only names no relationship mentions are retired.
   std::deque<std::pair<LookupKey, std::shared_ptr<const std::vector<uint32_t>>>> lookup_cache;
   static constexpr size_t kLookupCache = 128;
   HostSnapshot last_built;  // kept only for zg_debug_row / host-only engines
@@ -201,6 +202,16 @@ struct zg_engine {
   // zg_filter_counters: relationship filters (reads, deletes by filter, preconditions) answered from the snapshot on
   // the device and by Store::match, relationships the device returned, device filters by Device::FilterShape
   std::atomic<uint64_t> flt_device{0}, flt_host{0}, flt_returned{0}, flt_shape[3] = {};
+  // zg_name_counters: names retired by zg_retire_unused_names calls that read the mentions from the snapshots / from
+  // the host store (reset with the store by a schema load)
+  uint64_t retire_device = 0, retire_host = 0;
+  // Bumped by every zg_retire_unused_names call that retires a name, under the device lock and the exclusive names
+  // lock, before any freed id can be handed out again (with_stable_names).
+  std::atomic<uint64_t> name_epoch{0};
+  // zg_debug_set_resolve_hook: called by the string checks and lookups between resolving their names and answering
+  // (tests force a retirement and a reuse of the ids into that gap with it); nullptr = none
+  void (*resolve_hook)(void*) = nullptr;
+  void* resolve_hook_arg = nullptr;
   ~zg_engine() {
     if (group_pin) cudaFreeHost(group_pin);
   }
@@ -281,6 +292,21 @@ extern "C" size_t zg_last_error_copy(char* buf, size_t cap) {
     buf[m] = 0;
   }
   return n;
+}
+
+// The string calls resolve names under the shared names lock, release it, and answer later: a check queued for the
+// batcher, a lookup whose ids are turned back into names under the lock again. A retirement in between may free a
+// resolved name and hand its id to a new name, so the call would answer for, or print, the other name. Runs `call`
+// until no retirement happened between its start and its end (a retirement bumps name_epoch before any freed id can
+// be reused): then every id it resolved denoted the same name until it answered. A retry redoes the whole call.
+template <class F>
+static int with_stable_names(zg_engine* e, F&& call) {
+  if (!e) return call();
+  for (;;) {
+    const uint64_t epoch = e->name_epoch.load();
+    const int rc = call();
+    if (e->name_epoch.load() == epoch) return rc;
+  }
 }
 
 static uint32_t now_of(const zg_engine* e) {
@@ -423,6 +449,8 @@ extern "C" int zg_load_schema(zg_engine* e, const char* dsl, size_t len) {
   e->schema = std::move(s);
   e->has_schema = true;
   e->store.reset(&e->schema);
+  e->retire_device = e->retire_host = 0;  // with the store's count of retired names
+  ++e->name_epoch;                        // every name is gone
   if (!is_handle(e)) {  // a sharded handle's store holds every shard's relationships
     e->store.shard_count = e->dev.shard_count;
     e->store.shard_rank = e->dev.shard_rank;
@@ -969,6 +997,85 @@ extern "C" int zg_collect_expired(zg_engine* e, int64_t before_unix, uint64_t* n
   return delete_found(e, "collect expired", on_device ? &found : nullptr, &idx, &u, &changed, n_removed);
 }
 
+extern "C" int zg_retire_unused_names(zg_engine* e, uint64_t* n_retired) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (n_retired) *n_retired = 0;
+  LOCK_DEVICE(e);
+  LOCK_NAMES_UNIQUE(e);
+  if (e->store.shard_count > 1)
+    return fail(ZG_EINVAL, "retire unused names: this engine is one shard of several (zg_config.shard_count) and its store "
+                           "does not hold the other shards' relationships");
+  // Which ids some relationship of the store names: read from the snapshots when they are the store (every shard of a
+  // sharded handle scans its own; replicas hold the same snapshot, so the first device answers), else from the store.
+  Store::IdBits keep;
+  const bool on_device = filters_on_device(e);
+  if (on_device) {
+    const uint32_t S = is_handle(e) ? e->n_shards : 1;
+    std::vector<Store::IdBits> got(S);
+    std::vector<int> rcs(S, ZG_OK);
+    std::vector<std::string> errs(S);
+    auto one = [&](Device& dev, size_t k) { rcs[k] = dev.scan_mentions(e->schema, &got[k], &errs[k]); };
+    if (S == 1) one(e->dev, 0);
+    else on_all_devices(e, one);
+    std::string err;
+    if (int rc = first_error(rcs, errs, &err)) return fail(rc == ZG_ENOMEM ? ZG_ECUDA : rc, err);
+    keep.swap(got[0]);
+    for (uint32_t k = 1; k < S; ++k)
+      for (size_t t = 0; t < got[k].size(); ++t) {
+        if (keep[t].size() < got[k][t].size()) keep[t].resize(got[k][t].size(), 0);
+        for (size_t w = 0; w < got[k][t].size(); ++w) keep[t][w] |= got[k][t][w];
+      }
+  } else {
+    e->store.mentioned(&keep);
+  }
+  // zg_watch_read renders the retained changes' names when it is called: their ids keep their names
+  for (const auto& w : e->watch_log) {
+    Store::mark(&keep, e->schema.slots[w.t.rel].type, w.t.res);
+    if (w.t.srel != kWildcard) Store::mark(&keep, w.t.stype, w.t.subj);
+  }
+  const uint64_t n = e->store.retire(keep);
+  if (n) {
+    // the device mirrors of the names hold the retired records: they are rebuilt by the next device-ingress call
+    e->dev.ingress_reset();
+    for (auto& r : e->replicas) r->dev.ingress_reset();
+    if (on_device) e->retire_device += n;
+    else e->retire_host += n;
+    ++e->name_epoch;
+  }
+  if (n_retired) *n_retired = n;
+  return ZG_OK;
+}
+
+extern "C" int zg_debug_set_resolve_hook(zg_engine* e, void (*hook)(void*), void* arg) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  LOCK_DEVICE(e);
+  LOCK_NAMES_UNIQUE(e);
+  e->resolve_hook = hook;
+  e->resolve_hook_arg = arg;
+  return ZG_OK;
+}
+
+extern "C" int zg_name_counters(zg_engine* e, uint64_t* out) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (!out) return fail(ZG_EINVAL, "out is NULL");
+  LOCK_NAMES_SHARED(e);
+  const Store::NameCounts c = e->store.name_counts();
+  out[0] = c.named;
+  out[1] = e->store.retired_names;
+  out[2] = c.free_ids;
+  out[3] = c.extent;
+  out[4] = c.arena_bytes;
+  out[5] = e->retire_device;
+  out[6] = e->retire_host;
+  return ZG_OK;
+}
+
+extern "C" uint64_t zg_object_capacity(const zg_engine* e, int type_id) {
+  NEED_SCHEMA(e, 0);
+  LOCK_NAMES_SHARED(e);
+  return e->store.capacity(type_id);
+}
+
 static std::string tuple_text(const zg_engine* e, const zg_tuple& t) {
   const Schema& sc = e->schema;
   const SlotInfo& rel = sc.slots[t.rel];
@@ -1005,7 +1112,7 @@ extern "C" int zg_read_relationships(zg_engine* e, const zg_filter_str* filter, 
     uint64_t count = 0;
     bool too_big = false;
     if (int rc = match_on_device(e, f, now_of(e), &count, &found, &too_big)) return rc;
-    if (too_big) {  // writers wait for the device lock held here, and object ids never change: f stays resolved
+    if (too_big) {  // writers and retirements wait for the device lock held here: f stays resolved
       on_device = false;
       shared.unlock();
       exclusive.lock();
@@ -1598,9 +1705,9 @@ extern "C" int zg_resolve_checks_packed(zg_engine* e, const char* res_type, cons
   return resolve_packed_locked(e, res_type, relation, subj_type, subj_rel, res_ids, res_off, subj_ids, subj_off, n, out);
 }
 
-extern "C" int zg_check_bulk_packed(zg_engine* e, const char* res_type, const char* relation, const char* subj_type,
-                                    const char* subj_rel, const char* res_ids, const uint32_t* res_off, const char* subj_ids,
-                                    const uint32_t* subj_off, uint64_t n, uint8_t* out) {
+static int check_bulk_packed_once(zg_engine* e, const char* res_type, const char* relation, const char* subj_type,
+                                  const char* subj_rel, const char* res_ids, const uint32_t* res_off, const char* subj_ids,
+                                  const uint32_t* subj_off, uint64_t n, uint8_t* out) {
   NEED_SCHEMA(e, ZG_ENOSCHEMA);
   if (!PACKED_ARGS_OK()) return fail(ZG_EINVAL, "NULL argument");
   if (n == 0) return ZG_OK;
@@ -1612,10 +1719,20 @@ extern "C" int zg_check_bulk_packed(zg_engine* e, const char* res_type, const ch
     rc = resolve_packed_locked(e, res_type, relation, subj_type, subj_rel, res_ids, res_off, subj_ids, subj_off, n, c.data());
     if (rc) return rc;
   }
+  if (e->resolve_hook) e->resolve_hook(e->resolve_hook_arg);
   return zg_check_bulk(e, c.data(), n, out);
 }
 
-extern "C" int zg_check_bulk_str(zg_engine* e, const zg_rel_str* items, uint64_t n, uint8_t* out) {
+extern "C" int zg_check_bulk_packed(zg_engine* e, const char* res_type, const char* relation, const char* subj_type,
+                                    const char* subj_rel, const char* res_ids, const uint32_t* res_off, const char* subj_ids,
+                                    const uint32_t* subj_off, uint64_t n, uint8_t* out) {
+  return with_stable_names(e, [&] {
+    return check_bulk_packed_once(e, res_type, relation, subj_type, subj_rel, res_ids, res_off, subj_ids, subj_off,
+                                  n, out);
+  });
+}
+
+static int check_bulk_str_once(zg_engine* e, const zg_rel_str* items, uint64_t n, uint8_t* out) {
   NEED_SCHEMA(e, ZG_ENOSCHEMA);
   if ((!items || !out) && n) return fail(ZG_EINVAL, "NULL argument");
   std::vector<zg_check> c(n);
@@ -1625,10 +1742,15 @@ extern "C" int zg_check_bulk_str(zg_engine* e, const zg_rel_str* items, uint64_t
     LOCK_NAMES_SHARED(e);
     resolve_checks_locked(e, items, n, c.data());
   }
-  // Interned ids stay valid across later writes (interning only appends), so the launch can go
-  // through the batcher like any zg_check_bulk call: concurrent string callers -- one goroutine per
-  // rule check in the proxy, pkg/authz/check.go:77-93 -- share launches too.
+  // The launch goes through the batcher like any zg_check_bulk call, after the names lock is released: concurrent
+  // string callers -- one goroutine per rule check in the proxy, pkg/authz/check.go:77-93 -- share launches too. Ids
+  // keep their names across writes; a retirement in between is caught by zg_check_bulk_str (with_stable_names).
+  if (e->resolve_hook) e->resolve_hook(e->resolve_hook_arg);
   return zg_check_bulk(e, c.data(), n, out);
+}
+
+extern "C" int zg_check_bulk_str(zg_engine* e, const zg_rel_str* items, uint64_t n, uint8_t* out) {
+  return with_stable_names(e, [&] { return check_bulk_str_once(e, items, n, out); });
 }
 
 // ---- device ingress: packed ids resolved on the GPU against a mirror of the interned names ----------
@@ -1862,8 +1984,8 @@ extern "C" int zg_list_resolve(zg_engine* e, const char* body, size_t len, const
   return ZG_OK;
 }
 
-extern "C" int zg_list_postfilter(zg_engine* e, const char* body, size_t len, const zg_list_template* tpl, uint32_t n_tpl,
-                                  char* out, size_t cap, size_t* out_len) {
+static int list_postfilter_once(zg_engine* e, const char* body, size_t len, const zg_list_template* tpl, uint32_t n_tpl,
+                                char* out, size_t cap, size_t* out_len) {
   NEED_SCHEMA(e, ZG_ENOSCHEMA);
   if (!body || !out_len || (!tpl && n_tpl)) return fail(ZG_EINVAL, "NULL argument");
   auto passthrough = [&]() {
@@ -1916,6 +2038,11 @@ extern "C" int zg_list_postfilter(zg_engine* e, const char* body, size_t len, co
   }
   int rc = zg_list_filter(body, len, items.get(), N, keep.data(), ib, ie, ZG_LIST_EMPTY_AS_NULL, out, cap, out_len);
   return rc == ZG_EINVAL ? fail(rc, "zg_list_filter: inconsistent item ranges") : rc;
+}
+
+extern "C" int zg_list_postfilter(zg_engine* e, const char* body, size_t len, const zg_list_template* tpl, uint32_t n_tpl,
+                                  char* out, size_t cap, size_t* out_len) {
+  return with_stable_names(e, [&] { return list_postfilter_once(e, body, len, tpl, n_tpl, out, cap, out_len); });
 }
 
 // LookupResources on a sharded handle (ZG_FLAG_HANDLE_LOOKUPS): one round of dist.DeviceShardedLookup._round over
@@ -2340,9 +2467,9 @@ static int resolve_lookup_strs(zg_engine* e, const char* res_type, const char* p
   return ZG_OK;
 }
 
-extern "C" int zg_lookup_resources_str(zg_engine* e, const char* res_type, const char* perm, const char* subj_type,
-                                       const char* subj_id, const char* subj_rel, char* buf, size_t cap, size_t* need,
-                                       uint64_t* n_out) {
+static int lookup_resources_str_once(zg_engine* e, const char* res_type, const char* perm, const char* subj_type,
+                                     const char* subj_id, const char* subj_rel, char* buf, size_t cap, size_t* need,
+                                     uint64_t* n_out) {
   NEED_SCHEMA(e, ZG_ENOSCHEMA);
   if (!res_type || !perm || !subj_type || !subj_id) return fail(ZG_EINVAL, "NULL argument");
   int rt, p, st;
@@ -2355,6 +2482,7 @@ extern "C" int zg_lookup_resources_str(zg_engine* e, const char* res_type, const
   rc = lookup_queued(e, static_cast<uint16_t>(rt), static_cast<uint16_t>(p), static_cast<uint16_t>(st),
                      su == ZG_NO_OBJECT ? ZG_NO_OBJECT - 1 : su, sr, &ids, &self_member);
   if (rc) return rc;
+  if (e->resolve_hook) e->resolve_hook(e->resolve_hook_arg);
   std::vector<std::string> names;
   {
     LOCK_NAMES_SHARED(e);
@@ -2378,6 +2506,14 @@ extern "C" int zg_lookup_resources_str(zg_engine* e, const char* res_type, const
   }
   buf[w] = 0;
   return ZG_OK;
+}
+
+extern "C" int zg_lookup_resources_str(zg_engine* e, const char* res_type, const char* perm, const char* subj_type,
+                                       const char* subj_id, const char* subj_rel, char* buf, size_t cap, size_t* need,
+                                       uint64_t* n_out) {
+  return with_stable_names(e, [&] {
+    return lookup_resources_str_once(e, res_type, perm, subj_type, subj_id, subj_rel, buf, cap, need, n_out);
+  });
 }
 
 // ---- LookupSubjects --------------------------------------------------------------------------
@@ -2651,9 +2787,9 @@ extern "C" int zg_lookup_subjects(zg_engine* e, uint16_t perm, uint32_t res, uin
   return ZG_OK;
 }
 
-extern "C" int zg_lookup_subjects_str(zg_engine* e, const char* res_type, const char* res_id, const char* perm,
-                                      const char* subj_type, const char* subj_rel, uint32_t wildcard_option, char* buf,
-                                      size_t cap, size_t* need, uint64_t* n_out) {
+static int lookup_subjects_str_once(zg_engine* e, const char* res_type, const char* res_id, const char* perm,
+                                    const char* subj_type, const char* subj_rel, uint32_t wildcard_option, char* buf,
+                                    size_t cap, size_t* need, uint64_t* n_out) {
   NEED_SCHEMA(e, ZG_ENOSCHEMA);
   if (!res_type || !res_id || !perm || !subj_type) return fail(ZG_EINVAL, "NULL argument");
   int rt, p, st;
@@ -2687,6 +2823,7 @@ extern "C" int zg_lookup_subjects_str(zg_engine* e, const char* res_type, const 
     rc = lookup_subjects_ids(e, static_cast<uint16_t>(p), res, static_cast<uint16_t>(st), sr, wildcard_option, &ans);
     if (rc) return rc;
   }
+  if (e->resolve_hook) e->resolve_hook(e->resolve_hook_arg);
   // lines: concrete ids, then "*" and one "!<id>" per exclusion ('!' is outside SpiceDB's object-id charset)
   std::vector<std::string> lines;
   {
@@ -2714,6 +2851,15 @@ extern "C" int zg_lookup_subjects_str(zg_engine* e, const char* res_type, const 
   }
   buf[w] = 0;
   return ZG_OK;
+}
+
+extern "C" int zg_lookup_subjects_str(zg_engine* e, const char* res_type, const char* res_id, const char* perm,
+                                      const char* subj_type, const char* subj_rel, uint32_t wildcard_option, char* buf,
+                                      size_t cap, size_t* need, uint64_t* n_out) {
+  return with_stable_names(e, [&] {
+    return lookup_subjects_str_once(e, res_type, res_id, perm, subj_type, subj_rel, wildcard_option, buf, cap, need,
+                                    n_out);
+  });
 }
 
 extern "C" int zg_lookup_subjects_counters(zg_engine* e, uint64_t* out) {
@@ -2850,8 +2996,8 @@ extern "C" int zg_list_keep_allowed(zg_engine* e, const char* body, size_t len, 
   return ZG_OK;
 }
 
-extern "C" int zg_list_prefilter(zg_engine* e, const char* body, size_t len, uint32_t mode, const zg_list_template* tpl,
-                                 char* out, size_t cap, size_t* out_len) {
+static int list_prefilter_once(zg_engine* e, const char* body, size_t len, uint32_t mode, const zg_list_template* tpl,
+                               char* out, size_t cap, size_t* out_len) {
   NEED_SCHEMA(e, ZG_ENOSCHEMA);
   if (!body || !out_len || !tpl) return fail(ZG_EINVAL, "NULL argument");
   if (!tpl->res_type || !tpl->permission || !tpl->subj_type || !tpl->subj_id) return fail(ZG_EINVAL, "NULL template field");
@@ -2910,6 +3056,11 @@ extern "C" int zg_list_prefilter(zg_engine* e, const char* body, size_t len, uin
   if (rc) return rc;
   rc = zg_list_filter(body, len, items.get(), N, keep.data(), ib, ie, 0, out, cap, out_len);
   return rc == ZG_EINVAL ? fail(rc, "zg_list_filter: inconsistent item ranges") : rc;
+}
+
+extern "C" int zg_list_prefilter(zg_engine* e, const char* body, size_t len, uint32_t mode, const zg_list_template* tpl,
+                                 char* out, size_t cap, size_t* out_len) {
+  return with_stable_names(e, [&] { return list_prefilter_once(e, body, len, mode, tpl, out, cap, out_len); });
 }
 
 extern "C" int zg_stats_get(zg_engine* e, zg_stats* out) {

@@ -93,7 +93,7 @@ Device::~Device() {
   rb_cand_.release();
   for (auto* b : {&lb_params_, &lb_owner_, &lb_ctrl_, &lb_keys_[0], &lb_keys_[1]}) b->release();
   for (auto* b : {&ls_jobs_, &ls_codes_, &ls_has_, &ls_ids_, &ls_ctrl_}) b->release();
-  for (auto* b : {&flt_out_, &flt_exp_, &flt_ctrl_}) b->release();
+  for (auto* b : {&flt_out_, &flt_exp_, &flt_ctrl_, &mention_bits_}) b->release();
   for (auto& l : pl_)
     for (auto* b : {&l.in, &l.val, &l.out, &l.raised, &l.parent, &l.pos}) b->release();
   for (auto* b : {&home_, &home_pos_, &home_out_, &peer_ctrl_}) b->release();
@@ -2595,6 +2595,47 @@ int Device::run_filter(const Schema& sc, const Snapshot& s, const std::vector<Fi
   return ZG_OK;
 }
 
+int Device::scan_mentions(const Schema& sc, Store::IdBits* bits, std::string* err) {
+  std::shared_ptr<Snapshot> s = snap;
+  if (!s) {
+    if (err) *err = "no snapshot published";
+    return ZG_ENOSNAPSHOT;
+  }
+  std::vector<MentionType> types;
+  const uint64_t words = mention_types(sc, s->rels, s->cls, s->n_objects, &types);
+  if (bits->size() < types.size()) bits->resize(types.size());
+  if (words == 0) return ZG_OK;
+  ZG_CUDA(cudaSetDevice(device));
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  if (!mention_bits_.ensure(words * 4)) {
+    if (err) *err = "out of device memory (mention bitmaps)";
+    return ZG_ENOMEM;
+  }
+  MentionPlan p{};
+  p.row_ptr = s->row_ptr.as<uint32_t>();
+  p.rrow_ptr = s->rrow_ptr.as<uint32_t>();
+  p.bits = mention_bits_.as<uint32_t>();
+  const uint64_t want = (words + kFilterThreads / 32 - 1) / (kFilterThreads / 32);
+  const unsigned grid = static_cast<unsigned>(std::max<uint64_t>(1, std::min<uint64_t>(want, uint64_t(sm_count_) * 8)));
+  for (size_t at = 0; at < types.size(); at += kMaxMentionTypes) {
+    p.n_types = static_cast<uint32_t>(std::min<size_t>(kMaxMentionTypes, types.size() - at));
+    std::copy(types.begin() + at, types.begin() + at + p.n_types, p.type);
+    mention_scan_kernel<<<grid, kFilterThreads, 0, stream>>>(p);
+    ++launches;
+  }
+  ZG_CUDA(cudaGetLastError());
+  std::vector<uint32_t> host(words);
+  ZG_CUDA(cudaMemcpyAsync(host.data(), p.bits, words * 4, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  for (size_t t = 0; t < types.size(); ++t) {
+    const uint64_t n = (uint64_t(types[t].n_ids) + 31) / 32;
+    std::vector<uint32_t>& b = (*bits)[t];
+    if (b.size() < n) b.resize(n, 0);
+    for (uint64_t i = 0; i < n; ++i) b[i] |= host[types[t].word0 + i];
+  }
+  return ZG_OK;
+}
+
 // ---- device ingress ----------------------------------------------------------------------------
 
 IngressMirror::~IngressMirror() {
@@ -2616,7 +2657,8 @@ static unsigned ingress_grid(uint64_t n, int sm_count) {
   return static_cast<unsigned>(std::max<uint64_t>(1, std::min<uint64_t>(want, uint64_t(std::max(sm_count, 1)) * 16)));
 }
 
-// Names are append-only between schema loads, so the mirror only ever uploads the arena bytes it has not seen.
+// Names are appended between schema loads, so the mirror only ever uploads the arena bytes it has not seen. A
+// retirement rewrites the arena; zg_retire_unused_names then drops the mirror (ingress_reset) and the next call rebuilds it.
 int Device::ingress_sync(const Store& store, cudaStream_t st, std::string* err) {
   constexpr uint64_t kMinTable = 1024;
   if (!ingress_) ingress_.reset(new IngressMirror());

@@ -299,6 +299,10 @@ class Device {
   // with CF_EXPIRY are read. A count launch that finds nothing is the whole call.
   int match_expired(const Schema& sc, uint32_t before, uint64_t* count, std::vector<zg_tuple>* tuples, bool* too_big,
                     std::string* err);
+  // zg_retire_unused_names: per type, one bit per id of the snapshot's object capacity, set where a relationship of
+  // the snapshot names the id as its resource or its subject (filter.cuh mention_scan_kernel); OR-ed into *bits
+  // (Store::IdBits, grown to the capacities). One launch per 64 types, one copy back.
+  int scan_mentions(const Schema& sc, Store::IdBits* bits, std::string* err);
 
   // ---- device ingress (ingress.cuh): packed string ids -> interned checks against the mirror of the store's names ----
   // The literal fields of a packed call, resolved once on the host exactly as zg_resolve_checks_packed resolves them.
@@ -374,6 +378,7 @@ class Device {
   DevBuf lb_params_, lb_owner_, lb_ctrl_, lb_keys_[2];  // batched lookups
   DevBuf ls_jobs_, ls_codes_, ls_has_, ls_ids_, ls_ctrl_;   // LookupSubjects
   DevBuf flt_out_, flt_exp_, flt_ctrl_;                     // match_filter: records, expirations, the count
+  DevBuf mention_bits_;                                     // scan_mentions: every type's bitmap
   // sharded LookupResources round: walk state in rb_visited_ / lk_jobs_ / lb_owner_ / lb_params_ / lb_keys_ (a sharded
   // engine never runs lookup_batch), the round's home ranks, self-membership list and control words here
   DevBuf sl_home_, sl_self_, sl_ctrl_;

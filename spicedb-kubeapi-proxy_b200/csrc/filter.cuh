@@ -19,8 +19,10 @@
 #include <cuda_runtime.h>
 #endif
 #include <cstdint>
+#include <vector>
 
 #include "../../include/zgpu.h"
+#include "schema.h"
 
 namespace zg {
 
@@ -200,6 +202,87 @@ __global__ void __launch_bounds__(kFilterThreads) filter_scan_kernel(const Filte
 template <bool kEmit>
 __global__ void __launch_bounds__(kFilterThreads) filter_expired_kernel(const FilterPlan p) {
   filter_scan<kEmit, true>(p);
+}
+
+// ---- which ids the snapshot mentions (zg_retire_unused_names) ----
+// An id of type T is mentioned when some relationship names it as its resource or as its subject. The forward rows of
+// object o (every class of T's relations) sit together at fwd_base + o * fwd_stride, its reverse rows (every class T
+// can be a subject of, wildcard classes aside) at rev_base + o * rev_stride (DESIGN §3), so "o has a non-empty row" is
+// one difference of two offsets per direction. A warp covers 32 ids, one per lane, and its ballot is their bitmap
+// word: every word is written once, with no atomics. Expired entries still mention their ids; wildcard rows mention
+// none (their single reverse row lies outside every type's block, their forward entries name only the resource).
+// Device::scan_mentions plans from the snapshot's layout (mention_types) and ORs the bitmaps of a sharded handle's
+// shards; Store::mentioned builds the same bitmaps from the relationship list.
+constexpr int kMaxMentionTypes = 64;  // types per launch; a schema with more runs several launches
+
+struct MentionType {
+  unsigned long long fwd_base;  // row_ptr index of (object 0, the type's first class)
+  unsigned long long rev_base;  // rrow_ptr index of (object 0, the first class the type is a subject of)
+  unsigned long long word0;     // the type's first word of `bits`
+  uint32_t n_ids;               // the type's object capacity: bits cover ceil(n_ids / 32) words
+  uint32_t fwd_stride;          // classes of the type's relations; 0: the type has none
+  uint32_t rev_stride;          // classes the type is a subject of; 0: none
+  uint32_t pad;
+};
+
+struct MentionPlan {
+  const uint32_t *row_ptr, *rrow_ptr;
+  uint32_t* bits;
+  uint32_t n_types;
+  MentionType type[kMaxMentionTypes];
+};
+
+__global__ void __launch_bounds__(kFilterThreads) mention_scan_kernel(const MentionPlan p) {
+  const unsigned lane = threadIdx.x & 31;
+  const unsigned long long w = (blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x) >> 5;
+  const unsigned long long n_warps = (static_cast<unsigned long long>(gridDim.x) * blockDim.x) >> 5;
+  for (uint32_t k = 0; k < p.n_types; ++k) {
+    const MentionType& t = p.type[k];
+    const unsigned long long words = (static_cast<unsigned long long>(t.n_ids) + 31) >> 5;
+    for (unsigned long long wd = w; wd < words; wd += n_warps) {
+      const unsigned long long o = wd * 32 + lane;
+      bool hit = false;
+      if (o < t.n_ids) {
+        if (t.fwd_stride) {
+          const unsigned long long r = t.fwd_base + o * t.fwd_stride;
+          hit = __ldg(p.row_ptr + r + t.fwd_stride) != __ldg(p.row_ptr + r);
+        }
+        if (!hit && t.rev_stride) {
+          const unsigned long long r = t.rev_base + o * t.rev_stride;
+          hit = __ldg(p.rrow_ptr + r + t.rev_stride) != __ldg(p.rrow_ptr + r);
+        }
+      }
+      const unsigned word = __ballot_sync(kFilterFull, hit);
+      if (lane == 0) p.bits[t.word0 + wd] = word;
+    }
+  }
+}
+
+// The plan of every type of a snapshot's layout (its rels, cls and object capacities), bitmaps back to back in type
+// order. Returns the words they take. A type's first relation starts its forward block (Store::layout hands out the
+// rows of a type's relations in order), and its reverse block starts at the least rrow_base of its classes.
+inline uint64_t mention_types(const Schema& sc, const std::vector<DRel>& rels, const std::vector<DCls>& cls,
+                              const std::vector<uint32_t>& n_objects, std::vector<MentionType>* out) {
+  out->assign(n_objects.size(), MentionType{});
+  uint64_t words = 0;
+  for (size_t t = 0; t < n_objects.size(); ++t) {
+    MentionType& m = (*out)[t];
+    m.n_ids = n_objects[t];
+    m.word0 = words;
+    words += (uint64_t(n_objects[t]) + 31) / 32;
+    for (size_t ri = 0; ri < sc.rel_slots.size() && ri < rels.size(); ++ri)
+      if (sc.slots[sc.rel_slots[ri]].type == static_cast<int>(t)) {
+        m.fwd_base = rels[ri].row_base;
+        m.fwd_stride = rels[ri].stride;
+        break;
+      }
+    for (const DCls& c : cls)
+      if (c.stype == t && c.sslot != kWildcard && (!m.rev_stride || c.rrow_base < m.rev_base)) {
+        m.rev_base = c.rrow_base;
+        m.rev_stride = c.rstride;
+      }
+  }
+  return words;
 }
 
 }  // namespace zg

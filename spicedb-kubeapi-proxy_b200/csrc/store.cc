@@ -20,6 +20,7 @@ void Store::reset(const Schema* s) {
   index_.clear();
   indexed_ = true;
   live_ = 0;
+  retired_names = 0;
 }
 
 void Store::clear_relationships() {
@@ -49,15 +50,16 @@ uint32_t Store::TypeObjs::lookup(const char* s, size_t n) const {
   }
 }
 
+void Store::TypeObjs::place(uint64_t off) {
+  uint32_t id, len;
+  rec_read(arena, off, &id, &len);
+  const size_t mask = table.size() - 1;
+  size_t i = hash_bytes(arena.data() + off + 8, len) & mask;
+  while (table[i]) i = (i + 1) & mask;
+  table[i] = off + 1;
+}
+
 void Store::TypeObjs::insert(uint64_t rec) {
-  auto place = [&](uint64_t off) {
-    uint32_t id, len;
-    rec_read(arena, off, &id, &len);
-    const size_t mask = table.size() - 1;
-    size_t i = hash_bytes(arena.data() + off + 8, len) & mask;
-    while (table[i]) i = (i + 1) & mask;
-    table[i] = off + 1;
-  };
   if ((n_interned + 1) * 2 > table.size()) {  // grow and re-index from the records
     std::vector<uint64_t> old;
     old.swap(table);
@@ -73,9 +75,9 @@ uint32_t Store::intern(int type, const std::string& id) {
   TypeObjs& t = objs_[type];
   const uint32_t have = t.lookup(id.data(), id.size());
   if (have != ZG_NO_OBJECT) return have;
-  // keep string ids and bulk numeric ids in one id space
-  const uint32_t nid = std::max<uint32_t>(t.n_ids(), t.n_numeric);
-  t.rec_of.resize(nid + 1, 0);
+  // keep string ids and bulk numeric ids in one id space; the ids of retired names go first, lowest first
+  const uint32_t nid = t.n_free ? t.take_free() : std::max<uint32_t>(t.n_ids(), t.n_numeric);
+  if (nid >= t.n_ids()) t.rec_of.resize(nid + 1, 0);
   const uint64_t rec = t.arena.size();
   const uint32_t len = static_cast<uint32_t>(id.size());
   t.arena.resize(rec + 8 + len);
@@ -142,9 +144,11 @@ std::string Store::load(const zg_tuple* t, const uint32_t* ex, uint64_t n) {
     if (x.srel == kWildcard) x.subj = 0;
     TypeObjs& rt = objs_[schema->slots[x.rel].type];
     if (x.res + 1 > rt.n_numeric) rt.n_numeric = x.res + 1;
+    rt.claim(x.res);
     if (x.srel != kWildcard) {
       TypeObjs& st = objs_[x.stype];
       if (x.subj + 1 > st.n_numeric) st.n_numeric = x.subj + 1;
+      st.claim(x.subj);
     }
     if (shard_count > 1 && x.res % shard_count != shard_rank) continue;  // another shard owns it
     tuples.push_back(x);
@@ -234,9 +238,11 @@ std::string Store::apply(const zg_update* u, uint64_t n, int* code, std::vector<
     ++live_;
     TypeObjs& rt = objs_[schema->slots[t.rel].type];
     if (t.res + 1 > rt.n_numeric) rt.n_numeric = t.res + 1;
+    rt.claim(t.res);
     if (t.srel != kWildcard) {
       TypeObjs& st = objs_[t.stype];
       if (t.subj + 1 > st.n_numeric) st.n_numeric = t.subj + 1;
+      st.claim(t.subj);
     }
   }
   // compact tombstones when they dominate
@@ -293,6 +299,95 @@ void Store::expired(uint32_t before, std::vector<uint64_t>* idx) {
   ensure_index();
   for (uint64_t i = 0; i < tuples.size(); ++i)
     if (!(tuples[i].flags & 1) && expires[i] != 0 && expires[i] <= before) idx->push_back(i);
+}
+
+void Store::mark(IdBits* bits, int type, uint32_t id) {
+  std::vector<uint32_t>& b = (*bits)[type];
+  if ((id >> 5) >= b.size()) b.resize((id >> 5) + 1, 0);
+  b[id >> 5] |= 1u << (id & 31);
+}
+
+void Store::mentioned(IdBits* bits) const {
+  bits->assign(objs_.size(), {});
+  for (size_t t = 0; t < objs_.size(); ++t)
+    (*bits)[t].assign((std::max<uint32_t>(objs_[t].n_ids(), objs_[t].n_numeric) + 31) / 32, 0);
+  for (const zg_tuple& t : tuples) {  // a duplicate of a bulk load names the same ids as the copy it folds into
+    if (t.flags & 1) continue;
+    mark(bits, schema->slots[t.rel].type, t.res);
+    if (t.srel != kWildcard) mark(bits, t.stype, t.subj);
+  }
+}
+
+uint32_t Store::TypeObjs::take_free() {
+  while (!free_bits[free_word]) ++free_word;
+  const uint32_t b = static_cast<uint32_t>(__builtin_ctz(free_bits[free_word]));
+  free_bits[free_word] &= ~(1u << b);
+  --n_free;
+  return free_word * 32 + b;
+}
+
+uint64_t Store::retire(const IdBits& keep) {
+  uint64_t total = 0;
+  for (size_t ty = 0; ty < objs_.size(); ++ty) {
+    TypeObjs& t = objs_[ty];
+    const std::vector<uint32_t>* k = ty < keep.size() ? &keep[ty] : nullptr;
+    const uint32_t n = t.n_ids();
+    t.free_bits.resize((n + 31) / 32, 0);
+    uint32_t gone = 0, first_word = ~0u;
+    for (uint32_t w = 0; w * 32 < n; ++w) {
+      uint32_t named = 0;
+      for (uint32_t b = 0; b < 32 && w * 32 + b < n; ++b)
+        if (t.rec_of[w * 32 + b]) named |= 1u << b;
+      uint32_t drop = named & ~(k && w < k->size() ? (*k)[w] : 0u);
+      if (!drop) continue;
+      first_word = std::min(first_word, w);
+      t.free_bits[w] |= drop;
+      for (; drop; drop &= drop - 1) {
+        t.rec_of[w * 32 + static_cast<uint32_t>(__builtin_ctz(drop))] = 0;
+        ++gone;
+      }
+    }
+    if (!gone) continue;
+    // the arena keeps only the records rec_of still points at, in their old order; ids do not move
+    std::vector<char> arena;
+    arena.reserve(t.arena.size());
+    for (uint64_t off = 0; off < t.arena.size();) {
+      uint32_t id, len;
+      rec_read(t.arena, off, &id, &len);
+      if (t.rec_of[id] == off + 1) {
+        t.rec_of[id] = arena.size() + 1;
+        arena.insert(arena.end(), t.arena.begin() + off, t.arena.begin() + off + 8 + len);
+      }
+      off += 8 + len;
+    }
+    t.arena.swap(arena);
+    t.n_interned -= gone;
+    size_t cap = 64;
+    while (cap < uint64_t(t.n_interned) * 2 + 2) cap *= 2;
+    t.table.assign(cap, 0);
+    for (uint64_t off = 0; off < t.arena.size();) {
+      t.place(off);
+      uint32_t len;
+      std::memcpy(&len, t.arena.data() + off + 4, 4);
+      off += 8 + len;
+    }
+    t.n_free += gone;
+    t.free_word = std::min(t.free_word, first_word);
+    total += gone;
+  }
+  retired_names += total;
+  return total;
+}
+
+Store::NameCounts Store::name_counts() const {
+  NameCounts c;
+  for (const TypeObjs& t : objs_) {
+    c.named += t.n_interned;
+    c.free_ids += t.n_free;
+    c.extent += std::max<uint32_t>(t.n_ids(), t.n_numeric);
+    c.arena_bytes += t.arena.size();
+  }
+  return c;
 }
 
 HostSnapshot Store::layout() const {

@@ -62,10 +62,27 @@ class Store {
   // false for a numeric-only object (bulk loads) or an id out of range
   bool name(int type, uint32_t id, std::string_view* out) const;
   // Read-only view of a type's interned names, for the device mirror (ingress.cuh): the records
-  // [u32 id][u32 len][bytes] back to back (append-only until reset) and how many there are.
+  // [u32 id][u32 len][bytes] back to back (appended to; rewritten only by retire() and reset) and how many there are.
   size_t n_types() const { return objs_.size(); }
   const std::vector<char>& name_arena(int type) const { return objs_[type].arena; }
   uint32_t n_interned(int type) const { return objs_[type].n_interned; }
+
+  // ---- retiring names no relationship mentions (zg_retire_unused_names) ----
+  // Per type, one bit per id: set where a live or expired relationship of the store names the id as its resource or
+  // its subject (what Device::scan_mentions reads from a snapshot of this store). Bitmaps cover the id extent.
+  using IdBits = std::vector<std::vector<uint32_t>>;
+  void mentioned(IdBits* bits) const;
+  static void mark(IdBits* bits, int type, uint32_t id);
+  // Retires every name whose bit in `keep` is clear (bits past a bitmap's end are clear): the record leaves the
+  // type's arena, which is rewritten with the kept records (ids unchanged) and its table rebuilt; the id goes on the
+  // type's free list, which intern() hands out lowest first. Numeric-only ids are never touched. Returns how many.
+  uint64_t retire(const IdBits& keep);
+  uint64_t retired_names = 0;  // since reset()
+  struct NameCounts {
+    uint64_t named = 0, free_ids = 0, extent = 0, arena_bytes = 0;
+  };
+  NameCounts name_counts() const;
+  uint32_t capacity(int type) const { return type >= 0 && type < static_cast<int>(obj_cap_.size()) ? obj_cap_[type] : 0; }
 
   // Returns "" or an error message; `code` receives the ZG_* code.
   std::string validate(const zg_tuple& t, bool has_expiry) const;
@@ -144,9 +161,21 @@ class Store {
     std::vector<uint64_t> rec_of;
     uint32_t n_interned = 0;
     uint32_t n_numeric = 0;  // max numeric id seen in bulk loads + 1
+    // ids of retired names that no relationship has named since: one bit per id below n_ids()
+    std::vector<uint32_t> free_bits;
+    uint32_t n_free = 0, free_word = 0;  // free_word: no free id lies in an earlier word
     uint32_t lookup(const char* s, size_t n) const;
     void insert(uint64_t rec);  // record offset
+    void place(uint64_t rec);   // into a table with room
     uint32_t n_ids() const { return static_cast<uint32_t>(rec_of.size()); }
+    uint32_t take_free();  // the lowest free id, off the list
+    // a relationship names `id` directly (bulk load, raw update): it is no longer free
+    void claim(uint32_t id) {
+      if (n_free && (id >> 5) < free_bits.size() && (free_bits[id >> 5] >> (id & 31) & 1u)) {
+        free_bits[id >> 5] &= ~(1u << (id & 31));
+        --n_free;
+      }
+    }
   };
   std::vector<TypeObjs> objs_;
   mutable std::vector<uint32_t> obj_cap_;  // per type: capacity handed out by the last layout()
