@@ -267,6 +267,7 @@ std::string Device::publish_delta(const Store& store, const Schema& sc, uint64_t
   cudaEventRecord(e0, stream);
   std::vector<uint32_t> cls_delta;
   std::string err = gpu_apply_delta(store, sc, lay, stream, s.get(), &cls_delta, own_rank, own_count);
+  const uint64_t failures = closure_failures;
   if (err.empty() && !s->closure.empty()) {
     // a closure index whose classes this write changed is rebuilt from the merged reverse rows before anybody reads
     // the snapshot again: a stale index is never read
@@ -290,7 +291,8 @@ std::string Device::publish_delta(const Store& store, const Schema& sc, uint64_t
     snap.reset();  // the arrays may be half merged: nobody may read them; the caller rebuilds
     return err == "relayout" || err == "corrupt" ? "full" : err;
   }
-  bool structural = false;
+  // a pair that lost its index (a failed rebuild) republishes the program: its slots' SF_NO_RSET flags are recomputed
+  bool structural = closure_failures != failures;
   for (size_t c = 0; c < cls_delta.size(); ++c) {
     const uint64_t before = s->cls_count[c];
     s->cls_count[c] = before + static_cast<int32_t>(cls_delta[c]);
@@ -443,6 +445,14 @@ std::string Device::finish_publish(std::shared_ptr<Snapshot> s, const HostSnapsh
     }
     s->closure = std::move(pairs);
     build_closures(s.get(), h, nullptr);
+    // slots whose checks only meet over the indexes just built load no memberships at admission (kernels.cuh)
+    std::vector<uint16_t> indexed;
+    for (const auto& c : s->closure)
+      if (c.built) indexed.push_back(c.tgc);
+    if (!indexed.empty() && mark_rsetless_slots(&blob, indexed) &&
+        (cudaMemcpyAsync(s->prog.p, blob.data(), blob.size(), cudaMemcpyHostToDevice, stream) != cudaSuccess ||
+         cudaStreamSynchronize(stream) != cudaSuccess))
+      return std::string("snapshot upload failed: ") + cudaGetErrorString(cudaGetLastError());
   }
   s->revision = revision;
 

@@ -188,10 +188,11 @@ struct WarpCtx {
   uint32_t my_subj, my_ss;  // this lane's own query: subject id, stype<<16 | srel
   // Direction-optimised probes: rset[i * 32 + job] = resource id of every direct relationship
   // of the job's subject (its reverse rows), grouped by class (boundaries in my_cst), when
-  // there are <= kRsetCap.
+  // there are <= kRsetCap and some step of the job's permission may read them (SF_NO_RSET).
   uint32_t* rset;
   unsigned long long my_cst;  // class boundaries of this lane's own job (see cst_at)
-  unsigned inv_mask;  // jobs that may meet in the middle: their reverse rows fit, or (cst bit kOverCap) only batch_l2 meets
+  unsigned inv_mask;  // jobs that may meet in the middle: their reverse rows fit, or (cst bit kOverCap) only the
+                      // two-level meets (closure_meet, batch_l2), which do not read the set
   unsigned long long bytes;
   unsigned long long* events;
   bool fatal;
@@ -764,14 +765,15 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
 #endif
             }
           } else if (MEET != kMeetNone && (st.flags & kStepTargetL2) && meets && depth + 2 <= ZG_MAX_DEPTH &&
-                     (inverted || hi - lo <= static_cast<uint32_t>(kFCap))) {
+                     (ccol || inverted || hi - lo <= static_cast<uint32_t>(kFCap))) {
             // Two levels at once (namespace -> team#member -> group#member -> user): a child t of this
             // range matches iff some membership g of the subject (class tinv) is a subject of t in the
             // children's single class tgc. The reverse row of g in that class lists exactly those t, in
             // ascending order like this range: the answer is "do the two sorted segments intersect",
             // once per membership. The children are never visited, nothing is pushed. A subject with more
-            // memberships than the per-check set holds meets too (batch_l2 reads them from its reverse row);
-            // with more than kFCap children its range is walked.
+            // memberships than the per-check set holds meets too: over a closure index whatever the range's
+            // size (the index does not read the set), else through batch_l2, which reads them from its reverse
+            // row; without an index, a range of more than kFCap children is walked.
             const uint32_t kb = cst_at(cst, st.tinv), ke = stype == st.tstype ? cst_at(cst, st.tinv + 1u) : kb;
             if (ccol) {
               // The pair has a closure index: the union of the memberships' reverse rows is the subject's row of it.
@@ -943,7 +945,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
 #endif
     const unsigned long long q = base + lane;
     const bool valid = q < p.nq;
-    bool bad = false, expansive = false;
+    bool bad = false, expansive = false, no_rset = false;
     uint32_t nl = 0;
     c.my_subj = 0;
     c.my_ss = (0u << 16) | kNone;
@@ -962,6 +964,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
         bad = true;
       } else {
         const DSlot s = pr.slots()[perm];
+        no_rset = (s.flags & SF_NO_RSET) != 0;
         if (s.kind == SK_NONPURE) {
           const DTree t = pr.trees()[s.unit];
           tree = s.unit;
@@ -998,6 +1001,17 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
         }
       }
       const bool meet = inv;  // stays when the memberships overflow the set: the two-level meet reads them itself
+      if (no_rset) {
+        // No step this check evaluates at the root reads the set: its probes are not invertible and its pushes
+        // meet over a closure index (SF_NO_RSET). The check is admitted as one whose memberships overflow the set
+        // (kOverCap), a state every reader of the set already handles without it: a direct probe searches the
+        // forward row, the one-level meet is skipped (its range is visited), a two-level step with an index meets
+        // over the subject's closure row whatever the range's size (visit), one without reads the memberships from
+        // the subject's reverse row (batch_l2) or, past kFCap children, visits the range, and the children a step
+        // pushes at the depth limit are visited like any other check's. Nothing is loaded.
+        inv = false;
+        ncl = 0;
+      }
       const int maxcl = __reduce_max_sync(kFull, ncl);
       for (int i = 0; i < maxcl; ++i) {
         if (inv && i < ncl) {

@@ -775,4 +775,37 @@ std::vector<uint8_t> Schema::blob(const std::vector<DRel>& rels, const std::vect
   return out;
 }
 
+int mark_rsetless_slots(std::vector<uint8_t>* blob, const std::vector<uint16_t>& indexed_tgc) {
+  uint8_t* const b = blob->data();
+  const DHeader* h = reinterpret_cast<const DHeader*>(b);
+  DSlot* slots = reinterpret_cast<DSlot*>(b + h->off_slots);
+  const DUnit* units = reinterpret_cast<const DUnit*>(b + h->off_units);
+  const DStep* steps = reinterpret_cast<const DStep*>(b + h->off_steps);
+  const DTree* trees = reinterpret_cast<const DTree*>(b + h->off_trees);
+  const uint16_t* leaf_units = reinterpret_cast<const uint16_t*>(b + h->off_leaf_units);
+  auto unit_ok = [&](uint16_t u) {
+    const DUnit& x = units[u];
+    for (int i = x.step_begin; i < x.push_begin; ++i)
+      if (steps[i].kind == ST_DIRECT && (steps[i].flags & CF_INVERT)) return false;
+    for (int i = x.push_begin; i < x.step_end; ++i)
+      if (!(steps[i].flags & kStepTargetL2) ||
+          std::find(indexed_tgc.begin(), indexed_tgc.end(), steps[i].tgc) == indexed_tgc.end())
+        return false;
+    return true;
+  };
+  int marked = 0;
+  for (uint32_t s = 0; s < h->n_slots; ++s) {
+    bool ok = true;
+    if (slots[s].kind == SK_NONPURE) {
+      const DTree& t = trees[slots[s].unit];
+      for (uint16_t l = 0; l < t.n_leaves && ok; ++l) ok = unit_ok(leaf_units[t.leaf_begin + l]);
+    } else {
+      ok = unit_ok(slots[s].unit);
+    }
+    slots[s].flags = static_cast<uint16_t>(ok ? slots[s].flags | SF_NO_RSET : slots[s].flags & ~SF_NO_RSET);
+    marked += ok;
+  }
+  return marked;
+}
+
 }  // namespace zg

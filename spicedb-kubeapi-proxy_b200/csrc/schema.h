@@ -42,11 +42,15 @@ constexpr uint16_t kStepTargetL2 = 0x200;    // DStep.flags: the children's unit
                                              // children are UF_LEAF_INV visits (resource -> team#member -> user): the
                                              // whole two-level range is answered from the subject's reverse rows
 
+enum SlotFlags : uint16_t {
+  SF_NO_RSET = 1,  // no step of a unit the slot evaluates at the root reads the subject's per-check membership set
+                   // (set at publish once the closure indexes are built: mark_rsetless_slots)
+};
 struct DSlot {   // per slot (relation or permission)
   uint16_t kind;        // SlotKind
   uint16_t unit;        // SK_RELATION / SK_PURE: unit id ; SK_NONPURE: tree id
   uint16_t type;
-  uint16_t pad;
+  uint16_t flags;       // SlotFlags
 };
 struct DUnit {   // pure-union program evaluated at one object
   uint16_t op_begin, op_end;    // into ops[]
@@ -212,5 +216,11 @@ class Schema {
   std::string compile();
   int name_id(const std::string& n);
 };
+
+// Sets SF_NO_RSET in the slot table of a program blob (Schema::blob) for every slot whose checks never read the
+// per-check membership set: in every unit the slot evaluates at the root, no probe step is an invertible direct
+// class (CF_INVERT) and every push step is a two-level step (kStepTargetL2) whose class has a closure index
+// (indexed_tgc lists the tgc of every pair built). Returns the number of slots marked.
+int mark_rsetless_slots(std::vector<uint8_t>* blob, const std::vector<uint16_t>& indexed_tgc);
 
 }  // namespace zg
