@@ -511,6 +511,104 @@ func (c *Client) RetireUnusedNames() (uint64, error) {
 	return uint64(n), nil
 }
 
+// MirrorPage is one page of ReadMirrorPage: the lines ("type:id#rel@stype:sid[#srel]") in the page order, each line's
+// expiration (zero time: none) and the cursor that resumes after it, the cursor after the page, and whether more follow.
+type MirrorPage struct {
+	Lines   []string
+	Expires []time.Time
+	Cursors [][]byte
+	Next    []byte
+	More    bool
+}
+
+// ReadMirrorPage reads the first `limit` relationships of the mirror that match the filter and follow `after` (nil:
+// from the start), in the page order (resource type, resource, relation class, subject). A cursor stays valid across
+// writes; one from another filter is refused. It reads the mirror only: ReadRelationships keeps delegating to SpiceDB.
+func (c *Client) ReadMirrorPage(filter *v1.RelationshipFilter, limit uint64, after []byte) (*MirrorPage, error) {
+	var s cstrs
+	defer s.free()
+	var f C.zg_filter_str
+	s.fillFilter(&f, filter)
+	var cur *C.zg_read_cursor
+	if after != nil {
+		if len(after) != C.ZG_READ_CURSOR_BYTES {
+			return nil, status.Errorf(codes.InvalidArgument, "read cursor of %d bytes", len(after))
+		}
+		cur = (*C.zg_read_cursor)(C.CBytes(after))
+		defer C.free(unsafe.Pointer(cur))
+	}
+	if limit > 1<<16 { // a page returns at most this many lines: More reports the rest
+		limit = 1 << 16
+	}
+	for capBytes := uint64(1 << 16); ; {
+		buf := C.malloc(C.size_t(capBytes))
+		exp := make([]C.uint32_t, limit+1)
+		curs := make([]C.zg_read_cursor, limit+1)
+		var need C.size_t
+		var n C.uint64_t
+		var next C.zg_read_cursor
+		var more C.int32_t
+		big := false
+		err := call(func() C.int {
+			rc := C.zg_read_relationships_page(c.engine, &f, C.uint64_t(limit), cur, (*C.char)(buf), C.size_t(capBytes), &need,
+				&n, &exp[0], &curs[0], &next, &more)
+			big = rc == C.ZG_E2BIG
+			if big {
+				return 0
+			}
+			return rc
+		})
+		if err != nil || big {
+			C.free(buf)
+			if err != nil {
+				return nil, err
+			}
+			capBytes = uint64(need) + 16
+			continue
+		}
+		p := &MirrorPage{More: more != 0, Next: C.GoBytes(unsafe.Pointer(&next), C.ZG_READ_CURSOR_BYTES)}
+		text := C.GoString((*C.char)(buf))
+		C.free(buf)
+		if text != "" {
+			p.Lines = strings.Split(strings.TrimSuffix(text, "\n"), "\n")
+		}
+		for i := range p.Lines {
+			p.Cursors = append(p.Cursors, C.GoBytes(unsafe.Pointer(&curs[i]), C.ZG_READ_CURSOR_BYTES))
+			if exp[i] != 0 {
+				p.Expires = append(p.Expires, time.Unix(int64(exp[i]), 0))
+			} else {
+				p.Expires = append(p.Expires, time.Time{})
+			}
+		}
+		return p, nil
+	}
+}
+
+// DeleteMirrorLimited deletes from the mirror what DeleteRelationships with optional_limit and
+// optional_allow_partial_deletions deletes: more than `limit` matches fail with FailedPrecondition unless allowPartial,
+// which deletes the first `limit` in the page order and reports partial. limit 0 deletes every match. The shim's
+// DeleteRelationships keeps delegating to SpiceDB and mirroring the whole filter.
+func (c *Client) DeleteMirrorLimited(filter *v1.RelationshipFilter, limit uint64, allowPartial bool) (uint64, bool, error) {
+	c.mu.Lock()
+	defer c.mu.Unlock()
+	var s cstrs
+	defer s.free()
+	var f C.zg_filter_str
+	s.fillFilter(&f, filter)
+	var n C.uint64_t
+	var partial C.int32_t
+	allow := C.int(0)
+	if allowPartial {
+		allow = 1
+	}
+	if err := call(func() C.int {
+		return C.zg_delete_relationships_limited(c.engine, &f, nil, 0, C.uint64_t(limit), allow, &n, &partial)
+	}); err != nil {
+		return 0, false, err
+	}
+	return uint64(n), partial != 0, nil
+}
+
 // resync rebuilds the mirror from a full ReadRelationships per resource type. The mirror is EMPTIED
 // first: it runs when a mirrored write failed after SpiceDB committed, and a batch that was rejected as a
 // whole may have carried DELETEs -- re-TOUCHing what SpiceDB holds now would leave those revoked grants

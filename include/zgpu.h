@@ -20,6 +20,8 @@
  *   zg_collect_expired          the datastore's garbage collection of expired relationships (pkg/spicedb/spicedb.go:53)
  *   zg_retire_unused_names      frees the interned names no relationship mentions any more, for reuse
  *   zg_read_relationships       ReadRelationships      pkg/authz/distributedtx/activity.go:128-171
+ *   zg_read_relationships_page  ReadRelationships with optional_limit / optional_cursor (v1 API)
+ *   zg_delete_relationships_limited  DeleteRelationships with optional_limit / optional_allow_partial_deletions
  *   zg_watch_read               WatchService.Watch     pkg/authz/watch.go:27-48
  *   zg_engine_create/load_schema embedded SpiceDB ctor pkg/spicedb/spicedb.go:18-57
  *
@@ -299,6 +301,51 @@ int zg_debug_set_resolve_hook(zg_engine *e, void (*hook)(void *), void *arg);
  * lines, sorted. Returns 0 or ZG_E2BIG (*need = bytes required incl. NUL). */
 int zg_read_relationships(zg_engine *e, const zg_filter_str *filter, char *buf, size_t cap,
                           size_t *need, uint64_t *n_out);
+
+/* ---- pages of relationship reads, and deletes with a limit ---- */
+/* A resumable position in a filter's matches (ReadRelationships' optional_cursor / after_result_cursor). Opaque, with
+ * no public fields: it names the key of the last relationship returned, not a position, so it stays valid across
+ * writes, collections, retirements and publishes. A cursor made for another filter, or before the schema was loaded
+ * again, is refused with ZG_EINVAL. */
+#define ZG_READ_CURSOR_BYTES 32
+typedef struct zg_read_cursor {
+  uint8_t opaque[ZG_READ_CURSOR_BYTES];
+} zg_read_cursor;
+/* One page of zg_read_relationships: the first `limit` (>= 1, else ZG_EINVAL) live relationships that match the filter
+ * and follow `after` (NULL: from the start) in the page order. The page order is the key (resource type, resource id,
+ * class position, subject id): the class position is the index of the relationship's (relation, subject type, subject
+ * relation) among the classes of its resource type, in schema order. It depends on the schema and the interned ids
+ * alone, so every engine kind (replicated, sharded handle, host only) and both paths give identical pages.
+ *   - Lines use the text of zg_read_relationships, in the page order; expires[i] (NULL or *n_out entries) is line i's
+ *     expiration (0 = none), cursors[i] (NULL or *n_out entries) the cursor that resumes after line i.
+ *   - *next resumes after the page (after the last line; `after` itself, or the start, when the page is empty), *more
+ *     is 1 exactly when another match follows the page.
+ *   - A relationship that exists unchanged for the whole paging appears exactly once; one created or deleted between
+ *     pages may appear or not.
+ *   - ZG_E2BIG (*need = bytes required incl. NUL, *n_out = lines) fills nothing else: the caller's cursor still resumes
+ *     where it did.
+ *   - Locks and paths are those of zg_read_relationships: on a current snapshot the device answers (the first `limit` +
+ *     1 matches after the cursor, in order, without visiting the rest of the store), otherwise the host store. A page
+ *     never publishes. */
+int zg_read_relationships_page(zg_engine *e, const zg_filter_str *filter, uint64_t limit, const zg_read_cursor *after,
+                               char *buf, size_t cap, size_t *need, uint64_t *n_out, uint32_t *expires,
+                               zg_read_cursor *cursors, zg_read_cursor *next, int32_t *more);
+/* zg_delete_relationships with DeleteRelationships' optional_limit and optional_allow_partial_deletions. limit 0 is
+ * zg_delete_relationships (*partial = 0). Otherwise, when more than `limit` relationships match (expired ones included,
+ * as for zg_delete_relationships):
+ *   - allow_partial == 0: ZG_EPRECOND, nothing changes;
+ *   - allow_partial != 0: the first `limit` of them in the page order are deleted and *partial = 1
+ *     (DELETION_PROGRESS_PARTIAL).
+ * Else every match is deleted and *partial = 0 (DELETION_PROGRESS_COMPLETE). Preconditions, the watch feed and the
+ * publish are those of zg_delete_relationships. *n_deleted and *partial may be NULL. */
+int zg_delete_relationships_limited(zg_engine *e, const zg_filter_str *filter, const zg_precondition_str *pre,
+                                    uint64_t n_pre, uint64_t limit, int allow_partial, uint64_t *n_deleted,
+                                    int32_t *partial);
+/* Cumulative counters of the pages of zg_read_relationships_page and zg_delete_relationships_limited: out[0] pages
+ * served on the device, out[1] pages served by the host store, out[2] entries the device windows covered (forward
+ * entries of the scanned objects; the resource shape: the row entries counted; the subject shape: the candidates read),
+ * out[3] device launches. Pages also count in zg_filter_counters as filters. */
+int zg_page_counters(zg_engine *e, uint64_t *out);
 
 /* ---- the hot path -------------------------------------------------------- */
 /* CheckBulkPermissions: out[i] answers items[i] (same length, same order:

@@ -16,6 +16,7 @@ NO_OBJECT = 0xFFFFFFFF
 OP_TOUCH, OP_CREATE, OP_DELETE = 0, 1, 2
 PRECOND_MUST_MATCH, PRECOND_MUST_NOT_MATCH = 1, 2
 E2BIG = -7
+READ_CURSOR_BYTES = 32  # sizeof(zg_read_cursor)
 WILDCARDS_INCLUDE, WILDCARDS_EXCLUDE = 0, 1  # zg_lookup_subjects wildcard_option
 
 CHECK_DTYPE = np.dtype(
@@ -163,6 +164,12 @@ _SIGS = {
     "zg_debug_set_resolve_hook": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "zg_read_relationships": (C.c_int, [C.c_void_p, C.POINTER(_RelStr), C.c_char_p, C.c_size_t,
                                         C.POINTER(C.c_size_t), C.POINTER(C.c_uint64)]),
+    "zg_read_relationships_page": (C.c_int, [C.c_void_p, C.POINTER(_RelStr), C.c_uint64, C.c_void_p, C.c_char_p,
+                                             C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint64), C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.POINTER(C.c_int32)]),
+    "zg_delete_relationships_limited": (C.c_int, [C.c_void_p, C.POINTER(_RelStr), C.POINTER(_Precond), C.c_uint64,
+                                                  C.c_uint64, C.c_int, C.POINTER(C.c_uint64), C.POINTER(C.c_int32)]),
+    "zg_page_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
     "zg_watch_read": (C.c_int, [C.c_void_p, C.c_uint64, C.c_char_p, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t),
                                 C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "zg_check_bulk": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
@@ -484,6 +491,61 @@ class Engine:
                 continue
             self._ck(rc)
             return [l for l in buf.value.decode().split("\n") if l]
+
+    def read_relationships_page(self, limit: int, cursor: bytes | None = None, **flt):
+        """zg_read_relationships_page -> (lines, expires, cursors, next, more): the first `limit` relationships matching
+        the filter after `cursor` (None: from the start) in the page order, their expirations (0 = none), the cursor
+        after each line, the cursor after the page and whether more follow. Cursors are opaque bytes."""
+        f = self._filter(flt)
+        after = None if cursor is None else C.create_string_buffer(bytes(cursor), READ_CURSOR_BYTES)
+        cap = max(1 << 16, min(int(limit), 1 << 18) * 64)  # a line rarely takes more: no second run of the page
+        while True:
+            buf = C.create_string_buffer(cap)
+            need, n, more = C.c_size_t(0), C.c_uint64(0), C.c_int32(0)
+            rows = min(int(limit), cap // 8 + 1)  # a line takes at least 8 bytes
+            exp = np.zeros(rows, dtype=np.uint32)
+            curs = C.create_string_buffer(rows * READ_CURSOR_BYTES)
+            nxt = C.create_string_buffer(READ_CURSOR_BYTES)
+            rc = self._L.zg_read_relationships_page(self._h, C.byref(f), int(limit), after, buf, cap, C.byref(need),
+                                                    C.byref(n), exp.ctypes.data, curs, nxt, C.byref(more))
+            if rc == E2BIG:
+                cap = need.value + 16
+                continue
+            self._ck(rc)
+            k = n.value
+            lines = [l for l in buf.value.decode().split("\n") if l]
+            raw = curs.raw
+            cursors = [raw[i * READ_CURSOR_BYTES:(i + 1) * READ_CURSOR_BYTES] for i in range(k)]
+            return lines, exp[:k].tolist(), cursors, nxt.raw, bool(more.value)
+
+    def iter_relationships(self, limit: int, **flt):
+        """Every relationship matching the filter, read page by page (`limit` per page) in the page order."""
+        cursor = None
+        while True:
+            lines, _, _, cursor, more = self.read_relationships_page(limit, cursor, **flt)
+            yield from lines
+            if not more:
+                return
+
+    def delete_relationships_limited(self, flt: dict, preconditions=(), limit: int = 0, allow_partial: bool = False):
+        """zg_delete_relationships_limited -> (deleted, partial). limit 0 deletes every match; otherwise more than
+        `limit` matches raise ZgpuError(ZG_EPRECOND) unless allow_partial, which deletes the first `limit` of them in
+        the page order and returns partial=True."""
+        pre = (_Precond * max(len(preconditions), 1))()
+        for i, (op, f) in enumerate(preconditions):
+            pre[i] = _Precond(int(op), self._filter(f))
+        n, partial = C.c_uint64(0), C.c_int32(0)
+        f = self._filter(flt)
+        self._ck(self._L.zg_delete_relationships_limited(self._h, C.byref(f), pre, len(preconditions), int(limit),
+                                                         1 if allow_partial else 0, C.byref(n), C.byref(partial)))
+        return n.value, bool(partial.value)
+
+    def page_counters(self) -> dict:
+        """zg_page_counters: pages served on the device / by the host store, entries the device windows covered,
+        device launches."""
+        out = np.zeros(4, dtype=np.uint64)
+        self._ck(self._L.zg_page_counters(self._h, out.ctypes.data))
+        return dict(zip(("device_pages", "host_pages", "scanned", "launches"), (int(x) for x in out)))
 
     # -- hot path ---------------------------------------------------------------
     def watch_read(self, since_revision: int, res_type: str = ""):

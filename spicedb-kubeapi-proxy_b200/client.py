@@ -209,17 +209,48 @@ class WriteRelationshipsResponse:
 class DeleteRelationshipsRequest:
     relationship_filter: RelationshipFilter
     optional_preconditions: List[Precondition] = field(default_factory=list)
+    optional_limit: int = 0  # 0: every match
+    optional_allow_partial_deletions: bool = False
+
+
+DELETION_PROGRESS_COMPLETE, DELETION_PROGRESS_PARTIAL = 1, 2  # v1.DeleteRelationshipsResponse_DeletionProgress
+
+
+class DeleteRelationshipsResponse(int):
+    """The number of relationships deleted (what DeleteRelationships always returned), carrying deletion_progress."""
+
+    deletion_progress: int = DELETION_PROGRESS_COMPLETE
+
+    def __new__(cls, deleted: int, deletion_progress: int = DELETION_PROGRESS_COMPLETE):
+        r = super().__new__(cls, deleted)
+        r.deletion_progress = deletion_progress
+        return r
 
 
 @dataclass
 class ReadRelationshipsRequest:
     relationship_filter: RelationshipFilter
     fully_consistent: bool = True
+    optional_limit: int = 0  # 0: no limit
+    optional_cursor: Optional[bytes] = None  # an after_result_cursor of an earlier response
 
 
 @dataclass
 class ReadRelationshipsResponse:
     relationship: Relationship
+    after_result_cursor: Optional[bytes] = None  # set when the request had a limit or a cursor
+
+
+@dataclass
+class ExportBulkRelationshipsRequest:
+    optional_limit: int = 0  # relationships per response; 0: 1 000
+    optional_cursor: Optional[bytes] = None
+
+
+@dataclass
+class ExportBulkRelationshipsResponse:
+    after_result_cursor: bytes
+    relationships: List[Relationship]
 
 
 @dataclass
@@ -317,12 +348,16 @@ class PermissionsClient:
             raise _rpc(e) from None
         return WriteRelationshipsResponse(self.engine.stats()["revision"])
 
-    def DeleteRelationships(self, req: DeleteRelationshipsRequest) -> int:
+    def DeleteRelationships(self, req: DeleteRelationshipsRequest) -> DeleteRelationshipsResponse:
         pre = [(_PRE[p.operation], p.filter.fields()) for p in req.optional_preconditions]
         try:
-            return self.engine.delete_relationships(req.relationship_filter.fields(), pre)
+            if not req.optional_limit:
+                return DeleteRelationshipsResponse(self.engine.delete_relationships(req.relationship_filter.fields(), pre))
+            n, partial = self.engine.delete_relationships_limited(req.relationship_filter.fields(), pre, req.optional_limit,
+                                                                  req.optional_allow_partial_deletions)
         except ZgpuError as e:
             raise _rpc(e) from None
+        return DeleteRelationshipsResponse(n, DELETION_PROGRESS_PARTIAL if partial else DELETION_PROGRESS_COMPLETE)
 
     def Watch(self, req: WatchRequest) -> "WatchStream":
         """v1.WatchServiceClient.Watch (pkg/authz/watch.go:27-48). The returned stream is polled:
@@ -337,11 +372,37 @@ class PermissionsClient:
         return WatchStream(self.engine, list(req.optional_object_types), start)
 
     def ReadRelationships(self, req: ReadRelationshipsRequest) -> Iterator[ReadRelationshipsResponse]:
+        """Without a limit or a cursor: the unpaged read, sorted. With them: the matches after the cursor in the page
+        order (at most optional_limit of them), each with its expiration and the cursor that resumes after it."""
+        flt = req.relationship_filter.fields()
         try:
-            lines = self.engine.read_relationships(**req.relationship_filter.fields())
+            if not req.optional_limit and req.optional_cursor is None:
+                lines = self.engine.read_relationships(**flt)
+                return iter([ReadRelationshipsResponse(Relationship.parse(l)) for l in lines])
+            out, cursor, left = [], req.optional_cursor, req.optional_limit
+            while True:
+                lines, exp, curs, cursor, more = self.engine.read_relationships_page(min(left, 1000) if left else 1000,
+                                                                                    cursor, **flt)
+                out += [ReadRelationshipsResponse(Relationship.parse(l, x), c) for l, x, c in zip(lines, exp, curs)]
+                if req.optional_limit:
+                    left -= len(lines)
+                if not more or (req.optional_limit and left == 0):
+                    return iter(out)
         except ZgpuError as e:
             raise _rpc(e) from None
-        return iter([ReadRelationshipsResponse(Relationship.parse(l)) for l in lines])
+
+    def ExportBulkRelationships(self, req: ExportBulkRelationshipsRequest) -> Iterator[ExportBulkRelationshipsResponse]:
+        """Every relationship after the cursor, in the page order, optional_limit per response (the empty filter)."""
+        out, cursor = [], req.optional_cursor
+        try:
+            while True:
+                lines, exp, _, cursor, more = self.engine.read_relationships_page(req.optional_limit or 1000, cursor)
+                if lines:
+                    out.append(ExportBulkRelationshipsResponse(cursor, [Relationship.parse(l, x) for l, x in zip(lines, exp)]))
+                if not more:
+                    return iter(out)
+        except ZgpuError as e:
+            raise _rpc(e) from None
 
 
 _WATCH_OP = {"TOUCH": OPERATION_TOUCH, "CREATE": OPERATION_CREATE, "DELETE": OPERATION_DELETE}

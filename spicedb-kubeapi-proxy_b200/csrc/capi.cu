@@ -202,6 +202,9 @@ struct zg_engine {
   // zg_filter_counters: relationship filters (reads, deletes by filter, preconditions) answered from the snapshot on
   // the device and by Store::match, relationships the device returned, device filters by Device::FilterShape
   std::atomic<uint64_t> flt_device{0}, flt_host{0}, flt_returned{0}, flt_shape[3] = {};
+  // zg_page_counters: pages served on the device / by the host store, entries the device windows covered, launches
+  std::atomic<uint64_t> pg_device{0}, pg_host{0}, pg_scanned{0}, pg_launches{0};
+  uint32_t schema_gen = 0;  // schema loads: a page cursor names the schema it was made under
   // zg_name_counters: names retired by zg_retire_unused_names calls that read the mentions from the snapshots / from
   // the host store (reset with the store by a schema load)
   uint64_t retire_device = 0, retire_host = 0;
@@ -448,6 +451,7 @@ extern "C" int zg_load_schema(zg_engine* e, const char* dsl, size_t len) {
   if (!err.empty()) return fail(ZG_EINVAL, err);
   e->schema = std::move(s);
   e->has_schema = true;
+  ++e->schema_gen;
   e->store.reset(&e->schema);
   e->retire_device = e->retire_host = 0;  // with the store's count of retired names
   ++e->name_epoch;                        // every name is gone
@@ -1141,6 +1145,244 @@ extern "C" int zg_read_relationships(zg_engine* e, const zg_filter_str* filter, 
     buf[w++] = '\n';
   }
   buf[w] = 0;
+  return ZG_OK;
+}
+
+// ---- pages: zg_read_relationships_page, zg_delete_relationships_limited ----
+
+// The bytes of a zg_read_cursor. `fp` fingerprints the filter: its type, relation and subject-relation ids as resolved
+// against the schema, and the object names as given (a name need not exist, and keeps its meaning across retirements).
+struct CursorBits {
+  uint16_t version;  // kCursorVersion
+  uint16_t has_key;  // 0: the start
+  uint32_t schema_gen;
+  uint64_t fp;
+  PageKey key;
+};
+static_assert(sizeof(CursorBits) == ZG_READ_CURSOR_BYTES, "zg_read_cursor is CursorBits");
+constexpr uint16_t kCursorVersion = 1;
+
+static uint64_t filter_fingerprint(const Store::Filter& f, const zg_filter_str& s) {
+  uint64_t h = 0xcbf29ce484222325ull;
+  auto mix = [&](const void* p, size_t n) {
+    for (size_t i = 0; i < n; ++i) h = (h ^ static_cast<const uint8_t*>(p)[i]) * 0x100000001b3ull;
+  };
+  const int32_t ids[6] = {f.res_type, f.rel, f.subj_type, f.subj_wildcard, f.has_srel, f.srel};
+  mix(ids, sizeof ids);
+  for (const char* str : {s.res_id, s.subj_id}) {
+    const size_t n = str ? std::strlen(str) : 0;
+    mix(&n, sizeof n);
+    if (n) mix(str, n);
+  }
+  return h;
+}
+
+static zg_read_cursor make_cursor(const zg_engine* e, uint64_t fp, const PageKey* key) {
+  CursorBits c{};
+  c.version = kCursorVersion;
+  c.has_key = key != nullptr;
+  c.schema_gen = e->schema_gen;
+  c.fp = fp;
+  if (key) c.key = *key;
+  zg_read_cursor out;
+  std::memcpy(out.opaque, &c, sizeof c);
+  return out;
+}
+
+// The first `want` matches of f at clock `now` after *after in the page order, with their expirations, from the
+// resident snapshot(s). A sharded handle asks every shard (or the resource's owner) for its own first `want` and merges
+// them; replicas hold the same snapshot, so the first device answers. Counts the page in zg_page_counters and the
+// filter in zg_filter_counters. *too_big: see Device::page_filter. Caller holds e->mu and e->names (shared is enough)
+// and has seen filters_on_device.
+static int page_on_device(zg_engine* e, const Store::Filter& f, uint32_t now, const PageKey* after, uint64_t want,
+                          std::vector<zg_tuple>* found, std::vector<uint32_t>* exp, bool* too_big) {
+  const uint32_t S = is_handle(e) ? e->n_shards : 1;
+  const int owner = S > 1 && f.has_res ? static_cast<int>(f.res % S) : -1;
+  std::vector<std::vector<zg_tuple>> got(S);
+  std::vector<std::vector<uint32_t>> got_exp(S);
+  std::vector<Device::PageStats> st(S);
+  std::vector<int> rcs(S, ZG_OK);
+  std::vector<std::string> errs(S);
+  std::vector<char> big(S, 0);
+  auto one = [&](Device& dev, size_t k) {
+    bool b = false;
+    rcs[k] = dev.page_filter(e->schema, f, now, after, want, &got[k], &got_exp[k], &st[k], &b, &errs[k]);
+    big[k] = b;
+  };
+  if (S == 1) one(e->dev, 0);
+  else if (owner >= 0) one(shard(e, static_cast<uint32_t>(owner)), static_cast<size_t>(owner));
+  else on_all_devices(e, one);
+  std::string err;
+  if (int rc = first_error(rcs, errs, &err)) return fail(rc == ZG_ENOMEM ? ZG_ECUDA : rc, err);
+  *too_big = false;
+  for (uint32_t k = 0; k < S; ++k) *too_big = *too_big || big[k];
+  if (*too_big) return ZG_OK;
+  found->clear();
+  exp->clear();
+  if (S == 1) {
+    found->swap(got[0]);
+    exp->swap(got_exp[0]);
+  } else {  // every shard's list is in K order: merge and cut
+    std::vector<std::pair<PageKey, std::pair<uint32_t, uint32_t>>> keys;
+    for (uint32_t k = 0; k < S; ++k)
+      for (uint32_t i = 0; i < got[k].size(); ++i) keys.push_back({page_key(e->schema, got[k][i]), {k, i}});
+    std::sort(keys.begin(), keys.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+    if (keys.size() > want) keys.resize(want);
+    for (const auto& x : keys) {
+      found->push_back(got[x.second.first][x.second.second]);
+      exp->push_back(got_exp[x.second.first][x.second.second]);
+    }
+  }
+  ++e->pg_device;
+  for (const auto& x : st) {
+    e->pg_scanned += x.scanned;
+    e->pg_launches += x.launches;
+  }
+  ++e->flt_device;
+  ++e->flt_shape[Device::filter_shape(f)];
+  e->flt_returned += found->size();
+  return ZG_OK;
+}
+
+// The host path of a page: Store::page. Caller holds e->names exclusively (match() may build the index).
+static void page_on_host(zg_engine* e, const Store::Filter& f, uint32_t now, const PageKey* after, uint64_t want,
+                         std::vector<zg_tuple>* found, std::vector<uint32_t>* exp) {
+  std::vector<uint64_t> idx;
+  e->store.page(f, now, after, want, &idx);
+  found->clear();
+  exp->clear();
+  for (uint64_t i : idx) {
+    found->push_back(e->store.tuples[i]);
+    exp->push_back(e->store.expires[i]);
+  }
+  ++e->pg_host;
+  ++e->flt_host;
+}
+
+extern "C" int zg_read_relationships_page(zg_engine* e, const zg_filter_str* filter, uint64_t limit, const zg_read_cursor* after,
+                                          char* buf, size_t cap, size_t* need, uint64_t* n_out, uint32_t* expires,
+                                          zg_read_cursor* cursors, zg_read_cursor* next, int32_t* more) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (!filter) return fail(ZG_EINVAL, "NULL filter");
+  if (limit == 0) return fail(ZG_EINVAL, "page limit must be at least 1 (zg_read_relationships reads without one)");
+  // the locks of zg_read_relationships
+  std::unique_lock<FairMutex> dl(e->mu, std::defer_lock);
+  if (!e->host_only) dl.lock();
+  std::shared_lock<std::shared_mutex> shared(e->names, std::defer_lock);
+  std::unique_lock<std::shared_mutex> exclusive(e->names, std::defer_lock);
+  bool on_device = filters_on_device(e);
+  if (on_device) shared.lock();
+  else exclusive.lock();
+  std::string err;
+  Store::Filter f = resolve_filter(e, *filter, &err);
+  if (!err.empty()) return fail(ZG_EINVAL, err);
+  const uint64_t fp = filter_fingerprint(f, *filter);
+  CursorBits c{};
+  if (after) {
+    std::memcpy(&c, after->opaque, sizeof c);
+    if (c.version != kCursorVersion || c.has_key > 1)
+      return fail(ZG_EINVAL, "read cursor: not a cursor of this engine");
+    if (c.schema_gen != e->schema_gen || c.fp != fp)
+      return fail(ZG_EINVAL, "read cursor: it was made for another filter or under another schema");
+  }
+  const PageKey* from = after && c.has_key ? &c.key : nullptr;
+  // at most every relationship of the store matches: a larger limit asks the kernels for nothing more
+  const uint64_t want = std::min<uint64_t>(limit, e->store.size()) + 1;
+  std::vector<zg_tuple> found;
+  std::vector<uint32_t> exp;
+  if (on_device) {
+    bool too_big = false;
+    if (int rc = page_on_device(e, f, now_of(e), from, want, &found, &exp, &too_big)) return rc;
+    if (too_big) {  // as in zg_read_relationships: writers wait for the device lock held here, f stays resolved
+      on_device = false;
+      shared.unlock();
+      exclusive.lock();
+    }
+  }
+  if (!on_device) page_on_host(e, f, now_of(e), from, want, &found, &exp);
+  const bool has_more = found.size() > limit;
+  if (has_more) {
+    found.resize(limit);
+    exp.resize(limit);
+  }
+  std::vector<std::string> lines;
+  lines.reserve(found.size());
+  size_t total = 1;
+  for (const zg_tuple& t : found) {
+    lines.push_back(tuple_text(e, t));
+    total += lines.back().size() + 1;
+  }
+  if (need) *need = total;
+  if (n_out) *n_out = lines.size();
+  if (total > cap || !buf) return ZG_E2BIG;
+  size_t w = 0;
+  for (size_t i = 0; i < lines.size(); ++i) {
+    std::memcpy(buf + w, lines[i].data(), lines[i].size());
+    w += lines[i].size();
+    buf[w++] = '\n';
+    if (expires) expires[i] = exp[i];
+    if (cursors) {
+      const PageKey k = page_key(e->schema, found[i]);
+      cursors[i] = make_cursor(e, fp, &k);
+    }
+  }
+  buf[w] = 0;
+  if (next) {
+    if (found.empty()) *next = make_cursor(e, fp, from);
+    else {
+      const PageKey k = page_key(e->schema, found.back());
+      *next = make_cursor(e, fp, &k);
+    }
+  }
+  if (more) *more = has_more;
+  return ZG_OK;
+}
+
+extern "C" int zg_delete_relationships_limited(zg_engine* e, const zg_filter_str* filter, const zg_precondition_str* pre,
+                                               uint64_t n_pre, uint64_t limit, int allow_partial, uint64_t* n_deleted,
+                                               int32_t* partial) {
+  if (partial) *partial = 0;
+  if (limit == 0) return zg_delete_relationships(e, filter, pre, n_pre, n_deleted);
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (!filter || (!pre && n_pre)) return fail(ZG_EINVAL, "NULL argument");
+  LOCK_DEVICE(e);
+  LOCK_NAMES_UNIQUE(e);
+  std::string err;
+  Store::Filter f = resolve_filter(e, *filter, &err);
+  if (!err.empty()) return fail(ZG_EINVAL, err);
+  int rc = check_preconditions(e, pre, n_pre);
+  if (rc) return rc;
+  // the first limit + 1 matches in the page order, expired ones included (clock 0): is there more than the limit?
+  const uint64_t want = std::min<uint64_t>(limit, e->store.size()) + 1;
+  std::vector<zg_tuple> found;
+  std::vector<uint32_t> exp;
+  bool on_device = filters_on_device(e);
+  if (on_device) {
+    bool too_big = false;
+    if ((rc = page_on_device(e, f, 0, nullptr, want, &found, &exp, &too_big))) return rc;
+    on_device = !too_big;
+  }
+  if (!on_device) page_on_host(e, f, 0, nullptr, want, &found, &exp);
+  const bool cut = found.size() > limit;
+  if (cut && !allow_partial)  // the text of SpiceDB's DeleteRelationships
+    return fail(ZG_EPRECOND, "found more than " + std::to_string(limit) +
+                                 " relationships to be deleted and partial deletion was not requested");
+  if (cut) found.resize(limit);
+  std::vector<uint64_t> idx;
+  std::vector<zg_update> u;
+  std::vector<uint8_t> changed;
+  rc = delete_found(e, "delete by filter", &found, &idx, &u, &changed, n_deleted);
+  if (rc == ZG_OK) {
+    e->log_changes(u, changed);
+    if (partial) *partial = cut;
+  }
+  return rc;
+}
+
+extern "C" int zg_page_counters(zg_engine* e, uint64_t* out) {
+  if (!e || !out) return fail(ZG_EINVAL, "NULL argument");
+  const uint64_t c[4] = {e->pg_device.load(), e->pg_host.load(), e->pg_scanned.load(), e->pg_launches.load()};
+  std::memcpy(out, c, sizeof c);
   return ZG_OK;
 }
 

@@ -12,6 +12,8 @@
 #include <mutex>
 #include <thread>
 
+#include <cub/cub.cuh>
+
 #include "filter.cuh"
 #include "ingress.cuh"
 #include "kernels.cuh"
@@ -2451,26 +2453,15 @@ int Device::lookup_subjects(uint16_t res_type, uint32_t res, uint16_t perm, uint
 
 // ---- relationship filters (filter.cuh) --------------------------------------------------------
 
-int Device::match_filter(const Schema& sc, const Store::Filter& f, uint32_t now, uint64_t* count, std::vector<zg_tuple>* tuples,
-                         std::vector<uint32_t>* expires, bool* too_big, std::string* err) {
-  *count = 0;
-  *too_big = false;
-  if (tuples) tuples->clear();
-  if (expires) expires->clear();
-  std::shared_ptr<Snapshot> s = snap;
-  if (!s) {
-    if (err) *err = "no snapshot published";
-    return ZG_ENOSNAPSHOT;
-  }
-  if (f.impossible) return ZG_OK;
-  // the classes whose relation, subject type and subject relation agree with the filter
-  std::vector<FilterSel> sel;
-  for (size_t ri = 0; ri < sc.rel_slots.size() && ri < s->rels.size(); ++ri) {
+// The classes whose relation, subject type and subject relation agree with the filter, in data-relation order.
+static void select_classes(const Schema& sc, const Snapshot& s, const Store::Filter& f, std::vector<FilterSel>* sel) {
+  sel->clear();
+  for (size_t ri = 0; ri < sc.rel_slots.size() && ri < s.rels.size(); ++ri) {
     const int slot = sc.rel_slots[ri];
     if ((f.res_type >= 0 && sc.slots[slot].type != f.res_type) || (f.rel >= 0 && slot != f.rel)) continue;
-    const DRel& r = s->rels[ri];
+    const DRel& r = s.rels[ri];
     for (uint16_t k = 0; k < r.ncls; ++k) {
-      const DCls& c = s->cls[r.cls_begin + k];
+      const DCls& c = s.cls[r.cls_begin + k];
       if (f.subj_type >= 0 && c.stype != f.subj_type) continue;
       if (f.subj_wildcard && c.sslot != kWildcard) continue;
       if (f.has_subj && c.sslot == kWildcard) continue;  // a concrete id never matches a wildcard relationship
@@ -2485,9 +2476,27 @@ int Device::match_filter(const Schema& sc, const Store::Filter& f, uint32_t now,
       x.rel = static_cast<uint16_t>(slot);
       x.stype = c.stype;
       x.srel = c.sslot;
-      sel.push_back(x);
+      x.pos = static_cast<uint16_t>(page_class_pos(sc, slot, c.stype, c.sslot));
+      x.rtype = sc.slots[slot].type;
+      sel->push_back(x);
     }
   }
+}
+
+int Device::match_filter(const Schema& sc, const Store::Filter& f, uint32_t now, uint64_t* count, std::vector<zg_tuple>* tuples,
+                         std::vector<uint32_t>* expires, bool* too_big, std::string* err) {
+  *count = 0;
+  *too_big = false;
+  if (tuples) tuples->clear();
+  if (expires) expires->clear();
+  std::shared_ptr<Snapshot> s = snap;
+  if (!s) {
+    if (err) *err = "no snapshot published";
+    return ZG_ENOSNAPSHOT;
+  }
+  if (f.impossible) return ZG_OK;
+  std::vector<FilterSel> sel;
+  select_classes(sc, *s, f, &sel);
   if (sel.empty() || s->n_tuples == 0) return ZG_OK;
   FilterPlan p{};
   p.has_subj = f.has_subj;
@@ -2601,6 +2610,157 @@ int Device::run_filter(const Schema& sc, const Snapshot& s, const std::vector<Fi
   if (n2 != n) {  // the snapshot cannot change under the device lock
     if (err) *err = "filter: the emit launch found " + std::to_string(n2) + " relationships, the count launch " + std::to_string(n);
     return ZG_ECUDA;
+  }
+  return ZG_OK;
+}
+
+int Device::page_filter(const Schema& sc, const Store::Filter& f, uint32_t now, const PageKey* after, uint64_t want,
+                        std::vector<zg_tuple>* tuples, std::vector<uint32_t>* expires, PageStats* st, bool* too_big,
+                        std::string* err) {
+  tuples->clear();
+  expires->clear();
+  *too_big = false;
+  std::shared_ptr<Snapshot> s = snap;
+  if (!s) {
+    if (err) *err = "no snapshot published";
+    return ZG_ENOSNAPSHOT;
+  }
+  if (f.impossible || want == 0) return ZG_OK;
+  std::vector<FilterSel> sel;
+  select_classes(sc, *s, f, &sel);
+  if (sel.empty() || s->n_tuples == 0) return ZG_OK;
+  std::sort(sel.begin(), sel.end(), [](const FilterSel& a, const FilterSel& b) {
+    return a.rtype != b.rtype ? a.rtype < b.rtype : a.pos < b.pos;
+  });
+  const FilterShape shape = filter_shape(f);
+  // the output: `want` records (the subject shape: a segment of them per selected class), within a quarter of the free
+  // memory; one type's classes go into one plan
+  size_t free_b = 0, total_b = 0;
+  ZG_CUDA(cudaSetDevice(device));
+  ZG_CUDA(cudaMemGetInfo(&free_b, &total_b));
+  const uint64_t segs = shape == kBySubject ? sel.size() : 1;
+  const uint64_t bytes = segs * want * (sizeof(zg_tuple) + 4);
+  bool fits = bytes <= flt_out_.cap + flt_exp_.cap || bytes <= free_b / 4;
+  for (size_t g = 0, g0 = 0; fits && g <= sel.size(); ++g)
+    if (g == sel.size() || sel[g].rtype != sel[g0].rtype) {
+      fits = shape == kBySubject || g - g0 <= static_cast<size_t>(kMaxFilterSel);
+      g0 = g;
+    }
+  if (!fits) {
+    *too_big = true;
+    return ZG_OK;
+  }
+  if (!flt_out_.ensure(segs * want * sizeof(zg_tuple)) || !flt_exp_.ensure(segs * want * 4) || !flt_ctrl_.ensure(64)) {
+    if (err) *err = "out of device memory (page output)";
+    return ZG_ENOMEM;
+  }
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  PagePlan p{};
+  p.row_ptr = s->row_ptr.as<uint32_t>();
+  p.col = s->col.as<uint32_t>();
+  p.exp = sc.has_expiry ? s->exp.as<uint32_t>() : nullptr;
+  p.rrow_ptr = s->rrow_ptr.as<uint32_t>();
+  p.rcol = s->rcol.as<uint32_t>();
+  p.now = now;
+  p.has_subj = f.has_subj;
+  p.subj = f.has_subj ? f.subj : 0;
+  zg_tuple* d_out = flt_out_.as<zg_tuple>();
+  uint32_t* d_exp = flt_exp_.as<uint32_t>();
+  unsigned long long* ctrl = flt_ctrl_.as<unsigned long long>();
+
+  if (shape == kBySubject) {  // one warp per class, its segment of `want`; merged on the host (page_merge)
+    page_set_after(p, after);
+    p.want = want;
+    if (!pg_seg_.ensure(sel.size() * 4)) {
+      if (err) *err = "out of device memory (page segments)";
+      return ZG_ENOMEM;
+    }
+    for (size_t at = 0; at < sel.size(); at += kMaxFilterSel) {
+      p.n_sel = static_cast<uint32_t>(std::min<size_t>(kMaxFilterSel, sel.size() - at));
+      std::copy(sel.begin() + at, sel.begin() + at + p.n_sel, p.sel);
+      p.out = d_out + at * want;
+      p.out_exp = d_exp + at * want;
+      p.seg_count = pg_seg_.as<uint32_t>() + at;
+      page_subject_kernel<<<p.n_sel, 32, 0, stream>>>(p);
+      ++st->launches;
+    }
+    ZG_CUDA(cudaGetLastError());
+    std::vector<uint32_t> seg(sel.size());
+    ZG_CUDA(cudaMemcpyAsync(seg.data(), pg_seg_.p, seg.size() * 4, cudaMemcpyDeviceToHost, stream));
+    ZG_CUDA(cudaStreamSynchronize(stream));
+    std::vector<zg_tuple> rec(sel.size() * want);
+    std::vector<uint32_t> rec_exp(sel.size() * want);
+    for (size_t k = 0; k < sel.size(); ++k) {
+      if (!seg[k]) continue;
+      ZG_CUDA(cudaMemcpyAsync(rec.data() + k * want, d_out + k * want, seg[k] * sizeof(zg_tuple), cudaMemcpyDeviceToHost, stream));
+      ZG_CUDA(cudaMemcpyAsync(rec_exp.data() + k * want, d_exp + k * want, seg[k] * 4ull, cudaMemcpyDeviceToHost, stream));
+      st->scanned += seg[k];
+    }
+    ZG_CUDA(cudaStreamSynchronize(stream));
+    page_merge(sel, seg.data(), rec.data(), rec_exp.data(), want, tuples, expires);
+    return ZG_OK;
+  }
+
+  // scan and resource shapes: windows of one type's objects (page_walk)
+  struct Ops {
+    Device* d;
+    unsigned long long* ctrl;
+    zg_tuple* out;
+    uint32_t* out_exp;
+    PageStats* st;
+    std::string* err;
+    int window(const PagePlan& p, unsigned long long block, uint32_t stride, uint32_t obj0, unsigned long long entries,
+               uint32_t* obj1, unsigned long long* n) {
+      page_window_kernel<<<1, 32, 0, d->stream>>>(p.row_ptr, block, stride, obj0, p.sel[0].nres, entries, ctrl);
+      ++st->launches;
+      ZG_CUDA(cudaGetLastError());
+      unsigned long long h[2];
+      ZG_CUDA(cudaMemcpyAsync(h, ctrl, 16, cudaMemcpyDeviceToHost, d->stream));
+      ZG_CUDA(cudaStreamSynchronize(d->stream));
+      *obj1 = static_cast<uint32_t>(h[0]);
+      *n = h[1];
+      return ZG_OK;
+    }
+    int tiles(PagePlan& p, unsigned long long got, unsigned long long* total) {
+      const uint64_t n_tiles = (uint64_t(p.obj1 - p.obj0) + 31) / 32;
+      size_t tmp = 0;
+      cub::DeviceScan::ExclusiveSum(nullptr, tmp, d->pg_count_.as<unsigned long long>(), d->pg_off_.as<unsigned long long>(),
+                                    static_cast<int64_t>(n_tiles + 1), d->stream);
+      if (!d->pg_count_.ensure((n_tiles + 1) * 8) || !d->pg_off_.ensure((n_tiles + 1) * 8) || !d->pg_tmp_.ensure(tmp)) {
+        if (err) *err = "out of device memory (page tiles)";
+        return ZG_ENOMEM;
+      }
+      p.tile_count = d->pg_count_.as<unsigned long long>();
+      p.tile_off = d->pg_off_.as<unsigned long long>();
+      p.out = out + got;
+      p.out_exp = out_exp + got;
+      const uint64_t warps_per_block = kFilterThreads / 32;
+      const unsigned grid = static_cast<unsigned>(
+          std::max<uint64_t>(1, std::min<uint64_t>((n_tiles + warps_per_block - 1) / warps_per_block, uint64_t(d->sm_count_) * 16)));
+      ZG_CUDA(cudaMemsetAsync(p.tile_count + n_tiles, 0, 8, d->stream));
+      page_count_kernel<<<grid, kFilterThreads, 0, d->stream>>>(p);
+      ZG_CUDA(cudaGetLastError());
+      if (cub::DeviceScan::ExclusiveSum(d->pg_tmp_.p, tmp, p.tile_count, d->pg_off_.as<unsigned long long>(),
+                                        static_cast<int64_t>(n_tiles + 1), d->stream) != cudaSuccess) {
+        if (err) *err = "page: the scan of the tile counts failed";
+        return ZG_ECUDA;
+      }
+      page_emit_kernel<<<grid, kFilterThreads, 0, d->stream>>>(p);
+      ZG_CUDA(cudaGetLastError());
+      st->launches += 3;
+      ZG_CUDA(cudaMemcpyAsync(total, p.tile_off + n_tiles, 8, cudaMemcpyDeviceToHost, d->stream));
+      ZG_CUDA(cudaStreamSynchronize(d->stream));
+      return ZG_OK;
+    }
+  } ops{this, ctrl, d_out, d_exp, st, err};
+  unsigned long long got = 0;
+  if (int rc = page_walk(ops, p, sel, shape == kByResource, f.res, after, want, &got, &st->scanned)) return rc;
+  tuples->resize(got);
+  expires->resize(got);
+  if (got) {
+    ZG_CUDA(cudaMemcpyAsync(tuples->data(), d_out, got * sizeof(zg_tuple), cudaMemcpyDeviceToHost, stream));
+    ZG_CUDA(cudaMemcpyAsync(expires->data(), d_exp, got * 4, cudaMemcpyDeviceToHost, stream));
+    ZG_CUDA(cudaStreamSynchronize(stream));
   }
   return ZG_OK;
 }

@@ -299,6 +299,18 @@ class Device {
   // with CF_EXPIRY are read. A count launch that finds nothing is the whole call.
   int match_expired(const Schema& sc, uint32_t before, uint64_t* count, std::vector<zg_tuple>* tuples, bool* too_big,
                     std::string* err);
+  // A page (zg_read_relationships_page): the first `want` relationships of the resident snapshot that match f at
+  // clock `now` (0: expired ones too) and whose key follows *after (nullptr: from the start), in K order (PageKey),
+  // with their expirations. The scan and resource shapes walk windows of one type's objects at a time (filter.cuh
+  // page_walk), the subject shape takes `want` entries of every selected class's reverse row and merges them here.
+  // *too_big: the output would take more than a quarter of the free device memory, or a type has more selected
+  // classes than one plan holds; nothing else is valid and the caller pages on the host.
+  struct PageStats {
+    uint64_t scanned = 0, launches = 0;  // entries the windows covered (see zg_page_counters), kernel launches
+  };
+  int page_filter(const Schema& sc, const Store::Filter& f, uint32_t now, const PageKey* after, uint64_t want,
+                  std::vector<zg_tuple>* tuples, std::vector<uint32_t>* expires, PageStats* st, bool* too_big,
+                  std::string* err);
   // zg_retire_unused_names: per type, one bit per id of the snapshot's object capacity, set where a relationship of
   // the snapshot names the id as its resource or its subject (filter.cuh mention_scan_kernel); OR-ed into *bits
   // (Store::IdBits, grown to the capacities). One launch per 64 types, one copy back.
@@ -378,6 +390,7 @@ class Device {
   DevBuf lb_params_, lb_owner_, lb_ctrl_, lb_keys_[2];  // batched lookups
   DevBuf ls_jobs_, ls_codes_, ls_has_, ls_ids_, ls_ctrl_;   // LookupSubjects
   DevBuf flt_out_, flt_exp_, flt_ctrl_;                     // match_filter: records, expirations, the count
+  DevBuf pg_count_, pg_off_, pg_tmp_, pg_seg_;              // page_filter: tile counts, offsets, scan space, segments
   DevBuf mention_bits_;                                     // scan_mentions: every type's bitmap
   // sharded LookupResources round: walk state in rb_visited_ / lk_jobs_ / lb_owner_ / lb_params_ / lb_keys_ (a sharded
   // engine never runs lookup_batch), the round's home ranks, self-membership list and control words here

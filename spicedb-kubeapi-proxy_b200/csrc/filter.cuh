@@ -18,11 +18,14 @@
 #ifndef ZG_EMULATE  // tests/emu/: the same source under a CPU SIMT emulator (test infrastructure, never in libzgpu.so)
 #include <cuda_runtime.h>
 #endif
+#include <algorithm>
 #include <cstdint>
+#include <utility>
 #include <vector>
 
 #include "../../include/zgpu.h"
 #include "schema.h"
+#include "store.h"
 
 namespace zg {
 
@@ -37,8 +40,10 @@ struct FilterSel {  // one selected (data relation, class)
   uint32_t stride;               // forward row stride per object
   uint16_t rstride;              // reverse row stride per subject (0 for a wildcard class)
   uint16_t rel, stype, srel;     // what a record of this class says: relation slot, subject type, ZG_SREL_* or slot
-  uint16_t pad;
+  uint16_t pos;                  // pages: the class position, the class's index in its type's forward row block
+  uint16_t rtype;                // pages: the resource type
 };
+static_assert(sizeof(FilterSel) == 40, "FilterSel is the plans' array element: two fields fill its tail padding");
 
 struct FilterPlan {
   const uint32_t *row_ptr, *col, *exp, *rrow_ptr, *rcol;  // exp: nullptr when the schema has no expiration
@@ -202,6 +207,292 @@ __global__ void __launch_bounds__(kFilterThreads) filter_scan_kernel(const Filte
 template <bool kEmit>
 __global__ void __launch_bounds__(kFilterThreads) filter_expired_kernel(const FilterPlan p) {
   filter_scan<kEmit, true>(p);
+}
+
+// ---- pages of a filter (zg_read_relationships_page, zg_delete_relationships_limited) ----
+// A page is the first `want` (= limit + 1) live matches whose key K = (resource type, resource, class position,
+// subject) follows the cursor's key, in K order. Within one resource type K is the physical order of `col`: row_ptr is
+// object-major over every class of the type (DESIGN §3), and a row is sorted by subject. The host selects one type's
+// classes, sorted by position, and walks windows of its objects:
+//   page_window_kernel  from row_ptr alone, the least window end at which `entries` entries of the block follow
+//   page_count_kernel   per tile (32 objects x the selected classes) its matches, stopping at `want`
+//   (cub::DeviceScan)   exclusive offsets of the tile counts
+//   page_emit_kernel    every tile that starts before `want` writes its matches at its offset, in K order
+// The resource shape is the window of one object. The subject shape (page_subject_kernel) takes at most `want` live
+// entries after the cursor from the subject's reverse row of every selected class; the host merges them into K order.
+struct PagePlan {
+  const uint32_t *row_ptr, *col, *exp, *rrow_ptr, *rcol;  // exp: nullptr when the schema has no expiration
+  uint32_t n_sel;
+  uint32_t has_subj, subj;  // resource shape: only the entry `subj` of each row; subject shape: the subject (0: "*")
+  uint32_t now;             // 0: expired relationships match too
+  uint32_t has_after;       // the start key: only entries with K > (after_type, after_res, after_pos, after_subj)
+  uint32_t after_type, after_res, after_pos, after_subj;
+  uint32_t obj0, obj1;      // the window [obj0, obj1) of the type's objects
+  uint32_t pad;
+  unsigned long long want;  // matches still wanted: a tile stops counting there, and nothing is written past it
+  unsigned long long* tile_count;     // count: per tile (n_tiles + 1 entries, the last one 0)
+  const unsigned long long* tile_off; // emit: their exclusive scan
+  zg_tuple* out;                      // emit: `want` records and expirations; subject shape: n_sel segments of `want`
+  uint32_t* out_exp;
+  uint32_t* seg_count;                // subject shape: per selected class, the entries written to its segment
+  FilterSel sel[kMaxFilterSel];
+};
+
+// The entries of (object o, class s) a page may return: past the start key when o is the cursor's object, and only
+// `subj` with has_subj. o < s.nres.
+__device__ __forceinline__ void page_row(const PagePlan& p, const FilterSel& s, uint32_t o, uint32_t* b, uint32_t* e) {
+  const unsigned long long ri = s.row_base + static_cast<unsigned long long>(o) * s.stride;
+  *b = __ldg(p.row_ptr + ri);
+  *e = __ldg(p.row_ptr + ri + 1);
+  if (p.has_after && o == p.after_res) {
+    if (s.pos < p.after_pos || (s.pos == p.after_pos && p.after_subj == 0xFFFFFFFFu)) *e = *b;
+    else if (s.pos == p.after_pos) *b = filter_lower_bound(p.col, *b, *e, p.after_subj + 1);
+  }
+  if (p.has_subj) {
+    const uint32_t at = filter_lower_bound(p.col, *b, *e, p.subj);
+    if (at < *e && __ldg(p.col + at) == p.subj) *b = at, *e = at + 1;
+    else *e = *b;
+  }
+}
+
+// One thread: the least obj1 in (obj0, nres] at which at least `entries` entries of the type's block follow obj0
+// (nres when fewer do), and how many do. `block` = row_ptr index of (object 0, class position 0) of the type.
+__global__ void page_window_kernel(const uint32_t* row_ptr, unsigned long long block, uint32_t stride, uint32_t obj0,
+                                   uint32_t nres, unsigned long long entries, unsigned long long* out) {
+  if (threadIdx.x | blockIdx.x) return;
+  const uint32_t at0 = __ldg(row_ptr + block + static_cast<unsigned long long>(obj0) * stride);
+  uint32_t lo = obj0 + 1, hi = nres;
+  while (lo < hi) {
+    const uint32_t mid = lo + ((hi - lo) >> 1);
+    if (__ldg(row_ptr + block + static_cast<unsigned long long>(mid) * stride) - at0 < entries) lo = mid + 1; else hi = mid;
+  }
+  out[0] = lo;
+  out[1] = __ldg(row_ptr + block + static_cast<unsigned long long>(lo) * stride) - at0;
+}
+
+// Warp-collective walk of tile t: its matches in K order. kEmit: written from `base` on, never at or past p.want.
+// Returns how many it found, counting stopping once `base` + that reaches p.want.
+template <bool kEmit>
+__device__ __forceinline__ unsigned long long page_tile(const PagePlan& p, unsigned long long t, unsigned long long base,
+                                                        unsigned lane) {
+  const unsigned long long o64 = p.obj0 + t * 32 + lane;
+  const bool mine = o64 < p.obj1;
+  const uint32_t o = static_cast<uint32_t>(o64);
+  // the lane's object: does it have an entry the page may return, and how many (offsets only)
+  unsigned long long n = 0;
+  if (mine)
+    for (uint32_t k = 0; k < p.n_sel; ++k) {
+      if (o >= p.sel[k].nres) continue;
+      uint32_t b, e;
+      page_row(p, p.sel[k], o, &b, &e);
+      n += e - b;
+    }
+  if (!kEmit && !(p.exp && p.now)) {  // without expirations a count needs the offsets only
+    for (int d = 16; d > 0; d >>= 1) n += __shfl_xor_sync(kFilterFull, n, d);
+    return n;
+  }
+  unsigned long long got = 0;
+  unsigned objs = __ballot_sync(kFilterFull, n != 0);
+  while (objs && base + got < p.want) {
+    const int src = __ffs(objs) - 1;
+    objs &= objs - 1;
+    const uint32_t ob = static_cast<uint32_t>(p.obj0 + t * 32 + src);
+    for (uint32_t k = 0; k < p.n_sel && base + got < p.want; ++k) {
+      const FilterSel& s = p.sel[k];
+      if (ob >= s.nres) continue;
+      uint32_t b, e;
+      page_row(p, s, ob, &b, &e);
+      for (uint32_t i0 = b; i0 < e && base + got < p.want; i0 += 32) {
+        const uint32_t i = i0 + lane;
+        bool hit = i < e;
+        uint32_t subj = 0, ex = 0;
+        if (hit) {
+          subj = __ldg(p.col + i);
+          if (p.exp) ex = __ldg(p.exp + i);
+          hit = filter_live(ex, p.now);
+        }
+        const unsigned m = __ballot_sync(kFilterFull, hit);
+        const unsigned long long at = base + got + __popc(m & ((1u << lane) - 1u));
+        if (kEmit && hit && at < p.want) {
+          zg_tuple r;
+          r.res = ob;
+          r.subj = s.srel == ZG_SREL_WILDCARD ? 0u : subj;
+          r.rel = s.rel;
+          r.stype = s.stype;
+          r.srel = s.srel;
+          r.flags = 0;
+          p.out[at] = r;
+          p.out_exp[at] = ex;
+        }
+        got += __popc(m);
+      }
+    }
+  }
+  return got;
+}
+
+__global__ void __launch_bounds__(kFilterThreads) page_count_kernel(const PagePlan p) {
+  const unsigned lane = threadIdx.x & 31;
+  const unsigned long long w = (blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x) >> 5;
+  const unsigned long long n_warps = (static_cast<unsigned long long>(gridDim.x) * blockDim.x) >> 5;
+  const unsigned long long tiles = (static_cast<unsigned long long>(p.obj1 - p.obj0) + 31) >> 5;
+  for (unsigned long long t = w; t < tiles; t += n_warps) {
+    const unsigned long long n = page_tile<false>(p, t, 0, lane);
+    if (lane == 0) p.tile_count[t] = n;
+  }
+}
+
+__global__ void __launch_bounds__(kFilterThreads) page_emit_kernel(const PagePlan p) {
+  const unsigned lane = threadIdx.x & 31;
+  const unsigned long long w = (blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x) >> 5;
+  const unsigned long long n_warps = (static_cast<unsigned long long>(gridDim.x) * blockDim.x) >> 5;
+  const unsigned long long tiles = (static_cast<unsigned long long>(p.obj1 - p.obj0) + 31) >> 5;
+  for (unsigned long long t = w; t < tiles; t += n_warps) {
+    const unsigned long long base = __ldg(p.tile_off + t);
+    if (base >= p.want) continue;  // tiles are in K order: every later one starts at or past it too
+    if (__ldg(p.tile_count + t)) page_tile<true>(p, t, base, lane);
+  }
+}
+
+// Subject given, no resource: one warp per selected class. Its reverse row is sorted by resource, and K orders by
+// (type, resource, class position, subject) with the type, the position and the subject fixed for the row, so the
+// entries after the cursor are a suffix of the row. The first `want` live ones go to the class's segment in order;
+// expirations are found again in the forward row, as filter_subject_kernel does.
+__global__ void __launch_bounds__(32) page_subject_kernel(const PagePlan p) {
+  const unsigned lane = threadIdx.x & 31;
+  for (uint32_t k = blockIdx.x; k < p.n_sel; k += gridDim.x) {
+    const FilterSel& s = p.sel[k];
+    unsigned long long got = 0;
+    uint32_t start = 0;
+    bool none = p.subj >= s.nsubj;
+    if (p.has_after && !none) {
+      if (s.rtype < p.after_type) none = true;
+      else if (s.rtype == p.after_type) {  // (pos, subj) > (after_pos, after_subj): the cursor's resource is in
+        const bool same_res_after = s.pos > p.after_pos || (s.pos == p.after_pos && p.subj > p.after_subj);
+        if (same_res_after) start = p.after_res;
+        else if (p.after_res == 0xFFFFFFFFu) none = true;
+        else start = p.after_res + 1;
+      }
+    }
+    if (!none) {
+      const unsigned long long ri = s.rrow_base + static_cast<unsigned long long>(p.subj) * s.rstride;
+      const uint32_t e = __ldg(p.rrow_ptr + ri + 1);
+      const uint32_t b = filter_lower_bound(p.rcol, __ldg(p.rrow_ptr + ri), e, start);
+      zg_tuple* out = p.out + k * p.want;
+      uint32_t* out_exp = p.out_exp + k * p.want;
+      for (uint32_t i0 = b; i0 < e && got < p.want; i0 += 32) {
+        const uint32_t i = i0 + lane;
+        bool hit = i < e;
+        uint32_t res = 0, ex = 0;
+        if (hit) {
+          res = __ldg(p.rcol + i);
+          if (p.exp && res < s.nres) {
+            const unsigned long long fi = s.row_base + static_cast<unsigned long long>(res) * s.stride;
+            const uint32_t fb = __ldg(p.row_ptr + fi), fe = __ldg(p.row_ptr + fi + 1);
+            const uint32_t at = filter_lower_bound(p.col, fb, fe, p.subj);
+            if (at < fe && __ldg(p.col + at) == p.subj) ex = __ldg(p.exp + at);
+          }
+          hit = filter_live(ex, p.now);
+        }
+        const unsigned m = __ballot_sync(kFilterFull, hit);
+        const unsigned long long at = got + __popc(m & ((1u << lane) - 1u));
+        if (hit && at < p.want) {
+          zg_tuple r;
+          r.res = res;
+          r.subj = p.subj;
+          r.rel = s.rel;
+          r.stype = s.stype;
+          r.srel = s.srel;
+          r.flags = 0;
+          out[at] = r;
+          out_exp[at] = ex;
+        }
+        got += __popc(m);
+      }
+    }
+    if (lane == 0) p.seg_count[k] = static_cast<uint32_t>(got < p.want ? got : p.want);
+  }
+}
+
+// ---- the host side of a page: shared by Device::page_filter and the emulator's tests ----
+inline void page_set_after(PagePlan& p, const PageKey* after) {
+  p.has_after = after != nullptr;
+  if (after) p.after_type = after->type, p.after_res = after->res, p.after_pos = after->pos, p.after_subj = after->subj;
+}
+
+// The scan and resource shapes: the classes `sel` (one plan's worth or fewer per type, sorted by type and position; a
+// class's row_base - pos is its type's block) walked type by type, window by window, until `want` matches are found.
+// Ops supplies the launches:
+//   int window(const PagePlan&, block, stride, obj0, entries, *obj1, *n)   page_window_kernel, its answer copied back
+//   int tiles(PagePlan&, got, *total)   count launch, scan and emit launch into the output from record `got` on, and
+//                                       how many the window holds (the emit writes at most p.want of them)
+// The first window of a type asks for `want - got` entries of the block; every window that comes up short (expired
+// entries, classes not selected, the cursor's object) asks for at least twice as many as the one before it, more when
+// its density of matches says the rest of the page needs more. *scanned: the entries of the block the windows
+// covered. Returns 0 or what an op returned.
+template <class Ops>
+int page_walk(Ops& ops, PagePlan& p, const std::vector<FilterSel>& sel, bool by_resource, uint32_t res, const PageKey* after,
+              unsigned long long want, unsigned long long* got, uint64_t* scanned) {
+  *got = 0;
+  for (size_t g = 0; g < sel.size() && *got < want;) {
+    size_t g1 = g;
+    while (g1 < sel.size() && sel[g1].rtype == sel[g].rtype) ++g1;
+    if (g1 - g > static_cast<size_t>(kMaxFilterSel)) return ZG_EINVAL;  // the caller pages such a type on the host
+    const uint32_t type = sel[g].rtype, nres = sel[g].nres;
+    p.n_sel = static_cast<uint32_t>(g1 - g);
+    std::copy(sel.begin() + g, sel.begin() + g1, p.sel);
+    g = g1;
+    const bool at_cursor = after && after->type == type;
+    if (after && type < after->type) continue;
+    uint32_t obj = at_cursor ? after->res : 0, end = nres;
+    if (by_resource) {
+      if (at_cursor && res < after->res) continue;
+      obj = res;
+      end = res < nres ? res + 1 : res;
+    }
+    page_set_after(p, at_cursor ? after : nullptr);
+    unsigned long long ask = want - *got;
+    while (obj < end && *got < want) {
+      uint32_t obj1 = end;
+      unsigned long long n = 0;
+      if (!by_resource)
+        if (int rc = ops.window(p, p.sel[0].row_base - p.sel[0].pos, p.sel[0].stride, obj, ask, &obj1, &n)) return rc;
+      p.obj0 = obj;
+      p.obj1 = obj1;
+      p.want = want - *got;
+      unsigned long long total = 0;
+      if (int rc = ops.tiles(p, *got, &total)) return rc;
+      *scanned += by_resource ? total : n;
+      *got += total < p.want ? total : p.want;
+      obj = obj1;
+      // the next window: at least twice this one, and as many entries as this window's density of matches says the
+      // rest of the page needs, with a quarter more
+      const unsigned long long left = want - *got;
+      unsigned long long next = ask * 2;
+      if (total && n / total < (1ull << 20)) next = std::max(next, left * (n / total + 1) + left / 4);
+      ask = std::min(next, 1ull << 40);
+    }
+  }
+  return 0;
+}
+
+// The subject shape: the segments of page_subject_kernel (seg_count[k] records of class sel[k] at rec + k * want),
+// merged into K order and cut at `want`.
+inline void page_merge(const std::vector<FilterSel>& sel, const uint32_t* seg_count, const zg_tuple* rec, const uint32_t* rec_exp,
+                       unsigned long long want, std::vector<zg_tuple>* out, std::vector<uint32_t>* out_exp) {
+  std::vector<std::pair<PageKey, uint64_t>> keys;
+  for (size_t k = 0; k < sel.size(); ++k)
+    for (uint64_t i = 0; i < seg_count[k]; ++i) {
+      const zg_tuple& t = rec[k * want + i];
+      keys.push_back({PageKey{sel[k].rtype, t.res, sel[k].pos, t.subj}, k * want + i});
+    }
+  const size_t n = static_cast<size_t>(std::min<unsigned long long>(want, keys.size()));
+  std::partial_sort(keys.begin(), keys.begin() + n, keys.end(),
+                    [](const auto& a, const auto& b) { return a.first < b.first; });
+  for (size_t i = 0; i < n; ++i) {
+    out->push_back(rec[keys[i].second]);
+    out_exp->push_back(rec_exp[keys[i].second]);
+  }
 }
 
 // ---- which ids the snapshot mentions (zg_retire_unused_names) ----

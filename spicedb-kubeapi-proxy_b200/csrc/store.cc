@@ -282,6 +282,21 @@ void Store::match(const Filter& f, uint32_t now, std::vector<uint64_t>* idx) con
   }
 }
 
+void Store::page(const Filter& f, uint32_t now, const PageKey* after, uint64_t want, std::vector<uint64_t>* idx) const {
+  std::vector<uint64_t> all;
+  match(f, now, &all);
+  std::vector<std::pair<PageKey, uint64_t>> keys;
+  keys.reserve(all.size());
+  for (uint64_t i : all) {
+    const PageKey k = page_key(*schema, tuples[i]);
+    if (!after || *after < k) keys.push_back({k, i});
+  }
+  const size_t n = static_cast<size_t>(std::min<uint64_t>(want, keys.size()));
+  std::partial_sort(keys.begin(), keys.begin() + n, keys.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+  idx->resize(n);
+  for (size_t i = 0; i < n; ++i) (*idx)[i] = keys[i].second;
+}
+
 bool Store::locate(const zg_tuple* t, uint64_t n, std::vector<uint64_t>* idx) {
   ensure_index();
   idx->resize(n);

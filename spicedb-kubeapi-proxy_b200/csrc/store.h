@@ -32,6 +32,36 @@ inline Key key_of(const zg_tuple& t) {
              (uint64_t(t.res) << 32) | (t.srel == kWildcard ? 0u : t.subj)};
 }
 
+// The order of pages (zg_read_relationships_page): K = (resource type, resource, class position, subject), a wildcard
+// relationship's subject 0. It depends on the schema and the ids alone, so every engine kind and both paths agree.
+struct PageKey {
+  uint32_t type, res, pos, subj;
+  bool operator<(const PageKey& o) const {
+    if (type != o.type) return type < o.type;
+    if (res != o.res) return res < o.res;
+    if (pos != o.pos) return pos < o.pos;
+    return subj < o.subj;
+  }
+};
+
+// The class position of the relationships (rel_slot, stype, srel): where Store::layout puts their rows in the forward
+// block of their resource type. It depends on the schema alone. -1 when the schema has no such class.
+inline int page_class_pos(const Schema& sc, int rel_slot, uint16_t stype, uint16_t srel) {
+  const int k = sc.class_of(rel_slot, stype, srel);
+  if (k < 0) return -1;
+  int pos = k;
+  for (int rs : sc.rel_slots) {
+    if (rs == rel_slot) return pos;
+    if (sc.slots[rs].type == sc.slots[rel_slot].type) pos += static_cast<int>(sc.slots[rs].classes.size());
+  }
+  return -1;
+}
+
+inline PageKey page_key(const Schema& sc, const zg_tuple& t) {
+  return PageKey{sc.slots[t.rel].type, t.res, static_cast<uint32_t>(page_class_pos(sc, t.rel, t.stype, t.srel)),
+                 t.srel == kWildcard ? 0u : t.subj};
+}
+
 // CSR snapshot in host memory, ready to upload. Layout: DESIGN.md "Data layout in HBM".
 struct HostSnapshot {
   std::vector<uint32_t> row_ptr;  // pool: per data relation, nres x ncls offsets, +1 sentinel
@@ -123,6 +153,9 @@ class Store {
     bool impossible = false;  // names an object/relation that does not exist
   };
   void match(const Filter& f, uint32_t now, std::vector<uint64_t>* idx) const;
+  // The host path of a page: the first `want` relationships match() lists whose key follows *after (nullptr: from
+  // the start), in K order (PageKey), as positions in `tuples`.
+  void page(const Filter& f, uint32_t now, const PageKey* after, uint64_t want, std::vector<uint64_t>* idx) const;
   // Where the n live relationships t[] sit in `tuples`, ascending: the order match() lists them in. Builds the
   // relationship index when a bulk load left it behind. false when one of them is not in the store.
   bool locate(const zg_tuple* t, uint64_t n, std::vector<uint64_t>* idx);
