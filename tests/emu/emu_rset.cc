@@ -27,7 +27,7 @@ struct Indexed {
 
 extern "C" {
 
-// Builds the index of every two-level pair of the published program; mark: set SF_NO_RSET as a publish does.
+// Builds the index of each of the published program's first kMaxClosure two-level pairs, in step order; mark: set SF_NO_RSET as a publish does.
 void* emu_index_create(void* h, int mark, int* n_marked) {
   Emu* e = static_cast<Emu*>(h);
   if (!e->published) return nullptr;
@@ -40,6 +40,7 @@ void* emu_index_create(void* h, int mark, int* n_marked) {
   for (uint32_t i = 0; i < ph->n_steps; ++i) {
     const DStep& st = steps[i];
     if (!(st.flags & kStepTargetL2) || std::find(tgcs.begin(), tgcs.end(), st.tgc) != tgcs.end()) continue;
+    if (tgcs.size() == static_cast<size_t>(kMaxClosure)) continue;  // as device.cu: the first kMaxClosure pairs
     const uint16_t inner = e->sc.d_inv_cls[e->sc.d_type_inv[st.tstype].begin + st.tinv];
     const DCls &ci = e->h.cls[inner], &ct = e->h.cls[st.tgc];
     HostClosure c;
@@ -71,6 +72,9 @@ void* emu_index_create(void* h, int mark, int* n_marked) {
 }
 
 void emu_index_destroy(void* x) { delete static_cast<Indexed*>(x); }
+
+// The number of pairs indexed (at most kMaxClosure).
+int emu_index_pairs(void* x) { return static_cast<int>(static_cast<Indexed*>(x)->cl.size()); }
 
 uint32_t emu_index_slot_flags(void* x, int slot) {
   const Indexed* d = static_cast<Indexed*>(x);

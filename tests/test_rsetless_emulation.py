@@ -2,7 +2,8 @@
 a permission whose root units have no invertible probe and meet only over closure indexes loads none of the subject's
 memberships, and its checks take the paths of a subject whose memberships overflow the set. The answers with the flag
 on must equal the oracle's and the flag-off run's; the COUNT variant's bytes must fall by exactly the membership reads.
-The driver (tests/emu/emu_rset.cc) builds the 16-bit closure index of every two-level pair on the host."""
+The driver (tests/emu/emu_rset.cc) builds the 16-bit closure index of the first kMaxClosure two-level pairs, in step
+order, on the host, as a publish does."""
 import ctypes as C
 import os
 import sys
