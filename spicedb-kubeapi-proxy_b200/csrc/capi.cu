@@ -50,29 +50,79 @@ class FairMutex {
   }
 };
 
-// Coalescing batcher ("group commit") for zg_check_bulk. The proxy calls the boundary
-// from one goroutine per rule check (pkg/authz/check.go:77-93) and per list request
-// (pkg/authz/postfilter.go:127-134): many concurrent, mostly small calls. The first
-// caller to arrive becomes the leader; while its launch is in flight later callers
-// queue, and the next leader answers ALL of them with one launch sequence. No timer:
-// batching is driven purely by arrivals during the previous launch.
-struct BatchReq {
-  const zg_check* items;
-  uint64_t n;
-  uint8_t* out;
+// A caller's place in a GroupQueue, and its result.
+struct QueuedJob {
   int rc = ZG_OK;
   std::string err;
   bool done = false, lead = false;
   std::condition_variable cv;  // every waiter sleeps on its own: a finished group wakes exactly its members and
                                // ONE next leader, not every queued caller (1 000 of them under BASELINE config 5)
 };
-struct Batcher {
-  std::mutex m;
-  std::vector<BatchReq*> queue;
-  bool leader_active = false;
-  uint64_t groups = 0, waited = 0, handed_over = 0;  // protocol counters (ZGPU_BATCHER_STATS=1 prints them at destroy)
-  static constexpr uint64_t kMaxItemsPerLaunch = 1ull << 24;
+
+// Coalescing queue ("group commit") for zg_check_bulk and LookupResources. The proxy calls the boundary from one
+// goroutine per rule check (pkg/authz/check.go:77-93) and per list request (pkg/authz/postfilter.go:127-134): many
+// concurrent, mostly small calls. The first caller to arrive becomes the leader; while its group runs later callers
+// queue, and the next leader answers ALL of them (as many as one group takes) with one launch sequence. No timer:
+// batching is driven purely by arrivals during the previous group. Job derives from QueuedJob.
+template <class Job>
+class GroupQueue {
+  std::mutex m_;
+  std::vector<Job*> queue_;
+  bool leader_active_ = false;
+
+ public:
+  uint64_t groups = 0, waited = 0, handed_over = 0;  // protocol counters
+
+  // Queues `me` and returns once a group holding it has run. take(queue) = how many jobs from the front of the queue
+  // one group takes (at least one); run(group) answers them under the device lock and sets each job's rc / err.
+  template <class Take, class Run>
+  void submit(Job* me, FairMutex& device, Take&& take, Run&& run) {
+    std::unique_lock<std::mutex> lk(m_);
+    queue_.push_back(me);
+    if (leader_active_) {
+      ++waited;
+      me->cv.wait(lk, [&] { return me->done || me->lead; });
+    }
+    if (me->done) return;
+    // leader (nobody was leading, or the previous leader handed over to the head of the queue -- me): take as many
+    // queued jobs as one group takes, mine first, answer them, wake their callers, hand leadership on
+    leader_active_ = true;
+    std::vector<Job*> group;
+    lk.unlock();
+    {
+      // the device first, the group second: whatever queued while this leader waited for the GPU (behind another
+      // queue's group, a publish, the previous group's tail) rides along
+      std::lock_guard<FairMutex> dev_lock(device);
+      lk.lock();
+      const auto n = static_cast<long>(take(queue_));
+      group.assign(queue_.begin(), queue_.begin() + n);
+      queue_.erase(queue_.begin(), queue_.begin() + n);
+      lk.unlock();
+      run(group);
+    }
+    lk.lock();
+    ++groups;
+    for (Job* j : group) {
+      j->done = true;
+      if (j != me) j->cv.notify_one();
+    }
+    if (!queue_.empty()) {
+      ++handed_over;
+      queue_.front()->lead = true;
+      queue_.front()->cv.notify_one();
+    } else {
+      leader_active_ = false;
+    }
+  }
 };
+
+// One zg_check_bulk call.
+struct BatchReq : QueuedJob {
+  const zg_check* items = nullptr;
+  uint64_t n = 0;
+  uint8_t* out = nullptr;
+};
+static constexpr uint64_t kMaxItemsPerLaunch = 1ull << 24;  // of a check group (one caller's items are never split)
 
 // One engine may own several GPUs of the box (zg_config.n_devices): every device holds a REPLICA of the
 // snapshot (1e8 relationships = 2 GB, two orders of magnitude under one GPU's HBM) and answers its slice of
@@ -142,7 +192,7 @@ struct zg_engine {
   FairMutex mu;  // the device lock: one launch sequence or publish at a time
   mutable std::shared_mutex names;
   std::vector<std::unique_ptr<Replica>> replicas;  // devices 1 .. n-1 (device 0 is `dev`)
-  Batcher batcher;
+  GroupQueue<BatchReq> batcher;  // zg_check_bulk (ZGPU_BATCHER_STATS=1 prints its counters at destroy)
   Schema schema;
   bool has_schema = false;
   Store store;
@@ -163,21 +213,13 @@ struct zg_engine {
              srel == o.srel && clock == o.clock;
     }
   };
-  struct LookupJob {
+  struct LookupJob : QueuedJob {
     LookupKey key;       // revision / clock filled in by the leader
     bool want_self = false;
     std::vector<uint32_t> ids;
     bool self_member = false;
-    int rc = ZG_OK;
-    std::string err;
-    bool done = false, lead = false;
-    std::condition_variable cv;
   };
-  struct LookupBatcher {
-    std::mutex m;
-    std::vector<LookupJob*> queue;
-    bool leader_active = false;
-  } lookups;
+  GroupQueue<LookupJob> lookups;
   // ZG_E2BIG protocol: recent answers are kept so that a caller's retry with a larger buffer (same arguments,
   // same snapshot revision) does not recompute them. zg_retire_unused_names leaves them valid: every id in an answer is
   // mentioned by a relationship at that revision, and only names no relationship mentions are retired.
@@ -257,6 +299,7 @@ static void on_all_devices(zg_engine* e, const std::function<void(Device&, size_
 
 static thread_local std::string g_err;
 static constexpr size_t kMaxLookupGroup = 64;  // = kMaxLookupBatch (kernels.cuh)
+static const char* kHostOnlyMsg = "host-only engine: no CUDA device, and libzgpu has no CPU fallback";
 static const char* kShardedMsg =
     "sharded engine: use zg_shard_route_dev / zg_shard_pass_dev / zg_shard_fold_dev / zg_shard_unroute_dev "
     "(dist.DeviceShardedChecker)";
@@ -275,16 +318,73 @@ static const char* kHandleSubjectsMsg =
 static bool is_handle(const zg_engine* e) { return e->n_shards > 1; }
 // a sharded handle that answers LookupSubjects itself (run_sharded_subjects)
 static bool serves_subjects(const zg_engine* e) { return is_handle(e) && e->handle_subjects; }
-// why a sharded engine refuses LookupSubjects
-static const char* subjects_refusal(const zg_engine* e) {
-  return !is_handle(e) ? kShardedMsg : e->handle_lookups ? kHandleSubjectsMsg : kHandleLookupMsg;
-}
 // shard k of a sharded handle
 static Device& shard(zg_engine* e, uint32_t k) { return k == 0 ? e->dev : e->replicas[k - 1]->dev; }
 
 static int fail(int code, const std::string& msg) {
   g_err = msg;
   return code;
+}
+
+// The kinds of call an engine refuses by its mode: host-only, sharded handle (zg_config.n_shards > 1), or one shard of
+// several (zg_config.shard_count > 1).
+enum class Call {
+  kDevice,         // device work that any device engine serves
+  kDeviceBuffers,  // device buffers, no check answered: zg_count_alg_bytes, zg_resolve_checks_packed_device
+  kDeviceChecks,   // checks on device buffers or through the device ingress
+  kCheckGroup,     // a check group of zg_check_bulk, and the string calls that publish before queueing one
+  kLookup,         // LookupResources and the list pre-filter
+  kSubjects,       // LookupSubjects
+  kShardCall,      // zg_shard_*_dev: one shard per engine, driven by dist.py
+};
+
+// ZG_OK when e serves calls of kind c, else the code it refuses them with; the message goes to *msg when given (the
+// callers of a group), else to zg_last_error. A host-only engine is never one shard of several (it has no device).
+static int refuse(const zg_engine* e, Call c, std::string* msg = nullptr) {
+  const char* why = nullptr;
+  if (e->host_only) {
+    why = kHostOnlyMsg;
+  } else if (is_handle(e)) {
+    switch (c) {
+      case Call::kDeviceBuffers:
+      case Call::kDeviceChecks: why = kHandleDeviceMsg; break;
+      case Call::kLookup: why = e->handle_lookups ? nullptr : kHandleLookupMsg; break;
+      case Call::kSubjects: why = e->handle_subjects ? nullptr : e->handle_lookups ? kHandleSubjectsMsg : kHandleLookupMsg; break;
+      case Call::kShardCall: why = kHandleShardCallMsg; break;
+      default: break;
+    }
+  } else if (e->dev.shard_count > 1 && c != Call::kDevice && c != Call::kDeviceBuffers && c != Call::kShardCall) {
+    why = kShardedMsg;
+  }
+  if (!why) return ZG_OK;
+  if (msg) *msg = why;
+  else g_err = why;
+  return e->host_only ? ZG_ECUDA : ZG_EINVAL;
+}
+
+// The devices a step runs on: every device of the engine (concurrently), device 0 alone, or shard k >= 0 alone.
+constexpr int kEveryDevice = -1, kFirstDevice = -2;
+
+// Runs fn(device, k, &err) -> ZG_* on the devices `which` names (k: the device's index, shard k of a handle). Returns
+// the first failing device's code in device order, and that device's message in *err.
+template <class F>
+static int on_devices(zg_engine* e, int which, F&& fn, std::string* err) {
+  if (which != kEveryDevice) {
+    const uint32_t k = which == kFirstDevice ? 0 : static_cast<uint32_t>(which);
+    std::string m;
+    const int rc = fn(shard(e, k), static_cast<size_t>(k), &m);
+    if (rc) *err = std::move(m);
+    return rc;
+  }
+  std::vector<int> rcs(1 + e->replicas.size(), ZG_OK);
+  std::vector<std::string> errs(rcs.size());
+  on_all_devices(e, [&](Device& dev, size_t k) { rcs[k] = fn(dev, k, &errs[k]); });
+  for (size_t k = 0; k < rcs.size(); ++k)
+    if (rcs[k]) {
+      *err = std::move(errs[k]);
+      return rcs[k];
+    }
+  return ZG_OK;
 }
 extern "C" const char* zg_last_error(void) { return g_err.c_str(); }
 extern "C" size_t zg_last_error_copy(char* buf, size_t cap) {
@@ -388,19 +488,17 @@ extern "C" int zg_engine_create(const zg_config* cfg, zg_engine** out) {
       e->replicas.emplace_back(new Replica());
       e->replicas.back()->worker.start();
     }
-    std::vector<std::string> errs(S);
     const zg_config c = *cfg;
-    on_all_devices(e, [&](Device& dev, size_t k) {
-      if (k) errs[k] = dev.init(first + static_cast<int>(k % static_cast<size_t>(D)), c.subquery_capacity, c.work_budget);
-      if (c.flags & ZG_FLAG_FORWARD_ONLY) dev.invert = false;
-      dev.shard_rank = dev.own_rank = static_cast<uint32_t>(k);
-      dev.shard_count = dev.own_count = S;
-    });
-    for (const auto& m : errs)
-      if (!m.empty()) {
-        delete e;
-        return fail(ZG_ECUDA, m);
-      }
+    if (on_devices(e, kEveryDevice, [&](Device& dev, size_t k, std::string* m) {
+          if (k) *m = dev.init(first + static_cast<int>(k % static_cast<size_t>(D)), c.subquery_capacity, c.work_budget);
+          if (c.flags & ZG_FLAG_FORWARD_ONLY) dev.invert = false;
+          dev.shard_rank = dev.own_rank = static_cast<uint32_t>(k);
+          dev.shard_count = dev.own_count = S;
+          return m->empty() ? ZG_OK : ZG_ECUDA;
+        }, &err)) {
+      delete e;
+      return fail(ZG_ECUDA, err);
+    }
   } else if (cfg && cfg->n_devices > 1) {
     if (cfg->shard_count > 1) {
       delete e;
@@ -414,22 +512,20 @@ extern "C" int zg_engine_create(const zg_config* cfg, zg_engine** out) {
       delete e;
       return fail(ZG_EINVAL, "n_devices exceeds the visible CUDA devices");
     }
-    std::vector<std::string> errs(static_cast<size_t>(want));
     for (int d = 1; d < want; ++d) {
       e->replicas.emplace_back(new Replica());
       e->replicas.back()->worker.start();
     }
     const zg_config c = *cfg;
-    on_all_devices(e, [&](Device& dev, size_t i) {
-      if (i == 0) return;
-      errs[i] = dev.init(first + static_cast<int>(i), c.subquery_capacity, c.work_budget);
-      if (c.flags & ZG_FLAG_FORWARD_ONLY) dev.invert = false;
-    });
-    for (const auto& m : errs)
-      if (!m.empty()) {
-        delete e;
-        return fail(ZG_ECUDA, m);
-      }
+    if (on_devices(e, kEveryDevice, [&](Device& dev, size_t i, std::string* m) {
+          if (i == 0) return ZG_OK;
+          *m = dev.init(first + static_cast<int>(i), c.subquery_capacity, c.work_budget);
+          if (c.flags & ZG_FLAG_FORWARD_ONLY) dev.invert = false;
+          return m->empty() ? ZG_OK : ZG_ECUDA;
+        }, &err)) {
+      delete e;
+      return fail(ZG_ECUDA, err);
+    }
   }
   *out = e;
   return ZG_OK;
@@ -573,15 +669,15 @@ static int publish_locked(zg_engine* e) {
       // journal cannot express (bulk load, new layout, no snapshot yet) rebuilds
       const char* nd = std::getenv("ZGPU_NO_DELTA");
       const bool no_delta = nd && *nd && *nd != '0';
-      std::vector<std::string> errs(1 + e->replicas.size());
-      on_all_devices(e, [&](Device& dev, size_t i) {  // every replica merges / builds for itself, concurrently
-        std::string err = no_delta ? std::string("full") : dev.publish_delta(e->store, e->schema, e->revision + 1);
-        if (err == "full") err = dev.publish_gpu(e->store, e->schema, e->revision + 1, verify);
-        else if (err.empty() && verify) err = dev.verify_against_host(e->store, e->schema);
-        errs[i] = err;
-      });
-      for (const auto& err : errs)
-        if (!err.empty()) return publish_failed(e, err);
+      // every replica merges / builds for itself, concurrently
+      std::string err;
+      if (on_devices(e, kEveryDevice, [&](Device& dev, size_t, std::string* m) {
+            *m = no_delta ? std::string("full") : dev.publish_delta(e->store, e->schema, e->revision + 1);
+            if (*m == "full") *m = dev.publish_gpu(e->store, e->schema, e->revision + 1, verify);
+            else if (m->empty() && verify) *m = dev.verify_against_host(e->store, e->schema);
+            return m->empty() ? ZG_OK : ZG_ECUDA;
+          }, &err))
+        return publish_failed(e, err);
       ++e->revision;
       e->store.journal_clear();
       e->last_built = HostSnapshot();
@@ -590,13 +686,13 @@ static int publish_locked(zg_engine* e) {
       return ZG_OK;
     }
     if (is_handle(e)) {  // host-built shards: each holds the relationships it owns
-      std::vector<std::string> errs(e->n_shards);
-      on_all_devices(e, [&](Device& dev, size_t i) {
-        HostSnapshot h = e->store.build(dev.own_rank, dev.own_count);
-        errs[i] = h.err.empty() ? dev.publish(h, e->schema, e->revision + 1) : h.err;
-      });
-      for (const auto& err : errs)
-        if (!err.empty()) return publish_failed(e, err);
+      std::string err;
+      if (on_devices(e, kEveryDevice, [&](Device& dev, size_t, std::string* m) {
+            HostSnapshot h = e->store.build(dev.own_rank, dev.own_count);
+            *m = h.err.empty() ? dev.publish(h, e->schema, e->revision + 1) : h.err;
+            return m->empty() ? ZG_OK : ZG_ECUDA;
+          }, &err))
+        return publish_failed(e, err);
       ++e->revision;
       e->store.journal_clear();
       e->shard_built.clear();
@@ -702,8 +798,6 @@ static std::string resolve_write(zg_engine* e, const zg_rel_str& r, zg_tuple* t)
   return "";
 }
 
-static int first_error(const std::vector<int>& rcs, const std::vector<std::string>& errs, std::string* err);
-
 static Store::Filter resolve_filter(const zg_engine* e, const zg_filter_str& f, std::string* err) {
   const Schema& sc = e->schema;
   Store::Filter o;
@@ -789,9 +883,17 @@ static bool filters_on_device(const zg_engine* e) {
 // A device's part of a filter or a collection: Device::match_filter or Device::match_expired.
 using DeviceMatch = std::function<int(Device&, uint64_t* count, std::vector<zg_tuple>* tuples, bool* too_big, std::string* err)>;
 
-// Runs `ask` on the first device, or on every shard of a sharded handle, or on shard `owner` alone (>= 0), adds up
-// the counts and concatenates the records, and counts a device filter of `shape`.
-static int ask_devices(zg_engine* e, int owner, Device::FilterShape shape, const DeviceMatch& ask, uint64_t* count,
+// The devices that answer from the resident snapshot (on_devices): replicas hold the same snapshot, so the first
+// device answers; every shard of a sharded handle holds its own relationships, and when the filter `f` names the
+// resource, its owner alone.
+static int snapshot_devices(const zg_engine* e, const Store::Filter* f = nullptr) {
+  if (!is_handle(e)) return kFirstDevice;
+  return f && f->has_res ? static_cast<int>(f->res % e->n_shards) : kEveryDevice;
+}
+
+// Runs `ask` on the snapshot devices `which`, adds up the counts and concatenates the records, and counts a device
+// filter of `shape`.
+static int ask_devices(zg_engine* e, int which, Device::FilterShape shape, const DeviceMatch& ask, uint64_t* count,
                        std::vector<zg_tuple>* tuples, bool* too_big) {
   *count = 0;
   *too_big = false;
@@ -799,19 +901,15 @@ static int ask_devices(zg_engine* e, int owner, Device::FilterShape shape, const
   const uint32_t S = is_handle(e) ? e->n_shards : 1;
   std::vector<uint64_t> n(S, 0);
   std::vector<std::vector<zg_tuple>> got(tuples ? S : 0);
-  std::vector<int> rcs(S, ZG_OK);
-  std::vector<std::string> errs(S);
   std::vector<char> big(S, 0);
-  auto one = [&](Device& dev, size_t k) {
-    bool b = false;
-    rcs[k] = ask(dev, &n[k], tuples ? &got[k] : nullptr, &b, &errs[k]);
-    big[k] = b;
-  };
-  if (S == 1) one(e->dev, 0);
-  else if (owner >= 0) one(shard(e, static_cast<uint32_t>(owner)), static_cast<size_t>(owner));
-  else on_all_devices(e, one);
   std::string err;
-  if (int rc = first_error(rcs, errs, &err)) return fail(rc == ZG_ENOMEM ? ZG_ECUDA : rc, err);
+  if (int rc = on_devices(e, which, [&](Device& dev, size_t k, std::string* m) {
+        bool b = false;
+        const int arc = ask(dev, &n[k], tuples ? &got[k] : nullptr, &b, m);
+        big[k] = b;
+        return arc;
+      }, &err))
+    return fail(rc == ZG_ENOMEM ? ZG_ECUDA : rc, err);
   for (uint32_t k = 0; k < S; ++k) {
     *count += n[k];
     *too_big = *too_big || big[k];
@@ -833,8 +931,7 @@ static int ask_devices(zg_engine* e, int owner, Device::FilterShape shape, const
 // caller runs Store::match instead (holding e->names exclusively).
 static int match_on_device(zg_engine* e, const Store::Filter& f, uint32_t now, uint64_t* count, std::vector<zg_tuple>* tuples,
                            bool* too_big) {
-  const int owner = is_handle(e) && f.has_res ? static_cast<int>(f.res % e->n_shards) : -1;
-  return ask_devices(e, owner, Device::filter_shape(f), [&](Device& dev, uint64_t* n, std::vector<zg_tuple>* got, bool* big,
+  return ask_devices(e, snapshot_devices(e, &f), Device::filter_shape(f), [&](Device& dev, uint64_t* n, std::vector<zg_tuple>* got, bool* big,
                                                             std::string* err) {
     return dev.match_filter(e->schema, f, now, n, got, nullptr, big, err);
   }, count, tuples, too_big);
@@ -982,7 +1079,7 @@ extern "C" int zg_collect_expired(zg_engine* e, int64_t before_unix, uint64_t* n
   if (on_device) {
     uint64_t count = 0;
     bool too_big = false;
-    int rc = ask_devices(e, -1, Device::kByScan, [&](Device& dev, uint64_t* n, std::vector<zg_tuple>* got, bool* big,
+    int rc = ask_devices(e, snapshot_devices(e), Device::kByScan, [&](Device& dev, uint64_t* n, std::vector<zg_tuple>* got, bool* big,
                                                      std::string* err) {
       return dev.match_expired(e->schema, before, n, got, big, err);
     }, &count, &found, &too_big);
@@ -1016,13 +1113,11 @@ extern "C" int zg_retire_unused_names(zg_engine* e, uint64_t* n_retired) {
   if (on_device) {
     const uint32_t S = is_handle(e) ? e->n_shards : 1;
     std::vector<Store::IdBits> got(S);
-    std::vector<int> rcs(S, ZG_OK);
-    std::vector<std::string> errs(S);
-    auto one = [&](Device& dev, size_t k) { rcs[k] = dev.scan_mentions(e->schema, &got[k], &errs[k]); };
-    if (S == 1) one(e->dev, 0);
-    else on_all_devices(e, one);
     std::string err;
-    if (int rc = first_error(rcs, errs, &err)) return fail(rc == ZG_ENOMEM ? ZG_ECUDA : rc, err);
+    if (int rc = on_devices(e, snapshot_devices(e), [&](Device& dev, size_t k, std::string* m) {
+          return dev.scan_mentions(e->schema, &got[k], m);
+        }, &err))
+      return fail(rc == ZG_ENOMEM ? ZG_ECUDA : rc, err);
     keep.swap(got[0]);
     for (uint32_t k = 1; k < S; ++k)
       for (size_t t = 0; t < got[k].size(); ++t) {
@@ -1197,23 +1292,18 @@ static zg_read_cursor make_cursor(const zg_engine* e, uint64_t fp, const PageKey
 static int page_on_device(zg_engine* e, const Store::Filter& f, uint32_t now, const PageKey* after, uint64_t want,
                           std::vector<zg_tuple>* found, std::vector<uint32_t>* exp, bool* too_big) {
   const uint32_t S = is_handle(e) ? e->n_shards : 1;
-  const int owner = S > 1 && f.has_res ? static_cast<int>(f.res % S) : -1;
   std::vector<std::vector<zg_tuple>> got(S);
   std::vector<std::vector<uint32_t>> got_exp(S);
   std::vector<Device::PageStats> st(S);
-  std::vector<int> rcs(S, ZG_OK);
-  std::vector<std::string> errs(S);
   std::vector<char> big(S, 0);
-  auto one = [&](Device& dev, size_t k) {
-    bool b = false;
-    rcs[k] = dev.page_filter(e->schema, f, now, after, want, &got[k], &got_exp[k], &st[k], &b, &errs[k]);
-    big[k] = b;
-  };
-  if (S == 1) one(e->dev, 0);
-  else if (owner >= 0) one(shard(e, static_cast<uint32_t>(owner)), static_cast<size_t>(owner));
-  else on_all_devices(e, one);
   std::string err;
-  if (int rc = first_error(rcs, errs, &err)) return fail(rc == ZG_ENOMEM ? ZG_ECUDA : rc, err);
+  if (int rc = on_devices(e, snapshot_devices(e, &f), [&](Device& dev, size_t k, std::string* m) {
+        bool b = false;
+        const int prc = dev.page_filter(e->schema, f, now, after, want, &got[k], &got_exp[k], &st[k], &b, m);
+        big[k] = b;
+        return prc;
+      }, &err))
+    return fail(rc == ZG_ENOMEM ? ZG_ECUDA : rc, err);
   *too_big = false;
   for (uint32_t k = 0; k < S; ++k) *too_big = *too_big || big[k];
   if (*too_big) return ZG_OK;
@@ -1430,22 +1520,11 @@ extern "C" int zg_watch_read(zg_engine* e, uint64_t since_revision, const char* 
 // Makes pending writes visible before a string entry point resolves against them. Takes both locks only when
 // there is something to publish; call it with NO lock held.
 static int publish_if_needed(zg_engine* e) {
-  if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
-  if (e->dev.shard_count > 1 && !is_handle(e)) return fail(ZG_EINVAL, kShardedMsg);
+  if (int rc = refuse(e, Call::kCheckGroup)) return rc;
   if (!e->dirty.load() && e->dev.snap) return ZG_OK;
   LOCK_DEVICE(e);
   LOCK_NAMES_UNIQUE(e);
   if (e->dirty.load() || !e->dev.snap) return publish_locked(e);
-  return ZG_OK;
-}
-
-// The first failing shard's code and message (per-shard steps run concurrently).
-static int first_error(const std::vector<int>& rcs, const std::vector<std::string>& errs, std::string* err) {
-  for (size_t k = 0; k < rcs.size(); ++k)
-    if (rcs[k]) {
-      *err = errs[k];
-      return rcs[k];
-    }
   return ZG_OK;
 }
 
@@ -1456,6 +1535,25 @@ struct ShardLists {
   std::vector<uint64_t> n;
   std::vector<uint8_t*> out;
 };
+
+// Lays out the inboxes of one exchange among the S shards from its count matrix (counts[k * S + d]: entries shard k
+// sends to shard d), for destinations d < n_dest: in d's inbox, shard k's entries follow those of the lower shards, and
+// tab[k] says where shard k writes them. inbox(d, n) returns d's inbox grown to n entries, or nullptr (then false).
+template <class Inbox>
+static bool lay_out_inboxes(uint32_t S, uint32_t n_dest, const std::vector<uint64_t>& counts, std::vector<PeerTable>* tab,
+                            Inbox&& inbox) {
+  for (uint32_t d = 0; d < n_dest; ++d) {
+    uint64_t at = 0;
+    for (uint32_t k = 0; k < S; ++k) {
+      (*tab)[k].base[d] = at;
+      at += counts[size_t(k) * S + d];
+    }
+    void* p = inbox(d, at);
+    if (!p) return false;
+    for (uint32_t k = 0; k < S; ++k) (*tab)[k].p[d] = p;
+  }
+  return true;
+}
 
 // The levels of dist.DeviceShardedChecker.check_bulk, driven in this process. Every shard routes its list to the
 // owners. Per level, every shard writes its queries straight into the owners' inboxes (where, the host computes from
@@ -1468,16 +1566,13 @@ static int sharded_levels(zg_engine* e, const ShardLists& L, PeerCounts* pc, boo
   const uint32_t S = e->n_shards;
   *overflow_out = false;
   std::vector<uint64_t> counts(size_t(S) * S, 0);  // [k * S + d]: queries shard k sends to shard d this level
-  std::vector<int> rcs(S, ZG_OK);
-  std::vector<std::string> errs(S);
-  auto first_error = [&]() { return ::first_error(rcs, errs, err); };
   const uint32_t now = now_of(e);
-  on_all_devices(e, [&](Device& dev, size_t k) {
-    dev.now = now;
-    rcs[k] = dev.peer_begin(L.items[k], L.n[k], &counts[k * S], &errs[k]);
-  });
   ++pc->round_trips;
-  if (int rc = first_error()) return rc;
+  if (int rc = on_devices(e, kEveryDevice, [&](Device& dev, size_t k, std::string* m) {
+        dev.now = now;
+        return dev.peer_begin(L.items[k], L.n[k], &counts[k * S], m);
+      }, err))
+    return rc;
   std::vector<PeerTable> tab(S);
   std::vector<cudaEvent_t> wait(S);
   auto events = [&](int level) {
@@ -1488,33 +1583,30 @@ static int sharded_levels(zg_engine* e, const ShardLists& L, PeerCounts* pc, boo
   int level = 0;
   for (;; ++level) {
     uint64_t total = 0;
-    for (uint32_t d = 0; d < S; ++d) {
-      uint64_t at = 0;
-      for (uint32_t k = 0; k < S; ++k) {
-        tab[k].base[d] = at;
-        at += counts[size_t(k) * S + d];
-      }
-      zg_check* inbox = shard(e, d).peer_inbox(level, at, err);
-      if (!inbox) return ZG_ENOMEM;
-      for (uint32_t k = 0; k < S; ++k) tab[k].p[d] = inbox;
-      total += at;
-    }
+    if (!lay_out_inboxes(S, S, counts, &tab, [&](uint32_t d, uint64_t n) {
+          total += n;
+          return shard(e, d).peer_inbox(level, n, err);
+        }))
+      return ZG_ENOMEM;
     if (total == 0) break;
     if (level > ZG_MAX_DEPTH + 1) {
       *err = "sub-query passes exceeded the depth cap";
       return ZG_ECUDA;
     }
-    on_all_devices(e, [&](Device& dev, size_t k) { rcs[k] = dev.peer_scatter(level, tab[k], &errs[k]); });
-    if (int rc = first_error()) return rc;
+    if (int rc = on_devices(e, kEveryDevice, [&](Device& dev, size_t k, std::string* m) {
+          return dev.peer_scatter(level, tab[k], m);
+        }, err))
+      return rc;
     events(level);
-    on_all_devices(e, [&](Device& dev, size_t k) {
-      bool o = false;
-      rcs[k] = dev.peer_pass(level, wait, &nsub[k], &counts[k * S], &o, no_wildcards, &errs[k]);
-      overflow[k] = o;
-    });
     ++pc->round_trips;
     pc->levels = std::max<uint64_t>(pc->levels, static_cast<uint64_t>(level) + 1);
-    if (int rc = first_error()) return rc;
+    if (int rc = on_devices(e, kEveryDevice, [&](Device& dev, size_t k, std::string* m) {
+          bool o = false;
+          const int prc = dev.peer_pass(level, wait, &nsub[k], &counts[k * S], &o, no_wildcards, m);
+          overflow[k] = o;
+          return prc;
+        }, err))
+      return rc;
     if (std::find(overflow.begin(), overflow.end(), 1) != overflow.end()) {
       *overflow_out = true;
       return ZG_OK;
@@ -1522,23 +1614,25 @@ static int sharded_levels(zg_engine* e, const ShardLists& L, PeerCounts* pc, boo
     for (uint32_t k = 0; k < S; ++k) pc->subqueries += nsub[k];
   }
   // values back: the deepest pass raised nothing; every shallower level folds in its children's values
-  for (int lv = level - 2; lv >= 0; --lv) {
+  auto values_of = [&](int lv) {
     for (uint32_t d = 0; d < S; ++d) {
-      tab[0].p[d] = const_cast<uint8_t*>(shard(e, d).peer_values(lv + 1));
+      tab[0].p[d] = const_cast<uint8_t*>(shard(e, d).peer_values(lv));
       tab[0].base[d] = 0;
     }
-    events(lv + 1);
-    on_all_devices(e, [&](Device& dev, size_t k) { rcs[k] = dev.peer_fold(lv, tab[0], wait, &errs[k]); });
-    if (int rc = first_error()) return rc;
+    events(lv);
+  };
+  for (int lv = level - 2; lv >= 0; --lv) {
+    values_of(lv + 1);
+    if (int rc = on_devices(e, kEveryDevice, [&](Device& dev, size_t, std::string* m) {
+          return dev.peer_fold(lv, tab[0], wait, m);
+        }, err))
+      return rc;
   }
-  for (uint32_t d = 0; d < S; ++d) {
-    tab[0].p[d] = const_cast<uint8_t*>(shard(e, d).peer_values(0));
-    tab[0].base[d] = 0;
-  }
-  events(0);
-  on_all_devices(e, [&](Device& dev, size_t k) { rcs[k] = dev.peer_finish(tab[0], wait, L.out[k], &errs[k]); });
+  values_of(0);
   ++pc->round_trips;
-  return first_error();
+  return on_devices(e, kEveryDevice, [&](Device& dev, size_t k, std::string* m) {
+    return dev.peer_finish(tab[0], wait, L.out[k], m);
+  }, err);
 }
 
 // sharded_levels, and on overflow the same in halves (checks are independent): the first half of the items taken in
@@ -1580,24 +1674,18 @@ static int run_sharded(zg_engine* e, const zg_check* items, uint64_t n, uint8_t*
   return run_sharded_lists(e, L, pc, false, err);
 }
 
-// Runs one group of queued requests; the caller holds the device lock.
-static void run_group(zg_engine* e, std::vector<BatchReq*>& group) {
-  int rc = ZG_OK;
-  std::string err;
+// Answers one group of queued requests; the caller holds the device lock.
+static int run_group(zg_engine* e, const std::vector<BatchReq*>& group, std::string* err) {
+  if (int rc = refuse(e, Call::kCheckGroup, err)) return rc;
   bool published = e->dev.snap != nullptr;
-  for (uint32_t k = 1; k < e->n_shards && !e->host_only; ++k) published = published && shard(e, k).snap;
-  if (e->dev.shard_count > 1 && !is_handle(e)) {
-    rc = ZG_EINVAL;
-    err = kShardedMsg;
-  } else if (e->host_only) {
-    rc = ZG_ECUDA;
-    err = "host-only engine: no CUDA device, and libzgpu has no CPU fallback";
-  } else if (!published) {
-    rc = ZG_ENOSNAPSHOT;
-    err = "no snapshot published (call zg_publish)";
-  } else if (is_handle(e)) {
-    uint64_t total = 0;
-    for (BatchReq* r : group) total += r->n;
+  for (uint32_t k = 1; k < e->n_shards; ++k) published = published && shard(e, k).snap;
+  if (!published) {
+    *err = "no snapshot published (call zg_publish)";
+    return ZG_ENOSNAPSHOT;
+  }
+  uint64_t total = 0;
+  for (BatchReq* r : group) total += r->n;
+  if (is_handle(e)) {
     const size_t bytes = total * (sizeof(zg_check) + 1);  // the items, then their answers
     if (e->group_pin_cap < bytes) {
       if (e->group_pin) cudaFreeHost(e->group_pin);
@@ -1607,127 +1695,86 @@ static void run_group(zg_engine* e, std::vector<BatchReq*>& group) {
       else cudaGetLastError();
     }
     if (!e->group_pin) {
-      rc = ZG_ENOMEM;
-      err = "out of pinned host memory (sharded handle staging)";
-    } else {
-      zg_check* items = static_cast<zg_check*>(e->group_pin);
-      uint64_t off = 0;
-      for (BatchReq* r : group) {
-        std::memcpy(items + off, r->items, r->n * sizeof(zg_check));
-        off += r->n;
-      }
-      uint8_t* answers = reinterpret_cast<uint8_t*>(items + total);
-      e->last_group = PeerCounts();
-      rc = run_sharded(e, items, total, answers, &e->last_group, &err);
-      off = 0;
-      for (BatchReq* r : group) {
-        if (!rc) std::memcpy(r->out, answers + off, r->n);
-        off += r->n;
-      }
-      if (group.size() > 1) {
-        ++e->dev.coalesced_launches;
-        e->dev.coalesced_requests += group.size();
-      }
+      *err = "out of pinned host memory (sharded handle staging)";
+      return ZG_ENOMEM;
     }
-  } else {
-    std::vector<Device::HostReq> reqs;
-    reqs.reserve(group.size());
-    uint64_t total = 0;
+    zg_check* items = static_cast<zg_check*>(e->group_pin);
+    uint64_t off = 0;
     for (BatchReq* r : group) {
-      reqs.push_back({r->items, r->n, r->out});
-      total += r->n;
+      std::memcpy(items + off, r->items, r->n * sizeof(zg_check));
+      off += r->n;
     }
-    const size_t nd = 1 + e->replicas.size();
-    if (nd == 1 || total < nd * 4096) {
-      e->dev.now = now_of(e);
-      rc = e->dev.check_host_multi(reqs, &err);
-    } else {
-      // replicas: every device answers a contiguous slice of the group's items
-      std::vector<std::vector<Device::HostReq>> part(nd);
-      const uint64_t per = (total + nd - 1) / nd;
-      size_t d = 0;
-      uint64_t room = per;
-      for (const auto& r : reqs) {
-        uint64_t off = 0;
-        while (off < r.n) {
-          const uint64_t take = std::min(room, r.n - off);
-          part[d].push_back({r.items + off, take, r.out + off});
-          off += take;
-          room -= take;
-          if (room == 0 && d + 1 < nd) {
-            ++d;
-            room = per;
-          }
-        }
+    uint8_t* answers = reinterpret_cast<uint8_t*>(items + total);
+    e->last_group = PeerCounts();
+    const int rc = run_sharded(e, items, total, answers, &e->last_group, err);
+    off = 0;
+    for (BatchReq* r : group) {
+      if (!rc) std::memcpy(r->out, answers + off, r->n);
+      off += r->n;
+    }
+    if (group.size() > 1) {
+      ++e->dev.coalesced_launches;
+      e->dev.coalesced_requests += group.size();
+    }
+    return rc;
+  }
+  std::vector<Device::HostReq> reqs;
+  reqs.reserve(group.size());
+  for (BatchReq* r : group) reqs.push_back({r->items, r->n, r->out});
+  const size_t nd = 1 + e->replicas.size();
+  if (nd == 1 || total < nd * 4096) {
+    e->dev.now = now_of(e);
+    return e->dev.check_host_multi(reqs, err);
+  }
+  // replicas: every device answers a contiguous slice of the group's items
+  std::vector<std::vector<Device::HostReq>> part(nd);
+  const uint64_t per = (total + nd - 1) / nd;
+  size_t d = 0;
+  uint64_t room = per;
+  for (const auto& r : reqs) {
+    uint64_t off = 0;
+    while (off < r.n) {
+      const uint64_t take = std::min(room, r.n - off);
+      part[d].push_back({r.items + off, take, r.out + off});
+      off += take;
+      room -= take;
+      if (room == 0 && d + 1 < nd) {
+        ++d;
+        room = per;
       }
-      std::vector<int> rcs(nd, ZG_OK);
-      std::vector<std::string> errs(nd);
-      const uint32_t now = now_of(e);
-      on_all_devices(e, [&](Device& dev, size_t i) {
-        dev.now = now;
-        if (!part[i].empty()) rcs[i] = dev.check_host_multi(part[i], &errs[i]);
-      });
-      for (size_t i = 0; i < nd && !rc; ++i)
-        if (rcs[i]) {
-          rc = rcs[i];
-          err = errs[i];
-        }
     }
   }
-  for (BatchReq* r : group) {
-    r->rc = rc;
-    r->err = err;
-  }
+  const uint32_t now = now_of(e);
+  return on_devices(e, kEveryDevice, [&](Device& dev, size_t i, std::string* m) {
+    dev.now = now;
+    return part[i].empty() ? ZG_OK : dev.check_host_multi(part[i], m);
+  }, err);
 }
 
 extern "C" int zg_check_bulk(zg_engine* e, const zg_check* items, uint64_t n, uint8_t* out) {
   NEED_SCHEMA(e, ZG_ENOSCHEMA);
   if ((!items || !out) && n) return fail(ZG_EINVAL, "NULL argument");
   if (n == 0) return ZG_OK;
-  Batcher& b = e->batcher;
-  BatchReq me{items, n, out};
-  std::unique_lock<std::mutex> lk(b.m);
-  b.queue.push_back(&me);
-  if (b.leader_active) {
-    ++b.waited;
-    me.cv.wait(lk, [&] { return me.done || me.lead; });
-  }
-  if (!me.done) {
-    // leader (nobody was leading, or the previous leader handed over to the head of the queue -- me): take as many
-    // queued requests as fit one launch, mine first, answer them, wake their callers, hand leadership on
-    b.leader_active = true;
-    std::vector<BatchReq*> group;
-    lk.unlock();
-    {
-      // the device first, the group second: whatever queued while this leader waited for the GPU (behind a batch of
-      // lookups, a publish, the previous group's tail) rides along
-      std::lock_guard<FairMutex> dev_lock(e->mu);
-      lk.lock();
-      uint64_t total = 0;
-      size_t take = 0;
-      while (take < b.queue.size() && (group.empty() || total + b.queue[take]->n <= Batcher::kMaxItemsPerLaunch)) {
-        total += b.queue[take]->n;
-        group.push_back(b.queue[take++]);
-      }
-      b.queue.erase(b.queue.begin(), b.queue.begin() + static_cast<long>(take));
-      lk.unlock();
-      run_group(e, group);
-    }
-    lk.lock();
-    ++b.groups;
-    for (BatchReq* r : group) {
-      r->done = true;
-      if (r != &me) r->cv.notify_one();
-    }
-    if (!b.queue.empty()) {
-      ++b.handed_over;
-      b.queue.front()->lead = true;
-      b.queue.front()->cv.notify_one();
-    } else {
-      b.leader_active = false;
-    }
-  }
-  lk.unlock();
+  BatchReq me;
+  me.items = items;
+  me.n = n;
+  me.out = out;
+  e->batcher.submit(
+      &me, e->mu,
+      [](const std::vector<BatchReq*>& queue) {  // as many callers as fit one launch, and always the first
+        uint64_t total = queue[0]->n;
+        size_t take = 1;
+        while (take < queue.size() && total + queue[take]->n <= kMaxItemsPerLaunch) total += queue[take++]->n;
+        return take;
+      },
+      [e](const std::vector<BatchReq*>& group) {
+        std::string err;
+        const int rc = run_group(e, group, &err);
+        for (BatchReq* r : group) {
+          r->rc = rc;
+          r->err = err;
+        }
+      });
   return me.rc ? fail(me.rc, me.err) : ZG_OK;
 }
 
@@ -1735,9 +1782,7 @@ extern "C" int zg_check_bulk_device(zg_engine* e, const zg_check* d_items, uint6
   NEED_SCHEMA(e, ZG_ENOSCHEMA);
   if ((!d_items || !d_out) && n) return fail(ZG_EINVAL, "NULL argument");
   std::lock_guard<FairMutex> g(e->mu);
-  if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
-  if (is_handle(e)) return fail(ZG_EINVAL, kHandleDeviceMsg);
-  if (e->dev.shard_count > 1) return fail(ZG_EINVAL, kShardedMsg);
+  if (int rc = refuse(e, Call::kDeviceChecks)) return rc;
   e->dev.now = now_of(e);
   std::string err;
   int rc = e->dev.check_device(d_items, n, d_out, static_cast<cudaStream_t>(stream), true, nullptr, &err);
@@ -1748,8 +1793,7 @@ extern "C" int zg_count_alg_bytes(zg_engine* e, const zg_check* items, uint64_t 
   NEED_SCHEMA(e, ZG_ENOSCHEMA);
   if (!items || !bytes) return fail(ZG_EINVAL, "NULL argument");
   std::lock_guard<FairMutex> g(e->mu);
-  if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
-  if (is_handle(e)) return fail(ZG_EINVAL, kHandleDeviceMsg);
+  if (int rc = refuse(e, Call::kDeviceBuffers)) return rc;
   e->dev.now = now_of(e);
   std::string err;
   void *d_in = nullptr, *d_out = nullptr;
@@ -1771,7 +1815,7 @@ extern "C" int zg_phase_clocks(zg_engine* e, uint64_t cycles[5]) {
   NEED_SCHEMA(e, ZG_ENOSCHEMA);
   if (!cycles) return fail(ZG_EINVAL, "NULL argument");
   std::lock_guard<FairMutex> g(e->mu);
-  if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
+  if (int rc = refuse(e, Call::kDevice)) return rc;
   std::string err;
   const int rc = e->dev.read_phase_clocks(cycles, &err);
   return rc ? fail(rc, err) : ZG_OK;
@@ -2020,8 +2064,6 @@ static Device::IngressLiterals ingress_literals(zg_engine* e, const char* res_ty
   return lit;
 }
 
-static const char* kHostOnlyMsg = "host-only engine: no CUDA device, and libzgpu has no CPU fallback";
-
 extern "C" int zg_resolve_checks_packed_device(zg_engine* e, const char* res_type, const char* relation,
                                                const char* subj_type, const char* subj_rel, const char* d_res_ids,
                                                const uint32_t* d_res_off, const char* d_subj_ids,
@@ -2029,8 +2071,7 @@ extern "C" int zg_resolve_checks_packed_device(zg_engine* e, const char* res_typ
   NEED_SCHEMA(e, ZG_ENOSCHEMA);
   if (!(res_type && relation && subj_type && (n == 0 || (d_res_ids && d_res_off && d_subj_ids && d_out))))
     return fail(ZG_EINVAL, "NULL argument");
-  if (e->host_only) return fail(ZG_ECUDA, kHostOnlyMsg);
-  if (is_handle(e)) return fail(ZG_EINVAL, kHandleDeviceMsg);
+  if (int rc = refuse(e, Call::kDeviceBuffers)) return rc;
   if (n == 0) return ZG_OK;
   LOCK_DEVICE(e);
   LOCK_NAMES_SHARED(e);
@@ -2048,11 +2089,10 @@ extern "C" int zg_check_bulk_packed_ingress(zg_engine* e, const char* res_type, 
                                             uint64_t n, uint8_t* out) {
   NEED_SCHEMA(e, ZG_ENOSCHEMA);
   if (!PACKED_ARGS_OK()) return fail(ZG_EINVAL, "NULL argument");
-  if (e->host_only) return fail(ZG_ECUDA, kHostOnlyMsg);
-  if (is_handle(e)) return fail(ZG_EINVAL, kHandleDeviceMsg);
-  if (e->dev.shard_count > 1) return fail(ZG_EINVAL, kShardedMsg);
+  int rc = refuse(e, Call::kDeviceChecks);
+  if (rc) return rc;
   if (n == 0) return ZG_OK;
-  int rc = publish_if_needed(e);
+  rc = publish_if_needed(e);
   if (rc) return rc;
   LOCK_DEVICE(e);
   LOCK_NAMES_SHARED(e);
@@ -2287,6 +2327,116 @@ extern "C" int zg_list_postfilter(zg_engine* e, const char* body, size_t len, co
   return with_stable_names(e, [&] { return list_postfilter_once(e, body, len, tpl, n_tpl, out, cap, out_len); });
 }
 
+// The steps the handle's LookupResources and LookupSubjects rounds share (run_sharded_lookup, run_sharded_subjects).
+// end(dev, err) ends the round on one shard; a failed step ends it on every shard, so that no shard keeps its snapshot
+// resident. *waits counts the round's host waits (hl_round_trips / hs_waits), and `what` names the round's buffers in
+// out-of-memory messages.
+struct HandleRound {
+  zg_engine* e;
+  int (*end)(Device& dev, std::string* err);
+  const char* what;
+  uint64_t* waits;
+  std::string* err;
+
+  int fail_round(int rc) {
+    on_all_devices(e, [&](Device& dev, size_t) { end(dev, nullptr); });
+    return rc;
+  }
+  // fn(device, k, err) on every shard
+  template <class F>
+  int on_shards(F&& fn) {
+    const int rc = on_devices(e, kEveryDevice, fn, err);
+    return rc ? fail_round(rc) : ZG_OK;
+  }
+  // Every shard's candidates as check items in its hl.items, with room for their codes and answer keys: n[k] on shard
+  // k. cand(dev, items, cap, &n, err) with items == nullptr asks the capacity items needs. One wait.
+  template <class Cand>
+  int candidates(Cand&& cand, std::vector<uint64_t>* n) {
+    ++*waits;
+    return on_shards([&](Device& dev, size_t k, std::string* m) {
+      uint64_t need = 0;
+      const int rc = cand(dev, nullptr, 0, &need, m);
+      if (!rc && (!dev.hl_ensure(dev.hl.items, need * sizeof(zg_check)) || !dev.hl_ensure(dev.hl.codes, need) ||
+                  !dev.hl_ensure(dev.hl.routed, need * 8))) {
+        *m = std::string("out of device memory (sharded handle ") + what + " candidates)";
+        return ZG_ENOMEM;
+      }
+      return rc ? rc : cand(dev, dev.hl.items.as<zg_check>(), need, &(*n)[k], m);
+    });
+  }
+  // The n[k] checks of every shard's hl.items through the handle's check protocol, where they lie; codes in hl.codes.
+  int verify(const std::vector<uint64_t>& n, bool no_wildcards) {
+    ShardLists L;
+    for (uint32_t k = 0; k < e->n_shards; ++k) {
+      L.items.push_back(shard(e, k).hl.items.as<zg_check>());
+      L.n.push_back(n[k]);
+      L.out.push_back(shard(e, k).hl.codes.as<uint8_t>());
+    }
+    PeerCounts pc;
+    const int rc = run_sharded_lists(e, L, &pc, no_wildcards, err);
+    *waits += pc.round_trips;
+    return rc ? fail_round(rc) : ZG_OK;
+  }
+  // The answer keys, gathered on shard 0 (home 0: every key goes there). route(dev, k, counts, err) writes shard k's
+  // keys to its hl.routed and counts them by destination; every shard puts them into shard 0's hl.keys behind those of
+  // the lower shards. Once every put is done, finish(d0, n_keys, &n_ids, err) sorts and splits them on shard 0 into
+  // hl.ids while every other shard ends its round, and the n_ids ids are copied into *host.
+  template <class Route, class Finish>
+  int gather_keys(Route&& route, Finish&& finish, std::vector<uint32_t>* host) {
+    const uint32_t S = e->n_shards;
+    std::vector<uint64_t> counts(size_t(S) * S, 0);
+    ++*waits;
+    if (int rc = on_shards([&](Device& dev, size_t k, std::string* m) { return route(dev, k, &counts[k * S], m); }))
+      return rc;
+    std::vector<PeerTable> tab(S);
+    Device& d0 = e->dev;
+    uint64_t n_keys = 0;
+    if (!lay_out_inboxes(S, 1, counts, &tab, [&](uint32_t, uint64_t n) -> void* {
+          n_keys = n;
+          return d0.hl_ensure(d0.hl.keys, n * 8) && d0.hl_ensure(d0.hl.ids, n * 4) ? d0.hl.keys.p : nullptr;
+        })) {
+      *err = std::string("out of device memory (sharded handle ") + what + " keys)";
+      return fail_round(ZG_ENOMEM);
+    }
+    if (int rc = on_shards([&](Device& dev, size_t k, std::string* m) {
+          return dev.peer_put(dev.hl.routed.as<unsigned long long>(), counts[k * S], 1, tab[k], 0, m);
+        }))
+      return rc;
+    std::vector<cudaEvent_t> wait(S);
+    for (uint32_t k = 0; k < S; ++k) wait[k] = shard(e, k).peer_event(0);
+    uint64_t n_ids = 0;
+    ++*waits;
+    if (int rc = on_shards([&](Device& dev, size_t k, std::string* m) {
+          if (k) return end(dev, m);
+          const int wrc = dev.peer_wait(wait, m);
+          return wrc ? wrc : finish(dev, n_keys, &n_ids, m);
+        }))
+      return rc;
+    host->resize(n_ids);
+    if (n_ids) {
+      const cudaError_t ce = cudaSetDevice(d0.device) == cudaSuccess
+                                 ? cudaMemcpy(host->data(), d0.hl.ids.p, n_ids * 4, cudaMemcpyDeviceToHost)
+                                 : cudaGetLastError();
+      ++*waits;
+      if (ce != cudaSuccess) {
+        *err = std::string("cudaMemcpy (lookup answers): ") + cudaGetErrorString(ce);
+        return ZG_ECUDA;
+      }
+    }
+    return ZG_OK;
+  }
+};
+
+static int end_lookup_round(Device& dev, std::string* err) {
+  uint64_t mask = 0, none[kMaxLookupGroup];  // a round holds at most kMaxLookupGroup lookups
+  return dev.shard_lookup_finish(nullptr, 0, nullptr, none, &mask, err);
+}
+
+static int end_subjects_round(Device& dev, std::string* err) {
+  uint64_t listed = 0, excluded = 0;
+  return dev.shard_subjects_finish(nullptr, 0, nullptr, &listed, &excluded, err);
+}
+
 // LookupResources on a sharded handle (ZG_FLAG_HANDLE_LOOKUPS): one round of dist.DeviceShardedLookup._round over
 // reqs[lo, lo + K) (K <= 64), driven in this process; ids[i] / rcs[i] answer reqs[i]. The handle is every rank, so
 // every answer goes to shard 0. Shard k owns the objects whose id % S == k and discovers only those in its reverse
@@ -2307,28 +2457,17 @@ static int run_sharded_lookup(zg_engine* e, const std::vector<Device::LookupReq>
   const std::vector<Device::LookupReq> round(reqs.begin() + static_cast<long>(lo), reqs.begin() + static_cast<long>(lo + K));
   const std::vector<uint8_t> home(K, 0);
   const uint64_t cap = e->dev.lookup_walk_cap();
-  std::vector<int> src(S, ZG_OK);
-  std::vector<std::string> errs(S);
-  std::vector<uint64_t> per(K);
-  auto first_error = [&]() { return ::first_error(src, errs, err); };
-  // a failed round is ended on every shard, so that no shard keeps its snapshot resident
-  auto fail_round = [&](int rc) {
-    on_all_devices(e, [&](Device& dev, size_t) {
-      uint64_t mask = 0;
-      std::vector<uint64_t> none(K);
-      dev.shard_lookup_finish(nullptr, 0, nullptr, none.data(), &mask, nullptr);
-    });
-    return rc;
-  };
+  HandleRound R{e, end_lookup_round, "lookup", &e->hl_round_trips, err};
   ++e->hl_rounds;
-  on_all_devices(e, [&](Device& dev, size_t k) {
-    src[k] = !dev.hl_ensure(dev.hl.front[0], K * 8) || !dev.hl_ensure(dev.hl.next, cap * 8)
-                 ? ZG_ENOMEM
-                 : dev.shard_lookup_begin(round, home.data(), cap, dev.hl.front[0].as<unsigned long long>(), &errs[k]);
-    if (src[k] == ZG_ENOMEM && errs[k].empty()) errs[k] = "out of device memory (sharded handle lookup buffers)";
-  });
   ++e->hl_round_trips;
-  if (int rc = first_error()) return fail_round(rc);
+  if (int rc = R.on_shards([&](Device& dev, size_t, std::string* m) {
+        const int brc = !dev.hl_ensure(dev.hl.front[0], K * 8) || !dev.hl_ensure(dev.hl.next, cap * 8)
+                            ? ZG_ENOMEM
+                            : dev.shard_lookup_begin(round, home.data(), cap, dev.hl.front[0].as<unsigned long long>(), m);
+        if (brc == ZG_ENOMEM && m->empty()) *m = "out of device memory (sharded handle lookup buffers)";
+        return brc;
+      }))
+    return rc;
   // ---- the walk
   const bool exhaustive = !e->dev.use_rbfs;  // ZGPU_NO_RBFS=1: every owned resource of the type is a candidate
   bool overflow = false;
@@ -2338,17 +2477,18 @@ static int run_sharded_lookup(zg_engine* e, const std::vector<Device::LookupReq>
   std::vector<cudaEvent_t> wait;
   uint64_t n_in = K;
   for (int level = 0; !exhaustive; ++level) {
-    on_all_devices(e, [&](Device& dev, size_t k) {
-      bool o = false;
-      src[k] = level ? dev.peer_wait(wait, &errs[k]) : ZG_OK;
-      if (!src[k])
-        src[k] = dev.shard_lookup_expand(dev.hl.front[level & 1].as<unsigned long long>(), n_in, level,
-                                         dev.hl.next.as<unsigned long long>(), &n_out[k], &o, &errs[k]);
-      ovf[k] = o;
-    });
     ++e->hl_levels;
     ++e->hl_round_trips;
-    if (int rc = first_error()) return fail_round(rc);
+    if (int rc = R.on_shards([&](Device& dev, size_t k, std::string* m) {
+          bool o = false;
+          int xrc = level ? dev.peer_wait(wait, m) : ZG_OK;
+          if (!xrc)
+            xrc = dev.shard_lookup_expand(dev.hl.front[level & 1].as<unsigned long long>(), n_in, level,
+                                          dev.hl.next.as<unsigned long long>(), &n_out[k], &o, m);
+          ovf[k] = o;
+          return xrc;
+        }))
+      return rc;
     uint64_t total = 0;
     for (uint32_t k = 0; k < S; ++k) total += n_out[k];
     overflow = std::find(ovf.begin(), ovf.end(), 1) != ovf.end();
@@ -2364,14 +2504,14 @@ static int run_sharded_lookup(zg_engine* e, const std::vector<Device::LookupReq>
       Device& dev = shard(e, d);
       if (!dev.hl_ensure(dev.hl.front[(level + 1) & 1], total * 8)) {
         *err = "out of device memory (sharded handle lookup frontier)";
-        return fail_round(ZG_ENOMEM);
+        return R.fail_round(ZG_ENOMEM);
       }
       for (uint32_t k = 0; k < S; ++k) tab[k].p[d] = dev.hl.front[(level + 1) & 1].p;
     }
-    on_all_devices(e, [&](Device& dev, size_t k) {
-      src[k] = dev.peer_put(dev.hl.next.as<unsigned long long>(), n_out[k], S, tab[k], level, &errs[k]);
-    });
-    if (int rc = first_error()) return fail_round(rc);
+    if (int rc = R.on_shards([&](Device& dev, size_t k, std::string* m) {
+          return dev.peer_put(dev.hl.next.as<unsigned long long>(), n_out[k], S, tab[k], level, m);
+        }))
+      return rc;
     wait.clear();
     for (uint32_t k = 0; k < S; ++k) wait.push_back(shard(e, k).peer_event(level));
     e->hl_frontier += total;
@@ -2383,82 +2523,33 @@ static int run_sharded_lookup(zg_engine* e, const std::vector<Device::LookupReq>
     if (int rc = run_sharded_lookup(e, reqs, lo, h, ids, rcs, err)) return rc;
     return run_sharded_lookup(e, reqs, lo + h, K - h, ids, rcs, err);
   }
-  if (overflow || exhaustive) ++e->hl_fallbacks;
+  const bool every = overflow || exhaustive;
+  if (every) ++e->hl_fallbacks;
   // ---- the candidates, verified where they lie
   std::vector<uint64_t> nc(S);
-  on_all_devices(e, [&](Device& dev, size_t k) {
-    uint64_t need = 0;
-    src[k] = dev.shard_lookup_candidates(overflow || exhaustive, nullptr, 0, &need, &errs[k]);
-    if (!src[k] && (!dev.hl_ensure(dev.hl.items, need * sizeof(zg_check)) || !dev.hl_ensure(dev.hl.codes, need) ||
-                    !dev.hl_ensure(dev.hl.routed, need * 8))) {
-      src[k] = ZG_ENOMEM;
-      errs[k] = "out of device memory (sharded handle lookup candidates)";
-    }
-    if (!src[k]) src[k] = dev.shard_lookup_candidates(overflow || exhaustive, dev.hl.items.as<zg_check>(), need, &nc[k], &errs[k]);
-  });
-  ++e->hl_round_trips;
-  if (int rc = first_error()) return fail_round(rc);
-  ShardLists V;
-  for (uint32_t k = 0; k < S; ++k) {
-    V.items.push_back(shard(e, k).hl.items.as<zg_check>());
-    V.n.push_back(nc[k]);
-    V.out.push_back(shard(e, k).hl.codes.as<uint8_t>());
-    e->hl_candidates += nc[k];
-  }
-  PeerCounts pc;
-  int vrc = run_sharded_lists(e, V, &pc, false, err);
-  e->hl_round_trips += pc.round_trips;
-  if (vrc) return fail_round(vrc);
+  if (int rc = R.candidates([&](Device& dev, zg_check* items, uint64_t room, uint64_t* n, std::string* m) {
+        return dev.shard_lookup_candidates(every, items, room, n, m);
+      }, &nc))
+    return rc;
+  for (uint64_t n : nc) e->hl_candidates += n;
+  if (int rc = R.verify(nc, false)) return rc;
   // ---- the answer keys, gathered, sorted and split on shard 0
-  std::vector<uint64_t> counts(size_t(S) * S, 0);
-  on_all_devices(e, [&](Device& dev, size_t k) {
-    src[k] = dev.shard_lookup_route(dev.hl.codes.as<uint8_t>(), nc[k], S, dev.hl.routed.as<unsigned long long>(), &counts[k * S],
-                                    &errs[k]);
-  });
-  ++e->hl_round_trips;
-  if (int rc = first_error()) return fail_round(rc);
-  uint64_t n_keys = 0;
-  for (uint32_t k = 0; k < S; ++k) {
-    tab[k].base[0] = n_keys;
-    n_keys += counts[size_t(k) * S];
-  }
-  Device& d0 = e->dev;
-  if (!d0.hl_ensure(d0.hl.keys, n_keys * 8) || !d0.hl_ensure(d0.hl.ids, n_keys * 4)) {
-    *err = "out of device memory (sharded handle lookup keys)";
-    return fail_round(ZG_ENOMEM);
-  }
-  for (uint32_t k = 0; k < S; ++k) tab[k].p[0] = d0.hl.keys.p;
-  on_all_devices(e, [&](Device& dev, size_t k) {
-    src[k] = dev.peer_put(dev.hl.routed.as<unsigned long long>(), counts[k * S], 1, tab[k], 0, &errs[k]);
-  });
-  if (int rc = first_error()) return fail_round(rc);
-  wait.clear();
-  for (uint32_t k = 0; k < S; ++k) wait.push_back(shard(e, k).peer_event(0));
+  std::vector<uint64_t> per(K);
   uint64_t err_mask = 0;
-  on_all_devices(e, [&](Device& dev, size_t k) {
-    uint64_t mask = 0;
-    std::vector<uint64_t> none(K);
-    src[k] = k ? dev.shard_lookup_finish(nullptr, 0, nullptr, none.data(), &mask, &errs[k])  // ends the round
-               : dev.peer_wait(wait, &errs[k]);
-    if (!k && !src[k])
-      src[k] = dev.shard_lookup_finish(dev.hl.keys.as<unsigned long long>(), n_keys, dev.hl.ids.as<uint32_t>(), per.data(),
-                                       &err_mask, &errs[k]);
-  });
-  ++e->hl_round_trips;
-  if (int rc = first_error()) return fail_round(rc);
-  uint64_t n_ids = 0;
-  for (uint64_t m : per) n_ids += m;
-  std::vector<uint32_t> host(n_ids);
-  if (n_ids) {
-    const cudaError_t ce = cudaSetDevice(d0.device) == cudaSuccess
-                               ? cudaMemcpy(host.data(), d0.hl.ids.p, n_ids * 4, cudaMemcpyDeviceToHost)
-                               : cudaGetLastError();
-    ++e->hl_round_trips;
-    if (ce != cudaSuccess) {
-      *err = std::string("cudaMemcpy (lookup answers): ") + cudaGetErrorString(ce);
-      return ZG_ECUDA;
-    }
-  }
+  std::vector<uint32_t> host;
+  if (int rc = R.gather_keys(
+          [&](Device& dev, size_t k, uint64_t* counts, std::string* m) {
+            return dev.shard_lookup_route(dev.hl.codes.as<uint8_t>(), nc[k], S, dev.hl.routed.as<unsigned long long>(),
+                                          counts, m);
+          },
+          [&](Device& d0, uint64_t n_keys, uint64_t* n_ids, std::string* m) {
+            const int frc = d0.shard_lookup_finish(d0.hl.keys.as<unsigned long long>(), n_keys, d0.hl.ids.as<uint32_t>(),
+                                                   per.data(), &err_mask, m);
+            for (uint64_t x : per) *n_ids += x;
+            return frc;
+          },
+          &host))
+    return rc;
   uint64_t off = 0;
   for (size_t k = 0; k < K; ++k) {
     if ((err_mask >> k) & 1) (*rcs)[lo + k] = ZG_EDEPTH;
@@ -2477,9 +2568,9 @@ static void run_lookup_group(zg_engine* e, std::vector<zg_engine::LookupJob*>& g
       j->err = msg;
     }
   };
-  if (e->host_only) return fail_all(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
-  const bool handle = is_handle(e) && e->handle_lookups;
-  if (e->dev.shard_count > 1 && !handle) return fail_all(ZG_EINVAL, is_handle(e) ? kHandleLookupMsg : kShardedMsg);
+  std::string why;
+  if (int rc = refuse(e, Call::kLookup, &why)) return fail_all(rc, why);
+  const bool handle = is_handle(e);
   if (e->dirty.load() || !e->dev.snap) {  // a handle's failed publish clears every shard's snapshot
     LOCK_NAMES_UNIQUE(e);
     int rc = publish_locked(e);
@@ -2538,25 +2629,18 @@ static void run_lookup_group(zg_engine* e, std::vector<zg_engine::LookupJob*>& g
       }
       std::vector<std::vector<std::vector<uint32_t>>> pids(nd);
       std::vector<std::vector<int>> prcs(nd);
-      std::vector<int> drc(nd, ZG_OK);
-      std::vector<std::string> derr(nd);
       const uint32_t now = e->dev.now;
-      on_all_devices(e, [&](Device& dev, size_t i) {
+      rc = on_devices(e, kEveryDevice, [&](Device& dev, size_t i, std::string* m) {
         dev.now = now;
-        if (!part[i].empty()) drc[i] = dev.lookup_batch(part[i], &pids[i], &prcs[i], &derr[i]);
-      });
+        return part[i].empty() ? ZG_OK : dev.lookup_batch(part[i], &pids[i], &prcs[i], m);
+      }, &err);
       ids.resize(reqs.size());
       rcs.assign(reqs.size(), ZG_OK);
-      for (size_t i = 0; i < nd; ++i) {
-        if (drc[i] && !rc) {
-          rc = drc[i];
-          err = derr[i];
-        }
-        for (size_t k = 0; k < which[i].size() && !drc[i]; ++k) {
+      for (size_t i = 0; i < nd && !rc; ++i)
+        for (size_t k = 0; k < which[i].size(); ++k) {
           ids[which[i][k]] = std::move(pids[i][k]);
           rcs[which[i][k]] = prcs[i][k];
         }
-      }
     }
     if (rc) return fail_all(rc, err);
     for (size_t r = 0; r < reqs.size(); ++r) {
@@ -2636,36 +2720,10 @@ static int lookup_queued(zg_engine* e, uint16_t res_type, uint16_t perm, uint16_
   me.key.stype = stype;
   me.key.srel = srel;
   me.want_self = self_member != nullptr;
-  auto& b = e->lookups;
-  std::unique_lock<std::mutex> lk(b.m);
-  b.queue.push_back(&me);
-  if (b.leader_active) me.cv.wait(lk, [&] { return me.done || me.lead; });
-  if (!me.done) {  // leader: see zg_check_bulk
-    b.leader_active = true;
-    std::vector<zg_engine::LookupJob*> group;
-    lk.unlock();
-    {
-      std::lock_guard<FairMutex> dev_lock(e->mu);  // the device first, the group second (as for checks)
-      lk.lock();
-      const size_t take = std::min<size_t>(b.queue.size(), kMaxLookupGroup);
-      group.assign(b.queue.begin(), b.queue.begin() + static_cast<long>(take));
-      b.queue.erase(b.queue.begin(), b.queue.begin() + static_cast<long>(take));
-      lk.unlock();
-      run_lookup_group(e, group);
-    }
-    lk.lock();
-    for (auto* j : group) {
-      j->done = true;
-      if (j != &me) j->cv.notify_one();
-    }
-    if (!b.queue.empty()) {
-      b.queue.front()->lead = true;
-      b.queue.front()->cv.notify_one();
-    } else {
-      b.leader_active = false;
-    }
-  }
-  lk.unlock();
+  e->lookups.submit(
+      &me, e->mu,
+      [](const std::vector<zg_engine::LookupJob*>& queue) { return std::min<size_t>(queue.size(), kMaxLookupGroup); },
+      [e](std::vector<zg_engine::LookupJob*>& group) { run_lookup_group(e, group); });
   if (me.rc) return fail(me.rc, me.err);
   *ids = std::move(me.ids);
   if (self_member) *self_member = me.self_member;
@@ -2789,29 +2847,19 @@ static int run_sharded_subjects(zg_engine* e, const Device::SubjectsReq& req, bo
   const std::vector<Device::SubjectsReq> round{req};
   const uint8_t home = 0;
   const uint64_t cap = e->dev.lookup_walk_cap();
-  std::vector<int> src(S, ZG_OK);
-  std::vector<std::string> errs(S);
-  auto first_error = [&]() { return ::first_error(src, errs, err); };
-  auto end_round = [](Device& dev, std::string* e2) {
-    uint64_t listed = 0, excluded = 0;
-    return dev.shard_subjects_finish(nullptr, 0, nullptr, &listed, &excluded, e2);
-  };
-  // a failed round is ended on every shard, so that no shard keeps its snapshot resident
-  auto fail_round = [&](int rc) {
-    on_all_devices(e, [&](Device& dev, size_t) { end_round(dev, nullptr); });
-    return rc;
-  };
+  HandleRound R{e, end_subjects_round, "subjects", &e->hs_waits, err};
   ++e->hs_lookups;
   std::vector<uint64_t> n_front(S, 0);
-  on_all_devices(e, [&](Device& dev, size_t k) {
-    src[k] = !dev.hl_ensure(dev.hl.front[0], cap * 8)
-                 ? ZG_ENOMEM
-                 : dev.shard_subjects_begin(round, &home, include ? 1 : 0, cap, dev.hl.front[0].as<unsigned long long>(),
-                                            &n_front[k], &errs[k]);
-    if (src[k] == ZG_ENOMEM && errs[k].empty()) errs[k] = "out of device memory (sharded handle subjects frontier)";
-  });
   ++e->hs_waits;
-  if (int rc = first_error()) return fail_round(rc);
+  if (int rc = R.on_shards([&](Device& dev, size_t k, std::string* m) {
+        const int brc = !dev.hl_ensure(dev.hl.front[0], cap * 8)
+                            ? ZG_ENOMEM
+                            : dev.shard_subjects_begin(round, &home, include ? 1 : 0, cap,
+                                                       dev.hl.front[0].as<unsigned long long>(), &n_front[k], m);
+        if (brc == ZG_ENOMEM && m->empty()) *m = "out of device memory (sharded handle subjects frontier)";
+        return brc;
+      }))
+    return rc;
   // ---- the walk
   const bool exhaustive = !e->dev.use_rbfs;  // ZGPU_NO_RBFS=1: every owned object of the subject type is a candidate
   bool overflow = false;
@@ -2821,82 +2869,63 @@ static int run_sharded_subjects(zg_engine* e, const Device::SubjectsReq& req, bo
   std::vector<cudaEvent_t> wait(S);
   for (int level = 0; !exhaustive; ++level) {
     const bool expand = level <= ZG_MAX_DEPTH + 1;
-    on_all_devices(e, [&](Device& dev, size_t k) {
-      bool o = false;
-      src[k] = dev.shard_subjects_expand_count(dev.hl.front[0].as<unsigned long long>(), expand ? n_front[k] : 0,
-                                               &counts[k * S], &o, &errs[k]);
-      ovf[k] = o;
-    });
     ++e->hs_waits;
-    if (int rc = first_error()) return fail_round(rc);
+    if (int rc = R.on_shards([&](Device& dev, size_t k, std::string* m) {
+          bool o = false;
+          const int xrc = dev.shard_subjects_expand_count(dev.hl.front[0].as<unsigned long long>(), expand ? n_front[k] : 0,
+                                                          &counts[k * S], &o, m);
+          ovf[k] = o;
+          return xrc;
+        }))
+      return rc;
     if ((overflow = std::find(ovf.begin(), ovf.end(), 1) != ovf.end())) break;
     if (!expand || std::all_of(n_front.begin(), n_front.end(), [](uint64_t n) { return n == 0; })) break;
     ++e->hs_levels;
-    for (uint32_t d = 0; d < S; ++d) {
-      uint64_t at = 0;
-      for (uint32_t k = 0; k < S; ++k) {
-        tab[k].base[d] = at;
-        at += counts[size_t(k) * S + d];
-        if (k != d) e->hs_entries += counts[size_t(k) * S + d];
-      }
-      arrived[d] = at;
-      Device& dev = shard(e, d);
-      if (!dev.hl_ensure(dev.hl.inbox, at * 8)) {
-        *err = "out of device memory (sharded handle subjects inbox)";
-        return fail_round(ZG_ENOMEM);
-      }
-      for (uint32_t k = 0; k < S; ++k) tab[k].p[d] = dev.hl.inbox.p;
+    if (!lay_out_inboxes(S, S, counts, &tab, [&](uint32_t d, uint64_t n) -> void* {
+          for (uint32_t k = 0; k < S; ++k)
+            if (k != d) e->hs_entries += counts[size_t(k) * S + d];
+          arrived[d] = n;
+          Device& dev = shard(e, d);
+          return dev.hl_ensure(dev.hl.inbox, n * 8) ? dev.hl.inbox.p : nullptr;
+        })) {
+      *err = "out of device memory (sharded handle subjects inbox)";
+      return R.fail_round(ZG_ENOMEM);
     }
-    on_all_devices(e, [&](Device& dev, size_t k) {
-      uint64_t n = 0;
-      for (uint32_t d = 0; d < S; ++d) n += counts[k * S + d];
-      src[k] = dev.shard_subjects_scatter(n, tab[k], level, &errs[k]);
-    });
-    if (int rc = first_error()) return fail_round(rc);
+    if (int rc = R.on_shards([&](Device& dev, size_t k, std::string* m) {
+          uint64_t n = 0;
+          for (uint32_t d = 0; d < S; ++d) n += counts[k * S + d];
+          return dev.shard_subjects_scatter(n, tab[k], level, m);
+        }))
+      return rc;
     for (uint32_t k = 0; k < S; ++k) wait[k] = shard(e, k).peer_event(level);
-    on_all_devices(e, [&](Device& dev, size_t k) {
-      src[k] = dev.peer_wait(wait, &errs[k]);
-      if (!src[k])
-        src[k] = dev.shard_subjects_admit(dev.hl.inbox.as<unsigned long long>(), arrived[k],
-                                          dev.hl.front[0].as<unsigned long long>(), &n_front[k], &errs[k]);
-    });
     ++e->hs_waits;
-    if (int rc = first_error()) return fail_round(rc);
+    if (int rc = R.on_shards([&](Device& dev, size_t k, std::string* m) {
+          const int wrc = dev.peer_wait(wait, m);
+          return wrc ? wrc
+                     : dev.shard_subjects_admit(dev.hl.inbox.as<unsigned long long>(), arrived[k],
+                                                dev.hl.front[0].as<unsigned long long>(), &n_front[k], m);
+        }))
+      return rc;
   }
   const bool every = overflow || exhaustive;
   if (every) ++e->hs_fallbacks;
   // ---- the first verification, where the candidates lie
   std::vector<uint64_t> nc(S, 0);
-  on_all_devices(e, [&](Device& dev, size_t k) {
-    uint64_t need = 0;
-    src[k] = dev.shard_subjects_candidates(every, nullptr, 0, &need, &errs[k]);
-    if (!src[k] && (!dev.hl_ensure(dev.hl.items, need * sizeof(zg_check)) || !dev.hl_ensure(dev.hl.codes, need) ||
-                    !dev.hl_ensure(dev.hl.routed, need * 8))) {
-      src[k] = ZG_ENOMEM;
-      errs[k] = "out of device memory (sharded handle subjects candidates)";
-    }
-    if (!src[k]) src[k] = dev.shard_subjects_candidates(every, dev.hl.items.as<zg_check>(), need, &nc[k], &errs[k]);
-  });
-  ++e->hs_waits;
-  if (int rc = first_error()) return fail_round(rc);
-  ShardLists V;
-  for (uint32_t k = 0; k < S; ++k) {
-    V.items.push_back(shard(e, k).hl.items.as<zg_check>());
-    V.n.push_back(nc[k]);
-    V.out.push_back(shard(e, k).hl.codes.as<uint8_t>());
-    e->hs_candidates += nc[k];
-    ans->n_verified += nc[k];
+  if (int rc = R.candidates([&](Device& dev, zg_check* items, uint64_t room, uint64_t* n, std::string* m) {
+        return dev.shard_subjects_candidates(every, items, room, n, m);
+      }, &nc))
+    return rc;
+  for (uint64_t n : nc) {
+    e->hs_candidates += n;
+    ans->n_verified += n;
   }
-  PeerCounts pc;
-  int vrc = run_sharded_lists(e, V, &pc, false, err);
-  e->hs_waits += pc.round_trips;
-  if (vrc) return fail_round(vrc);
+  if (int rc = R.verify(nc, false)) return rc;
   std::vector<uint64_t> granted(S, 0), failed(S, 0);
-  on_all_devices(e, [&](Device& dev, size_t k) {
-    src[k] = dev.shard_subjects_verdicts(dev.hl.codes.as<uint8_t>(), nc[k], &granted[k], &failed[k], &errs[k]);
-  });
   ++e->hs_waits;
-  if (int rc = first_error()) return fail_round(rc);
+  if (int rc = R.on_shards([&](Device& dev, size_t k, std::string* m) {
+        return dev.shard_subjects_verdicts(dev.hl.codes.as<uint8_t>(), nc[k], &granted[k], &failed[k], m);
+      }))
+    return rc;
   uint64_t g = 0, f = 0;  // the probe's verdict is on the resource's owner, a failed candidate anywhere
   for (uint32_t k = 0; k < S; ++k) {
     g |= granted[k];
@@ -2904,73 +2933,37 @@ static int run_sharded_subjects(zg_engine* e, const Device::SubjectsReq& req, bo
   }
   if (f & 1) {
     *err = "LookupSubjects: a subject could not be decided (max dispatch depth / work budget exceeded)";
-    return fail_round(ZG_EDEPTH);
+    return R.fail_round(ZG_EDEPTH);
   }
   // ---- the keys of the first verification, and the no-wildcards verification of the HAS candidates when granted.
   // Its items and codes take the place of the first verification's, which shard_subjects_nowild has read (it waits).
   std::vector<uint64_t> nnw(S, 0);
-  on_all_devices(e, [&](Device& dev, size_t k) {
-    src[k] = dev.shard_subjects_nowild(dev.hl.codes.as<uint8_t>(), nc[k], g, f, dev.hl.items.as<zg_check>(), nc[k], &nnw[k],
-                                       &errs[k]);
-  });
   ++e->hs_waits;
-  if (int rc = first_error()) return fail_round(rc);
+  if (int rc = R.on_shards([&](Device& dev, size_t k, std::string* m) {
+        return dev.shard_subjects_nowild(dev.hl.codes.as<uint8_t>(), nc[k], g, f, dev.hl.items.as<zg_check>(), nc[k],
+                                         &nnw[k], m);
+      }))
+    return rc;
   if (g & 1) {
-    ShardLists W;
-    for (uint32_t k = 0; k < S; ++k) {
-      W.items.push_back(shard(e, k).hl.items.as<zg_check>());
-      W.n.push_back(nnw[k]);
-      W.out.push_back(shard(e, k).hl.codes.as<uint8_t>());
-      e->hs_nowild += nnw[k];
-    }
-    PeerCounts pw;
-    vrc = run_sharded_lists(e, W, &pw, true, err);
-    e->hs_waits += pw.round_trips;
-    if (vrc) return fail_round(vrc);
+    for (uint64_t n : nnw) e->hs_nowild += n;
+    if (int rc = R.verify(nnw, true)) return rc;
   }
-  // ---- the answer keys, gathered, sorted and split on shard 0 (home 0: every key is routed to destination 0)
-  on_all_devices(e, [&](Device& dev, size_t k) {
-    src[k] = dev.shard_subjects_route(dev.hl.codes.as<uint8_t>(), nnw[k], S, dev.hl.routed.as<unsigned long long>(),
-                                      &counts[k * S], &errs[k]);
-  });
-  ++e->hs_waits;
-  if (int rc = first_error()) return fail_round(rc);
-  uint64_t n_keys = 0;
-  for (uint32_t k = 0; k < S; ++k) {
-    tab[k].base[0] = n_keys;
-    n_keys += counts[size_t(k) * S];
-  }
-  Device& d0 = e->dev;
-  if (!d0.hl_ensure(d0.hl.keys, n_keys * 8) || !d0.hl_ensure(d0.hl.ids, n_keys * 4)) {
-    *err = "out of device memory (sharded handle subjects keys)";
-    return fail_round(ZG_ENOMEM);
-  }
-  for (uint32_t k = 0; k < S; ++k) tab[k].p[0] = d0.hl.keys.p;
-  on_all_devices(e, [&](Device& dev, size_t k) {
-    src[k] = dev.peer_put(dev.hl.routed.as<unsigned long long>(), counts[k * S], 1, tab[k], 0, &errs[k]);
-  });
-  if (int rc = first_error()) return fail_round(rc);
-  for (uint32_t k = 0; k < S; ++k) wait[k] = shard(e, k).peer_event(0);
+  // ---- the answer keys, gathered, sorted and split on shard 0
   uint64_t listed = 0, excluded = 0;
-  on_all_devices(e, [&](Device& dev, size_t k) {
-    src[k] = k ? end_round(dev, &errs[k]) : dev.peer_wait(wait, &errs[k]);
-    if (!k && !src[k])
-      src[k] = dev.shard_subjects_finish(dev.hl.keys.as<unsigned long long>(), n_keys, dev.hl.ids.as<uint32_t>(), &listed,
-                                         &excluded, &errs[k]);
-  });
-  ++e->hs_waits;
-  if (int rc = first_error()) return fail_round(rc);
-  std::vector<uint32_t> host(listed + excluded);
-  if (!host.empty()) {
-    const cudaError_t ce = cudaSetDevice(d0.device) == cudaSuccess
-                               ? cudaMemcpy(host.data(), d0.hl.ids.p, host.size() * 4, cudaMemcpyDeviceToHost)
-                               : cudaGetLastError();
-    ++e->hs_waits;
-    if (ce != cudaSuccess) {
-      *err = std::string("cudaMemcpy (lookup answers): ") + cudaGetErrorString(ce);
-      return ZG_ECUDA;
-    }
-  }
+  std::vector<uint32_t> host;
+  if (int rc = R.gather_keys(
+          [&](Device& dev, size_t k, uint64_t* to, std::string* m) {
+            return dev.shard_subjects_route(dev.hl.codes.as<uint8_t>(), nnw[k], S, dev.hl.routed.as<unsigned long long>(),
+                                            to, m);
+          },
+          [&](Device& d0, uint64_t n_keys, uint64_t* n_ids, std::string* m) {
+            const int frc = d0.shard_subjects_finish(d0.hl.keys.as<unsigned long long>(), n_keys, d0.hl.ids.as<uint32_t>(),
+                                                     &listed, &excluded, m);
+            *n_ids = listed + excluded;
+            return frc;
+          },
+          &host))
+    return rc;
   ans->ids.assign(host.begin(), host.begin() + static_cast<long>(listed));
   ans->wildcard = (g & 1) && include;
   if (ans->wildcard) ans->excluded.assign(host.begin() + static_cast<long>(listed), host.end());
@@ -2988,8 +2981,7 @@ static int lookup_subjects_ids(zg_engine* e, uint16_t perm, uint32_t res, uint16
   if (stype >= sc.types.size() || (srel != kNone && (srel >= sc.slots.size() || sc.slots[srel].type != stype)))
     return fail(ZG_EINVAL, "unknown subject type or relation");
   if (option != ZG_WILDCARDS_INCLUDE && option != ZG_WILDCARDS_EXCLUDE) return fail(ZG_EINVAL, "unknown wildcard option");
-  if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
-  if (e->dev.shard_count > 1 && !serves_subjects(e)) return fail(ZG_EINVAL, subjects_refusal(e));
+  if (int rc = refuse(e, Call::kSubjects)) return rc;
   LOCK_DEVICE(e);
   if (e->dirty.load() || !e->dev.snap) {  // a handle's failed publish clears every shard's snapshot
     LOCK_NAMES_UNIQUE(e);
@@ -3054,16 +3046,14 @@ static int lookup_subjects_str_once(zg_engine* e, const char* res_type, const ch
     res = e->store.find(rt, res_id);
   }
   Device::SubjectsAnswer ans;
-  int rc = ZG_OK;
   if (res == ZG_NO_OBJECT) {
     // never written: no relationship names the resource. The engine state is still checked as for any lookup.
     if (wildcard_option != ZG_WILDCARDS_INCLUDE && wildcard_option != ZG_WILDCARDS_EXCLUDE)
       return fail(ZG_EINVAL, "unknown wildcard option");
-    if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");
-    if (e->dev.shard_count > 1 && !serves_subjects(e)) return fail(ZG_EINVAL, subjects_refusal(e));
-  } else {
-    rc = lookup_subjects_ids(e, static_cast<uint16_t>(p), res, static_cast<uint16_t>(st), sr, wildcard_option, &ans);
-    if (rc) return rc;
+    if (int rc = refuse(e, Call::kSubjects)) return rc;
+  } else if (int rc = lookup_subjects_ids(e, static_cast<uint16_t>(p), res, static_cast<uint16_t>(st), sr, wildcard_option,
+                                          &ans)) {
+    return rc;
   }
   if (e->resolve_hook) e->resolve_hook(e->resolve_hook_arg);
   // lines: concrete ids, then "*" and one "!<id>" per exclusion ('!' is outside SpiceDB's object-id charset)
@@ -3244,7 +3234,7 @@ static int list_prefilter_once(zg_engine* e, const char* body, size_t len, uint3
   if (!body || !out_len || !tpl) return fail(ZG_EINVAL, "NULL argument");
   if (!tpl->res_type || !tpl->permission || !tpl->subj_type || !tpl->subj_id) return fail(ZG_EINVAL, "NULL template field");
   if (mode > ZG_LIST_PROTOBUF) return fail(ZG_EINVAL, "unknown mode");
-  if (is_handle(e) && !e->host_only && !e->handle_lookups) return fail(ZG_EINVAL, kHandleLookupMsg);
+  if (int rc = refuse(e, Call::kLookup)) return rc;
   // 1. the allowed ids (one LookupResources on the GPU; concurrent list requests share launches)
   std::vector<uint32_t> ids;
   std::string self;
@@ -3359,8 +3349,7 @@ extern "C" int zg_stats_get(zg_engine* e, zg_stats* out) {
 #define SHARD_PROLOGUE()                                                                                              \
   NEED_SCHEMA(e, ZG_ENOSCHEMA);                                                                                       \
   std::lock_guard<FairMutex> g(e->mu);                                                                               \
-  if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");      \
-  if (is_handle(e)) return fail(ZG_EINVAL, kHandleShardCallMsg);                                                     \
+  if (int rc_ = refuse(e, Call::kShardCall)) return rc_;                                                             \
   if (!e->dev.snap) return fail(ZG_ENOSNAPSHOT, "no snapshot published (call zg_publish)");
 
 extern "C" int zg_shard_route_dev(zg_engine* e, const zg_check* d_items, uint64_t n, int level, uint32_t n_dest,
@@ -3400,8 +3389,7 @@ extern "C" int zg_shard_unroute_dev(zg_engine* e, const uint32_t* d_src, const u
 #define SHARD_ONLY_PROLOGUE(unsharded_msg)                                                                            \
   NEED_SCHEMA(e, ZG_ENOSCHEMA);                                                                                       \
   std::lock_guard<FairMutex> g(e->mu);                                                                               \
-  if (e->host_only) return fail(ZG_ECUDA, "host-only engine: no CUDA device, and libzgpu has no CPU fallback");      \
-  if (is_handle(e)) return fail(ZG_EINVAL, kHandleShardCallMsg);                                                     \
+  if (int rc_ = refuse(e, Call::kShardCall)) return rc_;                                                             \
   if (e->dev.shard_count < 2) return fail(ZG_EINVAL, unsharded_msg);                                                 \
   if (!e->dev.snap) return fail(ZG_ENOSNAPSHOT, "no snapshot published (call zg_publish)");
 #define SHARD_LOOKUP_PROLOGUE() SHARD_ONLY_PROLOGUE("not a sharded engine: use zg_lookup_resources")
