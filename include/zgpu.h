@@ -473,6 +473,14 @@ int zg_closure_index_info(zg_engine *e, uint32_t pair, uint64_t *out);
 int zg_closure_index_copy(zg_engine *e, uint32_t pair, uint32_t *row_ptr, uint64_t row_cap, uint32_t *col,
                           uint64_t col_cap, uint64_t *n_rows, uint64_t *n_entries);
 
+/* Signatures of closure index `pair` (the check kernel tests a range's children against them and searches the row only
+ * on a "maybe"): out[0] 1 when built, out[1] 64-bit words per row, out[2] bits set per entry, out[3] device bytes,
+ * out[4] device microseconds of their last build. ZG_EINVAL when there is no such pair. */
+int zg_closure_signature_info(zg_engine *e, uint32_t pair, uint64_t *out);
+/* Copies the signatures of closure index `pair`, row-major (*n_words = rows x words per row). ZG_E2BIG (size filled)
+ * when the buffer is too small, ZG_EINVAL when the pair has none. For inspection and tests. */
+int zg_closure_signature_copy(zg_engine *e, uint32_t pair, uint64_t *words, uint64_t cap, uint64_t *n_words);
+
 /* Pinned host memory for request/response buffers: zg_check_bulk copies straight
  * from/to such buffers (no staging memcpy). */
 void *zg_host_alloc(size_t bytes);

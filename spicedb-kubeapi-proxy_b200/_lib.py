@@ -193,6 +193,8 @@ _SIGS = {
     "zg_filter_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
     "zg_closure_index_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
     "zg_closure_index_info": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p]),
+    "zg_closure_signature_info": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p]),
+    "zg_closure_signature_copy": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),
     "zg_closure_index_copy": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
                                         C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "zg_resolve_checks_packed_device": (C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]),
@@ -798,6 +800,24 @@ class Engine:
         self._ck(self._L.zg_closure_index_copy(self._h, pair, row_ptr.ctypes.data, row_ptr.size, col.ctypes.data, col.size,
                                                C.byref(nr), C.byref(ne)))
         return row_ptr, col[: ne.value]
+
+    def closure_signature_info(self, pair: int = 0) -> dict:
+        """Built flag, words per row, bits per entry, device bytes and last build time (device microseconds) of the
+        signatures of closure index `pair` (zg_closure_signature_info)."""
+        out = np.zeros(5, dtype=np.uint64)
+        self._ck(self._L.zg_closure_signature_info(self._h, pair, out.ctypes.data))
+        return {k: int(v) for k, v in zip(("built", "words", "k", "device_bytes", "build_us"), out)}
+
+    def closure_signature(self, pair: int = 0):
+        """Signatures of closure index `pair`: uint64 array of shape (rows, words per row) (zg_closure_signature_copy)."""
+        words = self.closure_signature_info(pair)["words"]
+        n = C.c_uint64(0)
+        rc = self._L.zg_closure_signature_copy(self._h, pair, None, 0, C.byref(n))
+        if rc != E2BIG:
+            self._ck(rc)
+        out = np.empty(max(n.value, 1), dtype=np.uint64)
+        self._ck(self._L.zg_closure_signature_copy(self._h, pair, out.ctypes.data, out.size, C.byref(n)))
+        return out[: n.value].reshape(-1, max(words, 1))
 
     HANDLE_LOOKUP_COUNTERS = ("rounds", "levels", "round_trips", "frontier_entries", "candidates", "halvings", "fallbacks")
 

@@ -24,6 +24,7 @@
 
 #include "delta.cuh"
 #include "device.h"
+#include "closure_sig.cuh"
 
 namespace zg {
 
@@ -194,6 +195,26 @@ __global__ void closure_unique_kernel(const uint32_t* sorted, const unsigned lon
   if (!out) ucnt[u + 1] = k;
 }
 
+// Signature of every closure row, one warp per row: lane w owns word w of the row's 2^lg, and every lane tests every
+// entry of the row (32 read at a time, then broadcast) for its word, so no word is written by two lanes.
+template <class E>
+__global__ void closure_sig_kernel(const uint32_t* row_ptr, const E* col, uint32_t n, uint32_t lg, unsigned long long* sig) {
+  const uint32_t lane = threadIdx.x & 31u;
+  const unsigned long long u = (static_cast<unsigned long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  if (u >= n) return;  // warp-uniform
+  const uint32_t lo = row_ptr[u], hi = row_ptr[u + 1];
+  unsigned long long w = 0;
+  for (uint32_t b = lo; b < hi; b += 32) {
+    const uint32_t mine = b + lane < hi ? static_cast<uint32_t>(col[b + lane]) : 0u;
+    const uint32_t cnt = min(32u, hi - b);
+    for (uint32_t j = 0; j < cnt; ++j) {
+      const uint32_t v = __shfl_sync(0xFFFFFFFFu, mine, j);
+      if (sig_word(v, lg) == lane) w |= sig_mask(v);
+    }
+  }
+  if (lane < (1u << lg)) sig[(u << lg) + lane] = w;
+}
+
 }  // namespace
 
 std::string gpu_build_closure(const Snapshot& s, const DCls& a, const DCls& b, uint64_t cap, Snapshot::Closure* c,
@@ -278,6 +299,43 @@ std::string gpu_build_closure(const Snapshot& s, const DCls& a, const DCls& b, u
   BCUDA(cudaGetLastError());
   c->entries = nu;
   c->built = true;
+  return "";
+}
+
+std::string gpu_build_closure_sig(Snapshot::Closure* c, uint32_t words, cudaStream_t st) {
+  c->sig_words = 0;
+  if (!c->built || words == 0) {
+    c->sig.release();
+    return "";
+  }
+  if (words == ~0u) {
+    words = 1;
+    while (words < 32 && 64ull * words * c->nsubj < 12ull * c->entries) words <<= 1;
+  } else {
+    words = 1u << (31 - __builtin_clz(std::min(words, 32u)));  // a power of two, at most 32
+  }
+  const uint32_t lg = static_cast<uint32_t>(__builtin_ctz(words));
+  const size_t bytes = (size_t(c->nsubj) << lg) * 8;
+  size_t free_b = 0, total_b = 0;
+  BCUDA(cudaMemGetInfo(&free_b, &total_b));
+  if (bytes > (free_b + c->sig.cap) / 4) {  // (counting the pair's old signature buffer as free: it is reused)
+    c->sig.release();
+    return "";
+  }
+  if (!c->sig.ensure(bytes ? bytes : 8)) return "out of device memory (closure signatures)";
+  if (c->nsubj) {
+    const unsigned blk = 256;
+    const unsigned long long grid = (static_cast<unsigned long long>(c->nsubj) * 32 + blk - 1) / blk;
+    if (c->width == 2)
+      closure_sig_kernel<<<grid, blk, 0, st>>>(c->row_ptr.as<uint32_t>(), c->col.as<uint16_t>(), c->nsubj, lg,
+                                               c->sig.as<unsigned long long>());
+    else
+      closure_sig_kernel<<<grid, blk, 0, st>>>(c->row_ptr.as<uint32_t>(), c->col.as<uint32_t>(), c->nsubj, lg,
+                                               c->sig.as<unsigned long long>());
+    BCUDA(cudaGetLastError());
+  }
+  BCUDA(cudaStreamSynchronize(st));
+  c->sig_words = words;
   return "";
 }
 

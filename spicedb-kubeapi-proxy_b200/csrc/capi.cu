@@ -3154,6 +3154,36 @@ extern "C" int zg_closure_index_info(zg_engine* e, uint32_t pair, uint64_t* out)
   return ZG_OK;
 }
 
+extern "C" int zg_closure_signature_info(zg_engine* e, uint32_t pair, uint64_t* out) {
+  if (!e || !out) return fail(ZG_EINVAL, "NULL argument");
+  LOCK_DEVICE(e);
+  const auto s = e->dev.snap;
+  if (!s) return fail(ZG_ENOSNAPSHOT, "no snapshot published (call zg_publish)");
+  if (pair >= s->closure.size()) return fail(ZG_EINVAL, "no two-level pair with this number");
+  const auto& x = s->closure[pair];
+  const bool b = x.built && x.sig_words;
+  const uint64_t c[5] = {b ? 1u : 0u, b ? x.sig_words : 0u, b ? 3u : 0u, b ? uint64_t(x.nsubj) * x.sig_words * 8 : 0u,
+                         b ? static_cast<uint64_t>(x.sig_ms * 1000.0) : 0u};
+  std::memcpy(out, c, sizeof c);
+  return ZG_OK;
+}
+
+extern "C" int zg_closure_signature_copy(zg_engine* e, uint32_t pair, uint64_t* words, uint64_t cap, uint64_t* n_words) {
+  if (!e || !n_words) return fail(ZG_EINVAL, "NULL argument");
+  LOCK_DEVICE(e);
+  const auto s = e->dev.snap;
+  if (!s) return fail(ZG_ENOSNAPSHOT, "no snapshot published (call zg_publish)");
+  if (pair >= s->closure.size() || !s->closure[pair].built || !s->closure[pair].sig_words)
+    return fail(ZG_EINVAL, "no closure signatures for this pair");
+  const auto& x = s->closure[pair];
+  *n_words = uint64_t(x.nsubj) * x.sig_words;
+  if (cap < *n_words || (!words && *n_words)) return fail(ZG_E2BIG, "buffer too small for the closure signatures");
+  cudaError_t ce = cudaSetDevice(e->dev.device);
+  if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->dev.stream);
+  if (ce == cudaSuccess && *n_words) ce = cudaMemcpy(words, x.sig.p, *n_words * 8, cudaMemcpyDeviceToHost);
+  return ce == cudaSuccess ? ZG_OK : fail(ZG_ECUDA, std::string("zg_closure_signature_copy: ") + cudaGetErrorString(ce));
+}
+
 extern "C" int zg_handle_lookup_counters(zg_engine* e, uint64_t* out) {
   if (!e || !out) return fail(ZG_EINVAL, "NULL argument");
   LOCK_DEVICE(e);

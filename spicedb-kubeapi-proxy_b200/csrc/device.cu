@@ -72,6 +72,7 @@ Snapshot::~Snapshot() {
   for (auto& c : closure) {
     c.row_ptr.release();
     c.col.release();
+    c.sig.release();
   }
 }
 
@@ -127,6 +128,8 @@ std::string Device::init(int dev, uint64_t subq_cap, uint32_t budget) {
   if (const char* v = std::getenv("ZGPU_NO_RBFS")) use_rbfs = !(*v && *v != '0');
   if (const char* v = std::getenv("ZGPU_LOOKUP_BATCH_CAP")) lb_cap_ = std::max<uint64_t>(1024, std::strtoull(v, nullptr, 10));
   if (const char* v = std::getenv("ZGPU_CLOSURE_CAP")) closure_cap_ = std::strtoull(v, nullptr, 10);  // tests: 0 = no index
+  if (const char* v = std::getenv("ZGPU_CLOSURE_SIG_WORDS"))  // tests: 0 = no signatures, 1 = one word (most tests maybe)
+    closure_sig_words_ = static_cast<uint32_t>(std::strtoul(v, nullptr, 10));
   int count = 0;
   cudaError_t e = cudaGetDeviceCount(&count);
   if (e != cudaSuccess || count == 0)
@@ -341,11 +344,28 @@ void Device::build_closures(Snapshot* s, const HostSnapshot& h, const std::vecto
       c.entries = 0;
       c.row_ptr.release();
       c.col.release();
+      c.sig.release();
+      c.sig_words = 0;
       cudaGetLastError();
       ++closure_failures;
       continue;
     }
     ++closure_builds;
+    // The signatures are optional too: without them (over budget, or a failed build) the pair meets through
+    // closure_meet over its index.
+    cudaEventRecord(e0, stream);
+    err = gpu_build_closure_sig(&c, closure_sig_words_, stream);
+    cudaEventRecord(e1, stream);
+    cudaEventSynchronize(e1);
+    ms = 0;
+    cudaEventElapsedTime(&ms, e0, e1);
+    closure_ms += ms;
+    c.sig_ms = ms;
+    if (!err.empty()) {
+      c.sig.release();
+      c.sig_words = 0;
+      cudaGetLastError();
+    }
   }
   if (e0) {
     cudaEventDestroy(e0);
@@ -435,6 +455,7 @@ std::string Device::finish_publish(std::shared_ptr<Snapshot> s, const HostSnapsh
         pairs.push_back(*old);
         old->row_ptr = DevBuf{};  // moved
         old->col = DevBuf{};
+        old->sig = DevBuf{};
       } else {
         pairs.emplace_back();
         pairs.back().inner = inner;
@@ -444,6 +465,7 @@ std::string Device::finish_publish(std::shared_ptr<Snapshot> s, const HostSnapsh
     for (auto& c : s->closure) {
       c.row_ptr.release();
       c.col.release();
+      c.sig.release();
     }
     s->closure = std::move(pairs);
     build_closures(s.get(), h, nullptr);
@@ -471,7 +493,10 @@ std::string Device::finish_publish(std::shared_ptr<Snapshot> s, const HostSnapsh
     if (sm > attr_bytes) {
       for (auto k : {check_kernel<false>, check_kernel<true>, check_kernel<false, true>, check_kernel<false, false, kMeetNone>,
                      check_kernel<true, false, kMeetNone>, check_kernel<false, true, kMeetNone>, check_kernel<false, false, kMeet16>,
-                     check_kernel<true, false, kMeet16>, check_kernel<false, true, kMeet16>})
+                     check_kernel<true, false, kMeet16>, check_kernel<false, true, kMeet16>,
+                     check_kernel<false, false, kMeetSig16>, check_kernel<true, false, kMeetSig16>,
+                     check_kernel<false, true, kMeetSig16>, check_kernel<false, false, kMeetSig32>,
+                     check_kernel<true, false, kMeetSig32>, check_kernel<false, true, kMeetSig32>})
         cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sm));
       attr_bytes = sm;
     }
@@ -533,11 +558,15 @@ int Device::run_pass(const Snapshot& s, const zg_check* queries, uint64_t nq, ui
   p.shard_rank = shard_rank;
   p.no_wildcards = no_wildcards_ ? 1 : 0;
   int meet = s.has_l2 ? kMeet32 : kMeetNone;
+  bool all_sig = true;
   for (const auto& c : s.closure)
     if (c.built) {
-      p.closure[p.n_closure++] = ClosureRef{c.row_ptr.as<uint32_t>(), c.col.p, c.nsubj, c.tgc, c.width};
+      p.closure[p.n_closure++] = ClosureRef{c.row_ptr.as<uint32_t>(), c.col.p, c.nsubj, c.tgc, c.width,
+                                            c.sig_words ? c.sig.as<unsigned long long>() : nullptr, c.sig_words};
       if (c.width == 2) meet = kMeet16;  // every built index of a snapshot has the same width
+      all_sig = all_sig && c.sig_words;
     }
+  if (p.n_closure && all_sig) meet |= kMeetSig;
   ZG_CUDA(cudaMemsetAsync(ctrl, 0, 16, st));  // next, subq_count
   const int per_sm = count ? blocks_per_sm_count_ : blocks_per_sm_;
   uint64_t want = (nq + kThreads - 1) / kThreads;
@@ -545,14 +574,19 @@ int Device::run_pass(const Snapshot& s, const zg_check* queries, uint64_t nq, ui
   if (grid < 1) grid = 1;
   size_t sm = smem_bytes(s.prog_bytes);
   // a schema without a two-level step runs the kernel built without the two-level meet; one with 16-bit closure
-  // indexes the kernel whose meet reads them
-  auto pick = [meet](auto none, auto m32, auto m16) { return meet == kMeetNone ? none : meet == kMeet16 ? m16 : m32; };
+  // indexes the kernel whose meet reads them; one whose every built index has signatures the kernel that tests them
+  auto pick = [meet](auto none, auto m32, auto m16, auto s32, auto s16) {
+    return meet == kMeetNone ? none : meet == kMeet16 ? m16 : meet == kMeetSig16 ? s16 : meet == kMeetSig32 ? s32 : m32;
+  };
   if (count)
-    pick(check_kernel<true, false, kMeetNone>, check_kernel<true>, check_kernel<true, false, kMeet16>)<<<grid, kThreads, sm, st>>>(p);
+    pick(check_kernel<true, false, kMeetNone>, check_kernel<true>, check_kernel<true, false, kMeet16>,
+         check_kernel<true, false, kMeetSig32>, check_kernel<true, false, kMeetSig16>)<<<grid, kThreads, sm, st>>>(p);
   else if (ready)
-    pick(check_kernel<false, true, kMeetNone>, check_kernel<false, true>, check_kernel<false, true, kMeet16>)<<<grid, kThreads, sm, st>>>(p);
+    pick(check_kernel<false, true, kMeetNone>, check_kernel<false, true>, check_kernel<false, true, kMeet16>,
+         check_kernel<false, true, kMeetSig32>, check_kernel<false, true, kMeetSig16>)<<<grid, kThreads, sm, st>>>(p);
   else
-    pick(check_kernel<false, false, kMeetNone>, check_kernel<false>, check_kernel<false, false, kMeet16>)<<<grid, kThreads, sm, st>>>(p);
+    pick(check_kernel<false, false, kMeetNone>, check_kernel<false>, check_kernel<false, false, kMeet16>,
+         check_kernel<false, false, kMeetSig32>, check_kernel<false, false, kMeetSig16>)<<<grid, kThreads, sm, st>>>(p);
   ZG_CUDA(cudaGetLastError());
   ++launches;
   return ZG_OK;

@@ -65,6 +65,11 @@ struct Snapshot {
     uint8_t width = 0;   // bytes per entry, 2 or 4: one width for every pair of the snapshot (build_closures)
     bool done = false;   // the budget was checked against this snapshot's relationships
     bool built = false;  // ... and the index built
+    // Signature of every row (kernels.cuh sig_word / sig_mask): sig_words 64-bit words per row, row-major. 0: none (the
+    // pair's steps meet through closure_meet).
+    DevBuf sig;
+    uint32_t sig_words = 0;
+    double sig_ms = 0;  // device time of its last build
   };
   std::vector<Closure> closure;
   uint64_t n_tuples = 0, bytes = 0, revision = 0;
@@ -358,11 +363,13 @@ class Device {
 
  private:
   uint64_t closure_cap_ = ~0ull;  // ZGPU_CLOSURE_CAP: entries a closure index may hold (tests; ~0 = the size budget)
+  uint32_t closure_sig_words_ = ~0u;  // ZGPU_CLOSURE_SIG_WORDS: signature words per row (tests; 0 = none, ~0 = chosen
+                                      // from the mean row length, gpu_build_closure_sig)
   // (Re)builds the closure index of every pair of s->closure that is not built yet (`rebuild` false) or whose inner or
   // tgc class is marked in `rebuild` (a write changed it), from the classes' reverse rows described by h.cls. Decides
   // the entry width from h's object capacities first: 16-bit when every pair's tgc resource type holds at most 65 536
   // objects, else 32-bit, and rebuilds every pair built at another width. A pair whose build fails is left without an
-  // index (closure_failures).
+  // index (closure_failures). Every index built here gets its signatures; a pair whose signatures fail keeps its index.
   void build_closures(Snapshot* s, const HostSnapshot& h, const std::vector<uint8_t>* rebuild);
   // match_filter / match_expired: the count launch over the classes `sel` (p holds the rest of the plan), then with
   // `tuples` the emit launch sized by it, of filter_expired_kernel (`expired`) or the kernel of `shape`.
@@ -473,5 +480,9 @@ constexpr uint64_t kClosureRatio = 16;
 // budget above) or more than a quarter of the free device memory; c->built tells which.
 std::string gpu_build_closure(const Snapshot& s, const DCls& a, const DCls& b, uint64_t cap, Snapshot::Closure* c,
                               cudaStream_t st);
+// Builds the signatures of the built closure index *c: `words` 64-bit words per row (a power of two, 1 .. 32), or, with
+// words = ~0u, the fewest with 64 * words >= 12 x the mean row length (about 1 % false "maybe"s per test at 3 bits per
+// entry). None (c->sig_words = 0) when they would take more than a quarter of the free device memory.
+std::string gpu_build_closure_sig(Snapshot::Closure* c, uint32_t words, cudaStream_t st);
 
 }  // namespace zg

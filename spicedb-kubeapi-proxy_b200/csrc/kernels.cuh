@@ -32,6 +32,7 @@
 #include <cstdint>
 
 #include "../../include/zgpu.h"
+#include "closure_sig.cuh"
 #include "schema.h"
 
 namespace zg {
@@ -88,11 +89,17 @@ struct ClosureRef {
   uint32_t nsubj;   // rows (subjects of the innermost direct class)
   uint16_t tgc;
   uint16_t width;   // 2 or 4; a kernel instantiated for one width reads only the indexes of that width
+  // Signature of every row (closure_sig.cuh): sig_words 64-bit words per row, row u at sig[u * sig_words]. nullptr: none.
+  const unsigned long long* sig;
+  uint32_t sig_words;  // a power of two, 1 .. 32
 };
-// check_kernel's MEET argument: no two-level step in the schema, or the width of the closure entries it reads
-constexpr int kMeetNone = 0, kMeet16 = 2, kMeet32 = 4;
+// check_kernel's MEET argument: no two-level step in the schema, or the width of the closure entries it reads, plus
+// kMeetSig when the meet tests the range against the rows' signatures (sig_meet) instead of streaming the rows
+constexpr int kMeetNone = 0, kMeet16 = 2, kMeet32 = 4, kMeetSig = 8;
+constexpr int kMeetSig16 = kMeet16 | kMeetSig, kMeetSig32 = kMeet32 | kMeetSig;
 template <int MEET> struct ClosureEntry { using type = uint32_t; };
 template <> struct ClosureEntry<kMeet16> { using type = uint16_t; };
+template <> struct ClosureEntry<kMeetSig16> { using type = uint16_t; };
 
 struct KParams {
   const uint32_t* row_ptr;
@@ -382,12 +389,12 @@ __device__ __forceinline__ void l2_filter(const uint32_t* __restrict__ col, uint
   }
 }
 // Is v an element of the sorted range col[a, b)? (the filter said maybe)
-template <bool COUNT>
-__device__ __forceinline__ bool l2_verify(const uint32_t* __restrict__ col, uint32_t a, uint32_t b, uint32_t v,
+template <bool COUNT, class T>
+__device__ __forceinline__ bool l2_verify(const T* __restrict__ col, uint32_t a, uint32_t b, uint32_t v,
                                           unsigned long long& nb) {
   while (a < b) {
     const uint32_t mid = a + ((b - a) >> 1), t = __ldg(col + mid);
-    if (COUNT) nb += 4;
+    if (COUNT) nb += sizeof(T);
     if (t == v) return true;
     if (t < v) a = mid + 1; else b = mid;
   }
@@ -626,12 +633,67 @@ __device__ __forceinline__ unsigned closure_meet(const uint32_t* __restrict__ co
   return hits;
 }
 
+// Two-level meet over a closure index with signatures: lane j wants "does its range col[lo, hi) list an element of its
+// subject's closure row ccol[rb, re)", whose signature (2^lg words) is at sig. The range is the small side (cfg3: ~10
+// children against a row of ~80), so each lane tests its own range's children against the row's signature, 8 children
+// per round with their loads in flight together, and only the "maybe"s are searched in the row. The searches of a round
+// run for the whole warp at once (one lane's search per test would stall the warp once per test). The COUNT variant
+// counts 4 bytes per child read, 8 per signature word and sizeof(E) per search probe. Returns the job slots answered.
+template <bool COUNT, class E>
+__device__ __forceinline__ unsigned sig_meet(const uint32_t* __restrict__ col, const E* __restrict__ ccol,
+                                             const unsigned long long* __restrict__ sig, uint32_t lg, bool want, uint32_t lo,
+                                             uint32_t hi, uint32_t rb, uint32_t re, uint32_t jslot,
+                                             unsigned long long* bytes) {
+  constexpr uint32_t kTests = 8;  // (4 spilled a little less and ran no faster on cfg3: DESIGN.md §6)
+  unsigned long long nb = 0;
+  unsigned hits = 0;
+  bool more = want && lo < hi;
+  while (__any_sync(kFull, more)) {
+    uint32_t v[kTests];
+    unsigned m = 0;  // the children of this round whose test said maybe
+    if (more) {
+      const uint32_t n = min(hi - lo, kTests);
+#pragma unroll
+      for (uint32_t i = 0; i < kTests; ++i) v[i] = i < n ? __ldg(col + lo + i) : 0u;
+      unsigned long long w[kTests];
+#pragma unroll
+      for (uint32_t i = 0; i < kTests; ++i) w[i] = i < n ? __ldg(sig + sig_word(v[i], lg)) : 0ull;
+#pragma unroll
+      for (uint32_t i = 0; i < kTests; ++i) {
+        const unsigned long long b = sig_mask(v[i]);
+        m |= (i < n && (w[i] & b) == b) ? 1u << i : 0u;
+      }
+      if (COUNT) nb += 12ull * n;
+      lo += n;
+    }
+    bool hit = false;
+    while (__any_sync(kFull, m != 0)) {
+      if (m) {
+        const uint32_t i = __ffs(m) - 1;
+        m &= m - 1;
+        uint32_t vi = v[0];
+#pragma unroll
+        for (uint32_t t = 1; t < kTests; ++t) vi = i == t ? v[t] : vi;
+        if (l2_verify<COUNT>(ccol, rb, re, vi, nb)) {
+          hit = true;
+          m = 0;
+        }
+      }
+    }
+    hits |= __reduce_or_sync(kFull, hit ? 1u << jslot : 0u);
+    more = more && lo < hi && !((hits >> jslot) & 1u);
+  }
+  if (COUNT) *bytes += nb;
+  return hits;
+}
+
 // Warp-collective node visit: every lane may carry one (job slot, object, unit).
 // Evaluates the unit's steps at the object: membership-of-itself test, direct and
 // wildcard probes (from the subject's reverse-row set when the job is inverted, else a
 // binary search of the row), and pushes the userset / arrow edge ranges. MEET = kMeetNone: the schema has no two-level
 // step, and the two-level meet is left out (its code costs the traversal loop registers: cfg4, DESIGN.md §6); else the
-// width of the closure entries the meet reads (kMeet16 / kMeet32: one closure_meet is inlined per instantiation).
+// width of the closure entries the meet reads (kMeet16 / kMeet32: one closure_meet is inlined per instantiation;
+// kMeetSig16 / kMeetSig32: sig_meet instead, for snapshots whose every built index has signatures).
 template <bool COUNT, int MEET>
 __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<COUNT>& c, bool active,
                                       uint32_t jslot, uint32_t obj, uint32_t unit, uint32_t depth) {
@@ -691,9 +753,11 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
   const int maxsteps = __reduce_max_sync(kFull, npush);
   for (int i = 0; i < maxsteps; ++i) {
     using CE = typename ClosureEntry<MEET>::type;
+    constexpr bool kSig = (MEET & kMeetSig) != 0;
     bool want = false, l2_want = false, cl_want = false;
-    uint32_t l2_lo = 0, l2_hi = 0, l2_k = 0, cl_rb = 0, cl_re = 0;
+    uint32_t l2_lo = 0, l2_hi = 0, l2_k = 0, cl_rb = 0, cl_re = 0, cl_lg = 0;
     const CE* cl_col = nullptr;
+    const unsigned long long* cl_sig = nullptr;
     uint4 item = make_uint4(0, 0, 0, 0);
     if (i < npush && !hit) {
       const DStep st = pr.steps()[sb + i];
@@ -712,15 +776,29 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
           uint32_t cn = 0;
 #pragma unroll
           for (int k = 0; k < kMaxClosure; ++k)  // (by value: the address of a kernel parameter costs a local copy)
-            if (k < static_cast<int>(p.n_closure) && p.closure[k].tgc == st.tgc && p.closure[k].width == sizeof(CE)) {
+            if (k < static_cast<int>(p.n_closure) && p.closure[k].tgc == st.tgc && p.closure[k].width == sizeof(CE) &&
+                (!kSig || p.closure[k].sig)) {
               crow = p.closure[k].row_ptr;
               ccol = static_cast<const CE*>(p.closure[k].col);
               cn = p.closure[k].nsubj;
+              if (kSig) {
+                cl_sig = p.closure[k].sig;
+                cl_lg = __ffs(p.closure[k].sig_words) - 1;
+              }
             }
           if (crow && stype == st.tstype && sid < cn) {
             rb = __ldg(crow + sid);
             re = __ldg(crow + sid + 1);
             crow_read = true;
+            if (kSig) {
+              cl_sig += static_cast<unsigned long long>(sid) << cl_lg;
+              // The signature's line is wanted two dependent loads later (after the range's offsets and children):
+              // fetched into L1 now, its tests hit there (cfg3 +0.5 %, H100, DESIGN.md §6; prefetching the row's
+              // lines for the searches as well cost 18 %).
+#ifndef ZG_EMULATE
+              asm volatile("prefetch.global.L1 [%0];" ::"l"(cl_sig));
+#endif
+            }
           }
         }
         if (hi > lo) {
@@ -780,7 +858,7 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
               // Ranges of up to kFCap children are handed to the whole warp below (closure_meet); a larger one is
               // intersected with the row by this lane.
               if (COUNT && crow_read) c.bytes += 8;
-              if (hi - lo <= static_cast<uint32_t>(kFCap)) {
+              if (kSig || hi - lo <= static_cast<uint32_t>(kFCap)) {  // (sig_meet's cost does not grow with the row)
                 cl_want = re > rb;
                 l2_lo = lo;
                 l2_hi = hi;
@@ -833,9 +911,13 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
       const long long t2 = clock64();
 #endif
       unsigned long long cb = 0;
-      c.found |= closure_meet<COUNT>(p.col, cl_col, reinterpret_cast<unsigned long long*>(c.rset + (kRsetCap + kStateWords) * 32),
-                                     c.lane, cl_want && !((c.found >> jslot) & 1u), l2_lo, l2_hi, cl_rb, cl_re, jslot & 31u,
-                                     COUNT ? &cb : nullptr);
+      if constexpr (kSig)
+        c.found |= sig_meet<COUNT>(p.col, cl_col, cl_sig, cl_lg, cl_want && !((c.found >> jslot) & 1u), l2_lo, l2_hi, cl_rb,
+                                   cl_re, jslot & 31u, COUNT ? &cb : nullptr);
+      else
+        c.found |= closure_meet<COUNT>(p.col, cl_col, reinterpret_cast<unsigned long long*>(c.rset + (kRsetCap + kStateWords) * 32),
+                                       c.lane, cl_want && !((c.found >> jslot) & 1u), l2_lo, l2_hi, cl_rb, cl_re, jslot & 31u,
+                                       COUNT ? &cb : nullptr);
       if (COUNT) c.bytes += cb;
 #if ZG_PHASE_CLOCKS
       c.ph[2] += clock64() - t2;
