@@ -481,6 +481,16 @@ int zg_closure_signature_info(zg_engine *e, uint32_t pair, uint64_t *out);
  * when the buffer is too small, ZG_EINVAL when the pair has none. For inspection and tests. */
 int zg_closure_signature_copy(zg_engine *e, uint32_t pair, uint64_t *words, uint64_t cap, uint64_t *n_words);
 
+/* Set table of closure index `pair` (the check kernel looks a range's children up in it, exactly, instead of testing
+ * signatures): out[0] 1 when built, out[1] buckets, out[2] 16-bit slots per bucket, out[3] device bytes (headers and
+ * buckets), out[4] device microseconds of its last build. ZG_EINVAL when there is no such pair. */
+int zg_closure_table_info(zg_engine *e, uint32_t pair, uint64_t *out);
+/* Copies the set table of closure index `pair`: one header word per row (first bucket in bits 0-31, bucket count in
+ * bits 32-55, seed in bits 56-63) and the buckets (four 16-bit slots each, 0xFFFF empty). ZG_E2BIG (sizes filled) when
+ * a buffer is too small, ZG_EINVAL when the pair has none. For inspection and tests. */
+int zg_closure_table_copy(zg_engine *e, uint32_t pair, uint64_t *hdr, uint64_t hdr_cap, uint64_t *buckets,
+                          uint64_t bucket_cap, uint64_t *n_rows, uint64_t *n_buckets);
+
 /* Pinned host memory for request/response buffers: zg_check_bulk copies straight
  * from/to such buffers (no staging memcpy). */
 void *zg_host_alloc(size_t bytes);

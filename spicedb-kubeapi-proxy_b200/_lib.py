@@ -195,6 +195,9 @@ _SIGS = {
     "zg_closure_index_info": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p]),
     "zg_closure_signature_info": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p]),
     "zg_closure_signature_copy": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),
+    "zg_closure_table_info": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p]),
+    "zg_closure_table_copy": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
+                                        C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "zg_closure_index_copy": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
                                         C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "zg_resolve_checks_packed_device": (C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]),
@@ -818,6 +821,26 @@ class Engine:
         out = np.empty(max(n.value, 1), dtype=np.uint64)
         self._ck(self._L.zg_closure_signature_copy(self._h, pair, out.ctypes.data, out.size, C.byref(n)))
         return out[: n.value].reshape(-1, max(words, 1))
+
+    def closure_table_info(self, pair: int = 0) -> dict:
+        """Built flag, buckets, slots per bucket, device bytes and last build time (device microseconds) of the set
+        table of closure index `pair` (zg_closure_table_info)."""
+        out = np.zeros(5, dtype=np.uint64)
+        self._ck(self._L.zg_closure_table_info(self._h, pair, out.ctypes.data))
+        return {k: int(v) for k, v in zip(("built", "buckets", "slots", "device_bytes", "build_us"), out)}
+
+    def closure_table(self, pair: int = 0):
+        """Set table of closure index `pair`: (uint64 header per row, uint16 array of shape (buckets, 4))
+        (zg_closure_table_copy)."""
+        nr, nb = C.c_uint64(0), C.c_uint64(0)
+        rc = self._L.zg_closure_table_copy(self._h, pair, None, 0, None, 0, C.byref(nr), C.byref(nb))
+        if rc != E2BIG:
+            self._ck(rc)
+        hdr = np.empty(max(nr.value, 1), dtype=np.uint64)
+        tab = np.empty(max(nb.value, 1), dtype=np.uint64)
+        self._ck(self._L.zg_closure_table_copy(self._h, pair, hdr.ctypes.data, hdr.size, tab.ctypes.data, tab.size,
+                                               C.byref(nr), C.byref(nb)))
+        return hdr[: nr.value], tab[: nb.value].view(np.uint16).reshape(-1, 4)
 
     HANDLE_LOOKUP_COUNTERS = ("rounds", "levels", "round_trips", "frontier_entries", "candidates", "halvings", "fallbacks")
 

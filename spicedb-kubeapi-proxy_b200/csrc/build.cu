@@ -215,6 +215,67 @@ __global__ void closure_sig_kernel(const uint32_t* row_ptr, const E* col, uint32
   if (lane < (1u << lg)) sig[(u << lg) + lane] = w;
 }
 
+// Set table of every 16-bit closure row (closure_sig.cuh), one warp per row, in two launches over the same placement:
+// the row's entries are dealt 32 at a time, lanes with the same bucket find each other (__match_any_sync), and each
+// takes the bucket's next slot in entry order from a per-warp histogram in shared memory, so a bucket holds its entries
+// ascending. Choose (tab == nullptr): tries bucket counts from table_first_nb on, growing by table_grow_nb, `seeds` seeds
+// each, until no bucket gets more than kTableSlots entries; writes the row's bucket count into cnt[u + 1] and nb / seed into
+// hdr[u], or sets *failed when the row needs more than kTableMaxBuckets buckets. Fill: cnt holds the rows' first
+// buckets; writes the entries into tab (all 0xFFFF before) and completes hdr[u].
+constexpr unsigned kTableWarps = 4;
+__global__ void __launch_bounds__(kTableWarps * 32)
+    closure_table_kernel(const uint32_t* row_ptr, const uint16_t* col, uint32_t n, uint32_t seeds,
+                         unsigned long long* cnt, unsigned long long* hdr, uint16_t* tab, uint32_t* failed) {
+  __shared__ uint32_t hist_words[kTableWarps][kTableMaxBuckets / 4];
+  const uint32_t lane = threadIdx.x & 31u, below = (1u << lane) - 1u;
+  const unsigned long long u = (static_cast<unsigned long long>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5;
+  if (u >= n) return;  // warp-uniform
+  uint32_t* hw = hist_words[threadIdx.x >> 5];
+  uint8_t* hist = reinterpret_cast<uint8_t*>(hw);
+  const uint32_t lo = row_ptr[u], hi = row_ptr[u + 1];
+  // places the row into nb buckets under `seed`: false as soon as a bucket would get a fifth entry; writes the entries
+  // to out when it is given (counts stay below 4 + 32, so a byte holds them)
+  auto place = [&](uint32_t nb, uint32_t seed, uint16_t* out) -> bool {
+    for (uint32_t i = lane; i < (nb + 3) / 4; i += 32) hw[i] = 0;
+    __syncwarp();
+    for (uint32_t b = lo; b < hi; b += 32) {
+      const bool mine = b + lane < hi;
+      const uint32_t v = mine ? col[b + lane] : 0u;
+      const uint32_t k = mine ? table_bucket(v, seed, nb) : ~0u;
+      const unsigned peers = __match_any_sync(0xFFFFFFFFu, k);
+      const uint32_t base = mine ? hist[k] : 0u, slot = base + __popc(peers & below);
+      __syncwarp();
+      if (mine && !(peers & below)) hist[k] = static_cast<uint8_t>(base + __popc(peers));
+      __syncwarp();
+      if (__any_sync(0xFFFFFFFFu, mine && slot >= kTableSlots)) return false;
+      if (out && mine) out[static_cast<unsigned long long>(k) * kTableSlots + slot] = static_cast<uint16_t>(v);
+    }
+    return true;
+  };
+  if (!tab) {
+    uint32_t nb = table_first_nb(hi - lo), seed = 0;
+    bool ok = hi == lo;
+    while (!ok && nb <= kTableMaxBuckets) {
+      for (seed = 0; seed < seeds; ++seed)
+        if ((ok = place(nb, seed, nullptr))) break;
+      if (!ok) nb = table_grow_nb(nb);
+    }
+    if (!ok) {
+      if (lane == 0) atomicExch(failed, 1u);
+      return;
+    }
+    if (lane == 0) {
+      cnt[u + 1] = nb;
+      hdr[u] = table_header(0, nb, seed);
+    }
+  } else {
+    const unsigned long long h = hdr[u], off = cnt[u];
+    const uint32_t nb = static_cast<uint32_t>(h >> 32) & 0xFFFFFFu, seed = static_cast<uint32_t>(h >> 56);
+    place(nb, seed, tab + off * kTableSlots);
+    if (lane == 0) hdr[u] = table_header(static_cast<uint32_t>(off), nb, seed);
+  }
+}
+
 }  // namespace
 
 std::string gpu_build_closure(const Snapshot& s, const DCls& a, const DCls& b, uint64_t cap, Snapshot::Closure* c,
@@ -336,6 +397,63 @@ std::string gpu_build_closure_sig(Snapshot::Closure* c, uint32_t words, cudaStre
   }
   BCUDA(cudaStreamSynchronize(st));
   c->sig_words = words;
+  return "";
+}
+
+std::string gpu_build_closure_table(Snapshot::Closure* c, uint32_t seeds, cudaStream_t st) {
+  c->set_built = false;
+  c->set_buckets = 0;
+  auto none = [c]() {
+    c->set_hdr.release();
+    c->set_tab.release();
+    return std::string();
+  };
+  if (!c->built || c->width != 2 || c->nsubj == 0 || seeds == 0) return none();
+  seeds = std::min(seeds, 256u);  // (8 bits of the header)
+  const size_t n = c->nsubj;
+  DevBuf d_cnt, d_tmp, d_failed;
+  struct Release {
+    std::vector<DevBuf*> v;
+    ~Release() {
+      for (DevBuf* x : v) x->release();
+    }
+  } rel{{&d_cnt, &d_tmp, &d_failed}};
+  if (!c->set_hdr.ensure(n * 8) || !d_cnt.ensure((n + 1) * 8) || !d_failed.ensure(4))
+    return "out of device memory (closure set table)";
+  unsigned long long* cnt = d_cnt.as<unsigned long long>();
+  BCUDA(cudaMemsetAsync(cnt, 0, (n + 1) * 8, st));
+  BCUDA(cudaMemsetAsync(d_failed.p, 0, 4, st));
+  const unsigned blk = kTableWarps * 32;
+  const unsigned long long grid = (static_cast<unsigned long long>(n) * 32 + blk - 1) / blk;
+  const uint32_t* rp = c->row_ptr.as<uint32_t>();
+  const uint16_t* col = c->col.as<uint16_t>();
+  closure_table_kernel<<<grid, blk, 0, st>>>(rp, col, c->nsubj, seeds, cnt, c->set_hdr.as<unsigned long long>(), nullptr,
+                                             d_failed.as<uint32_t>());
+  BCUDA(cudaGetLastError());
+  size_t tb = 0;
+  cub::DeviceScan::InclusiveSum(nullptr, tb, cnt, cnt, n + 1, st);
+  if (!d_tmp.ensure(tb + 256)) return "out of device memory (closure set table)";
+  tb = d_tmp.cap;
+  BCUDA(cub::DeviceScan::InclusiveSum(d_tmp.p, tb, cnt, cnt, n + 1, st));
+  unsigned long long total = 0;
+  uint32_t failed = 0;
+  BCUDA(cudaMemcpyAsync(&total, cnt + n, 8, cudaMemcpyDeviceToHost, st));
+  BCUDA(cudaMemcpyAsync(&failed, d_failed.p, 4, cudaMemcpyDeviceToHost, st));
+  BCUDA(cudaStreamSynchronize(st));
+  // a row that needs more buckets than the build takes, or a first bucket past 32 bits: no table
+  if (failed || total >= (1ull << 32)) return none();
+  const size_t bytes = size_t(total) * 8;
+  size_t free_b = 0, total_b = 0;
+  BCUDA(cudaMemGetInfo(&free_b, &total_b));
+  if (bytes + n * 8 > (free_b + c->set_tab.cap + c->set_hdr.cap) / 4) return none();  // (the pair's old buffers are reused)
+  if (!c->set_tab.ensure(bytes ? bytes : 8)) return "out of device memory (closure set table)";
+  BCUDA(cudaMemsetAsync(c->set_tab.p, 0xFF, bytes ? bytes : 8, st));
+  closure_table_kernel<<<grid, blk, 0, st>>>(rp, col, c->nsubj, seeds, cnt, c->set_hdr.as<unsigned long long>(),
+                                             c->set_tab.as<uint16_t>(), d_failed.as<uint32_t>());
+  BCUDA(cudaGetLastError());
+  BCUDA(cudaStreamSynchronize(st));
+  c->set_buckets = total;
+  c->set_built = true;
   return "";
 }
 

@@ -20,6 +20,7 @@
 #include <vector>
 
 #include "../../include/zgpu.h"
+#include "closure_sig.cuh"
 #include "device.h"
 #include "schema.h"
 #include "store.h"
@@ -3182,6 +3183,40 @@ extern "C" int zg_closure_signature_copy(zg_engine* e, uint32_t pair, uint64_t* 
   if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->dev.stream);
   if (ce == cudaSuccess && *n_words) ce = cudaMemcpy(words, x.sig.p, *n_words * 8, cudaMemcpyDeviceToHost);
   return ce == cudaSuccess ? ZG_OK : fail(ZG_ECUDA, std::string("zg_closure_signature_copy: ") + cudaGetErrorString(ce));
+}
+
+extern "C" int zg_closure_table_info(zg_engine* e, uint32_t pair, uint64_t* out) {
+  if (!e || !out) return fail(ZG_EINVAL, "NULL argument");
+  LOCK_DEVICE(e);
+  const auto s = e->dev.snap;
+  if (!s) return fail(ZG_ENOSNAPSHOT, "no snapshot published (call zg_publish)");
+  if (pair >= s->closure.size()) return fail(ZG_EINVAL, "no two-level pair with this number");
+  const auto& x = s->closure[pair];
+  const bool b = x.built && x.set_built;
+  const uint64_t c[5] = {b ? 1u : 0u, b ? x.set_buckets : 0u, b ? zg::kTableSlots : 0u,
+                         b ? (uint64_t(x.nsubj) + x.set_buckets) * 8 : 0u, b ? static_cast<uint64_t>(x.set_ms * 1000.0) : 0u};
+  std::memcpy(out, c, sizeof c);
+  return ZG_OK;
+}
+
+extern "C" int zg_closure_table_copy(zg_engine* e, uint32_t pair, uint64_t* hdr, uint64_t hdr_cap, uint64_t* buckets,
+                                     uint64_t bucket_cap, uint64_t* n_rows, uint64_t* n_buckets) {
+  if (!e || !n_rows || !n_buckets) return fail(ZG_EINVAL, "NULL argument");
+  LOCK_DEVICE(e);
+  const auto s = e->dev.snap;
+  if (!s) return fail(ZG_ENOSNAPSHOT, "no snapshot published (call zg_publish)");
+  if (pair >= s->closure.size() || !s->closure[pair].built || !s->closure[pair].set_built)
+    return fail(ZG_EINVAL, "no closure set table for this pair");
+  const auto& x = s->closure[pair];
+  *n_rows = x.nsubj;
+  *n_buckets = x.set_buckets;
+  if (hdr_cap < *n_rows || bucket_cap < *n_buckets || (!hdr && *n_rows) || (!buckets && *n_buckets))
+    return fail(ZG_E2BIG, "buffer too small for the closure set table");
+  cudaError_t ce = cudaSetDevice(e->dev.device);
+  if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->dev.stream);
+  if (ce == cudaSuccess && *n_rows) ce = cudaMemcpy(hdr, x.set_hdr.p, *n_rows * 8, cudaMemcpyDeviceToHost);
+  if (ce == cudaSuccess && *n_buckets) ce = cudaMemcpy(buckets, x.set_tab.p, *n_buckets * 8, cudaMemcpyDeviceToHost);
+  return ce == cudaSuccess ? ZG_OK : fail(ZG_ECUDA, std::string("zg_closure_table_copy: ") + cudaGetErrorString(ce));
 }
 
 extern "C" int zg_handle_lookup_counters(zg_engine* e, uint64_t* out) {

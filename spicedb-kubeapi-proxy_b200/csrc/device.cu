@@ -73,6 +73,8 @@ Snapshot::~Snapshot() {
     c.row_ptr.release();
     c.col.release();
     c.sig.release();
+    c.set_hdr.release();
+    c.set_tab.release();
   }
 }
 
@@ -130,6 +132,7 @@ std::string Device::init(int dev, uint64_t subq_cap, uint32_t budget) {
   if (const char* v = std::getenv("ZGPU_CLOSURE_CAP")) closure_cap_ = std::strtoull(v, nullptr, 10);  // tests: 0 = no index
   if (const char* v = std::getenv("ZGPU_CLOSURE_SIG_WORDS"))  // tests: 0 = no signatures, 1 = one word (most tests maybe)
     closure_sig_words_ = static_cast<uint32_t>(std::strtoul(v, nullptr, 10));
+  if (const char* v = std::getenv("ZGPU_CLOSURE_TABLE")) closure_table_ = !(*v == '0' && !v[1]);  // tests: 0 = no tables
   int count = 0;
   cudaError_t e = cudaGetDeviceCount(&count);
   if (e != cudaSuccess || count == 0)
@@ -346,6 +349,9 @@ void Device::build_closures(Snapshot* s, const HostSnapshot& h, const std::vecto
       c.col.release();
       c.sig.release();
       c.sig_words = 0;
+      c.set_hdr.release();
+      c.set_tab.release();
+      c.set_built = false;
       cudaGetLastError();
       ++closure_failures;
       continue;
@@ -364,6 +370,23 @@ void Device::build_closures(Snapshot* s, const HostSnapshot& h, const std::vecto
     if (!err.empty()) {
       c.sig.release();
       c.sig_words = 0;
+      cudaGetLastError();
+    }
+    // And the set tables, for 16-bit indexes whose target type leaves 0xFFFF free to mark an empty slot: without them
+    // sig_meet searches the row for each "maybe" (or, without signatures, the pair meets through closure_meet).
+    const bool table = closure_table_ && width == 2 && h.n_objects[cls[c.tgc].rtype] < 65536u;
+    cudaEventRecord(e0, stream);
+    err = gpu_build_closure_table(&c, table ? kTableSeeds : 0u, stream);
+    cudaEventRecord(e1, stream);
+    cudaEventSynchronize(e1);
+    ms = 0;
+    cudaEventElapsedTime(&ms, e0, e1);
+    closure_ms += ms;
+    c.set_ms = ms;
+    if (!err.empty()) {
+      c.set_hdr.release();
+      c.set_tab.release();
+      c.set_built = false;
       cudaGetLastError();
     }
   }
@@ -456,6 +479,8 @@ std::string Device::finish_publish(std::shared_ptr<Snapshot> s, const HostSnapsh
         old->row_ptr = DevBuf{};  // moved
         old->col = DevBuf{};
         old->sig = DevBuf{};
+        old->set_hdr = DevBuf{};
+        old->set_tab = DevBuf{};
       } else {
         pairs.emplace_back();
         pairs.back().inner = inner;
@@ -466,6 +491,8 @@ std::string Device::finish_publish(std::shared_ptr<Snapshot> s, const HostSnapsh
       c.row_ptr.release();
       c.col.release();
       c.sig.release();
+      c.set_hdr.release();
+      c.set_tab.release();
     }
     s->closure = std::move(pairs);
     build_closures(s.get(), h, nullptr);
@@ -496,7 +523,9 @@ std::string Device::finish_publish(std::shared_ptr<Snapshot> s, const HostSnapsh
                      check_kernel<true, false, kMeet16>, check_kernel<false, true, kMeet16>,
                      check_kernel<false, false, kMeetSig16>, check_kernel<true, false, kMeetSig16>,
                      check_kernel<false, true, kMeetSig16>, check_kernel<false, false, kMeetSig32>,
-                     check_kernel<true, false, kMeetSig32>, check_kernel<false, true, kMeetSig32>})
+                     check_kernel<true, false, kMeetSig32>, check_kernel<false, true, kMeetSig32>,
+                     check_kernel<false, false, kMeetSet16>, check_kernel<true, false, kMeetSet16>,
+                     check_kernel<false, true, kMeetSet16>})
         cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sm));
       attr_bytes = sm;
     }
@@ -558,15 +587,19 @@ int Device::run_pass(const Snapshot& s, const zg_check* queries, uint64_t nq, ui
   p.shard_rank = shard_rank;
   p.no_wildcards = no_wildcards_ ? 1 : 0;
   int meet = s.has_l2 ? kMeet32 : kMeetNone;
-  bool all_sig = true;
+  bool all_sig = true, all_set = true;
   for (const auto& c : s.closure)
     if (c.built) {
       p.closure[p.n_closure++] = ClosureRef{c.row_ptr.as<uint32_t>(), c.col.p, c.nsubj, c.tgc, c.width,
-                                            c.sig_words ? c.sig.as<unsigned long long>() : nullptr, c.sig_words};
+                                            c.sig_words ? c.sig.as<unsigned long long>() : nullptr, c.sig_words,
+                                            c.set_built ? c.set_hdr.as<unsigned long long>() : nullptr,
+                                            c.set_built ? c.set_tab.as<unsigned long long>() : nullptr};
       if (c.width == 2) meet = kMeet16;  // every built index of a snapshot has the same width
       all_sig = all_sig && c.sig_words;
+      all_set = all_set && c.set_built;
     }
-  if (p.n_closure && all_sig) meet |= kMeetSig;
+  if (p.n_closure && all_sig && all_set && meet == kMeet16) meet = kMeetSet16;
+  else if (p.n_closure && all_sig) meet |= kMeetSig;
   ZG_CUDA(cudaMemsetAsync(ctrl, 0, 16, st));  // next, subq_count
   const int per_sm = count ? blocks_per_sm_count_ : blocks_per_sm_;
   uint64_t want = (nq + kThreads - 1) / kThreads;
@@ -574,19 +607,28 @@ int Device::run_pass(const Snapshot& s, const zg_check* queries, uint64_t nq, ui
   if (grid < 1) grid = 1;
   size_t sm = smem_bytes(s.prog_bytes);
   // a schema without a two-level step runs the kernel built without the two-level meet; one with 16-bit closure
-  // indexes the kernel whose meet reads them; one whose every built index has signatures the kernel that tests them
-  auto pick = [meet](auto none, auto m32, auto m16, auto s32, auto s16) {
-    return meet == kMeetNone ? none : meet == kMeet16 ? m16 : meet == kMeetSig16 ? s16 : meet == kMeetSig32 ? s32 : m32;
+  // indexes the kernel whose meet reads them; one whose every built index has signatures the kernel that tests them,
+  // and one whose every built index also has a set table the kernel that confirms the signatures' "maybe"s in it
+  auto pick = [meet](auto none, auto m32, auto m16, auto s32, auto s16, auto t16) {
+    return meet == kMeetNone    ? none
+           : meet == kMeet16    ? m16
+           : meet == kMeetSig16 ? s16
+           : meet == kMeetSig32 ? s32
+           : meet == kMeetSet16 ? t16
+                                : m32;
   };
   if (count)
     pick(check_kernel<true, false, kMeetNone>, check_kernel<true>, check_kernel<true, false, kMeet16>,
-         check_kernel<true, false, kMeetSig32>, check_kernel<true, false, kMeetSig16>)<<<grid, kThreads, sm, st>>>(p);
+         check_kernel<true, false, kMeetSig32>, check_kernel<true, false, kMeetSig16>,
+         check_kernel<true, false, kMeetSet16>)<<<grid, kThreads, sm, st>>>(p);
   else if (ready)
     pick(check_kernel<false, true, kMeetNone>, check_kernel<false, true>, check_kernel<false, true, kMeet16>,
-         check_kernel<false, true, kMeetSig32>, check_kernel<false, true, kMeetSig16>)<<<grid, kThreads, sm, st>>>(p);
+         check_kernel<false, true, kMeetSig32>, check_kernel<false, true, kMeetSig16>,
+         check_kernel<false, true, kMeetSet16>)<<<grid, kThreads, sm, st>>>(p);
   else
     pick(check_kernel<false, false, kMeetNone>, check_kernel<false>, check_kernel<false, false, kMeet16>,
-         check_kernel<false, false, kMeetSig32>, check_kernel<false, false, kMeetSig16>)<<<grid, kThreads, sm, st>>>(p);
+         check_kernel<false, false, kMeetSig32>, check_kernel<false, false, kMeetSig16>,
+         check_kernel<false, false, kMeetSet16>)<<<grid, kThreads, sm, st>>>(p);
   ZG_CUDA(cudaGetLastError());
   ++launches;
   return ZG_OK;

@@ -70,6 +70,13 @@ struct Snapshot {
     DevBuf sig;
     uint32_t sig_words = 0;
     double sig_ms = 0;  // device time of its last build
+    // Set table of every row (closure_sig.cuh table_bucket; 16-bit indexes whose target type holds fewer than 65 536
+    // objects): set_hdr one header word per row, set_tab set_buckets buckets of four 16-bit slots. Empty when
+    // !set_built (the pair's steps meet through sig_meet or closure_meet).
+    DevBuf set_hdr, set_tab;
+    uint64_t set_buckets = 0;
+    bool set_built = false;
+    double set_ms = 0;  // device time of its last build
   };
   std::vector<Closure> closure;
   uint64_t n_tuples = 0, bytes = 0, revision = 0;
@@ -365,6 +372,7 @@ class Device {
   uint64_t closure_cap_ = ~0ull;  // ZGPU_CLOSURE_CAP: entries a closure index may hold (tests; ~0 = the size budget)
   uint32_t closure_sig_words_ = ~0u;  // ZGPU_CLOSURE_SIG_WORDS: signature words per row (tests; 0 = none, ~0 = chosen
                                       // from the mean row length, gpu_build_closure_sig)
+  bool closure_table_ = true;  // ZGPU_CLOSURE_TABLE: build the rows' set tables (tests; 0 = none)
   // (Re)builds the closure index of every pair of s->closure that is not built yet (`rebuild` false) or whose inner or
   // tgc class is marked in `rebuild` (a write changed it), from the classes' reverse rows described by h.cls. Decides
   // the entry width from h's object capacities first: 16-bit when every pair's tgc resource type holds at most 65 536
@@ -484,5 +492,10 @@ std::string gpu_build_closure(const Snapshot& s, const DCls& a, const DCls& b, u
 // words = ~0u, the fewest with 64 * words >= 12 x the mean row length (about 1 % false "maybe"s per test at 3 bits per
 // entry). None (c->sig_words = 0) when they would take more than a quarter of the free device memory.
 std::string gpu_build_closure_sig(Snapshot::Closure* c, uint32_t words, cudaStream_t st);
+// Builds the set table of the built 16-bit closure index *c (closure_sig.cuh), trying `seeds` seeds per bucket count.
+// None (c->set_built false) when the index is 32-bit, a row would need more than kTableMaxBuckets buckets, or the table
+// would take more than a quarter of the free device memory. The caller builds it only for a target type of fewer than
+// 65 536 objects (0xFFFF marks an empty slot).
+std::string gpu_build_closure_table(Snapshot::Closure* c, uint32_t seeds, cudaStream_t st);
 
 }  // namespace zg

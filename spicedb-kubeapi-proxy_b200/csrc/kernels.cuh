@@ -92,14 +92,20 @@ struct ClosureRef {
   // Signature of every row (closure_sig.cuh): sig_words 64-bit words per row, row u at sig[u * sig_words]. nullptr: none.
   const unsigned long long* sig;
   uint32_t sig_words;  // a power of two, 1 .. 32
+  // Set table of every row (closure_sig.cuh table_bucket): row u's header at set_hdr[u], its buckets from
+  // set_tab[header's first bucket]. nullptr: none.
+  const unsigned long long* set_hdr;
+  const unsigned long long* set_tab;
 };
 // check_kernel's MEET argument: no two-level step in the schema, or the width of the closure entries it reads, plus
-// kMeetSig when the meet tests the range against the rows' signatures (sig_meet) instead of streaming the rows
-constexpr int kMeetNone = 0, kMeet16 = 2, kMeet32 = 4, kMeetSig = 8;
-constexpr int kMeetSig16 = kMeet16 | kMeetSig, kMeetSig32 = kMeet32 | kMeetSig;
+// kMeetSig when the meet tests the range against the rows' signatures (sig_meet) instead of streaming the rows, or
+// also kMeetSet when the signatures' "maybe"s are confirmed in the rows' set tables (16-bit indexes only)
+constexpr int kMeetNone = 0, kMeet16 = 2, kMeet32 = 4, kMeetSig = 8, kMeetSet = 16;
+constexpr int kMeetSig16 = kMeet16 | kMeetSig, kMeetSig32 = kMeet32 | kMeetSig, kMeetSet16 = kMeetSig16 | kMeetSet;
 template <int MEET> struct ClosureEntry { using type = uint32_t; };
 template <> struct ClosureEntry<kMeet16> { using type = uint16_t; };
 template <> struct ClosureEntry<kMeetSig16> { using type = uint16_t; };
+template <> struct ClosureEntry<kMeetSet16> { using type = uint16_t; };
 
 struct KParams {
   const uint32_t* row_ptr;
@@ -639,11 +645,14 @@ __device__ __forceinline__ unsigned closure_meet(const uint32_t* __restrict__ co
 // per round with their loads in flight together, and only the "maybe"s are searched in the row. The searches of a round
 // run for the whole warp at once (one lane's search per test would stall the warp once per test). The COUNT variant
 // counts 4 bytes per child read, 8 per signature word and sizeof(E) per search probe. Returns the job slots answered.
-template <bool COUNT, class E>
+// SET (the row has a set table, closure_sig.cuh): rb is the row's first bucket in tab, re its bucket count | seed << 24,
+// and the "maybe"s of a round are confirmed by one exact lookup each, all in flight together, instead of searches: one
+// dependent load per round instead of ~7 per "maybe", and no lane waits on another's search. 8 bytes per lookup.
+template <bool COUNT, bool SET = false, class E>
 __device__ __forceinline__ unsigned sig_meet(const uint32_t* __restrict__ col, const E* __restrict__ ccol,
                                              const unsigned long long* __restrict__ sig, uint32_t lg, bool want, uint32_t lo,
                                              uint32_t hi, uint32_t rb, uint32_t re, uint32_t jslot,
-                                             unsigned long long* bytes) {
+                                             unsigned long long* bytes, const unsigned long long* __restrict__ tab = nullptr) {
   constexpr uint32_t kTests = 8;  // (4 spilled a little less and ran no faster on cfg3: DESIGN.md §6)
   unsigned long long nb = 0;
   unsigned hits = 0;
@@ -665,9 +674,23 @@ __device__ __forceinline__ unsigned sig_meet(const uint32_t* __restrict__ col, c
       }
       if (COUNT) nb += 12ull * n;
       lo += n;
+      if constexpr (SET) {
+        const uint32_t nbk = re & 0xFFFFFFu, seed = re >> 24;
+#pragma unroll
+        for (uint32_t i = 0; i < kTests; ++i) w[i] = (m >> i) & 1u ? __ldg(tab + rb + table_bucket(v[i], seed, nbk)) : ~0ull;
+        bool h = false;
+#pragma unroll
+        for (uint32_t i = 0; i < kTests; ++i) h = h || (((m >> i) & 1u) && table_has(w[i], v[i]));
+        if (COUNT) nb += 8ull * __popc(m);
+        m = h ? 1u : 0u;  // (as a hit below)
+      }
     }
     bool hit = false;
-    while (__any_sync(kFull, m != 0)) {
+    if constexpr (SET) {
+      hit = m != 0;
+      m = 0;
+    }
+    while (!SET && __any_sync(kFull, m != 0)) {
       if (m) {
         const uint32_t i = __ffs(m) - 1;
         m &= m - 1;
@@ -693,7 +716,8 @@ __device__ __forceinline__ unsigned sig_meet(const uint32_t* __restrict__ col, c
 // binary search of the row), and pushes the userset / arrow edge ranges. MEET = kMeetNone: the schema has no two-level
 // step, and the two-level meet is left out (its code costs the traversal loop registers: cfg4, DESIGN.md §6); else the
 // width of the closure entries the meet reads (kMeet16 / kMeet32: one closure_meet is inlined per instantiation;
-// kMeetSig16 / kMeetSig32: sig_meet instead, for snapshots whose every built index has signatures).
+// kMeetSig16 / kMeetSig32: sig_meet instead, for snapshots whose every built index has signatures; kMeetSet16:
+// sig_meet confirming in set tables, for snapshots whose every built index has signatures and a set table).
 template <bool COUNT, int MEET>
 __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<COUNT>& c, bool active,
                                       uint32_t jslot, uint32_t obj, uint32_t unit, uint32_t depth) {
@@ -753,11 +777,12 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
   const int maxsteps = __reduce_max_sync(kFull, npush);
   for (int i = 0; i < maxsteps; ++i) {
     using CE = typename ClosureEntry<MEET>::type;
-    constexpr bool kSig = (MEET & kMeetSig) != 0;
+    constexpr bool kSig = (MEET & kMeetSig) != 0, kSet = (MEET & kMeetSet) != 0;
     bool want = false, l2_want = false, cl_want = false;
     uint32_t l2_lo = 0, l2_hi = 0, l2_k = 0, cl_rb = 0, cl_re = 0, cl_lg = 0;
     const CE* cl_col = nullptr;
     const unsigned long long* cl_sig = nullptr;
+    const unsigned long long* cl_tab = nullptr;  // kSet: the set table's buckets
     uint4 item = make_uint4(0, 0, 0, 0);
     if (i < npush && !hit) {
       const DStep st = pr.steps()[sb + i];
@@ -777,18 +802,25 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
 #pragma unroll
           for (int k = 0; k < kMaxClosure; ++k)  // (by value: the address of a kernel parameter costs a local copy)
             if (k < static_cast<int>(p.n_closure) && p.closure[k].tgc == st.tgc && p.closure[k].width == sizeof(CE) &&
-                (!kSig || p.closure[k].sig)) {
-              crow = p.closure[k].row_ptr;
+                (!kSig || p.closure[k].sig) && (!kSet || p.closure[k].set_hdr)) {
+              crow = kSet ? reinterpret_cast<const uint32_t*>(p.closure[k].set_hdr) : p.closure[k].row_ptr;
               ccol = static_cast<const CE*>(p.closure[k].col);
               cn = p.closure[k].nsubj;
               if (kSig) {
                 cl_sig = p.closure[k].sig;
                 cl_lg = __ffs(p.closure[k].sig_words) - 1;
               }
+              if (kSet) cl_tab = p.closure[k].set_tab;
             }
           if (crow && stype == st.tstype && sid < cn) {
-            rb = __ldg(crow + sid);
-            re = __ldg(crow + sid + 1);
+            if (kSet) {  // rb: the row's first bucket, re: its bucket count | seed << 24 (closure_sig.cuh table_header)
+              const unsigned long long h = __ldg(reinterpret_cast<const unsigned long long*>(crow) + sid);
+              rb = static_cast<uint32_t>(h);
+              re = static_cast<uint32_t>(h >> 32);
+            } else {
+              rb = __ldg(crow + sid);
+              re = __ldg(crow + sid + 1);
+            }
             crow_read = true;
             if (kSig) {
               cl_sig += static_cast<unsigned long long>(sid) << cl_lg;
@@ -859,7 +891,7 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
               // intersected with the row by this lane.
               if (COUNT && crow_read) c.bytes += 8;
               if (kSig || hi - lo <= static_cast<uint32_t>(kFCap)) {  // (sig_meet's cost does not grow with the row)
-                cl_want = re > rb;
+                cl_want = kSet ? (re & 0xFFFFFFu) != 0 : re > rb;
                 l2_lo = lo;
                 l2_hi = hi;
                 cl_rb = rb;
@@ -911,7 +943,10 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
       const long long t2 = clock64();
 #endif
       unsigned long long cb = 0;
-      if constexpr (kSig)
+      if constexpr (kSet)
+        c.found |= sig_meet<COUNT, true>(p.col, cl_col, cl_sig, cl_lg, cl_want && !((c.found >> jslot) & 1u), l2_lo, l2_hi,
+                                         cl_rb, cl_re, jslot & 31u, COUNT ? &cb : nullptr, cl_tab);
+      else if constexpr (kSig)
         c.found |= sig_meet<COUNT>(p.col, cl_col, cl_sig, cl_lg, cl_want && !((c.found >> jslot) & 1u), l2_lo, l2_hi, cl_rb,
                                    cl_re, jslot & 31u, COUNT ? &cb : nullptr);
       else
