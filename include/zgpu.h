@@ -188,6 +188,9 @@ typedef struct {
   uint64_t last_levels;        /* sharded handle, last coalesced group: pass levels run over the shards  */
   uint64_t last_subqueries;    /*   sub-queries the shards raised to each other                          */
   uint64_t last_round_trips;   /*   times the host waited for the devices                                */
+  uint64_t flat_slots;         /* slots of the published program whose checks the lean flat-check kernel */
+                               /*   answers (SF_FLAT; 0 when ZGPU_FLAT_CHECK=0)                          */
+  uint64_t flat_residual;      /* checks of those kernel's batches it left to the check kernel, in all   */
 } zg_stats;
 
 /* ---- lifecycle --------------------------------------------------------- */

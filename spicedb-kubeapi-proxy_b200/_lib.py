@@ -68,7 +68,8 @@ class _Stats(C.Structure):
                 ("delta_publishes", C.c_uint64), ("full_publishes", C.c_uint64), ("last_publish_ms", C.c_double),
                 ("streamed_calls", C.c_uint64), ("lookup_batches", C.c_uint64), ("lookups_batched", C.c_uint64),
                 ("devices", C.c_uint64), ("shards", C.c_uint64), ("last_levels", C.c_uint64),
-                ("last_subqueries", C.c_uint64), ("last_round_trips", C.c_uint64)]
+                ("last_subqueries", C.c_uint64), ("last_round_trips", C.c_uint64), ("flat_slots", C.c_uint64),
+                ("flat_residual", C.c_uint64)]
 
 
 class _Update(C.Structure):

@@ -3401,7 +3401,9 @@ extern "C" int zg_stats_get(zg_engine* e, zg_stats* out) {
   if (e->dev.snap) {
     out->tuples = e->dev.snap->n_tuples;
     out->snapshot_bytes = e->dev.snap->bytes;
+    out->flat_slots = e->dev.snap->flat_slots;
   }
+  if (!e->host_only) out->flat_residual = e->dev.flat_residual();
   for (uint32_t k = 1; k < e->n_shards && !e->host_only; ++k)  // a sharded handle: every shard's part
     if (const auto s = shard(e, k).snap) {
       out->tuples += s->n_tuples;

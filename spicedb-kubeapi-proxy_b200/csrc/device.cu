@@ -84,6 +84,8 @@ Device::~Device() {
   spill_.release();
   ctrl_.release();
   memo_.release();
+  flat_ctrl_.release();
+  flat_idx_.release();
   for (auto* v : {&q_, &parent_, &val_})
     for (auto& b : *v) b.release();
   stage_in_.release();
@@ -133,6 +135,7 @@ std::string Device::init(int dev, uint64_t subq_cap, uint32_t budget) {
   if (const char* v = std::getenv("ZGPU_CLOSURE_SIG_WORDS"))  // tests: 0 = no signatures, 1 = one word (most tests maybe)
     closure_sig_words_ = static_cast<uint32_t>(std::strtoul(v, nullptr, 10));
   if (const char* v = std::getenv("ZGPU_CLOSURE_TABLE")) closure_table_ = !(*v == '0' && !v[1]);  // tests: 0 = no tables
+  if (const char* v = std::getenv("ZGPU_FLAT_CHECK")) flat_check_ = !(*v == '0' && !v[1]);  // tests, A/B: 0 = no SF_FLAT
   int count = 0;
   cudaError_t e = cudaGetDeviceCount(&count);
   if (e != cudaSuccess || count == 0)
@@ -158,8 +161,9 @@ std::string Device::init(int dev, uint64_t subq_cap, uint32_t budget) {
   cudaEventCreateWithFlags(&ev_reset_, cudaEventDisableTiming);
   if (subq_cap) subq_cap_ = subq_cap;
   if (budget) budget_ = budget;
-  if (!ctrl_.ensure(128)) return "out of device memory";
+  if (!ctrl_.ensure(128) || !flat_ctrl_.ensure(16)) return "out of device memory";
   cudaMemset(ctrl_.p, 0, 128);
+  cudaMemset(flat_ctrl_.p, 0, 16);
   return "";
 }
 
@@ -496,14 +500,22 @@ std::string Device::finish_publish(std::shared_ptr<Snapshot> s, const HostSnapsh
     }
     s->closure = std::move(pairs);
     build_closures(s.get(), h, nullptr);
-    // slots whose checks only meet over the indexes just built load no memberships at admission (kernels.cuh)
-    std::vector<uint16_t> indexed;
+    // slots whose checks only meet over the indexes just built load no memberships at admission (kernels.cuh), and
+    // those of them whose meets all have signatures and set tables are answered by flat_check_kernel
+    std::vector<uint16_t> indexed, tabled;
     for (const auto& c : s->closure)
-      if (c.built) indexed.push_back(c.tgc);
-    if (!indexed.empty() && mark_rsetless_slots(&blob, indexed) &&
-        (cudaMemcpyAsync(s->prog.p, blob.data(), blob.size(), cudaMemcpyHostToDevice, stream) != cudaSuccess ||
-         cudaStreamSynchronize(stream) != cudaSuccess))
-      return std::string("snapshot upload failed: ") + cudaGetErrorString(cudaGetLastError());
+      if (c.built) {
+        indexed.push_back(c.tgc);
+        if (c.sig_words && c.set_built) tabled.push_back(c.tgc);
+      }
+    if (!flat_check_) tabled.clear();
+    s->flat_slots = 0;
+    if (!indexed.empty() && mark_rsetless_slots(&blob, indexed)) {
+      s->flat_slots = static_cast<uint32_t>(mark_flat_slots(&blob, tabled));
+      if (cudaMemcpyAsync(s->prog.p, blob.data(), blob.size(), cudaMemcpyHostToDevice, stream) != cudaSuccess ||
+          cudaStreamSynchronize(stream) != cudaSuccess)
+        return std::string("snapshot upload failed: ") + cudaGetErrorString(cudaGetLastError());
+    }
   }
   s->revision = revision;
 
@@ -525,7 +537,8 @@ std::string Device::finish_publish(std::shared_ptr<Snapshot> s, const HostSnapsh
                      check_kernel<false, true, kMeetSig16>, check_kernel<false, false, kMeetSig32>,
                      check_kernel<true, false, kMeetSig32>, check_kernel<false, true, kMeetSig32>,
                      check_kernel<false, false, kMeetSet16>, check_kernel<true, false, kMeetSet16>,
-                     check_kernel<false, true, kMeetSet16>})
+                     check_kernel<false, true, kMeetSet16>, check_kernel<false, false, kMeetSet16, true>,
+                     check_kernel<true, false, kMeetSet16, true>})
         cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(sm));
       attr_bytes = sm;
     }
@@ -549,7 +562,7 @@ std::string Device::finish_publish(std::shared_ptr<Snapshot> s, const HostSnapsh
 
 int Device::run_pass(const Snapshot& s, const zg_check* queries, uint64_t nq, uint8_t* val, uint8_t* out, bool final_codes,
                      bool raw, zg_check* subq, uint32_t* subq_parent, cudaStream_t st, bool count, std::string* err,
-                     const unsigned long long* ready) {
+                     const unsigned long long* ready, bool lean) {
   KParams p{};
   p.ready = ready;
   p.row_ptr = s.row_ptr.as<uint32_t>();
@@ -600,7 +613,11 @@ int Device::run_pass(const Snapshot& s, const zg_check* queries, uint64_t nq, ui
     }
   if (p.n_closure && all_sig && all_set && meet == kMeet16) meet = kMeetSet16;
   else if (p.n_closure && all_sig) meet |= kMeetSig;
-  ZG_CUDA(cudaMemsetAsync(ctrl, 0, 16, st));  // next, subq_count
+  // SF_FLAT slots are marked only where every pair they meet over has signatures and a set table, but another pair
+  // may lack them (the snapshot then meets through kMeetSig16): flat_check_kernel runs only with kMeetSet16, whose
+  // check_kernel answers its residual. Not for streamed items, which are still landing.
+  const bool flat = lean && s.flat_slots && meet == kMeetSet16 && p.invert && !ready && nq < (1ull << 32);
+  if (!flat) ZG_CUDA(cudaMemsetAsync(ctrl, 0, 16, st));  // next, subq_count (flat_check_kernel clears them itself)
   const int per_sm = count ? blocks_per_sm_count_ : blocks_per_sm_;
   uint64_t want = (nq + kThreads - 1) / kThreads;
   int grid = static_cast<int>(std::min<uint64_t>(want, static_cast<uint64_t>(sm_count_) * per_sm));
@@ -617,6 +634,36 @@ int Device::run_pass(const Snapshot& s, const zg_check* queries, uint64_t nq, ui
            : meet == kMeetSet16 ? t16
                                 : m32;
   };
+  if (flat) {
+    if (!flat_idx_.ensure(nq * sizeof(uint32_t))) {
+      if (err) *err = "out of device memory (residual list)";
+      return ZG_ENOMEM;
+    }
+    p.idx = flat_idx_.as<uint32_t>();
+    p.nq_dev = flat_ctrl_.as<unsigned long long>();
+    ZG_CUDA(cudaMemsetAsync(p.nq_dev, 0, 8, st));
+    const unsigned fgrid = static_cast<unsigned>((nq + kFlatThreads - 1) / kFlatThreads);
+    if (count) flat_check_kernel<true><<<fgrid, kFlatThreads, 0, st>>>(p);
+    else flat_check_kernel<false><<<fgrid, kFlatThreads, 0, st>>>(p);
+    ZG_CUDA(cudaGetLastError());
+    ++launches;
+    // the residual pass, launched as a programmatic dependent (Hopper): its blocks start as the lean kernel's finish
+    // and wait in cudaGridDependencySynchronize for its residual list, instead of after a full launch gap
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(grid);
+    cfg.blockDim = dim3(kThreads);
+    cfg.dynamicSmemBytes = sm;
+    cfg.stream = st;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    ZG_CUDA(count ? cudaLaunchKernelEx(&cfg, check_kernel<true, false, kMeetSet16, true>, p)
+                  : cudaLaunchKernelEx(&cfg, check_kernel<false, false, kMeetSet16, true>, p));
+    ++launches;
+    return ZG_OK;
+  }
   if (count)
     pick(check_kernel<true, false, kMeetNone>, check_kernel<true>, check_kernel<true, false, kMeet16>,
          check_kernel<true, false, kMeetSig32>, check_kernel<true, false, kMeetSig16>,
@@ -632,6 +679,16 @@ int Device::run_pass(const Snapshot& s, const zg_check* queries, uint64_t nq, ui
   ZG_CUDA(cudaGetLastError());
   ++launches;
   return ZG_OK;
+}
+
+uint64_t Device::flat_residual() {
+  unsigned long long n[2] = {0, 0};
+  // after the last call's kernels, whichever stream the caller enqueued them on
+  if (flat_ctrl_.p && cudaSetDevice(device) == cudaSuccess &&
+      (!have_last_ || cudaStreamWaitEvent(stream, last_done_, 0) == cudaSuccess) &&
+      cudaMemcpyAsync(n, flat_ctrl_.p, sizeof n, cudaMemcpyDeviceToHost, stream) == cudaSuccess)
+    cudaStreamSynchronize(stream);
+  return n[1];
 }
 
 void Device::read_events(uint64_t* spills, uint64_t* memo_batches) {
@@ -690,7 +747,7 @@ int Device::check_device(const zg_check* d_items, uint64_t n, uint8_t* d_out, cu
   int rc = ZG_OK;
   if (!s->has_nonpure) {
     // every slot is a relation or a pure union: one leaf per check, answered in one launch
-    rc = run_pass(*s, d_items, n, nullptr, d_out, true, raw_items, nullptr, nullptr, st, count, err, ready);
+    rc = run_pass(*s, d_items, n, nullptr, d_out, true, raw_items, nullptr, nullptr, st, count, err, ready, true);
     if (rc) return rc;
   } else {
     if (n * L >= (1ull << 32)) {
@@ -729,7 +786,8 @@ int Device::check_device(const zg_check* d_items, uint64_t n, uint8_t* d_out, cu
       // Level 0 writes the v1 codes straight into d_out: when the pass raises no sub-query (the
       // common case: edges into a non-pure permission are rare) they are final and nothing is folded.
       rc = run_pass(*s, queries, cur, val_[lv].as<uint8_t>(), lv == 0 ? d_out : nullptr, true, raw,
-                    q_[lv + 1].as<zg_check>(), parent_[lv + 1].as<uint32_t>(), st, count, err, lv == 0 ? ready : nullptr);
+                    q_[lv + 1].as<zg_check>(), parent_[lv + 1].as<uint32_t>(), st, count, err, lv == 0 ? ready : nullptr,
+                    lv == 0);
       if (rc) return rc;
       unsigned long long host_ctrl[4];
       ZG_CUDA(cudaMemcpyAsync(host_ctrl, ctrl, sizeof host_ctrl, cudaMemcpyDeviceToHost, st));

@@ -55,6 +55,7 @@ struct Snapshot {
   uint32_t max_leaves = 1;
   bool has_nonpure = false;
   bool has_l2 = false;  // some step of the program meets two levels (kStepTargetL2)
+  uint32_t flat_slots = 0;  // slots marked SF_FLAT at publish (mark_flat_slots): checks flat_check_kernel answers
   // Closure index of every (innermost direct class, userset class tgc) pair of the two-level steps (kernels.cuh
   // ClosureRef; built by gpu_build_closure, unsharded engines only). A pair over the size budget has none.
   struct Closure {
@@ -367,12 +368,16 @@ class Device {
   bool invert = true;  // direction-optimised probes (ZG_FLAG_FORWARD_ONLY / ZGPU_NO_INVERT=1 disable)
   uint32_t now = 0;  // clock for expiration, set by the caller before each hot-path call
   uint64_t last_alg_bytes = 0;
+  // Checks of flat_check_kernel's passes left to check_kernel so far: a synchronous device read, ordered after the
+  // last check call's kernels on whatever stream they were enqueued (zg_stats_get)
+  uint64_t flat_residual();
 
  private:
   uint64_t closure_cap_ = ~0ull;  // ZGPU_CLOSURE_CAP: entries a closure index may hold (tests; ~0 = the size budget)
   uint32_t closure_sig_words_ = ~0u;  // ZGPU_CLOSURE_SIG_WORDS: signature words per row (tests; 0 = none, ~0 = chosen
                                       // from the mean row length, gpu_build_closure_sig)
   bool closure_table_ = true;  // ZGPU_CLOSURE_TABLE: build the rows' set tables (tests; 0 = none)
+  bool flat_check_ = true;     // ZGPU_FLAT_CHECK: mark SF_FLAT slots at publish (tests and A/B runs; 0 = none)
   // (Re)builds the closure index of every pair of s->closure that is not built yet (`rebuild` false) or whose inner or
   // tgc class is marked in `rebuild` (a write changed it), from the classes' reverse rows described by h.cls. Decides
   // the entry width from h's object capacities first: 16-bit when every pair's tgc resource type holds at most 65 536
@@ -387,14 +392,17 @@ class Device {
   int ingress_sync(const Store& store, cudaStream_t st, std::string* err);
   std::string finish_publish(std::shared_ptr<Snapshot> s, const HostSnapshot& lay, const Schema& sc, uint64_t revision);
   // One check_kernel launch over `nq` queries: val (may be null) receives the per-(query, leaf) value
-  // bits, out (may be null) the per-query v1 codes / value bits.
+  // bits, out (may be null) the per-query v1 codes / value bits. lean: the queries are callers' (level 0 of an
+  // unsharded engine): when the snapshot has SF_FLAT slots and meets through set tables, flat_check_kernel answers
+  // theirs first and check_kernel only the rest.
   int run_pass(const Snapshot& s, const zg_check* queries, uint64_t nq, uint8_t* val, uint8_t* out, bool final_codes,
                bool raw, zg_check* subq, uint32_t* subq_parent, cudaStream_t st, bool count, std::string* err,
-               const unsigned long long* ready = nullptr);
+               const unsigned long long* ready = nullptr, bool lean = false);
   int sm_count_ = 0, blocks_per_sm_ = 0, blocks_per_sm_count_ = 0;
   uint32_t spill_cap_ = 4096, budget_ = 1u << 20;
   uint64_t subq_cap_ = 1ull << 22;
   DevBuf spill_, ctrl_, memo_;
+  DevBuf flat_ctrl_, flat_idx_;  // flat_check_kernel: [0] the pass's residual, [1] the running total; the residual list
   uint32_t memo_entries_ = 8192, memo_after_ = 2048;  // ctrl: [0] next, [1] subq_count, [2] alg_bytes, then flags u32;
                                                       // [8 .. 9] events, [10] items landed, [11 .. 15] phase clocks
   std::vector<DevBuf> q_, parent_, val_;  // per pass level: queries, raising (query, leaf), leaf values

@@ -157,6 +157,11 @@ struct KParams {
   // two-level steps whose pair has a closure index meet over it; the others keep batch_l2
   ClosureRef closure[kMaxClosure];
   uint32_t n_closure;
+  // The residual pass after flat_check_kernel (check_kernel<..., RESIDUAL = true> only): the pass's i-th query is
+  // queries[idx[i]], and the pass has *nq_dev queries (nq is only the grid's bound). flat_check_kernel writes both:
+  // nq_dev[0] = this pass's residual, nq_dev[1] += it (a running total). nullptr: queries[i], nq.
+  uint32_t* idx;
+  unsigned long long* nq_dev;
 };
 
 // View of the program blob. Only the base pointer is kept in registers; table addresses are
@@ -293,6 +298,26 @@ __device__ __forceinline__ bool probe(const KParams& p, WarpCtx<COUNT>& c, uint3
   return true;
 }
 
+// A probe step (ST_DIRECT / ST_WILD) answered from the forward rows: is sid a direct subject of obj in the step's class,
+// or has obj a wildcard relationship of it, unexpired at p.now. visit's non-inverted probes and flat_check_kernel's.
+// expiry: the step's class has CF_EXPIRY.
+template <bool COUNT>
+__device__ __forceinline__ bool probe_step(const KParams& p, WarpCtx<COUNT>& c, const DStep& st, uint32_t obj,
+                                           uint32_t sid, bool expiry) {
+  if (obj >= st.nres) return false;
+  const unsigned long long ridx = st.row_base + static_cast<unsigned long long>(obj) * st.ncls;
+  const uint32_t lo = __ldg(p.row_ptr + ridx), hi = __ldg(p.row_ptr + ridx + 1);
+  if (COUNT) c.bytes += 8;
+  if (hi <= lo) return false;
+  if (st.kind == ST_DIRECT) return probe(p, c, lo, hi, sid, expiry);
+  if (expiry) {  // ST_WILD
+    const uint32_t e = __ldg(p.exp + lo);
+    if (COUNT) c.bytes += 4;
+    return e == 0 || e > p.now;
+  }
+  return true;
+}
+
 // Two independent binary searches advanced in lock step (two loads in flight per lane).
 template <bool COUNT>
 __device__ __forceinline__ void probe2(const uint32_t* __restrict__ arr, WarpCtx<COUNT>& c, uint32_t lo0, uint32_t hi0,
@@ -362,7 +387,6 @@ constexpr uint32_t kOverCap = 63;
 __device__ __forceinline__ uint32_t cst_at(unsigned long long cst, uint32_t i) {
   return static_cast<uint32_t>(cst >> (5u * i)) & 31u;
 }
-constexpr int kMaxInvClasses = 11;
 static_assert(kRsetCap <= 31, "class boundaries are 5-bit fields");
 
 // Filter of batch_l2: two bits per object id in 128 (two 64-bit words). False-positive rate (1 - e^(-2n/128))^2 over
@@ -648,12 +672,49 @@ __device__ __forceinline__ unsigned closure_meet(const uint32_t* __restrict__ co
 // SET (the row has a set table, closure_sig.cuh): rb is the row's first bucket in tab, re its bucket count | seed << 24,
 // and the "maybe"s of a round are confirmed by one exact lookup each, all in flight together, instead of searches: one
 // dependent load per round instead of ~7 per "maybe", and no lane waits on another's search. 8 bytes per lookup.
+constexpr uint32_t kSigTests = 8;  // children per round of a signature meet (4 spilled a little less in check_kernel
+                                   // and ran no faster on cfg3: DESIGN.md §6)
+// One round of a lane's signature meet: loads the children col[lo, lo + n) (n <= kSigTests) into v, all in flight
+// together, then their signature words, and returns the mask of the children whose test said maybe. 12 bytes per child.
+template <bool COUNT>
+__device__ __forceinline__ unsigned sig_round(const uint32_t* __restrict__ col, uint32_t lo, uint32_t n,
+                                              const unsigned long long* __restrict__ sig, uint32_t lg, uint32_t (&v)[kSigTests],
+                                              unsigned long long& nb) {
+#pragma unroll
+  for (uint32_t i = 0; i < kSigTests; ++i) v[i] = i < n ? __ldg(col + lo + i) : 0u;
+  unsigned long long w[kSigTests];
+#pragma unroll
+  for (uint32_t i = 0; i < kSigTests; ++i) w[i] = i < n ? __ldg(sig + sig_word(v[i], lg)) : 0ull;
+  unsigned m = 0;
+#pragma unroll
+  for (uint32_t i = 0; i < kSigTests; ++i) {
+    const unsigned long long b = sig_mask(v[i]);
+    m |= (i < n && (w[i] & b) == b) ? 1u << i : 0u;
+  }
+  if (COUNT) nb += 12ull * n;
+  return m;
+}
+// The "maybe"s m of a round confirmed in the row's set table (buckets tab[0, nbk), hashed under seed): one exact lookup
+// each, all in flight together. True iff one of them is in the row. 8 bytes per lookup.
+template <bool COUNT>
+__device__ __forceinline__ bool table_round(const unsigned long long* __restrict__ tab, uint32_t nbk, uint32_t seed,
+                                            unsigned m, const uint32_t (&v)[kSigTests], unsigned long long& nb) {
+  unsigned long long w[kSigTests];
+#pragma unroll
+  for (uint32_t i = 0; i < kSigTests; ++i) w[i] = (m >> i) & 1u ? __ldg(tab + table_bucket(v[i], seed, nbk)) : ~0ull;
+  bool h = false;
+#pragma unroll
+  for (uint32_t i = 0; i < kSigTests; ++i) h = h || (((m >> i) & 1u) && table_has(w[i], v[i]));
+  if (COUNT) nb += 8ull * __popc(m);
+  return h;
+}
+
 template <bool COUNT, bool SET = false, class E>
 __device__ __forceinline__ unsigned sig_meet(const uint32_t* __restrict__ col, const E* __restrict__ ccol,
                                              const unsigned long long* __restrict__ sig, uint32_t lg, bool want, uint32_t lo,
                                              uint32_t hi, uint32_t rb, uint32_t re, uint32_t jslot,
                                              unsigned long long* bytes, const unsigned long long* __restrict__ tab = nullptr) {
-  constexpr uint32_t kTests = 8;  // (4 spilled a little less and ran no faster on cfg3: DESIGN.md §6)
+  constexpr uint32_t kTests = kSigTests;
   unsigned long long nb = 0;
   unsigned hits = 0;
   bool more = want && lo < hi;
@@ -662,28 +723,9 @@ __device__ __forceinline__ unsigned sig_meet(const uint32_t* __restrict__ col, c
     unsigned m = 0;  // the children of this round whose test said maybe
     if (more) {
       const uint32_t n = min(hi - lo, kTests);
-#pragma unroll
-      for (uint32_t i = 0; i < kTests; ++i) v[i] = i < n ? __ldg(col + lo + i) : 0u;
-      unsigned long long w[kTests];
-#pragma unroll
-      for (uint32_t i = 0; i < kTests; ++i) w[i] = i < n ? __ldg(sig + sig_word(v[i], lg)) : 0ull;
-#pragma unroll
-      for (uint32_t i = 0; i < kTests; ++i) {
-        const unsigned long long b = sig_mask(v[i]);
-        m |= (i < n && (w[i] & b) == b) ? 1u << i : 0u;
-      }
-      if (COUNT) nb += 12ull * n;
+      m = sig_round<COUNT>(col, lo, n, sig, lg, v, nb);
       lo += n;
-      if constexpr (SET) {
-        const uint32_t nbk = re & 0xFFFFFFu, seed = re >> 24;
-#pragma unroll
-        for (uint32_t i = 0; i < kTests; ++i) w[i] = (m >> i) & 1u ? __ldg(tab + rb + table_bucket(v[i], seed, nbk)) : ~0ull;
-        bool h = false;
-#pragma unroll
-        for (uint32_t i = 0; i < kTests; ++i) h = h || (((m >> i) & 1u) && table_has(w[i], v[i]));
-        if (COUNT) nb += 8ull * __popc(m);
-        m = h ? 1u : 0u;  // (as a hit below)
-      }
+      if constexpr (SET) m = table_round<COUNT>(tab + rb, re & 0xFFFFFFu, re >> 24, m, v, nb) ? 1u : 0u;  // (as a hit below)
     }
     bool hit = false;
     if constexpr (SET) {
@@ -754,21 +796,8 @@ __device__ __forceinline__ void visit(const KParams& p, const Prog& pr, WarpCtx<
       const uint32_t kb = cst_at(cst, st.tinv), ke = cst_at(cst, st.tinv + 1u);
       for (uint32_t r = kb; r < ke; ++r)
         hit = hit || c.rset[r * 32 + (jslot & 31)] == obj;
-    } else if (obj < st.nres) {
-      const unsigned long long ridx = st.row_base + static_cast<unsigned long long>(obj) * st.ncls;
-      const uint32_t lo = __ldg(p.row_ptr + ridx), hi = __ldg(p.row_ptr + ridx + 1);
-      if (COUNT) c.bytes += 8;
-      if (hi > lo) {
-        if (st.kind == ST_DIRECT) {
-          hit = probe(p, c, lo, hi, sid, expiry);
-        } else if (expiry) {  // ST_WILD
-          const uint32_t e = __ldg(p.exp + lo);
-          if (COUNT) c.bytes += 4;
-          hit = e == 0 || e > p.now;
-        } else {
-          hit = true;
-        }
-      }
+    } else {
+      hit = probe_step(p, c, st, obj, sid, expiry);
     }
   }
   if (hit) npush = 0;
@@ -1024,8 +1053,22 @@ __device__ __noinline__ void wait_ready(const unsigned long long* ready, unsigne
 // Per-lane query state parked in shared memory while the warp traverses (kStateWords words):
 //   0 resource object, 1 depth | leaves << 8 | is-tree << 15 | leaf_begin-or-unit << 16,
 //   2 tree id, 3 / 4 leaf values (2 bits each)
-template <bool COUNT, bool STREAMED = false, int MEET = kMeet32>
+// RESIDUAL: the residual pass of flat_check_kernel (KParams::idx / nq_dev; kMeetSet16, not streamed). Its own
+// instantiation: the fields cost the plain kernel's traversal loop spills (DESIGN.md §4).
+template <bool COUNT, bool STREAMED = false, int MEET = kMeet32, bool RESIDUAL = false>
 __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KParams p) {
+  static_assert(!RESIDUAL || (MEET == kMeetSet16 && !STREAMED), "the residual pass follows flat_check_kernel");
+  constexpr bool kResidual = RESIDUAL;
+  unsigned long long nq = p.nq;
+  if (kResidual) {
+#ifndef ZG_EMULATE
+    cudaGridDependencySynchronize();  // launched as flat_check_kernel's programmatic dependent: wait for its residual
+#endif
+    nq = *p.nq_dev;
+    if (nq == 0) return;
+  }
+  // the index in queries / out / val of the pass's i-th query
+  auto qidx = [&](unsigned long long i) -> unsigned long long { return kResidual ? p.idx[i] : i; };
   ZG_DYNAMIC_SMEM(smem);
   for (uint32_t i = threadIdx.x; i < p.prog_bytes / 16; i += blockDim.x)
     reinterpret_cast<uint4*>(smem)[i] = reinterpret_cast<const uint4*>(p.prog)[i];
@@ -1053,15 +1096,15 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
     if (lane == 0) {
       base = atomicAdd(p.next, 32ull);
       // the copy engine is still feeding the queries: wait until this batch has landed
-      if (STREAMED && base < p.nq) wait_ready(p.ready, base + 32 < p.nq ? base + 32 : p.nq, p.flags);
+      if (STREAMED && base < nq) wait_ready(p.ready, base + 32 < nq ? base + 32 : nq, p.flags);
     }
     base = __shfl_sync(kFull, base, 0);
-    if (base >= p.nq) break;
+    if (base >= nq) break;
 #if ZG_PHASE_CLOCKS
     const long long t_adm = clock64();
 #endif
     const unsigned long long q = base + lane;
-    const bool valid = q < p.nq;
+    const bool valid = q < nq;
     bool bad = false, expansive = false, no_rset = false;
     uint32_t nl = 0;
     c.my_subj = 0;
@@ -1069,7 +1112,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
     if (valid) {
       // ld.global.cg when the items are streamed in: nothing about them may come from a non-coherent cache
       const uint4 raw = STREAMED ? __ldcg(reinterpret_cast<const uint4*>(p.queries) + q)
-                                 : __ldg(reinterpret_cast<const uint4*>(p.queries) + q);
+                                 : __ldg(reinterpret_cast<const uint4*>(p.queries) + qidx(q));
       if (COUNT) c.bytes += 17;
       c.my_subj = raw.y;
       const uint32_t perm = raw.z & 0xFFFFu, stype = raw.z >> 16;
@@ -1295,7 +1338,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
               sq.srel = static_cast<uint16_t>(sq_ss & 0xFFFFu);
               sq.flags = static_cast<uint16_t>(cdepth);
               p.subq[at] = sq;
-              p.subq_parent[at] = static_cast<uint32_t>((base + jslot) * p.L + l);
+              p.subq_parent[at] = static_cast<uint32_t>(qidx(base + jslot) * p.L + l);
             } else {
               atomicOr(p.flags, 2u);
             }
@@ -1314,7 +1357,7 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
 
       if (act) {
         const bool t = (c.found >> lane) & 1u, e = (c.err >> lane) & 1u, r = (c.raised >> lane) & 1u;
-        if (p.val) p.val[q * p.L + l] = t ? kValT : (e ? kValE : 0);
+        if (p.val) p.val[qidx(q) * p.L + l] = t ? kValT : (e ? kValE : 0);
         // a leaf that raised sub-queries is not final unless it is already true
         const uint32_t v = t ? 1u : ((e || r) ? 2u : 0u);
         const uint32_t w1 = state[32];
@@ -1333,8 +1376,9 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
       }
     }
     if (valid && p.out) {
-      if (p.final_codes) p.out[q] = res == 1 ? ZG_HAS_PERMISSION : (res == 2 ? ZG_ITEM_ERROR : ZG_NO_PERMISSION);
-      else p.out[q] = res == 1 ? kValT : (res == 2 ? kValE : 0);
+      const unsigned long long qi = qidx(q);
+      if (p.final_codes) p.out[qi] = res == 1 ? ZG_HAS_PERMISSION : (res == 2 ? ZG_ITEM_ERROR : ZG_NO_PERMISSION);
+      else p.out[qi] = res == 1 ? kValT : (res == 2 ? kValE : 0);
     }
     __syncwarp();
   }
@@ -1348,6 +1392,155 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
   if (lane == 0)
     for (int i = 0; i < kPhases; ++i) atomicAdd(p.events + 3 + i, static_cast<unsigned long long>(c.ph[i]));
 #endif
+}
+
+// ---- flat checks: a slot whose checks are direct probes and two-level meets only (SF_FLAT) -----------------------
+//
+// One check per thread, no shared memory, no warp-collective traversal: the program's records are read from global
+// memory (a few hundred bytes, L1-resident). A check is answered here only when every step takes the branch
+// check_kernel<kMeetSet16> takes for it: a valid item without a subject relation, of an SF_FLAT slot, with room for the
+// two-level meet (hop depth + 2 <= ZG_MAX_DEPTH), and whose subject is of each meet step's type and has a row in its
+// closure index. Every other item is appended to the residual list (KParams::idx, count in nq_dev) that check_kernel
+// answers next. The answer is the same as check_kernel's, and so is the COUNT variant's byte count: the probes in step
+// order until one hits, then per meet step 8 bytes for the range's offsets, 8 for the subject's table header when the
+// range is not empty, and sig_meet's rounds (sig_round, table_round) until one finds the check.
+#ifndef ZG_FLAT_MIN_BLOCKS
+#define ZG_FLAT_MIN_BLOCKS 4
+#endif
+constexpr int kFlatThreads = 256;
+// 4 CTAs (32 warps) per SM, 64 registers: eight children's signature words and buckets in flight per thread. Measured on
+// cfg3 (H100, DESIGN.md §6): 1.19x faster than 6 CTAs at 40 registers with rounds of four children, which spill
+// nothing either, and 1.35x faster than 8 CTAs at 32.
+constexpr int kFlatMinBlocks = ZG_FLAT_MIN_BLOCKS;
+
+// A program record read through the read-only cache (records of 8-byte multiples, 8-byte aligned in the blob).
+template <class T>
+__device__ __forceinline__ T ldg_rec(const T* r) {
+  static_assert(sizeof(T) % 8 == 0, "8-byte words");
+  union {
+    unsigned long long w[sizeof(T) / 8];
+    T t;
+  } u;
+#pragma unroll
+  for (unsigned i = 0; i < sizeof(T) / 8; ++i) u.w[i] = __ldg(reinterpret_cast<const unsigned long long*>(r) + i);
+  return u.t;
+}
+
+template <bool COUNT>
+// (the COUNT variant is an instrument: it takes the registers it needs instead of the occupancy)
+__global__ void __launch_bounds__(kFlatThreads, COUNT ? 1 : kFlatMinBlocks) flat_check_kernel(const KParams p) {
+  const DHeader* const h = reinterpret_cast<const DHeader*>(p.prog);
+  const DStep* const steps = reinterpret_cast<const DStep*>(p.prog + __ldg(&h->off_steps));
+  const unsigned long long q = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x;
+  const unsigned lane = threadIdx.x & 31;
+  const bool valid = q < p.nq;
+  uint4 it = make_uint4(0, 0, 0, 0);
+  if (valid) it = __ldg(reinterpret_cast<const uint4*>(p.queries) + q);
+  const uint32_t obj = it.x, sid = it.y, perm = it.z & 0xFFFFu, stype = it.z >> 16;
+  const uint32_t depth = p.raw_items ? 0u : (it.w >> 16) & kJobDepthMask;
+  bool flat = valid && (it.w & 0xFFFFu) == kNone && perm < __ldg(&h->n_slots) && depth + 2 <= ZG_MAX_DEPTH;
+  DUnit u{};
+  if (flat) {
+    const DSlot s = ldg_rec(reinterpret_cast<const DSlot*>(p.prog + __ldg(&h->off_slots)) + perm);
+    flat = (s.flags & SF_FLAT) != 0;
+    if (flat) u = ldg_rec(reinterpret_cast<const DUnit*>(p.prog + __ldg(&h->off_units)) + s.unit);
+  }
+  // the closure index of a meet step (by value from the parameters: their address costs a local copy)
+  auto closure_of = [&](uint32_t tgc, uint32_t& nsubj, const unsigned long long*& hdr, const unsigned long long*& sig,
+                        uint32_t& sig_words, const unsigned long long*& tab) {
+#pragma unroll
+    for (int k = 0; k < kMaxClosure; ++k)
+      if (k < static_cast<int>(p.n_closure) && p.closure[k].tgc == tgc) {
+        nsubj = p.closure[k].nsubj;
+        hdr = p.closure[k].set_hdr;
+        sig = p.closure[k].sig;
+        sig_words = p.closure[k].sig_words;
+        tab = p.closure[k].set_tab;
+      }
+  };
+  for (int i = u.push_begin; flat && i < u.step_end; ++i) {
+    const DStep st = ldg_rec(steps + i);
+    uint32_t nsubj = 0, words = 0;
+    const unsigned long long *hdr = nullptr, *sig = nullptr, *tab = nullptr;
+    closure_of(st.tgc, nsubj, hdr, sig, words, tab);
+    flat = stype == st.tstype && sid < nsubj && hdr && sig;
+  }
+  // The residual pass's batch and sub-query counters, which it reads only after this grid has finished
+  // (cudaGridDependencySynchronize): cleared here instead of by a memset of their own.
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    *p.next = 0;
+    *p.subq_count = 0;
+  }
+  // the rest goes to check_kernel: one atomic per warp
+  const bool residual = valid && !flat;
+  const unsigned rm = __ballot_sync(kFull, residual);
+  if (rm) {
+    const int leader = __ffs(rm) - 1;
+    unsigned long long at = 0;
+    if (static_cast<int>(lane) == leader) {
+      at = atomicAdd(p.nq_dev, static_cast<unsigned long long>(__popc(rm)));
+      atomicAdd(p.nq_dev + 1, static_cast<unsigned long long>(__popc(rm)));
+    }
+    at = __shfl_sync(kFull, at, leader);
+    if (residual) p.idx[at + __popc(rm & ((1u << lane) - 1u))] = static_cast<uint32_t>(q);
+  }
+  WarpCtx<COUNT> c;  // (probe_step's byte count)
+  c.bytes = 0;
+  if (flat) {
+    if (COUNT) c.bytes += 17;
+    bool hit = false;
+    // direct and wildcard probes, in step order (visit's non-inverted branch: an SF_FLAT slot has no CF_INVERT probe)
+    for (int i = u.step_begin; i < u.push_begin && !hit; ++i) {
+      const DStep st = ldg_rec(steps + i);
+      if (stype != st.stype || (st.kind == ST_WILD && p.no_wildcards)) continue;
+      hit = probe_step(p, c, st, obj, sid, (st.flags & CF_EXPIRY) != 0);
+    }
+    // two-level meets: the range's offsets, the subject's table header and signature line are loaded together
+    for (int i = u.push_begin; !hit && i < u.step_end; ++i) {
+      const DStep st = ldg_rec(steps + i);
+      if (obj >= st.nres) continue;
+      uint32_t nsubj = 0, words = 0;
+      const unsigned long long *hdr = nullptr, *sig = nullptr, *tab = nullptr;
+      closure_of(st.tgc, nsubj, hdr, sig, words, tab);
+      const unsigned long long ridx = st.row_base + static_cast<unsigned long long>(obj) * st.ncls;
+      uint32_t lo = __ldg(p.row_ptr + ridx);
+      const uint32_t hi = __ldg(p.row_ptr + ridx + 1);
+      const unsigned long long hw = __ldg(hdr + sid);
+      const uint32_t lg = __ffs(words) - 1;
+      sig += static_cast<unsigned long long>(sid) << lg;
+#ifndef ZG_EMULATE
+      asm volatile("prefetch.global.L1 [%0];" ::"l"(sig));
+#endif
+      if (COUNT) c.bytes += 8;
+      if (hi <= lo) continue;
+      if (COUNT) c.bytes += 8;
+      const uint32_t nbk = static_cast<uint32_t>(hw >> 32) & 0xFFFFFFu, seed = static_cast<uint32_t>(hw >> 56);
+      tab += static_cast<uint32_t>(hw);
+      while (nbk && lo < hi && !hit) {  // sig_meet's rounds, whose early exit the byte model follows
+        uint32_t v[kSigTests];
+        const uint32_t n = min(hi - lo, kSigTests);
+        const unsigned m = sig_round<COUNT>(p.col, lo, n, sig, lg, v, c.bytes);
+        lo += n;
+        hit = table_round<COUNT>(tab, nbk, seed, m, v, c.bytes);
+      }
+      // check_kernel still reads (and counts) the offsets and header of the steps after the one that finds the check
+      if (COUNT && hit)
+        for (int j = i + 1; j < u.step_end; ++j) {
+          const DStep sj = ldg_rec(steps + j);
+          if (obj >= sj.nres) continue;
+          const unsigned long long rj = sj.row_base + static_cast<unsigned long long>(obj) * sj.ncls;
+          c.bytes += __ldg(p.row_ptr + rj + 1) > __ldg(p.row_ptr + rj) ? 16 : 8;
+        }
+    }
+    if (p.out) p.out[q] = p.final_codes ? (hit ? ZG_HAS_PERMISSION : ZG_NO_PERMISSION) : (hit ? kValT : 0);
+    if (p.val) p.val[q * p.L] = hit ? kValT : 0;
+  }
+  if (COUNT) {
+    unsigned long long b = c.bytes;
+#pragma unroll
+    for (int d = 16; d >= 1; d >>= 1) b += __shfl_xor_sync(kFull, b, d);
+    if (lane == 0 && b) atomicAdd(p.alg_bytes, b);
+  }
 }
 
 // ---- multi-pass runs: the boolean fold of a level whose queries raised sub-queries -------------

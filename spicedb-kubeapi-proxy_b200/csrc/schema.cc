@@ -808,4 +808,28 @@ int mark_rsetless_slots(std::vector<uint8_t>* blob, const std::vector<uint16_t>&
   return marked;
 }
 
+int mark_flat_slots(std::vector<uint8_t>* blob, const std::vector<uint16_t>& tabled_tgc) {
+  uint8_t* const b = blob->data();
+  const DHeader* h = reinterpret_cast<const DHeader*>(b);
+  DSlot* slots = reinterpret_cast<DSlot*>(b + h->off_slots);
+  const DUnit* units = reinterpret_cast<const DUnit*>(b + h->off_units);
+  const DStep* steps = reinterpret_cast<const DStep*>(b + h->off_steps);
+  const DTypeInv* type_inv = reinterpret_cast<const DTypeInv*>(b + h->off_type_inv);
+  int marked = 0;
+  for (uint32_t s = 0; s < h->n_slots; ++s) {
+    bool ok = slots[s].kind != SK_NONPURE && (slots[s].flags & SF_NO_RSET) && !tabled_tgc.empty();
+    if (ok) {
+      const DUnit& u = units[slots[s].unit];
+      const int npush = u.step_end - u.push_begin;
+      ok = npush >= 1 && npush <= kFlatSteps;
+      for (int i = u.push_begin; i < u.step_end && ok; ++i)
+        ok = std::find(tabled_tgc.begin(), tabled_tgc.end(), steps[i].tgc) != tabled_tgc.end() &&
+             type_inv[steps[i].tstype].end - type_inv[steps[i].tstype].begin <= kMaxInvClasses;
+    }
+    slots[s].flags = static_cast<uint16_t>(ok ? slots[s].flags | SF_FLAT : slots[s].flags & ~SF_FLAT);
+    marked += ok;
+  }
+  return marked;
+}
+
 }  // namespace zg

@@ -45,7 +45,12 @@ constexpr uint16_t kStepTargetL2 = 0x200;    // DStep.flags: the children's unit
 enum SlotFlags : uint16_t {
   SF_NO_RSET = 1,  // no step of a unit the slot evaluates at the root reads the subject's per-check membership set
                    // (set at publish once the closure indexes are built: mark_rsetless_slots)
+  SF_FLAT = 2,     // the slot's checks are answered by flat_check_kernel (kernels.cuh): SF_NO_RSET, a pure slot whose
+                   // push steps (1 .. kFlatSteps) all meet over closure indexes with signatures and set tables
+                   // (mark_flat_slots)
 };
+constexpr int kFlatSteps = 4;       // push steps of an SF_FLAT slot, at most
+constexpr int kMaxInvClasses = 11;  // invertible classes of a subject type the check kernel's admission takes
 struct DSlot {   // per slot (relation or permission)
   uint16_t kind;        // SlotKind
   uint16_t unit;        // SK_RELATION / SK_PURE: unit id ; SK_NONPURE: tree id
@@ -222,5 +227,11 @@ class Schema {
 // class (CF_INVERT) and every push step is a two-level step (kStepTargetL2) whose class has a closure index
 // (indexed_tgc lists the tgc of every pair built). Returns the number of slots marked.
 int mark_rsetless_slots(std::vector<uint8_t>* blob, const std::vector<uint16_t>& indexed_tgc);
+
+// Sets SF_FLAT (and clears it elsewhere) in a program blob whose SF_NO_RSET flags are marked, for every pure slot that
+// has SF_NO_RSET, between 1 and kFlatSteps push steps, every one of them over a pair in tabled_tgc (the tgc of every
+// pair built with signatures and set tables), and whose two-level steps' subject types have at most kMaxInvClasses
+// invertible classes. Pass an empty tabled_tgc to clear every flag. Returns the number of slots marked.
+int mark_flat_slots(std::vector<uint8_t>* blob, const std::vector<uint16_t>& tabled_tgc);
 
 }  // namespace zg
