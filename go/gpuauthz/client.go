@@ -33,6 +33,7 @@ import "C"
 
 import (
 	"context"
+	"encoding/base64"
 	"fmt"
 	"io"
 	"runtime"
@@ -266,6 +267,9 @@ func (c *Client) LookupResources(ctx context.Context, req *v1.LookupResourcesReq
 	if c.broken.Load() {
 		return nil, errBroken
 	}
+	if req.GetOptionalLimit() != 0 || req.GetOptionalCursor() != nil {
+		return c.lookupResourcesPaged(ctx, req)
+	}
 	var s cstrs
 	defer s.free()
 	subj := req.GetSubject()
@@ -302,10 +306,90 @@ func (c *Client) LookupResources(ctx context.Context, req *v1.LookupResourcesReq
 	}
 }
 
+// lookupResourcesPaged answers a LookupResources with OptionalLimit or OptionalCursor through
+// zg_lookup_resources_page_str: with a limit, one page of at most OptionalLimit resources after the cursor; with only
+// a cursor, every resource after it. Resources come in ascending interned id order (SpiceDB promises no order), each
+// with the AfterResultCursor that resumes after it. The cursor token is the base64 of the engine's 32 opaque bytes.
+func (c *Client) lookupResourcesPaged(ctx context.Context, req *v1.LookupResourcesRequest) (v1.PermissionsService_LookupResourcesClient, error) {
+	var s cstrs
+	defer s.free()
+	subj := req.GetSubject()
+	var cur *C.zg_read_cursor
+	if tok := req.GetOptionalCursor().GetToken(); tok != "" {
+		raw, err := base64.StdEncoding.DecodeString(tok)
+		if err != nil || len(raw) != C.ZG_READ_CURSOR_BYTES {
+			return nil, status.Errorf(codes.InvalidArgument, "lookup cursor: not a cursor of this engine")
+		}
+		cur = (*C.zg_read_cursor)(C.CBytes(raw))
+		defer C.free(unsafe.Pointer(cur))
+	}
+	limit := uint64(req.GetOptionalLimit())
+	page := limit
+	if page == 0 || page > 1<<16 { // no limit: pages of 1 000; a larger limit is cut into pages of 1 << 16
+		page = 1000
+		if limit != 0 {
+			page = 1 << 16
+		}
+	}
+	st := &sliceStream{ctx: ctx}
+	for capBytes := uint64(1 << 16); ; {
+		buf := C.malloc(C.size_t(capBytes))
+		curs := make([]C.zg_read_cursor, page+1)
+		var need C.size_t
+		var n C.uint64_t
+		var next C.zg_read_cursor
+		var more C.int32_t
+		big := false
+		err := call(func() C.int {
+			rc := C.zg_lookup_resources_page_str(c.engine, s.add(req.GetResourceObjectType()), s.add(req.GetPermission()),
+				s.add(subj.GetObject().GetObjectType()), s.add(subj.GetObject().GetObjectId()), s.add(subj.GetOptionalRelation()),
+				C.uint64_t(page), cur, (*C.char)(buf), C.size_t(capBytes), &need, &n, &curs[0], &next, &more)
+			big = rc == C.ZG_E2BIG
+			if big {
+				return 0
+			}
+			return rc
+		})
+		if err != nil || big {
+			C.free(buf)
+			if err != nil {
+				return nil, err
+			}
+			capBytes = uint64(need) + 16
+			continue
+		}
+		text := C.GoString((*C.char)(buf))
+		C.free(buf)
+		if text != "" {
+			for i, id := range strings.Split(strings.TrimSuffix(text, "\n"), "\n") {
+				st.ids = append(st.ids, id)
+				st.cursors = append(st.cursors, base64.StdEncoding.EncodeToString(C.GoBytes(unsafe.Pointer(&curs[i]), C.ZG_READ_CURSOR_BYTES)))
+			}
+		}
+		done := more == 0
+		if limit != 0 {
+			limit -= uint64(n)
+			done = done || limit == 0
+			if limit < page {
+				page = limit
+			}
+		}
+		if done {
+			return st, nil
+		}
+		if cur == nil {
+			cur = (*C.zg_read_cursor)(C.malloc(C.ZG_READ_CURSOR_BYTES))
+			defer C.free(unsafe.Pointer(cur))
+		}
+		*cur = next
+	}
+}
+
 type sliceStream struct {
-	ctx context.Context
-	ids []string
-	pos int
+	ctx     context.Context
+	ids     []string
+	cursors []string // AfterResultCursor tokens of a paged lookup (nil: unpaged)
+	pos     int
 }
 
 func (s *sliceStream) Recv() (*v1.LookupResourcesResponse, error) {
@@ -316,9 +400,13 @@ func (s *sliceStream) Recv() (*v1.LookupResourcesResponse, error) {
 		return nil, io.EOF
 	}
 	id := s.ids[s.pos]
+	r := &v1.LookupResourcesResponse{ResourceObjectId: id,
+		Permissionship: v1.LookupPermissionship_LOOKUP_PERMISSIONSHIP_HAS_PERMISSION}
+	if s.cursors != nil {
+		r.AfterResultCursor = &v1.Cursor{Token: s.cursors[s.pos]}
+	}
 	s.pos++
-	return &v1.LookupResourcesResponse{ResourceObjectId: id,
-		Permissionship: v1.LookupPermissionship_LOOKUP_PERMISSIONSHIP_HAS_PERMISSION}, nil
+	return r, nil
 }
 func (s *sliceStream) Header() (metadata.MD, error) { return nil, nil }
 func (s *sliceStream) Trailer() metadata.MD         { return nil }

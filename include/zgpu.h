@@ -411,6 +411,38 @@ int zg_lookup_resources(zg_engine *e, uint16_t res_type, uint16_t perm, uint16_t
 int zg_lookup_resources_str(zg_engine *e, const char *res_type, const char *perm,
                             const char *subj_type, const char *subj_id, const char *subj_rel,
                             char *buf, size_t cap, size_t *need, uint64_t *n_out);
+/* Pages of LookupResources (optional_limit, optional_cursor, after_result_cursor). The order is ascending interned
+ * resource id, the order zg_lookup_resources returns; it is not name order. A page is the first `limit` (>= 1, else
+ * ZG_EINVAL) ids of the unpaged answer that follow `after` (NULL: from the start).
+ *   - *more is 1 exactly when another answer follows the page. *next resumes after the page's last id (`after`
+ *     itself, or the start, when the page is empty); cursors[i] (NULL or *n_out entries) resumes after id i.
+ *   - The cursor is a zg_read_cursor under its own tag: it names the schema generation, the request (resource type,
+ *     permission, subject type and relation, the subject as given: its id, or its name in the string form) and the
+ *     last id. A read cursor, a cursor of another request or form, or one made before a schema load is ZG_EINVAL.
+ *   - Pending writes are published first; the page is evaluated at the engine's clock. A cursor names an id, not a
+ *     position: a resource that holds the permission for the whole paging appears exactly once, one that gains or
+ *     loses it between pages may appear or not.
+ *   - ZG_EDEPTH only when a candidate that cannot be decided lies after the cursor and at or before the page's
+ *     deciding answer (the (limit + 1)-th, or the end when fewer follow). Where zg_lookup_resources succeeds, every page
+ *     does; a page that ends before an undecidable resource succeeds where zg_lookup_resources fails. A sharded handle
+ *     fails a page whenever the whole lookup has an undecidable candidate.
+ *   - A replicated engine verifies only the candidates the page needs, in windows, on its first device. A sharded
+ *     handle with ZG_FLAG_HANDLE_LOOKUPS runs the whole lookup and cuts the page from it (identical pages and cursors).
+ *     Everything else is refused as zg_lookup_resources is (ZG_EINVAL; ZG_ECUDA on a host-only engine).
+ * The string form renders at most `limit` names. A never-written userset subject that names itself (Check says so)
+ * has no id: its name comes after every id, and its cursor is past the ids. ZG_E2BIG (*need = bytes incl. NUL, *n_out
+ * = lines) fills nothing else, so the caller's cursor still resumes where it did; the retry runs the page again. */
+int zg_lookup_resources_page(zg_engine *e, uint16_t res_type, uint16_t perm, uint16_t stype, uint32_t subj,
+                             uint16_t srel, uint64_t limit, const zg_read_cursor *after, uint32_t *ids /* limit */,
+                             uint64_t *n_out, zg_read_cursor *cursors, zg_read_cursor *next, int32_t *more);
+int zg_lookup_resources_page_str(zg_engine *e, const char *res_type, const char *perm, const char *subj_type,
+                                 const char *subj_id, const char *subj_rel, uint64_t limit,
+                                 const zg_read_cursor *after, char *buf, size_t cap, size_t *need, uint64_t *n_out,
+                                 zg_read_cursor *cursors, zg_read_cursor *next, int32_t *more);
+/* Cumulative counters of LookupResources pages (zg_stats keeps its layout): out[0] pages answered by windowed
+ * verification, out[1] pages cut from a whole answer (sharded handle), out[2] candidates after the cursor, out[3]
+ * candidates verified, out[4] verification windows launched. */
+int zg_lookup_page_counters(zg_engine *e, uint64_t *out);
 
 /* LookupSubjects: which subjects of type stype[#srel] have `perm` on object `res` (of perm's type).
  * Subjects granted through their own relationships are listed in ids (ascending). When a wildcard

@@ -17,6 +17,7 @@ OP_TOUCH, OP_CREATE, OP_DELETE = 0, 1, 2
 PRECOND_MUST_MATCH, PRECOND_MUST_NOT_MATCH = 1, 2
 E2BIG = -7
 READ_CURSOR_BYTES = 32  # sizeof(zg_read_cursor)
+MAX_LOOKUP_PAGE = 1 << 24  # ids of one lookup_resources_page: its buffers are allocated for the limit
 WILDCARDS_INCLUDE, WILDCARDS_EXCLUDE = 0, 1  # zg_lookup_subjects wildcard_option
 
 CHECK_DTYPE = np.dtype(
@@ -183,6 +184,13 @@ _SIGS = {
                                       C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),
     "zg_lookup_resources_str": (C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p,
                                           C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint64)]),
+    "zg_lookup_resources_page": (C.c_int, [C.c_void_p, C.c_uint16, C.c_uint16, C.c_uint16, C.c_uint32, C.c_uint16,
+                                           C.c_uint64, C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64), C.c_void_p,
+                                           C.c_void_p, C.POINTER(C.c_int32)]),
+    "zg_lookup_resources_page_str": (C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p,
+                                               C.c_uint64, C.c_void_p, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t),
+                                               C.POINTER(C.c_uint64), C.c_void_p, C.c_void_p, C.POINTER(C.c_int32)]),
+    "zg_lookup_page_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
     "zg_lookup_subjects": (C.c_int, [C.c_void_p, C.c_uint16, C.c_uint32, C.c_uint16, C.c_uint16, C.c_uint32, C.c_void_p,
                                      C.c_uint64, C.POINTER(C.c_uint64), C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64),
                                      C.POINTER(C.c_int32)]),
@@ -740,6 +748,62 @@ class Engine:
                 continue
             self._ck(rc)
             return [l for l in buf.value.decode().split("\n") if l]
+
+    def lookup_resources_page(self, res_type, perm, subj_type, subj, srel=None, limit: int = 1000,
+                              after: bytes | None = None):
+        """zg_lookup_resources_page -> (ids, cursors, next, more): the first `limit` ids (ascending) of the
+        LookupResources answer after the cursor `after` (None: from the start), the cursor after each id, the cursor
+        after the page and whether more follow. Cursors are opaque bytes."""
+        rt = self.type_id(res_type)
+        sr = SREL_NONE if srel is None else self.slot_id(subj_type, srel)
+        rows = min(int(limit), MAX_LOOKUP_PAGE)
+        a = None if after is None else C.create_string_buffer(bytes(after), READ_CURSOR_BYTES)
+        out = np.empty(rows, dtype=np.uint32)
+        curs, nxt = C.create_string_buffer(rows * READ_CURSOR_BYTES), C.create_string_buffer(READ_CURSOR_BYTES)
+        n, more = C.c_uint64(0), C.c_int32(0)
+        self._ck(self._L.zg_lookup_resources_page(self._h, rt, self.slot_id(res_type, perm), self.type_id(subj_type),
+                                                  int(subj), sr, rows, a, out.ctypes.data, C.byref(n), curs, nxt,
+                                                  C.byref(more)))
+        k, raw = n.value, curs.raw
+        return (out[:k].copy(), [raw[i * READ_CURSOR_BYTES:(i + 1) * READ_CURSOR_BYTES] for i in range(k)], nxt.raw,
+                bool(more.value))
+
+    def lookup_resources_page_str(self, res_type, perm, subj_type, subj_id, subj_rel="", limit: int = 1000,
+                                  after: bytes | None = None):
+        """zg_lookup_resources_page_str -> (names, cursors, next, more), as lookup_resources_page."""
+        rows = min(int(limit), MAX_LOOKUP_PAGE)
+        a = None if after is None else C.create_string_buffer(bytes(after), READ_CURSOR_BYTES)
+        cap = max(1 << 16, min(rows, 1 << 18) * 64)  # a name rarely takes more: no second run of the page
+        while True:
+            buf = C.create_string_buffer(cap)
+            curs, nxt = C.create_string_buffer(rows * READ_CURSOR_BYTES), C.create_string_buffer(READ_CURSOR_BYTES)
+            need, n, more = C.c_size_t(0), C.c_uint64(0), C.c_int32(0)
+            rc = self._L.zg_lookup_resources_page_str(self._h, _b(res_type), _b(perm), _b(subj_type), _b(subj_id),
+                                                      _b(subj_rel or ""), rows, a, buf, cap, C.byref(need),
+                                                      C.byref(n), curs, nxt, C.byref(more))
+            if rc == E2BIG:
+                cap = need.value + 16
+                continue
+            self._ck(rc)
+            k, raw = n.value, curs.raw
+            names = [l for l in buf.value.decode().split("\n") if l]
+            return names, [raw[i * READ_CURSOR_BYTES:(i + 1) * READ_CURSOR_BYTES] for i in range(k)], nxt.raw, bool(more.value)
+
+    def iter_lookup_resources(self, res_type, perm, subj_type, subj, srel=None, limit: int = 1000):
+        """Every id of the LookupResources answer, looked up page by page (`limit` per page), ascending."""
+        cursor = None
+        while True:
+            ids, _, cursor, more = self.lookup_resources_page(res_type, perm, subj_type, subj, srel, limit, cursor)
+            yield from (int(i) for i in ids)
+            if not more:
+                return
+
+    def lookup_page_counters(self) -> dict:
+        """zg_lookup_page_counters: pages answered by windowed verification / cut from a whole answer (sharded handle),
+        candidates after the cursor, candidates verified, verification windows."""
+        out = np.zeros(5, dtype=np.uint64)
+        self._ck(self._L.zg_lookup_page_counters(self._h, out.ctypes.data))
+        return dict(zip(("windowed_pages", "cut_pages", "after_cursor", "verified", "windows"), (int(x) for x in out)))
 
     def lookup_subjects_ids(self, res_type, res, perm, subj_type, srel=None, wildcards=WILDCARDS_INCLUDE, cap=1 << 14):
         """LookupSubjects by ids -> (ids ascending, wildcard: bool, excluded ids ascending)."""

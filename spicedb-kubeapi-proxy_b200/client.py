@@ -130,12 +130,15 @@ class LookupResourcesRequest:
     permission: str
     subject: SubjectReference
     fully_consistent: bool = True
+    optional_limit: int = 0  # 0: no limit
+    optional_cursor: Optional[bytes] = None  # an after_result_cursor of an earlier response
 
 
 @dataclass
 class LookupResourcesResponse:
     resource_object_id: str
     permissionship: int = LOOKUP_PERMISSIONSHIP_HAS_PERMISSION
+    after_result_cursor: Optional[bytes] = None  # set when the request had a limit or a cursor
 
 
 @dataclass
@@ -314,14 +317,24 @@ class PermissionsClient:
         return CheckPermissionResponse(pair.item.permissionship)
 
     def LookupResources(self, req: LookupResourcesRequest) -> Iterator[LookupResourcesResponse]:
-        """Slice-backed stand-in for the server stream (pkg/authz/lookups.go:74-88)."""
+        """Slice-backed stand-in for the server stream (pkg/authz/lookups.go:74-88). Without a limit or a cursor: the
+        unpaged answer. With a limit: one page of at most optional_limit resources after the cursor; with only a
+        cursor: every resource after it. Resources come in ascending interned id order, each with the cursor that
+        resumes after it."""
+        q = (req.resource_object_type, req.permission, req.subject.object.object_type, req.subject.object.object_id,
+             req.subject.optional_relation)
         try:
-            ids = self.engine.lookup_resources_str(req.resource_object_type, req.permission,
-                                                   req.subject.object.object_type, req.subject.object.object_id,
-                                                   req.subject.optional_relation)
+            if not req.optional_limit and req.optional_cursor is None:
+                return iter([LookupResourcesResponse(i) for i in self.engine.lookup_resources_str(*q)])
+            out, cursor = [], req.optional_cursor
+            while True:
+                names, curs, cursor, more = self.engine.lookup_resources_page_str(*q, limit=req.optional_limit or 1000,
+                                                                                  after=cursor)
+                out += [LookupResourcesResponse(n, after_result_cursor=c) for n, c in zip(names, curs)]
+                if not more or req.optional_limit:
+                    return iter(out)
         except ZgpuError as e:
             raise _rpc(e) from None
-        return iter([LookupResourcesResponse(i) for i in ids])
 
     def LookupSubjects(self, req: LookupSubjectsRequest) -> Iterator[LookupSubjectsResponse]:
         """Slice-backed stand-in for the server stream: the concrete subjects, then (when a wildcard grants the

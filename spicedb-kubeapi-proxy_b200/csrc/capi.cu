@@ -247,6 +247,9 @@ struct zg_engine {
   std::atomic<uint64_t> flt_device{0}, flt_host{0}, flt_returned{0}, flt_shape[3] = {};
   // zg_page_counters: pages served on the device / by the host store, entries the device windows covered, launches
   std::atomic<uint64_t> pg_device{0}, pg_host{0}, pg_scanned{0}, pg_launches{0};
+  // zg_lookup_page_counters: LookupResources pages answered by windowed verification / cut from a whole answer (a
+  // sharded handle), candidates after the cursor, candidates verified, verification windows
+  std::atomic<uint64_t> lp_windowed{0}, lp_cut{0}, lp_after{0}, lp_verified{0}, lp_windows{0};
   uint32_t schema_gen = 0;  // schema loads: a page cursor names the schema it was made under
   // zg_name_counters: names retired by zg_retire_unused_names calls that read the mentions from the snapshots / from
   // the host store (reset with the store by a schema load)
@@ -1257,6 +1260,11 @@ struct CursorBits {
 };
 static_assert(sizeof(CursorBits) == ZG_READ_CURSOR_BYTES, "zg_read_cursor is CursorBits");
 constexpr uint16_t kCursorVersion = 1;
+// LookupResources pages (zg_lookup_resources_page*) use the same bytes under their own version, so that a read cursor
+// and a lookup cursor are never taken for each other. key.type = the resource type, key.res = the last id returned;
+// has_key = kPastIds: after the ids, past a never-written userset subject's own name (the string form's last line).
+constexpr uint16_t kLookupCursorVersion = 0x8001;
+constexpr uint16_t kPastIds = 2;
 
 static uint64_t filter_fingerprint(const Store::Filter& f, const zg_filter_str& s) {
   uint64_t h = 0xcbf29ce484222325ull;
@@ -1273,10 +1281,12 @@ static uint64_t filter_fingerprint(const Store::Filter& f, const zg_filter_str& 
   return h;
 }
 
-static zg_read_cursor make_cursor(const zg_engine* e, uint64_t fp, const PageKey* key) {
+// version: kCursorVersion, or kLookupCursorVersion for a LookupResources page; has_key: what a non-null key holds
+static zg_read_cursor make_cursor(const zg_engine* e, uint64_t fp, const PageKey* key, uint16_t version = kCursorVersion,
+                                  uint16_t has_key = 1) {
   CursorBits c{};
-  c.version = kCursorVersion;
-  c.has_key = key != nullptr;
+  c.version = version;
+  c.has_key = key ? has_key : 0;
   c.schema_gen = e->schema_gen;
   c.fp = fp;
   if (key) c.key = *key;
@@ -2560,6 +2570,22 @@ static int run_sharded_lookup(zg_engine* e, const std::vector<Device::LookupReq>
   return ZG_OK;
 }
 
+// A never-written userset subject T:x#r of a lookup of type T (the subject id is the sentinel): still a member of
+// T:x#perm when r is perm itself or a relation inlined into its union. Check decides. Device lock held.
+static int never_written_self(zg_engine* e, uint16_t perm, uint16_t stype, uint16_t srel, bool* member, std::string* err) {
+  zg_check self{};
+  self.res = self.subj = ZG_NO_OBJECT;  // the same never-written object on both sides
+  self.perm = perm;
+  self.stype = stype;
+  self.srel = srel;
+  uint8_t code = 0;
+  PeerCounts pc;  // a handle checks the one item through its check protocol
+  const int rc = is_handle(e) ? run_sharded(e, &self, 1, &code, &pc, err) : e->dev.check_host(&self, 1, &code, err);
+  e->hl_round_trips += pc.round_trips;
+  if (!rc) *member = code == ZG_HAS_PERMISSION;
+  return rc;
+}
+
 // Answers a group of queued lookups under the engine lock: cache hits first, the rest in one batched launch
 // sequence, then the self-membership of userset subjects (Check is the arbiter of LookupResources).
 static void run_lookup_group(zg_engine* e, std::vector<zg_engine::LookupJob*>& group) {  // device lock held
@@ -2681,24 +2707,11 @@ static void run_lookup_group(zg_engine* e, std::vector<zg_engine::LookupJob*>& g
       j->rc = src->rc;
       j->err = src->err;
     }
-    // never-written userset subject T:x#r (subj is the sentinel): still a member of T:x#perm when r is perm
-    // itself or a relation inlined into its union
     if (!j->rc && j->want_self && j->key.srel != kNone && j->key.stype == j->key.res_type && j->key.subj >= ZG_NO_OBJECT - 1) {
-      zg_check self{};
-      self.res = self.subj = ZG_NO_OBJECT;  // the same never-written object on both sides
-      self.perm = j->key.perm;
-      self.stype = j->key.stype;
-      self.srel = j->key.srel;
-      uint8_t code = 0;
       std::string cerr;
-      PeerCounts pc;  // a handle checks the one item through its check protocol
-      int crc = handle ? run_sharded(e, &self, 1, &code, &pc, &cerr) : e->dev.check_host(&self, 1, &code, &cerr);
-      e->hl_round_trips += pc.round_trips;
-      if (crc) {
+      if (int crc = never_written_self(e, j->key.perm, j->key.stype, j->key.srel, &j->self_member, &cerr)) {
         j->rc = crc;
         j->err = cerr;
-      } else {
-        j->self_member = code == ZG_HAS_PERMISSION;
       }
     }
   }
@@ -2815,6 +2828,212 @@ extern "C" int zg_lookup_resources_str(zg_engine* e, const char* res_type, const
   return with_stable_names(e, [&] {
     return lookup_resources_str_once(e, res_type, perm, subj_type, subj_id, subj_rel, buf, cap, need, n_out);
   });
+}
+
+// ---- pages of LookupResources: zg_lookup_resources_page, zg_lookup_resources_page_str ----
+
+// The request a lookup cursor was made for: the resolved type, permission, subject type and subject relation ids, the
+// form, and the subject as given (its id in the id form, its name in the string form: a name need not exist).
+static uint64_t lookup_fingerprint(uint16_t rt, uint16_t perm, uint16_t st, uint16_t srel, const char* subj_name,
+                                   uint32_t subj) {
+  uint64_t h = 0xcbf29ce484222325ull;
+  auto mix = [&](const void* p, size_t n) {
+    for (size_t i = 0; i < n; ++i) h = (h ^ static_cast<const uint8_t*>(p)[i]) * 0x100000001b3ull;
+  };
+  mix("LookupResources", 15);
+  const uint16_t ids[5] = {rt, perm, st, srel, static_cast<uint16_t>(subj_name ? 1 : 0)};
+  mix(ids, sizeof ids);
+  if (subj_name) {
+    const size_t n = std::strlen(subj_name);
+    mix(&n, sizeof n);
+    mix(subj_name, n);
+  } else {
+    mix(&subj, sizeof subj);
+  }
+  return h;
+}
+
+// *after -> *c (zeroed when after is NULL: the start). ZG_EINVAL for a read cursor, a cursor of another request or
+// form, or one made before the schema was loaded again.
+static int lookup_cursor(const zg_engine* e, const zg_read_cursor* after, uint64_t fp, bool str_form, CursorBits* c) {
+  *c = CursorBits{};
+  if (!after) return ZG_OK;
+  std::memcpy(c, after->opaque, sizeof *c);
+  if (c->version != kLookupCursorVersion || c->has_key > (str_form ? kPastIds : 1))
+    return fail(ZG_EINVAL, "lookup cursor: not a LookupResources cursor of this engine");
+  if (c->schema_gen != e->schema_gen || c->fp != fp)
+    return fail(ZG_EINVAL, "lookup cursor: it was made for another lookup or under another schema");
+  return ZG_OK;
+}
+
+static zg_read_cursor lookup_cursor_at(const zg_engine* e, uint64_t fp, uint16_t rt, uint32_t id, uint16_t has_key = 1) {
+  const PageKey k{rt, id, 0, 0};
+  return make_cursor(e, fp, &k, kLookupCursorVersion, has_key);
+}
+
+// One page of LookupResources: the first `limit` ids of the unpaged answer after `after` (every id when !has_after) in
+// *ids, *more = 1 when another id follows. A replicated engine verifies windows of the candidates on its first device
+// (Device::lookup_page); a sharded handle runs its whole round and cuts the page from the answer. self_member (NULL:
+// not asked): whether the never-written userset subject is a member of itself, asked only once the ids ran out.
+static int lookup_page_ids(zg_engine* e, uint16_t rt, uint16_t perm, uint16_t st, uint32_t subj, uint16_t srel, uint64_t limit,
+                           bool has_after, uint32_t after, std::vector<uint32_t>* ids, bool* more, bool* self_member) {
+  if (int rc = refuse(e, Call::kLookup)) return rc;
+  LOCK_DEVICE(e);
+  if (e->dirty.load() || !e->dev.snap) {  // a handle's failed publish clears every shard's snapshot
+    LOCK_NAMES_UNIQUE(e);
+    if (int rc = publish_locked(e)) return rc;
+  }
+  const uint32_t now = now_of(e);
+  const uint64_t want = std::min<uint64_t>(limit, ZG_NO_OBJECT) + 1;  // no type holds more ids than that
+  zg_check proto{};
+  proto.subj = subj;
+  proto.perm = perm;
+  proto.stype = st;
+  proto.srel = srel;
+  std::string err;
+  if (is_handle(e)) {
+    for (uint32_t k = 0; k < e->n_shards; ++k) shard(e, k).now = now;
+    std::vector<std::vector<uint32_t>> all(1);
+    std::vector<int> rcs(1, ZG_OK);
+    if (int rc = run_sharded_lookup(e, {Device::LookupReq{rt, proto}}, 0, 1, &all, &rcs, &err)) return fail(rc, err);
+    if (rcs[0])  // the round reports an undecidable candidate per lookup, not per id: the page fails as the whole call
+      return fail(rcs[0], "LookupResources: a candidate could not be decided (max dispatch depth / work budget exceeded)");
+    const auto from = has_after ? std::upper_bound(all[0].begin(), all[0].end(), after) : all[0].begin();
+    const uint64_t left = static_cast<uint64_t>(all[0].end() - from);
+    ids->assign(from, from + static_cast<long>(std::min(left, want)));
+    ++e->lp_cut;
+    e->lp_after += left;
+  } else {
+    // the userset subject's own object is a candidate (the walk reaches it only through stored edges)
+    const uint32_t self = srel != kNone && st == rt && subj < ZG_NO_OBJECT - 1 ? subj : ZG_NO_OBJECT;
+    Device::LookupPageStats ps;
+    e->dev.now = now;
+    if (int rc = e->dev.lookup_page(rt, proto, has_after, after, want, self, ids, &ps, &err)) return fail(rc, err);
+    ++e->lp_windowed;
+    e->lp_after += ps.after;
+    e->lp_verified += ps.verified;
+    e->lp_windows += ps.windows;
+  }
+  *more = ids->size() > limit;
+  if (*more) ids->resize(limit);
+  if (self_member) {
+    *self_member = false;
+    if (!*more && srel != kNone && st == rt) {
+      if (int rc = never_written_self(e, perm, st, srel, self_member, &err)) return fail(rc, err);
+    }
+  }
+  return ZG_OK;
+}
+
+extern "C" int zg_lookup_resources_page(zg_engine* e, uint16_t res_type, uint16_t perm, uint16_t stype, uint32_t subj,
+                                        uint16_t srel, uint64_t limit, const zg_read_cursor* after, uint32_t* ids,
+                                        uint64_t* n_out, zg_read_cursor* cursors, zg_read_cursor* next, int32_t* more) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (!ids || !n_out) return fail(ZG_EINVAL, "NULL ids / n_out");
+  if (limit == 0) return fail(ZG_EINVAL, "page limit must be at least 1 (zg_lookup_resources looks up without one)");
+  const Schema& sc = e->schema;
+  if (res_type >= sc.types.size() || perm >= sc.slots.size() || sc.slots[perm].type != res_type)
+    return fail(ZG_EINVAL, "unknown resource type or permission");
+  if (stype >= sc.types.size() || (srel != kNone && (srel >= sc.slots.size() || sc.slots[srel].type != stype)))
+    return fail(ZG_EINVAL, "unknown subject type or relation");
+  const uint64_t fp = lookup_fingerprint(res_type, perm, stype, srel, nullptr, subj);
+  CursorBits c;
+  if (int rc = lookup_cursor(e, after, fp, false, &c)) return rc;
+  std::vector<uint32_t> got;
+  bool has_more = false;
+  if (int rc = lookup_page_ids(e, res_type, perm, stype, subj, srel, limit, c.has_key, c.key.res, &got, &has_more, nullptr))
+    return rc;
+  *n_out = got.size();
+  if (!got.empty()) std::memcpy(ids, got.data(), got.size() * 4);
+  if (cursors)
+    for (size_t i = 0; i < got.size(); ++i) cursors[i] = lookup_cursor_at(e, fp, res_type, got[i]);
+  if (next) *next = got.empty() ? (after ? *after : make_cursor(e, fp, nullptr, kLookupCursorVersion))
+                                : lookup_cursor_at(e, fp, res_type, got.back());
+  if (more) *more = has_more;
+  return ZG_OK;
+}
+
+static int lookup_page_str_once(zg_engine* e, const char* res_type, const char* perm, const char* subj_type,
+                                const char* subj_id, const char* subj_rel, uint64_t limit, const zg_read_cursor* after,
+                                char* buf, size_t cap, size_t* need, uint64_t* n_out, zg_read_cursor* cursors,
+                                zg_read_cursor* next, int32_t* more) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (!res_type || !perm || !subj_type || !subj_id) return fail(ZG_EINVAL, "NULL argument");
+  if (limit == 0) return fail(ZG_EINVAL, "page limit must be at least 1 (zg_lookup_resources_str looks up without one)");
+  int rt, p, st;
+  uint16_t sr;
+  uint32_t su;
+  if (int rc = resolve_lookup_strs(e, res_type, perm, subj_type, subj_id, subj_rel, &rt, &p, &st, &sr, &su)) return rc;
+  const uint64_t fp = lookup_fingerprint(static_cast<uint16_t>(rt), static_cast<uint16_t>(p), static_cast<uint16_t>(st), sr,
+                                         subj_id, 0);
+  CursorBits c;
+  if (int rc = lookup_cursor(e, after, fp, true, &c)) return rc;
+  std::vector<uint32_t> ids;
+  bool has_more = false, self_member = false;
+  if (c.has_key != kPastIds) {  // past the ids, the never-written subject's own name was the last line
+    const bool never_written = su == ZG_NO_OBJECT;
+    if (int rc = lookup_page_ids(e, static_cast<uint16_t>(rt), static_cast<uint16_t>(p), static_cast<uint16_t>(st),
+                                 never_written ? ZG_NO_OBJECT - 1 : su, sr, limit, c.has_key, c.key.res, &ids, &has_more,
+                                 never_written ? &self_member : nullptr))
+      return rc;
+  } else if (int rc = refuse(e, Call::kLookup)) {
+    return rc;
+  }
+  if (e->resolve_hook) e->resolve_hook(e->resolve_hook_arg);
+  // the never-written subject that names itself comes after every id
+  const bool self_line = self_member && ids.size() < limit;
+  if (self_member && !self_line) has_more = true;
+  std::vector<std::string> names;
+  {
+    LOCK_NAMES_SHARED(e);
+    for (uint32_t id : ids) {
+      std::string_view n;
+      names.push_back(e->store.name(rt, id, &n) ? std::string(n) : std::to_string(id));
+    }
+  }
+  if (self_line) names.push_back(subj_id);
+  size_t total = 1;
+  for (const auto& n : names) total += n.size() + 1;
+  if (need) *need = total;
+  if (n_out) *n_out = names.size();
+  if (total > cap || !buf) return ZG_E2BIG;
+  size_t w = 0;
+  for (const auto& n : names) {
+    std::memcpy(buf + w, n.data(), n.size());
+    w += n.size();
+    buf[w++] = '\n';
+  }
+  buf[w] = 0;
+  const uint16_t t = static_cast<uint16_t>(rt);
+  if (cursors) {
+    for (size_t i = 0; i < ids.size(); ++i) cursors[i] = lookup_cursor_at(e, fp, t, ids[i]);
+    if (self_line) cursors[ids.size()] = lookup_cursor_at(e, fp, t, 0, kPastIds);
+  }
+  if (next) {
+    if (self_line) *next = lookup_cursor_at(e, fp, t, 0, kPastIds);
+    else if (!ids.empty()) *next = lookup_cursor_at(e, fp, t, ids.back());
+    else *next = after ? *after : make_cursor(e, fp, nullptr, kLookupCursorVersion);
+  }
+  if (more) *more = has_more;
+  return ZG_OK;
+}
+
+extern "C" int zg_lookup_resources_page_str(zg_engine* e, const char* res_type, const char* perm, const char* subj_type,
+                                            const char* subj_id, const char* subj_rel, uint64_t limit,
+                                            const zg_read_cursor* after, char* buf, size_t cap, size_t* need,
+                                            uint64_t* n_out, zg_read_cursor* cursors, zg_read_cursor* next, int32_t* more) {
+  return with_stable_names(e, [&] {
+    return lookup_page_str_once(e, res_type, perm, subj_type, subj_id, subj_rel, limit, after, buf, cap, need, n_out,
+                                cursors, next, more);
+  });
+}
+
+extern "C" int zg_lookup_page_counters(zg_engine* e, uint64_t* out) {
+  if (!e || !out) return fail(ZG_EINVAL, "NULL argument");
+  const uint64_t c[5] = {e->lp_windowed.load(), e->lp_cut.load(), e->lp_after.load(), e->lp_verified.load(),
+                         e->lp_windows.load()};
+  std::memcpy(out, c, sizeof c);
+  return ZG_OK;
 }
 
 // ---- LookupSubjects --------------------------------------------------------------------------

@@ -131,6 +131,9 @@ std::string Device::init(int dev, uint64_t subq_cap, uint32_t budget) {
   if (const char* v = std::getenv("ZGPU_NO_INVERT")) invert = !(*v && *v != '0');
   if (const char* v = std::getenv("ZGPU_NO_RBFS")) use_rbfs = !(*v && *v != '0');
   if (const char* v = std::getenv("ZGPU_LOOKUP_BATCH_CAP")) lb_cap_ = std::max<uint64_t>(1024, std::strtoull(v, nullptr, 10));
+  if (const char* v = std::getenv("ZGPU_LOOKUP_PAGE_WINDOW")) lp_first_ = std::max<uint64_t>(1, std::strtoull(v, nullptr, 10));
+  if (const char* v = std::getenv("ZGPU_LOOKUP_PAGE_GROWTH"))
+    lp_growth_ = std::max<uint32_t>(2, static_cast<uint32_t>(std::strtoul(v, nullptr, 10)));
   if (const char* v = std::getenv("ZGPU_CLOSURE_CAP")) closure_cap_ = std::strtoull(v, nullptr, 10);  // tests: 0 = no index
   if (const char* v = std::getenv("ZGPU_CLOSURE_SIG_WORDS"))  // tests: 0 = no signatures, 1 = one word (most tests maybe)
     closure_sig_words_ = static_cast<uint32_t>(std::strtoul(v, nullptr, 10));
@@ -2246,6 +2249,184 @@ int Device::lookup(uint16_t res_type, const zg_check& proto, std::vector<uint32_
     ZG_CUDA(cudaMemcpyAsync(ids->data(), src, cnt * 4, cudaMemcpyDeviceToHost, stream));
     ZG_CUDA(cudaStreamSynchronize(stream));
     if (cnt <= 2048) std::sort(ids->begin(), ids->end());
+  }
+  return ZG_OK;
+}
+
+int Device::lookup_page(uint16_t res_type, const zg_check& proto, bool has_after, uint32_t after, uint64_t want, uint32_t self,
+                        std::vector<uint32_t>* ids, LookupPageStats* st, std::string* err) {
+  ids->clear();
+  *st = LookupPageStats{};
+  std::shared_ptr<Snapshot> s = snap;
+  if (!s) {
+    if (err) *err = "no snapshot published";
+    return ZG_ENOSNAPSHOT;
+  }
+  if (res_type >= s->resources.size()) {
+    if (err) *err = "unknown resource type";
+    return ZG_EINVAL;
+  }
+  if (want == 0) return ZG_OK;
+  ZG_CUDA(cudaSetDevice(device));
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  if (!lp_ctrl_.ensure(4 * 8)) {
+    if (err) *err = "out of device memory (lookup page)";
+    return ZG_ENOMEM;
+  }
+  unsigned long long* ctrl = lp_ctrl_.as<unsigned long long>();  // [0] selected / found, [1] self seen / error, [2] bound
+  unsigned long long h[3] = {0, 0, 0};
+  ZG_CUDA(cudaMemsetAsync(ctrl, 0, 4 * 8, stream));
+  // ---- the candidates: those of lookup()
+  const uint32_t* cand = nullptr;
+  uint64_t n = 0;
+  bool flat = false, sorted = false;
+  if (use_rbfs && proto.srel == kNone && proto.perm < s->flat_n.size() && s->flat_n[proto.perm] >= 0) {
+    const uint64_t cap = rb_cap_;
+    if (!rb_cand_.ensure(cap * 4 + 8)) return ZG_ENOMEM;
+    unsigned long long* d_count = rb_cand_.as<unsigned long long>();  // as in lookup(): [count u64][ids ...]
+    lookup_flat_kernel<<<1, 32, 0, stream>>>(s->rrow_ptr.as<uint32_t>(), s->rcol.as<uint32_t>(),
+                                             s->flat_cls[proto.perm].as<FlatLookupClass>(), s->flat_n[proto.perm], proto.stype,
+                                             proto.subj, rb_cand_.as<uint32_t>() + 2, cap, d_count);
+    ++launches;
+    unsigned long long cnt = 0;
+    ZG_CUDA(cudaMemcpyAsync(&cnt, d_count, 8, cudaMemcpyDeviceToHost, stream));
+    ZG_CUDA(cudaStreamSynchronize(stream));
+    if ((flat = cnt <= cap)) {  // more rows than the buffer: the general path
+      ++lookups_flat;
+      cand = rb_cand_.as<uint32_t>() + 2;
+      n = cnt;
+    }
+  }
+  if (!flat) {
+    if (s->resources_stale) {
+      std::string rerr = gpu_resource_lists(s.get(), stream);
+      if (!rerr.empty()) {
+        if (err) *err = rerr;
+        return ZG_ECUDA;
+      }
+    }
+    n = s->n_resources[res_type];
+    cand = s->resources[res_type].as<uint32_t>();
+    bool walked = false;
+    if (n == 0) {
+      // no resource of the type: only the self candidate, if any
+    } else if (use_rbfs && proto.stype < s->n_objects.size()) {
+      uint64_t nc = 0;
+      bool overflow = false;
+      if (int rc = lookup_candidates(*s, res_type, proto, &nc, &overflow, err)) return rc;
+      if ((walked = !overflow)) {
+        ++lookups_rbfs;
+        n = nc;
+        cand = rb_cand_.as<uint32_t>();
+      } else {
+        ++lookups_exhaustive;
+      }
+    } else {
+      ++lookups_exhaustive;
+    }
+    // the exhaustive list is ascending without repeats: the candidates after the cursor are a suffix of it
+    sorted = !walked && self == ZG_NO_OBJECT;
+  }
+  // ---- select: the candidates after the cursor, ascending
+  const uint32_t* sel = cand;
+  uint64_t m = n;
+  uint32_t quiet = ZG_NO_OBJECT;
+  const unsigned blk = 256;
+  if (sorted) {
+    if (has_after && n) {
+      lookup_bound_kernel<<<1, 1, 0, stream>>>(cand, n, after, ctrl + 2);
+      ++launches;
+      ZG_CUDA(cudaMemcpyAsync(h, ctrl, sizeof h, cudaMemcpyDeviceToHost, stream));
+      ZG_CUDA(cudaStreamSynchronize(stream));
+      sel = cand + h[2];
+      m = n - h[2];
+    }
+  } else {
+    const uint64_t n_sel = n + (self != ZG_NO_OBJECT ? 1 : 0);
+    if (!lp_sel_.ensure(n_sel * 4 + 4) || !lp_sorted_.ensure(n_sel * 4 + 4)) {
+      if (err) *err = "out of device memory (lookup page candidates)";
+      return ZG_ENOMEM;
+    }
+    if (n_sel) {
+      lookup_select_kernel<<<static_cast<unsigned>((n_sel + blk - 1) / blk), blk, 0, stream>>>(
+          cand, n, has_after ? 1u : 0u, after, self, lp_sel_.as<uint32_t>(), ctrl);
+      ++launches;
+    }
+    ZG_CUDA(cudaMemcpyAsync(h, ctrl, sizeof h, cudaMemcpyDeviceToHost, stream));
+    ZG_CUDA(cudaStreamSynchronize(stream));
+    m = h[0];
+    if (self != ZG_NO_OBJECT && !h[1]) quiet = self;
+    sel = lp_sel_.as<uint32_t>();
+    if (m > 1) {
+      std::string serr = sort_u32(lp_sel_.as<uint32_t>(), lp_sorted_.as<uint32_t>(), m, stream);
+      if (!serr.empty()) {
+        if (err) *err = serr;
+        return ZG_ECUDA;
+      }
+      sel = lp_sorted_.as<uint32_t>();
+    }
+  }
+  st->after = m;
+  if (m == 0) return ZG_OK;
+  if (!lp_out_.ensure(std::min(want, m) * 4)) {
+    if (err) *err = "out of device memory (lookup page answers)";
+    return ZG_ENOMEM;
+  }
+  ZG_CUDA(cudaMemsetAsync(ctrl, 0, 2 * 8, stream));
+  // ---- verify in windows from the front, in id order, until `want` answers are found
+  uint64_t found = 0;
+  if (flat) {  // every row entry is an answer: one scan takes the first `want` distinct ids
+    lookup_window_kernel<<<1, kWindowThreads, 0, stream>>>(sel, m, 0, nullptr, ZG_NO_OBJECT, want, lp_out_.as<uint32_t>(), ctrl);
+    ++launches;
+    ZG_CUDA(cudaMemcpyAsync(h, ctrl, 2 * 8, cudaMemcpyDeviceToHost, stream));
+    ZG_CUDA(cudaStreamSynchronize(stream));
+    found = h[0];
+  } else {
+    uint64_t pos = 0, w = std::max<uint64_t>(lp_first_, 2 * want);
+    for (;;) {
+      w = std::min(w, m - pos);
+      if (!lk_jobs_.ensure(w * sizeof(zg_check)) || !lk_codes_.ensure(w)) {
+        if (err) *err = "out of device memory (lookup page window)";
+        return ZG_ENOMEM;
+      }
+      lookup_fill_kernel<<<static_cast<unsigned>((w + blk - 1) / blk), blk, 0, stream>>>(sel + pos, w, proto, lk_jobs_.as<zg_check>());
+      ++launches;
+      if (int rc = check_device(lk_jobs_.as<zg_check>(), w, lk_codes_.as<uint8_t>(), stream, true, nullptr, err)) return rc;
+      lookup_window_kernel<<<1, kWindowThreads, 0, stream>>>(sel + pos, w, pos > 0 ? 1u : 0u, lk_codes_.as<uint8_t>(), quiet,
+                                                             want, lp_out_.as<uint32_t>(), ctrl);
+      ++launches;
+      uint32_t cflags = 0;
+      ZG_CUDA(cudaMemcpyAsync(h, ctrl, 2 * 8, cudaMemcpyDeviceToHost, stream));
+      ZG_CUDA(cudaMemcpyAsync(&cflags, ctrl_.as<unsigned long long>() + 3, 4, cudaMemcpyDeviceToHost, stream));
+      ZG_CUDA(cudaStreamSynchronize(stream));
+      ++st->windows;
+      st->verified += w;
+      if (cflags & 1u) {
+        if (err) *err = "expansion stack overflow (per-warp spill area exhausted)";
+        return ZG_ENOMEM;
+      }
+      if (h[1]) {  // as the unpaged call, but only for a candidate the page's answer depends on
+        if (err) *err = "LookupResources: a candidate could not be decided (max dispatch depth / work budget exceeded)";
+        return ZG_EDEPTH;
+      }
+      pos += w;
+      found = h[0];
+      if (found >= want || pos == m) break;
+      // the next window: `growth` times this one at least, and enough for the answers still missing at the density of
+      // answers seen so far (with a quarter to spare)
+      const uint64_t left = m - pos;
+      uint64_t next = std::min(left, w * lp_growth_);
+      if (found) {
+        const double est = static_cast<double>(want - found) * static_cast<double>(pos) / static_cast<double>(found) * 1.25;
+        next = est >= static_cast<double>(left) ? left : std::max(next, static_cast<uint64_t>(est) + 1);
+      }
+      w = next;
+    }
+  }
+  ids->resize(found);
+  if (found) {
+    ZG_CUDA(cudaMemcpyAsync(ids->data(), lp_out_.p, found * 4, cudaMemcpyDeviceToHost, stream));
+    ZG_CUDA(cudaStreamSynchronize(stream));
   }
   return ZG_OK;
 }

@@ -155,6 +155,19 @@ class Device {
   int lookup_batch(const std::vector<LookupReq>& reqs, std::vector<std::vector<uint32_t>>* ids, std::vector<int>* rcs,
                    std::string* err);
   uint64_t lookup_batches = 0, lookups_batched = 0;
+  // One page of LookupResources: the first `want` answers with id > after (every id when !has_after), ascending, in
+  // *ids. The candidates are those of lookup() (the reverse walk, the exhaustive list, the flat union), plus `self`
+  // (ZG_NO_OBJECT: none), the userset subject's own object. Those after the cursor are sorted once, then verified in
+  // windows from the front, each larger than the last, until `want` answers are found or the candidates run out.
+  // ZG_EDEPTH when a candidate at or before the last answer found (the end, when fewer than `want` follow) cannot be
+  // decided.
+  struct LookupPageStats {
+    uint64_t after = 0;     // candidates after the cursor (a repeat of the flat union counts per row)
+    uint64_t verified = 0;  // candidates run through the check kernel
+    uint64_t windows = 0;   // verification windows
+  };
+  int lookup_page(uint16_t res_type, const zg_check& proto, bool has_after, uint32_t after, uint64_t want, uint32_t self,
+                  std::vector<uint32_t>* ids, LookupPageStats* st, std::string* err);
   // LookupSubjects (T:res#perm, subjects of type stype[#srel]): forward walk from the resource (else every object of
   // stype when the walk overflows or use_rbfs is off), the wildcard probe, one verification launch, a second
   // one without wildcard relationships when the wildcard is granted, compaction, sort, one copy back. ids:
@@ -411,6 +424,9 @@ class Device {
   DevBuf stage_in_, stage_out_, lk_jobs_, lk_codes_, lk_ids_;
   DevBuf rb_visited_, rb_front_[2], rb_cand_;
   DevBuf lb_params_, lb_owner_, lb_ctrl_, lb_keys_[2];  // batched lookups
+  DevBuf lp_sel_, lp_sorted_, lp_out_, lp_ctrl_;        // lookup pages: selected and sorted candidates, answers, control
+  uint64_t lp_first_ = 1024;  // lookup pages: the first window's floor (ZGPU_LOOKUP_PAGE_WINDOW)
+  uint32_t lp_growth_ = 4;    // and the least factor a window grows by (ZGPU_LOOKUP_PAGE_GROWTH)
   DevBuf ls_jobs_, ls_codes_, ls_has_, ls_ids_, ls_ctrl_;   // LookupSubjects
   DevBuf flt_out_, flt_exp_, flt_ctrl_;                     // match_filter: records, expirations, the count
   DevBuf pg_count_, pg_off_, pg_tmp_, pg_seg_;              // page_filter: tile counts, offsets, scan space, segments

@@ -1999,6 +1999,98 @@ __global__ void lookup_compact_kernel(const uint32_t* cand, const uint8_t* codes
   }
 }
 
+// ---- pages of LookupResources (Device::lookup_page) -------------------------------------
+//
+// A page needs the answers in ascending id order after the cursor, up to the (limit + 1)-th one. The candidates after
+// the cursor are selected and sorted once; then windows of the sorted candidates, from the front, are verified and
+// scanned in order until limit + 1 answers are found or the candidates run out.
+
+// Candidates with id > after (every candidate when !has_after) -> out (unordered), plus `self` (ZG_NO_OBJECT: none),
+// the userset subject's own object, which the walk reaches only through stored edges. ctrl[0]: out's count; ctrl[1]
+// = 1 when `self` is among the n candidates themselves (then its check failing fails the page, as it fails the
+// unpaged call).
+__global__ void lookup_select_kernel(const uint32_t* cand, unsigned long long n, uint32_t has_after, uint32_t after,
+                                     uint32_t self, uint32_t* out, unsigned long long* ctrl) {
+  const unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x;
+  const bool in = i < n + (self != ZG_NO_OBJECT ? 1 : 0);
+  const uint32_t id = !in ? 0u : i < n ? cand[i] : self;
+  if (in && i < n && id == self) ctrl[1] = 1;
+  const bool keep = in && (!has_after || id > after);
+  const unsigned m = __ballot_sync(kFull, keep);
+  if (!m) return;
+  const unsigned lane = threadIdx.x & 31;
+  unsigned long long base = 0;
+  if (lane == 0) base = atomicAdd(ctrl, static_cast<unsigned long long>(__popc(m)));
+  base = __shfl_sync(kFull, base, 0);
+  if (keep) out[base + __popc(m & ((1u << lane) - 1u))] = id;
+}
+
+// *at = the first index of ids[0, n) (ascending) whose id > after: the exhaustive list needs no selection.
+__global__ void lookup_bound_kernel(const uint32_t* ids, unsigned long long n, uint32_t after, unsigned long long* at) {
+  unsigned long long lo = 0, hi = n;
+  while (lo < hi) {
+    const unsigned long long mid = (lo + hi) / 2;
+    if (ids[mid] <= after) lo = mid + 1;
+    else hi = mid;
+  }
+  *at = lo;
+}
+
+// One window ids[0, n) of the sorted candidates, in id order, with their codes (nullptr: every candidate is an answer,
+// the flat path). An id equal to its predecessor (ids[-1] too when has_prev) is a repeat and counts once. ctrl[0]
+// holds the answers found by the earlier windows; the window's answers take ranks from there, and those of rank <
+// want go to out[rank]. ctrl[1] = 1 when a candidate whose check ended in ZG_ITEM_ERROR lies at or before the answer
+// of rank want - 1 (anywhere in the window when the window does not reach that rank): that answer decides the page,
+// so an undecidable candidate before it fails the page. `quiet`: the self candidate when the walk did not reach it;
+// like the unpaged call, its failed check leaves it out without failing. One block scans tile after tile and stops
+// at the deciding answer.
+constexpr unsigned kWindowThreads = 1024;
+__global__ void __launch_bounds__(kWindowThreads) lookup_window_kernel(const uint32_t* ids, unsigned long long n,
+                                                                      uint32_t has_prev, const uint8_t* codes,
+                                                                      uint32_t quiet, unsigned long long want,
+                                                                      uint32_t* out, unsigned long long* ctrl) {
+  ZG_BLOCK_SHARED_U32(sh, 34);  // [0, 32) the warps' offsets in the tile, [32] the tile's answers, [33] the deciding thread
+  const unsigned t = threadIdx.x, lane = t & 31, wid = t >> 5;
+  unsigned long long found = ctrl[0];  // the same in every thread
+  for (unsigned long long base = 0; base < n; base += kWindowThreads) {
+    const unsigned long long i = base + t;
+    bool has = false, bad = false;
+    uint32_t id = 0;
+    if (i < n) {
+      id = ids[i];
+      const bool dup = i > 0 ? ids[i - 1] == id : has_prev && ids[-1] == id;
+      const uint8_t c = codes ? codes[i] : static_cast<uint8_t>(ZG_HAS_PERMISSION);
+      has = !dup && c == ZG_HAS_PERMISSION;
+      bad = !dup && c == ZG_ITEM_ERROR && id != quiet;
+    }
+    const unsigned m = __ballot_sync(kFull, has);
+    if (lane == 0) sh[wid] = __popc(m);
+    __syncthreads();
+    if (wid == 0) {  // exclusive prefix of the warps' counts, the tile's total, no deciding thread yet
+      const unsigned v = sh[lane];
+      unsigned x = v;
+      for (unsigned d = 1; d < 32; d <<= 1) {
+        const unsigned y = __shfl_up_sync(kFull, x, d);
+        if (lane >= d) x += y;
+      }
+      sh[lane] = x - v;
+      if (lane == 31) {
+        sh[32] = x;
+        sh[33] = ~0u;
+      }
+    }
+    __syncthreads();
+    const unsigned long long rank = found + sh[wid] + __popc(m & ((1u << lane) - 1u));
+    if (has && rank < want) out[rank] = id;
+    if (has && rank == want - 1) sh[33] = t;
+    __syncthreads();
+    if (bad && t <= sh[33]) ctrl[1] = 1;
+    found += sh[32];
+    if (found >= want) break;  // uniform: the page is decided in this tile
+  }
+  if (t == 0) ctrl[0] = found < want ? found : want;
+}
+
 // ---- LookupResources on the object-hash sharded store (dist.DeviceShardedLookup) ------------------------------
 //
 // Shard k holds the reverse rows of the relationships whose resource it owns, so every object it discovers with
