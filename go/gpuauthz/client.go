@@ -586,6 +586,102 @@ func (c *Client) CollectExpired(before time.Time) (uint64, error) {
 	return uint64(n), nil
 }
 
+// ImportBulkRelationships: the stream is buffered, forwarded to SpiceDB when the caller closes it, and on success
+// imported into the mirror in one zg_import_relationships call (one group per class, packed ids: no C string per
+// relationship). A mirror failure resyncs, as WriteRelationships does.
+func (c *Client) ImportBulkRelationships(ctx context.Context, opts ...grpc.CallOption) (grpc.ClientStreamingClient[v1.ImportBulkRelationshipsRequest, v1.ImportBulkRelationshipsResponse], error) {
+	inner, err := c.PermissionsServiceClient.ImportBulkRelationships(ctx, opts...)
+	if err != nil {
+		return nil, err
+	}
+	return &importStream{ClientStreamingClient: inner, c: c, ctx: ctx}, nil
+}
+
+type importStream struct {
+	grpc.ClientStreamingClient[v1.ImportBulkRelationshipsRequest, v1.ImportBulkRelationshipsResponse]
+	c    *Client
+	ctx  context.Context
+	rels []*v1.Relationship
+}
+
+func (s *importStream) Send(req *v1.ImportBulkRelationshipsRequest) error {
+	s.rels = append(s.rels, req.GetRelationships()...)
+	return s.ClientStreamingClient.Send(req)
+}
+
+func (s *importStream) CloseAndRecv() (*v1.ImportBulkRelationshipsResponse, error) {
+	s.c.mu.Lock()
+	defer s.c.mu.Unlock()
+	resp, err := s.ClientStreamingClient.CloseAndRecv()
+	if err != nil {
+		return nil, err
+	}
+	if err := s.c.importMirror(s.rels); err != nil {
+		if rerr := s.c.resync(s.ctx); rerr != nil {
+			s.c.broken.Store(true)
+			return nil, status.Errorf(codes.Internal, "gpu mirror failed (%v) and resync failed: %v", err, rerr)
+		}
+	}
+	return resp, nil
+}
+
+// importMirror groups the relationships by class (first appearance of the class, then stream order) and imports them.
+func (c *Client) importMirror(rels []*v1.Relationship) error {
+	type group struct {
+		rt, rel, st, srel string
+		res, subj          []byte
+		roff, soff         []C.uint32_t
+		exp                []C.uint32_t
+		expiring           bool
+	}
+	var order []*group
+	byClass := map[[4]string]*group{}
+	for _, r := range rels {
+		k := [4]string{r.GetResource().GetObjectType(), r.GetRelation(), r.GetSubject().GetObject().GetObjectType(),
+			r.GetSubject().GetOptionalRelation()}
+		g := byClass[k]
+		if g == nil {
+			g = &group{rt: k[0], rel: k[1], st: k[2], srel: k[3], roff: []C.uint32_t{0}, soff: []C.uint32_t{0}}
+			byClass[k] = g
+			order = append(order, g)
+		}
+		g.res = append(g.res, r.GetResource().GetObjectId()...)
+		g.subj = append(g.subj, r.GetSubject().GetObject().GetObjectId()...)
+		g.roff = append(g.roff, C.uint32_t(len(g.res)))
+		g.soff = append(g.soff, C.uint32_t(len(g.subj)))
+		var e C.uint32_t
+		if ts := r.GetOptionalExpiresAt(); ts != nil {
+			e = C.uint32_t(ts.GetSeconds())
+			g.expiring = true
+		}
+		g.exp = append(g.exp, e)
+	}
+	if len(order) == 0 {
+		return nil
+	}
+	var s cstrs
+	defer s.free()
+	arr := (*C.zg_import_group)(C.calloc(C.size_t(len(order)), C.size_t(unsafe.Sizeof(C.zg_import_group{}))))
+	defer C.free(unsafe.Pointer(arr))
+	gs := unsafe.Slice(arr, len(order))
+	for i, g := range order {
+		gs[i].res_type, gs[i].relation, gs[i].subj_type, gs[i].subj_rel = s.add(g.rt), s.add(g.rel), s.add(g.st), s.add(g.srel)
+		gs[i].res_ids = (*C.char)(C.CBytes(append(g.res, 0)))
+		gs[i].subj_ids = (*C.char)(C.CBytes(append(g.subj, 0)))
+		gs[i].res_off = (*C.uint32_t)(C.CBytes(unsafe.Slice((*byte)(unsafe.Pointer(&g.roff[0])), len(g.roff)*4)))
+		gs[i].subj_off = (*C.uint32_t)(C.CBytes(unsafe.Slice((*byte)(unsafe.Pointer(&g.soff[0])), len(g.soff)*4)))
+		s.p = append(s.p, unsafe.Pointer(gs[i].res_ids), unsafe.Pointer(gs[i].subj_ids), unsafe.Pointer(gs[i].res_off),
+			unsafe.Pointer(gs[i].subj_off))
+		if g.expiring {
+			gs[i].expires_at = (*C.uint32_t)(C.CBytes(unsafe.Slice((*byte)(unsafe.Pointer(&g.exp[0])), len(g.exp)*4)))
+			s.p = append(s.p, unsafe.Pointer(gs[i].expires_at))
+		}
+		gs[i].n = C.uint64_t(len(g.exp))
+	}
+	var n C.uint64_t
+	return call(func() C.int { return C.zg_import_relationships(c.engine, arr, C.uint64_t(len(order)), &n) })
+}
+
 // RetireUnusedNames frees the interned names that no relationship of the mirror and no retained watch change mentions
 // any more, and returns how many; later names reuse their ids, so the id space stays flat under the proxy's churn.
 // The shim passes only strings and holds no ids, so nothing it caches goes stale. Run it right after CollectExpired.

@@ -247,6 +247,41 @@ void zg_set_clock(zg_engine *e, int64_t unix_seconds);
  * write is visible to every check that starts after return (FullyConsistent). */
 int zg_write_relationships(zg_engine *e, const zg_update_str *updates, uint64_t n,
                            const zg_precondition_str *pre, uint64_t n_pre);
+/* v1 ImportBulkRelationships: every relationship is a CREATE, and the call is all-or-nothing. Relationships come
+ * in groups of one class, packed as zg_check_bulk_packed takes them. */
+typedef struct {
+  const char *res_type, *relation, *subj_type, *subj_rel; /* one class; subj_rel NULL or "" = none */
+  const char *res_ids;                                    /* blob of resource ids */
+  const uint32_t *res_off;                                /* n + 1 offsets into res_ids */
+  const char *subj_ids;                                   /* blob of subject ids; "*" = the wildcard subject */
+  const uint32_t *subj_off;                               /* n + 1 offsets into subj_ids */
+  const uint32_t *expires_at;                             /* n, or NULL; 0 = no expiration */
+  uint64_t n;
+} zg_import_group;
+/* Imports the groups' relationships in call order (groups in order, items in order) and publishes once.
+ *   - Each relationship gets the checks zg_write_relationships makes of a CREATE. One that is already stored (an
+ *     expired one not yet collected included), or that appears earlier in the call, fails with ZG_EEXIST. The error
+ *     is that of the first failing relationship in call order: the code and message the write path gives for it,
+ *     prefixed "relationship <call position> (<text>): ". On failure nothing changes: no name is interned, nothing
+ *     is stored, the revision does not move and the watch feed gets no entry.
+ *   - New names get the ids the same relationships would get written in the same order through
+ *     zg_write_relationships: first appearance, the subject's name before the resource's; freed ids lowest first.
+ *   - Pending changes are published with the import; the revision advances by one. Every relationship is recorded in
+ *     the watch feed as a CREATE; an import larger than the feed holds clears it, and the feed restarts at the new
+ *     revision as after zg_clear_relationships.
+ *   - Names are resolved and interned, and duplicates found, on the GPU (the environment variable
+ *     ZGPU_IMPORT_HOST=1 selects the host path); host-only engines run the host path. A sharded handle imports into
+ *     its one store and rebuilds every shard. ZG_EINVAL on a standalone shard (zg_config.shard_count > 1): it cannot
+ *     see the other shards' relationships.
+ *   - At most 2^30 relationships per call (ZG_EINVAL above). The device scratch is freed when the call returns.
+ *   - Takes the device lock, then the names lock exclusively, as a write does. *n_imported may be NULL. */
+int zg_import_relationships(zg_engine *e, const zg_import_group *groups, uint64_t n_groups, uint64_t *n_imported);
+/* out[0..4] = successful imports run on the device, on the host, relationships imported, name occurrences found
+ * already interned, names interned new. */
+int zg_import_counters(zg_engine *e, uint64_t *out);
+/* The last successful import's steps, in milliseconds: ms[0..6] = names, sort and duplicates (device events; 0 on
+ * the host path), the host's checks and interning, the store and its index, the publish, the whole call. */
+int zg_import_last_times(zg_engine *e, double *ms);
 /* v1 DeleteRelationships by filter; *n_deleted may be NULL. */
 int zg_delete_relationships(zg_engine *e, const zg_filter_str *filter,
                             const zg_precondition_str *pre, uint64_t n_pre, uint64_t *n_deleted);

@@ -52,6 +52,12 @@ class _Precond(C.Structure):
     _fields_ = [("op", C.c_uint32), ("filter", _RelStr)]
 
 
+class _ImportGroup(C.Structure):
+    _fields_ = [("res_type", C.c_char_p), ("relation", C.c_char_p), ("subj_type", C.c_char_p), ("subj_rel", C.c_char_p),
+                ("res_ids", C.c_char_p), ("res_off", C.c_void_p), ("subj_ids", C.c_char_p), ("subj_off", C.c_void_p),
+                ("expires_at", C.c_void_p), ("n", C.c_uint64)]
+
+
 class _ListTemplate(C.Structure):
     _fields_ = [(k, C.c_char_p) for k in ("res_type", "permission", "subj_type", "subj_id", "subj_rel", "req_name",
                                           "req_namespace")] + [("id_kind", C.c_uint32), ("flags", C.c_uint32)]
@@ -157,6 +163,9 @@ _SIGS = {
     "zg_num_tuples": (C.c_uint64, [C.c_void_p]),
     "zg_set_clock": (None, [C.c_void_p, C.c_int64]),
     "zg_write_relationships": (C.c_int, [C.c_void_p, C.POINTER(_UpdateStr), C.c_uint64, C.POINTER(_Precond), C.c_uint64]),
+    "zg_import_relationships": (C.c_int, [C.c_void_p, C.POINTER(_ImportGroup), C.c_uint64, C.POINTER(C.c_uint64)]),
+    "zg_import_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "zg_import_last_times": (C.c_int, [C.c_void_p, C.c_void_p]),
     "zg_delete_relationships": (C.c_int, [C.c_void_p, C.POINTER(_RelStr), C.POINTER(_Precond), C.c_uint64,
                                           C.POINTER(C.c_uint64)]),
     "zg_collect_expired": (C.c_int, [C.c_void_p, C.c_int64, C.POINTER(C.c_uint64)]),
@@ -471,6 +480,58 @@ class Engine:
         for i, (op, f) in enumerate(preconditions):
             pre[i] = _Precond(int(op), self._filter(f))
         self._ck(self._L.zg_write_relationships(self._h, arr, n, pre, len(preconditions)))
+
+    def import_relationships(self, groups) -> int:
+        """zg_import_relationships: ImportBulkRelationships, all-or-nothing, published once. groups: iterable of
+        (res_type, relation, subj_type, subj_rel, res_ids, subj_ids, expires) with res_ids / subj_ids lists of ids
+        (str or bytes; "*" = the wildcard subject) and expires None or a list of unix seconds (0 = none). Returns how
+        many relationships were imported."""
+        groups = list(groups)
+        arr = (_ImportGroup * max(len(groups), 1))()
+        keep = []  # buffers must outlive the call
+        for i, (rt, rel, st, srel, res_ids, subj_ids, expires) in enumerate(groups):
+            rblob, roff = self.pack_ids(res_ids)
+            sblob, soff = self.pack_ids(subj_ids)
+            if len(res_ids) != len(subj_ids):
+                raise ValueError("res_ids and subj_ids differ in length")
+            ex = None if expires is None else np.ascontiguousarray(expires, dtype=np.uint32)
+            if ex is not None and ex.size != len(res_ids):
+                raise ValueError("expires and res_ids differ in length")
+            rblob, sblob = rblob or b"\0", sblob or b"\0"
+            parts = (_b(rt), _b(rel), _b(st), _b(srel or ""), rblob, sblob)
+            keep.append((parts, roff, soff, ex))
+            arr[i] = _ImportGroup(parts[0], parts[1], parts[2], parts[3], rblob, roff.ctypes.data, sblob, soff.ctypes.data,
+                                  None if ex is None else ex.ctypes.data, len(res_ids))
+        n = C.c_uint64(0)
+        self._ck(self._L.zg_import_relationships(self._h, arr, len(groups), C.byref(n)))
+        return n.value
+
+    @staticmethod
+    def import_groups(rels):
+        """[(relationship text 'type:id#rel@stype:sid[#srel]', expires_at)] -> import_relationships groups: one group
+        per class in order of first appearance, items in the order given within a group. The call order of the import
+        is that of the groups, so it equals the given order when each class's relationships are contiguous."""
+        groups = {}
+        for rel, exp in rels:
+            rt, rid, r, st, sid, srel = split_rel(rel)
+            g = groups.setdefault((rt, r, st, srel), ([], [], []))
+            g[0].append(rid)
+            g[1].append(sid)
+            g[2].append(int(exp))
+        return [(rt, r, st, srel, res, subj, ex if any(ex) else None) for (rt, r, st, srel), (res, subj, ex) in groups.items()]
+
+    def import_counters(self) -> dict:
+        """zg_import_counters: successful imports on the device / on the host, relationships imported, name
+        occurrences the store had, names interned new."""
+        out = np.zeros(5, dtype=np.uint64)
+        self._ck(self._L.zg_import_counters(self._h, out.ctypes.data))
+        return dict(zip(("device", "host", "relationships", "names_found", "names_new"), (int(x) for x in out)))
+
+    def import_last_times(self) -> dict:
+        """zg_import_last_times: the last successful import's steps in milliseconds."""
+        out = np.zeros(7, dtype=np.float64)
+        self._ck(self._L.zg_import_last_times(self._h, out.ctypes.data))
+        return dict(zip(("names", "sort", "duplicates", "host", "index", "build", "total"), (float(x) for x in out)))
 
     @staticmethod
     def _filter(f):

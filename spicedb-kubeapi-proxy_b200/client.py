@@ -22,7 +22,7 @@ Go toolchain, this Python class drives the identical C ABI.
 from __future__ import annotations
 
 from dataclasses import dataclass, field
-from typing import Iterator, List, Optional
+from typing import Iterable, Iterator, List, Optional
 
 from . import _lib
 from ._lib import Engine, ZgpuError
@@ -257,6 +257,16 @@ class ExportBulkRelationshipsResponse:
 
 
 @dataclass
+class ImportBulkRelationshipsRequest:
+    relationships: List[Relationship]
+
+
+@dataclass
+class ImportBulkRelationshipsResponse:
+    num_loaded: int
+
+
+@dataclass
 class WatchRequest:
     optional_object_types: List[str] = field(default_factory=list)
     optional_start_cursor: Optional[int] = None  # revision; None = changes after the call (watch.go:29-31)
@@ -416,6 +426,18 @@ class PermissionsClient:
                     return iter(out)
         except ZgpuError as e:
             raise _rpc(e) from None
+
+    def ImportBulkRelationships(self, requests: Iterable[ImportBulkRelationshipsRequest]) -> ImportBulkRelationshipsResponse:
+        """The client stream of ImportBulkRelationships: every request's relationships are CREATEs of one transaction,
+        imported all-or-nothing and published once. They are grouped by class (first appearance of the class, then
+        the order given), and new names get their ids in that order. The `relationship <i>` of an error message counts
+        in that grouped order too; it equals the stream's order when each class's relationships arrive together."""
+        rels = [(r.text(), r.optional_expires_at) for req in requests for r in req.relationships]
+        try:
+            n = self.engine.import_relationships(self.engine.import_groups(rels))
+        except ZgpuError as e:
+            raise _rpc(e) from None
+        return ImportBulkRelationshipsResponse(n)
 
 
 _WATCH_OP = {"TOUCH": OPERATION_TOUCH, "CREATE": OPERATION_CREATE, "DELETE": OPERATION_DELETE}

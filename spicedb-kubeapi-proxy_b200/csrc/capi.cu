@@ -1,6 +1,7 @@
 // capi.cu -- the C ABI declared in include/zgpu.h. Thin glue: argument checks,
 // string <-> id resolution, locking; the work is in store.cc and device.cu.
 #include <algorithm>
+#include <chrono>
 #include <condition_variable>
 #include <cctype>
 #include <cstdio>
@@ -17,6 +18,8 @@
 #include <string>
 #include <string_view>
 #include <thread>
+#include <unordered_map>
+#include <unordered_set>
 #include <vector>
 
 #include "../../include/zgpu.h"
@@ -261,6 +264,10 @@ struct zg_engine {
   // (tests force a retirement and a reuse of the ids into that gap with it); nullptr = none
   void (*resolve_hook)(void*) = nullptr;
   void* resolve_hook_arg = nullptr;
+  // zg_import_counters: successful imports on the device / on the host, relationships imported, name occurrences the
+  // store had, names interned new; zg_import_last_times: the last successful import's steps, in milliseconds
+  uint64_t imp_device = 0, imp_host = 0, imp_rels = 0, imp_found = 0, imp_new = 0;
+  double imp_ms[7] = {};
   ~zg_engine() {
     if (group_pin) cudaFreeHost(group_pin);
   }
@@ -283,6 +290,21 @@ struct zg_engine {
       watch_log.pop_front();
     }
     // a revision is dropped whole: a reader never sees part of a write
+    while (!watch_log.empty() && watch_log.front().revision <= watch_floor) watch_log.pop_front();
+  }
+  // An import: every relationship a CREATE. One larger than the feed holds cannot be read change by change: readers
+  // restart from its revision, as after zg_clear_relationships.
+  void log_import(const std::vector<zg_tuple>& t, const std::vector<uint32_t>& ex) {
+    if (t.size() > kWatchCap) {
+      watch_log.clear();
+      watch_floor = revision;
+      return;
+    }
+    for (size_t i = 0; i < t.size(); ++i) watch_log.push_back(WatchEntry{revision, t[i], ex[i], ZG_OP_CREATE});
+    while (watch_log.size() > kWatchCap) {
+      watch_floor = watch_log.front().revision;
+      watch_log.pop_front();
+    }
     while (!watch_log.empty() && watch_log.front().revision <= watch_floor) watch_log.pop_front();
   }
 };
@@ -758,8 +780,7 @@ static std::string rel_text(const zg_rel_str& r) {
 }
 
 // SpiceDB object-id validation (v1 API): 1..1024 characters of [a-zA-Z0-9/_|\-=+], or "*".
-static bool valid_object_id(const char* id) {
-  size_t n = std::strlen(id);
+static bool valid_object_id(const char* id, size_t n) {
   if (n == 0 || n > 1024) return false;
   if (n == 1 && id[0] == '*') return true;
   for (size_t i = 0; i < n; ++i) {
@@ -768,6 +789,7 @@ static bool valid_object_id(const char* id) {
   }
   return true;
 }
+static bool valid_object_id(const char* id) { return valid_object_id(id, std::strlen(id)); }
 
 // Resolve a relationship to WRITE (interns objects). Returns "" or an error.
 static std::string resolve_write(zg_engine* e, const zg_rel_str& r, zg_tuple* t) {
@@ -1031,6 +1053,360 @@ extern "C" int zg_write_relationships(zg_engine* e, const zg_update_str* ups, ui
   rc = publish_locked(e);
   if (rc == ZG_OK) e->log_changes(u, changed);
   return rc;
+}
+
+// ---- ImportBulkRelationships ------------------------------------------------------------------------
+
+static constexpr uint64_t kMaxImport = 1ull << 30;  // relationships in one call
+
+// One group's literal fields, resolved once, and what the write path would say of its items by their kind (wildcard
+// subject or not, expiring or not).
+struct ImportLit {
+  int rt = -1, st = -1, rel = -1;
+  uint16_t srel = kNone;        // of a non-wildcard subject
+  bool has_srel = false;        // the group names a subject relation
+  std::string lit_err;          // every item fails with it before its ids are looked at
+  std::string srel_err;         // the subject relation does not exist: every non-wildcard item fails with it
+  std::string val_err[2][2];    // Store::validate of an item [wildcard][expiring]
+  bool all_ok = false;          // no item kind fails: only the ids can
+};
+
+static ImportLit import_literals(const zg_engine* e, const zg_import_group& g) {
+  const Schema& sc = e->schema;
+  ImportLit l;
+  if (!g.res_type || !g.relation || !g.subj_type) {
+    l.lit_err = "relationship has NULL fields";
+    return l;
+  }
+  l.rt = sc.type_id(g.res_type);
+  l.st = sc.type_id(g.subj_type);
+  if (l.rt < 0) l.lit_err = std::string("object definition `") + g.res_type + "` not found";
+  else if (l.st < 0) l.lit_err = std::string("object definition `") + g.subj_type + "` not found";
+  if (!l.lit_err.empty()) return l;
+  l.rel = sc.slot_id(l.rt, g.relation);
+  if (l.rel < 0 || sc.slots[l.rel].is_perm) {
+    l.lit_err = std::string("relation `") + g.relation + "` not found under definition `" + g.res_type + "`";
+    return l;
+  }
+  l.has_srel = !none_rel(g.subj_rel);
+  if (l.has_srel) {
+    const int sr = sc.slot_id(l.st, g.subj_rel);
+    if (sr < 0) l.srel_err = std::string("relation `") + g.subj_rel + "` not found under definition `" + g.subj_type + "`";
+    else l.srel = static_cast<uint16_t>(sr);
+  }
+  l.all_ok = true;
+  for (int w = 0; w < 2; ++w)
+    for (int x = 0; x < 2; ++x) {
+      zg_tuple t{};
+      t.rel = static_cast<uint16_t>(l.rel);
+      t.stype = static_cast<uint16_t>(l.st);
+      t.srel = w ? kWildcard : l.srel;
+      if (w ? l.has_srel : !l.srel_err.empty()) {
+        l.all_ok = false;
+        continue;
+      }
+      l.val_err[w][x] = e->store.validate(t, x != 0);
+      if (!l.val_err[w][x].empty()) l.all_ok = false;
+    }
+  return l;
+}
+
+static bool import_wild(const zg_import_group& g, uint64_t j) {
+  return g.subj_off[j + 1] - g.subj_off[j] == 1 && g.subj_ids[g.subj_off[j]] == '*';
+}
+
+// What the write path says of item j of group g at call position i, short of the duplicate checks: ZG_OK, or the code
+// with the message in *msg. syntax: check the ids too (the device path checks them on the device).
+static int import_item_error(const zg_import_group& g, const ImportLit& l, uint64_t j, uint64_t i, bool syntax,
+                             std::string* msg) {
+  const char* rid = g.res_ids + g.res_off[j];
+  const char* sid = g.subj_ids + g.subj_off[j];
+  const size_t rl = g.res_off[j + 1] - g.res_off[j], sl = g.subj_off[j + 1] - g.subj_off[j];
+  const bool wild = import_wild(g, j), expiring = g.expires_at && g.expires_at[j];
+  auto text = [&] {
+    const std::string r(rid, rl), su(sid, sl);
+    zg_rel_str x{g.res_type, r.c_str(), g.relation, g.subj_type, su.c_str(), g.subj_rel};
+    return rel_text(x);
+  };
+  std::string err = l.lit_err;
+  if (err.empty() && syntax) {
+    if (!valid_object_id(rid, rl) || (rl == 1 && rid[0] == '*'))
+      err = "invalid resource object id `" + std::string(rid, rl) + "`";
+    else if (!valid_object_id(sid, sl))
+      err = "invalid subject object id `" + std::string(sid, sl) + "`";
+  }
+  if (err.empty() && wild && l.has_srel) err = "wildcard subjects cannot have a relation";
+  if (err.empty() && !wild) err = l.srel_err;
+  if (!err.empty()) {
+    *msg = "relationship " + std::to_string(i) + " (" + text() + "): " + err;
+    return ZG_EINVAL;
+  }
+  const std::string& v = l.val_err[wild][expiring];
+  if (!v.empty()) {
+    *msg = "relationship " + std::to_string(i) + ": " + v;
+    return ZG_EINVAL;
+  }
+  return ZG_OK;
+}
+
+static int import_exists(uint64_t i) {
+  return fail(ZG_EEXIST, "relationship " + std::to_string(i) + ": relationship already exists");
+}
+
+// The error of the first failing relationship, at call position `first` (known to fail).
+static int import_fail_at(const zg_import_group* g, const std::vector<ImportLit>& lits, const std::vector<uint64_t>& item0,
+                          uint64_t first) {
+  const size_t k = static_cast<size_t>(std::upper_bound(item0.begin(), item0.end(), first) - item0.begin() - 1);
+  std::string msg;
+  const int rc = import_item_error(g[k], lits[k], first - item0[k], first, true, &msg);
+  return rc ? fail(rc, msg) : import_exists(first);
+}
+
+static double ms_since(const std::chrono::steady_clock::time_point& t0) {
+  return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+}
+
+// The host path: every relationship in call order through the write path's checks, new names in a per-call table with
+// temporary ids above each type's extent, duplicates against the relationship index and within the call. Then the new
+// names are interned in first-appearance order, which hands out the ids the write path would. Fills *t (ids final) and
+// *new_names; changes nothing else.
+static int import_on_host(zg_engine* e, const zg_import_group* g, uint64_t ng, const std::vector<ImportLit>& lits,
+                          std::vector<zg_tuple>* t, uint64_t* found, uint64_t* new_names) {
+  Store& st = e->store;
+  const size_t nt = e->schema.types.size();
+  std::vector<uint32_t> extent(nt);
+  for (size_t ty = 0; ty < nt; ++ty) extent[ty] = st.extent(static_cast<int>(ty));
+  std::vector<std::unordered_map<std::string_view, uint32_t>> fresh(nt);
+  std::vector<std::vector<std::string_view>> order(nt);
+  auto id_of = [&](int ty, const char* s, size_t len, bool* known) {
+    const uint32_t have = st.find(ty, s, len);
+    if (have != ZG_NO_OBJECT) {
+      ++*found;
+      return have;
+    }
+    *known = false;
+    const std::string_view v(s, len);
+    auto it = fresh[ty].find(v);
+    if (it != fresh[ty].end()) return it->second;
+    const uint32_t tmp = extent[ty] + static_cast<uint32_t>(order[ty].size());
+    order[ty].push_back(v);
+    fresh[ty].emplace(v, tmp);
+    return tmp;
+  };
+  std::unordered_set<Key, KeyHash> seen;
+  uint64_t i = 0;
+  for (uint64_t k = 0; k < ng; ++k)
+    for (uint64_t j = 0; j < g[k].n; ++j, ++i) {
+      const ImportLit& l = lits[k];
+      std::string msg;
+      if (int rc = import_item_error(g[k], l, j, i, true, &msg)) return fail(rc, msg);
+      zg_tuple x{};
+      x.rel = static_cast<uint16_t>(l.rel);
+      x.stype = static_cast<uint16_t>(l.st);
+      bool known = true;
+      if (import_wild(g[k], j)) {
+        x.srel = kWildcard;
+      } else {
+        x.srel = l.srel;
+        x.subj = id_of(l.st, g[k].subj_ids + g[k].subj_off[j], g[k].subj_off[j + 1] - g[k].subj_off[j], &known);
+      }
+      x.res = id_of(l.rt, g[k].res_ids + g[k].res_off[j], g[k].res_off[j + 1] - g[k].res_off[j], &known);
+      if ((known && st.contains(x)) || !seen.insert(key_of(x)).second) return import_exists(i);
+      t->push_back(x);
+    }
+  std::vector<std::vector<uint32_t>> ids(nt);
+  for (size_t ty = 0; ty < nt; ++ty) {
+    for (std::string_view v : order[ty]) ids[ty].push_back(st.intern(static_cast<int>(ty), std::string(v)));
+    *new_names += order[ty].size();
+  }
+  for (zg_tuple& x : *t) {
+    const uint32_t rt = e->schema.slots[x.rel].type;
+    if (x.res >= extent[rt]) x.res = ids[rt][x.res - extent[rt]];
+    if (x.srel != kWildcard && x.subj >= extent[x.stype]) x.subj = ids[x.stype][x.subj - extent[x.stype]];
+  }
+  return ZG_OK;
+}
+
+// The device path (import.cuh): names, sort and duplicates on the GPU; the host checks the item kinds the literal
+// fields decide (no id bytes read but a subject's first) and interns the new names the device found, with their
+// hashes, in first-appearance order. Fills *t and the counts; changes nothing but the name mirror's sync on failure.
+static int import_on_device(zg_engine* e, const zg_import_group* g, uint64_t ng, const std::vector<ImportLit>& lits,
+                            const std::vector<uint64_t>& item0, uint64_t total, bool locate, std::vector<zg_tuple>* t,
+                            uint64_t* found, uint64_t* new_names, double* ms) {
+  Store& st = e->store;
+  const Schema& sc = e->schema;
+  // the first item the literal fields fail: only the items before it can be the first to fail
+  uint64_t first = total;
+  for (uint64_t k = 0; k < ng && first == total; ++k) {
+    const ImportLit& l = lits[k];
+    if (l.all_ok || !g[k].n) continue;
+    if (!l.lit_err.empty()) {
+      first = item0[k];
+      break;
+    }
+    for (uint64_t j = 0; j < g[k].n; ++j) {
+      const bool wild = import_wild(g[k], j), expiring = g[k].expires_at && g[k].expires_at[j];
+      if ((wild ? l.has_srel : !l.srel_err.empty()) || !l.val_err[wild][expiring].empty()) {
+        first = item0[k] + j;
+        break;
+      }
+    }
+  }
+  std::vector<Device::ImportGroup> dg;
+  for (uint64_t k = 0; k < ng && item0[k] < first; ++k) {
+    if (!g[k].n) continue;
+    const ImportLit& l = lits[k];
+    Device::ImportGroup d{};
+    d.res_ids = g[k].res_ids;
+    d.subj_ids = g[k].subj_ids;
+    d.res_off = g[k].res_off;
+    d.subj_off = g[k].subj_off;
+    d.item0 = item0[k];
+    d.n = std::min<uint64_t>(g[k].n, first - item0[k]);
+    d.rtype = static_cast<uint32_t>(l.rt);
+    d.stype = static_cast<uint32_t>(l.st);
+    d.rel = static_cast<uint32_t>(l.rel);
+    d.rel_index = static_cast<uint32_t>(sc.slots[l.rel].rel_index);
+    d.srel = l.srel;
+    d.pos_plain = static_cast<uint32_t>(page_class_pos(sc, l.rel, static_cast<uint16_t>(l.st), l.srel));
+    d.pos_wild = static_cast<uint32_t>(page_class_pos(sc, l.rel, static_cast<uint16_t>(l.st), kWildcard));
+    d.k_plain = static_cast<uint32_t>(sc.class_of(l.rel, static_cast<uint16_t>(l.st), l.srel));
+    d.k_wild = static_cast<uint32_t>(sc.class_of(l.rel, static_cast<uint16_t>(l.st), kWildcard));
+    dg.push_back(d);
+  }
+  const uint64_t n = first;
+  const size_t nt = sc.types.size();
+  std::vector<uint32_t> extent(nt);
+  for (size_t ty = 0; ty < nt; ++ty) extent[ty] = st.extent(static_cast<int>(ty));
+  Device::ImportCheck chk;
+  std::string err;
+  if (int rc = e->dev.import_check(st, dg, n, extent, locate && !is_handle(e), &chk, &err)) return fail(rc == ZG_ENOMEM ? ZG_ECUDA : rc, err);
+  uint64_t dup = chk.dup;
+  if (locate && is_handle(e)) {
+    std::vector<uint64_t> d(e->n_shards, ~0ull);
+    if (int rc = on_devices(e, kEveryDevice, [&](Device& dev, size_t k, std::string* m) { return dev.import_locate(e->dev, &d[k], m); }, &err))
+      return fail(rc == ZG_ENOMEM ? ZG_ECUDA : rc, err);
+    for (uint64_t x : d) dup = std::min(dup, x);
+  }
+  ms[0] = chk.ms_names;
+  ms[1] = chk.ms_sort;
+  ms[2] = chk.ms_dups;
+  first = std::min({first, chk.bad, dup});
+  if (first < total) return import_fail_at(g, lits, item0, first);
+
+  // every check passed: the ids the host hands out, lowest free first, then the extent
+  const auto t0 = std::chrono::steady_clock::now();
+  std::vector<uint32_t> ids;
+  std::vector<uint64_t> base(nt, 0);
+  std::vector<uint32_t> next;
+  for (size_t ty = 0; ty < nt; ++ty) {
+    base[ty] = ids.size();
+    st.next_ids(static_cast<int>(ty), chk.type_count[ty], &next);
+    ids.insert(ids.end(), next.begin(), next.end());
+  }
+  std::vector<uint32_t> rtype_of_rel(sc.slots.size());
+  for (size_t r = 0; r < sc.slots.size(); ++r) rtype_of_rel[r] = sc.slots[r].type;
+  if (int rc = e->dev.import_finish(ids, base, rtype_of_rel, t, &err)) return fail(rc == ZG_ENOMEM ? ZG_ECUDA : rc, err);
+  for (size_t j = 0; j < chk.new_keys.size(); ++j) {
+    const int ty = static_cast<int>(chk.new_keys[j] >> 48);
+    const uint64_t o = chk.new_keys[j] & ((1ull << 48) - 1), item = o >> 1;
+    const size_t k = static_cast<size_t>(std::upper_bound(item0.begin(), item0.end(), item) - item0.begin() - 1);
+    const uint64_t at = item - item0[k];
+    const char* s = (o & 1) ? g[k].res_ids + g[k].res_off[at] : g[k].subj_ids + g[k].subj_off[at];
+    const uint32_t len = (o & 1) ? g[k].res_off[at + 1] - g[k].res_off[at] : g[k].subj_off[at + 1] - g[k].subj_off[at];
+    st.intern_new(ty, s, len, chk.new_hash[j]);
+  }
+  *found += chk.found;
+  *new_names += chk.new_keys.size();
+  ms[3] = ms_since(t0);
+  return ZG_OK;
+}
+
+extern "C" int zg_import_relationships(zg_engine* e, const zg_import_group* groups, uint64_t n_groups, uint64_t* n_imported) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (n_imported) *n_imported = 0;
+  if (!groups && n_groups) return fail(ZG_EINVAL, "NULL groups");
+  std::vector<uint64_t> item0(n_groups);
+  uint64_t total = 0;
+  for (uint64_t k = 0; k < n_groups; ++k) {
+    item0[k] = total;
+    if (!groups[k].n) continue;
+    if (!groups[k].res_ids || !groups[k].res_off || !groups[k].subj_ids || !groups[k].subj_off)
+      return fail(ZG_EINVAL, "group " + std::to_string(k) + ": NULL ids or offsets");
+    for (uint64_t j = 0; j < groups[k].n; ++j)
+      if (groups[k].res_off[j + 1] < groups[k].res_off[j] || groups[k].subj_off[j + 1] < groups[k].subj_off[j])
+        return fail(ZG_EINVAL, "group " + std::to_string(k) + ": offsets must not decrease");
+    total += groups[k].n;
+  }
+  // the device path indexes the new-name table (>= 4 slots per relationship) with 32-bit slot numbers
+  if (total > kMaxImport) return fail(ZG_EINVAL, "more than 2^30 relationships in one import");
+  LOCK_DEVICE(e);
+  LOCK_NAMES_UNIQUE(e);
+  if (e->store.shard_count > 1)
+    return fail(ZG_EINVAL, "import relationships: this engine is one shard of several (zg_config.shard_count) and its store "
+                           "does not hold the other shards' relationships");
+  std::vector<ImportLit> lits(n_groups);
+  for (uint64_t k = 0; k < n_groups; ++k) lits[k] = import_literals(e, groups[k]);
+  const char* ih = std::getenv("ZGPU_IMPORT_HOST");
+  // the device finds duplicates against the resident snapshot: it must be the store, or the store must be empty
+  const bool current = filters_on_device(e);
+  const bool on_device = !e->host_only && !(ih && *ih && *ih != '0') && (current || e->store.tuples.empty());
+  std::vector<zg_tuple> t;
+  t.reserve(total);
+  uint64_t found = 0, fresh = 0;
+  double ms[7] = {};  // zg_import_last_times: kept only when the import succeeds
+  const auto t0 = std::chrono::steady_clock::now();
+  struct Release {  // the scratch goes with the call, whatever its outcome
+    zg_engine* e;
+    ~Release() {
+      e->dev.import_release();
+      for (auto& r : e->replicas) r->dev.import_release();
+    }
+  } release{e};
+  const int rc = on_device ? import_on_device(e, groups, n_groups, lits, item0, total, current && !e->store.tuples.empty(), &t, &found, &fresh, ms)
+                           : import_on_host(e, groups, n_groups, lits, &t, &found, &fresh);
+  if (rc) return rc;
+  if (!on_device) ms[3] = ms_since(t0);
+  std::vector<uint32_t> ex(total, 0);
+  for (uint64_t k = 0; k < n_groups; ++k)
+    if (groups[k].expires_at) std::memcpy(ex.data() + item0[k], groups[k].expires_at, groups[k].n * 4);
+  const auto t1 = std::chrono::steady_clock::now();
+  e->store.import(t.data(), ex.data(), total);
+  ms[4] = ms_since(t1);
+  e->dirty = true;  // until the publish succeeds the snapshot is not the store: filters_on_device
+  const auto t2 = std::chrono::steady_clock::now();
+  const int prc = publish_locked(e);
+  ms[5] = ms_since(t2);
+  ms[6] = ms_since(t0);
+  if (prc) return prc;
+  std::memcpy(e->imp_ms, ms, sizeof(ms));
+  e->log_import(t, ex);
+  ++(on_device ? e->imp_device : e->imp_host);
+  e->imp_rels += total;
+  e->imp_found += found;
+  e->imp_new += fresh;
+  if (n_imported) *n_imported = total;
+  return ZG_OK;
+}
+
+extern "C" int zg_import_counters(zg_engine* e, uint64_t* out) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (!out) return fail(ZG_EINVAL, "out is NULL");
+  LOCK_DEVICE(e);
+  out[0] = e->imp_device;
+  out[1] = e->imp_host;
+  out[2] = e->imp_rels;
+  out[3] = e->imp_found;
+  out[4] = e->imp_new;
+  return ZG_OK;
+}
+
+extern "C" int zg_import_last_times(zg_engine* e, double* ms) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (!ms) return fail(ZG_EINVAL, "ms is NULL");
+  LOCK_DEVICE(e);
+  std::memcpy(ms, e->imp_ms, sizeof(e->imp_ms));
+  return ZG_OK;
 }
 
 extern "C" int zg_delete_relationships(zg_engine* e, const zg_filter_str* filter, const zg_precondition_str* pre,

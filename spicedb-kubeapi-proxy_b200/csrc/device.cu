@@ -15,6 +15,7 @@
 #include <cub/cub.cuh>
 
 #include "filter.cuh"
+#include "import.cuh"
 #include "ingress.cuh"
 #include "kernels.cuh"
 
@@ -34,6 +35,26 @@ namespace zg {
 const char* build_info() {
   return "libzgpu sm_90a built " __DATE__ " " __TIME__ " STACK_CAP=" ZG_STR(ZG_STACK_CAP) " RSET_CAP=" ZG_STR(ZG_RSET_CAP) " MIN_BLOCKS=" ZG_STR(ZG_MIN_BLOCKS);
 }
+
+// zg_import_relationships' scratch (import.cuh): the staged call, the new-name table, the items' tuples and keys.
+struct Device::ImportScratch {
+  DevBuf groups, blob, offs, tables;
+  DevBuf slots, first, hash, slot_type, occ_id, occ_slot;
+  DevBuf new_keys, new_vals, new_keys2, new_vals2, slot_tmp, out_hash, extent, type_start;
+  DevBuf tuples, key_hi, key_lo, key_hi2, key_lo2, vals, vals2, known;
+  DevBuf ctrl;  // [0] bad, [1] dup, [2] found, [3] new names
+  DevBuf cub, ids, base, rtype_of_rel;
+  uint64_t n = 0;
+  uint32_t n_groups = 0;
+  ~ImportScratch() {
+    for (DevBuf* b : {&groups, &blob, &offs, &tables, &slots, &first, &hash, &slot_type, &occ_id, &occ_slot, &new_keys,
+                      &new_vals, &new_keys2, &new_vals2, &slot_tmp, &out_hash, &extent, &type_start, &tuples, &key_hi,
+                      &key_lo, &key_hi2, &key_lo2, &vals, &vals2, &known, &ctrl, &cub, &ids, &base, &rtype_of_rel})
+      b->release();
+  }
+};
+
+void Device::ImportScratchFree::operator()(ImportScratch* x) const { delete x; }
 
 bool DevBuf::ensure(size_t bytes) {
   if (bytes <= cap) return true;
@@ -264,11 +285,10 @@ std::string Device::verify_against_host(const Store& store, const Schema& sc) {
 }
 
 std::string Device::publish_delta(const Store& store, const Schema& sc, uint64_t revision) {
-  constexpr size_t kMaxDelta = 1u << 16;
   std::shared_ptr<Snapshot> s = snap;
   // an engine that is one shard of a store per process (shard_count > 1 over a store of its own) always rebuilds
   const bool own_store_shard = shard_count > 1 && own_count < 2;
-  if (!s || !s->delta_ok || !store.journal_ok || own_store_shard || store.journal.size() > kMaxDelta || !store.layout_stable())
+  if (!s || !s->delta_ok || !store.journal_ok || own_store_shard || store.journal.size() > Store::kMaxJournal || !store.layout_stable())
     return "full";
   cudaSetDevice(device);
   closure_ms = 0;
@@ -3329,6 +3349,302 @@ int Device::ingress_check_host(const Store& store, const IngressLiterals& lit, c
   ZG_CUDA(cudaMemcpyAsync(m.pin_out, m.out.p, n, cudaMemcpyDeviceToHost, stream));
   ZG_CUDA(cudaStreamSynchronize(stream));
   std::memcpy(out, m.pin_out, n);
+  return ZG_OK;
+}
+
+// ---- zg_import_relationships -----------------------------------------------------------------------
+
+static unsigned import_grid(uint64_t n, int sm_count) {
+  const uint64_t want = (n + kImportThreads - 1) / kImportThreads;
+  return static_cast<unsigned>(std::max<uint64_t>(1, std::min<uint64_t>(want, uint64_t(std::max(sm_count, 1)) * 16)));
+}
+
+int Device::import_check(const Store& store, const std::vector<ImportGroup>& groups, uint64_t n,
+                         const std::vector<uint32_t>& extent, bool locate, ImportCheck* out, std::string* err) {
+  ZG_CUDA(cudaSetDevice(device));
+  *out = ImportCheck{};
+  out->type_count.assign(extent.size(), 0);
+  if (!import_) import_.reset(new ImportScratch());
+  ImportScratch& x = *import_;
+  x.n = n;
+  x.n_groups = static_cast<uint32_t>(groups.size());
+  if (n == 0) return ZG_OK;
+  int rc = ingress_sync(store, stream, err);
+  if (rc) return rc;
+  auto need = [&](DevBuf& b, size_t bytes) {
+    if (b.ensure(bytes)) return true;
+    if (err) *err = "out of device memory (import scratch)";
+    return false;
+  };
+  // stage: every group's blobs and offsets (res_off then subj_off), and the groups
+  std::shared_ptr<Snapshot> snap_now = snap;
+  std::vector<ImportGroupDev> gd(groups.size());
+  uint64_t blob_bytes = 0, off_words = 0;
+  for (size_t g = 0; g < groups.size(); ++g) {
+    const ImportGroup& h = groups[g];
+    ImportGroupDev& d = gd[g];
+    d.item0 = h.item0;
+    d.n = h.n;
+    d.res_blob = blob_bytes;
+    blob_bytes += h.res_off[h.n];
+    d.subj_blob = blob_bytes;
+    blob_bytes += h.subj_off[h.n];
+    d.off0 = off_words;
+    off_words += 2 * (h.n + 1);
+    d.rtype = h.rtype;
+    d.stype = h.stype;
+    d.rel = h.rel;
+    d.srel = h.srel;
+    d.pos_plain = h.pos_plain;
+    d.pos_wild = h.pos_wild;
+    d.k_plain = h.k_plain;
+    d.k_wild = h.k_wild;
+    if (snap_now && h.rel_index < snap_now->rels.size()) {
+      const DRel& r = snap_now->rels[h.rel_index];
+      d.row_base = r.row_base;
+      d.stride = r.stride;
+      d.nres = r.nres;
+    }
+  }
+  const uint64_t occ = 2 * n;
+  uint64_t cap = 64;
+  while (cap < 2 * occ) cap *= 2;
+  const size_t nt = extent.size();
+  if (!need(x.groups, gd.size() * sizeof(ImportGroupDev)) || !need(x.blob, blob_bytes + 8) || !need(x.offs, off_words * 4) ||
+      !need(x.tables, nt * sizeof(IngressTable)) || !need(x.slots, cap * 8) || !need(x.first, cap * 8) ||
+      !need(x.hash, cap * 8) || !need(x.slot_type, cap * 4) || !need(x.occ_id, occ * 4) || !need(x.occ_slot, occ * 4) ||
+      !need(x.ctrl, 4 * 8) || !need(x.extent, nt * 4) || !need(x.type_start, nt * 8))
+    return ZG_ENOMEM;
+  for (size_t g = 0; g < groups.size(); ++g) {
+    const ImportGroup& h = groups[g];
+    ZG_CUDA(cudaMemcpyAsync(x.blob.as<char>() + gd[g].res_blob, h.res_ids, h.res_off[h.n], cudaMemcpyHostToDevice, stream));
+    ZG_CUDA(cudaMemcpyAsync(x.blob.as<char>() + gd[g].subj_blob, h.subj_ids, h.subj_off[h.n], cudaMemcpyHostToDevice, stream));
+    ZG_CUDA(cudaMemcpyAsync(x.offs.as<uint32_t>() + gd[g].off0, h.res_off, (h.n + 1) * 4, cudaMemcpyHostToDevice, stream));
+    ZG_CUDA(cudaMemcpyAsync(x.offs.as<uint32_t>() + gd[g].off0 + h.n + 1, h.subj_off, (h.n + 1) * 4, cudaMemcpyHostToDevice,
+                            stream));
+  }
+  ZG_CUDA(cudaMemcpyAsync(x.groups.p, gd.data(), gd.size() * sizeof(ImportGroupDev), cudaMemcpyHostToDevice, stream));
+  std::vector<IngressTable> tabs(nt, IngressTable{nullptr, nullptr, 0});
+  for (size_t t = 0; t < nt && t < ingress_->types.size(); ++t)
+    if (ingress_->types[t].cap) {
+      tabs[t].arena = ingress_->types[t].arena.as<uint8_t>();
+      tabs[t].slots = ingress_->types[t].slots.as<unsigned long long>();
+      tabs[t].mask = ingress_->types[t].cap - 1;
+    }
+  ZG_CUDA(cudaMemcpyAsync(x.tables.p, tabs.data(), nt * sizeof(IngressTable), cudaMemcpyHostToDevice, stream));
+  ZG_CUDA(cudaMemcpyAsync(x.extent.p, extent.data(), nt * 4, cudaMemcpyHostToDevice, stream));
+  ZG_CUDA(cudaMemsetAsync(x.slots.p, 0, cap * 8, stream));
+  ZG_CUDA(cudaMemsetAsync(x.first.p, 0xFF, cap * 8, stream));
+  ZG_CUDA(cudaMemsetAsync(x.ctrl.p, 0xFF, 2 * 8, stream));
+  ZG_CUDA(cudaMemsetAsync(x.ctrl.as<unsigned long long>() + 2, 0, 2 * 8, stream));
+  unsigned long long* ctrl = x.ctrl.as<unsigned long long>();
+  ImportCall call{x.groups.as<ImportGroupDev>(), x.n_groups, x.blob.as<uint8_t>(), x.offs.as<uint32_t>(), n};
+  cudaEvent_t ev[4];
+  for (auto& e : ev) ZG_CUDA(cudaEventCreate(&e));
+  struct Events {
+    cudaEvent_t* e;
+    ~Events() {
+      for (int i = 0; i < 4; ++i) cudaEventDestroy(e[i]);
+    }
+  } ev_guard{ev};
+  ZG_CUDA(cudaEventRecord(ev[0], stream));
+
+  // 1. names
+  ImportNamesParams np{};
+  np.c = call;
+  np.tables = x.tables.as<IngressTable>();
+  np.slots = x.slots.as<unsigned long long>();
+  np.mask = cap - 1;
+  np.first = x.first.as<unsigned long long>();
+  np.hash = x.hash.as<unsigned long long>();
+  np.slot_type = x.slot_type.as<uint32_t>();
+  np.occ_id = x.occ_id.as<uint32_t>();
+  np.occ_slot = x.occ_slot.as<uint32_t>();
+  np.bad = ctrl;
+  np.tag_mask = kIngressTagMask;
+  np.found = ctrl + 2;
+  import_names_kernel<<<import_grid(occ, sm_count_), kImportThreads, 0, stream>>>(np);
+  ZG_CUDA(cudaGetLastError());
+  ++launches;
+
+  // 2. new names sorted by (type, first occurrence); the host needs each type's first rank for the temporary ids
+  uint64_t n_new = 0;
+  {
+    if (!need(x.new_keys, cap * 8) || !need(x.new_vals, cap * 4)) return ZG_ENOMEM;
+    import_compact_kernel<<<import_grid(cap, sm_count_), kImportThreads, 0, stream>>>(
+        x.slots.as<unsigned long long>(), cap, x.first.as<unsigned long long>(), x.slot_type.as<uint32_t>(),
+        x.new_keys.as<unsigned long long>(), x.new_vals.as<uint32_t>(), ctrl + 3);
+    ZG_CUDA(cudaGetLastError());
+    ++launches;
+    unsigned long long h[4];
+    ZG_CUDA(cudaMemcpyAsync(h, ctrl, sizeof(h), cudaMemcpyDeviceToHost, stream));
+    ZG_CUDA(cudaStreamSynchronize(stream));
+    out->bad = h[0];
+    out->found = h[2];
+    n_new = h[3];
+  }
+  ZG_CUDA(cudaEventRecord(ev[1], stream));
+  if (n_new) {
+    if (!need(x.new_keys2, n_new * 8) || !need(x.new_vals2, n_new * 4) || !need(x.slot_tmp, cap * 4) ||
+        !need(x.out_hash, n_new * 8))
+      return ZG_ENOMEM;
+    size_t tmp = 0;
+    int end_bit = 48;
+    while ((uint64_t(1) << (end_bit - 48)) < nt) ++end_bit;
+    ZG_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tmp, x.new_keys.as<unsigned long long>(), x.new_keys2.as<unsigned long long>(),
+                                            x.new_vals.as<uint32_t>(), x.new_vals2.as<uint32_t>(), n_new, 0, end_bit, stream));
+    if (!need(x.cub, tmp)) return ZG_ENOMEM;
+    ZG_CUDA(cub::DeviceRadixSort::SortPairs(x.cub.p, tmp, x.new_keys.as<unsigned long long>(), x.new_keys2.as<unsigned long long>(),
+                                            x.new_vals.as<uint32_t>(), x.new_vals2.as<uint32_t>(), n_new, 0, end_bit, stream));
+    out->new_keys.resize(n_new);
+    ZG_CUDA(cudaMemcpyAsync(out->new_keys.data(), x.new_keys2.p, n_new * 8, cudaMemcpyDeviceToHost, stream));
+    ZG_CUDA(cudaStreamSynchronize(stream));
+    std::vector<uint64_t> start(nt, 0);
+    for (uint64_t j = n_new; j-- > 0;) {
+      const uint32_t t = static_cast<uint32_t>(out->new_keys[j] >> 48);
+      start[t] = j;
+      ++out->type_count[t];
+    }
+    ZG_CUDA(cudaMemcpyAsync(x.type_start.p, start.data(), nt * 8, cudaMemcpyHostToDevice, stream));
+    import_rank_kernel<<<import_grid(n_new, sm_count_), kImportThreads, 0, stream>>>(
+        x.new_keys2.as<unsigned long long>(), x.new_vals2.as<uint32_t>(), n_new, x.extent.as<uint32_t>(),
+        x.type_start.as<unsigned long long>(), x.hash.as<unsigned long long>(), x.slot_tmp.as<uint32_t>(),
+        x.out_hash.as<unsigned long long>());
+    ZG_CUDA(cudaGetLastError());
+    ++launches;
+    out->new_hash.resize(n_new);
+    ZG_CUDA(cudaMemcpyAsync(out->new_hash.data(), x.out_hash.p, n_new * 8, cudaMemcpyDeviceToHost, stream));
+  }
+
+  // 3. tuples and keys, sorted stably by K (low word, then high word)
+  if (!need(x.tuples, n * sizeof(zg_tuple)) || !need(x.key_hi, n * 8) || !need(x.key_lo, n * 8) || !need(x.key_hi2, n * 8) ||
+      !need(x.key_lo2, n * 8) || !need(x.vals, n * 4) || !need(x.vals2, n * 4) || !need(x.known, n) || !need(x.slot_tmp, 4))
+    return ZG_ENOMEM;
+  ImportAssembleParams ap{};
+  ap.c = call;
+  ap.occ_id = x.occ_id.as<uint32_t>();
+  ap.occ_slot = x.occ_slot.as<uint32_t>();
+  ap.slot_tmp = x.slot_tmp.as<uint32_t>();
+  ap.tuples = x.tuples.as<zg_tuple>();
+  ap.key_hi = x.key_hi.as<unsigned long long>();
+  ap.key_lo = x.key_lo.as<unsigned long long>();
+  ap.vals = x.vals.as<uint32_t>();
+  ap.known = x.known.as<uint8_t>();
+  import_assemble_kernel<<<import_grid(n, sm_count_), kImportThreads, 0, stream>>>(ap);
+  ZG_CUDA(cudaGetLastError());
+  ++launches;
+  {
+    // two stable passes: by the low words, then by the high words gathered into that order; equal keys keep call order
+    size_t t1 = 0, t2 = 0;
+    ZG_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t1, x.key_lo.as<unsigned long long>(), x.key_lo2.as<unsigned long long>(),
+                                            x.vals.as<uint32_t>(), x.vals2.as<uint32_t>(), n, 0, 64, stream));
+    ZG_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, t2, x.key_hi2.as<unsigned long long>(), x.key_lo2.as<unsigned long long>(),
+                                            x.vals2.as<uint32_t>(), x.vals.as<uint32_t>(), n, 0, 64, stream));
+    if (!need(x.cub, std::max(t1, t2))) return ZG_ENOMEM;
+    ZG_CUDA(cub::DeviceRadixSort::SortPairs(x.cub.p, t1, x.key_lo.as<unsigned long long>(), x.key_lo2.as<unsigned long long>(),
+                                            x.vals.as<uint32_t>(), x.vals2.as<uint32_t>(), n, 0, 64, stream));
+    import_gather_kernel<<<import_grid(n, sm_count_), kImportThreads, 0, stream>>>(
+        x.key_hi.as<unsigned long long>(), x.vals2.as<uint32_t>(), n, x.key_hi2.as<unsigned long long>());
+    ZG_CUDA(cudaGetLastError());
+    ++launches;
+    ZG_CUDA(cub::DeviceRadixSort::SortPairs(x.cub.p, t2, x.key_hi2.as<unsigned long long>(), x.key_lo2.as<unsigned long long>(),
+                                            x.vals2.as<uint32_t>(), x.vals.as<uint32_t>(), n, 0, 64, stream));
+  }
+  ZG_CUDA(cudaEventRecord(ev[2], stream));
+
+  // 4. duplicates: equal neighbours in K order, and the items the resident snapshot holds
+  import_adjacent_kernel<<<import_grid(n, sm_count_), kImportThreads, 0, stream>>>(
+      x.key_hi.as<unsigned long long>(), x.key_lo.as<unsigned long long>(), x.vals.as<uint32_t>(), n, ctrl + 1);
+  ZG_CUDA(cudaGetLastError());
+  ++launches;
+  if (locate && snap_now) {
+    ImportLocateParams lp{};
+    lp.c = call;
+    lp.tuples = x.tuples.as<zg_tuple>();
+    lp.known = x.known.as<uint8_t>();
+    lp.row_ptr = snap_now->row_ptr.as<uint32_t>();
+    lp.col = snap_now->col.as<uint32_t>();
+    lp.owner_rank = 0;
+    lp.owner_count = 1;
+    lp.dup = ctrl + 1;
+    import_locate_kernel<<<import_grid(n, sm_count_), kImportThreads, 0, stream>>>(lp);
+    ZG_CUDA(cudaGetLastError());
+    ++launches;
+  }
+  ZG_CUDA(cudaEventRecord(ev[3], stream));
+  unsigned long long dup = 0;
+  ZG_CUDA(cudaMemcpyAsync(&dup, ctrl + 1, 8, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  out->dup = dup;
+  float a = 0, b = 0, c = 0;
+  cudaEventElapsedTime(&a, ev[0], ev[1]);
+  cudaEventElapsedTime(&b, ev[1], ev[2]);
+  cudaEventElapsedTime(&c, ev[2], ev[3]);
+  out->ms_names = a;
+  out->ms_sort = b;
+  out->ms_dups = c;
+  return ZG_OK;
+}
+
+void Device::import_release() {
+  if (!import_) return;
+  cudaSetDevice(device);
+  import_.reset();
+}
+
+int Device::import_locate(const Device& src, uint64_t* dup, std::string* err) {
+  *dup = ~0ull;
+  const ImportScratch* x = src.import_.get();
+  std::shared_ptr<Snapshot> s = snap;
+  if (!x || !x->n || !s) return ZG_OK;
+  ZG_CUDA(cudaSetDevice(device));
+  if (!import_) import_.reset(new ImportScratch());
+  if (!import_->ctrl.ensure(8)) {
+    if (err) *err = "out of device memory (import scratch)";
+    return ZG_ENOMEM;
+  }
+  unsigned long long* d = import_->ctrl.as<unsigned long long>();
+  ZG_CUDA(cudaMemsetAsync(d, 0xFF, 8, stream));
+  ImportLocateParams lp{};
+  lp.c = ImportCall{x->groups.as<ImportGroupDev>(), x->n_groups, x->blob.as<uint8_t>(), x->offs.as<uint32_t>(), x->n};
+  lp.tuples = x->tuples.as<zg_tuple>();
+  lp.known = x->known.as<uint8_t>();
+  lp.row_ptr = s->row_ptr.as<uint32_t>();
+  lp.col = s->col.as<uint32_t>();
+  lp.owner_rank = own_rank;
+  lp.owner_count = own_count;
+  lp.dup = d;
+  import_locate_kernel<<<import_grid(x->n, sm_count_), kImportThreads, 0, stream>>>(lp);
+  ZG_CUDA(cudaGetLastError());
+  ++launches;
+  unsigned long long h = 0;
+  ZG_CUDA(cudaMemcpyAsync(&h, d, 8, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  *dup = h;
+  return ZG_OK;
+}
+
+int Device::import_finish(const std::vector<uint32_t>& ids, const std::vector<uint64_t>& base,
+                          const std::vector<uint32_t>& rtype_of_rel, std::vector<zg_tuple>* tuples, std::string* err) {
+  ZG_CUDA(cudaSetDevice(device));
+  ImportScratch& x = *import_;
+  tuples->resize(x.n);
+  if (!x.n) return ZG_OK;
+  if (!x.ids.ensure(std::max<size_t>(ids.size(), 1) * 4) || !x.base.ensure(base.size() * 8) ||
+      !x.rtype_of_rel.ensure(rtype_of_rel.size() * 4)) {
+    if (err) *err = "out of device memory (import scratch)";
+    return ZG_ENOMEM;
+  }
+  if (!ids.empty()) ZG_CUDA(cudaMemcpyAsync(x.ids.p, ids.data(), ids.size() * 4, cudaMemcpyHostToDevice, stream));
+  ZG_CUDA(cudaMemcpyAsync(x.base.p, base.data(), base.size() * 8, cudaMemcpyHostToDevice, stream));
+  ZG_CUDA(cudaMemcpyAsync(x.rtype_of_rel.p, rtype_of_rel.data(), rtype_of_rel.size() * 4, cudaMemcpyHostToDevice, stream));
+  import_remap_kernel<<<import_grid(x.n, sm_count_), kImportThreads, 0, stream>>>(
+      x.tuples.as<zg_tuple>(), x.n, x.rtype_of_rel.as<uint32_t>(), x.extent.as<uint32_t>(), x.base.as<unsigned long long>(),
+      x.ids.as<uint32_t>());
+  ZG_CUDA(cudaGetLastError());
+  ++launches;
+  ZG_CUDA(cudaMemcpyAsync(tuples->data(), x.tuples.p, x.n * sizeof(zg_tuple), cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaStreamSynchronize(stream));
   return ZG_OK;
 }
 

@@ -365,6 +365,42 @@ class Device {
   void ingress_reset() { ingress_.reset(); }  // a schema (re)load: the names are gone
   std::unique_ptr<IngressMirror> ingress_;     // nullptr until the first device-ingress call
 
+  // ---- zg_import_relationships (import.cuh) ----
+  // One group of an import, its literal fields resolved on the host (HOST blobs and offsets, as the caller passed them).
+  struct ImportGroup {
+    const char *res_ids, *subj_ids;
+    const uint32_t *res_off, *subj_off;
+    uint64_t item0, n;  // call position of its first item, its items
+    uint32_t rtype, stype, rel, rel_index, srel;
+    uint32_t pos_plain, pos_wild, k_plain, k_wild;  // class positions in K and class indexes (~0u: no such class)
+  };
+  struct ImportCheck {
+    uint64_t bad = ~0ull, dup = ~0ull;  // smallest call positions of a malformed id / a duplicate
+    uint64_t found = 0;                 // name occurrences the store had
+    std::vector<uint64_t> new_keys;     // the new names, (type << 48 | first occurrence), sorted
+    std::vector<uint64_t> new_hash;     // their hash_bytes, in that order
+    std::vector<uint64_t> type_count;   // new names per type
+    double ms_names = 0, ms_sort = 0, ms_dups = 0;  // device time of the steps
+  };
+  // Steps 1-4 of import.cuh for the n items of `groups` (syncing the name mirror first): new names, temporary ids, the
+  // smallest positions of malformed ids and of duplicates in the call and, when `locate`, against this device's
+  // resident snapshot. Changes nothing but the import's scratch. `extent`: every type's id extent (Store::extent).
+  int import_check(const Store& store, const std::vector<ImportGroup>& groups, uint64_t n, const std::vector<uint32_t>& extent,
+                   bool locate, ImportCheck* out, std::string* err);
+  // A shard of a sharded handle: the duplicates against its own snapshot of the items `src` (the shard that ran
+  // import_check, its scratch read through peer memory) holds, of the resources it owns; the smallest position in *dup.
+  int import_locate(const Device& src, uint64_t* dup, std::string* err);
+  // Step 5: the temporary ids to `ids` (per type, concatenated from base[type]), and the n tuples back in call order.
+  int import_finish(const std::vector<uint32_t>& ids, const std::vector<uint64_t>& base, const std::vector<uint32_t>& rtype_of_rel,
+                    std::vector<zg_tuple>* tuples, std::string* err);
+  // Frees the import's scratch: an import is a rare load or resync call, and its scratch is several times its input.
+  void import_release();
+  struct ImportScratch;
+  struct ImportScratchFree {  // defined in device.cu, where ImportScratch is complete
+    void operator()(ImportScratch* x) const;
+  };
+  std::unique_ptr<ImportScratch, ImportScratchFree> import_;
+
   std::shared_ptr<Snapshot> snap;
   cudaStream_t stream = nullptr;
   int device = 0;

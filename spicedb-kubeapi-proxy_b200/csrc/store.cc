@@ -53,8 +53,11 @@ uint32_t Store::TypeObjs::lookup(const char* s, size_t n) const {
 void Store::TypeObjs::place(uint64_t off) {
   uint32_t id, len;
   rec_read(arena, off, &id, &len);
+  place(off, hash_bytes(arena.data() + off + 8, len));
+}
+void Store::TypeObjs::place(uint64_t off, uint64_t hash) {
   const size_t mask = table.size() - 1;
-  size_t i = hash_bytes(arena.data() + off + 8, len) & mask;
+  size_t i = hash & mask;
   while (table[i]) i = (i + 1) & mask;
   table[i] = off + 1;
 }
@@ -72,22 +75,66 @@ void Store::TypeObjs::insert(uint64_t rec) {
 }
 
 uint32_t Store::intern(int type, const std::string& id) {
-  TypeObjs& t = objs_[type];
-  const uint32_t have = t.lookup(id.data(), id.size());
+  const uint32_t have = objs_[type].lookup(id.data(), id.size());
   if (have != ZG_NO_OBJECT) return have;
+  return intern_new(type, id.data(), static_cast<uint32_t>(id.size()), hash_bytes(id.data(), id.size()));
+}
+void Store::next_ids(int type, uint64_t count, std::vector<uint32_t>* out) const {
+  const TypeObjs& t = objs_[type];
+  out->clear();
+  out->reserve(count);
+  for (uint32_t w = t.free_word; t.n_free && w < t.free_bits.size() && out->size() < count; ++w)
+    for (uint32_t b = t.free_bits[w]; b && out->size() < count; b &= b - 1)
+      out->push_back(w * 32 + static_cast<uint32_t>(__builtin_ctz(b)));
+  for (uint32_t id = extent(type); out->size() < count; ++id) out->push_back(id);
+}
+
+uint32_t Store::intern_new(int type, const char* s, uint32_t len, uint64_t hash) {
+  TypeObjs& t = objs_[type];
   // keep string ids and bulk numeric ids in one id space; the ids of retired names go first, lowest first
   const uint32_t nid = t.n_free ? t.take_free() : std::max<uint32_t>(t.n_ids(), t.n_numeric);
   if (nid >= t.n_ids()) t.rec_of.resize(nid + 1, 0);
   const uint64_t rec = t.arena.size();
-  const uint32_t len = static_cast<uint32_t>(id.size());
   t.arena.resize(rec + 8 + len);
   std::memcpy(t.arena.data() + rec, &nid, 4);
   std::memcpy(t.arena.data() + rec + 4, &len, 4);
-  std::memcpy(t.arena.data() + rec + 8, id.data(), len);
+  std::memcpy(t.arena.data() + rec + 8, s, len);
   t.rec_of[nid] = rec + 1;
-  t.insert(rec);
+  if ((t.n_interned + 1) * 2 > t.table.size()) {
+    t.insert(rec);  // grows the table, re-hashing every record
+  } else {
+    t.place(rec, hash);
+    ++t.n_interned;
+  }
   return nid;
 }
+
+void Store::import(const zg_tuple* t, const uint32_t* ex, uint64_t n) {
+  if (journal_ok && journal.size() + n > kMaxJournal) {  // only a rebuild publishes this many
+    journal.clear();
+    journal_ok = false;
+  }
+  if (indexed_) index_.reserve(index_.size() + n);
+  tuples.reserve(tuples.size() + n);
+  expires.reserve(tuples.capacity());
+  for (uint64_t i = 0; i < n; ++i) {
+    zg_tuple x = t[i];
+    x.flags = 0;
+    if (x.srel == kWildcard) x.subj = 0;
+    const uint32_t e = ex ? ex[i] : 0;
+    if (indexed_) index_.emplace(key_of(x), tuples.size());
+    if (journal_ok) journal.push_back(JournalEntry{x, e, kInserted});
+    tuples.push_back(x);
+    expires.push_back(e);
+  }
+  live_ += n;
+}
+
+bool Store::contains(const zg_tuple& t) {
+  ensure_index();
+  return index_.count(key_of(t)) != 0;
+}
+
 uint32_t Store::find(int type, const std::string& id) const { return find(type, id.data(), id.size()); }
 uint32_t Store::find(int type, const char* id, size_t len) const {
   if (type < 0 || type >= static_cast<int>(objs_.size())) return ZG_NO_OBJECT;

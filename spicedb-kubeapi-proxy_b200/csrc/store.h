@@ -3,6 +3,7 @@
 // pkg/authz/distributedtx/activity.go:54-76) and the CSR snapshot builder whose
 // output the engine uploads to HBM.
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <string>
 #include <string_view>
@@ -114,6 +115,23 @@ class Store {
   NameCounts name_counts() const;
   uint32_t capacity(int type) const { return type >= 0 && type < static_cast<int>(obj_cap_.size()) ? obj_cap_[type] : 0; }
 
+  // ---- importing named relationships (zg_import_relationships) ----
+  // The id space of a type: ids below it are named or used by a bulk load; interning extends it.
+  uint32_t extent(int type) const { return std::max<uint32_t>(objs_[type].n_ids(), objs_[type].n_numeric); }
+  // The ids that interning `count` new names of `type` hands out, in order: free ids lowest first, then the extent.
+  // Changes nothing.
+  void next_ids(int type, uint64_t count, std::vector<uint32_t>* out) const;
+  // Interns a name known not to be interned, whose hash_bytes() is `hash` (computed on the device): the id intern()
+  // would give it. Returns the id.
+  uint32_t intern_new(int type, const char* s, uint32_t len, uint64_t hash);
+  // Appends n relationships known to be valid and new (no duplicate among them or in the store), whose names are
+  // interned. A current relationship index stays current; the journal records them while it can.
+  void import(const zg_tuple* t, const uint32_t* expires, uint64_t n);
+  // true when the store holds a live relationship with t's key; builds the index when a bulk load left it behind
+  bool contains(const zg_tuple& t);
+  // the most changes the journal holds for an incremental publish (Device::publish_delta); more rebuild
+  static constexpr size_t kMaxJournal = 1u << 16;
+
   // Returns "" or an error message; `code` receives the ZG_* code.
   std::string validate(const zg_tuple& t, bool has_expiry) const;
   std::string load(const zg_tuple* t, const uint32_t* expires, uint64_t n);
@@ -200,6 +218,7 @@ class Store {
     uint32_t lookup(const char* s, size_t n) const;
     void insert(uint64_t rec);  // record offset
     void place(uint64_t rec);   // into a table with room
+    void place(uint64_t rec, uint64_t hash);
     uint32_t n_ids() const { return static_cast<uint32_t>(rec_of.size()); }
     uint32_t take_free();  // the lowest free id, off the list
     // a relationship names `id` directly (bulk load, raw update): it is no longer free
