@@ -37,6 +37,7 @@ import (
 	"fmt"
 	"io"
 	"runtime"
+	"strconv"
 	"strings"
 	"sync"
 	"sync/atomic"
@@ -503,6 +504,81 @@ func (s *subjectStream) CloseSend() error             { return nil }
 func (s *subjectStream) Context() context.Context     { return s.ctx }
 func (s *subjectStream) SendMsg(any) error            { return nil }
 func (s *subjectStream) RecvMsg(any) error            { return io.EOF }
+
+// ExpandPermissionTree: the permission's subject tree at the resource, built on the GPU from zg_expand_permission_tree_str
+// (one line per node in pre-order: "<depth> <U|I|X|L> <type>:<id>#<relation>[ <subject>]*"). A sharded engine delegates
+// to the embedded SpiceDB.
+func (c *Client) ExpandPermissionTree(ctx context.Context, req *v1.ExpandPermissionTreeRequest, opts ...grpc.CallOption) (*v1.ExpandPermissionTreeResponse, error) {
+	if c.sharded {
+		return c.PermissionsServiceClient.ExpandPermissionTree(ctx, req, opts...)
+	}
+	if c.broken.Load() {
+		return nil, errBroken
+	}
+	var s cstrs
+	defer s.free()
+	capacity := C.size_t(1 << 16)
+	for {
+		buf := (*C.char)(C.malloc(capacity))
+		var need C.size_t
+		var n C.uint64_t
+		var rc C.int
+		err := call(func() C.int {
+			rc = C.zg_expand_permission_tree_str(c.engine, s.add(req.GetResource().GetObjectType()),
+				s.add(req.GetResource().GetObjectId()), s.add(req.GetPermission()), buf, capacity, &need, &n)
+			if rc == C.ZG_E2BIG {
+				return 0
+			}
+			return rc
+		})
+		if rc == C.ZG_E2BIG {
+			C.free(unsafe.Pointer(buf))
+			capacity = need + 16
+			continue
+		}
+		if err != nil {
+			C.free(unsafe.Pointer(buf))
+			return nil, err
+		}
+		lines := strings.Split(strings.TrimSuffix(C.GoString(buf), "\n"), "\n")
+		C.free(unsafe.Pointer(buf))
+		ops := map[string]v1.AlgebraicSubjectSet_Operation{"U": v1.AlgebraicSubjectSet_OPERATION_UNION,
+			"I": v1.AlgebraicSubjectSet_OPERATION_INTERSECTION, "X": v1.AlgebraicSubjectSet_OPERATION_EXCLUSION}
+		ref := func(s string) (*v1.ObjectReference, string) { // "type:id[#rel]"
+			t, rest, _ := strings.Cut(s, ":")
+			id, rel, _ := strings.Cut(rest, "#")
+			return &v1.ObjectReference{ObjectType: t, ObjectId: id}, rel
+		}
+		var root *v1.PermissionRelationshipTree
+		var stack []*v1.PermissionRelationshipTree // the open ancestors of the next line, by depth
+		for _, line := range lines {
+			f := strings.Split(line, " ")
+			depth, _ := strconv.Atoi(f[0])
+			at := strings.LastIndex(f[2], "#")
+			obj, _ := ref(f[2][:at])
+			node := &v1.PermissionRelationshipTree{ExpandedObject: obj, ExpandedRelation: f[2][at+1:]}
+			if f[1] == "L" {
+				leaf := &v1.DirectSubjectSet{}
+				for _, x := range f[3:] {
+					o, rel := ref(x)
+					leaf.Subjects = append(leaf.Subjects, &v1.SubjectReference{Object: o, OptionalRelation: rel})
+				}
+				node.TreeType = &v1.PermissionRelationshipTree_Leaf{Leaf: leaf}
+			} else {
+				node.TreeType = &v1.PermissionRelationshipTree_Intermediate{Intermediate: &v1.AlgebraicSubjectSet{Operation: ops[f[1]]}}
+			}
+			stack = stack[:depth]
+			if depth == 0 {
+				root = node
+			} else {
+				parent := stack[depth-1].GetIntermediate()
+				parent.Children = append(parent.Children, node)
+			}
+			stack = append(stack, node)
+		}
+		return &v1.ExpandPermissionTreeResponse{TreeRoot: root}, nil
+	}
+}
 
 // WriteRelationships: SpiceDB stays the source of truth (preconditions, idempotency keys
 // with expiry: pkg/authz/distributedtx/activity.go:54-102); a successful write is mirrored

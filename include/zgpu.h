@@ -507,6 +507,59 @@ int zg_lookup_subjects_str(zg_engine *e, const char *res_type, const char *res_i
  * by the forward walk, out[1] lookups that verified every object of the subject type, out[2] check items of
  * their first verification launches (the probe included). */
 int zg_lookup_subjects_counters(zg_engine *e, uint64_t *out);
+
+/* ExpandPermissionTree (v1, shallow): the subject tree of object `res` (of perm's type, ZG_NO_OBJECT: a never-written
+ * one) for relation or permission `perm`, built on the device from the resident forward CSR, one arrow level per
+ * launch sequence (DESIGN.md §2 "ExpandPermissionTree" for the tree's shape). Pending writes are published first;
+ * expired relationships are invisible at the engine's clock.
+ *   - Every node has an expanded object (object, of `slot`'s type) and relation (`slot`) and is an intermediate node
+ *     (ZG_EXPAND_UNION / INTERSECTION / EXCLUSION) or a leaf listing subjects[subjects, subjects + n_subjects): a
+ *     relation's live relationships in class order, then ascending id, userset subjects not expanded further.
+ *   - nodes[] holds the trees of the requests in order; a parent precedes its children, which rebuild the tree from
+ *     (parent, rank). parent is UINT32_MAX for a root and otherwise an index into nodes[]; otherwise the order is the
+ *     engine's, deterministic for one snapshot.
+ *   - status[i]: ZG_OK, or ZG_EDEPTH when the tree would hold a subtree reached through more than ZG_MAX_DEPTH arrows
+ *     (an arrow cycle); such a request contributes no node and the others are unaffected.
+ * Returns ZG_OK; ZG_E2BIG with *n_nodes / *n_subjects = the required sizes (a retry computes the trees again);
+ * ZG_EINVAL for an unknown slot, an id past the type's capacity, a slot whose tree template is too large, or a sharded
+ * handle / standalone shard; ZG_ENOMEM when the call's nodes plus subjects, with the jobs of the next arrow level or
+ * the (object, relation leaf or arrow) pairs of one level, pass the cap (ZGPU_EXPAND_CAP, default 2^26); ZG_ECUDA on a
+ * host-only engine. A multi-device engine answers on its first device. */
+#define ZG_EXPAND_UNION 1u /* v1 AlgebraicSubjectSet.Operation */
+#define ZG_EXPAND_INTERSECTION 2u
+#define ZG_EXPAND_EXCLUSION 3u
+#define ZG_EXPAND_LEAF 4u
+typedef struct {
+  uint16_t perm;
+  uint16_t pad;
+  uint32_t res; /* may be ZG_NO_OBJECT */
+} zg_expand_request;
+typedef struct {
+  uint32_t request, parent, rank; /* parent UINT32_MAX for a root; rank = position among the parent's children */
+  uint32_t object;
+  uint16_t slot, op;
+  uint32_t n_subjects;
+  uint64_t subjects; /* ZG_EXPAND_LEAF: its subjects[subjects, subjects + n_subjects) */
+} zg_expand_node;
+typedef struct {
+  uint32_t id;
+  uint16_t type, srel; /* srel: ZG_SREL_NONE, ZG_SREL_WILDCARD (id 0), or the userset's slot */
+} zg_expand_subject;
+int zg_expand_permission_trees(zg_engine *e, const zg_expand_request *reqs, uint64_t n, int32_t *status,
+                               zg_expand_node *nodes, uint64_t node_cap, uint64_t *n_nodes,
+                               zg_expand_subject *subjects, uint64_t subj_cap, uint64_t *n_subjects);
+/* String form of one tree: one '\n'-terminated line per node in pre-order, children in rank order:
+ * "<depth> <U|I|X|L> <type>:<id>#<relation>[ <subject>]*", depth = nesting depth (root 0), a subject written
+ * type:id, type:id#rel or type:*. A never-written res_id gives the tree with empty leaves. *n_lines = nodes,
+ * *need = bytes incl. NUL; ZG_E2BIG when cap is short; ZG_EDEPTH as status above; ZG_EINVAL for unknown names. */
+int zg_expand_permission_tree_str(zg_engine *e, const char *res_type, const char *res_id, const char *perm, char *buf,
+                                  size_t cap, size_t *need, uint64_t *n_lines);
+/* Cumulative counters of the engine's first device: out[0] trees answered, out[1] levels launched, out[2] nodes,
+ * out[3] subjects. */
+int zg_expand_counters(zg_engine *e, uint64_t *out);
+/* Device time of the last zg_expand_permission_trees call on the first device: per level, the count, scan and emit
+ * milliseconds (CUDA events), 3 per level. *n = values; ZG_E2BIG when cap is short. */
+int zg_expand_last_times(zg_engine *e, double *ms, uint64_t cap, uint64_t *n);
 /* Cumulative LookupResources counters of a sharded handle with ZG_FLAG_HANDLE_LOOKUPS (zeros on any other engine):
  * out[0] rounds begun on the shards (a round answers up to 64 lookups; a halved round counts its halves too), out[1]
  * walk levels expanded, out[2] times the host waited for the shards (the verification's included), out[3] frontier

@@ -27,6 +27,32 @@ TUPLE_DTYPE = np.dtype(
     [("res", "<u4"), ("subj", "<u4"), ("rel", "<u2"), ("stype", "<u2"), ("srel", "<u2"), ("flags", "<u2")]
 )
 
+EDEPTH = -9
+EXPAND_UNION, EXPAND_INTERSECTION, EXPAND_EXCLUSION, EXPAND_LEAF = 1, 2, 3, 4  # zg_expand_node.op
+EXPAND_REQUEST_DTYPE = np.dtype([("perm", "<u2"), ("pad", "<u2"), ("res", "<u4")])
+EXPAND_NODE_DTYPE = np.dtype([("request", "<u4"), ("parent", "<u4"), ("rank", "<u4"), ("object", "<u4"), ("slot", "<u2"),
+                              ("op", "<u2"), ("n_subjects", "<u4"), ("subjects", "<u8")])
+EXPAND_SUBJECT_DTYPE = np.dtype([("id", "<u4"), ("type", "<u2"), ("srel", "<u2")])
+_EXPAND_OP = {EXPAND_UNION: "U", EXPAND_INTERSECTION: "I", EXPAND_EXCLUSION: "X", EXPAND_LEAF: "L"}
+
+
+def parse_expand_lines(lines):
+    """zg_expand_permission_tree_str's lines -> nested tree: {"op": U|I|X|L, "object": "type:id", "relation": str,
+    "subjects": ["type:id", "type:id#rel", "type:*", ...], "children": [...]}."""
+    root, stack = None, []
+    for line in lines:
+        depth, op, node, *subjects = line.split(" ")
+        obj, _, rel = node.rpartition("#")
+        n = {"op": op, "object": obj, "relation": rel, "subjects": subjects, "children": []}
+        depth = int(depth)
+        del stack[depth:]
+        if stack:
+            stack[-1]["children"].append(n)
+        else:
+            root = n
+        stack.append(n)
+    return root
+
 
 class ZgpuError(RuntimeError):
     def __init__(self, code, msg):
@@ -206,6 +232,12 @@ _SIGS = {
     "zg_lookup_subjects_str": (C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_uint32,
                                          C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint64)]),
     "zg_lookup_subjects_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "zg_expand_permission_trees": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64,
+                                             C.POINTER(C.c_uint64), C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),
+    "zg_expand_permission_tree_str": (C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_size_t,
+                                                C.POINTER(C.c_size_t), C.POINTER(C.c_uint64)]),
+    "zg_expand_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "zg_expand_last_times": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),
     "zg_handle_lookup_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
     "zg_handle_subjects_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
     "zg_filter_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
@@ -904,6 +936,90 @@ class Engine:
         out = np.zeros(3, dtype=np.uint64)
         self._ck(self._L.zg_lookup_subjects_counters(self._h, out.ctypes.data))
         return {"walks": int(out[0]), "fallbacks": int(out[1]), "items_verified": int(out[2])}
+
+    def expand_permission_trees(self, requests, node_cap=1 << 12, subj_cap=1 << 14):
+        """ExpandPermissionTree by ids. requests: [(res_type, res id or NO_OBJECT, relation or permission)]. Returns one
+        entry per request: its tree, or the ZgpuError it failed with (ZG_EDEPTH). A tree node is {"op": U|I|X|L,
+        "type": str, "object": int, "relation": str, "subjects": [(type, id, srel)], "children": [...]}, children in
+        rank order, a subject's srel None (plain), "*" (wildcard, id 0) or the userset's relation name."""
+        reqs = np.zeros(len(requests), dtype=EXPAND_REQUEST_DTYPE)
+        for i, (rt, res, perm) in enumerate(requests):
+            p = self.slot_id(rt, perm)
+            if p < 0:
+                raise ZgpuError(-1, f"relation/permission `{perm}` not found under definition `{rt}`")
+            reqs[i] = (p, 0, int(res))
+        return self.expand_trees_from(reqs.size, *self.expand_permission_arrays(reqs, node_cap, subj_cap))
+
+    def expand_permission_arrays(self, reqs, node_cap=1 << 12, subj_cap=1 << 14, out=None):
+        """zg_expand_permission_trees on EXPAND_REQUEST_DTYPE requests -> (status, nodes, subjects) arrays. out: (nodes,
+        subjects) arrays to answer into (views of them are returned) while they are large enough."""
+        reqs = np.ascontiguousarray(reqs, dtype=EXPAND_REQUEST_DTYPE)
+        status = np.zeros(max(len(reqs), 1), dtype=np.int32)
+        while True:  # ZG_E2BIG reports both required sizes
+            if out is not None and out[0].size >= node_cap and out[1].size >= subj_cap:
+                nodes, subj = out
+                node_cap, subj_cap = nodes.size, subj.size
+            else:
+                nodes, subj = np.zeros(node_cap, dtype=EXPAND_NODE_DTYPE), np.zeros(subj_cap, dtype=EXPAND_SUBJECT_DTYPE)
+            nn, ns = C.c_uint64(0), C.c_uint64(0)
+            rc = self._L.zg_expand_permission_trees(self._h, reqs.ctypes.data, len(reqs), status.ctypes.data,
+                                                    nodes.ctypes.data, node_cap, C.byref(nn), subj.ctypes.data, subj_cap,
+                                                    C.byref(ns))
+            if rc == E2BIG:
+                node_cap, subj_cap = max(node_cap, int(nn.value)), max(subj_cap, int(ns.value))
+                continue
+            self._ck(rc)
+            return status, nodes[: nn.value], subj[: ns.value]
+
+    def expand_trees_from(self, n_requests, status, nodes, subj):
+        """zg_expand_permission_trees' arrays -> the nested trees of expand_permission_trees."""
+        slots = self.slot_table()
+        tnames = [self._L.zg_type_name(self._h, t).decode() for t in range(self._L.zg_num_types(self._h))]
+        out = [ZgpuError(int(status[i]), "ExpandPermissionTree: the tree passes the maximum depth")
+               if status[i] else None for i in range(n_requests)]
+        built = []
+        for nd in nodes:
+            _, t, rel, _ = slots[int(nd["slot"])]
+            b = int(nd["subjects"])
+            n = {"op": _EXPAND_OP[int(nd["op"])], "type": t, "object": int(nd["object"]), "relation": rel, "children": [],
+                 "subjects": [(tnames[int(x["type"])], int(x["id"]),
+                               None if x["srel"] == SREL_NONE else "*" if x["srel"] == SREL_WILDCARD else slots[int(x["srel"])][2])
+                              for x in subj[b: b + int(nd["n_subjects"])]], "_rank": int(nd["rank"])}
+            built.append(n)
+            if nd["parent"] == 0xFFFFFFFF:
+                out[int(nd["request"])] = n
+            else:
+                built[int(nd["parent"])]["children"].append(n)
+        for n in built:
+            n["children"].sort(key=lambda c: c["_rank"])
+        for n in built:
+            del n["_rank"]
+        return out
+
+    def expand_permission_tree_str(self, res_type, res_id, perm, cap=1 << 16):
+        """ExpandPermissionTree by names -> the lines of zg_expand_permission_tree_str (parse_expand_lines nests them)."""
+        while True:
+            buf = C.create_string_buffer(cap)
+            need, n = C.c_size_t(0), C.c_uint64(0)
+            rc = self._L.zg_expand_permission_tree_str(self._h, _b(res_type), _b(res_id), _b(perm), buf, cap, C.byref(need),
+                                                       C.byref(n))
+            if rc == E2BIG:
+                cap = need.value + 16
+                continue
+            self._ck(rc)
+            return [l for l in buf.value.decode().split("\n") if l]
+
+    def expand_counters(self) -> dict:
+        out = np.zeros(4, dtype=np.uint64)
+        self._ck(self._L.zg_expand_counters(self._h, out.ctypes.data))
+        return dict(zip(("trees", "levels", "nodes", "subjects"), (int(x) for x in out)))
+
+    def expand_last_times(self) -> np.ndarray:
+        """Per level of the last expand call: (count, scan, emit) device milliseconds."""
+        n = C.c_uint64(0)
+        out = np.zeros(3 * 64, dtype=np.float64)
+        self._ck(self._L.zg_expand_last_times(self._h, out.ctypes.data, out.size, C.byref(n)))
+        return out[: n.value].reshape(-1, 3)
 
     CLOSURE_INDEX_COUNTERS = ("indexed", "over_budget", "entries", "device_bytes", "builds", "last_build_us", "failures")
 

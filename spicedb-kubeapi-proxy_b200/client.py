@@ -12,6 +12,7 @@ these methods on it:
     WriteRelationships     pkg/authz/distributedtx/activity.go:60
     ReadRelationships      pkg/authz/distributedtx/activity.go:107,154
     DeleteRelationships    (v1 API; the proxy deletes by read-then-write, workflow.go:354-389)
+    ExpandPermissionTree   (v1 API; debugging tools: `zed permission expand`)
 
 Same method names, same request/response field names and the same error behaviour
 (per-pair errors inside a successful bulk response; a failed precondition fails the
@@ -36,6 +37,8 @@ PERMISSIONSHIP_CONDITIONAL_PERMISSION = 3
 LOOKUP_PERMISSIONSHIP_HAS_PERMISSION = 1
 # v1.LookupSubjectsRequest_WildcardOption
 WILDCARD_OPTION_UNSPECIFIED, WILDCARD_OPTION_INCLUDE_WILDCARDS, WILDCARD_OPTION_EXCLUDE_WILDCARDS = 0, 1, 2
+# v1.AlgebraicSubjectSet_Operation
+OPERATION_UNSPECIFIED, OPERATION_UNION, OPERATION_INTERSECTION, OPERATION_EXCLUSION = 0, 1, 2, 3
 # v1.RelationshipUpdate_Operation
 OPERATION_CREATE, OPERATION_TOUCH, OPERATION_DELETE = 1, 2, 3
 # v1.Precondition_Operation
@@ -161,6 +164,53 @@ class ResolvedSubject:
 class LookupSubjectsResponse:
     subject: ResolvedSubject
     excluded_subjects: List[ResolvedSubject] = field(default_factory=list)  # only on the wildcard
+
+
+@dataclass
+class ExpandPermissionTreeRequest:
+    resource: ObjectReference
+    permission: str
+    fully_consistent: bool = True
+
+
+@dataclass
+class DirectSubjectSet:
+    subjects: List[SubjectReference]
+
+
+@dataclass
+class AlgebraicSubjectSet:
+    operation: int
+    children: List["PermissionRelationshipTree"]
+
+
+@dataclass
+class PermissionRelationshipTree:
+    expanded_object: ObjectReference
+    expanded_relation: str
+    intermediate: Optional[AlgebraicSubjectSet] = None  # exactly one of intermediate and leaf is set
+    leaf: Optional[DirectSubjectSet] = None
+
+
+@dataclass
+class ExpandPermissionTreeResponse:
+    tree_root: PermissionRelationshipTree
+
+
+_EXPAND_OP = {"U": OPERATION_UNION, "I": OPERATION_INTERSECTION, "X": OPERATION_EXCLUSION}
+
+
+def _expand_tree(n: dict) -> PermissionRelationshipTree:
+    obj = ObjectReference(*n["object"].split(":", 1))
+    if n["op"] == "L":
+        subjects = []
+        for x in n["subjects"]:
+            t, rest = x.split(":", 1)
+            sid, _, srel = rest.partition("#")
+            subjects.append(SubjectReference(ObjectReference(t, sid), srel))
+        return PermissionRelationshipTree(obj, n["relation"], leaf=DirectSubjectSet(subjects))
+    return PermissionRelationshipTree(obj, n["relation"], intermediate=AlgebraicSubjectSet(
+        _EXPAND_OP[n["op"]], [_expand_tree(c) for c in n["children"]]))
 
 
 @dataclass
@@ -360,6 +410,15 @@ class PermissionsClient:
         if wild:
             out.append(LookupSubjectsResponse(ResolvedSubject("*"), [ResolvedSubject(x) for x in excluded]))
         return iter(out)
+
+    def ExpandPermissionTree(self, req: ExpandPermissionTreeRequest) -> ExpandPermissionTreeResponse:
+        """The permission's subject tree at the resource, one level of usersets deep (v1's shallow expansion): leaves
+        list the relationships' subjects, arrows expand into the subtrees of their targets."""
+        try:
+            lines = self.engine.expand_permission_tree_str(req.resource.object_type, req.resource.object_id, req.permission)
+        except ZgpuError as e:
+            raise _rpc(e) from None
+        return ExpandPermissionTreeResponse(_expand_tree(_lib.parse_expand_lines(lines)))
 
     # -- relationships ------------------------------------------------------------
     def WriteRelationships(self, req: WriteRelationshipsRequest) -> WriteRelationshipsResponse:

@@ -341,6 +341,8 @@ static const char* kHandleShardCallMsg =
 static const char* kHandleSubjectsMsg =
     "sharded handle (zg_config.n_shards > 1): LookupSubjects is not served by it, with or without "
     "ZG_FLAG_HANDLE_LOOKUPS; run it on one engine per shard (dist.DeviceShardedLookup) or on a replica";
+static const char* kHandleExpandMsg =
+    "sharded handle (zg_config.n_shards > 1): ExpandPermissionTree is not served by it; run it on a replica";
 static bool is_handle(const zg_engine* e) { return e->n_shards > 1; }
 // a sharded handle that answers LookupSubjects itself (run_sharded_subjects)
 static bool serves_subjects(const zg_engine* e) { return is_handle(e) && e->handle_subjects; }
@@ -361,6 +363,7 @@ enum class Call {
   kCheckGroup,     // a check group of zg_check_bulk, and the string calls that publish before queueing one
   kLookup,         // LookupResources and the list pre-filter
   kSubjects,       // LookupSubjects
+  kExpand,         // ExpandPermissionTree
   kShardCall,      // zg_shard_*_dev: one shard per engine, driven by dist.py
 };
 
@@ -377,6 +380,7 @@ static int refuse(const zg_engine* e, Call c, std::string* msg = nullptr) {
       case Call::kLookup: why = e->handle_lookups ? nullptr : kHandleLookupMsg; break;
       case Call::kSubjects: why = e->handle_subjects ? nullptr : e->handle_lookups ? kHandleSubjectsMsg : kHandleLookupMsg; break;
       case Call::kShardCall: why = kHandleShardCallMsg; break;
+      case Call::kExpand: why = kHandleExpandMsg; break;
       default: break;
     }
   } else if (e->dev.shard_count > 1 && c != Call::kDevice && c != Call::kDeviceBuffers && c != Call::kShardCall) {
@@ -3696,6 +3700,154 @@ extern "C" int zg_lookup_subjects_counters(zg_engine* e, uint64_t* out) {
   out[0] = e->dev.subject_lookups_walk;
   out[1] = e->dev.subject_lookups_exhaustive;
   out[2] = e->dev.subject_items_verified;
+  return ZG_OK;
+}
+
+// ExpandPermissionTree (Device::expand). Arguments are checked before anything else, against the ids handed out so far
+// (a host-only engine still reports ZG_EINVAL for them); then, as for LookupSubjects, the device lock (FIFO), pending
+// writes published, and the first device answers at the engine's clock.
+static int expand_ids(zg_engine* e, const zg_expand_request* reqs, uint64_t n, std::vector<int32_t>* status,
+                      std::vector<zg_expand_node>* nodes, std::vector<zg_expand_subject>* subjects) {
+  const Schema& sc = e->schema;
+  std::vector<Device::ExpandReq> xr(n);
+  {
+    LOCK_NAMES_SHARED(e);
+    for (uint64_t i = 0; i < n; ++i) {
+      const zg_expand_request& r = reqs[i];
+      if (r.perm >= sc.slots.size()) return fail(ZG_EINVAL, "request " + std::to_string(i) + ": unknown relation or permission");
+      const SlotInfo& si = sc.slots[r.perm];
+      const std::string what = sc.types[si.type].name + "#" + si.name;
+      if (!sc.x_ok[r.perm])
+        return fail(ZG_EINVAL, "request " + std::to_string(i) + ": the tree of " + what + " has more than " +
+                                   std::to_string(kMaxExpandTemplate) + " nodes per object");
+      if (r.res != ZG_NO_OBJECT && r.res >= std::max(e->store.capacity(si.type), e->store.extent(si.type)))
+        return fail(ZG_EINVAL, "request " + std::to_string(i) + ": object id " + std::to_string(r.res) +
+                                   " is past the capacity of " + sc.types[si.type].name);
+      xr[i] = Device::ExpandReq{r.res, sc.x_root[r.perm], sc.x_nodes[sc.x_root[r.perm]].ncount};
+    }
+  }
+  if (int rc = refuse(e, Call::kExpand)) return rc;
+  uint64_t cap = 1ull << 26;
+  if (const char* v = std::getenv("ZGPU_EXPAND_CAP")) cap = std::strtoull(v, nullptr, 10);
+  LOCK_DEVICE(e);
+  if (e->dirty.load() || !e->dev.snap) {
+    LOCK_NAMES_UNIQUE(e);
+    int rc = publish_locked(e);
+    if (rc) return rc;
+  }
+  e->dev.now = now_of(e);
+  std::string err;
+  const int rc = e->dev.expand(xr, cap, nodes, subjects, status, &err);
+  return rc ? fail(rc, err) : ZG_OK;
+}
+
+extern "C" int zg_expand_permission_trees(zg_engine* e, const zg_expand_request* reqs, uint64_t n, int32_t* status,
+                                          zg_expand_node* nodes, uint64_t node_cap, uint64_t* n_nodes,
+                                          zg_expand_subject* subjects, uint64_t subj_cap, uint64_t* n_subjects) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (!n_nodes || !n_subjects || (n && (!reqs || !status))) return fail(ZG_EINVAL, "NULL argument");
+  std::vector<int32_t> st;
+  std::vector<zg_expand_node> nv;
+  std::vector<zg_expand_subject> sv;
+  if (int rc = expand_ids(e, reqs, n, &st, &nv, &sv)) return rc;
+  *n_nodes = nv.size();
+  *n_subjects = sv.size();
+  if (nv.size() > node_cap || sv.size() > subj_cap || (!nodes && !nv.empty()) || (!subjects && !sv.empty()))
+    return fail(ZG_E2BIG, "output buffers too small");
+  if (n) std::memcpy(status, st.data(), n * sizeof(int32_t));
+  if (!nv.empty()) std::memcpy(nodes, nv.data(), nv.size() * sizeof(zg_expand_node));
+  if (!sv.empty()) std::memcpy(subjects, sv.data(), sv.size() * sizeof(zg_expand_subject));
+  return ZG_OK;
+}
+
+static int expand_str_once(zg_engine* e, const char* res_type, const char* res_id, const char* perm, char* buf, size_t cap,
+                           size_t* need, uint64_t* n_lines) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (!res_type || !res_id || !perm) return fail(ZG_EINVAL, "NULL argument");
+  zg_expand_request r{};
+  {
+    LOCK_NAMES_SHARED(e);
+    const Schema& sc = e->schema;
+    const int rt = sc.type_id(res_type);
+    if (rt < 0) return fail(ZG_EINVAL, std::string("object definition `") + res_type + "` not found");
+    const int p = sc.slot_id(rt, perm);
+    if (p < 0) return fail(ZG_EINVAL, std::string("relation/permission `") + perm + "` not found under definition `" + res_type + "`");
+    r.perm = static_cast<uint16_t>(p);
+    r.res = e->store.find(rt, res_id);
+  }
+  std::vector<int32_t> st;
+  std::vector<zg_expand_node> nv;
+  std::vector<zg_expand_subject> sv;
+  if (int rc = expand_ids(e, &r, 1, &st, &nv, &sv)) return rc;
+  if (st[0] == ZG_EDEPTH)
+    return fail(ZG_EDEPTH, std::string("ExpandPermissionTree: the tree of ") + res_type + ":" + res_id + "#" + perm +
+                               " passes the maximum depth (" + std::to_string(ZG_MAX_DEPTH) + " arrow hops)");
+  if (e->resolve_hook) e->resolve_hook(e->resolve_hook_arg);
+  // children in rank order; a parent precedes its children, so one pass fills every list
+  std::vector<std::vector<uint32_t>> kids(nv.size());
+  for (size_t i = 0; i < nv.size(); ++i)
+    if (nv[i].parent != UINT32_MAX) {
+      auto& k = kids[nv[i].parent];
+      if (k.size() <= nv[i].rank) k.resize(nv[i].rank + 1, UINT32_MAX);
+      k[nv[i].rank] = static_cast<uint32_t>(i);
+    }
+  std::string out;
+  {
+    LOCK_NAMES_SHARED(e);
+    const Schema& sc = e->schema;
+    auto name = [&](int t, uint32_t id) {
+      if (id == ZG_NO_OBJECT) return std::string(res_id);  // the never-written resource and its same-object nodes
+      std::string_view n;
+      return e->store.name(t, id, &n) ? std::string(n) : std::to_string(id);
+    };
+    static const char kOp[] = "?UIXL";
+    std::vector<std::pair<uint32_t, uint32_t>> stack;  // node, depth
+    if (!nv.empty()) stack.push_back({0, 0});
+    while (!stack.empty()) {
+      const auto [i, d] = stack.back();
+      stack.pop_back();
+      const zg_expand_node& o = nv[i];
+      const SlotInfo& si = sc.slots[o.slot];
+      out += std::to_string(d) + " " + kOp[o.op <= 4 ? o.op : 0] + " " + sc.types[si.type].name + ":" + name(si.type, o.object) +
+             "#" + si.name;
+      for (uint64_t j = o.subjects; j < o.subjects + o.n_subjects; ++j) {
+        const zg_expand_subject& x = sv[j];
+        out += " " + sc.types[x.type].name + ":" + (x.srel == kWildcard ? std::string("*") : name(x.type, x.id));
+        if (x.srel != kWildcard && x.srel != kNone) out += "#" + sc.slots[x.srel].name;
+      }
+      out += "\n";
+      for (auto it = kids[i].rbegin(); it != kids[i].rend(); ++it) stack.push_back({*it, d + 1});
+    }
+  }
+  if (need) *need = out.size() + 1;
+  if (n_lines) *n_lines = nv.size();
+  if (out.size() + 1 > cap || !buf) return fail(ZG_E2BIG, "output buffer too small");
+  std::memcpy(buf, out.c_str(), out.size() + 1);
+  return ZG_OK;
+}
+
+extern "C" int zg_expand_permission_tree_str(zg_engine* e, const char* res_type, const char* res_id, const char* perm,
+                                             char* buf, size_t cap, size_t* need, uint64_t* n_lines) {
+  return with_stable_names(e, [&] { return expand_str_once(e, res_type, res_id, perm, buf, cap, need, n_lines); });
+}
+
+extern "C" int zg_expand_counters(zg_engine* e, uint64_t* out) {
+  if (!e || !out) return fail(ZG_EINVAL, "NULL argument");
+  LOCK_DEVICE(e);
+  out[0] = e->dev.x_trees;
+  out[1] = e->dev.x_levels;
+  out[2] = e->dev.x_nodes_out;
+  out[3] = e->dev.x_subjects_out;
+  return ZG_OK;
+}
+
+extern "C" int zg_expand_last_times(zg_engine* e, double* ms, uint64_t cap, uint64_t* n) {
+  if (!e || !n) return fail(ZG_EINVAL, "NULL argument");
+  LOCK_DEVICE(e);
+  const auto& t = e->dev.x_last_ms;
+  *n = t.size();
+  if (t.size() > cap || (!ms && !t.empty())) return fail(ZG_E2BIG, "output buffer too small");
+  if (!t.empty()) std::memcpy(ms, t.data(), t.size() * sizeof(double));
   return ZG_OK;
 }
 

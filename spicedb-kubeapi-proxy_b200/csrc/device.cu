@@ -14,6 +14,7 @@
 
 #include <cub/cub.cuh>
 
+#include "expand.cuh"
 #include "filter.cuh"
 #include "import.cuh"
 #include "ingress.cuh"
@@ -90,6 +91,7 @@ Snapshot::~Snapshot() {
   ls_fwd.release();
   ls_type_off.release();
   ls_mask.release();
+  for (DevBuf* b : {&x_nodes, &x_tgts, &x_counted, &x_rels, &x_cls}) b->release();
   for (auto& c : closure) {
     c.row_ptr.release();
     c.col.release();
@@ -448,6 +450,9 @@ std::string Device::finish_publish(std::shared_ptr<Snapshot> s, const HostSnapsh
     s->ls_mask_words = sc.fwd_mask_words;
     if (ok) ok = up(s->ls_fwd, fwd.data(), fwd.size() * sizeof(FwdClass)) && up(s->ls_type_off, type_off.data(), type_off.size() * 4) &&
                  up(s->ls_mask, sc.fwd_mask.data(), sc.fwd_mask.size() * 4);
+    if (ok) ok = up(s->x_nodes, sc.x_nodes.data(), sc.x_nodes.size() * sizeof(XNode)) &&
+                 up(s->x_tgts, sc.x_tgts.data(), sc.x_tgts.size() * 4) && up(s->x_counted, sc.x_counted.data(), sc.x_counted.size() * 4) &&
+                 up(s->x_rels, h.rels.data(), h.rels.size() * sizeof(DRel)) && up(s->x_cls, h.cls.data(), h.cls.size() * sizeof(DCls));
   }
   if (!ok || cudaStreamSynchronize(stream) != cudaSuccess)
     return std::string("snapshot upload failed: ") + cudaGetErrorString(cudaGetLastError());
@@ -3645,6 +3650,166 @@ int Device::import_finish(const std::vector<uint32_t>& ids, const std::vector<ui
   ++launches;
   ZG_CUDA(cudaMemcpyAsync(tuples->data(), x.tuples.p, x.n * sizeof(zg_tuple), cudaMemcpyDeviceToHost, stream));
   ZG_CUDA(cudaStreamSynchronize(stream));
+  return ZG_OK;
+}
+
+int Device::expand(const std::vector<ExpandReq>& reqs, uint64_t cap, std::vector<zg_expand_node>* nodes,
+                   std::vector<zg_expand_subject>* subjects, std::vector<int32_t>* status, std::string* err) {
+  nodes->clear();
+  subjects->clear();
+  status->assign(reqs.size(), ZG_OK);
+  x_last_ms.clear();
+  std::shared_ptr<Snapshot> s = snap;
+  if (!s) {
+    if (err) *err = "no snapshot published";
+    return ZG_ENOSNAPSHOT;
+  }
+  if (reqs.empty()) return ZG_OK;
+  ZG_CUDA(cudaSetDevice(device));
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  // An Expand is a rare debugging call whose output can be large: its scratch is freed when it returns.
+  struct Scratch {
+    DevBuf jobs[2], failed, cnt, off, cub, nodes, subj, mask;
+    std::vector<cudaEvent_t> ev;
+    ~Scratch() {
+      for (DevBuf* b : {&jobs[0], &jobs[1], &failed, &cnt, &off, &cub, &nodes, &subj, &mask}) b->release();
+      for (cudaEvent_t e : ev) cudaEventDestroy(e);
+    }
+  } x;
+  auto oom = [&](const char* what) {
+    if (err) *err = std::string("out of device memory (ExpandPermissionTree ") + what + ")";
+    return ZG_ENOMEM;
+  };
+  // grows b to `want` bytes, keeping its first `used`
+  auto grow = [&](DevBuf& b, size_t used, size_t want) -> bool {
+    if (want <= b.cap) return true;
+    DevBuf nb;
+    if (!nb.ensure(std::max(want, b.cap * 2))) return false;
+    if (used && cudaMemcpyAsync(nb.p, b.p, used, cudaMemcpyDeviceToDevice, stream) != cudaSuccess) {
+      nb.release();
+      return false;
+    }
+    b.release();  // cudaFree waits for the copy
+    b = nb;
+    return true;
+  };
+  const uint64_t R = reqs.size();
+  unsigned long long mask = 0;  // bit c: a job of the level has a template of c counted nodes
+  {
+    std::vector<XJob> j0(R);
+    for (uint64_t i = 0; i < R; ++i) {
+      j0[i] = XJob{static_cast<uint32_t>(i), UINT32_MAX, 0, reqs[i].res, reqs[i].tmpl, 0};
+      mask |= 1ull << reqs[i].ncount;
+    }
+    if (!x.jobs[0].ensure(R * sizeof(XJob)) || !x.failed.ensure(R * 4) || !x.mask.ensure(8)) return oom("jobs");
+    ZG_CUDA(cudaMemcpyAsync(x.jobs[0].p, j0.data(), R * sizeof(XJob), cudaMemcpyHostToDevice, stream));
+    ZG_CUDA(cudaMemsetAsync(x.failed.p, 0, R * 4, stream));
+  }
+  XParams p{};
+  p.row_ptr = s->row_ptr.as<uint32_t>();
+  p.col = s->col.as<uint32_t>();
+  p.exp = s->exp.p ? s->exp.as<uint32_t>() : nullptr;
+  p.rels = s->x_rels.as<DRel>();
+  p.cls = s->x_cls.as<DCls>();
+  p.nodes = s->x_nodes.as<XNode>();
+  p.tgts = s->x_tgts.as<uint32_t>();
+  p.counted = s->x_counted.as<uint32_t>();
+  p.now = now;
+  p.failed = x.failed.as<uint32_t>();
+  p.next_mask = x.mask.as<unsigned long long>();
+  auto over_cap = [&]() {
+    if (err)
+      *err = "ExpandPermissionTree: the trees pass " + std::to_string(cap) +
+             " nodes plus subjects (ZGPU_EXPAND_CAP); expand fewer or smaller trees per call";
+    return ZG_ENOMEM;
+  };
+  uint64_t n_jobs = R, n_nodes = 0, n_subj = 0, levels = 0;
+  int cur = 0;
+  while (n_jobs) {
+    p.m = expand_warps(mask);
+    // every (job, counted node) is a node of the output: the level's scratch stays within the cap's size
+    if (n_nodes + n_subj + n_jobs * p.m > cap) return over_cap();
+    const uint64_t n = n_jobs * p.m;
+    if (!x.cnt.ensure((3 * n + 1) * 8) || !x.off.ensure((3 * n + 1) * 8)) return oom("counts");
+    unsigned long long* cnt = x.cnt.as<unsigned long long>();
+    unsigned long long* off = x.off.as<unsigned long long>();
+    size_t tb = 0;
+    ZG_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt, off, 3 * n + 1, stream));
+    if (!x.cub.ensure(tb)) return oom("scan");
+    while (x.ev.size() < 5 * (levels + 1)) {  // count, scan, emit: begin and end (emit after the allocations)
+      cudaEvent_t e;
+      ZG_CUDA(cudaEventCreate(&e));
+      x.ev.push_back(e);
+    }
+    cudaEvent_t* ev = x.ev.data() + 5 * levels;
+    ZG_CUDA(cudaMemsetAsync(cnt + 3 * n, 0, 8, stream));
+    p.jobs = x.jobs[cur].as<XJob>();
+    p.n_jobs = n_jobs;
+    p.cnt = cnt;
+    p.off = off;
+    const unsigned blocks = static_cast<unsigned>((n * 32 + kExpandThreads - 1) / kExpandThreads);
+    ZG_CUDA(cudaEventRecord(ev[0], stream));
+    expand_count_kernel<<<blocks, kExpandThreads, 0, stream>>>(p);
+    ZG_CUDA(cudaGetLastError());
+    ZG_CUDA(cudaEventRecord(ev[1], stream));
+    ZG_CUDA(cub::DeviceScan::ExclusiveSum(x.cub.p, tb, cnt, off, 3 * n + 1, stream));
+    ZG_CUDA(cudaEventRecord(ev[2], stream));
+    unsigned long long tot[3];
+    for (int i = 0; i < 3; ++i)
+      ZG_CUDA(cudaMemcpyAsync(tot + i, off + (i + 1) * n, 8, cudaMemcpyDeviceToHost, stream));
+    ZG_CUDA(cudaStreamSynchronize(stream));
+    const uint64_t lvl_nodes = tot[0], lvl_subj = tot[1] - tot[0], next = tot[2] - tot[1];
+    // each next-level job is at least one node
+    if (n_nodes + lvl_nodes + n_subj + lvl_subj + next > cap) return over_cap();
+    if (!grow(x.nodes, n_nodes * sizeof(zg_expand_node), (n_nodes + lvl_nodes) * sizeof(zg_expand_node)) ||
+        !grow(x.subj, n_subj * sizeof(zg_expand_subject), (n_subj + lvl_subj) * sizeof(zg_expand_subject)) ||
+        !x.jobs[cur ^ 1].ensure(next * sizeof(XJob)))
+      return oom("output");
+    p.node_base = n_nodes;
+    p.subj_base = n_subj;
+    p.out_nodes = x.nodes.as<zg_expand_node>();
+    p.out_subj = x.subj.as<zg_expand_subject>();
+    p.next = x.jobs[cur ^ 1].as<XJob>();
+    ZG_CUDA(cudaMemsetAsync(p.next_mask, 0, 8, stream));
+    ZG_CUDA(cudaEventRecord(ev[3], stream));
+    expand_emit_kernel<<<blocks, kExpandThreads, 0, stream>>>(p);
+    ZG_CUDA(cudaGetLastError());
+    ZG_CUDA(cudaEventRecord(ev[4], stream));
+    if (next) {
+      ZG_CUDA(cudaMemcpyAsync(&mask, p.next_mask, 8, cudaMemcpyDeviceToHost, stream));
+      ZG_CUDA(cudaStreamSynchronize(stream));
+    }
+    launches += 2;
+    n_nodes += lvl_nodes;
+    n_subj += lvl_subj;
+    n_jobs = next;
+    cur ^= 1;
+    ++levels;
+  }
+  std::vector<uint32_t> failed(R);
+  nodes->resize(n_nodes);
+  subjects->resize(n_subj);
+  if (n_nodes) ZG_CUDA(cudaMemcpyAsync(nodes->data(), x.nodes.p, n_nodes * sizeof(zg_expand_node), cudaMemcpyDeviceToHost, stream));
+  if (n_subj) ZG_CUDA(cudaMemcpyAsync(subjects->data(), x.subj.p, n_subj * sizeof(zg_expand_subject), cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaMemcpyAsync(failed.data(), x.failed.p, R * 4, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  for (uint64_t l = 0; l < levels; ++l)
+    for (int i : {0, 1, 3}) {
+      float ms = 0;
+      cudaEventElapsedTime(&ms, x.ev[5 * l + i], x.ev[5 * l + i + 1]);
+      x_last_ms.push_back(ms);
+    }
+  bool any_failed = false;
+  for (uint64_t i = 0; i < R; ++i)
+    if (failed[i]) {
+      (*status)[i] = ZG_EDEPTH;
+      any_failed = true;
+    }
+  if (any_failed) expand_drop_failed(failed, nodes, subjects);
+  for (uint64_t i = 0; i < R; ++i) x_trees += failed[i] ? 0 : 1;
+  x_levels += levels;
+  x_nodes_out += nodes->size();
+  x_subjects_out += subjects->size();
   return ZG_OK;
 }
 

@@ -50,6 +50,8 @@ struct Snapshot {
   // LookupSubjects' forward walk: Schema::forward_tables / fwd_mask of this layout
   DevBuf ls_fwd, ls_type_off, ls_mask;
   uint32_t ls_mask_words = 1;
+  // ExpandPermissionTree (expand.cuh): the schema's templates (Schema::x_*) and this layout's relation and class tables
+  DevBuf x_nodes, x_tgts, x_counted, x_rels, x_cls;
   std::vector<uint64_t> n_resources;
   uint32_t prog_bytes = 0;
   uint32_t max_leaves = 1;
@@ -364,6 +366,21 @@ class Device {
                          const char* subj_ids, const uint32_t* subj_off, uint64_t n, uint8_t* out, std::string* err);
   void ingress_reset() { ingress_.reset(); }  // a schema (re)load: the names are gone
   std::unique_ptr<IngressMirror> ingress_;     // nullptr until the first device-ingress call
+
+  // ---- ExpandPermissionTree (expand.cuh) ----
+  struct ExpandReq {
+    uint32_t res;   // ZG_NO_OBJECT or past the snapshot's objects: a never-written object
+    uint32_t tmpl;    // the slot's template root (Schema::x_root)
+    uint32_t ncount;  // its counted (relation leaf / arrow) nodes
+  };
+  // The trees of reqs, level by level: *nodes / *subjects as zg_expand_permission_trees returns them (the failed
+  // requests' nodes compacted away), (*status)[i] = ZG_OK / ZG_EDEPTH. ZG_ENOMEM when the nodes plus subjects of the
+  // call, with the next level's jobs and a level's (job, counted node) pairs, pass `cap`. The scratch is freed before
+  // returning.
+  int expand(const std::vector<ExpandReq>& reqs, uint64_t cap, std::vector<zg_expand_node>* nodes,
+             std::vector<zg_expand_subject>* subjects, std::vector<int32_t>* status, std::string* err);
+  uint64_t x_trees = 0, x_levels = 0, x_nodes_out = 0, x_subjects_out = 0;
+  std::vector<double> x_last_ms;  // the last call: per level, count, scan and emit milliseconds (CUDA events)
 
   // ---- zg_import_relationships (import.cuh) ----
   // One group of an import, its literal fields resolved on the host (HOST blobs and offsets, as the caller passed them).

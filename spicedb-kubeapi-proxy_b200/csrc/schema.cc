@@ -592,7 +592,145 @@ std::string Schema::compile() {
     d_type_rcls[t].end = static_cast<uint16_t>(d_rcls.size());
   }
   compute_forward_masks();
+  compute_expand_templates();
   return "";
+}
+
+// The tree of Expand(T:r, P) restricted to what r's own rows decide (DESIGN.md §2, "ExpandPermissionTree"): a chain of
+// + or & is one n-ary node, - stays binary, a bare operand is a one-child union, a same-object reference is the
+// referenced slot's subtree and an arrow is a node whose children the next level expands.
+void Schema::compute_expand_templates() {
+  const size_t ns = slots.size();
+  x_nodes.clear();
+  x_tgts.clear();
+  x_counted.clear();
+  x_root.assign(ns, kNoTemplate);
+  x_ok.assign(ns, 0);
+  for (size_t s = 0; s < ns; ++s) {
+    std::vector<XNode> t;
+    std::vector<uint8_t> kids;
+    std::vector<std::vector<uint32_t>> tgts;  // per node: the arrow's target slot per class
+    bool over = false;
+    auto add = [&](uint16_t op, int slot, int parent) -> int {
+      if (t.size() >= static_cast<size_t>(kMaxExpandTemplate)) {
+        over = true;
+        return -1;
+      }
+      XNode n{};
+      n.op = op;
+      n.slot = static_cast<uint16_t>(slot);
+      if (parent >= 0) {
+        n.parent = static_cast<uint8_t>(parent);
+        n.rank = kids[parent]++;
+      }
+      t.push_back(n);
+      kids.push_back(0);
+      tgts.emplace_back();
+      return static_cast<int>(t.size()) - 1;
+    };
+    std::function<void(int, int)> of_slot;
+    std::function<void(int, int, int)> of_expr, operand;
+    auto flatten = [&](int e, Expr::Kind k, std::vector<int>* out) {
+      std::function<void(int)> go = [&](int x) {
+        if (exprs[x].kind == k) {
+          go(exprs[x].l);
+          go(exprs[x].r);
+        } else {
+          out->push_back(x);
+        }
+      };
+      go(e);
+    };
+    of_slot = [&](int slot, int parent) {
+      if (over) return;
+      const SlotInfo& si = slots[slot];
+      if (!si.is_perm) {
+        const int n = add(X_REL, slot, parent);
+        if (n >= 0) t[n].rel = static_cast<uint16_t>(si.rel_index);
+        return;
+      }
+      of_expr(si.expr, slot, parent);
+    };
+    of_expr = [&](int e, int at, int parent) {
+      if (over) return;
+      const Expr& x = exprs[e];
+      if (x.kind == Expr::UNION || x.kind == Expr::INTER) {
+        const int n = add(x.kind == Expr::UNION ? X_UNION : X_INTER, at, parent);
+        std::vector<int> ops;
+        flatten(e, x.kind, &ops);
+        for (int o : ops) operand(o, at, n);
+      } else if (x.kind == Expr::EXCL) {
+        const int n = add(X_EXCL, at, parent);
+        operand(x.l, at, n);
+        operand(x.r, at, n);
+      } else {
+        operand(e, at, add(X_UNION, at, parent));
+      }
+    };
+    operand = [&](int e, int at, int parent) {
+      if (over) return;
+      const Expr& x = exprs[e];
+      switch (x.kind) {
+        case Expr::REF: of_slot(x.slot, parent); break;
+        case Expr::NIL: add(X_NIL, at, parent); break;
+        case Expr::ARROW: {
+          const int n = add(X_ARROW, at, parent);
+          if (n < 0) return;
+          t[n].rel = static_cast<uint16_t>(slots[x.slot].rel_index);
+          for (const ClassInfo& c : slots[x.slot].classes) {
+            const int target = c.sslot == kWildcard ? -1 : slot_by_name_id(c.stype, x.name);
+            tgts[n].push_back(target < 0 ? kNoTemplate : static_cast<uint32_t>(target));
+          }
+          break;
+        }
+        default: of_expr(e, at, parent);
+      }
+    };
+    of_slot(static_cast<int>(s), -1);
+    if (over) continue;
+    const uint32_t base = static_cast<uint32_t>(x_nodes.size());
+    t[0].size = static_cast<uint8_t>(t.size());
+    t[0].counted = static_cast<uint32_t>(x_counted.size());
+    for (size_t i = 0; i < t.size(); ++i) {
+      if (t[i].op == X_REL || t[i].op == X_ARROW) {
+        t[i].count = t[0].ncount++;
+        x_counted.push_back(static_cast<uint32_t>(i));
+      }
+      if (t[i].op == X_ARROW) {
+        t[i].tgt = static_cast<uint32_t>(x_tgts.size());
+        x_tgts.insert(x_tgts.end(), tgts[i].begin(), tgts[i].end());  // slots for now: roots below
+      }
+    }
+    x_nodes.insert(x_nodes.end(), t.begin(), t.end());
+    x_root[s] = base;
+    x_ok[s] = 1;
+  }
+  // a slot is expandable when its template and every template its arrows reach fit
+  for (bool changed = true; changed;) {
+    changed = false;
+    for (size_t s = 0; s < ns; ++s) {
+      if (!x_ok[s]) continue;
+      const XNode* t = x_nodes.data() + x_root[s];
+      for (uint32_t i = 0; i < t[0].size && x_ok[s]; ++i) {
+        if (t[i].op != X_ARROW) continue;
+        for (size_t k = 0; k < slots[rel_slots[t[i].rel]].classes.size(); ++k) {
+          const uint32_t target = x_tgts[t[i].tgt + k];
+          if (target != kNoTemplate && !x_ok[target]) {
+            x_ok[s] = 0;
+            changed = true;
+            break;
+          }
+        }
+      }
+    }
+  }
+  for (XNode& n : x_nodes) {
+    if (n.op != X_ARROW) continue;
+    for (size_t k = 0; k < slots[rel_slots[n.rel]].classes.size(); ++k) {
+      uint32_t& target = x_tgts[n.tgt + k];
+      if (target != kNoTemplate) target = x_root[target];
+    }
+  }
 }
 
 void Schema::compute_forward_masks() {

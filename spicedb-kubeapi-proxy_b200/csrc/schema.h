@@ -122,6 +122,25 @@ struct FwdClass {  // LookupSubjects' forward walk: one non-wildcard edge class,
 struct DTypeInv {  // per subject type: the invertible direct classes (inv_cls[begin, end))
   uint16_t begin, end;
 };
+// ExpandPermissionTree (expand.cuh): every slot lowered into a pre-order template of the tree one object contributes.
+// Same-object references are inlined; arrows end the template, their children are the next level's jobs.
+enum XOpKind : uint16_t { X_UNION = 1, X_INTER = 2, X_EXCL = 3, X_REL = 4, X_NIL = 5, X_ARROW = 6 };
+constexpr int kMaxExpandTemplate = 32;  // nodes of one template: a warp writes them, one per lane
+struct XNode {
+  uint16_t op;      // XOpKind
+  uint16_t slot;    // the expanded relation
+  uint8_t parent;   // template index of the parent (0 at the root, which has none)
+  uint8_t rank;     // position among the parent's children
+  uint8_t count;    // X_REL / X_ARROW: index among the template's counted nodes
+  uint8_t size;     // root only: nodes of the template
+  uint8_t ncount;   // root only: counted (X_REL / X_ARROW) nodes
+  uint8_t pad;
+  uint16_t rel;     // X_REL: data relation; X_ARROW: the tupleset's data relation
+  uint32_t tgt;     // X_ARROW: x_tgts[tgt + k] = template root of class k's target, kNoTemplate: an empty leaf
+  uint32_t counted; // root only: x_counted[counted + i] = template index of counted node i
+};
+constexpr uint32_t kNoTemplate = 0xFFFFFFFFu;
+
 struct DTree {   // postfix boolean program of a non-pure permission
   uint16_t op_begin, op_end;     // into tree_ops[]
   uint16_t leaf_begin, n_leaves; // leaf_units[leaf_begin + i] = unit id
@@ -215,9 +234,15 @@ class Schema {
   // Per resource type, its relations' non-wildcard classes with their rows in this snapshot's layout:
   // fwd[type_off[t], type_off[t + 1]).
   void forward_tables(const std::vector<DRel>& rels, std::vector<FwdClass>* fwd, std::vector<uint32_t>* type_off) const;
+  // ExpandPermissionTree templates (XNode): x_root[slot] = root of the slot's template in x_nodes. x_ok[slot] = 0 when
+  // its template, or one an arrow of it reaches, has more than kMaxExpandTemplate nodes: expanding it is refused.
+  std::vector<XNode> x_nodes;
+  std::vector<uint32_t> x_tgts, x_counted, x_root;
+  std::vector<uint8_t> x_ok;
 
  private:
   void compute_forward_masks();
+  void compute_expand_templates();
   std::string compile();
   int name_id(const std::string& n);
 };
