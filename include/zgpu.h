@@ -614,6 +614,16 @@ int zg_closure_table_info(zg_engine *e, uint32_t pair, uint64_t *out);
 int zg_closure_table_copy(zg_engine *e, uint32_t pair, uint64_t *hdr, uint64_t hdr_cap, uint64_t *buckets,
                           uint64_t bucket_cap, uint64_t *n_rows, uint64_t *n_buckets);
 
+/* Range records `k` (the lean check kernel loads a range's children from them, by object, instead of through the
+ * range's offsets): out[0] 1 when built, out[1] the edge class, out[2] objects, out[3] device bytes, out[4] rows longer
+ * than a record holds (read through their offsets), out[5] device microseconds of their last build. ZG_EINVAL when
+ * there are no such records. */
+int zg_flat_record_info(zg_engine *e, uint32_t k, uint64_t *out);
+/* Copies range records `k`: per object, one record of 16-bit slots (slot 0 the row's length, or 0xFFFF when it is too
+ * long for the record; then the children in row order; 0xFFFF after them); *n_slots = objects x slots per record.
+ * ZG_E2BIG (size filled) when the buffer is too small, ZG_EINVAL when there are none. For inspection and tests. */
+int zg_flat_record_copy(zg_engine *e, uint32_t k, uint16_t *slots, uint64_t cap, uint64_t *n_slots);
+
 /* Pinned host memory for request/response buffers: zg_check_bulk copies straight
  * from/to such buffers (no staging memcpy). */
 void *zg_host_alloc(size_t bytes);

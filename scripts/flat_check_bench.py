@@ -54,13 +54,19 @@ def measure(args):
     torch.cuda.synchronize()
     ms = sorted(a.elapsed_time(b) for a, b in evs)
     st1 = eng.stats()
-    res = {"flat_check": os.environ.get("ZGPU_FLAT_CHECK", "1"), "lib": os.environ.get("ZGPU_LIB", "default"),
+    res = {"flat_check": os.environ.get("ZGPU_FLAT_CHECK", "1"), "flat_records": os.environ.get("ZGPU_FLAT_RECORDS", "1"),
+           "lib": os.environ.get("ZGPU_LIB", "default"),
            "sig_words": os.environ.get("ZGPU_CLOSURE_SIG_WORDS", "chosen"), "checks": n,
            "mean_ms": sum(ms) / len(ms), "median_ms": ms[len(ms) // 2], "min_ms": ms[0],
            "mchecks_per_s": n / (sum(ms) / len(ms)) / 1e3, "alg_bytes_per_check": round(alg, 2),
            "launches_per_step": (st1["launches"] - st0["launches"]) / args.steps,
            "flat_slots": st1["flat_slots"], "residual_per_step": (st1["flat_residual"] - st0["flat_residual"]) / args.steps,
            "answers_sha": __import__("hashlib").sha1(d_out.cpu().numpy().tobytes()).hexdigest()[:16]}
+    if hasattr(eng, "flat_record_info"):
+        try:
+            res["records"] = eng.flat_record_info(0)
+        except Exception as ex:  # no records in this configuration
+            res["records"] = repr(ex)[:80]
     if args.profile:
         from torch.profiler import ProfilerActivity, profile
 
@@ -93,7 +99,7 @@ def main():
                              capture_output=True, text=True).stdout.strip(), flush=True)
     except OSError:
         pass
-    confs = [{}, {"ZGPU_FLAT_CHECK": "0"}]
+    confs = [{}, {"ZGPU_FLAT_CHECK": "0"}, {"ZGPU_FLAT_RECORDS": "0"}]
     confs += [{"ZGPU_LIB": p.split("=", 1)[1]} for p in args.libs]
     confs += [{"ZGPU_CLOSURE_SIG_WORDS": x} for x in args.sig_words.split(",") if x]
     base = [sys.executable, os.path.abspath(__file__), "--child", "--steps", str(args.steps), "--scale", str(args.scale)]
@@ -106,7 +112,7 @@ def main():
         if r.returncode == 0:
             shas.append(json.loads(line)["answers_sha"])
     if args.profile:
-        for c in confs[:2]:
+        for c in confs[:3]:
             r = subprocess.run(base + ["--profile"], env=dict(os.environ, **c), capture_output=True, text=True)
             print((r.stdout.strip().splitlines() or [""])[-1] if r.returncode == 0 else r.stderr[-2000:], flush=True)
     print(json.dumps({"answers_identical": len(set(shas)) == 1, "configs": len(shas), "time": time.time()}), flush=True)

@@ -31,11 +31,13 @@ def gpu_info():
 
 
 def updates(e, w, rng, n):
-    """n updates of group#member@user and team#member@group#member: half deletes of loaded relationships, half
-    inserts of new pairings between existing objects (one update per relationship)."""
+    """n updates of group#member@user, team#member@group#member and namespace#viewer@team#member (the lean kernel's
+    range records): half deletes of loaded relationships, half inserts of new pairings between existing objects (one
+    update per relationship)."""
     ups = np.zeros(n, dtype=zgpu.UPDATE_DTYPE)
+    gs = w.groups[:2] + [g for g in w.groups if (g.res_type, g.rel, g.subj_type) == ("namespace", "viewer", "team")]
     for i in range(n):
-        g = w.groups[int(rng.integers(0, 2))]
+        g = gs[int(rng.integers(0, len(gs)))]
         ups["rel"][i], ups["stype"][i] = e.slot_id(g.res_type, g.rel), e.type_id(g.subj_type)
         ups["srel"][i] = zgpu.SREL_NONE if g.srel is None else e.slot_id(g.subj_type, g.srel)
         k = int(rng.integers(0, g.res.size))
@@ -67,4 +69,6 @@ out = {**gpu_info(), "store_tuples": int(st["tuples"]), "updates_per_write": a.u
        "full_rebuild_wall_ms": full_wall * 1e3, "first_write_after_load_wall_ms": first_write_wall * 1e3}
 if hasattr(e, "closure_index_counters"):
     out["closure_index"] = e.closure_index_counters()
+if hasattr(e, "flat_record_info"):
+    out["flat_records"] = e.flat_record_info(0)  # build_us: the last rebuild, after the last write
 print(json.dumps(out))

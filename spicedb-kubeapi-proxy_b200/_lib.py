@@ -250,6 +250,8 @@ _SIGS = {
                                         C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "zg_closure_index_copy": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
                                         C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    "zg_flat_record_info": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p]),
+    "zg_flat_record_copy": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),
     "zg_resolve_checks_packed_device": (C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p]),
     "zg_check_bulk_packed_ingress": (C.c_int, [C.c_void_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_char_p, C.c_void_p, C.c_char_p, C.c_void_p, C.c_uint64, C.c_void_p]),
     "zg_intern_objects_packed": (C.c_int, [C.c_void_p, C.c_int, C.c_char_p, C.c_void_p, C.c_uint64, C.c_void_p]),
@@ -1083,6 +1085,24 @@ class Engine:
         self._ck(self._L.zg_closure_table_copy(self._h, pair, hdr.ctypes.data, hdr.size, tab.ctypes.data, tab.size,
                                                C.byref(nr), C.byref(nb)))
         return hdr[: nr.value], tab[: nb.value].view(np.uint16).reshape(-1, 4)
+
+    def flat_record_info(self, k: int = 0) -> dict:
+        """Built flag, edge class, objects, device bytes, rows kept on the offsets path and last build time (device
+        microseconds) of range records `k` (zg_flat_record_info)."""
+        out = np.zeros(6, dtype=np.uint64)
+        self._ck(self._L.zg_flat_record_info(self._h, k, out.ctypes.data))
+        return {k: int(v) for k, v in zip(("built", "cls", "objects", "device_bytes", "long_rows", "build_us"), out)}
+
+    def flat_records(self, k: int = 0):
+        """Range records `k`: uint16 array of shape (objects, slots per record) (zg_flat_record_copy)."""
+        n = C.c_uint64(0)
+        rc = self._L.zg_flat_record_copy(self._h, k, None, 0, C.byref(n))
+        if rc != E2BIG:
+            self._ck(rc)
+        out = np.empty(max(n.value, 1), dtype=np.uint16)
+        self._ck(self._L.zg_flat_record_copy(self._h, k, out.ctypes.data, out.size, C.byref(n)))
+        objects = self.flat_record_info(k)["objects"]
+        return out[: n.value].reshape(objects, -1) if objects else out[:0].reshape(0, 1)
 
     HANDLE_LOOKUP_COUNTERS = ("rounds", "levels", "round_trips", "frontier_entries", "candidates", "halvings", "fallbacks")
 

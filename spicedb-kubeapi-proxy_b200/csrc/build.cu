@@ -276,6 +276,23 @@ __global__ void __launch_bounds__(kTableWarps * 32)
   }
 }
 
+// Range records of one class (closure_sig.cuh kRecSlots): one thread per 16-bit slot, so that a warp writes two
+// records whole. Counts the rows longer than a record holds in *n_long.
+__global__ void flat_record_kernel(const uint32_t* row_ptr, const uint32_t* col, unsigned long long row_base, uint32_t ncls,
+                                   uint32_t nres, uint16_t* rec, unsigned long long* n_long) {
+  const unsigned long long t = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x;
+  if (t >= static_cast<unsigned long long>(nres) * kRecSlots) return;
+  const uint32_t obj = static_cast<uint32_t>(t / kRecSlots), k = static_cast<uint32_t>(t % kRecSlots);
+  const unsigned long long row = row_base + static_cast<unsigned long long>(obj) * ncls;
+  const uint32_t lo = row_ptr[row], n = row_ptr[row + 1] - lo;
+  const bool inline_row = n < kRecSlots;
+  uint32_t v = kRecLong;
+  if (k == 0) v = inline_row ? n : kRecLong;
+  else if (inline_row && k <= n) v = col[lo + k - 1];
+  rec[t] = static_cast<uint16_t>(v);
+  if (k == 0 && !inline_row) atomicAdd(n_long, 1ull);
+}
+
 }  // namespace
 
 std::string gpu_build_closure(const Snapshot& s, const DCls& a, const DCls& b, uint64_t cap, Snapshot::Closure* c,
@@ -454,6 +471,39 @@ std::string gpu_build_closure_table(Snapshot::Closure* c, uint32_t seeds, cudaSt
   BCUDA(cudaStreamSynchronize(st));
   c->set_buckets = total;
   c->set_built = true;
+  return "";
+}
+
+std::string gpu_build_flat_records(const Snapshot& s, Snapshot::FlatRecords* r, cudaStream_t st) {
+  r->built = false;
+  r->long_rows = 0;
+  const size_t bytes = size_t(r->nres) * kRecSlots * 2;
+  size_t free_b = 0, total_b = 0;
+  BCUDA(cudaMemGetInfo(&free_b, &total_b));
+  if (bytes > (free_b + r->rec.cap) / 4) {  // (counting the class's old records as free: they are reused)
+    r->rec.release();
+    return "";
+  }
+  DevBuf d_long;
+  if (!r->rec.ensure(bytes ? bytes : 16) || !d_long.ensure(8)) {
+    d_long.release();
+    return "out of device memory (range records)";
+  }
+  unsigned long long n_long = 0;
+  cudaError_t ce = cudaMemsetAsync(d_long.p, 0, 8, st);
+  if (ce == cudaSuccess && bytes) {
+    const unsigned blk = 256;
+    const unsigned long long grid = (static_cast<unsigned long long>(r->nres) * kRecSlots + blk - 1) / blk;
+    flat_record_kernel<<<grid, blk, 0, st>>>(s.row_ptr.as<uint32_t>(), s.col.as<uint32_t>(), r->row_base, r->ncls,
+                                              r->nres, r->rec.as<uint16_t>(), d_long.as<unsigned long long>());
+    ce = cudaGetLastError();
+  }
+  if (ce == cudaSuccess) ce = cudaMemcpyAsync(&n_long, d_long.p, 8, cudaMemcpyDeviceToHost, st);
+  if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+  d_long.release();
+  if (ce != cudaSuccess) return std::string("range records: ") + cudaGetErrorString(ce);
+  r->long_rows = n_long;
+  r->built = true;
   return "";
 }
 

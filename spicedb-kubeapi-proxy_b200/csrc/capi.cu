@@ -3966,6 +3966,35 @@ extern "C" int zg_closure_table_copy(zg_engine* e, uint32_t pair, uint64_t* hdr,
   return ce == cudaSuccess ? ZG_OK : fail(ZG_ECUDA, std::string("zg_closure_table_copy: ") + cudaGetErrorString(ce));
 }
 
+extern "C" int zg_flat_record_info(zg_engine* e, uint32_t k, uint64_t* out) {
+  if (!e || !out) return fail(ZG_EINVAL, "NULL argument");
+  LOCK_DEVICE(e);
+  const auto s = e->dev.snap;
+  if (!s) return fail(ZG_ENOSNAPSHOT, "no snapshot published (call zg_publish)");
+  if (k >= s->records.size()) return fail(ZG_EINVAL, "no range records with this number");
+  const auto& r = s->records[k];
+  const bool b = r.built;
+  const uint64_t c[6] = {b ? 1u : 0u, r.gc, r.nres, b ? uint64_t(r.nres) * zg::kRecSlots * 2 : 0u, b ? r.long_rows : 0u,
+                         b ? static_cast<uint64_t>(r.ms * 1000.0) : 0u};
+  std::memcpy(out, c, sizeof c);
+  return ZG_OK;
+}
+
+extern "C" int zg_flat_record_copy(zg_engine* e, uint32_t k, uint16_t* slots, uint64_t cap, uint64_t* n_slots) {
+  if (!e || !n_slots) return fail(ZG_EINVAL, "NULL argument");
+  LOCK_DEVICE(e);
+  const auto s = e->dev.snap;
+  if (!s) return fail(ZG_ENOSNAPSHOT, "no snapshot published (call zg_publish)");
+  if (k >= s->records.size() || !s->records[k].built) return fail(ZG_EINVAL, "no range records with this number");
+  const auto& r = s->records[k];
+  *n_slots = uint64_t(r.nres) * zg::kRecSlots;
+  if (cap < *n_slots || (!slots && *n_slots)) return fail(ZG_E2BIG, "buffer too small for the range records");
+  cudaError_t ce = cudaSetDevice(e->dev.device);
+  if (ce == cudaSuccess) ce = cudaStreamSynchronize(e->dev.stream);
+  if (ce == cudaSuccess && *n_slots) ce = cudaMemcpy(slots, r.rec.p, *n_slots * 2, cudaMemcpyDeviceToHost);
+  return ce == cudaSuccess ? ZG_OK : fail(ZG_ECUDA, std::string("zg_flat_record_copy: ") + cudaGetErrorString(ce));
+}
+
 extern "C" int zg_handle_lookup_counters(zg_engine* e, uint64_t* out) {
   if (!e || !out) return fail(ZG_EINVAL, "NULL argument");
   LOCK_DEVICE(e);

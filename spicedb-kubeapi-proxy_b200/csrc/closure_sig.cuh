@@ -48,4 +48,16 @@ __host__ __device__ __forceinline__ bool table_has(unsigned long long w, uint32_
   return ((x - 0x0001000100010001ull) & ~x & 0x8000800080008000ull) != 0;
 }
 
+// Range record of one object in one edge class (build.cu gpu_build_flat_records; kernels.cuh flat_check_kernel): the
+// object's range col[row_ptr[row], row_ptr[row + 1]) copied into a fixed-stride record of kRecSlots 16-bit slots at
+// rec + obj * kRecSlots. Slot 0 holds the range's length n, slots 1 .. n its children in CSR order, the rest 0xFFFF. A
+// range longer than kRecSlots - 1 has kRecLong in slot 0 and is read from the CSR. The children are objects of a meet's
+// target type, which has fewer than 65 536 objects wherever set tables exist.
+#ifndef ZG_FLAT_RECORD_SLOTS
+#define ZG_FLAT_RECORD_SLOTS 32  // 64-byte records (32-byte records, 15 inline children: 16)
+#endif
+constexpr uint32_t kRecSlots = ZG_FLAT_RECORD_SLOTS;
+constexpr uint32_t kRecLong = 0xFFFFu;
+static_assert(kRecSlots == 16 || kRecSlots == 32, "records of 32 or 64 bytes");
+
 }  // namespace zg

@@ -99,6 +99,7 @@ Snapshot::~Snapshot() {
     c.set_hdr.release();
     c.set_tab.release();
   }
+  for (auto& r : records) r.rec.release();
 }
 
 Device::~Device() {
@@ -162,6 +163,7 @@ std::string Device::init(int dev, uint64_t subq_cap, uint32_t budget) {
     closure_sig_words_ = static_cast<uint32_t>(std::strtoul(v, nullptr, 10));
   if (const char* v = std::getenv("ZGPU_CLOSURE_TABLE")) closure_table_ = !(*v == '0' && !v[1]);  // tests: 0 = no tables
   if (const char* v = std::getenv("ZGPU_FLAT_CHECK")) flat_check_ = !(*v == '0' && !v[1]);  // tests, A/B: 0 = no SF_FLAT
+  if (const char* v = std::getenv("ZGPU_FLAT_RECORDS")) flat_records_ = !(*v == '0' && !v[1]);  // tests, A/B: 0 = none
   int count = 0;
   cudaError_t e = cudaGetDeviceCount(&count);
   if (e != cudaSuccess || count == 0)
@@ -305,15 +307,16 @@ std::string Device::publish_delta(const Store& store, const Schema& sc, uint64_t
   std::vector<uint32_t> cls_delta;
   std::string err = gpu_apply_delta(store, sc, lay, stream, s.get(), &cls_delta, own_rank, own_count);
   const uint64_t failures = closure_failures;
-  if (err.empty() && !s->closure.empty()) {
-    // a closure index whose classes this write changed is rebuilt from the merged reverse rows before anybody reads
-    // the snapshot again: a stale index is never read
+  if (err.empty() && (!s->closure.empty() || !s->records.empty())) {
+    // a closure index or range records whose classes this write changed are rebuilt from the merged rows before
+    // anybody reads the snapshot again: stale ones are never read
     std::vector<uint8_t> touched(lay.cls.size(), 0);
     for (const auto& j : store.journal) {
       const int k = sc.class_of(j.t.rel, j.t.stype, j.t.srel);
       if (k >= 0) touched[lay.rels[sc.slots[j.t.rel].rel_index].cls_begin + k] = 1;
     }
-    build_closures(s.get(), lay, &touched);
+    if (!s->closure.empty()) build_closures(s.get(), lay, &touched);
+    build_flat_records(s.get(), &touched);
   }
   cudaEventRecord(e1, stream);
   cudaEventRecord(last_done_, stream);
@@ -416,6 +419,33 @@ void Device::build_closures(Snapshot* s, const HostSnapshot& h, const std::vecto
       c.set_hdr.release();
       c.set_tab.release();
       c.set_built = false;
+      cudaGetLastError();
+    }
+  }
+  if (e0) {
+    cudaEventDestroy(e0);
+    cudaEventDestroy(e1);
+  }
+}
+
+void Device::build_flat_records(Snapshot* s, const std::vector<uint8_t>* rebuild) {
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  for (auto& r : s->records) {
+    if (rebuild && !(*rebuild)[r.gc]) continue;
+    if (!e0) {
+      cudaEventCreate(&e0);
+      cudaEventCreate(&e1);
+    }
+    cudaEventRecord(e0, stream);
+    std::string err = gpu_build_flat_records(*s, &r, stream);
+    cudaEventRecord(e1, stream);
+    cudaEventSynchronize(e1);
+    float ms = 0;
+    cudaEventElapsedTime(&ms, e0, e1);
+    r.ms = ms;
+    if (!err.empty()) {  // the records are optional: the class's steps read the CSR
+      r.built = false;
+      r.rec.release();
       cudaGetLastError();
     }
   }
@@ -544,6 +574,28 @@ std::string Device::finish_publish(std::shared_ptr<Snapshot> s, const HostSnapsh
           cudaStreamSynchronize(stream) != cudaSuccess)
         return std::string("snapshot upload failed: ") + cudaGetErrorString(cudaGetLastError());
     }
+    // the range records of the SF_FLAT slots' push step classes, built whole from this layout's rows (a class whose
+    // children may reach 0xFFFF has none: record_meet marks its unused lookups with it)
+    for (auto& r : s->records) r.rec.release();
+    s->records.clear();
+    const DSlot* slots = reinterpret_cast<const DSlot*>(blob.data() + ph->off_slots);
+    const DUnit* units = reinterpret_cast<const DUnit*>(blob.data() + ph->off_units);
+    for (uint32_t sl = 0; flat_records_ && s->flat_slots && sl < ph->n_slots; ++sl) {
+      if (!(slots[sl].flags & SF_FLAT)) continue;
+      const DUnit& u = units[slots[sl].unit];
+      for (int i = u.push_begin; i < u.step_end; ++i) {
+        const DStep& st = steps[i];
+        bool seen = h.n_objects[h.cls[st.gc].stype] >= 65536u;
+        for (const auto& r : s->records) seen = seen || r.gc == st.gc;
+        if (seen || s->records.size() == static_cast<size_t>(kMaxFlatRecords)) continue;
+        s->records.emplace_back();
+        s->records.back().gc = st.gc;
+        s->records.back().row_base = st.row_base;
+        s->records.back().nres = st.nres;
+        s->records.back().ncls = st.ncls;
+      }
+    }
+    build_flat_records(s.get(), nullptr);
   }
   s->revision = revision;
 
@@ -639,6 +691,8 @@ int Device::run_pass(const Snapshot& s, const zg_check* queries, uint64_t nq, ui
       all_sig = all_sig && c.sig_words;
       all_set = all_set && c.set_built;
     }
+  for (const auto& r : s.records)
+    if (r.built) p.rec[p.n_rec++] = FlatRecordRef{r.rec.as<uint4>(), r.nres, r.gc};
   if (p.n_closure && all_sig && all_set && meet == kMeet16) meet = kMeetSet16;
   else if (p.n_closure && all_sig) meet |= kMeetSig;
   // SF_FLAT slots are marked only where every pair they meet over has signatures and a set table, but another pair

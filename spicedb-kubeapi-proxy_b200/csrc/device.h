@@ -82,6 +82,20 @@ struct Snapshot {
     double set_ms = 0;  // device time of its last build
   };
   std::vector<Closure> closure;
+  // Range records (kernels.cuh FlatRecordRef; gpu_build_flat_records) of the class gc of every push step of an SF_FLAT
+  // slot: object obj's row is row_ptr[row_base + obj * ncls], obj < nres. Rebuilt whole by every publish that may change
+  // the class's rows (finish_publish, and publish_delta when the journal touches gc). Empty when !built (over budget,
+  // or a failed build): its steps then read the CSR.
+  struct FlatRecords {
+    uint16_t gc = 0;
+    uint64_t row_base = 0;
+    uint32_t nres = 0, ncls = 0;
+    DevBuf rec;
+    bool built = false;
+    uint64_t long_rows = 0;  // rows longer than a record holds, read from the CSR
+    double ms = 0;           // device time of its last build
+  };
+  std::vector<FlatRecords> records;
   uint64_t n_tuples = 0, bytes = 0, revision = 0;
   ~Snapshot();
 };
@@ -444,12 +458,16 @@ class Device {
                                       // from the mean row length, gpu_build_closure_sig)
   bool closure_table_ = true;  // ZGPU_CLOSURE_TABLE: build the rows' set tables (tests; 0 = none)
   bool flat_check_ = true;     // ZGPU_FLAT_CHECK: mark SF_FLAT slots at publish (tests and A/B runs; 0 = none)
+  bool flat_records_ = true;   // ZGPU_FLAT_RECORDS: build the SF_FLAT push steps' range records (tests and A/B; 0 = none)
   // (Re)builds the closure index of every pair of s->closure that is not built yet (`rebuild` false) or whose inner or
   // tgc class is marked in `rebuild` (a write changed it), from the classes' reverse rows described by h.cls. Decides
   // the entry width from h's object capacities first: 16-bit when every pair's tgc resource type holds at most 65 536
   // objects, else 32-bit, and rebuilds every pair built at another width. A pair whose build fails is left without an
   // index (closure_failures). Every index built here gets its signatures; a pair whose signatures fail keeps its index.
   void build_closures(Snapshot* s, const HostSnapshot& h, const std::vector<uint8_t>* rebuild);
+  // (Re)builds the range records of s->records whose class is marked in `rebuild` (every one when null). A build that
+  // fails leaves the class without records.
+  void build_flat_records(Snapshot* s, const std::vector<uint8_t>* rebuild);
   // match_filter / match_expired: the count launch over the classes `sel` (p holds the rest of the plan), then with
   // `tuples` the emit launch sized by it, of filter_expired_kernel (`expired`) or the kernel of `shape`.
   int run_filter(const Schema& sc, const Snapshot& s, const std::vector<FilterSel>& sel, FilterPlan& p, FilterShape shape,
@@ -574,5 +592,9 @@ std::string gpu_build_closure_sig(Snapshot::Closure* c, uint32_t words, cudaStre
 // would take more than a quarter of the free device memory. The caller builds it only for a target type of fewer than
 // 65 536 objects (0xFFFF marks an empty slot).
 std::string gpu_build_closure_table(Snapshot::Closure* c, uint32_t seeds, cudaStream_t st);
+// Builds the range records *r of one class from the resident forward CSR of s (kernels.cuh FlatRecordRef). None
+// (r->built false) when they would take more than a quarter of the free device memory. The caller builds them only
+// for a class whose subjects' type holds fewer than 65 536 objects.
+std::string gpu_build_flat_records(const Snapshot& s, Snapshot::FlatRecords* r, cudaStream_t st);
 
 }  // namespace zg

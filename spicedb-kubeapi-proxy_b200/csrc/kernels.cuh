@@ -102,6 +102,16 @@ struct ClosureRef {
 // also kMeetSet when the signatures' "maybe"s are confirmed in the rows' set tables (16-bit indexes only)
 constexpr int kMeetNone = 0, kMeet16 = 2, kMeet32 = 4, kMeetSig = 8, kMeetSet = 16;
 constexpr int kMeetSig16 = kMeet16 | kMeetSig, kMeetSig32 = kMeet32 | kMeetSig, kMeetSet16 = kMeetSig16 | kMeetSet;
+// Range records of a push step's class (closure_sig.cuh kRecSlots), read by flat_check_kernel. The record's address
+// depends on obj alone, so it is loaded beside the subject's table header and signature line instead of after the
+// range's offsets.
+constexpr int kMaxFlatRecords = 4;
+constexpr uint32_t kRecVecs = kRecSlots / 8;  // 16-byte loads per record
+struct FlatRecordRef {
+  const uint4* rec;  // nres records of kRecSlots 16-bit slots
+  uint32_t nres;
+  uint16_t gc;
+};
 template <int MEET> struct ClosureEntry { using type = uint32_t; };
 template <> struct ClosureEntry<kMeet16> { using type = uint16_t; };
 template <> struct ClosureEntry<kMeetSig16> { using type = uint16_t; };
@@ -162,6 +172,9 @@ struct KParams {
   // nq_dev[0] = this pass's residual, nq_dev[1] += it (a running total). nullptr: queries[i], nq.
   uint32_t* idx;
   unsigned long long* nq_dev;
+  // flat_check_kernel only: the range records of the push steps' classes (a class without one reads the CSR)
+  FlatRecordRef rec[kMaxFlatRecords];
+  uint32_t n_rec;
 };
 
 // View of the program blob. Only the base pointer is kept in registers; table addresses are
@@ -1405,12 +1418,12 @@ __global__ void __launch_bounds__(kThreads, kMinBlocks) check_kernel(const KPara
 // order until one hits, then per meet step 8 bytes for the range's offsets, 8 for the subject's table header when the
 // range is not empty, and sig_meet's rounds (sig_round, table_round) until one finds the check.
 #ifndef ZG_FLAT_MIN_BLOCKS
-#define ZG_FLAT_MIN_BLOCKS 4
+#define ZG_FLAT_MIN_BLOCKS 3
 #endif
 constexpr int kFlatThreads = 256;
-// 4 CTAs (32 warps) per SM, 64 registers: eight children's signature words and buckets in flight per thread. Measured on
-// cfg3 (H100, DESIGN.md §6): 1.19x faster than 6 CTAs at 40 registers with rounds of four children, which spill
-// nothing either, and 1.35x faster than 8 CTAs at 32.
+// 3 CTAs (24 warps) per SM, 80 registers: a range record and eight children's signature words in flight per thread,
+// no spills. Measured on cfg3 (H100 80GB HBM3, 700 W, DESIGN.md §6): 1.06x faster than 4 CTAs at 64 registers, which
+// spill one word. Before the records, 4 CTAs at 64 registers were 1.19x faster than 6 at 40 and 1.35x than 8 at 32.
 constexpr int kFlatMinBlocks = ZG_FLAT_MIN_BLOCKS;
 
 // A program record read through the read-only cache (records of 8-byte multiples, 8-byte aligned in the blob).
@@ -1424,6 +1437,62 @@ __device__ __forceinline__ T ldg_rec(const T* r) {
 #pragma unroll
   for (unsigned i = 0; i < sizeof(T) / 8; ++i) u.w[i] = __ldg(reinterpret_cast<const unsigned long long*>(r) + i);
   return u.t;
+}
+
+// The two-level meet of a range held inline in its record r (n <= kRecSlots - 1 children, slot j + 1 = child j): every
+// child tested against the subject's signature, kSigTests at a time from L1, then the "maybe"s confirmed in the set
+// table, kSigTests lookups in flight together. One dependent round trip (the buckets) after the record, where sig_meet's
+// rounds take two per kSigTests children. The COUNT variant confirms every "maybe" and counts what those rounds read: 12
+// bytes per child and 8 per "maybe", in rounds of kSigTests up to and including the first that holds a member.
+template <bool COUNT>
+__device__ __forceinline__ bool record_meet(const uint16_t* __restrict__ rs, const uint32_t (&r)[kRecSlots / 2], uint32_t n,
+                                            const unsigned long long* __restrict__ sig, uint32_t lg,
+                                            const unsigned long long* __restrict__ tab, uint32_t nbk, uint32_t seed,
+                                            unsigned long long& nb) {
+  unsigned maybe = 0;  // bit j: child j
+#pragma unroll
+  for (uint32_t c0 = 0; c0 < kRecSlots - 1; c0 += kSigTests) {
+    if (c0 >= n) break;
+    uint32_t v[kSigTests];
+    unsigned long long w[kSigTests];
+#pragma unroll
+    for (uint32_t i = 0; i < kSigTests; ++i) {
+      const uint32_t k = c0 + i + 1;
+      v[i] = k < kRecSlots ? (r[k >> 1] >> (16 * (k & 1))) & 0xFFFFu : 0u;
+      w[i] = c0 + i < n ? __ldg(sig + sig_word(v[i], lg)) : 0ull;
+    }
+#pragma unroll
+    for (uint32_t i = 0; i < kSigTests; ++i) {
+      const unsigned long long b = sig_mask(v[i]);
+      maybe |= (c0 + i < n && (w[i] & b) == b) ? 1u << (c0 + i) : 0u;
+    }
+  }
+  // The "maybe"s are read again from the record (an L1 hit: it was just loaded) rather than picked out of r, which would
+  // keep r live and spill. A child is never 0xFFFF: it marks the unused lookups of a batch, whose bucket word 0 is empty.
+  unsigned found = 0, todo = maybe;  // found: the confirmed children (COUNT), or 1 once one is
+  while (todo && (COUNT || !found)) {
+    uint32_t v[kSigTests], at[kSigTests];
+#pragma unroll
+    for (uint32_t t = 0; t < kSigTests; ++t) {
+      const uint32_t a = todo ? __ffs(todo) - 1 : 32u;
+      if (COUNT) at[t] = a;
+      todo &= todo - 1;
+      v[t] = a < 32 ? __ldg(rs + a + 1) : 0xFFFFu;
+    }
+    unsigned long long w[kSigTests];
+#pragma unroll
+    for (uint32_t t = 0; t < kSigTests; ++t) w[t] = v[t] != 0xFFFFu ? __ldg(tab + table_bucket(v[t], seed, nbk)) : 0ull;
+#pragma unroll
+    for (uint32_t t = 0; t < kSigTests; ++t) found |= table_has(w[t], v[t]) ? (COUNT ? 1u << at[t] : 1u) : 0u;
+  }
+  if (COUNT)
+    for (uint32_t c0 = 0; c0 < n; c0 += kSigTests) {
+      const uint32_t m = min(n - c0, kSigTests);
+      const unsigned rm = ((1u << m) - 1u) << c0;
+      nb += 12ull * m + 8ull * __popc(maybe & rm);
+      if (found & rm) break;
+    }
+  return found != 0;
 }
 
 template <bool COUNT>
@@ -1495,16 +1564,28 @@ __global__ void __launch_bounds__(kFlatThreads, COUNT ? 1 : kFlatMinBlocks) flat
       if (stype != st.stype || (st.kind == ST_WILD && p.no_wildcards)) continue;
       hit = probe_step(p, c, st, obj, sid, (st.flags & CF_EXPIRY) != 0);
     }
-    // two-level meets: the range's offsets, the subject's table header and signature line are loaded together
+    // two-level meets: the range's record (or its offsets), the subject's table header and signature line are loaded
+    // together
     for (int i = u.push_begin; !hit && i < u.step_end; ++i) {
       const DStep st = ldg_rec(steps + i);
       if (obj >= st.nres) continue;
       uint32_t nsubj = 0, words = 0;
       const unsigned long long *hdr = nullptr, *sig = nullptr, *tab = nullptr;
       closure_of(st.tgc, nsubj, hdr, sig, words, tab);
-      const unsigned long long ridx = st.row_base + static_cast<unsigned long long>(obj) * st.ncls;
-      uint32_t lo = __ldg(p.row_ptr + ridx);
-      const uint32_t hi = __ldg(p.row_ptr + ridx + 1);
+      const uint4* rec = nullptr;
+#pragma unroll
+      for (int k = 0; k < kMaxFlatRecords; ++k)
+        if (k < static_cast<int>(p.n_rec) && p.rec[k].gc == st.gc && obj < p.rec[k].nres) rec = p.rec[k].rec;
+      uint32_t r[kRecSlots / 2];  // the record's slots, two per word
+      if (rec)
+#pragma unroll
+        for (uint32_t k = 0; k < kRecVecs; ++k) {
+          const uint4 x = __ldg(rec + static_cast<unsigned long long>(obj) * kRecVecs + k);
+          r[4 * k] = x.x;
+          r[4 * k + 1] = x.y;
+          r[4 * k + 2] = x.z;
+          r[4 * k + 3] = x.w;
+        }
       const unsigned long long hw = __ldg(hdr + sid);
       const uint32_t lg = __ffs(words) - 1;
       sig += static_cast<unsigned long long>(sid) << lg;
@@ -1512,16 +1593,28 @@ __global__ void __launch_bounds__(kFlatThreads, COUNT ? 1 : kFlatMinBlocks) flat
       asm volatile("prefetch.global.L1 [%0];" ::"l"(sig));
 #endif
       if (COUNT) c.bytes += 8;
-      if (hi <= lo) continue;
-      if (COUNT) c.bytes += 8;
       const uint32_t nbk = static_cast<uint32_t>(hw >> 32) & 0xFFFFFFu, seed = static_cast<uint32_t>(hw >> 56);
       tab += static_cast<uint32_t>(hw);
-      while (nbk && lo < hi && !hit) {  // sig_meet's rounds, whose early exit the byte model follows
-        uint32_t v[kSigTests];
-        const uint32_t n = min(hi - lo, kSigTests);
-        const unsigned m = sig_round<COUNT>(p.col, lo, n, sig, lg, v, c.bytes);
-        lo += n;
-        hit = table_round<COUNT>(tab, nbk, seed, m, v, c.bytes);
+      const uint32_t n = rec ? r[0] & 0xFFFFu : kRecLong;
+      if (n != kRecLong) {
+        if (n == 0) continue;
+        if (COUNT) c.bytes += 8;
+        if (nbk)
+          hit = record_meet<COUNT>(reinterpret_cast<const uint16_t*>(rec + static_cast<unsigned long long>(obj) * kRecVecs),
+                                   r, n, sig, lg, tab, nbk, seed, c.bytes);
+      } else {  // no record, or a range too long for one: its offsets, then sig_meet's rounds
+        const unsigned long long ridx = st.row_base + static_cast<unsigned long long>(obj) * st.ncls;
+        uint32_t lo = __ldg(p.row_ptr + ridx);
+        const uint32_t hi = __ldg(p.row_ptr + ridx + 1);
+        if (hi <= lo) continue;
+        if (COUNT) c.bytes += 8;
+        while (nbk && lo < hi && !hit) {  // sig_meet's rounds, whose early exit the byte model follows
+          uint32_t v[kSigTests];
+          const uint32_t m = min(hi - lo, kSigTests);
+          const unsigned mb = sig_round<COUNT>(p.col, lo, m, sig, lg, v, c.bytes);
+          lo += m;
+          hit = table_round<COUNT>(tab, nbk, seed, mb, v, c.bytes);
+        }
       }
       // check_kernel still reads (and counts) the offsets and header of the steps after the one that finds the check
       if (COUNT && hit)
