@@ -187,6 +187,12 @@ func (s *cstrs) fillRel(dst *C.zg_rel_str, res *v1.ObjectReference, relation str
 	dst.subj_rel = s.add(subj.GetOptionalRelation())
 }
 
+// fillFilterEx: fillFilter and optional_resource_id_prefix ("" = unset).
+func (s *cstrs) fillFilterEx(dst *C.zg_filter_ex, f *v1.RelationshipFilter) {
+	s.fillFilter(&dst.f, f)
+	dst.res_id_prefix = s.add(f.GetOptionalResourceIdPrefix())
+}
+
 func (s *cstrs) fillFilter(dst *C.zg_filter_str, f *v1.RelationshipFilter) {
 	dst.res_type = s.add(f.GetResourceType())
 	dst.res_id = s.add(f.GetOptionalResourceId())
@@ -637,9 +643,9 @@ func (c *Client) DeleteRelationships(ctx context.Context, req *v1.DeleteRelation
 	}
 	var s cstrs
 	defer s.free()
-	var f C.zg_filter_str
-	s.fillFilter(&f, req.GetRelationshipFilter())
-	if err := call(func() C.int { return C.zg_delete_relationships(c.engine, &f, nil, 0, nil) }); err != nil {
+	var f C.zg_filter_ex
+	s.fillFilterEx(&f, req.GetRelationshipFilter())
+	if err := call(func() C.int { return C.zg_delete_relationships_limited_ex(c.engine, &f, nil, 0, 0, 0, nil, nil) }); err != nil {
 		if rerr := c.resync(ctx); rerr != nil {
 			c.broken.Store(true)
 			return nil, status.Errorf(codes.Internal, "gpu mirror delete failed (%v) and resync failed: %v", err, rerr)
@@ -787,8 +793,8 @@ type MirrorPage struct {
 func (c *Client) ReadMirrorPage(filter *v1.RelationshipFilter, limit uint64, after []byte) (*MirrorPage, error) {
 	var s cstrs
 	defer s.free()
-	var f C.zg_filter_str
-	s.fillFilter(&f, filter)
+	var f C.zg_filter_ex
+	s.fillFilterEx(&f, filter)
 	var cur *C.zg_read_cursor
 	if after != nil {
 		if len(after) != C.ZG_READ_CURSOR_BYTES {
@@ -810,7 +816,7 @@ func (c *Client) ReadMirrorPage(filter *v1.RelationshipFilter, limit uint64, aft
 		var more C.int32_t
 		big := false
 		err := call(func() C.int {
-			rc := C.zg_read_relationships_page(c.engine, &f, C.uint64_t(limit), cur, (*C.char)(buf), C.size_t(capBytes), &need,
+			rc := C.zg_read_relationships_page_ex(c.engine, &f, C.uint64_t(limit), cur, (*C.char)(buf), C.size_t(capBytes), &need,
 				&n, &exp[0], &curs[0], &next, &more)
 			big = rc == C.ZG_E2BIG
 			if big {
@@ -853,8 +859,8 @@ func (c *Client) DeleteMirrorLimited(filter *v1.RelationshipFilter, limit uint64
 	defer c.mu.Unlock()
 	var s cstrs
 	defer s.free()
-	var f C.zg_filter_str
-	s.fillFilter(&f, filter)
+	var f C.zg_filter_ex
+	s.fillFilterEx(&f, filter)
 	var n C.uint64_t
 	var partial C.int32_t
 	allow := C.int(0)
@@ -862,7 +868,7 @@ func (c *Client) DeleteMirrorLimited(filter *v1.RelationshipFilter, limit uint64
 		allow = 1
 	}
 	if err := call(func() C.int {
-		return C.zg_delete_relationships_limited(c.engine, &f, nil, 0, C.uint64_t(limit), allow, &n, &partial)
+		return C.zg_delete_relationships_limited_ex(c.engine, &f, nil, 0, C.uint64_t(limit), allow, &n, &partial)
 	}); err != nil {
 		return 0, false, err
 	}

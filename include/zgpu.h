@@ -385,6 +385,48 @@ int zg_delete_relationships_limited(zg_engine *e, const zg_filter_str *filter, c
  * out[3] device launches. Pages also count in zg_filter_counters as filters. */
 int zg_page_counters(zg_engine *e, uint64_t *out);
 
+/* ---- filters by resource id prefix (v1.RelationshipFilter.optional_resource_id_prefix) ---- */
+/* A zg_filter_str with a resource id prefix. res_id_prefix NULL or "" = unset: the filter is the zg_filter_str alone,
+ * and every _ex call answers exactly as the call without _ex.
+ *   - Match rule: a relationship matches when its resource has an interned name that starts with the prefix's bytes
+ *     (byte-wise, case-sensitive). Ids that bulk loads use without a name never match, as they never match res_id.
+ *     A retired name matches nothing; a reused id matches by its new name.
+ *   - Validation: 1..1024 characters of [a-zA-Z0-9/_|\-=+] (`*` is not allowed), else ZG_EINVAL. res_id and the
+ *     prefix together are ZG_EINVAL, as in SpiceDB.
+ *   - The prefix needs no resource type: without one it selects matching resources of every type. (res_id and
+ *     relation still need one.)
+ *   - Everything else is as without the prefix: expiry at the engine's clock, deletes include expired relationships,
+ *     limited deletes take the first `limit` in the page order, preconditions count matches, deletes write the watch
+ *     feed and publish once.
+ *   - A page cursor fingerprints the prefix when it is set: a cursor made with another prefix, or with none, is
+ *     ZG_EINVAL. An unprefixed filter's cursors are those of zg_read_relationships_page.
+ *   - On a current snapshot the device answers: it scans the device mirror of the interned names (the one device
+ *     ingress keeps) for the matching resources, one bitmap per type, then runs the filter kernels against it. */
+typedef struct {
+  zg_filter_str f;
+  const char *res_id_prefix; /* NULL/"" = unset */
+} zg_filter_ex;
+typedef struct {
+  uint32_t op; /* ZG_PRECOND_* */
+  zg_filter_ex filter;
+} zg_precondition_ex;
+int zg_read_relationships_ex(zg_engine *e, const zg_filter_ex *filter, char *buf, size_t cap, size_t *need,
+                             uint64_t *n_out);
+int zg_read_relationships_page_ex(zg_engine *e, const zg_filter_ex *filter, uint64_t limit, const zg_read_cursor *after,
+                                  char *buf, size_t cap, size_t *need, uint64_t *n_out, uint32_t *expires,
+                                  zg_read_cursor *cursors, zg_read_cursor *next, int32_t *more);
+/* limit 0 = unlimited (zg_delete_relationships). */
+int zg_delete_relationships_limited_ex(zg_engine *e, const zg_filter_ex *filter, const zg_precondition_ex *pre,
+                                       uint64_t n_pre, uint64_t limit, int allow_partial, uint64_t *n_deleted,
+                                       int32_t *partial);
+int zg_write_relationships_ex(zg_engine *e, const zg_update_str *updates, uint64_t n, const zg_precondition_ex *pre,
+                              uint64_t n_pre);
+/* Cumulative counters of prefix filters (zg_filter_counters keeps its layout): out[0] prefix filters answered on the
+ * device, out[1] prefix filters answered by the host store, out[2] names the device scanned, out[3] resources the
+ * device matched, out[4] device launches of the prefix scans and their match lists, out[5] syncs of the names mirror
+ * that uploaded bytes. */
+int zg_prefix_counters(zg_engine *e, uint64_t *out);
+
 /* ---- the hot path -------------------------------------------------------- */
 /* CheckBulkPermissions: out[i] answers items[i] (same length, same order:
  * pkg/authz/check.go:54-57). HOST buffers; copies are inside the call. */

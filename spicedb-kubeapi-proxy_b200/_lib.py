@@ -78,6 +78,14 @@ class _Precond(C.Structure):
     _fields_ = [("op", C.c_uint32), ("filter", _RelStr)]
 
 
+class _FilterEx(C.Structure):
+    _fields_ = [("f", _RelStr), ("res_id_prefix", C.c_char_p)]
+
+
+class _PrecondEx(C.Structure):
+    _fields_ = [("op", C.c_uint32), ("filter", _FilterEx)]
+
+
 class _ImportGroup(C.Structure):
     _fields_ = [("res_type", C.c_char_p), ("relation", C.c_char_p), ("subj_type", C.c_char_p), ("subj_rel", C.c_char_p),
                 ("res_ids", C.c_char_p), ("res_off", C.c_void_p), ("subj_ids", C.c_char_p), ("subj_off", C.c_void_p),
@@ -207,6 +215,16 @@ _SIGS = {
     "zg_delete_relationships_limited": (C.c_int, [C.c_void_p, C.POINTER(_RelStr), C.POINTER(_Precond), C.c_uint64,
                                                   C.c_uint64, C.c_int, C.POINTER(C.c_uint64), C.POINTER(C.c_int32)]),
     "zg_page_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "zg_read_relationships_ex": (C.c_int, [C.c_void_p, C.POINTER(_FilterEx), C.c_char_p, C.c_size_t,
+                                           C.POINTER(C.c_size_t), C.POINTER(C.c_uint64)]),
+    "zg_read_relationships_page_ex": (C.c_int, [C.c_void_p, C.POINTER(_FilterEx), C.c_uint64, C.c_void_p, C.c_char_p,
+                                                C.c_size_t, C.POINTER(C.c_size_t), C.POINTER(C.c_uint64), C.c_void_p,
+                                                C.c_void_p, C.c_void_p, C.POINTER(C.c_int32)]),
+    "zg_delete_relationships_limited_ex": (C.c_int, [C.c_void_p, C.POINTER(_FilterEx), C.POINTER(_PrecondEx), C.c_uint64,
+                                                     C.c_uint64, C.c_int, C.POINTER(C.c_uint64), C.POINTER(C.c_int32)]),
+    "zg_write_relationships_ex": (C.c_int, [C.c_void_p, C.POINTER(_UpdateStr), C.c_uint64, C.POINTER(_PrecondEx),
+                                            C.c_uint64]),
+    "zg_prefix_counters": (C.c_int, [C.c_void_p, C.c_void_p]),
     "zg_watch_read": (C.c_int, [C.c_void_p, C.c_uint64, C.c_char_p, C.c_char_p, C.c_size_t, C.POINTER(C.c_size_t),
                                 C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
     "zg_check_bulk": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
@@ -510,6 +528,9 @@ class Engine:
             parts = [_b(x) for x in split_rel(rel)]
             keep.append(parts)
             arr[i] = _UpdateStr(_RelStr(*parts), int(exp), int(op))
+        if self._any_prefix(f for _, f in preconditions):
+            self._ck(self._L.zg_write_relationships_ex(self._h, arr, n, self._preconds_ex(preconditions), len(preconditions)))
+            return
         pre = (_Precond * max(len(preconditions), 1))()
         for i, (op, f) in enumerate(preconditions):
             pre[i] = _Precond(int(op), self._filter(f))
@@ -572,7 +593,26 @@ class Engine:
         return _RelStr(_b(f.get("res_type", "")), _b(f.get("res_id", "")), _b(f.get("rel", "")),
                        _b(f.get("subj_type", "")), _b(f.get("subj_id", "")), _b(f.get("subj_rel", "")))
 
+    # A filter dict's "res_id_prefix" (optional_resource_id_prefix) goes through the _ex calls, and only when set: a
+    # filter without one takes the calls it always took.
+    @staticmethod
+    def _any_prefix(filters) -> bool:
+        return any(f.get("res_id_prefix") for f in filters)
+
+    @classmethod
+    def _filter_ex(cls, f):
+        return _FilterEx(cls._filter(f), _b(f.get("res_id_prefix") or ""))
+
+    @classmethod
+    def _preconds_ex(cls, preconditions):
+        pre = (_PrecondEx * max(len(preconditions), 1))()
+        for i, (op, f) in enumerate(preconditions):
+            pre[i] = _PrecondEx(int(op), cls._filter_ex(f))
+        return pre
+
     def delete_relationships(self, flt: dict, preconditions=()):
+        if self._any_prefix([flt, *(f for _, f in preconditions)]):
+            return self.delete_relationships_limited(flt, preconditions)[0]
         pre = (_Precond * max(len(preconditions), 1))()
         for i, (op, f) in enumerate(preconditions):
             pre[i] = _Precond(int(op), self._filter(f))
@@ -589,12 +629,16 @@ class Engine:
         return n.value
 
     def read_relationships(self, **flt):
-        f = self._filter(flt)
+        """ReadRelationships: the matching lines, sorted. flt: res_type, res_id, res_id_prefix, rel, subj_type,
+        subj_id, subj_rel."""
+        ex = self._any_prefix([flt])
+        f = self._filter_ex(flt) if ex else self._filter(flt)
+        read = self._L.zg_read_relationships_ex if ex else self._L.zg_read_relationships
         cap = 1 << 16
         while True:
             buf = C.create_string_buffer(cap)
             need, n = C.c_size_t(0), C.c_uint64(0)
-            rc = self._L.zg_read_relationships(self._h, C.byref(f), buf, cap, C.byref(need), C.byref(n))
+            rc = read(self._h, C.byref(f), buf, cap, C.byref(need), C.byref(n))
             if rc == E2BIG:
                 cap = need.value + 16
                 continue
@@ -605,7 +649,9 @@ class Engine:
         """zg_read_relationships_page -> (lines, expires, cursors, next, more): the first `limit` relationships matching
         the filter after `cursor` (None: from the start) in the page order, their expirations (0 = none), the cursor
         after each line, the cursor after the page and whether more follow. Cursors are opaque bytes."""
-        f = self._filter(flt)
+        ex = self._any_prefix([flt])
+        f = self._filter_ex(flt) if ex else self._filter(flt)
+        page = self._L.zg_read_relationships_page_ex if ex else self._L.zg_read_relationships_page
         after = None if cursor is None else C.create_string_buffer(bytes(cursor), READ_CURSOR_BYTES)
         cap = max(1 << 16, min(int(limit), 1 << 18) * 64)  # a line rarely takes more: no second run of the page
         while True:
@@ -615,8 +661,8 @@ class Engine:
             exp = np.zeros(rows, dtype=np.uint32)
             curs = C.create_string_buffer(rows * READ_CURSOR_BYTES)
             nxt = C.create_string_buffer(READ_CURSOR_BYTES)
-            rc = self._L.zg_read_relationships_page(self._h, C.byref(f), int(limit), after, buf, cap, C.byref(need),
-                                                    C.byref(n), exp.ctypes.data, curs, nxt, C.byref(more))
+            rc = page(self._h, C.byref(f), int(limit), after, buf, cap, C.byref(need), C.byref(n), exp.ctypes.data, curs,
+                      nxt, C.byref(more))
             if rc == E2BIG:
                 cap = need.value + 16
                 continue
@@ -640,6 +686,13 @@ class Engine:
         """zg_delete_relationships_limited -> (deleted, partial). limit 0 deletes every match; otherwise more than
         `limit` matches raise ZgpuError(ZG_EPRECOND) unless allow_partial, which deletes the first `limit` of them in
         the page order and returns partial=True."""
+        if self._any_prefix([flt, *(f for _, f in preconditions)]):
+            n, partial = C.c_uint64(0), C.c_int32(0)
+            f = self._filter_ex(flt)
+            self._ck(self._L.zg_delete_relationships_limited_ex(self._h, C.byref(f), self._preconds_ex(preconditions),
+                                                                len(preconditions), int(limit), 1 if allow_partial else 0,
+                                                                C.byref(n), C.byref(partial)))
+            return n.value, bool(partial.value)
         pre = (_Precond * max(len(preconditions), 1))()
         for i, (op, f) in enumerate(preconditions):
             pre[i] = _Precond(int(op), self._filter(f))
@@ -655,6 +708,15 @@ class Engine:
         out = np.zeros(4, dtype=np.uint64)
         self._ck(self._L.zg_page_counters(self._h, out.ctypes.data))
         return dict(zip(("device_pages", "host_pages", "scanned", "launches"), (int(x) for x in out)))
+
+    PREFIX_COUNTERS = ("device_filters", "host_filters", "names_scanned", "matched", "launches", "mirror_syncs")
+
+    def prefix_counters(self) -> dict:
+        """zg_prefix_counters: prefix filters answered on the device / by the host store, names the device scanned,
+        resources it matched, launches of the prefix scans and their match lists, names-mirror syncs that uploaded."""
+        out = np.zeros(len(self.PREFIX_COUNTERS), dtype=np.uint64)
+        self._ck(self._L.zg_prefix_counters(self._h, out.ctypes.data))
+        return {k: int(v) for k, v in zip(self.PREFIX_COUNTERS, out)}
 
     # -- hot path ---------------------------------------------------------------
     def watch_read(self, since_revision: int, res_type: str = ""):

@@ -232,9 +232,13 @@ class RelationshipFilter:
     optional_resource_id: str = ""
     optional_relation: str = ""
     optional_subject_filter: Optional[SubjectFilter] = None
+    # only relationships whose resource's id starts with it (every resource type when resource_type is empty)
+    optional_resource_id_prefix: str = ""
 
     def fields(self) -> dict:
         f = {"res_type": self.resource_type, "res_id": self.optional_resource_id, "rel": self.optional_relation}
+        if self.optional_resource_id_prefix:
+            f["res_id_prefix"] = self.optional_resource_id_prefix
         if self.optional_subject_filter:
             s = self.optional_subject_filter
             f.update(subj_type=s.subject_type, subj_id=s.optional_subject_id, subj_rel=s.optional_relation)

@@ -250,6 +250,9 @@ struct zg_engine {
   std::atomic<uint64_t> flt_device{0}, flt_host{0}, flt_returned{0}, flt_shape[3] = {};
   // zg_page_counters: pages served on the device / by the host store, entries the device windows covered, launches
   std::atomic<uint64_t> pg_device{0}, pg_host{0}, pg_scanned{0}, pg_launches{0};
+  // zg_prefix_counters: prefix filters answered on the device / by the host store, names the device scanned, resources
+  // it matched, launches of the scans and match lists, names-mirror syncs that uploaded bytes
+  std::atomic<uint64_t> px_device{0}, px_host{0}, px_names{0}, px_matched{0}, px_launches{0}, px_syncs{0};
   // zg_lookup_page_counters: LookupResources pages answered by windowed verification / cut from a whole answer (a
   // sharded handle), candidates after the cursor, candidates verified, verification windows
   std::atomic<uint64_t> lp_windowed{0}, lp_cut{0}, lp_after{0}, lp_verified{0}, lp_windows{0};
@@ -828,10 +831,28 @@ static std::string resolve_write(zg_engine* e, const zg_rel_str& r, zg_tuple* t)
   return "";
 }
 
-static Store::Filter resolve_filter(const zg_engine* e, const zg_filter_str& f, std::string* err) {
+// SpiceDB's pattern for optional_resource_id_prefix: 1..1024 characters of [a-zA-Z0-9/_|\-=+] ("*" is not one).
+static bool valid_id_prefix(const char* p) {
+  const size_t n = std::strlen(p);
+  return n <= 1024 && valid_object_id(p, n) && std::strcmp(p, "*") != 0;
+}
+
+static Store::Filter resolve_filter(const zg_engine* e, const zg_filter_ex& fx, std::string* err) {
   const Schema& sc = e->schema;
+  const zg_filter_str& f = fx.f;
   Store::Filter o;
   auto set = [](const char* s) { return s && *s; };
+  if (set(fx.res_id_prefix)) {
+    if (!valid_id_prefix(fx.res_id_prefix)) {
+      *err = std::string("invalid resource id prefix `") + fx.res_id_prefix + "`";
+      return o;
+    }
+    if (set(f.res_id)) {
+      *err = "resource id and resource id prefix cannot both be given";
+      return o;
+    }
+    o.prefix = fx.res_id_prefix;
+  }
   if (set(f.res_type)) {
     o.res_type = sc.type_id(f.res_type);
     if (o.res_type < 0) {
@@ -954,6 +975,26 @@ static int ask_devices(zg_engine* e, int which, Device::FilterShape shape, const
   return ZG_OK;
 }
 
+// A filter answered by the host store: counted in zg_filter_counters, and in zg_prefix_counters with a prefix.
+static void count_host(zg_engine* e, const Store::Filter& f) {
+  ++e->flt_host;
+  if (!f.prefix.empty()) ++e->px_host;
+}
+
+// The bitmaps of f's prefix (Device::prefix_scan), built once on the first device from the handle's names; every shard
+// of a sharded handle reads them there through peer memory (replicas answer on that device). *too_big: over the
+// output budget, and the caller answers on the host. Caller holds e->mu and e->names (shared is enough).
+static int prefix_on_device(zg_engine* e, const Store::Filter& f, PrefixBits* px, bool* too_big) {
+  PrefixStats st;
+  std::string err;
+  const int rc = e->dev.prefix_scan(e->store, e->schema, f.res_type, f.prefix, px, &st, too_big, &err);
+  e->px_names += st.names;
+  e->px_matched += st.matched;
+  e->px_launches += st.launches;
+  e->px_syncs += st.syncs;
+  return rc ? fail(rc == ZG_ENOMEM ? ZG_ECUDA : rc, err) : ZG_OK;
+}
+
 // The device path of a filter. Caller holds e->mu and e->names (shared is enough) and has seen filters_on_device.
 // *count = the matching relationships; with `tuples`, the records in no particular order. A sharded handle asks every
 // shard (they own disjoint relationships), or the owner alone when the resource is given; replicas hold the same
@@ -961,10 +1002,19 @@ static int ask_devices(zg_engine* e, int which, Device::FilterShape shape, const
 // caller runs Store::match instead (holding e->names exclusively).
 static int match_on_device(zg_engine* e, const Store::Filter& f, uint32_t now, uint64_t* count, std::vector<zg_tuple>* tuples,
                            bool* too_big) {
-  return ask_devices(e, snapshot_devices(e, &f), Device::filter_shape(f), [&](Device& dev, uint64_t* n, std::vector<zg_tuple>* got, bool* big,
+  PrefixBits px;
+  const bool has_prefix = !f.prefix.empty();
+  if (has_prefix) {
+    *count = 0;
+    if (int rc = prefix_on_device(e, f, &px, too_big)) return rc;
+    if (*too_big) return ZG_OK;
+  }
+  const int rc = ask_devices(e, snapshot_devices(e, &f), Device::filter_shape(f), [&](Device& dev, uint64_t* n, std::vector<zg_tuple>* got, bool* big,
                                                             std::string* err) {
-    return dev.match_filter(e->schema, f, now, n, got, nullptr, big, err);
+    return dev.match_filter(e->schema, f, now, n, got, nullptr, big, err, has_prefix ? &px : nullptr);
   }, count, tuples, too_big);
+  if (!rc && has_prefix && !*too_big) ++e->px_device;
+  return rc;
 }
 
 // Removes the relationships a delete by filter or a collection found. On the device path the records `found` (any
@@ -990,7 +1040,7 @@ static int delete_found(zg_engine* e, const char* what, const std::vector<zg_tup
 }
 
 // Caller holds e->mu AND e->names exclusively (every writer does).
-static int check_preconditions(zg_engine* e, const zg_precondition_str* pre, uint64_t n_pre) {
+static int check_preconditions(zg_engine* e, const zg_precondition_ex* pre, uint64_t n_pre) {
   std::vector<uint64_t> idx;
   const bool on_device = n_pre && filters_on_device(e);
   for (uint64_t i = 0; i < n_pre; ++i) {
@@ -998,12 +1048,13 @@ static int check_preconditions(zg_engine* e, const zg_precondition_str* pre, uin
     Store::Filter f = resolve_filter(e, pre[i].filter, &err);
     if (!err.empty()) return fail(ZG_EINVAL, "precondition " + std::to_string(i) + ": " + err);
     uint64_t count = 0;
-    bool too_big = false;  // never: a count needs no output
+    bool too_big = false;  // a count needs no output: only a prefix's bitmaps can be over the budget
     if (on_device) {
       if (int rc = match_on_device(e, f, now_of(e), &count, nullptr, &too_big)) return rc;
-    } else {
+    }
+    if (!on_device || too_big) {
       e->store.match(f, now_of(e), &idx);
-      ++e->flt_host;
+      count_host(e, f);
       count = idx.size();
     }
     const bool any = count != 0;
@@ -1017,8 +1068,22 @@ static int check_preconditions(zg_engine* e, const zg_precondition_str* pre, uin
   return ZG_OK;
 }
 
+// The preconditions of the calls without _ex, with the prefix unset.
+static std::vector<zg_precondition_ex> pre_ex(const zg_precondition_str* pre, uint64_t n_pre) {
+  std::vector<zg_precondition_ex> x(pre ? n_pre : 0);
+  for (size_t i = 0; i < x.size(); ++i) x[i] = zg_precondition_ex{pre[i].op, zg_filter_ex{pre[i].filter, nullptr}};
+  return x;
+}
+
 extern "C" int zg_write_relationships(zg_engine* e, const zg_update_str* ups, uint64_t n, const zg_precondition_str* pre,
                                       uint64_t n_pre) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (!pre && n_pre) return fail(ZG_EINVAL, "NULL argument");
+  return zg_write_relationships_ex(e, ups, n, pre_ex(pre, n_pre).data(), n_pre);
+}
+
+extern "C" int zg_write_relationships_ex(zg_engine* e, const zg_update_str* ups, uint64_t n, const zg_precondition_ex* pre,
+                                         uint64_t n_pre) {
   NEED_SCHEMA(e, ZG_ENOSCHEMA);
   if ((!ups && n) || (!pre && n_pre)) return fail(ZG_EINVAL, "NULL argument");
   if (n > 1000)  // pkg/spicedb/spicedb.go:34 WithMaximumUpdatesPerWrite(1000)
@@ -1413,8 +1478,8 @@ extern "C" int zg_import_last_times(zg_engine* e, double* ms) {
   return ZG_OK;
 }
 
-extern "C" int zg_delete_relationships(zg_engine* e, const zg_filter_str* filter, const zg_precondition_str* pre,
-                                       uint64_t n_pre, uint64_t* n_deleted) {
+static int delete_all(zg_engine* e, const zg_filter_ex* filter, const zg_precondition_ex* pre, uint64_t n_pre,
+                      uint64_t* n_deleted) {
   NEED_SCHEMA(e, ZG_ENOSCHEMA);
   if (!filter || (!pre && n_pre)) return fail(ZG_EINVAL, "NULL argument");
   LOCK_DEVICE(e);
@@ -1436,13 +1501,21 @@ extern "C" int zg_delete_relationships(zg_engine* e, const zg_filter_str* filter
   }
   if (!on_device) {
     e->store.match(f, 0, &idx);
-    ++e->flt_host;
+    count_host(e, f);
   }
   std::vector<zg_update> u;
   std::vector<uint8_t> changed;
   rc = delete_found(e, "delete by filter", on_device ? &found : nullptr, &idx, &u, &changed, n_deleted);
   if (rc == ZG_OK) e->log_changes(u, changed);
   return rc;
+}
+
+extern "C" int zg_delete_relationships(zg_engine* e, const zg_filter_str* filter, const zg_precondition_str* pre,
+                                       uint64_t n_pre, uint64_t* n_deleted) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (!filter || (!pre && n_pre)) return fail(ZG_EINVAL, "NULL argument");
+  const zg_filter_ex f{*filter, nullptr};
+  return delete_all(e, &f, pre_ex(pre, n_pre).data(), n_pre, n_deleted);
 }
 
 extern "C" int zg_collect_expired(zg_engine* e, int64_t before_unix, uint64_t* n_removed) {
@@ -1577,6 +1650,14 @@ extern "C" int zg_read_relationships(zg_engine* e, const zg_filter_str* filter, 
                                      uint64_t* n_out) {
   NEED_SCHEMA(e, ZG_ENOSCHEMA);
   if (!filter) return fail(ZG_EINVAL, "NULL filter");
+  const zg_filter_ex f{*filter, nullptr};
+  return zg_read_relationships_ex(e, &f, buf, cap, need, n_out);
+}
+
+extern "C" int zg_read_relationships_ex(zg_engine* e, const zg_filter_ex* filter, char* buf, size_t cap, size_t* need,
+                                        uint64_t* n_out) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (!filter) return fail(ZG_EINVAL, "NULL filter");
   // Device path: the device lock, then the names lock SHARED, the order every other call uses; checks keep resolving
   // their strings beside the read, and the store's relationship index is never built. Host scan: the names lock
   // exclusively, since match() may (re)build that index.
@@ -1604,7 +1685,7 @@ extern "C" int zg_read_relationships(zg_engine* e, const zg_filter_str* filter, 
   if (!on_device) {
     std::vector<uint64_t> idx;
     e->store.match(f, now_of(e), &idx);
-    ++e->flt_host;
+    count_host(e, f);
     found.reserve(idx.size());
     for (uint64_t i : idx) found.push_back(e->store.tuples[i]);
   }
@@ -1646,7 +1727,7 @@ constexpr uint16_t kCursorVersion = 1;
 constexpr uint16_t kLookupCursorVersion = 0x8001;
 constexpr uint16_t kPastIds = 2;
 
-static uint64_t filter_fingerprint(const Store::Filter& f, const zg_filter_str& s) {
+static uint64_t filter_fingerprint(const Store::Filter& f, const zg_filter_str& s) {  // f.prefix: mixed in when set
   uint64_t h = 0xcbf29ce484222325ull;
   auto mix = [&](const void* p, size_t n) {
     for (size_t i = 0; i < n; ++i) h = (h ^ static_cast<const uint8_t*>(p)[i]) * 0x100000001b3ull;
@@ -1657,6 +1738,13 @@ static uint64_t filter_fingerprint(const Store::Filter& f, const zg_filter_str& 
     const size_t n = str ? std::strlen(str) : 0;
     mix(&n, sizeof n);
     if (n) mix(str, n);
+  }
+  if (!f.prefix.empty()) {  // an unprefixed filter's cursors stay those it always had
+    const char tag[] = "prefix";
+    mix(tag, sizeof tag);
+    const size_t n = f.prefix.size();
+    mix(&n, sizeof n);
+    mix(f.prefix.data(), n);
   }
   return h;
 }
@@ -1688,9 +1776,16 @@ static int page_on_device(zg_engine* e, const Store::Filter& f, uint32_t now, co
   std::vector<Device::PageStats> st(S);
   std::vector<char> big(S, 0);
   std::string err;
+  PrefixBits px;
+  const bool has_prefix = !f.prefix.empty();
+  if (has_prefix) {
+    if (int rc = prefix_on_device(e, f, &px, too_big)) return rc;
+    if (*too_big) return ZG_OK;
+  }
   if (int rc = on_devices(e, snapshot_devices(e, &f), [&](Device& dev, size_t k, std::string* m) {
         bool b = false;
-        const int prc = dev.page_filter(e->schema, f, now, after, want, &got[k], &got_exp[k], &st[k], &b, m);
+        const int prc = dev.page_filter(e->schema, f, now, after, want, &got[k], &got_exp[k], &st[k], &b, m,
+                                        has_prefix ? &px : nullptr);
         big[k] = b;
         return prc;
       }, &err))
@@ -1718,7 +1813,9 @@ static int page_on_device(zg_engine* e, const Store::Filter& f, uint32_t now, co
   for (const auto& x : st) {
     e->pg_scanned += x.scanned;
     e->pg_launches += x.launches;
+    e->px_launches += x.list_launches;
   }
+  if (has_prefix) ++e->px_device;
   ++e->flt_device;
   ++e->flt_shape[Device::filter_shape(f)];
   e->flt_returned += found->size();
@@ -1737,12 +1834,21 @@ static void page_on_host(zg_engine* e, const Store::Filter& f, uint32_t now, con
     exp->push_back(e->store.expires[i]);
   }
   ++e->pg_host;
-  ++e->flt_host;
+  count_host(e, f);
 }
 
 extern "C" int zg_read_relationships_page(zg_engine* e, const zg_filter_str* filter, uint64_t limit, const zg_read_cursor* after,
                                           char* buf, size_t cap, size_t* need, uint64_t* n_out, uint32_t* expires,
                                           zg_read_cursor* cursors, zg_read_cursor* next, int32_t* more) {
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (!filter) return fail(ZG_EINVAL, "NULL filter");
+  const zg_filter_ex f{*filter, nullptr};
+  return zg_read_relationships_page_ex(e, &f, limit, after, buf, cap, need, n_out, expires, cursors, next, more);
+}
+
+extern "C" int zg_read_relationships_page_ex(zg_engine* e, const zg_filter_ex* filter, uint64_t limit, const zg_read_cursor* after,
+                                             char* buf, size_t cap, size_t* need, uint64_t* n_out, uint32_t* expires,
+                                             zg_read_cursor* cursors, zg_read_cursor* next, int32_t* more) {
   NEED_SCHEMA(e, ZG_ENOSCHEMA);
   if (!filter) return fail(ZG_EINVAL, "NULL filter");
   if (limit == 0) return fail(ZG_EINVAL, "page limit must be at least 1 (zg_read_relationships reads without one)");
@@ -1757,7 +1863,7 @@ extern "C" int zg_read_relationships_page(zg_engine* e, const zg_filter_str* fil
   std::string err;
   Store::Filter f = resolve_filter(e, *filter, &err);
   if (!err.empty()) return fail(ZG_EINVAL, err);
-  const uint64_t fp = filter_fingerprint(f, *filter);
+  const uint64_t fp = filter_fingerprint(f, filter->f);
   CursorBits c{};
   if (after) {
     std::memcpy(&c, after->opaque, sizeof c);
@@ -1826,6 +1932,17 @@ extern "C" int zg_delete_relationships_limited(zg_engine* e, const zg_filter_str
   if (limit == 0) return zg_delete_relationships(e, filter, pre, n_pre, n_deleted);
   NEED_SCHEMA(e, ZG_ENOSCHEMA);
   if (!filter || (!pre && n_pre)) return fail(ZG_EINVAL, "NULL argument");
+  const zg_filter_ex f{*filter, nullptr};
+  return zg_delete_relationships_limited_ex(e, &f, pre_ex(pre, n_pre).data(), n_pre, limit, allow_partial, n_deleted, partial);
+}
+
+extern "C" int zg_delete_relationships_limited_ex(zg_engine* e, const zg_filter_ex* filter, const zg_precondition_ex* pre,
+                                                  uint64_t n_pre, uint64_t limit, int allow_partial, uint64_t* n_deleted,
+                                                  int32_t* partial) {
+  if (partial) *partial = 0;
+  if (limit == 0) return delete_all(e, filter, pre, n_pre, n_deleted);
+  NEED_SCHEMA(e, ZG_ENOSCHEMA);
+  if (!filter || (!pre && n_pre)) return fail(ZG_EINVAL, "NULL argument");
   LOCK_DEVICE(e);
   LOCK_NAMES_UNIQUE(e);
   std::string err;
@@ -1863,6 +1980,14 @@ extern "C" int zg_delete_relationships_limited(zg_engine* e, const zg_filter_str
 extern "C" int zg_page_counters(zg_engine* e, uint64_t* out) {
   if (!e || !out) return fail(ZG_EINVAL, "NULL argument");
   const uint64_t c[4] = {e->pg_device.load(), e->pg_host.load(), e->pg_scanned.load(), e->pg_launches.load()};
+  std::memcpy(out, c, sizeof c);
+  return ZG_OK;
+}
+
+extern "C" int zg_prefix_counters(zg_engine* e, uint64_t* out) {
+  if (!e || !out) return fail(ZG_EINVAL, "NULL argument");
+  const uint64_t c[6] = {e->px_device.load(), e->px_host.load(), e->px_names.load(), e->px_matched.load(),
+                         e->px_launches.load(), e->px_syncs.load()};
   std::memcpy(out, c, sizeof c);
   return ZG_OK;
 }

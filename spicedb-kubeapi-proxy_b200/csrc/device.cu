@@ -2847,6 +2847,8 @@ int Device::lookup_subjects(uint16_t res_type, uint32_t res, uint16_t perm, uint
 
 // ---- relationship filters (filter.cuh) --------------------------------------------------------
 
+static unsigned ingress_grid(uint64_t n, int sm_count);  // device ingress, below
+
 // The classes whose relation, subject type and subject relation agree with the filter, in data-relation order.
 static void select_classes(const Schema& sc, const Snapshot& s, const Store::Filter& f, std::vector<FilterSel>* sel) {
   sel->clear();
@@ -2877,8 +2879,15 @@ static void select_classes(const Schema& sc, const Snapshot& s, const Store::Fil
   }
 }
 
+// The bitmap of every selected class: its resource type's (px->type).
+static std::vector<const uint32_t*> class_bits(const PrefixBits& px, const std::vector<FilterSel>& sel) {
+  std::vector<const uint32_t*> bits(sel.size());
+  for (size_t k = 0; k < sel.size(); ++k) bits[k] = px.type[sel[k].rtype];
+  return bits;
+}
+
 int Device::match_filter(const Schema& sc, const Store::Filter& f, uint32_t now, uint64_t* count, std::vector<zg_tuple>* tuples,
-                         std::vector<uint32_t>* expires, bool* too_big, std::string* err) {
+                         std::vector<uint32_t>* expires, bool* too_big, std::string* err, const PrefixBits* px) {
   *count = 0;
   *too_big = false;
   if (tuples) tuples->clear();
@@ -2897,7 +2906,9 @@ int Device::match_filter(const Schema& sc, const Store::Filter& f, uint32_t now,
   p.res = f.res;
   p.subj = f.has_subj ? f.subj : 0;
   p.now = now;
-  return run_filter(sc, *s, sel, p, filter_shape(f), false, count, tuples, expires, too_big, err);
+  if (!px) return run_filter(sc, *s, sel, p, filter_shape(f), false, count, tuples, expires, too_big, err);
+  const std::vector<const uint32_t*> bits = class_bits(*px, sel);
+  return run_filter(sc, *s, sel, p, filter_shape(f), false, count, tuples, expires, too_big, err, &bits, px->bytes);
 }
 
 int Device::match_expired(const Schema& sc, uint32_t before, uint64_t* count, std::vector<zg_tuple>* tuples, bool* too_big,
@@ -2935,7 +2946,7 @@ int Device::match_expired(const Schema& sc, uint32_t before, uint64_t* count, st
 
 int Device::run_filter(const Schema& sc, const Snapshot& s, const std::vector<FilterSel>& sel, FilterPlan& p, FilterShape shape,
                        bool expired, uint64_t* count, std::vector<zg_tuple>* tuples, std::vector<uint32_t>* expires,
-                       bool* too_big, std::string* err) {
+                       bool* too_big, std::string* err, const std::vector<const uint32_t*>* bits, uint64_t held) {
   ZG_CUDA(cudaSetDevice(device));
   if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
   if (!flt_ctrl_.ensure(8)) {
@@ -2955,7 +2966,16 @@ int Device::run_filter(const Schema& sc, const Snapshot& s, const std::vector<Fi
     for (size_t at = 0; at < sel.size(); at += kMaxFilterSel) {
       p.n_sel = static_cast<uint32_t>(std::min<size_t>(kMaxFilterSel, sel.size() - at));
       std::copy(sel.begin() + at, sel.begin() + at + p.n_sel, p.sel);
-      if (expired) {
+      if (bits) {  // a prefix: the resource shape never has one (res_id and a prefix are refused together)
+        std::copy(bits->begin() + at, bits->begin() + at + p.n_sel, p.bits);
+        if (shape == kBySubject) {
+          if (emit) filter_subject_kernel<true, true><<<grid, kFilterThreads, 0, stream>>>(p);
+          else filter_subject_kernel<false, true><<<grid, kFilterThreads, 0, stream>>>(p);
+        } else {
+          if (emit) filter_scan_kernel<true, true><<<grid, kFilterThreads, 0, stream>>>(p);
+          else filter_scan_kernel<false, true><<<grid, kFilterThreads, 0, stream>>>(p);
+        }
+      } else if (expired) {
         if (emit) filter_expired_kernel<true><<<grid, kFilterThreads, 0, stream>>>(p);
         else filter_expired_kernel<false><<<grid, kFilterThreads, 0, stream>>>(p);
       } else if (shape == kByResource) {
@@ -2982,7 +3002,7 @@ int Device::run_filter(const Schema& sc, const Snapshot& s, const std::vector<Fi
   size_t free_b = 0, total_b = 0;
   ZG_CUDA(cudaMemGetInfo(&free_b, &total_b));
   const size_t bytes = n * (sizeof(zg_tuple) + 4);
-  if (bytes > flt_out_.cap + flt_exp_.cap && bytes > free_b / 4) {
+  if (bytes > flt_out_.cap + flt_exp_.cap && bytes + held > free_b / 4) {
     *too_big = true;
     return ZG_OK;
   }
@@ -3010,7 +3030,7 @@ int Device::run_filter(const Schema& sc, const Snapshot& s, const std::vector<Fi
 
 int Device::page_filter(const Schema& sc, const Store::Filter& f, uint32_t now, const PageKey* after, uint64_t want,
                         std::vector<zg_tuple>* tuples, std::vector<uint32_t>* expires, PageStats* st, bool* too_big,
-                        std::string* err) {
+                        std::string* err, const PrefixBits* px) {
   tuples->clear();
   expires->clear();
   *too_big = false;
@@ -3034,7 +3054,14 @@ int Device::page_filter(const Schema& sc, const Store::Filter& f, uint32_t now, 
   ZG_CUDA(cudaMemGetInfo(&free_b, &total_b));
   const uint64_t segs = shape == kBySubject ? sel.size() : 1;
   const uint64_t bytes = segs * want * (sizeof(zg_tuple) + 4);
-  bool fits = bytes <= flt_out_.cap + flt_exp_.cap || bytes <= free_b / 4;
+  // a prefix: its bitmaps, and for the scan shape the largest match list (ids, entries, their sums, the word scan)
+  uint64_t held = 0;
+  if (px) {
+    held = px->bytes;
+    if (shape == kByScan)
+      for (const FilterSel& x : sel) held = std::max<uint64_t>(held, px->bytes + uint64_t(px->n_ids[x.rtype]) * 24 + (1u << 20));
+  }
+  bool fits = bytes <= flt_out_.cap + flt_exp_.cap ? held <= free_b / 4 : bytes + held <= free_b / 4;
   for (size_t g = 0, g0 = 0; fits && g <= sel.size(); ++g)
     if (g == sel.size() || sel[g].rtype != sel[g0].rtype) {
       fits = shape == kBySubject || g - g0 <= static_cast<size_t>(kMaxFilterSel);
@@ -3075,7 +3102,12 @@ int Device::page_filter(const Schema& sc, const Store::Filter& f, uint32_t now, 
       p.out = d_out + at * want;
       p.out_exp = d_exp + at * want;
       p.seg_count = pg_seg_.as<uint32_t>() + at;
-      page_subject_kernel<<<p.n_sel, 32, 0, stream>>>(p);
+      if (px) {
+        for (uint32_t k = 0; k < p.n_sel; ++k) p.bits[k] = px->type[p.sel[k].rtype];
+        page_subject_kernel<true><<<p.n_sel, 32, 0, stream>>>(p);
+      } else {
+        page_subject_kernel<<<p.n_sel, 32, 0, stream>>>(p);
+      }
       ++st->launches;
     }
     ZG_CUDA(cudaGetLastError());
@@ -3103,9 +3135,61 @@ int Device::page_filter(const Schema& sc, const Store::Filter& f, uint32_t now, 
     uint32_t* out_exp;
     PageStats* st;
     std::string* err;
+    const PrefixBits* px;
+    int list_type = -1;  // a prefix: the type whose match list px_ids_ / px_sum_ hold
+    uint32_t list_m = 0;
+    // A prefix page: the ascending ids of the type's matches and the exclusive sum of their entries in the block.
+    int build_list(const PagePlan& p, unsigned long long block, uint32_t stride) {
+      const int type = p.sel[0].rtype;
+      const uint32_t n_ids = px->n_ids[type], words = (n_ids + 31) / 32, nres = p.sel[0].nres;
+      const uint32_t* bits = px->type[type];
+      size_t t1 = 0, t2 = 0;
+      cub::DeviceScan::ExclusiveSum(nullptr, t1, d->px_first_.as<uint32_t>(), d->px_first_.as<uint32_t>(),
+                                    static_cast<int64_t>(words) + 1, d->stream);
+      cub::DeviceScan::ExclusiveSum(nullptr, t2, d->px_ent_.as<unsigned long long>(), d->px_sum_.as<unsigned long long>(),
+                                    static_cast<int64_t>(n_ids) + 1, d->stream);
+      if (!d->px_first_.ensure((uint64_t(words) + 1) * 4) || !d->px_ids_.ensure((uint64_t(n_ids) + 1) * 4) ||
+          !d->px_ent_.ensure((uint64_t(n_ids) + 1) * 8) || !d->px_sum_.ensure((uint64_t(n_ids) + 1) * 8) ||
+          !d->px_tmp_.ensure(std::max(t1, t2))) {
+        if (err) *err = "out of device memory (prefix match list)";
+        return ZG_ENOMEM;
+      }
+      uint32_t* first = d->px_first_.as<uint32_t>();
+      const unsigned grid = ingress_grid(uint64_t(words) + 1, d->sm_count_);
+      prefix_word_count_kernel<<<grid, kFilterThreads, 0, d->stream>>>(bits, words, first);
+      ZG_CUDA(cudaGetLastError());
+      if (cub::DeviceScan::ExclusiveSum(d->px_tmp_.p, t1, first, first, static_cast<int64_t>(words) + 1, d->stream) != cudaSuccess) {
+        if (err) *err = "page: the scan of the prefix bitmap failed";
+        return ZG_ECUDA;
+      }
+      uint32_t m = 0;
+      ZG_CUDA(cudaMemcpyAsync(&m, first + words, 4, cudaMemcpyDeviceToHost, d->stream));
+      prefix_list_kernel<<<grid, kFilterThreads, 0, d->stream>>>(bits, words, first, p.row_ptr, block, stride, nres,
+                                                                d->px_ids_.as<uint32_t>(), d->px_ent_.as<unsigned long long>());
+      ZG_CUDA(cudaGetLastError());
+      ZG_CUDA(cudaStreamSynchronize(d->stream));
+      if (cub::DeviceScan::ExclusiveSum(d->px_tmp_.p, t2, d->px_ent_.as<unsigned long long>(), d->px_sum_.as<unsigned long long>(),
+                                        static_cast<int64_t>(m) + 1, d->stream) != cudaSuccess) {
+        if (err) *err = "page: the scan of the prefix match list failed";
+        return ZG_ECUDA;
+      }
+      st->launches += 4;
+      st->list_launches += 4;
+      list_type = type;
+      list_m = m;
+      return ZG_OK;
+    }
     int window(const PagePlan& p, unsigned long long block, uint32_t stride, uint32_t obj0, unsigned long long entries,
                uint32_t* obj1, unsigned long long* n) {
-      page_window_kernel<<<1, 32, 0, d->stream>>>(p.row_ptr, block, stride, obj0, p.sel[0].nres, entries, ctrl);
+      if (px) {
+        if (list_type != p.sel[0].rtype)
+          if (int rc = build_list(p, block, stride)) return rc;
+        prefix_window_kernel<<<1, 32, 0, d->stream>>>(d->px_ids_.as<uint32_t>(), d->px_sum_.as<unsigned long long>(), list_m,
+                                                      obj0, p.sel[0].nres, entries, ctrl);
+        ++st->list_launches;
+      } else {
+        page_window_kernel<<<1, 32, 0, d->stream>>>(p.row_ptr, block, stride, obj0, p.sel[0].nres, entries, ctrl);
+      }
       ++st->launches;
       ZG_CUDA(cudaGetLastError());
       unsigned long long h[2];
@@ -3132,23 +3216,28 @@ int Device::page_filter(const Schema& sc, const Store::Filter& f, uint32_t now, 
       const unsigned grid = static_cast<unsigned>(
           std::max<uint64_t>(1, std::min<uint64_t>((n_tiles + warps_per_block - 1) / warps_per_block, uint64_t(d->sm_count_) * 16)));
       ZG_CUDA(cudaMemsetAsync(p.tile_count + n_tiles, 0, 8, d->stream));
-      page_count_kernel<<<grid, kFilterThreads, 0, d->stream>>>(p);
+      if (px) page_count_kernel<true><<<grid, kFilterThreads, 0, d->stream>>>(p);
+      else page_count_kernel<<<grid, kFilterThreads, 0, d->stream>>>(p);
       ZG_CUDA(cudaGetLastError());
       if (cub::DeviceScan::ExclusiveSum(d->pg_tmp_.p, tmp, p.tile_count, d->pg_off_.as<unsigned long long>(),
                                         static_cast<int64_t>(n_tiles + 1), d->stream) != cudaSuccess) {
         if (err) *err = "page: the scan of the tile counts failed";
         return ZG_ECUDA;
       }
-      page_emit_kernel<<<grid, kFilterThreads, 0, d->stream>>>(p);
+      if (px) page_emit_kernel<true><<<grid, kFilterThreads, 0, d->stream>>>(p);
+      else page_emit_kernel<<<grid, kFilterThreads, 0, d->stream>>>(p);
       ZG_CUDA(cudaGetLastError());
       st->launches += 3;
       ZG_CUDA(cudaMemcpyAsync(total, p.tile_off + n_tiles, 8, cudaMemcpyDeviceToHost, d->stream));
       ZG_CUDA(cudaStreamSynchronize(d->stream));
       return ZG_OK;
     }
-  } ops{this, ctrl, d_out, d_exp, st, err};
+  } ops{this, ctrl, d_out, d_exp, st, err, px};
   unsigned long long got = 0;
-  if (int rc = page_walk(ops, p, sel, shape == kByResource, f.res, after, want, &got, &st->scanned)) return rc;
+  std::vector<const uint32_t*> bits;
+  if (px) bits = class_bits(*px, sel);
+  if (int rc = page_walk(ops, p, sel, shape == kByResource, f.res, after, want, &got, &st->scanned, px ? &bits : nullptr))
+    return rc;
   tuples->resize(got);
   expires->resize(got);
   if (got) {
@@ -3197,6 +3286,97 @@ int Device::scan_mentions(const Schema& sc, Store::IdBits* bits, std::string* er
     if (b.size() < n) b.resize(n, 0);
     for (uint64_t i = 0; i < n; ++i) b[i] |= host[types[t].word0 + i];
   }
+  return ZG_OK;
+}
+
+// ---- resource id prefixes ---------------------------------------------------------------------
+
+int Device::prefix_scan(const Store& store, const Schema& sc, int res_type, const std::string& prefix, PrefixBits* out,
+                        PrefixStats* st, bool* too_big, std::string* err) {
+  *too_big = false;
+  std::shared_ptr<Snapshot> s = snap;
+  if (!s) {
+    if (err) *err = "no snapshot published";
+    return ZG_ENOSNAPSHOT;
+  }
+  // the types a filter of res_type may select, each covering the larger of its object capacity and its rows
+  const size_t nt = sc.types.size();
+  out->type.assign(nt, nullptr);
+  out->n_ids.assign(nt, 0);
+  std::vector<uint64_t> word0(nt, 0);
+  std::vector<char> want(nt, 0);
+  for (size_t ri = 0; ri < sc.rel_slots.size() && ri < s->rels.size(); ++ri) {
+    const int t = sc.slots[sc.rel_slots[ri]].type;
+    if (res_type >= 0 && t != res_type) continue;
+    want[t] = 1;
+    out->n_ids[t] = std::max(out->n_ids[t], s->rels[ri].nres);
+  }
+  uint64_t words = 0;
+  for (size_t t = 0; t < nt; ++t) {
+    if (!want[t]) continue;
+    if (t < s->n_objects.size()) out->n_ids[t] = std::max(out->n_ids[t], s->n_objects[t]);
+    word0[t] = words;
+    words += (uint64_t(out->n_ids[t]) + 31) / 32;
+  }
+  out->bytes = words * 4;
+  ZG_CUDA(cudaSetDevice(device));
+  size_t free_b = 0, total_b = 0;
+  ZG_CUDA(cudaMemGetInfo(&free_b, &total_b));
+  if (out->bytes > px_bits_.cap && out->bytes > free_b / 4) {
+    *too_big = true;
+    return ZG_OK;
+  }
+  if (have_last_) ZG_CUDA(cudaStreamWaitEvent(stream, last_done_, 0));
+  if (!px_bits_.ensure(std::max<uint64_t>(out->bytes, 4)) || !px_str_.ensure(prefix.size()) || !px_ctrl_.ensure(8)) {
+    if (err) *err = "out of device memory (prefix bitmaps)";
+    return ZG_ENOMEM;
+  }
+  const uint64_t uploads = ingress_ ? ingress_->sync_uploads : 0;
+  if (int rc = ingress_sync(store, stream, err)) {
+    if (rc != ZG_ENOMEM) return rc;
+    // the mirror did not fit: the host store answers, as for bitmaps over the budget. A sync that stopped part way
+    // leaves the mirror behind the store, so it is dropped and the next call builds it again.
+    ingress_reset();
+    *too_big = true;
+    return ZG_OK;
+  }
+  st->syncs += ingress_->sync_uploads - uploads;
+  PrefixPlan p{};
+  p.prefix = px_str_.as<uint8_t>();
+  p.len = prefix.size();
+  p.matched = px_ctrl_.as<unsigned long long>();
+  ZG_CUDA(cudaMemcpyAsync(px_str_.p, prefix.data(), prefix.size(), cudaMemcpyHostToDevice, stream));
+  ZG_CUDA(cudaMemsetAsync(px_bits_.p, 0, out->bytes, stream));
+  ZG_CUDA(cudaMemsetAsync(p.matched, 0, 8, stream));
+  std::vector<PrefixType> types;
+  uint64_t recs = 0;
+  for (size_t t = 0; t < nt; ++t) {
+    if (!want[t]) continue;
+    out->type[t] = px_bits_.as<uint32_t>() + word0[t];
+    if (t >= ingress_->types.size() || ingress_->types[t].host_offs.empty()) continue;  // no interned name
+    const IngressMirror::Type& y = ingress_->types[t];
+    PrefixType x{};
+    x.arena = y.arena.as<uint8_t>();
+    x.offs = y.offs.as<unsigned long long>();
+    x.n_recs = y.host_offs.size();
+    x.bits = px_bits_.as<uint32_t>() + word0[t];
+    x.n_ids = out->n_ids[t];
+    types.push_back(x);
+    recs = std::max<uint64_t>(recs, x.n_recs);
+  }
+  for (size_t at = 0; at < types.size(); at += kMaxPrefixTypes) {
+    p.n_types = static_cast<uint32_t>(std::min<size_t>(kMaxPrefixTypes, types.size() - at));
+    std::copy(types.begin() + at, types.begin() + at + p.n_types, p.type);
+    for (uint32_t k = 0; k < p.n_types; ++k) st->names += p.type[k].n_recs;
+    prefix_match_kernel<<<ingress_grid(recs, sm_count_), kIngressThreads, 0, stream>>>(p);
+    ++launches;
+    ++st->launches;
+  }
+  ZG_CUDA(cudaGetLastError());
+  unsigned long long matched = 0;
+  ZG_CUDA(cudaMemcpyAsync(&matched, p.matched, 8, cudaMemcpyDeviceToHost, stream));
+  ZG_CUDA(cudaStreamSynchronize(stream));
+  st->matched += matched;
   return ZG_OK;
 }
 

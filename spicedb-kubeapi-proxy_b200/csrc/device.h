@@ -130,6 +130,16 @@ struct PeerTable {
   unsigned long long base[kMaxShards];
 };
 
+// A prefix filter's bitmaps (Device::prefix_scan): per type, ids whose interned name has the prefix.
+struct PrefixBits {
+  std::vector<const uint32_t*> type;  // per type: its bitmap, nullptr when the filter cannot select the type
+  std::vector<uint32_t> n_ids;        // per type: the ids it covers (the snapshot's object capacity)
+  uint64_t bytes = 0;                 // device bytes of the bitmaps
+};
+struct PrefixStats {
+  uint64_t names = 0, matched = 0, launches = 0, syncs = 0;  // records scanned, ids set, launches, syncs that uploaded
+};
+
 class Device {
  public:
   ~Device();
@@ -334,8 +344,10 @@ class Device {
   // returns for the store the snapshot was published from: *count of them, and with `tuples` the records, in no
   // particular order (expires, optional, parallel to them). A count launch sizes the output, then an emit launch fills
   // it. *too_big: the records would take more than a quarter of the free device memory; only *count is valid.
+  // px: the filter's prefix bitmaps (prefix_scan; nullptr when the filter has no prefix), whose bytes count against
+  // that budget.
   int match_filter(const Schema& sc, const Store::Filter& f, uint32_t now, uint64_t* count, std::vector<zg_tuple>* tuples,
-                   std::vector<uint32_t>* expires, bool* too_big, std::string* err);
+                   std::vector<uint32_t>* expires, bool* too_big, std::string* err, const PrefixBits* px = nullptr);
   // The relationships of the resident snapshot whose expiration is set and <= before (zg_collect_expired), what
   // Store::expired returns for the store the snapshot was published from; otherwise as match_filter. Only the classes
   // with CF_EXPIRY are read. A count launch that finds nothing is the whole call.
@@ -347,16 +359,29 @@ class Device {
   // page_walk), the subject shape takes `want` entries of every selected class's reverse row and merges them here.
   // *too_big: the output would take more than a quarter of the free device memory, or a type has more selected
   // classes than one plan holds; nothing else is valid and the caller pages on the host.
+  // With a prefix (px), the scan shape's windows are sized over the ascending list of each type's matched ids
+  // (filter.cuh prefix_list_kernel), which counts against the budget with the bitmaps.
   struct PageStats {
     uint64_t scanned = 0, launches = 0;  // entries the windows covered (see zg_page_counters), kernel launches
+    uint64_t list_launches = 0;          // of those, the launches that built and searched the match lists
   };
   int page_filter(const Schema& sc, const Store::Filter& f, uint32_t now, const PageKey* after, uint64_t want,
                   std::vector<zg_tuple>* tuples, std::vector<uint32_t>* expires, PageStats* st, bool* too_big,
-                  std::string* err);
+                  std::string* err, const PrefixBits* px = nullptr);
   // zg_retire_unused_names: per type, one bit per id of the snapshot's object capacity, set where a relationship of
   // the snapshot names the id as its resource or its subject (filter.cuh mention_scan_kernel); OR-ed into *bits
   // (Store::IdBits, grown to the capacities). One launch per 64 types, one copy back.
   int scan_mentions(const Schema& sc, Store::IdBits* bits, std::string* err);
+
+  // ---- resource id prefixes (ingress.cuh prefix_match_kernel) ----
+  // Brings the names mirror in step with the store (ingress_sync), then sets, per type the filter may select (res_type,
+  // or every type with a relation when res_type < 0), one bit per id of the snapshot's object capacity whose name
+  // starts with `prefix`: one launch per 64 types. The bitmaps live on this device until the next call; the shards of a
+  // sharded handle read them through peer memory. *too_big: they would take more than a quarter of the free device
+  // memory, or the names mirror could not be brought up to date for lack of device memory (the mirror is then
+  // dropped); nothing else is valid and the caller answers on the host. The caller holds the device lock and the names lock (shared is enough).
+  int prefix_scan(const Store& store, const Schema& sc, int res_type, const std::string& prefix, PrefixBits* out,
+                  PrefixStats* st, bool* too_big, std::string* err);
 
   // ---- device ingress (ingress.cuh): packed string ids -> interned checks against the mirror of the store's names ----
   // The literal fields of a packed call, resolved once on the host exactly as zg_resolve_checks_packed resolves them.
@@ -472,7 +497,7 @@ class Device {
   // `tuples` the emit launch sized by it, of filter_expired_kernel (`expired`) or the kernel of `shape`.
   int run_filter(const Schema& sc, const Snapshot& s, const std::vector<FilterSel>& sel, FilterPlan& p, FilterShape shape,
                  bool expired, uint64_t* count, std::vector<zg_tuple>* tuples, std::vector<uint32_t>* expires, bool* too_big,
-                 std::string* err);
+                 std::string* err, const std::vector<const uint32_t*>* bits = nullptr, uint64_t held = 0);
   int ingress_sync(const Store& store, cudaStream_t st, std::string* err);
   std::string finish_publish(std::shared_ptr<Snapshot> s, const HostSnapshot& lay, const Schema& sc, uint64_t revision);
   // One check_kernel launch over `nq` queries: val (may be null) receives the per-(query, leaf) value
@@ -502,6 +527,8 @@ class Device {
   DevBuf flt_out_, flt_exp_, flt_ctrl_;                     // match_filter: records, expirations, the count
   DevBuf pg_count_, pg_off_, pg_tmp_, pg_seg_;              // page_filter: tile counts, offsets, scan space, segments
   DevBuf mention_bits_;                                     // scan_mentions: every type's bitmap
+  DevBuf px_bits_, px_str_, px_ctrl_;                       // prefix_scan: bitmaps, the prefix's bytes, the match count
+  DevBuf px_first_, px_ids_, px_ent_, px_sum_, px_tmp_;     // prefix pages: a type's match list and its entry sums
   // sharded LookupResources round: walk state in rb_visited_ / lk_jobs_ / lb_owner_ / lb_params_ / lb_keys_ (a sharded
   // engine never runs lookup_batch), the round's home ranks, self-membership list and control words here
   DevBuf sl_home_, sl_self_, sl_ctrl_;

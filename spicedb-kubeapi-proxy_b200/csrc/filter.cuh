@@ -56,6 +56,9 @@ struct FilterPlan {
   unsigned long long cap;
   unsigned long long* count;
   FilterSel sel[kMaxFilterSel];
+  // kPrefix instantiations: per selected class, its resource type's bitmap of the ids whose name has the filter's
+  // prefix (prefix_match_kernel). Last, so that the fields above keep their offsets.
+  const uint32_t* bits[kMaxFilterSel];
 };
 
 __device__ __forceinline__ uint32_t filter_lower_bound(const uint32_t* a, uint32_t lo, uint32_t hi, uint32_t key) {
@@ -67,6 +70,18 @@ __device__ __forceinline__ uint32_t filter_lower_bound(const uint32_t* a, uint32
 }
 __device__ __forceinline__ bool filter_live(uint32_t expires, uint32_t now) { return now == 0 || expires == 0 || expires > now; }
 __device__ __forceinline__ bool filter_expired(uint32_t expires, uint32_t before) { return expires != 0 && expires <= before; }
+// Bit `id` of a prefix bitmap covering `n` ids: the id's name has the prefix.
+__device__ __forceinline__ bool filter_bit(const uint32_t* bits, uint32_t id, uint32_t n) {
+  return id < n && (__ldg(bits + (id >> 5)) >> (id & 31) & 1u);
+}
+// The expiration of (res, subj) in class s, found in res's forward row (res < s.nres); 0 when absent.
+__device__ __forceinline__ uint32_t filter_find_exp(const uint32_t* row_ptr, const uint32_t* col, const uint32_t* exp,
+                                                    const FilterSel& s, uint32_t res, uint32_t subj) {
+  const unsigned long long fi = s.row_base + static_cast<unsigned long long>(res) * s.stride;
+  const uint32_t fb = __ldg(row_ptr + fi), fe = __ldg(row_ptr + fi + 1);
+  const uint32_t at = filter_lower_bound(col, fb, fe, subj);
+  return at < fe && __ldg(col + at) == subj ? __ldg(exp + at) : 0u;
+}
 
 // Warp-collective: counts the lanes with `hit`, and (kEmit) appends their records behind one reservation.
 template <bool kEmit>
@@ -131,7 +146,7 @@ __global__ void __launch_bounds__(kFilterThreads) filter_resource_kernel(const F
 
 // Subject given, no resource: one relationship per entry of the subject's reverse row. The reverse CSR carries no
 // expirations, so when they matter the entry is found again in the forward row of its resource.
-template <bool kEmit>
+template <bool kEmit, bool kPrefix = false>
 __global__ void __launch_bounds__(kFilterThreads) filter_subject_kernel(const FilterPlan p) {
   const unsigned lane = threadIdx.x & 31;
   const unsigned long long w = (blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x) >> 5;
@@ -146,7 +161,16 @@ __global__ void __launch_bounds__(kFilterThreads) filter_subject_kernel(const Fi
       const unsigned long long i = i0 + lane;
       bool hit = i < e;
       uint32_t res = 0, ex = 0;
-      if (hit) {
+      // kPrefix: an entry whose resource's bit is clear is dropped before its expiration is looked up. The two
+      // branches are kept apart so that the unprefixed instantiations compile to the code they always had.
+      if constexpr (kPrefix) {
+        if (hit) {
+          res = __ldg(p.rcol + i);
+          hit = filter_bit(p.bits[k], res, s.nres);
+          if (hit && want_exp) ex = filter_find_exp(p.row_ptr, p.col, p.exp, s, res, p.subj);
+          hit = hit && filter_live(ex, p.now);
+        }
+      } else if (hit) {
         res = __ldg(p.rcol + i);
         if (want_exp && res < s.nres) {
           const unsigned long long fi = s.row_base + static_cast<unsigned long long>(res) * s.stride;
@@ -165,7 +189,9 @@ __global__ void __launch_bounds__(kFilterThreads) filter_subject_kernel(const Fi
 // works each non-empty row together. A count that does not depend on expirations needs the offsets only. kExpired:
 // the entries filter_expired selects, which always depends on them. The plan is taken by value: inlined into the
 // kernels it stays the kernel parameter, and filter_scan_kernel compiles to the SASS it had as a kernel of its own.
-template <bool kEmit, bool kExpired>
+// kPrefix: only the objects whose bit is set in the class's prefix bitmap. A warp's 32 objects are 32-aligned, so they
+// are one bitmap word, read before any row offset: a word of unmatched objects costs that one load.
+template <bool kEmit, bool kExpired, bool kPrefix = false>
 __device__ __forceinline__ void filter_scan(const FilterPlan p) {
   const unsigned lane = threadIdx.x & 31;
   const unsigned long long w = (blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x) >> 5;
@@ -174,9 +200,14 @@ __device__ __forceinline__ void filter_scan(const FilterPlan p) {
   for (uint32_t k = 0; k < p.n_sel; ++k) {
     const FilterSel& s = p.sel[k];
     for (unsigned long long obj0 = w * 32; obj0 < s.nres; obj0 += n_warps * 32) {
+      uint32_t word = kFilterFull;
+      if (kPrefix) {
+        word = __ldg(p.bits[k] + (obj0 >> 5));
+        if (!word) continue;
+      }
       const unsigned long long obj = obj0 + lane;
       uint32_t b = 0, e = 0;
-      if (obj < s.nres) {
+      if (obj < s.nres && (!kPrefix || (word >> lane & 1u))) {
         const unsigned long long ri = s.row_base + obj * s.stride;
         b = __ldg(p.row_ptr + ri);
         e = __ldg(p.row_ptr + ri + 1);
@@ -198,9 +229,9 @@ __device__ __forceinline__ void filter_scan(const FilterPlan p) {
   }
 }
 
-template <bool kEmit>
+template <bool kEmit, bool kPrefix = false>
 __global__ void __launch_bounds__(kFilterThreads) filter_scan_kernel(const FilterPlan p) {
-  filter_scan<kEmit, false>(p);
+  filter_scan<kEmit, false, kPrefix>(p);
 }
 
 // Expired relationships of the selected classes: p.now is the collection's `before` (never 0).
@@ -236,6 +267,7 @@ struct PagePlan {
   uint32_t* out_exp;
   uint32_t* seg_count;                // subject shape: per selected class, the entries written to its segment
   FilterSel sel[kMaxFilterSel];
+  const uint32_t* bits[kMaxFilterSel];  // kPrefix: as FilterPlan::bits
 };
 
 // The entries of (object o, class s) a page may return: past the start key when o is the cursor's object, and only
@@ -272,12 +304,18 @@ __global__ void page_window_kernel(const uint32_t* row_ptr, unsigned long long b
 
 // Warp-collective walk of tile t: its matches in K order. kEmit: written from `base` on, never at or past p.want.
 // Returns how many it found, counting stopping once `base` + that reaches p.want.
-template <bool kEmit>
+// kPrefix: only objects whose bit is set; the classes of a window share one resource type and so one bitmap, and a tile
+// none of whose objects is set returns before it loads a row offset.
+template <bool kEmit, bool kPrefix = false>
 __device__ __forceinline__ unsigned long long page_tile(const PagePlan& p, unsigned long long t, unsigned long long base,
                                                         unsigned lane) {
   const unsigned long long o64 = p.obj0 + t * 32 + lane;
-  const bool mine = o64 < p.obj1;
+  bool mine = o64 < p.obj1;
   const uint32_t o = static_cast<uint32_t>(o64);
+  if (kPrefix) {
+    mine = mine && filter_bit(p.bits[0], o, p.sel[0].nres);
+    if (!__ballot_sync(kFilterFull, mine)) return 0;
+  }
   // the lane's object: does it have an entry the page may return, and how many (offsets only)
   unsigned long long n = 0;
   if (mine)
@@ -331,17 +369,19 @@ __device__ __forceinline__ unsigned long long page_tile(const PagePlan& p, unsig
   return got;
 }
 
+template <bool kPrefix = false>
 __global__ void __launch_bounds__(kFilterThreads) page_count_kernel(const PagePlan p) {
   const unsigned lane = threadIdx.x & 31;
   const unsigned long long w = (blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x) >> 5;
   const unsigned long long n_warps = (static_cast<unsigned long long>(gridDim.x) * blockDim.x) >> 5;
   const unsigned long long tiles = (static_cast<unsigned long long>(p.obj1 - p.obj0) + 31) >> 5;
   for (unsigned long long t = w; t < tiles; t += n_warps) {
-    const unsigned long long n = page_tile<false>(p, t, 0, lane);
+    const unsigned long long n = page_tile<false, kPrefix>(p, t, 0, lane);
     if (lane == 0) p.tile_count[t] = n;
   }
 }
 
+template <bool kPrefix = false>
 __global__ void __launch_bounds__(kFilterThreads) page_emit_kernel(const PagePlan p) {
   const unsigned lane = threadIdx.x & 31;
   const unsigned long long w = (blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x) >> 5;
@@ -350,14 +390,16 @@ __global__ void __launch_bounds__(kFilterThreads) page_emit_kernel(const PagePla
   for (unsigned long long t = w; t < tiles; t += n_warps) {
     const unsigned long long base = __ldg(p.tile_off + t);
     if (base >= p.want) continue;  // tiles are in K order: every later one starts at or past it too
-    if (__ldg(p.tile_count + t)) page_tile<true>(p, t, base, lane);
+    if (__ldg(p.tile_count + t)) page_tile<true, kPrefix>(p, t, base, lane);
   }
 }
 
 // Subject given, no resource: one warp per selected class. Its reverse row is sorted by resource, and K orders by
 // (type, resource, class position, subject) with the type, the position and the subject fixed for the row, so the
 // entries after the cursor are a suffix of the row. The first `want` live ones go to the class's segment in order;
-// expirations are found again in the forward row, as filter_subject_kernel does.
+// expirations are found again in the forward row, as filter_subject_kernel does. kPrefix: only entries whose resource's
+// bit is set in the class's bitmap.
+template <bool kPrefix = false>
 __global__ void __launch_bounds__(32) page_subject_kernel(const PagePlan p) {
   const unsigned lane = threadIdx.x & 31;
   for (uint32_t k = blockIdx.x; k < p.n_sel; k += gridDim.x) {
@@ -384,7 +426,14 @@ __global__ void __launch_bounds__(32) page_subject_kernel(const PagePlan p) {
         const uint32_t i = i0 + lane;
         bool hit = i < e;
         uint32_t res = 0, ex = 0;
-        if (hit) {
+        if constexpr (kPrefix) {  // as in filter_subject_kernel
+          if (hit) {
+            res = __ldg(p.rcol + i);
+            hit = filter_bit(p.bits[k], res, s.nres);
+            if (hit && p.exp) ex = filter_find_exp(p.row_ptr, p.col, p.exp, s, res, p.subj);
+            hit = hit && filter_live(ex, p.now);
+          }
+        } else if (hit) {
           res = __ldg(p.rcol + i);
           if (p.exp && res < s.nres) {
             const unsigned long long fi = s.row_base + static_cast<unsigned long long>(res) * s.stride;
@@ -429,10 +478,12 @@ inline void page_set_after(PagePlan& p, const PageKey* after) {
 // The first window of a type asks for `want - got` entries of the block; every window that comes up short (expired
 // entries, classes not selected, the cursor's object) asks for at least twice as many as the one before it, more when
 // its density of matches says the rest of the page needs more. *scanned: the entries of the block the windows
-// covered. Returns 0 or what an op returned.
+// covered. `bits` (optional, parallel to sel): the classes' prefix bitmaps, copied into p.bits with them. Returns 0 or
+// what an op returned.
 template <class Ops>
 int page_walk(Ops& ops, PagePlan& p, const std::vector<FilterSel>& sel, bool by_resource, uint32_t res, const PageKey* after,
-              unsigned long long want, unsigned long long* got, uint64_t* scanned) {
+              unsigned long long want, unsigned long long* got, uint64_t* scanned,
+              const std::vector<const uint32_t*>* bits = nullptr) {
   *got = 0;
   for (size_t g = 0; g < sel.size() && *got < want;) {
     size_t g1 = g;
@@ -441,6 +492,7 @@ int page_walk(Ops& ops, PagePlan& p, const std::vector<FilterSel>& sel, bool by_
     const uint32_t type = sel[g].rtype, nres = sel[g].nres;
     p.n_sel = static_cast<uint32_t>(g1 - g);
     std::copy(sel.begin() + g, sel.begin() + g1, p.sel);
+    if (bits) std::copy(bits->begin() + g, bits->begin() + g1, p.bits);
     g = g1;
     const bool at_cursor = after && after->type == type;
     if (after && type < after->type) continue;
@@ -474,6 +526,71 @@ int page_walk(Ops& ops, PagePlan& p, const std::vector<FilterSel>& sel, bool by_
     }
   }
   return 0;
+}
+
+// ---- selective pages of a prefix filter ----
+// page_window_kernel sizes a window from row_ptr alone: with a prefix that matches few objects it would walk window
+// after window of unmatched ones. A prefix page instead compacts a type's bitmap into the ascending list of its
+// matched ids, with the exclusive sum of their entries in the type's block, and sizes windows over list positions:
+//   prefix_word_count_kernel  per bitmap word, its set bits (then an exclusive scan gives each word's first position)
+//   prefix_list_kernel        every matched id at its position, with its entries in the block
+//   (exclusive scan of the entries)
+//   prefix_window_kernel      the window from obj0 of at least `entries` entries of matched objects
+// so the launches of a page depend on the matches it walks, never on the unmatched objects between them.
+__global__ void __launch_bounds__(kFilterThreads) prefix_word_count_kernel(const uint32_t* bits, uint32_t words,
+                                                                          uint32_t* count) {
+  const uint64_t stride = uint64_t(gridDim.x) * blockDim.x;
+  for (uint64_t w = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; w <= words; w += stride)
+    count[w] = w < words ? __popc(__ldg(bits + w)) : 0u;
+}
+
+// ids[pos] = the matched id, ent[pos] = its entries in the block at (row_ptr + block, stride); ent[m] = 0.
+__global__ void __launch_bounds__(kFilterThreads) prefix_list_kernel(const uint32_t* bits, uint32_t words, const uint32_t* first,
+                                                                     const uint32_t* row_ptr, unsigned long long block,
+                                                                     uint32_t stride, uint32_t nres, uint32_t* ids,
+                                                                     unsigned long long* ent) {
+  const uint64_t step = uint64_t(gridDim.x) * blockDim.x;
+  for (uint64_t w = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; w <= words; w += step) {
+    if (w == words) {
+      ent[__ldg(first + words)] = 0;
+      continue;
+    }
+    uint32_t word = __ldg(bits + w), pos = __ldg(first + w);
+    while (word) {
+      const uint32_t id = static_cast<uint32_t>(w * 32) + (__ffs(word) - 1);
+      word &= word - 1;
+      unsigned long long n = 0;
+      if (id < nres) {
+        const unsigned long long r = block + static_cast<unsigned long long>(id) * stride;
+        n = __ldg(row_ptr + r + stride) - __ldg(row_ptr + r);
+      }
+      ids[pos] = id;
+      ent[pos] = n;
+      ++pos;
+    }
+  }
+}
+
+// One thread: from the first list position i whose id >= obj0, the least j in (i, m] at which the matched objects
+// [i, j) hold at least `entries` entries (m when fewer do); out[0] = obj1 (ids[j], or nres at the list's end), out[1]
+// = their entries. csum: the exclusive sum of the list's entries (m + 1 values).
+__global__ void prefix_window_kernel(const uint32_t* ids, const unsigned long long* csum, uint32_t m, uint32_t obj0,
+                                     uint32_t nres, unsigned long long entries, unsigned long long* out) {
+  if (threadIdx.x | blockIdx.x) return;
+  uint32_t i = filter_lower_bound(ids, 0, m, obj0);
+  if (i == m) {
+    out[0] = nres;
+    out[1] = 0;
+    return;
+  }
+  const unsigned long long at0 = __ldg(csum + i);
+  uint32_t lo = i + 1, hi = m;
+  while (lo < hi) {
+    const uint32_t mid = lo + ((hi - lo) >> 1);
+    if (__ldg(csum + mid) - at0 < entries) lo = mid + 1; else hi = mid;
+  }
+  out[0] = lo < m ? __ldg(ids + lo) : nres;
+  out[1] = __ldg(csum + lo) - at0;
 }
 
 // The subject shape: the segments of page_subject_kernel (seg_count[k] records of class sel[k] at rec + k * want),

@@ -164,4 +164,48 @@ __global__ void __launch_bounds__(kIngressThreads) ingress_resolve_kernel(const 
   }
 }
 
+// ---- resource id prefixes (optional_resource_id_prefix) ----
+// The ids of a type whose interned name starts with a prefix, read from the type's mirror: every record [u32 id][u32
+// len][bytes] whose name is at least as long as the prefix and whose first bytes equal it sets bit `id` of the type's
+// bitmap (n_ids bits: the snapshot's object capacity; an id at or past it is interned after the snapshot and no
+// relationship of the snapshot names it). The comparison (ingress_equal) reads the name through a WordStream of the
+// prefix's length, so no read leaves the record; names shorter than the prefix are never read. One launch covers every selected type.
+constexpr int kMaxPrefixTypes = 64;  // types per launch; a schema with more runs several launches
+
+struct PrefixType {
+  const uint8_t* arena;
+  const unsigned long long* offs;  // record offsets
+  unsigned long long n_recs;
+  uint32_t* bits;                  // ceil(n_ids / 32) words, zeroed by the host
+  uint32_t n_ids;
+  uint32_t pad;
+};
+
+struct PrefixPlan {
+  const uint8_t* prefix;    // device bytes, 8-byte aligned
+  unsigned long long len;   // 1 .. 1024
+  unsigned long long* matched;  // += records that set a bit
+  uint32_t n_types;
+  uint32_t pad;
+  PrefixType type[kMaxPrefixTypes];
+};
+
+__global__ void __launch_bounds__(kIngressThreads) prefix_match_kernel(const PrefixPlan p) {
+  const uint64_t stride = uint64_t(gridDim.x) * blockDim.x;
+  unsigned long long found = 0;
+  for (uint32_t k = 0; k < p.n_types; ++k) {
+    const PrefixType& t = p.type[k];
+    for (uint64_t r = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x; r < t.n_recs; r += stride) {
+      const uint8_t* rec = t.arena + t.offs[r];
+      const uint64_t hdr = WordStream(rec, 8).next();  // records are not aligned
+      const uint32_t id = static_cast<uint32_t>(hdr);
+      if ((hdr >> 32) < p.len || id >= t.n_ids || !ingress_equal(rec + 8, p.prefix, p.len)) continue;
+      atomicOr(t.bits + (id >> 5), 1u << (id & 31));
+      ++found;
+    }
+  }
+  for (int d = 16; d > 0; d >>= 1) found += __shfl_xor_sync(0xFFFFFFFFu, found, d);
+  if ((threadIdx.x & 31) == 0 && found) atomicAdd(p.matched, found);
+}
+
 }  // namespace zg

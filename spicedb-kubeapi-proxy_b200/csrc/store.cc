@@ -151,6 +151,11 @@ bool Store::name(int type, uint32_t id, std::string_view* out) const {
   return true;
 }
 
+bool Store::name_has_prefix(int type, uint32_t id, const std::string& prefix) const {
+  std::string_view n;
+  return name(type, id, &n) && n.size() >= prefix.size() && std::memcmp(n.data(), prefix.data(), prefix.size()) == 0;
+}
+
 std::string Store::validate(const zg_tuple& t, bool has_expiry) const {
   const Schema& sc = *schema;
   if (t.rel >= sc.slots.size() || sc.slots[t.rel].is_perm) return "relationship does not name a relation";
@@ -320,6 +325,7 @@ void Store::match(const Filter& f, uint32_t now, std::vector<uint64_t>* idx) con
     if (expires[i] != 0 && expires[i] <= now) continue;
     if (f.res_type >= 0 && schema->slots[t.rel].type != f.res_type) continue;
     if (f.has_res && t.res != f.res) continue;
+    if (!f.prefix.empty() && !name_has_prefix(schema->slots[t.rel].type, t.res, f.prefix)) continue;
     if (f.rel >= 0 && t.rel != f.rel) continue;
     if (f.subj_type >= 0 && t.stype != f.subj_type) continue;
     if (f.subj_wildcard && t.srel != kWildcard) continue;

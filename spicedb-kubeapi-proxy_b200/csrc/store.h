@@ -169,7 +169,11 @@ class Store {
     bool has_srel = false;
     uint16_t srel = kNone;
     bool impossible = false;  // names an object/relation that does not exist
+    // optional_resource_id_prefix: only resources whose interned name starts with these bytes (empty = unset)
+    std::string prefix;
   };
+  // true when (type, id) has an interned name that starts with `prefix` (byte-wise, case-sensitive)
+  bool name_has_prefix(int type, uint32_t id, const std::string& prefix) const;
   void match(const Filter& f, uint32_t now, std::vector<uint64_t>* idx) const;
   // The host path of a page: the first `want` relationships match() lists whose key follows *after (nullptr: from
   // the start), in K order (PageKey), as positions in `tuples`.
